@@ -18,30 +18,39 @@
 // The fully unrolled rounds are far larger than the 32 KB instruction cache; with the field multiplication out of line
 // (one shared 80-instruction body) the pass kernels are much smaller.  The large transforms use inlined multiplies with small
 // register rounds instead (ntt_inl.cu): the small rounds keep the unrolled code near the instruction-cache size without a call per multiply.
+// Each kernel is specialised at compile time for one pass kind (PassKind, ntt_pass.cuh), so it holds only its own input and output
+// paths; at the default shape (4-element register rounds, 512 threads, 64 registers) the kernels of the 2^20-step proof do not spill.
 #define DG_MUL_CALL 1
 #include "ntt_pass.cuh"
 
 namespace dg {
 
 // kernel variants (ntt_pass.cuh): RMAX stages per register round, BT threads per block; inline-multiply instantiations live in ntt_inl.cu
-PassKernel pass_kernel_inline(bool lane_major, int log_l, int rmax, int bt);       // nullptr when that combination is not instantiated
-template <bool LM, int RMAX, int BT, int MINB> static PassKernel pass_kernel_t(int log_l) {
-    switch (log_l) {
-        case 1: return ntt_pass_kernel<1, LM, RMAX, BT, MINB, 0>;  case 2: return ntt_pass_kernel<2, LM, RMAX, BT, MINB, 0>;
-        case 3: return ntt_pass_kernel<3, LM, RMAX, BT, MINB, 0>;  case 4: return ntt_pass_kernel<4, LM, RMAX, BT, MINB, 0>;
-        case 5: return ntt_pass_kernel<5, LM, RMAX, BT, MINB, 0>;  case 6: return ntt_pass_kernel<6, LM, RMAX, BT, MINB, 0>;
-        case 7: return ntt_pass_kernel<7, LM, RMAX, BT, MINB, 0>;  case 8: return ntt_pass_kernel<8, LM, RMAX, BT, MINB, 0>;
-        case 9: return ntt_pass_kernel<9, LM, RMAX, BT, MINB, 0>;  case 10: return ntt_pass_kernel<10, LM, RMAX, BT, MINB, 0>;
+PassKernel pass_kernel_inline(int kind, int log_l, int rmax, int bt);       // nullptr when that combination is not instantiated
+
+// the kernel specialisation of a pass, from the flags run_transform sets
+static int pass_kind(const PassGeom &g) {
+    if (!g.lane_major) {
+        DG_REQUIRE(g.tw_on && !g.has_scale, "strided NTT pass without inter-pass twiddle");
+        if (g.coset_fast) return g.tw_full ? PK_COSET_TWFULL : PK_COSET_TW;
+        return g.coset_on ? PK_FOLD_TW : PK_TW;
     }
-    throw Error(-1, "unsupported sub-transform size");
+    DG_REQUIRE(!g.tw_on, "contiguous NTT pass with inter-pass twiddle");
+    if (g.coset_on) {
+        DG_REQUIRE(!g.has_scale, "scaled coset transform");
+        return g.coset_fast ? PK_COSET_ONE : PK_FOLD_ONE;
+    }
+    return g.has_scale ? PK_LAST_SCALE : PK_LAST;
 }
 
-// Kernel configuration per pass kind: A = strided passes (first / middle), B = the contiguous last pass; "f" variants are used by the
-// transforms whose first pass folds 8 coefficient blocks (constraint / composition LDE).  H100 SXM (700 W), stage 1 of the 2^20-step
-// proof (26 columns, LDE x32), tools/variant_bench.py, ms:
-//   default: inline multiply, 8-element units (rmax 3), 512 threads for A and B     60.8 - 61.3
-//   A = 4-element units, 512 threads 61.5;  A = 256 threads 68.0;  A = 1024 threads + 8192-element tiles 71.7
-//   B = 4-element units, 512 threads 61.6;  B = 256 threads 62.5;  AF = 8-element units or 256 threads: no change in stages 5 / 6
+// Kernel configuration per pass position: A = strided passes (first / middle), B = the contiguous last pass; "f" variants are used by the
+// transforms whose first pass folds 8 coefficient blocks (constraint / composition LDE).  H100 SXM 80 GB (700 W power limit), stage 1 of
+// the 2^20-step proof (26 columns, LDE x32), tools/variant_bench.py, ms:
+//   default: inline multiply, 4-element units (rmax 2), 512 threads for A and B: 52.7 (no spills at the 64-register cap)
+//   A = B = 8-element units (rmax 3), 512 threads: 56.9 (150-570 bytes of spills per kernel at the 64-register cap)
+//   measured before the kernels were specialised per pass kind (every kind's path in one kernel, a call per multiply):
+//   rmax 3 for A and B 60.8 - 61.3;  A = 256 threads 68.0;  A = 1024 threads + 8192-element tiles 71.7;  B = 256 threads 62.5;
+//   AF = 8-element units or 256 threads: no change in stages 5 / 6
 // Environment overrides (read once): DG_NTT_A / DG_NTT_B / DG_NTT_AF = "rmax,threads,inline", DG_NTT_TILE = log2 of the tile size.
 struct PassCfg { int rmax, bt, inl; };
 struct NttConfig { PassCfg a, b, af; int tile_log; };
@@ -56,8 +65,8 @@ static const NttConfig &ntt_config() {
     static NttConfig cfg;
     static bool init = false;
     if (!init) {
-        cfg.a = parse_cfg("DG_NTT_A", PassCfg{3, 512, 1});
-        cfg.b = parse_cfg("DG_NTT_B", PassCfg{3, 512, 1});
+        cfg.a = parse_cfg("DG_NTT_A", PassCfg{2, 512, 1});
+        cfg.b = parse_cfg("DG_NTT_B", PassCfg{2, 512, 1});
         cfg.af = parse_cfg("DG_NTT_AF", PassCfg{2, 512, 1});
         const char *e = getenv("DG_NTT_TILE");
         cfg.tile_log = e ? atoi(e) : 12;
@@ -73,18 +82,19 @@ static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *ds
     const size_t smem = ((size_t)L + data) * sizeof(fe);
     const NttConfig &nc = ntt_config();
     const PassCfg cfg = g.lane_major ? nc.b : ((g.coset_on && !g.coset_fast) ? nc.af : nc.a);
+    const int kind = pass_kind(g);
     int rmax = cfg.rmax, bt = cfg.bt;
     PassKernel k = nullptr;
-    if (cfg.inl) k = pass_kernel_inline(g.lane_major != 0, log_l, rmax, bt);
+    if (cfg.inl) k = pass_kernel_inline(kind, log_l, rmax, bt);
     if (!k) {
-        const bool lm = g.lane_major != 0;
         if (bt == 1024) bt = 512;
-        if (rmax == 4) { bt = 256; k = lm ? pass_kernel_t<true, 4, 256, 2>(log_l) : pass_kernel_t<false, 4, 256, 2>(log_l); }
-        else if (rmax == 3 && bt == 512) k = lm ? pass_kernel_t<true, 3, 512, 2>(log_l) : pass_kernel_t<false, 3, 512, 2>(log_l);
-        else if (rmax == 3) k = lm ? pass_kernel_t<true, 3, 256, 3>(log_l) : pass_kernel_t<false, 3, 256, 3>(log_l);
-        else if (bt == 512) k = lm ? pass_kernel_t<true, 2, 512, 2>(log_l) : pass_kernel_t<false, 2, 512, 2>(log_l);
-        else k = lm ? pass_kernel_t<true, 2, 256, 4>(log_l) : pass_kernel_t<false, 2, 256, 4>(log_l);
+        if (rmax == 4) { bt = 256; k = pass_kernel_of<4, 256, 2, 0, 1, MAX_LOG_L>(kind, log_l); }
+        else if (rmax == 3 && bt == 512) k = pass_kernel_of<3, 512, 2, 0, 1, MAX_LOG_L>(kind, log_l);
+        else if (rmax == 3) k = pass_kernel_of<3, 256, 3, 0, 1, MAX_LOG_L>(kind, log_l);
+        else if (bt == 512) k = pass_kernel_of<2, 512, 2, 0, 1, MAX_LOG_L>(kind, log_l);
+        else k = pass_kernel_of<2, 256, 4, 0, 1, MAX_LOG_L>(kind, log_l);
     }
+    DG_REQUIRE(k, "unsupported sub-transform size");
     int threads = (L * T) >> (log_l < rmax ? log_l : rmax);           // one unit per thread in the largest round
     if (threads > bt) threads = bt;
     if (threads < 32) threads = 32;
@@ -300,8 +310,10 @@ void lde_batch(Context &c, const fe *src, fe *dst, int log_n, int log_blowup, in
                unsigned coset0, unsigned ncosets) {
     DG_REQUIRE(log_n >= 1 && log_n + log_blowup <= 30, "LDE domain too large");
     const size_t n = (size_t)1 << log_n;
-    const unsigned cosets = ncosets ? ncosets : (1u << log_blowup);
-    DG_REQUIRE(coset0 + cosets <= (1u << log_blowup), "coset range out of bounds");
+    DG_REQUIRE(log_blowup >= 0 && log_blowup <= 16 && fold >= 1, "bad LDE shape");
+    const unsigned b = 1u << log_blowup, cosets = ncosets ? ncosets : b;
+    // any sub-range works (blockIdx.y = coset - coset0 indexes the streamed twiddles and dst); a range beyond the domain does not
+    DG_REQUIRE(coset0 < b && cosets <= b - coset0, "coset range out of bounds");
     static int prefold = -1;
     if (prefold < 0) { const char *e = getenv("DG_LDE_PREFOLD"); prefold = e ? atoi(e) : 1; }
     if (prefold && fold == 8 && batch == 1 && cosets == (1u << log_blowup) && log_blowup >= 3 && log_blowup <= 8) {

@@ -5,21 +5,12 @@
 
 namespace dg {
 
-template <bool LM, int RMAX, int BT, int MINB> static PassKernel inl_t(int log_l) {
-    switch (log_l) {
-        case 8: return ntt_pass_kernel<8, LM, RMAX, BT, MINB, 1>;
-        case 9: return ntt_pass_kernel<9, LM, RMAX, BT, MINB, 1>;
-        case 10: return ntt_pass_kernel<10, LM, RMAX, BT, MINB, 1>;
-    }
-    return nullptr;
-}
-
-PassKernel pass_kernel_inline(bool lm, int log_l, int rmax, int bt) {
-    if (rmax == 3 && bt == 1024) return lm ? inl_t<true, 3, 1024, 1>(log_l) : inl_t<false, 3, 1024, 1>(log_l);
-    if (rmax == 3 && bt == 512) return lm ? inl_t<true, 3, 512, 2>(log_l) : inl_t<false, 3, 512, 2>(log_l);
-    if (rmax == 3) return lm ? inl_t<true, 3, 256, 3>(log_l) : inl_t<false, 3, 256, 3>(log_l);
-    if (rmax == 2 && bt == 512) return lm ? inl_t<true, 2, 512, 2>(log_l) : inl_t<false, 2, 512, 2>(log_l);
-    if (rmax == 2) return lm ? inl_t<true, 2, 256, 4>(log_l) : inl_t<false, 2, 256, 4>(log_l);
+PassKernel pass_kernel_inline(int kind, int log_l, int rmax, int bt) {
+    if (rmax == 3 && bt == 1024) return pass_kernel_of<3, 1024, 1, 1, 8, 10>(kind, log_l);
+    if (rmax == 3 && bt == 512) return pass_kernel_of<3, 512, 2, 1, 8, 10>(kind, log_l);
+    if (rmax == 3) return pass_kernel_of<3, 256, 3, 1, 8, 10>(kind, log_l);
+    if (rmax == 2 && bt == 512) return pass_kernel_of<2, 512, 2, 1, 8, 10>(kind, log_l);
+    if (rmax == 2) return pass_kernel_of<2, 256, 4, 1, 8, 10>(kind, log_l);
     return nullptr;
 }
 

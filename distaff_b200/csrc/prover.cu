@@ -102,6 +102,21 @@ void write_felt_vec(fs::ByteWriter &w, const std::vector<fe> &v) {
 
 int ilog2(uint64_t v) { int l = 0; while ((1ULL << l) < v) l++; return l; }
 
+// Trace LDE of `cols` columns (polynomials `polys`, stride n) onto the cosets [c0, c0 + nc), written to ext (column stride N_loc).
+// Coset 0 is P(w_n^k), which is register row k itself (polys = iNTT(regs) exactly): when the range starts at coset 0 and the registers
+// are on the device (`regs`, stride n; null if not), slab 0 is copied from them and only the other cosets are transformed.
+void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
+                          unsigned nc) {
+    const size_t n = (size_t)1 << log_n;
+    if (c0 != 0 || !regs) {
+        lde_batch(c, polys, ext, log_n, log_b, 1, cols, n, N_loc, c0, nc);
+        return;
+    }
+    DG_REQUIRE(nc >= 2, "coset range too small");
+    lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
+    DG_CUDA(cudaMemcpy2DAsync(ext, N_loc * sizeof(fe), regs, n * sizeof(fe), n * sizeof(fe), cols, cudaMemcpyDeviceToDevice, c.stream));
+}
+
 struct FriLayerDev {
     DevBuf leaves, nodes, folded;     // row hashes, tree, and the folded values (= values of the next layer)
     const fe *vals;                   // replicated layer: the whole vector; sharded layer: this rank's cosets [c - c0][k]
@@ -261,7 +276,7 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
     if (G == 1) {
         if (!host_cols) {
             ntt_batch(c, d_regs, polys.as<fe>(), log_n, w, n, n, true);
-            lde_batch(c, polys.as<fe>(), ext.as<fe>(), log_n, log_b, 1, w, n, N_loc, c0, (unsigned)nc);
+            extend_trace_columns(c, polys.as<fe>(), d_regs, ext.as<fe>(), w, log_n, log_b, N_loc, c0, (unsigned)nc);
         } else {
             // chunks of ~64 MB, but a short ramp first (1, 2 columns): the first transform starts after one column's worth of copying
             const int chunk = (int)std::max<uint64_t>(1, std::min<uint64_t>(w, ((uint64_t)1 << 26) / (n * 16)));
@@ -272,7 +287,8 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
                 const int j0 = bounds[i], cols = bounds[i + 1] - j0;
                 up.wait_chunk(i);
                 ntt_batch(c, d_regs + (size_t)j0 * n, polys.as<fe>() + (size_t)j0 * n, log_n, cols, n, n, true);
-                lde_batch(c, polys.as<fe>() + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * N_loc, log_n, log_b, 1, cols, n, N_loc, c0, (unsigned)nc);
+                extend_trace_columns(c, polys.as<fe>() + (size_t)j0 * n, d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * N_loc, cols, log_n, log_b, N_loc,
+                                     c0, (unsigned)nc);
             }
         }
     } else {
@@ -305,13 +321,15 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
                 DG_CUDA(cudaMemcpyAsync(polys.as<fe>() + (size_t)col_start(r) * n, slots.as<fe>() + (size_t)r * cpr * n, (size_t)col_count(r) * n * 16,
                                         cudaMemcpyDeviceToDevice, c.comm_stream));
         DG_CUDA(cudaEventRecord(ev_all, c.comm_stream));
-        if (mine > 0) lde_batch(c, own.as<fe>(), ext.as<fe>() + (size_t)j0 * N_loc, log_n, log_b, 1, mine, n, N_loc, c0, (unsigned)nc);
+        if (mine > 0)
+            extend_trace_columns(c, own.as<fe>(), d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * N_loc, mine, log_n, log_b, N_loc, c0, (unsigned)nc);
     sub.mark("1.lde_own");
         DG_CUDA(cudaStreamWaitEvent(c.stream, ev_all, 0));
-        if (j0 > 0) lde_batch(c, polys.as<fe>(), ext.as<fe>(), log_n, log_b, 1, j0, n, N_loc, c0, (unsigned)nc);
+        // the other ranks' registers are on this device only when the trace was given in device memory (a host trace uploads own columns only)
+        if (j0 > 0) extend_trace_columns(c, polys.as<fe>(), host_cols ? nullptr : d_regs, ext.as<fe>(), j0, log_n, log_b, N_loc, c0, (unsigned)nc);
         if (j0 + mine < w)
-            lde_batch(c, polys.as<fe>() + (size_t)(j0 + mine) * n, ext.as<fe>() + (size_t)(j0 + mine) * N_loc, log_n, log_b, 1, w - j0 - mine, n, N_loc, c0,
-                      (unsigned)nc);
+            extend_trace_columns(c, polys.as<fe>() + (size_t)(j0 + mine) * n, host_cols ? nullptr : d_regs + (size_t)(j0 + mine) * n,
+                                 ext.as<fe>() + (size_t)(j0 + mine) * N_loc, w - j0 - mine, log_n, log_b, N_loc, c0, (unsigned)nc);
         cudaEventDestroy(ev_own);
         cudaEventDestroy(ev_all);
     }

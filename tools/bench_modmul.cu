@@ -12,6 +12,7 @@ template <int V> __device__ __forceinline__ fe mulv(fe a, fe b) {
     if (V == 1) return ptx::fe_mul_v1(a, b);
     if (V == 2) return ptx::fe_mul_v3(a, b);
     if (V == 3) return ptx::fe_mul_v4(a, b);
+    if (V == 4) return ptx::fe_mul_v4t<false>(a, b);      // the NTT pass kernels' multiply: rare canonicalisation inline, no call
 #endif
     return portable::fe_mul(a, b);
 }
@@ -136,12 +137,14 @@ int main() {
     check<2><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v3");
 #endif
     check<3><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v4");
+    check<4><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v4 inline");
     run<0>("portable", d_in, d_out, blocks, iters);
     run<1>("ptx", d_in, d_out, blocks, iters);
 #ifdef DG_HAVE_V3
     run<2>("v3", d_in, d_out, blocks, iters);
 #endif
     run<3>("v4", d_in, d_out, blocks, iters);
+    run<4>("v4 inline", d_in, d_out, blocks, iters);
     run_call<0>("bfly inline", d_in, d_out, blocks, iters / 2);
     run_call<1>("bfly 1 mul per call", d_in, d_out, blocks, iters / 2);
     run_call<2>("bfly 2 muls per call", d_in, d_out, blocks, iters / 2);
