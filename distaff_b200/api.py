@@ -90,6 +90,75 @@ def prove_device(d_registers, width, length, ctx_depth, loop_depth, public_input
     return _collect(handle, stats)
 
 
+def _batch_io(public_inputs_list, outputs_list):
+    """per-trace public inputs / outputs as the pointer and count arrays of dg_prove_batch (the arrays are kept alive by the caller)"""
+    ins = [felt.from_ints(x) for x in public_inputs_list]
+    outs = [felt.from_ints(x) for x in outputs_list]
+    k = len(ins)
+    arrays = ((backend.vp * k)(*[a.ctypes.data for a in ins]), (backend.u32 * k)(*[len(a) for a in ins]),
+              (backend.vp * k)(*[a.ctypes.data for a in outs]), (backend.u32 * k)(*[len(a) for a in outs]))
+    return ins + outs, arrays
+
+
+def _collect_batch(handles, status, stats):
+    """one entry per trace: a StarkProof, or the DgError of a trace that failed with the library's message for it (stats: the
+    whole batch)"""
+    out = []
+    msg = ctypes.create_string_buffer(512)
+    for i, (h, rc) in enumerate(zip(handles, status)):
+        if rc == 0:
+            out.append(_collect(h, stats))
+        else:
+            backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
+            out.append(backend.DgError(rc, msg.value.decode(errors="replace")))
+    return out
+
+
+def prove_batch(traces, options=None):
+    """Proves many hostvm.ExecutionTraces.  Traces of one shape (width, length, ctx_depth, loop_depth) are proven together by one
+    dg_prove_batch call, each stage launched once for all of them.  Returns a list in input order: a StarkProof (byte-identical to
+    prove() of the same trace) or, for a trace that failed, a backend.DgError instance (returned, not raised).  Errors of a whole call
+    (bad options, no device) raise as in prove()."""
+    options = options or ProofOptions()
+    opt = options._c()
+    traces = list(traces)
+    groups = {}
+    for i, tr in enumerate(traces):
+        groups.setdefault((tr.registers.shape[0], tr.registers.shape[1], tr.ctx_depth, tr.loop_depth), []).append(i)
+    result = [None] * len(traces)
+    for (w, n, ctx_depth, loop_depth), idx in groups.items():
+        k = len(idx)
+        regs = [np.ascontiguousarray(traces[i].registers, dtype=np.uint64) for i in idx]
+        cols = [(backend.vp * w)(*[r[j].ctypes.data for j in range(w)]) for r in regs]
+        ts = (backend.DgTrace * k)(*[backend.DgTrace(cols[m], w, n, ctx_depth, loop_depth) for m in range(k)])
+        keep, (pin, nin, pout, nout) = _batch_io([traces[i].public_inputs for i in idx], [traces[i].outputs for i in idx])
+        handles = (backend.vp * k)()
+        status = (ctypes.c_int * k)()
+        stats = backend.DgStats()
+        backend.check(backend.lib().dg_prove_batch(ts, k, pin, nin, pout, nout, ctypes.byref(opt), handles, status, ctypes.byref(stats)))
+        for i, entry in zip(idx, _collect_batch(list(handles), list(status), stats)):
+            result[i] = entry
+        del keep, regs, cols
+    return result
+
+
+def prove_batch_device(d_registers, count, width, length, ctx_depth, loop_depth, public_inputs_list, outputs_list, options=None):
+    """prove_batch for `count` traces of one shape already in device memory: one allocation, proof-major [count][width][length]
+    elements (backend.DeviceBuffer or raw pointer).  public_inputs_list / outputs_list hold one list per trace."""
+    options = options or ProofOptions()
+    assert len(public_inputs_list) == count and len(outputs_list) == count, "one list of public inputs and outputs per trace"
+    ptr = d_registers.ptr if isinstance(d_registers, backend.DeviceBuffer) else int(d_registers)
+    opt = options._c()
+    keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
+    handles = (backend.vp * max(count, 1))()
+    status = (ctypes.c_int * max(count, 1))()
+    stats = backend.DgStats()
+    backend.check(backend.lib().dg_prove_batch_device(ptr, count, width, length, ctx_depth, loop_depth, pin, nin, pout, nout, ctypes.byref(opt),
+                                                     handles, status, ctypes.byref(stats)))
+    del keep
+    return _collect_batch(list(handles)[:count], list(status)[:count], stats)
+
+
 def verify(program_hash, public_inputs, outputs, proof):
     """distaff::verify (lib.rs:68-75 -> stark/verifier.rs:11-75) on the GPU.  Returns None when the proof is accepted, otherwise the
     reference's error string (what `Err(msg)` carries); raises DgError for bytes that are not a serialized StarkProof."""

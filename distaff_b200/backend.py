@@ -50,6 +50,11 @@ EXPORTS = {
     "dg_device_info": [ctypes.c_char_p, ctypes.c_size_t, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_size_t)],
     "dg_prove": [ctypes.POINTER(DgTrace), vp, u32, vp, u32, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(DgStats)],
     "dg_prove_device": [vp, u32, u64, u32, u32, vp, u32, vp, u32, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(DgStats)],
+    "dg_prove_batch": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                       ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_prove_batch_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                              ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
     "dg_verify": [vp, vp, u32, vp, u32, vp, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t],
     "dg_proof_serialized_len": [vp, ctypes.POINTER(ctypes.c_size_t)],
     "dg_proof_serialize": [vp, vp, ctypes.c_size_t],

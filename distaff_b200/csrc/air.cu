@@ -496,7 +496,8 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_kernel(cons
 // extra row BLOCK for the last thread).  Context / loop / user-stack registers are then addressed dynamically in shared memory instead
 // of in per-thread arrays, which the runtime loop bounds used to force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
 // STAGE_DEC: the 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
-template <int BLOCK, int MIN_BLOCKS, bool STAGE_DEC, bool WIDE_SLOTS>
+// BATCH: blockIdx.y is the proof of a batch (AirParams strides); a separate instantiation, so that one proof compiles as before.
+template <int BLOCK, int MIN_BLOCKS, bool STAGE_DEC, bool WIDE_SLOTS, bool BATCH = false>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel(const AirParams P) {
     extern __shared__ __align__(16) unsigned char air_smem[];
     fe *s_rows = reinterpret_cast<fe *>(air_smem);
@@ -513,8 +514,9 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     const int stride = 1 << (P.log_blowup - 3);
     const unsigned long long N = P.col_stride;                         // column stride of the local slab
     const unsigned long long lde_index = s * (unsigned long long)stride;   // = k*blowup + c8*stride
-    const fe *cur_p = P.ext + (c8_local * stride) * n + k;            // the slab starts at coset c8_base*stride
-    const fe *nxt_p = P.ext + (c8_local * stride) * n + ((k + 1) & (n - 1));
+    const fe *const ext = BATCH ? P.ext + blockIdx.y * P.ext_stride : P.ext;
+    const fe *cur_p = ext + (c8_local * stride) * n + k;              // the slab starts at coset c8_base*stride
+    const fe *nxt_p = ext + (c8_local * stride) * n + ((k + 1) & (n - 1));
     const unsigned long long out_idx = (c8_local << P.log_n) + k;
 
     const int cl = P.cl, ll = P.ll, sl = P.sl;
@@ -530,7 +532,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         if (tid < staged) {
             const unsigned long long gl = (unsigned long long)blockIdx.x * BLOCK + (BLOCK - 1);
             const unsigned long long cl8 = gl >> P.log_n, kl = gl & (n - 1);
-            s_rows[tid * PITCH + BLOCK] = P.ext[(unsigned long long)(S0 + tid) * N + (cl8 * stride) * n + ((kl + 1) & (n - 1))];
+            s_rows[tid * PITCH + BLOCK] = ext[(unsigned long long)(S0 + tid) * N + (cl8 * stride) * n + ((kl + 1) & (n - 1))];
         }
     }
     fe cur_dec[STAGE_DEC ? 1 : 15], nxt_dec[STAGE_DEC ? 1 : 15];
@@ -583,7 +585,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     acc.first = true;
 #pragma unroll
     for (int g = 0; g < 6; g++) acc.adj[g] = ZERO;
-    acc.cA = P.coefA; acc.cB = P.coefB; acc.nonzero = false;
+    acc.cA = BATCH ? P.coefA + blockIdx.y * P.coef_stride : P.coefA; acc.cB = BATCH ? P.coefB + blockIdx.y * P.coef_stride : P.coefB; acc.nonzero = false;
 
     const fe *per = P.per_override ? P.per_override : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
 
@@ -928,10 +930,10 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], P.xpow_override ? P.xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
     if (!P.verify_mode && c8 == 0 && k != n - 1) {
-        if (acc.nonzero && live) atomicExch(P.violation, (unsigned)(k + 1));
+        if (acc.nonzero && live) atomicExch(BATCH ? P.violation + blockIdx.y : P.violation, (unsigned)(k + 1));
         t_res = ZERO;
     }
-    if (live) P.t_ev[out_idx] = t_res;
+    if (live) (BATCH ? P.t_ev + blockIdx.y * P.t_ev_stride : P.t_ev)[out_idx] = t_res;
 }
 
 #undef DCUR
@@ -950,7 +952,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 #undef nsp
 #undef ncf
 
-void launch_constraint_eval(Context &c, const AirParams &P) {
+void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     air_upload_constants(c);
     const unsigned long long E = (unsigned long long)P.num_c8 << P.log_n;
     static int variant = -1;
@@ -963,11 +965,30 @@ void launch_constraint_eval(Context &c, const AirParams &P) {
         set_func_smem(c, (const void *)k, smem);                                                                                     \
         k<<<(unsigned)(E / BLOCK), BLOCK, smem, c.stream>>>(P);                                                                      \
     } while (0)
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "constraint evaluation batch out of range");
     int v = variant;
     const unsigned long long n = 1ULL << P.log_n;
     // the shared-memory variants need whole blocks inside one coset and at most ~200 KB of rows per block
     if (v < 5 || v > 7) v = 1;
     if (v >= 5 && (n < 128 || (size_t)P.w * 129 * sizeof(fe) > 200 * 1024)) v = 1;
+    if (batch > 1 && v == 7) {                      // the default variant: all proofs of the batch in one launch
+        const size_t smem = (size_t)P.w * 129 * sizeof(fe);
+        auto k = constraint_eval_smem_kernel<128, 4, true, true, true>;
+        set_func_smem(c, (const void *)k, smem);
+        k<<<dim3((unsigned)(E / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
+        c.launches++;
+        DG_CUDA(cudaGetLastError());
+        return;
+    }
+    if (batch > 1) {                                // other variants: one launch per proof
+        for (int q = 0; q < batch; q++) {
+            AirParams Q = P;
+            Q.ext += q * P.ext_stride; Q.t_ev += q * P.t_ev_stride;
+            Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride; Q.violation += q;
+            launch_constraint_eval(c, Q, 1);
+        }
+        return;
+    }
     // H100 SXM (700 W), stage 3 of the 2^20-step proof x 26 registers (tools/variant_bench.py): per-thread arrays (variant 1) 24.8 ms;
     // shared-memory rows, stack-like columns only (5) 23.7; all columns (6) 23.2; all columns + unreduced per-slot sums (7) 22.2
     switch (v) {

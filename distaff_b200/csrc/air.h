@@ -22,8 +22,13 @@ struct AirParams {
     int verify_mode;
     const fe *per_override;             // 23 values, or null
     const fe *xpow_override;            // 6 values, or null
+    // batched proving: proof q of the batch reads ext + q * ext_stride and coefA / coefB + q * coef_stride, writes t_ev + q * t_ev_stride
+    // and violation[q]
+    unsigned long long ext_stride, t_ev_stride, coef_stride;
 };
 
-void launch_constraint_eval(Context &c, const AirParams &P);
+// evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P); the default variant runs them in
+// one launch (blockIdx.y = proof), the measurement variants (DG_AIR_CFG != 7) launch once per proof
+void launch_constraint_eval(Context &c, const AirParams &P, int batch = 1);
 
 }  // namespace dg

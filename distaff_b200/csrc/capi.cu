@@ -8,7 +8,6 @@
 #include <thread>
 
 namespace dg {
-void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup);
 void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L);
 unsigned long long pow_search(Context &c, const uint8_t seed[32], unsigned grinding);
 void pow_hash(const uint8_t seed[32], unsigned long long nonce, uint8_t out[32]);
@@ -28,6 +27,7 @@ bool host_plan_verify_batch(const std::vector<uint64_t> &indexes, int depth, siz
 using namespace dg;
 
 static thread_local std::string t_last_error;
+static thread_local std::vector<std::string> t_batch_messages;     // per trace of the calling thread's last batched call
 
 template <typename F>
 static int guarded(F &&f) {
@@ -388,6 +388,39 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
         }
         *proof_out = (dg_proof_t *)prove_device(c, (const fe *)d_registers, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16,
                                                 n_outputs, *options, stats, 0.0f);
+    });
+}
+int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                   int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        prove_batch_host(c, traces, count, inputs16, n_inputs, outputs16, n_outputs, *options, (Proof **)proofs_out, status, t_batch_messages, stats);
+    });
+}
+int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                          const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                          const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(d_registers && options && proofs_out && status, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        prove_batch_device(c, (const fe *)d_registers, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+                           *options, (Proof **)proofs_out, status, t_batch_messages, stats);
+    });
+}
+int dg_batch_message(uint32_t index, char *message, size_t cap) {
+    return guarded([&] {
+        DG_REQUIRE(message && cap, "null argument");
+        DG_REQUIRE(index < t_batch_messages.size(), "no such trace in this thread's last batched call");
+        strncpy(message, t_batch_messages[index].c_str(), cap - 1);
+        message[cap - 1] = 0;
     });
 }
 int dg_set_rng_callbacks(const dg_rng_callbacks_t *callbacks) {

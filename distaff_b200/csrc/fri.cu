@@ -16,10 +16,14 @@
 
 namespace dg {
 
-__global__ void __launch_bounds__(256) fri_hash_rows_kernel(const fe *__restrict__ v, Layout in, Layout rows, uint4 *__restrict__ leaves) {
+// blockIdx.y = layer of a batch: values v_stride elements apart, leaves R digests apart
+__global__ void __launch_bounds__(256) fri_hash_rows_kernel(const fe *__restrict__ v, Layout in, Layout rows, uint4 *__restrict__ leaves,
+                                                            unsigned long long v_stride) {
     const unsigned long long R = 1ULL << rows.log_d;
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= R) return;
+    v += blockIdx.y * v_stride;
+    leaves += blockIdx.y * 2 * R;
     const unsigned long long r = rows.logical(t);
     uint32_t m[16], cv[8];
 #pragma unroll
@@ -31,9 +35,11 @@ __global__ void __launch_bounds__(256) fri_hash_rows_kernel(const fe *__restrict
     leaves[2 * r] = make_uint4(cv[0], cv[1], cv[2], cv[3]);
     leaves[2 * r + 1] = make_uint4(cv[4], cv[5], cv[6], cv[7]);
 }
-void fri_hash_rows(Context &c, const fe *values, Layout in, Layout rows, void *leaves) {
+void fri_hash_rows(Context &c, const fe *values, Layout in, Layout rows, void *leaves, int batch, unsigned long long values_stride) {
     const unsigned long long R = 1ULL << rows.log_d;
-    fri_hash_rows_kernel<<<(unsigned)((R + 255) / 256), 256, 0, c.stream>>>(values, in, rows, (uint4 *)leaves); c.launches++;
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "FRI batch out of range");
+    fri_hash_rows_kernel<<<dim3((unsigned)((R + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(values, in, rows, (uint4 *)leaves, values_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -42,8 +48,13 @@ void fri_hash_rows(Context &c, const fe *values, Layout in, Layout rows, void *l
 // draw by M with rejection of low halves > M - 1 -- the same steps as fs::Rng::field (host_fs.cu), which the CPU tests pin.
 __device__ __forceinline__ uint32_t rol32(uint32_t x, int n) { return (x << n) | (x >> (32 - n)); }
 #define DG_QRD(a, b, c, d) a += b; d = rol32(d ^ a, 16); c += d; b = rol32(b ^ c, 12); a += b; d = rol32(d ^ a, 8); c += d; b = rol32(b ^ c, 7);
-__global__ void fri_alpha_kernel(const uint32_t *__restrict__ root, fe *__restrict__ alpha, uint32_t *__restrict__ root_copy) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+// block b: the root root_stride words after block 0's, alpha[b], root_copy + 8 b
+__global__ void fri_alpha_kernel(const uint32_t *__restrict__ root, fe *__restrict__ alpha, uint32_t *__restrict__ root_copy,
+                                 unsigned long long root_stride) {
+    if (threadIdx.x != 0) return;
+    root += blockIdx.x * root_stride;
+    alpha += blockIdx.x;
+    root_copy += 8 * blockIdx.x;
     typedef unsigned __int128 u128;
     uint32_t key[8];
     for (int i = 0; i < 8; i++) { key[i] = root[i]; root_copy[i] = root[i]; }
@@ -77,17 +88,21 @@ __global__ void fri_alpha_kernel(const uint32_t *__restrict__ root, fe *__restri
         if (lo <= Mv - 1) { *alpha = fe_make((unsigned long long)hi, (unsigned long long)(hi >> 64)); return; }
     }
 }
-void fri_alpha(Context &c, const void *root_dev, fe *alpha_dev, void *root_copy_dev) {
-    fri_alpha_kernel<<<1, 32, 0, c.stream>>>((const uint32_t *)root_dev, alpha_dev, (uint32_t *)root_copy_dev); c.launches++;
+void fri_alpha(Context &c, const void *root_dev, fe *alpha_dev, void *root_copy_dev, int batch, unsigned long long root_stride_bytes) {
+    DG_REQUIRE(batch >= 1 && root_stride_bytes % 4 == 0, "FRI batch out of range");
+    fri_alpha_kernel<<<batch, 32, 0, c.stream>>>((const uint32_t *)root_dev, alpha_dev, (uint32_t *)root_copy_dev, root_stride_bytes / 4); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
+// blockIdx.y = layer of a batch: values v_stride elements apart, next R elements apart, folding point alpha_p[blockIdx.y]
 __global__ void __launch_bounds__(256) fri_fold_kernel(const fe *__restrict__ v, Layout in, fe *__restrict__ next, Layout out, const fe *__restrict__ alpha_p,
-                                                       TwiddleRef inv_root, int shift, fe tau_inv, fe inv4) {
-    const fe alpha = *alpha_p;
+                                                       TwiddleRef inv_root, int shift, fe tau_inv, fe inv4, unsigned long long v_stride) {
+    const fe alpha = alpha_p[blockIdx.y];
     const unsigned long long R = 1ULL << out.log_d;
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= R) return;
+    v += blockIdx.y * v_stride;
+    next += blockIdx.y * R;
     const unsigned long long r = out.logical(t);
     fe y0 = v[in.phys(r)], y1 = v[in.phys(r + R)], y2 = v[in.phys(r + 2 * R)], y3 = v[in.phys(r + 3 * R)];
     // x_r^-1 = (w_N^-1)^(r << shift)
@@ -102,10 +117,13 @@ __global__ void __launch_bounds__(256) fri_fold_kernel(const fe *__restrict__ v,
     next[t] = fe_mul(acc, inv4);
 }
 void fri_fold(Context &c, const fe *values, Layout in, fe *next, Layout out, const fe *alpha, const TwiddleRef &inv_root_table, int log_n_total,
-              fe tau_inv, fe inv4) {
+              fe tau_inv, fe inv4, int batch, unsigned long long values_stride) {
     const unsigned long long R = 1ULL << out.log_d;
     const int shift = log_n_total - in.log_d;            // layer domain is the 4^depth-th powers of the LDE domain
-    fri_fold_kernel<<<(unsigned)((R + 255) / 256), 256, 0, c.stream>>>(values, in, next, out, alpha, inv_root_table, shift, tau_inv, inv4); c.launches++;
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "FRI batch out of range");
+    fri_fold_kernel<<<dim3((unsigned)((R + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(values, in, next, out, alpha, inv_root_table, shift,
+                                                                                              tau_inv, inv4, values_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 

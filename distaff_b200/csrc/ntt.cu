@@ -265,8 +265,11 @@ void ntt_batch(Context &c, const fe *src, fe *dst, int log_n, int batch, size_t 
 // For all cosets together the inner sums are a b-point DFT of the zero-padded 8-vector: with c = (b/8) q + r it is, per residue r, a
 // twist by zeta^(r f) (7 multiplications) and an 8-point DFT over q (5 multiplications); the outer factor is a geometric progression in
 // q.  One thread per (r, j): 29 multiplications for 8 outputs instead of 72.  The result feeds b plain size-n transforms.
+// blockIdx.y = vector of a batch: src + y * src_stride in, dst + y * (b n) out.
 __global__ void __launch_bounds__(256) prefold8_kernel(const fe *__restrict__ src, fe *__restrict__ dst, int log_n, int log_b, const fe *__restrict__ zeta,
-                                                       TwiddleRef twN, fe w8, fe w8_2, fe w8_3) {
+                                                       TwiddleRef twN, fe w8, fe w8_2, fe w8_3, unsigned long long src_stride) {
+    src += blockIdx.y * src_stride;
+    dst += (unsigned long long)blockIdx.y << (log_n + log_b);
     const unsigned long long n = 1ULL << log_n;
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >> (log_n + log_b - 3)) return;
@@ -316,15 +319,18 @@ void lde_batch(Context &c, const fe *src, fe *dst, int log_n, int log_blowup, in
     DG_REQUIRE(coset0 < b && cosets <= b - coset0, "coset range out of bounds");
     static int prefold = -1;
     if (prefold < 0) { const char *e = getenv("DG_LDE_PREFOLD"); prefold = e ? atoi(e) : 1; }
-    if (prefold && fold == 8 && batch == 1 && cosets == (1u << log_blowup) && log_blowup >= 3 && log_blowup <= 8) {
-        // all cosets: input transform for every coset in one kernel, then b plain transforms (H100 SXM, 700 W, 2^20-step proof: stage 5 5.35 -> 3.83 ms, stage 6 5.83 -> 4.30 ms)
-        DevBuf pre((size_t)n * cosets * sizeof(fe));
+    if (prefold && fold == 8 && cosets == (1u << log_blowup) && log_blowup >= 3 && log_blowup <= 8 && (batch == 1 || dst_stride == n * cosets) &&
+        batch <= 65535) {
+        // all cosets: input transform for every coset in one kernel, then b plain transforms (H100 SXM, 700 W, 2^20-step proof: stage 5 5.35 -> 3.83 ms, stage 6 5.83 -> 4.30 ms);
+        // a batch of vectors whose outputs are contiguous runs both steps once for all of them
+        DevBuf pre((size_t)n * cosets * batch * sizeof(fe));
         const fe w8 = host_root_of_unity(3), w8_2 = fe_mul(w8, w8);
         const unsigned long long threads = (unsigned long long)n << (log_blowup - 3);
-        prefold8_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c.stream>>>(src, pre.as<fe>(), log_n, log_blowup, c.single_table(log_blowup),
-                                                                                 c.twiddle(log_n + log_blowup, false), w8, w8_2, fe_mul(w8_2, w8)); c.launches++;
+        prefold8_kernel<<<dim3((unsigned)((threads + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(
+            src, pre.as<fe>(), log_n, log_blowup, c.single_table(log_blowup), c.twiddle(log_n + log_blowup, false), w8, w8_2, fe_mul(w8_2, w8),
+            (unsigned long long)src_stride); c.launches++;
         DG_CUDA(cudaGetLastError());
-        ntt_batch(c, pre.as<fe>(), dst, log_n, (int)cosets, n, n, false);
+        ntt_batch(c, pre.as<fe>(), dst, log_n, (int)cosets * batch, n, n, false);
         return;
     }
     // scratch of the two-pass transforms: one intermediate of n * cosets elements per vector; more vectors per launch = fewer passes over

@@ -24,6 +24,36 @@ __global__ void pow_fill_kernel(fe *lo, fe base, unsigned long long lo_n, fe *hi
     else if (i < lo_n + hi_n) hi[i - lo_n] = fe_pow_u64(step, i - lo_n);
 }
 
+// table q = blockIdx.y: (base, step) = bs[2q], bs[2q + 1], written to lo + q lo_n and hi + q hi_n
+__global__ void pow_fill_batch_kernel(fe *lo, unsigned long long lo_n, fe *hi, unsigned long long hi_n, const fe *__restrict__ bs) {
+    const fe base = bs[2 * blockIdx.y], step = bs[2 * blockIdx.y + 1];
+    lo += blockIdx.y * lo_n;
+    hi += blockIdx.y * hi_n;
+    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < lo_n) lo[i] = fe_pow_u64(base, i);
+    else if (i < lo_n + hi_n) hi[i - lo_n] = fe_pow_u64(step, i - lo_n);
+}
+
+static int pow_lo_bits(unsigned long long len) {
+    int lo_bits = 1;
+    while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
+    return lo_bits;
+}
+
+fe PowTables::step(fe base, unsigned long long len) { return fe_pow_u64(base, 1ULL << pow_lo_bits(len)); }
+
+PowTables::PowTables(Context &c, const fe *base_step, int batch, unsigned long long len) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "power table batch out of range");
+    lo_bits = pow_lo_bits(len);
+    lo_n = 1ULL << lo_bits;
+    hi_n = (len + lo_n - 1) / lo_n + 1;
+    lo.alloc(lo_n * batch * sizeof(fe));
+    hi.alloc(hi_n * batch * sizeof(fe));
+    pow_fill_batch_kernel<<<dim3((unsigned)((lo_n + hi_n + 127) / 128), (unsigned)batch), 128, 0, c.stream>>>(lo.as<fe>(), lo_n, hi.as<fe>(), hi_n, base_step);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
 PowTable::PowTable(Context &c, fe base, unsigned long long len) {
     lo_bits = 1;
     while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
@@ -140,14 +170,30 @@ __device__ __forceinline__ void st_cg_fe(fe *p, fe v) {
     __stcg(reinterpret_cast<uint4 *>(p), make_uint4((unsigned)v.lo, (unsigned)(v.lo >> 32), (unsigned)v.hi, (unsigned)(v.hi >> 32)));
 }
 
+// BATCH: `batch` vectors in one launch (SynDivBatch strides); one ticket counter over all their blocks, ticket t = (vector t / nblocks,
+// block nblocks - 1 - t % nblocks): a block only waits on blocks of its own vector with smaller tickets, so the look-back keeps its
+// forward-progress guarantee.  A separate instantiation, so that one vector compiles as before.
+struct SynDivBatch { unsigned long long in_stride, out_stride, b_stride_lo, b_stride_hi, binv_stride_lo, binv_stride_hi; const fe *sub0; };
+template <bool BATCH>
 __global__ void __launch_bounds__(SCAN_THREADS) syn_div_chained_kernel(const fe *__restrict__ in, fe *__restrict__ out, unsigned long long len, PowRef bp,
-                                                                       PowRef binvp, fe sub0, ScanDesc *desc, unsigned *ticket, unsigned nblocks) {
+                                                                       PowRef binvp, fe sub0, ScanDesc *desc, unsigned *ticket, unsigned nblocks,
+                                                                       SynDivBatch sb) {
     __shared__ fe s_warp[SCAN_THREADS / 32];
     __shared__ fe s_carry;
     __shared__ unsigned s_ticket;
     if (threadIdx.x == 0) s_ticket = atomicAdd(ticket, 1u);
     __syncthreads();
-    const unsigned blk = nblocks - 1u - s_ticket;
+    unsigned t = s_ticket;
+    if constexpr (BATCH) {
+        const unsigned q = t / nblocks;
+        t -= q * nblocks;
+        in += q * sb.in_stride; out += q * sb.out_stride;
+        bp.lo += q * sb.b_stride_lo; bp.hi += q * sb.b_stride_hi;
+        binvp.lo += q * sb.binv_stride_lo; binvp.hi += q * sb.binv_stride_hi;
+        sub0 = sb.sub0[q];
+        desc += (unsigned long long)q * nblocks;
+    }
+    const unsigned blk = nblocks - 1u - t;
     const unsigned long long base = (unsigned long long)blk * SCAN_BLOCK + (unsigned long long)threadIdx.x * SCAN_PER_THREAD;
     fe x[SCAN_PER_THREAD];
     fe v = fe_make(0, 0);
@@ -215,7 +261,8 @@ void syn_div(Context &c, const fe *in, fe *out, fe *scratch, unsigned long long 
         DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
         ScanDesc *desc = d.as<ScanDesc>();
         unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk);
-        syn_div_chained_kernel<<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, sub0, desc, ticket, (unsigned)nblk); c.launches++;
+        syn_div_chained_kernel<false><<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, sub0, desc, ticket, (unsigned)nblk,
+                                                                                    SynDivBatch{}); c.launches++;
         DG_CUDA(cudaGetLastError());
         return;
     }
@@ -227,11 +274,40 @@ void syn_div(Context &c, const fe *in, fe *out, fe *scratch, unsigned long long 
     DG_CUDA(cudaGetLastError());
 }
 
+void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, fe *scratch,
+                   unsigned long long len, const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
+                   unsigned long long binv_lo_stride, unsigned long long binv_hi_stride, const fe *sub0_dev, const fe *sub0_host) {
+    static int chained = -1;
+    if (chained < 0) { const char *e = getenv("DG_SCAN_CHAINED"); chained = e ? atoi(e) : 1; }
+    if (!chained || batch == 1) {             // the multi-pass form (measurement only), or one vector: one syn_div per vector
+        for (int q = 0; q < batch; q++) {
+            PowRef b = b_pows, bi = binv_pows;
+            b.lo += q * b_lo_stride; b.hi += q * b_hi_stride; bi.lo += q * binv_lo_stride; bi.hi += q * binv_hi_stride;
+            syn_div(c, in + q * in_stride, out + q * out_stride, scratch, len, b, bi, sub0_host[q]);
+        }
+        return;
+    }
+    const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
+    DG_REQUIRE(nblk * batch < (1ULL << 31), "division batch too large for one launch");
+    DevBuf d((size_t)nblk * batch * sizeof(ScanDesc) + 16);
+    DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
+    ScanDesc *desc = d.as<ScanDesc>();
+    unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk * batch);
+    const SynDivBatch sb{in_stride, out_stride, b_lo_stride, b_hi_stride, binv_lo_stride, binv_hi_stride, sub0_dev};
+    syn_div_chained_kernel<true><<<(unsigned)(nblk * batch), SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, fe_make(0, 0), desc, ticket,
+                                                                                          (unsigned)nblk, sb); c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
 // ---- division by (x^n - 1) / (x - e) -----------------------------------------------------------------------------------------------------
 // s[i + m n] = sum_{m' >= m} a[i + m' n]
-__global__ void strided_suffix_kernel(const fe *__restrict__ a, fe *__restrict__ s, unsigned long long n, int blocks_m) {
+// blockIdx.y = vector of a batch, a_stride / s_stride elements apart
+__global__ void strided_suffix_kernel(const fe *__restrict__ a, fe *__restrict__ s, unsigned long long n, int blocks_m, unsigned long long a_stride,
+                                      unsigned long long s_stride) {
     unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    a += blockIdx.y * a_stride;
+    s += blockIdx.y * s_stride;
     fe run = fe_make(0, 0);
     for (int m = blocks_m - 1; m >= 0; m--) {
         run = fe_add(run, a[i + (unsigned long long)m * n]);
@@ -239,10 +315,16 @@ __global__ void strided_suffix_kernel(const fe *__restrict__ a, fe *__restrict__
     }
 }
 // out[idx] = s[idx+n-1] - e * s[idx+n]  for idx <= len-n (with s[len] = 0), else 0 ; optionally accumulated: out = base0 + base1 + that
+// blockIdx.y = vector of a batch: s at s_stride, add0 / add1 at in_stride, out at out_stride elements apart
 __global__ void expanded_stencil_kernel(const fe *__restrict__ s, const fe *__restrict__ add0, const fe *__restrict__ add1, fe *__restrict__ out,
-                                        unsigned long long n, unsigned long long len, fe e) {
+                                        unsigned long long n, unsigned long long len, fe e, unsigned long long s_stride, unsigned long long in_stride,
+                                        unsigned long long out_stride) {
     unsigned long long idx = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= len) return;
+    s += blockIdx.y * s_stride;
+    if (add0) add0 += blockIdx.y * in_stride;
+    if (add1) add1 += blockIdx.y * in_stride;
+    out += blockIdx.y * out_stride;
     fe v = fe_make(0, 0);
     if (idx <= len - n) {
         v = s[idx + n - 1];
@@ -252,20 +334,30 @@ __global__ void expanded_stencil_kernel(const fe *__restrict__ s, const fe *__re
     if (add1) v = fe_add(v, add1[idx]);
     out[idx] = v;
 }
-void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, const fe *add1, fe *out, unsigned long long n, unsigned long long len, fe e) {
-    strided_suffix_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(a, scratch, n, (int)(len / n)); c.launches++;
-    expanded_stencil_kernel<<<(unsigned)((len + 255) / 256), 256, 0, c.stream>>>(scratch, add0, add1, out, n, len, e); c.launches++;
+void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, const fe *add1, fe *out, unsigned long long n, unsigned long long len, fe e,
+                          int batch, unsigned long long in_stride, unsigned long long out_stride) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "division batch out of range");
+    strided_suffix_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(a, scratch, n, (int)(len / n), in_stride, len);
+    c.launches++;
+    expanded_stencil_kernel<<<dim3((unsigned)((len + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(scratch, add0, add1, out, n, len, e, len, in_stride,
+                                                                                                        out_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
 // ---- evaluation of many polynomials at two points (DEEP values) -----------------------------------------------------------------------------
 // partial[(col*2 + p) * chunks + chunk] = sum_{k in chunk} poly[col][k] * x_p^k,  x_0 = z (table zt), x_1 = z*g (zt * gt)
 static const int EVAL_CHUNK = 4096;
+// columns of a batch: column col uses the table of its proof col / cols_per_proof, zt_stride_lo / zt_stride_hi elements apart
 __global__ void __launch_bounds__(256) eval2_partial_kernel(const fe *__restrict__ polys, unsigned long long n, PowRef zt, TwiddleRef gt, fe *__restrict__ partial,
-                                                            int two_points) {
+                                                            int two_points, unsigned cols_per_proof, unsigned long long zt_stride_lo,
+                                                            unsigned long long zt_stride_hi) {
     __shared__ fe s_warp[2][8];
     const unsigned long long col = blockIdx.y, chunk = blockIdx.x, chunks = gridDim.x;
     const fe *p = polys + col * n;
+    const unsigned q = blockIdx.y / cols_per_proof;
+    zt.lo += q * zt_stride_lo;
+    zt.hi += q * zt_stride_hi;
     fe a0 = fe_make(0, 0), a1 = fe_make(0, 0);
     for (int u = 0; u < EVAL_CHUNK / 256; u++) {
         unsigned long long k = chunk * EVAL_CHUNK + (unsigned long long)u * 256 + threadIdx.x;
@@ -303,20 +395,27 @@ __global__ void reduce_partials_kernel(const fe *__restrict__ partial, fe *__res
     if (threadIdx.x == 0) out[o] = a;
 }
 // out[col*2 + p] = poly_col(x_p)
-void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, const PowRef &zt, const TwiddleRef &gt, bool two_points, fe *out) {
+void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, const PowRef &zt, const TwiddleRef &gt, bool two_points, fe *out,
+                   int cols_per_proof, unsigned long long zt_stride_lo, unsigned long long zt_stride_hi) {
     const unsigned chunks = (unsigned)((n + EVAL_CHUNK - 1) / EVAL_CHUNK);
+    DG_REQUIRE(cols >= 1 && cols <= 65535 && cols_per_proof >= 1, "too many polynomials for one launch");
     DevBuf partial((size_t)cols * 2 * chunks * sizeof(fe));
-    eval2_partial_kernel<<<dim3(chunks, cols), 256, 0, c.stream>>>(polys, n, zt, gt, partial.as<fe>(), two_points ? 1 : 0); c.launches++;
+    eval2_partial_kernel<<<dim3(chunks, cols), 256, 0, c.stream>>>(polys, n, zt, gt, partial.as<fe>(), two_points ? 1 : 0, (unsigned)cols_per_proof,
+                                                                   zt_stride_lo, zt_stride_hi); c.launches++;
     reduce_partials_kernel<<<cols * 2, 32, 0, c.stream>>>(partial.as<fe>(), out, chunks); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
 // ---- linear combinations ------------------------------------------------------------------------------------------------------------------
 // t1[k] = sum_i cc1[i] P_i[k],  t2[k] = sum_i cc2[i] P_i[k]
+// blockIdx.y = proof of a batch: polys w n, cc1 / cc2 cc_stride, t1 / t2 t_stride elements apart
 __global__ void lincomb2_kernel(const fe *__restrict__ polys, unsigned long long n, int w, const fe *__restrict__ cc1, const fe *__restrict__ cc2,
-                                fe *__restrict__ t1, fe *__restrict__ t2) {
+                                fe *__restrict__ t1, fe *__restrict__ t2, unsigned long long cc_stride, unsigned long long t_stride) {
     unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
+    polys += blockIdx.y * (unsigned long long)w * n;
+    cc1 += blockIdx.y * cc_stride; cc2 += blockIdx.y * cc_stride;
+    t1 += blockIdx.y * t_stride; t2 += blockIdx.y * t_stride;
     // w < 128 products per sum: accumulated unreduced (288 bits), one reduction each (fp128.cuh: fe_wide)
     fe_wide a, b;
     for (int i = 0; i < w; i++) {
@@ -326,8 +425,11 @@ __global__ void lincomb2_kernel(const fe *__restrict__ polys, unsigned long long
     }
     t1[k] = DG_REDUCE_WIDE(a); t2[k] = DG_REDUCE_WIDE(b);
 }
-void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe *cc1, const fe *cc2, fe *t1, fe *t2) {
-    lincomb2_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(polys, n, w, cc1, cc2, t1, t2); c.launches++;
+void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe *cc1, const fe *cc2, fe *t1, fe *t2, int batch,
+              unsigned long long cc_stride, unsigned long long t_stride) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "linear combination batch out of range");
+    lincomb2_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, w, cc1, cc2, t1, t2, cc_stride, t_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -337,10 +439,19 @@ void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe
 //   I = (sum_j a_j T_j - Ka) + x^adj (sum_j b_j T_j - Kb),     Ka = sum_j a_j in_j,  Kb = sum_j b_j in_j
 // whose coefficients are two linear combinations of the trace polynomials' coefficients: n*nb multiplications instead of 8n*nb.
 // coef = [a_init | b_init | a_final | b_final], nb entries each; ic / fc receive the 8n coefficients of the first / last step numerators.
+// BATCH: blockIdx.y = proof of a batch: polys poly_stride, coef coef_stride, ic / fc out_stride elements apart, its constants
+// K[4 y .. 4 y + 4) instead of the by-value ones (a separate instantiation, so that one proof compiles as before)
+template <bool BATCH>
 __global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned long long n, int nb, const fe *__restrict__ coef, fe KiA, fe KiB,
-                                       fe KfA, fe KfB, unsigned long long adj, fe *__restrict__ ic, fe *__restrict__ fc) {
+                                       fe KfA, fe KfB, unsigned long long adj, fe *__restrict__ ic, fe *__restrict__ fc, const fe *__restrict__ K,
+                                       unsigned long long poly_stride, unsigned long long coef_stride, unsigned long long out_stride) {
     const unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
+    if constexpr (BATCH) {
+        polys += blockIdx.y * poly_stride; coef += blockIdx.y * coef_stride;
+        ic += blockIdx.y * out_stride; fc += blockIdx.y * out_stride;
+        KiA = K[4 * blockIdx.y]; KiB = K[4 * blockIdx.y + 1]; KfA = K[4 * blockIdx.y + 2]; KfB = K[4 * blockIdx.y + 3];
+    }
     // nb < 128 products per sum: accumulated unreduced (288 bits), one reduction each
     fe_wide wa, wb, wc, wd;
     for (int j = 0; j < nb; j++) {
@@ -363,7 +474,19 @@ __global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned lo
         if (q < adj || q >= adj + n) { ic[q] = zero; fc[q] = zero; }
 }
 void boundary_coeffs(Context &c, const fe *polys, unsigned long long n, int nb, const fe *coef, fe KiA, fe KiB, fe KfA, fe KfB, fe *ic, fe *fc) {
-    boundary_coeffs_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(polys, n, nb, coef, KiA, KiB, KfA, KfB, 6 * n + 2, ic, fc); c.launches++;
+    boundary_coeffs_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(polys, n, nb, coef, KiA, KiB, KfA, KfB, 6 * n + 2, ic, fc, nullptr, 0,
+                                                                                      0, 0);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+void boundary_coeffs_batch(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
+                           unsigned long long coef_stride, const fe *K, const fe *K_host, fe *ic, fe *fc, unsigned long long out_stride) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "boundary batch out of range");
+    if (batch == 1) { boundary_coeffs(c, polys, n, nb, coef, K_host[0], K_host[1], K_host[2], K_host[3], ic, fc); return; }
+    const fe z = fe_make(0, 0);
+    boundary_coeffs_kernel<true><<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, nb, coef, z, z, z, z, 6 * n + 2, ic, fc, K,
+                                                                                                      poly_stride, coef_stride, out_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -373,9 +496,13 @@ void boundary_coeffs(Context &c, const fe *polys, unsigned long long n, int nb, 
 // factor w_E^(c m0) and runs the 8-point inverse DFT across the cosets.  Output: the 8n coefficients in natural order, exactly what
 // interpolate_fft of the natural-order evaluation vector returns (constraint_table.rs:54-63) -- no transposition, no 8n-point transform.
 // b: [8][n]; tw: powers of w_E^-1; w8i[j] = w_8^-j, j = 1..3; inv8 = 1/8.
-__global__ void coset_interp_finish_kernel(const fe *__restrict__ b, fe *__restrict__ out, unsigned long long n, TwiddleRef tw, fe w8i1, fe w8i2, fe w8i3, fe inv8) {
+// blockIdx.y = vector of a batch: b b_stride, out out_stride elements apart
+__global__ void coset_interp_finish_kernel(const fe *__restrict__ b, fe *__restrict__ out, unsigned long long n, TwiddleRef tw, fe w8i1, fe w8i2, fe w8i3, fe inv8,
+                                           unsigned long long b_stride, unsigned long long out_stride) {
     const unsigned long long m0 = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (m0 >= n) return;
+    b += blockIdx.y * b_stride;
+    out += blockIdx.y * out_stride;
     fe x[8];
     x[0] = fe_mul(b[m0], inv8);
 #pragma unroll
@@ -403,22 +530,31 @@ __global__ void coset_interp_finish_kernel(const fe *__restrict__ b, fe *__restr
 #pragma unroll
     for (int m1 = 0; m1 < 8; m1++) out[m0 + n * (unsigned long long)m1] = X[m1];
 }
-void coset_interp_finish(Context &c, const fe *b, fe *out, int log_n) {
+void coset_interp_finish(Context &c, const fe *b, fe *out, int log_n, int batch, unsigned long long b_stride, unsigned long long out_stride) {
     const unsigned long long n = 1ULL << log_n;
     const fe w8i = host_inv(host_root_of_unity(3));
     const fe w8i2 = fe_mul(w8i, w8i);
-    coset_interp_finish_kernel<<<(unsigned)((n + 127) / 128), 128, 0, c.stream>>>(b, out, n, c.twiddle(log_n + 3, true), w8i, w8i2, fe_mul(w8i2, w8i),
-                                                                              host_inv(fe_make(8, 0)));
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "interpolation batch out of range");
+    coset_interp_finish_kernel<<<dim3((unsigned)((n + 127) / 128), (unsigned)batch), 128, 0, c.stream>>>(
+        b, out, n, c.twiddle(log_n + 3, true), w8i, w8i2, fe_mul(w8i2, w8i), host_inv(fe_make(8, 0)), b_stride, out_stride);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
 // composition polynomial (trace_table.rs:241-258, constraint_poly.rs:49):
 //   comp[k] = cq[k]*kc + [k < n] (t1q[k]+t2q[k])*k1 + [inc <= k < inc+n] (t1q[k-inc]+t2q[k-inc])*k2
+// BATCH: blockIdx.y = proof of a batch: t1q / t2q t_stride, cq / comp len elements apart, its k1, k2, kc = ks[3 y ..] instead of the by-value ones
+template <bool BATCH>
 __global__ void compose_kernel(const fe *__restrict__ t1q, const fe *__restrict__ t2q, const fe *__restrict__ cq, fe *__restrict__ comp,
-                               unsigned long long n, unsigned long long len, unsigned long long inc, fe k1, fe k2, fe kc) {
+                               unsigned long long n, unsigned long long len, unsigned long long inc, fe k1, fe k2, fe kc, const fe *__restrict__ ks,
+                               unsigned long long t_stride) {
     unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= len) return;
+    if constexpr (BATCH) {
+        t1q += blockIdx.y * t_stride; t2q += blockIdx.y * t_stride;
+        cq += blockIdx.y * len; comp += blockIdx.y * len;
+        k1 = ks[3 * blockIdx.y]; k2 = ks[3 * blockIdx.y + 1]; kc = ks[3 * blockIdx.y + 2];
+    }
     fe v = fe_mul(cq[k], kc);
     if (k < n) v = fe_add(v, fe_mul(fe_add(t1q[k], t2q[k]), k1));
     if (k >= inc && k < inc + n) v = fe_add(v, fe_mul(fe_add(t1q[k - inc], t2q[k - inc]), k2));
@@ -426,7 +562,16 @@ __global__ void compose_kernel(const fe *__restrict__ t1q, const fe *__restrict_
 }
 void compose(Context &c, const fe *t1q, const fe *t2q, const fe *cq, fe *comp, unsigned long long n, unsigned long long len, unsigned long long inc,
              fe k1, fe k2, fe kc) {
-    compose_kernel<<<(unsigned)((len + 255) / 256), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, k1, k2, kc); c.launches++;
+    compose_kernel<false><<<(unsigned)((len + 255) / 256), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, k1, k2, kc, nullptr, 0); c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+void compose_batch(Context &c, int batch, const fe *t1q, const fe *t2q, unsigned long long t_stride, const fe *cq, fe *comp, unsigned long long n,
+                   unsigned long long len, unsigned long long inc, const fe *ks, const fe *ks_host) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "composition batch out of range");
+    if (batch == 1) { compose(c, t1q, t2q, cq, comp, n, len, inc, ks_host[0], ks_host[1], ks_host[2]); return; }
+    const fe z = fe_make(0, 0);
+    compose_kernel<true><<<dim3((unsigned)((len + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, z, z, z, ks, t_stride);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 

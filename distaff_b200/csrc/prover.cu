@@ -118,7 +118,8 @@ void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, 
 }
 
 struct FriLayerDev {
-    DevBuf leaves, nodes, folded;     // row hashes, tree, and the folded values (= values of the next layer)
+    DevBuf leaves, nodes, folded;     // sharded layer: row hashes, tree and folded values of this rank
+    const void *leaves_p = nullptr, *nodes_p = nullptr;     // replicated layer: row hashes and tree (buffers shared by the batch's proofs)
     const fe *vals;                   // replicated layer: the whole vector; sharded layer: this rank's cosets [c - c0][k]
     Layout layout;                    // layout of the (whole) layer (domain size 2^layout.log_d)
     bool sharded = false;             // multi-GPU: rows hashed / folded per coset range, tree = ShardedTree over [k'][c - c0] items
@@ -218,13 +219,66 @@ private:
     std::vector<std::thread> workers_;
 };
 
-// d_regs: register traces in device memory; when `host_cols` is given they are not there yet: column chunks are uploaded on the
-// copy stream while the previous chunk is being interpolated and extended (the upload hides behind the LDE)
-static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth,
-                         uint32_t loop_depth, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
-                         const dg_options_t &opt, dg_prove_stats_t *stats) {
+namespace {
+
+typedef std::vector<std::vector<size_t>> Offsets;
+
+// Per-proof host state of a batch.  A proof that fails (unsatisfied constraints, exhausted query positions) is marked dead and
+// takes part in no later host-side work; its device lanes in the batched transforms keep computing on meaningless values.
+struct ProofState {
+    bool live = true;
+    int status = DG_OK;
+    std::string message;
+    std::unique_ptr<Proof> proof{new Proof()};
+    std::vector<fe> inputs, outputs;
+    fe op_count;
+    fs::ConstraintCoefficients cc;
+    fs::CompositionCoefficients dc;
+    std::vector<fe> state1, state2;
+    ShardedTree t_tree, c_tree;
+    std::vector<FriLayerDev> layers;
+    std::vector<uint64_t> positions;
+    void fail(int code, const std::string &m) { live = false; status = code; message = m; }
+};
+
+// the 32-byte roots at `roots_dev` on the host: one copy for one tree, one FetchBatch for many
+std::vector<Digest> fetch_roots(Context &c, const std::vector<const void *> &roots_dev) {
+    std::vector<Digest> out(roots_dev.size());
+    if (roots_dev.size() == 1) {
+        d2h(c, out[0].data(), roots_dev[0], 32);
+        return out;
+    }
+    FetchBatch fb(c);
+    std::vector<size_t> off;
+    for (const void *r : roots_dev) off.push_back(fb.add32(FetchRef{r, 0, -1}));
+    fb.run();
+    for (size_t i = 0; i < off.size(); i++) out[i] = fb.digest(off[i]);
+    return out;
+}
+
+// everything a proof opens, as offsets into the batch's FetchBatch (stage 9)
+struct LayerOpen { std::vector<uint64_t> pos; std::vector<size_t> val_off; Offsets node_off; uint8_t depth; };
+struct OpenPlan {
+    std::vector<size_t> row_off;
+    fs::BatchPlan tplan, cplan;
+    Offsets t_off, c_off;
+    std::vector<size_t> cval_off, rem_off;
+    std::vector<LayerOpen> fri_open;
+};
+
+}  // namespace
+
+// Proves K traces of one shape (K == 1: dg_prove / dg_prove_device).  Every device buffer is proof-major ([K][...] with the single-proof
+// layout inside), so the transforms run once over the K proofs' columns, and each host round trip (violation flags, roots, DEEP values,
+// FRI roots, PoW, openings) moves the values of all K proofs at once.
+// d_regs: register traces in device memory, [K][w][n]; when `host_cols` (K * w column pointers) is given they are not there yet: column
+// chunks are uploaded on the copy stream while the previous chunk is being interpolated and extended (the upload hides behind the LDE).
+static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, int K, uint32_t width, uint64_t length, uint32_t ctx_depth,
+                       uint32_t loop_depth, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats) {
     // ---- argument checks (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) -----------------------------------------------
     const uint64_t n = length, b = opt.extension_factor;
+    DG_REQUIRE(K >= 1 && (int)ps.size() == K, "batch must hold at least one trace");
+    DG_REQUIRE((uint64_t)K * width <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
     DG_REQUIRE(opt.hash_id == 0, "unsupported hash function (only blake3 is serialisable, options.rs:107)");
     DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
     DG_REQUIRE(opt.num_queries > 0 && opt.num_queries <= 128, "num_queries must be in 1..128");
@@ -234,33 +288,36 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
     DG_REQUIRE(loop_depth <= 8, "loop depth cannot be greater than 8");
     DG_REQUIRE(width < 128, "execution trace cannot have more than 128 registers");
     DG_REQUIRE(width > 15 + ctx_depth + loop_depth, "user stack must consist of at least one register");
-    DG_REQUIRE(n_inputs <= 8 && n_outputs <= 8, "cannot have more than 8 public inputs / outputs");
+    for (auto &s : ps) DG_REQUIRE(s.inputs.size() <= 8 && s.outputs.size() <= 8, "cannot have more than 8 public inputs / outputs");
     const int w = (int)width, log_n = ilog2(n), log_b = ilog2(b), log_N = log_n + log_b;
     DG_REQUIRE(log_N <= 30, "LDE domain too large");
     const uint64_t N = n * b, E = n * 8;
     const int stack_depth = w - 15 - (int)ctx_depth - (int)loop_depth;
     DG_REQUIRE(stack_depth <= 32, "stack depth cannot be greater than 32");
-    std::vector<fe> inputs(n_inputs), outputs(n_outputs);
-    if (n_inputs) memcpy(inputs.data(), inputs16, n_inputs * 16);
-    if (n_outputs) memcpy(outputs.data(), outputs16, n_outputs * 16);
+    auto any_live = [&] { for (auto &s : ps) if (s.live) return true; return false; };
 
     ArenaScope arena_scope;                   // all DevBufs below come from the per-proof arena (no driver allocation inside a proof)
     StageClock clk(c.stream);
     SubClock sub(c.stream);
     if (sub.on) c.mark = [&sub](const char *name) { sub.mark(name); }; else c.mark = nullptr;
     struct MarkReset { Context &c; ~MarkReset() { c.mark = nullptr; } } mark_reset{c};
+    // the proofs' trees and FRI layers come from the arena too: release them before the arena scope closes
+    struct DeviceStateReset {
+        std::vector<ProofState> &ps;
+        ~DeviceStateReset() { for (auto &s : ps) { s.t_tree = ShardedTree(); s.c_tree = ShardedTree(); s.layers.clear(); } }
+    } state_reset{ps};
     const unsigned long long launches0 = c.launches;
-    Proof *proof = new Proof();
-    std::unique_ptr<Proof> guard(proof);
 
     // ---- sharding: rank g owns the LDE cosets [c0, c0 + nc) of every column (world == 1: all of them) ------------------------------
     const int G = c.world, g = c.rank;
+    DG_REQUIRE(G == 1 || K == 1, "a batch of proofs runs on one GPU (the context spans several)");
     int log_g = 0;
     while ((1 << log_g) < G) log_g++;
     DG_REQUIRE((b >> log_g) >= 4 && G <= 8, "extension factor too small for this many GPUs (need >= 4 cosets per rank)");
     const int log_nc = log_b - log_g;
     const uint64_t nc = 1ULL << log_nc, N_loc = n * nc;
     const unsigned c0 = (unsigned)(g * nc);
+    const size_t W = (size_t)K * w;                            // columns of the whole batch
 
     // ---- 1: extend execution trace ---------------------------------------------------------------------------------------------------
     clk.mark(0);
@@ -272,17 +329,18 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
     const int cpr = (w + G - 1) / G;                           // slot size of the gather = largest share
     auto col_count = [&](int r) { return w / G + (r < w % G ? 1 : 0); };
     auto col_start = [&](int r) { return r * (w / G) + std::min(r, w % G); };
-    DevBuf polys((size_t)w * n * 16), ext((size_t)w * N_loc * 16);
+    DevBuf polys(W * n * 16), ext(W * N_loc * 16);
     if (G == 1) {
+        // the K proofs' registers are K * w columns of one batch
         if (!host_cols) {
-            ntt_batch(c, d_regs, polys.as<fe>(), log_n, w, n, n, true);
-            extend_trace_columns(c, polys.as<fe>(), d_regs, ext.as<fe>(), w, log_n, log_b, N_loc, c0, (unsigned)nc);
+            ntt_batch(c, d_regs, polys.as<fe>(), log_n, (int)W, n, n, true);
+            extend_trace_columns(c, polys.as<fe>(), d_regs, ext.as<fe>(), (int)W, log_n, log_b, N_loc, c0, (unsigned)nc);
         } else {
             // chunks of ~64 MB, but a short ramp first (1, 2 columns): the first transform starts after one column's worth of copying
-            const int chunk = (int)std::max<uint64_t>(1, std::min<uint64_t>(w, ((uint64_t)1 << 26) / (n * 16)));
+            const int chunk = (int)std::max<uint64_t>(1, std::min<uint64_t>(W, ((uint64_t)1 << 26) / (n * 16)));
             std::vector<int> bounds = {0};
-            for (int step = 1; bounds.back() < w; step = std::min(chunk, step * 2)) bounds.push_back(std::min(w, bounds.back() + step));
-            TraceUploader up(c, d_regs, host_cols, w, n, bounds);
+            for (int step = 1; bounds.back() < (int)W; step = std::min(chunk, step * 2)) bounds.push_back(std::min((int)W, bounds.back() + step));
+            TraceUploader up(c, d_regs, host_cols, (int)W, n, bounds);
             for (int i = 0; i < up.chunks(); i++) {
                 const int j0 = bounds[i], cols = bounds[i + 1] - j0;
                 up.wait_chunk(i);
@@ -333,32 +391,45 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
         cudaEventDestroy(ev_own);
         cudaEventDestroy(ev_all);
     }
+    auto ext_of = [&](int p) { return ext.as<fe>() + (size_t)p * w * N_loc; };
 
     // ---- 2: trace Merkle tree ----------------------------------------------------------------------------------------------------------
     clk.mark(1);
     sub.mark("1.lde");
-    DevBuf t_leaves(N_loc * 32);
-    hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc);          // local rows, [k][c - c0]
+    DevBuf t_leaves((size_t)K * N_loc * 32), t_nodes;
+    hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, (size_t)w * N_loc);      // local rows, [k][c - c0], per proof
     sub.mark("2.hash_rows");
-    ShardedTree t_tree;
-    t_tree.build(c, t_leaves.p, n, log_nc);
-    memcpy(proof->trace_root, t_tree.root.data(), 32);
+    {
+        // one GPU: the K trees level by level in one launch per level; several GPUs (K == 1): the sharded tree
+        if (G == 1) {
+            t_nodes.alloc((size_t)K * N_loc * 32);
+            merkle_build_batch(c, t_leaves.p, t_nodes.p, N_loc, K);
+        }
+        std::vector<const void *> roots;
+        for (int p = 0; p < K; p++) {
+            const uint8_t *leaves = (const uint8_t *)t_leaves.p + (size_t)p * N_loc * 32;
+            if (G == 1) ps[p].t_tree.attach(c, leaves, (const uint8_t *)t_nodes.p + (size_t)p * N_loc * 32, n, log_nc);
+            else ps[p].t_tree.build(c, leaves, n, log_nc, false);
+            roots.push_back(ps[p].t_tree.root_dev());
+        }
+        std::vector<Digest> r = fetch_roots(c, roots);
+        for (int p = 0; p < K; p++) memcpy(ps[p].proof->trace_root, r[p].data(), 32);
+    }
 
     // ---- 3: evaluate constraints --------------------------------------------------------------------------------------------------------
     clk.mark(2);
     sub.mark("2.tree");
-    fe last_row[3];     // op_counter and program hash of the last trace step (evaluator.rs:73-74)
+    std::vector<fe> last_rows((size_t)3 * K);      // op_counter and program hash of the last trace step of every proof (evaluator.rs:73-74)
     if (host_cols) {
-        for (int j = 0; j < 3; j++) memcpy(&last_row[j], host_cols[j] + (n - 1) * 16, 16);
+        for (int p = 0; p < K; p++)
+            for (int j = 0; j < 3; j++) memcpy(&last_rows[3 * p + j], host_cols[(size_t)p * w + j] + (n - 1) * 16, 16);
     } else {
-        DevBuf d_last(48);
-        for (int j = 0; j < 3; j++) DG_CUDA(cudaMemcpyAsync((uint8_t *)d_last.p + 16 * j, d_regs + (size_t)j * n + (n - 1), 16, cudaMemcpyDeviceToDevice, c.stream));
-        d2h(c, last_row, d_last.p, 48);
+        DevBuf d_last((size_t)48 * K);
+        for (int j = 0; j < 3; j++)
+            DG_CUDA(cudaMemcpy2DAsync((uint8_t *)d_last.p + 16 * j, 48, d_regs + (size_t)j * n + (n - 1), (size_t)w * n * 16, 16, K,
+                                      cudaMemcpyDeviceToDevice, c.stream));
+        d2h(c, last_rows.data(), d_last.p, (size_t)48 * K);
     }
-    const fe op_count = last_row[0];
-    const fe program_hash[2] = {last_row[1], last_row[2]};
-    fs::ConstraintCoefficients cc = fs::draw_constraint_coefficients(proof->trace_root, ctx_depth, loop_depth, stack_depth, inputs, outputs,
-                                                                      op_count, program_hash);
     DevBuf &d_periodic = c.d_periodic;
     if (!d_periodic.p) {
         std::vector<fe> per = fs::periodic_tables();
@@ -366,25 +437,50 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
         h2d(c, d_periodic.p, per.data(), per.size() * 16);
         DG_CUDA(cudaStreamSynchronize(c.stream));
     }
-    const size_t T = cc.coefA.size(), nb = cc.bAi.size();
-    DevBuf d_coef((2 * T + 4 * nb) * 16), d_violation(4);
+    DevBuf d_coef, d_violation((size_t)4 * K);
+    // per proof [coefA | coefB | bAi | bBi | bAf | bBf], coef_stride elements apart, then the boundary constants [K][KiA, KiB, KfA, KfB].
+    // The transition coefficients have the same count for every proof of a shape; the boundary vectors have one entry per register that
+    // carries a boundary constraint, which depends on the number of public inputs / outputs: they are padded with zero coefficients to
+    // the largest count nbm (a zero coefficient adds nothing to the boundary numerators).
+    size_t coef_stride = 0, T = 0, nbm = 0;
+    std::vector<fe> bconst;                       // the boundary constants on the host, [K][4]
     {
-        std::vector<fe> pack;
-        pack.insert(pack.end(), cc.coefA.begin(), cc.coefA.end());
-        pack.insert(pack.end(), cc.coefB.begin(), cc.coefB.end());
-        pack.insert(pack.end(), cc.bAi.begin(), cc.bAi.end());
-        pack.insert(pack.end(), cc.bBi.begin(), cc.bBi.end());
-        pack.insert(pack.end(), cc.bAf.begin(), cc.bAf.end());
-        pack.insert(pack.end(), cc.bBf.begin(), cc.bBf.end());
+        for (int p = 0; p < K; p++) {
+            ProofState &s = ps[p];
+            s.op_count = last_rows[3 * p];
+            const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
+            s.cc = fs::draw_constraint_coefficients(s.proof->trace_root, ctx_depth, loop_depth, stack_depth, s.inputs, s.outputs, s.op_count,
+                                                    program_hash);
+            DG_REQUIRE(s.cc.coefA.size() == ps[0].cc.coefA.size(), "transition constraint counts differ inside a batch");
+            T = s.cc.coefA.size();
+            nbm = std::max(nbm, s.cc.bAi.size());
+        }
+        DG_REQUIRE(nbm <= (size_t)w, "more boundary registers than registers");
+        coef_stride = 2 * T + 4 * nbm;
+        std::vector<fe> pack(coef_stride * K + 4 * K, fe_make(0, 0));
+        for (int p = 0; p < K; p++) {
+            ProofState &s = ps[p];
+            auto at = pack.begin() + (size_t)p * coef_stride;
+            std::copy(s.cc.coefA.begin(), s.cc.coefA.end(), at);
+            std::copy(s.cc.coefB.begin(), s.cc.coefB.end(), at + T);
+            int slot = 0;
+            for (const auto *v : {&s.cc.bAi, &s.cc.bBi, &s.cc.bAf, &s.cc.bBf}) std::copy(v->begin(), v->end(), at + 2 * T + (slot++) * nbm);
+            const fe consts[4] = {s.cc.KiA, s.cc.KiB, s.cc.KfA, s.cc.KfB};
+            std::copy(consts, consts + 4, pack.begin() + coef_stride * K + 4 * p);
+        }
+        bconst.assign(pack.begin() + coef_stride * K, pack.end());
+        d_coef.alloc(pack.size() * 16);
         h2d(c, d_coef.p, pack.data(), pack.size() * 16);
         DG_CUDA(cudaStreamSynchronize(c.stream));
     }
-    DG_CUDA(cudaMemsetAsync(d_violation.p, 0, 4, c.stream));
-    DevBuf evals(3 * E * 16);                 // [boundary numerator, first step | boundary numerator, last step | transition combination]
+    DG_CUDA(cudaMemsetAsync(d_violation.p, 0, (size_t)4 * K, c.stream));
+    // per proof: [boundary numerator, first step | boundary numerator, last step | transition combination]
+    DevBuf evals((size_t)K * 3 * E * 16);
     {
         const int num_c8 = 8 >> log_g;
         const uint64_t E_loc = n * num_c8;
-        DevBuf evals_loc(E_loc * 16), gathered(E * 16);
+        DevBuf evals_loc((size_t)K * E_loc * 16), gathered;
+        if (G > 1) gathered.alloc(E * 16);
         AirParams P;
         memset(&P, 0, sizeof P);
         P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
@@ -400,135 +496,203 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
         static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
         for (int gi = 0; gi < 6; gi++) P.inc[gi] = (8 * n - 1) - (n - 1) * GROUP_DEG[gi];
         P.violation = d_violation.as<unsigned>();
+        P.ext_stride = (size_t)w * N_loc; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
     sub.mark("3.setup");
-        launch_constraint_eval(c, P);
+        launch_constraint_eval(c, P, K);
     sub.mark("3.eval");
         comm_all_reduce_max_u32(c, d_violation.as<unsigned>(), 1);
-        unsigned violation = 0;
-        d2h(c, &violation, d_violation.p, 4);
-        if (violation) throw Error(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation - 1) + " were not satisfied");
+        std::vector<unsigned> violation(K);
+        d2h(c, violation.data(), d_violation.p, (size_t)4 * K);
+        for (int p = 0; p < K; p++)
+            if (violation[p])
+                ps[p].fail(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation[p] - 1) + " were not satisfied");
+        if (!any_live()) return;
         // interpolation of the transition combination (constraint_table.rs:54-63), coset by coset: size-n inverse transforms of the own
         // cosets (sharded), all-gather, then the 8-point inverse DFT across cosets (poly.cu: coset_interp_finish) -> the 8n coefficients
         // in natural order; no transposition and no replicated 8n-point transform
     sub.mark("3.violation_sync");
-        ntt_batch(c, evals_loc.as<fe>(), evals_loc.as<fe>(), log_n, num_c8, n, n, true);
-        comm_all_gather(c, evals_loc.as<fe>(), gathered.as<fe>(), E_loc * 16);
+        ntt_batch(c, evals_loc.as<fe>(), evals_loc.as<fe>(), log_n, K * num_c8, n, n, true);
+        if (G > 1) comm_all_gather(c, evals_loc.as<fe>(), gathered.as<fe>(), E_loc * 16);
     sub.mark("3.intt+gather");
-        coset_interp_finish(c, gathered.as<fe>(), evals.as<fe>() + 2 * E, log_n);
+        coset_interp_finish(c, G > 1 ? gathered.as<fe>() : evals_loc.as<fe>(), evals.as<fe>() + 2 * E, log_n, K, E_loc, 3 * E);
         // boundary constraints (evaluator.rs:181-326), directly as the 8n coefficients the reference obtains by interpolation
-        boundary_coeffs(c, polys.as<fe>(), n, (int)nb, base + 2 * T, cc.KiA, cc.KiB, cc.KfA, cc.KfB, evals.as<fe>(), evals.as<fe>() + E);
+        boundary_coeffs_batch(c, K, polys.as<fe>(), (size_t)w * n, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
+                              bconst.data(), evals.as<fe>(), evals.as<fe>() + E, 3 * E);
     }
-    debug_dump(c, "t_coeffs", evals.as<fe>() + 2 * E, E * 16);
+    if (K == 1) debug_dump(c, "t_coeffs", evals.as<fe>() + 2 * E, E * 16);
 
     // ---- 4: convert constraint evaluations into a polynomial -----------------------------------------------------------------------------
     clk.mark(3);
     sub.mark("3.finish+boundary");
-    DevBuf combined(E * 16), scratch(E * 16), scratch2(E * 16);
+    DevBuf combined((size_t)K * E * 16), scratch((size_t)K * E * 16), scratch2((size_t)K * E * 16);
     const fe root_n = host_root_of_unity(log_n);
     const fe x_last = host_inv(root_n);                        // w_n^(n-1)   (evaluator.rs:128-131)
     {
-        debug_dump(c, "i_coeffs", evals.as<fe>(), E * 16);
-        debug_dump(c, "f_coeffs", evals.as<fe>() + E, E * 16);
-        fe *ic = evals.as<fe>(), *fc = evals.as<fe>() + E, *tc = evals.as<fe>() + 2 * E;
+        if (K == 1) {
+            debug_dump(c, "i_coeffs", evals.as<fe>(), E * 16);
+            debug_dump(c, "f_coeffs", evals.as<fe>() + E, E * 16);
+        }
         PowTable one_t(c, fe_make(1, 0), E + 1), xl_t(c, x_last, E + 1), xli_t(c, root_n, E + 1);
-        syn_div(c, ic, ic, scratch.as<fe>(), E, one_t.ref(), one_t.ref(), fe_make(0, 0));            // / (x - 1)
-        syn_div(c, fc, fc, scratch.as<fe>(), E, xl_t.ref(), xli_t.ref(), fe_make(0, 0));             // / (x - x_last)
-        syn_div_expanded_sum(c, tc, scratch.as<fe>(), ic, fc, combined.as<fe>(), n, E, x_last);      // / ((x^n - 1)/(x - x_last)), summed
+        const std::vector<fe> zeros(K, fe_make(0, 0));
+        DevBuf d_zeros((size_t)16 * K);
+        DG_CUDA(cudaMemsetAsync(d_zeros.p, 0, d_zeros.bytes, c.stream));
+        fe *ic = evals.as<fe>(), *fc = evals.as<fe>() + E, *tc = evals.as<fe>() + 2 * E;          // of proof 0; proof p at + 3 E p
+        syn_div_batch(c, K, ic, 3 * E, ic, 3 * E, scratch.as<fe>(), E, one_t.ref(), 0, 0, one_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - 1)
+        syn_div_batch(c, K, fc, 3 * E, fc, 3 * E, scratch.as<fe>(), E, xl_t.ref(), 0, 0, xli_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - x_last)
+        syn_div_expanded_sum(c, tc, scratch.as<fe>(), ic, fc, combined.as<fe>(), n, E, x_last, K, 3 * E, E);   // / ((x^n - 1)/(x - x_last)), summed
     }
-    debug_dump(c, "constraint_poly", combined.p, E * 16);
+    if (K == 1) debug_dump(c, "constraint_poly", combined.p, E * 16);
 
     // ---- 5: constraint evaluations over the LDE domain + their Merkle tree -----------------------------------------------------------------
     clk.mark(4);
     sub.mark("4.combine");
-    DevBuf c_ext(N_loc * 16), c_items((N_loc / 4) * 32);
-    lde_batch(c, combined.as<fe>(), c_ext.as<fe>(), log_n, log_b, 8, 1, E, N_loc, c0, (unsigned)nc);
+    DevBuf c_ext((size_t)K * N_loc * 16), c_items((size_t)K * (N_loc / 4) * 32), c_nodes;
+    auto c_ext_of = [&](int p) { return c_ext.as<fe>() + (size_t)p * N_loc; };
+    lde_batch(c, combined.as<fe>(), c_ext.as<fe>(), log_n, log_b, 8, K, E, N_loc, c0, (unsigned)nc);
     sub.mark("5.lde");
-    constraint_items_local(c, c_ext.as<fe>(), log_n, log_nc, c_items.p);      // first tree level: H(4 evaluations), [k][c4 local]
+    constraint_items_local(c, c_ext.as<fe>(), log_n, log_nc, c_items.p, K);      // first tree level: H(4 evaluations), [k][c4 local], per proof
     sub.mark("5.items");
-    ShardedTree c_tree;
-    c_tree.build(c, c_items.p, n, log_nc - 2);
-    memcpy(proof->constraint_root, c_tree.root.data(), 32);
+    {
+        if (G == 1) {
+            c_nodes.alloc((size_t)K * (N_loc / 4) * 32);
+            merkle_build_batch(c, c_items.p, c_nodes.p, N_loc / 4, K);
+        }
+        std::vector<const void *> roots;
+        std::vector<int> who;
+        for (int p = 0; p < K; p++) {
+            if (!ps[p].live) continue;
+            const uint8_t *items = (const uint8_t *)c_items.p + (size_t)p * (N_loc / 4) * 32;
+            if (G == 1) ps[p].c_tree.attach(c, items, (const uint8_t *)c_nodes.p + (size_t)p * (N_loc / 4) * 32, n, log_nc - 2);
+            else ps[p].c_tree.build(c, items, n, log_nc - 2, false);
+            roots.push_back(ps[p].c_tree.root_dev());
+            who.push_back(p);
+        }
+        std::vector<Digest> r = fetch_roots(c, roots);
+        for (size_t i = 0; i < who.size(); i++) memcpy(ps[who[i]].proof->constraint_root, r[i].data(), 32);
+    }
 
     // ---- 6: DEEP composition polynomial ---------------------------------------------------------------------------------------------------------
     clk.mark(5);
     sub.mark("5.tree");
-    fs::CompositionCoefficients dc = fs::draw_composition_coefficients(proof->constraint_root, w);
-    const fe z = dc.z, zg = fe_mul(z, root_n);
-    std::vector<fe> state1(w), state2(w);
-    DevBuf comp(E * 16), comp_ext(N_loc * 16);
+    DevBuf comp((size_t)K * E * 16), comp_ext((size_t)K * N_loc * 16);
     {
-        PowTable z_t(c, z, E + 1), zi_t(c, host_inv(z), E + 1), zg_t(c, zg, n + 1), zgi_t(c, host_inv(zg), n + 1);
         TwiddleRef g_t = c.twiddle(log_n, false);
-        // trace polynomials at z and z*g: every rank evaluates its own columns (the split of stage 1); slots of 2 cpr values are gathered
+        // trace polynomials at z and z*g: every rank evaluates its own columns (the split of stage 1); slots of 2 cpr values are gathered.
+        // d_deep = [K][2 wp] trace values, then [K][2] values of the constraint polynomial at z
         const int wp = cpr * G;
-        DevBuf d_deep((size_t)(2 * wp + 2) * 16);
+        DevBuf d_deep((size_t)K * (2 * wp + 2) * 16);
+        fe *deep_c = d_deep.as<fe>() + (size_t)K * 2 * wp;
         DG_CUDA(cudaMemsetAsync(d_deep.p, 0, d_deep.bytes, c.stream));
-        {
-            const int j0 = col_start(g), mine = col_count(g);
-            if (mine > 0) eval_polys_at(c, polys.as<fe>() + (size_t)j0 * n, n, mine, z_t.ref(), g_t, true, d_deep.as<fe>() + (size_t)2 * g * cpr);
-            if (G > 1) comm_all_gather(c, d_deep.as<fe>() + (size_t)2 * g * cpr, d_deep.p, (size_t)2 * cpr * 16);
-        }
-        eval_polys_at(c, combined.as<fe>(), E, 1, z_t.ref(), g_t, false, d_deep.as<fe>() + 2 * wp);
-        std::vector<fe> deep_slots(2 * wp + 2), deep(2 * w + 2);
-        d2h(c, deep_slots.data(), d_deep.p, deep_slots.size() * 16);
-        for (int r = 0; r < G; r++)
-            for (int o = 0; o < col_count(r); o++) {
-                deep[2 * (col_start(r) + o)] = deep_slots[2 * (r * cpr + o)];
-                deep[2 * (col_start(r) + o) + 1] = deep_slots[2 * (r * cpr + o) + 1];
+        // powers of z, 1/z, z g, 1/(z g) of every proof: four batched tables from one upload of the (base, step) pairs, [table][proof][2]
+        std::vector<fe> base_step((size_t)8 * K, fe_make(0, 0));
+        for (int p = 0; p < K; p++) {
+            ProofState &s = ps[p];
+            if (!s.live) continue;
+            s.dc = fs::draw_composition_coefficients(s.proof->constraint_root, w);
+            const fe z = s.dc.z, zg = fe_mul(z, root_n);
+            const fe bases[4] = {z, host_inv(z), zg, host_inv(zg)};
+            for (int t = 0; t < 4; t++) {
+                base_step[(size_t)2 * (t * K + p)] = bases[t];
+                base_step[(size_t)2 * (t * K + p) + 1] = PowTables::step(bases[t], t < 2 ? E + 1 : n + 1);
             }
-        deep[2 * w] = deep_slots[2 * wp];
-    sub.mark("6.deep_values");
-        fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
-        for (int i = 0; i < w; i++) {
-            state1[i] = deep[2 * i]; state2[i] = deep[2 * i + 1];
-            sub1 = fe_add(sub1, fe_mul(state1[i], dc.trace1[i]));
-            sub2 = fe_add(sub2, fe_mul(state2[i], dc.trace2[i]));
         }
-        const fe c_at_z = deep[2 * w];
-        DevBuf d_cc((size_t)2 * w * 16), t12(2 * n * 16);
-        h2d(c, d_cc.p, dc.trace1.data(), (size_t)w * 16);
-        h2d(c, d_cc.as<fe>() + w, dc.trace2.data(), (size_t)w * 16);
-        fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;
-        lincomb2(c, polys.as<fe>(), n, w, d_cc.as<fe>(), d_cc.as<fe>() + w, t1, t2);
-        syn_div(c, t1, t1, scratch.as<fe>(), n, z_t.ref(), zi_t.ref(), sub1);                          // (T1(x) - T1(z)) / (x - z)
-        syn_div(c, t2, t2, scratch.as<fe>(), n, zg_t.ref(), zgi_t.ref(), sub2);                        // (T2(x) - T2(zg)) / (x - zg)
-        syn_div(c, combined.as<fe>(), scratch2.as<fe>(), scratch.as<fe>(), E, z_t.ref(), zi_t.ref(), c_at_z);   // (C(x) - C(z)) / (x - z)
+        DevBuf d_base_step(base_step.size() * 16);
+        h2d(c, d_base_step.p, base_step.data(), base_step.size() * 16);
+        const fe *bs = d_base_step.as<fe>();
+        PowTables z_t(c, bs, K, E + 1), zi_t(c, bs + 2 * K, K, E + 1), zg_t(c, bs + 4 * K, K, n + 1), zgi_t(c, bs + 6 * K, K, n + 1);
+        if (G == 1) {
+            eval_polys_at(c, polys.as<fe>(), n, K * w, z_t.ref(0), g_t, true, d_deep.as<fe>(), w, z_t.lo_n, z_t.hi_n);
+        } else {
+            const int j0 = col_start(g), mine = col_count(g);
+            if (mine > 0) eval_polys_at(c, polys.as<fe>() + (size_t)j0 * n, n, mine, z_t.ref(0), g_t, true, d_deep.as<fe>() + (size_t)2 * g * cpr);
+            comm_all_gather(c, d_deep.as<fe>() + (size_t)2 * g * cpr, d_deep.p, (size_t)2 * cpr * 16);
+        }
+        eval_polys_at(c, combined.as<fe>(), E, K, z_t.ref(0), g_t, false, deep_c, 1, z_t.lo_n, z_t.hi_n);
+        std::vector<fe> deep_slots((size_t)K * (2 * wp + 2));
+        d2h(c, deep_slots.data(), d_deep.p, deep_slots.size() * 16);
+    sub.mark("6.deep_values");
+        // one upload: [K][2w] coefficients of the trace combinations | sub0 of the three divisions [3][K] | compose's k1, k2, kc [K][3]
+        std::vector<fe> pack((size_t)K * (2 * w + 6), fe_make(0, 0));
+        fe *ccs = pack.data(), *subs = ccs + (size_t)K * 2 * w, *ks = subs + (size_t)3 * K;
+        for (int p = 0; p < K; p++) {
+            ProofState &s = ps[p];
+            if (!s.live) continue;
+            const fe *slots = deep_slots.data() + (size_t)p * 2 * wp;
+            std::vector<fe> deep(2 * w);
+            for (int r = 0; r < G; r++)
+                for (int o = 0; o < col_count(r); o++) {
+                    deep[2 * (col_start(r) + o)] = slots[2 * (r * cpr + o)];
+                    deep[2 * (col_start(r) + o) + 1] = slots[2 * (r * cpr + o) + 1];
+                }
+            s.state1.resize(w); s.state2.resize(w);
+            fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
+            for (int i = 0; i < w; i++) {
+                s.state1[i] = deep[2 * i]; s.state2[i] = deep[2 * i + 1];
+                sub1 = fe_add(sub1, fe_mul(s.state1[i], s.dc.trace1[i]));
+                sub2 = fe_add(sub2, fe_mul(s.state2[i], s.dc.trace2[i]));
+            }
+            subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[(size_t)K * 2 * wp + 2 * p];
+            std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + w, ccs + (size_t)p * 2 * w);
+            std::copy(s.dc.trace2.begin(), s.dc.trace2.begin() + w, ccs + (size_t)p * 2 * w + w);
+            ks[3 * p] = s.dc.t1_degree; ks[3 * p + 1] = s.dc.t2_degree; ks[3 * p + 2] = s.dc.constraints;
+        }
+        DevBuf d_pack(pack.size() * 16), t12((size_t)K * 2 * n * 16);
+        h2d(c, d_pack.p, pack.data(), pack.size() * 16);
+        const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * w, *d_ks = d_subs + (size_t)3 * K;
+        fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
+        lincomb2(c, polys.as<fe>(), n, w, d_cc, d_cc + w, t1, t2, K, 2 * w, 2 * n);
+        syn_div_batch(c, K, t1, 2 * n, t1, 2 * n, scratch.as<fe>(), n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs, subs);
+        //                                                                                                   (T1(x) - T1(z)) / (x - z)
+        syn_div_batch(c, K, t2, 2 * n, t2, 2 * n, scratch.as<fe>(), n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K,
+                      subs + K);                                                                           // (T2(x) - T2(zg)) / (x - zg)
+        syn_div_batch(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, scratch.as<fe>(), E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n,
+                      zi_t.hi_n, d_subs + 2 * K, subs + 2 * K);                                            // (C(x) - C(z)) / (x - z)
     sub.mark("6.lincomb+syndiv");
-        compose(c, t1, t2, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, dc.t1_degree, dc.t2_degree, dc.constraints);
-        debug_dump(c, "composition_poly", comp.p, E * 16);
+        compose_batch(c, K, t1, t2, 2 * n, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, d_ks, ks);
+        if (K == 1) debug_dump(c, "composition_poly", comp.p, E * 16);
         // every rank extends its own cosets; the first FRI layers work on these slabs directly (no all-gather of the N evaluations)
-        lde_batch(c, comp.as<fe>(), comp_ext.as<fe>(), log_n, log_b, 8, 1, E, N_loc, c0, (unsigned)nc);
+        lde_batch(c, comp.as<fe>(), comp_ext.as<fe>(), log_n, log_b, 8, K, E, N_loc, c0, (unsigned)nc);
     }
 
     // ---- 7: FRI layers ---------------------------------------------------------------------------------------------------------------------------
     clk.mark(6);
     sub.mark("6.compose+lde");
-    std::vector<FriLayerDev> layers;
     DevBuf fri_gathered;                                       // multi-GPU: the first replicated layer, gathered from the ranks' slabs
+    std::vector<DevBuf> layer_bufs;                            // replicated layers: row hashes, trees and folded values of all K proofs
+    size_t n_layers = 0;
     {
         TwiddleRef inv_root = c.twiddle(log_N, true);
         const fe tau_inv = host_inv(host_root_of_unity(2));
         const fe inv4 = host_inv(fe_make(4, 0));
+        // the K proofs' layers are one buffer each: layer d of proof p = cur + p * cur_stride
         const fe *cur = comp_ext.as<fe>();
+        uint64_t cur_stride = N_loc;
         Layout lay{log_N, log_b};
-        bool local = G > 1;                                    // `cur` is this rank's coset slab of the layer
-        // layer roots and folding points stay on the device (special_x = prng(root) is derived by fri_alpha): the host sees the roots
-        // in one copy after the last layer.  With host RNG callbacks registered each layer asks the host instead.
+        bool local = G > 1;                                    // `cur` is this rank's coset slab of the layer (K == 1)
+        // layer roots and folding points stay on the device, [layer][proof] (special_x = prng(root) is derived by fri_alpha): the host
+        // sees the roots in one copy after the last layer.  With host RNG callbacks registered each layer asks the host instead: one
+        // copy of the layer's K roots, the callbacks of the live proofs in proof order, one upload of the K folding points.
         const int MAX_LAYERS = 20;
-        DevBuf d_alpha(MAX_LAYERS * 16), d_roots(MAX_LAYERS * 32);
+        DevBuf d_alpha((size_t)MAX_LAYERS * K * 16), d_roots((size_t)MAX_LAYERS * K * 32);
         const bool host_rng = fs::rng_hooks_active();
-        auto folding_point = [&](const void *root_dev, size_t layer) -> const fe * {
-            DG_REQUIRE(layer < (size_t)MAX_LAYERS, "too many FRI layers");
-            fe *a_dev = d_alpha.as<fe>() + layer;
-            uint8_t *r_dev = (uint8_t *)d_roots.p + 32 * layer;
-            if (!host_rng) { fri_alpha(c, root_dev, a_dev, r_dev); return a_dev; }
-            Digest r;
-            d2h(c, r.data(), root_dev, 32);
-            const fe alpha = fs::prng_vector(r.data(), 1)[0];          // field::prng(seed) = first draw of the generator (field.rs:264-269)
-            DG_CUDA(cudaMemcpyAsync(r_dev, root_dev, 32, cudaMemcpyDeviceToDevice, c.stream));
-            DG_CUDA(cudaMemcpyAsync(a_dev, &alpha, 16, cudaMemcpyHostToDevice, c.stream));
+        auto alpha_dev = [&](size_t layer) { return d_alpha.as<fe>() + layer * K; };
+        auto root_slots = [&](size_t layer) { return (uint8_t *)d_roots.p + 32 * layer * K; };
+        // the K roots of layer `li`, root_stride bytes apart from root0, into their slots
+        auto copy_roots = [&](const void *root0, size_t root_stride, size_t li) {
+            DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
+            DG_CUDA(cudaMemcpy2DAsync(root_slots(li), 32, root0, std::max<size_t>(root_stride, 32), 32, K, cudaMemcpyDeviceToDevice, c.stream));
+        };
+        auto folding_points = [&](const void *root0, size_t root_stride, size_t li) {
+            DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
+            if (!host_rng) { fri_alpha(c, root0, alpha_dev(li), root_slots(li), K, root_stride); return; }
+            copy_roots(root0, root_stride, li);
+            std::vector<uint8_t> r((size_t)32 * K);
+            d2h(c, r.data(), root_slots(li), r.size());
+            std::vector<fe> alphas(K, fe_make(0, 0));
+            for (int p = 0; p < K; p++)
+                if (ps[p].live) alphas[p] = fs::prng_vector(r.data() + 32 * p, 1)[0];   // field::prng(seed) = first draw of the generator (field.rs:264-269)
+            DG_CUDA(cudaMemcpyAsync(alpha_dev(li), alphas.data(), (size_t)16 * K, cudaMemcpyHostToDevice, c.stream));
             DG_CUDA(cudaStreamSynchronize(c.stream));
-            return a_dev;
         };
         for (;;) {
             const int log_r = lay.log_d - 2;
@@ -541,97 +705,117 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
                 cur = fri_gathered.as<fe>();
                 local = false;
             }
-            layers.emplace_back();
-            const size_t li = layers.size() - 1;
-            FriLayerDev &L = layers.back();
-            L.vals = cur; L.layout = lay; L.sharded = local;
+            const size_t li = n_layers++;
             if (local) {
+                FriLayerDev &L = ps[0].layers.emplace_back();
+                L.vals = cur; L.layout = lay; L.sharded = true;
                 // rows r = b k' + c of the own cosets: hashes in ShardedTree order, n' = R / b subtrees of nc leaves per rank
                 L.leaves.alloc((R >> log_g) * 32);
                 fri_hash_rows_local(c, cur, lay.log_d, log_b, log_nc, L.leaves.p);
                 L.tree.build(c, L.leaves.p, R >> log_b, log_nc, false);
-                const fe *alpha = folding_point(L.tree.root_dev(), li);
+                folding_points(L.tree.root_dev(), 0, li);
                 L.folded.alloc((R >> log_g) * 16);
-                fri_fold_local(c, cur, lay.log_d, log_b, log_nc, c0, L.folded.as<fe>(), alpha, inv_root, log_N, tau_inv, inv4);
+                fri_fold_local(c, cur, lay.log_d, log_b, log_nc, c0, L.folded.as<fe>(), alpha_dev(li), inv_root, log_N, tau_inv, inv4);
                 cur = L.folded.as<fe>();
                 lay = Layout{log_r, log_b};
                 continue;
             }
             const Layout rows{log_r, (lay.log_b >= 0 && log_r >= lay.log_b) ? lay.log_b : -1};
-            L.leaves.alloc(R * 32); L.nodes.alloc(R * 32);
-            fri_hash_rows(c, cur, lay, rows, L.leaves.p);
-            merkle_build(c, L.leaves.p, L.nodes.p, R);
+            layer_bufs.emplace_back((size_t)K * R * 32);
+            const uint8_t *leaves = layer_bufs.back().as<uint8_t>();
+            layer_bufs.emplace_back((size_t)K * R * 32);
+            const uint8_t *nodes = layer_bufs.back().as<uint8_t>();
+            fri_hash_rows(c, cur, lay, rows, (void *)leaves, K, cur_stride);
+            merkle_build_batch(c, leaves, (void *)nodes, R, K);
+            for (int p = 0; p < K; p++) {
+                if (!ps[p].live) continue;
+                FriLayerDev &L = ps[p].layers.emplace_back();
+                L.vals = cur + (size_t)p * cur_stride; L.layout = lay; L.sharded = false;
+                L.leaves_p = leaves + (size_t)p * R * 32; L.nodes_p = nodes + (size_t)p * R * 32;
+            }
             if (R * 4 <= 256) {                                    // MAX_REMAINDER_LENGTH (fri/mod.rs:13): the remainder's root only
-                DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
-                DG_CUDA(cudaMemcpyAsync((uint8_t *)d_roots.p + 32 * li, (const uint8_t *)L.nodes.p + 32, 32, cudaMemcpyDeviceToDevice, c.stream));
+                copy_roots(nodes + 32, R * 32, li);
                 break;
             }
-            const fe *alpha = folding_point((const uint8_t *)L.nodes.p + 32, li);     // special_x = prng(root)  (fri/prover.rs:29)
-            L.folded.alloc(R * 16);                                // values of the next layer, owned by this one
-            fri_fold(c, cur, lay, L.folded.as<fe>(), rows, alpha, inv_root, log_N, tau_inv, inv4);
-            cur = L.folded.as<fe>();
+            folding_points(nodes + 32, R * 32, li);                // special_x = prng(root)  (fri/prover.rs:29)
+            layer_bufs.emplace_back((size_t)K * R * 16);           // values of the next layer
+            fe *folded = layer_bufs.back().as<fe>();
+            fri_fold(c, cur, lay, folded, rows, alpha_dev(li), inv_root, log_N, tau_inv, inv4, K, cur_stride);
+            cur = folded;
+            cur_stride = R;
             lay = rows;
         }
-        std::vector<uint8_t> roots(32 * layers.size());
+        std::vector<uint8_t> roots(32 * n_layers * K);
         d2h(c, roots.data(), d_roots.p, roots.size());
-        for (size_t i = 0; i < layers.size(); i++) memcpy(layers[i].root.data(), roots.data() + 32 * i, 32);
+        for (int p = 0; p < K; p++)
+            if (ps[p].live)
+                for (size_t i = 0; i < n_layers; i++) memcpy(ps[p].layers[i].root.data(), roots.data() + 32 * (i * K + p), 32);
     }
 
     // ---- 8: query positions ------------------------------------------------------------------------------------------------------------------------
     clk.mark(7);
     sub.mark("7.fri");
-    std::vector<uint64_t> positions;
     {
-        std::vector<uint8_t> roots;
-        for (auto &L : layers) roots.insert(roots.end(), L.root.begin(), L.root.end());
-        uint8_t seed[32];
-        debug_dump_host("fri_roots", roots.data(), roots.size());
-        fs::blake3_short(roots.data(), roots.size(), seed);
-        proof->pow_nonce = pow_search(c, seed, opt.grinding_factor);
-        pow_hash(seed, proof->pow_nonce, proof->pow_seed);
-        try {
-            positions = fs::query_positions(proof->pow_seed, N, b, opt.num_queries);
-        } catch (const std::exception &e) { throw Error(DG_ERR_EXHAUSTED, e.what()); }
-        debug_dump_host("positions", positions.data(), positions.size() * 8);
+        std::vector<std::array<uint8_t, 32>> seeds;
+        std::vector<int> who;
+        for (int p = 0; p < K; p++) {
+            if (!ps[p].live) continue;
+            std::vector<uint8_t> roots;
+            for (auto &L : ps[p].layers) roots.insert(roots.end(), L.root.begin(), L.root.end());
+            if (K == 1) debug_dump_host("fri_roots", roots.data(), roots.size());
+            seeds.emplace_back();
+            fs::blake3_short(roots.data(), roots.size(), seeds.back().data());
+            who.push_back(p);
+        }
+        std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, opt.grinding_factor);
+        for (size_t i = 0; i < who.size(); i++) {
+            ProofState &s = ps[who[i]];
+            s.proof->pow_nonce = nonces[i];
+            pow_hash(seeds[i].data(), s.proof->pow_nonce, s.proof->pow_seed);
+            try {
+                s.positions = fs::query_positions(s.proof->pow_seed, N, b, opt.num_queries);
+            } catch (const std::exception &e) { s.fail(DG_ERR_EXHAUSTED, e.what()); continue; }
+            if (K == 1) debug_dump_host("positions", s.positions.data(), s.positions.size() * 8);
+        }
+        if (!any_live()) return;
     }
 
-    // ---- 9: build proof object -------------------------------------------------------------------------------------------------------------------------
+    // ---- 9: build proof objects --------------------------------------------------------------------------------------------------------------------------
     clk.mark(8);
     sub.mark("8.pow");
-    fs::ByteWriter out;
-    {
-        // Plan every opening on the host, fetch all opened values / digests in one batched pass (FetchBatch), then serialise.
+    // Plan every opening of every proof on the host, fetch all opened values / digests in one batched pass (FetchBatch), then serialise.
+    FetchBatch fb(c);
+    // registers the nodes of a batch-proof plan; leaf_ref / node_ref map leaf indices / heap indices to fetch references
+    auto plan_offsets = [&](const fs::BatchPlan &plan, auto leaf_ref, auto node_ref) {
+        Offsets o(plan.nodes.size());
+        for (size_t sidx = 0; sidx < plan.nodes.size(); sidx++)
+            for (auto &r : plan.nodes[sidx]) o[sidx].push_back(fb.add32(r.leaf ? leaf_ref(r.index) : node_ref(r.index)));
+        return o;
+    };
+    auto digests_at = [&](const Offsets &o) {
+        std::vector<std::vector<Digest>> v(o.size());
+        for (size_t i = 0; i < o.size(); i++)
+            for (size_t off : o[i]) v[i].push_back(fb.digest(off));
+        return v;
+    };
+    auto plan_openings = [&](ProofState &s, const fe *ext_p, const fe *c_ext_p) {
+        OpenPlan O;
+        const std::vector<uint64_t> &positions = s.positions;
         const int nq = (int)positions.size();
-        FetchBatch fb(c);
-        typedef std::vector<std::vector<size_t>> Offsets;
-        // registers the nodes of a batch-proof plan; leaf_ref / node_ref map leaf indices / heap indices to fetch references
-        auto plan_offsets = [&](const fs::BatchPlan &plan, auto leaf_ref, auto node_ref) {
-            Offsets o(plan.nodes.size());
-            for (size_t sidx = 0; sidx < plan.nodes.size(); sidx++)
-                for (auto &r : plan.nodes[sidx]) o[sidx].push_back(fb.add32(r.leaf ? leaf_ref(r.index) : node_ref(r.index)));
-            return o;
-        };
-        auto digests_at = [&](const Offsets &o) {
-            std::vector<std::vector<Digest>> v(o.size());
-            for (size_t i = 0; i < o.size(); i++)
-                for (size_t off : o[i]) v[i].push_back(fb.digest(off));
-            return v;
-        };
-
         // trace rows at the queried positions (trace_table.rs:127-134): the rank owning the position's coset reads the row
-        std::vector<size_t> row_off(nq);
+        O.row_off.resize(nq);
         for (int q = 0; q < nq; q++) {
             const uint64_t cpos = positions[q] & (b - 1), k = positions[q] >> log_b;
             const int owner = (int)(cpos >> log_nc);
             const uint64_t phys = ((cpos - (uint64_t)owner * nc) << log_n) + k;
             for (int j = 0; j < w; j++) {
-                const size_t off = fb.add16(FetchRef{ext.as<fe>() + (size_t)j * N_loc, phys, owner});
-                if (j == 0) row_off[q] = off;
+                const size_t off = fb.add16(FetchRef{ext_p + (size_t)j * N_loc, phys, owner});
+                if (j == 0) O.row_off[q] = off;
             }
         }
         // trace tree openings: leaves are the row hashes
-        fs::BatchPlan tplan = fs::plan_batch_proof(positions, N);
-        Offsets t_off = plan_offsets(tplan, [&](uint64_t i) { return t_tree.item_ref(i); }, [&](uint64_t h) { return t_tree.node_ref(h); });
+        O.tplan = fs::plan_batch_proof(positions, N);
+        O.t_off = plan_offsets(O.tplan, [&](uint64_t i) { return s.t_tree.item_ref(i); }, [&](uint64_t h) { return s.t_tree.node_ref(h); });
 
         // constraint tree openings: leaf j = evaluations (2j, 2j+1), unhashed (prover.rs:180-187); evaluation 2j+1 lives in the next
         // coset at the same k, i.e. n elements further in the owner's slab: two 16-byte units registered back to back = one 32-byte item
@@ -639,35 +823,33 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
             const uint64_t i = 2 * j, cpos = i & (b - 1), k = i >> log_b;
             const int owner = (int)(cpos >> log_nc);
             const uint64_t p0 = ((cpos - (uint64_t)owner * nc) << log_n) + k;
-            const size_t off = fb.add16(FetchRef{c_ext.as<fe>(), p0, owner});
-            fb.add16(FetchRef{c_ext.as<fe>(), p0 + n, owner});
+            const size_t off = fb.add16(FetchRef{c_ext_p, p0, owner});
+            fb.add16(FetchRef{c_ext_p, p0 + n, owner});
             return off;
         };
         std::vector<uint64_t> c_positions = fs::constraint_positions(positions);
-        fs::BatchPlan cplan = fs::plan_batch_proof(c_positions, N / 2);
-        std::vector<size_t> cval_off;
-        for (uint64_t j : cplan.value_leaves) cval_off.push_back(constraint_leaf(j));
-        Offsets c_off(cplan.nodes.size());
-        for (size_t sidx = 0; sidx < cplan.nodes.size(); sidx++)
-            for (auto &r : cplan.nodes[sidx]) {
+        O.cplan = fs::plan_batch_proof(c_positions, N / 2);
+        for (uint64_t j : O.cplan.value_leaves) O.cval_off.push_back(constraint_leaf(j));
+        O.c_off.resize(O.cplan.nodes.size());
+        for (size_t sidx = 0; sidx < O.cplan.nodes.size(); sidx++)
+            for (auto &r : O.cplan.nodes[sidx]) {
                 // heap indices of the tree over N/2 leaves: [N/4, N/2) is the first hashed level (= level-0 items of c_tree)
-                if (r.leaf) c_off[sidx].push_back(constraint_leaf(r.index));
-                else if (r.index >= N / 4) c_off[sidx].push_back(fb.add32(c_tree.item_ref(r.index - N / 4)));
-                else c_off[sidx].push_back(fb.add32(c_tree.node_ref(r.index)));
+                if (r.leaf) O.c_off[sidx].push_back(constraint_leaf(r.index));
+                else if (r.index >= N / 4) O.c_off[sidx].push_back(fb.add32(s.c_tree.item_ref(r.index - N / 4)));
+                else O.c_off[sidx].push_back(fb.add32(s.c_tree.node_ref(r.index)));
             }
 
         // FRI layers (fri/prover.rs:55-95)
-        struct LayerOpen { std::vector<uint64_t> pos; std::vector<size_t> val_off; Offsets node_off; uint8_t depth; };
-        std::vector<LayerOpen> fri_open(layers.size() - 1);
+        O.fri_open.resize(s.layers.size() - 1);
         std::vector<uint64_t> fpos = positions;
-        for (size_t d = 0; d + 1 < layers.size(); d++) {
-            FriLayerDev &L = layers[d];
-            LayerOpen &O = fri_open[d];
+        for (size_t d = 0; d + 1 < s.layers.size(); d++) {
+            FriLayerDev &L = s.layers[d];
+            LayerOpen &lo = O.fri_open[d];
             const uint64_t D = 1ULL << L.layout.log_d, R = D / 4;
             fpos = fs::augmented_positions(fpos, D);
-            O.pos = fpos;
+            lo.pos = fpos;
             fs::BatchPlan plan = fs::plan_batch_proof(fpos, R);
-            O.depth = plan.depth;
+            lo.depth = plan.depth;
             for (uint64_t p : fpos)
                 for (int j = 0; j < 4; j++) {
                     size_t off;
@@ -678,71 +860,196 @@ static Proof *prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols
                     } else {
                         off = fb.add16(FetchRef{L.vals, L.layout.phys(p + j * R), -1});
                     }
-                    if (j == 0) O.val_off.push_back(off);
+                    if (j == 0) lo.val_off.push_back(off);
                 }
-            if (L.sharded) O.node_off = plan_offsets(plan, [&](uint64_t i) { return L.tree.item_ref(i); }, [&](uint64_t h) { return L.tree.node_ref(h); });
-            else O.node_off = plan_offsets(plan, [&](uint64_t i) { return FetchRef{L.leaves.p, i, -1}; }, [&](uint64_t h) { return FetchRef{L.nodes.p, h, -1}; });
+            if (L.sharded) lo.node_off = plan_offsets(plan, [&](uint64_t i) { return L.tree.item_ref(i); }, [&](uint64_t h) { return L.tree.node_ref(h); });
+            else lo.node_off = plan_offsets(plan, [&](uint64_t i) { return FetchRef{L.leaves_p, i, -1}; }, [&](uint64_t h) { return FetchRef{L.nodes_p, h, -1}; });
         }
-        std::vector<size_t> rem_off;
         {
-            FriLayerDev &L = layers.back();
+            FriLayerDev &L = s.layers.back();
             const uint64_t D = 1ULL << L.layout.log_d;
-            for (uint64_t i = 0; i < D; i++) rem_off.push_back(fb.add16(FetchRef{L.vals, L.layout.phys(i), -1}));   // remainder, natural order
+            for (uint64_t i = 0; i < D; i++) O.rem_off.push_back(fb.add16(FetchRef{L.vals, L.layout.phys(i), -1}));   // remainder, natural order
         }
-        fb.run();
-
-        // ---- serialise (proof.rs:10-37; bincode: u64 length prefixes, arrays raw, little endian)
+        return O;
+    };
+    // serialise (proof.rs:10-37; bincode: u64 length prefixes, arrays raw, little endian)
+    auto serialise = [&](ProofState &s, const OpenPlan &O) {
+        fs::ByteWriter out;
+        Proof *proof = s.proof.get();
+        const int nq = (int)s.positions.size();
         out.raw(proof->trace_root, 32);
-        out.u8(tplan.depth); out.u8((uint8_t)ctx_depth); out.u8((uint8_t)loop_depth); out.u8((uint8_t)stack_depth);
-        out.u32((uint32_t)op_count.lo);                                               // op_count as u32 (proof.rs:62)
-        write_digest_vv(out, digests_at(t_off));
+        out.u8(O.tplan.depth); out.u8((uint8_t)ctx_depth); out.u8((uint8_t)loop_depth); out.u8((uint8_t)stack_depth);
+        out.u32((uint32_t)s.op_count.lo);                                             // op_count as u32 (proof.rs:62)
+        write_digest_vv(out, digests_at(O.t_off));
         out.u64(nq);
         for (int q = 0; q < nq; q++) {
             out.u64(w);
-            for (int j = 0; j < w; j++) out.felt(fb.value(row_off[q] + j));
+            for (int j = 0; j < w; j++) out.felt(fb.value(O.row_off[q] + j));
         }
         out.raw(proof->constraint_root, 32);
-        out.u64(cval_off.size());
-        for (size_t off : cval_off) { Digest dgt = fb.digest(off); out.raw(dgt.data(), 32); }
-        write_digest_vv(out, digests_at(c_off));
-        out.u8(cplan.depth);
-        write_felt_vec(out, state1);
-        write_felt_vec(out, state2);
+        out.u64(O.cval_off.size());
+        for (size_t off : O.cval_off) { Digest dgt = fb.digest(off); out.raw(dgt.data(), 32); }
+        write_digest_vv(out, digests_at(O.c_off));
+        out.u8(O.cplan.depth);
+        write_felt_vec(out, s.state1);
+        write_felt_vec(out, s.state2);
 
-        out.u64(layers.size() - 1);
-        for (size_t d = 0; d + 1 < layers.size(); d++) {
-            LayerOpen &O = fri_open[d];
-            out.raw(layers[d].root.data(), 32);
-            out.u64(O.pos.size());
-            for (size_t off : O.val_off)
+        out.u64(s.layers.size() - 1);
+        for (size_t d = 0; d + 1 < s.layers.size(); d++) {
+            const LayerOpen &lo = O.fri_open[d];
+            out.raw(s.layers[d].root.data(), 32);
+            out.u64(lo.pos.size());
+            for (size_t off : lo.val_off)
                 for (int j = 0; j < 4; j++) out.felt(fb.value(off + j));
-            write_digest_vv(out, digests_at(O.node_off));
-            out.u8(O.depth);
+            write_digest_vv(out, digests_at(lo.node_off));
+            out.u8(lo.depth);
         }
-        out.raw(layers.back().root.data(), 32);
-        out.u64(rem_off.size());
-        for (size_t off : rem_off) out.felt(fb.value(off));
+        out.raw(s.layers.back().root.data(), 32);
+        out.u64(O.rem_off.size());
+        for (size_t off : O.rem_off) out.felt(fb.value(off));
         out.u64(proof->pow_nonce);
         out.u8((uint8_t)log_b); out.u8((uint8_t)opt.num_queries); out.u8((uint8_t)opt.grinding_factor); out.u8(0);
+        proof->bytes = std::move(out.b);
+    };
+    {
+        std::vector<OpenPlan> plans(K);
+        for (int p = 0; p < K; p++)
+            if (ps[p].live) plans[p] = plan_openings(ps[p], ext_of(p), c_ext_of(p));
+        fb.run();
+        for (int p = 0; p < K; p++)
+            if (ps[p].live) serialise(ps[p], plans[p]);
     }
     clk.mark(9);
     sub.mark("9.openings");
     sub.report(c.rank);
     DG_CUDA(cudaStreamSynchronize(c.stream));
-    proof->bytes = std::move(out.b);
     if (stats) {
         for (int i = 0; i < 9; i++) stats->stage_ms[i] = clk.between(i, i + 1);
         stats->h2d_ms = 0.0f;                        // host variant: uploads overlap stage 1 and are part of stage_ms[0]
         stats->total_ms = clk.between(0, 9);
         stats->kernel_launches = c.launches - launches0;
     }
-    return guard.release();
 }
+
+namespace {
+
+std::vector<ProofState> make_states(uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16,
+                                    const uint32_t *n_outputs) {
+    std::vector<ProofState> ps(count);
+    for (uint32_t i = 0; i < count; i++) {
+        const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
+        DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
+        DG_REQUIRE((ni == 0 || (inputs16 && inputs16[i])) && (no == 0 || (outputs16 && outputs16[i])), "null public inputs / outputs");
+        ps[i].inputs.resize(ni);
+        ps[i].outputs.resize(no);
+        if (ni) memcpy(ps[i].inputs.data(), inputs16[i], ni * 16);
+        if (no) memcpy(ps[i].outputs.data(), outputs16[i], no * 16);
+    }
+    return ps;
+}
+
+// the single-trace entry points: a batch of one whose failure is the call's error
+Proof *prove_one(Context &c, fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                 const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
+                 dg_prove_stats_t *stats) {
+    std::vector<ProofState> ps = make_states(1, &inputs16, &n_inputs, &outputs16, &n_outputs);
+    prove_core(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, ps, opt, stats);
+    if (ps[0].status != DG_OK) throw Error(ps[0].status, ps[0].message);
+    return ps[0].proof.release();
+}
+
+// Device bytes one proof of this shape takes in a batch on one GPU: the buffers prove_core allocates per proof, stage by stage (every
+// one stays in the bump arena until the group ends), plus its register columns (the upload buffer of a host batch).
+size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b) {
+    const size_t N = (size_t)n * b, E = (size_t)n * 8, fe16 = 16, dg32 = 32;
+    size_t f = 0;
+    f += (size_t)w * n * fe16;                // registers (host batch: upload buffer)
+    f += (size_t)w * n * fe16;                // 1: polynomials
+    f += (size_t)w * N * fe16;                // 1: trace LDE
+    f += 2 * N * dg32;                        // 2: row hashes + tree
+    f += 3 * E * fe16 + E * fe16;             // 3: i / f / t coefficients, coset-local transition evaluations
+    f += 3 * E * fe16;                        // 4: combined polynomial + the two division scratch vectors
+    f += N * fe16 + 2 * (N / 4) * dg32;       // 5: constraint LDE, first hashed level + tree
+    f += 2 * N * fe16;                        // 5, 6: prefolded input of the two fold-8 extensions (both live until the group ends)
+    f += E * fe16 + N * fe16;                 // 6: composition polynomial + its LDE
+    f += 2 * n * fe16;                        // 6: the two trace quotients
+    size_t pow_n = 0;                         // 6: the four power tables of z, 1/z (E + 1 entries), z g, 1/(z g) (n + 1 entries)
+    for (uint64_t len : {E + 1, E + 1, (uint64_t)n + 1, (uint64_t)n + 1}) {
+        int lo_bits = 1;
+        while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
+        pow_n += (1ULL << lo_bits) + (len + (1ULL << lo_bits) - 1) / (1ULL << lo_bits) + 1;
+    }
+    f += pow_n * fe16;
+    f += (N / 4) * (2 * dg32 + fe16) * 4 / 3; // 7: FRI layers (R = D / 4 row hashes, tree and folded values per layer, D = N, N / 4, ...)
+    f += (size_t)1 << 20;                     // coefficients, DEEP values, scan descriptors, evaluation partials, PoW, openings (< 1 MB)
+    return f + f / 16;                        // + 256-byte alignment of every arena allocation
+}
+
+// Largest group of one launch: the batched kernels put the proof (and the DEEP evaluation every column of every proof) on the grid's y
+// dimension, which holds at most 65535 blocks.
+int max_group_for_grid(uint32_t w) { return (int)(65535 / std::max<uint32_t>(w, 1)); }
+
+int batch_group_size(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count) {
+    const size_t per = proof_footprint(w, n, b);
+    long long k = std::min<long long>(count, max_group_for_grid(w));
+    if ((size_t)count * per > c.arena.cap) {                 // does not fit in the arena the library already holds: ask the driver
+        size_t free_b = 0, total_b = 0;
+        DG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        const size_t avail = (free_b + c.arena.cap) / 10 * 8;
+        k = std::min<long long>(k, (long long)std::max<size_t>(1, avail / per));
+    }
+    if (const char *e = getenv("DG_BATCH_GROUP")) {
+        const long long cap = atoll(e);
+        DG_REQUIRE(cap >= 1, "DG_BATCH_GROUP must be a positive integer");
+        k = std::min(k, cap);
+    }
+    return (int)k;
+}
+
+void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
+    for (int i = 0; i < 9; i++) sum->stage_ms[i] += s.stage_ms[i];
+    sum->h2d_ms += s.h2d_ms;
+    sum->total_ms += s.total_ms;
+    sum->kernel_launches += s.kernel_launches;
+}
+
+// runs the batch group by group; run_group(first, k, states, stats) proves traces [first, first + k)
+template <typename F>
+void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_options_t &opt, std::vector<ProofState> &all, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, F &&run_group) {
+    DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
+    const int group = batch_group_size(c, w, n, opt.extension_factor, count);
+    if (stats) memset(stats, 0, sizeof *stats);
+    for (uint32_t i = 0; i < count; i++) { proofs_out[i] = nullptr; status[i] = DG_OK; }
+    messages.assign(count, std::string());
+    // a group that fails as a whole fails the call: the proofs of the earlier groups are freed, nothing is returned
+    struct ReleaseOnError {
+        Proof **out; uint32_t count; bool done = false;
+        ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
+    } release{proofs_out, count};
+    for (uint32_t first = 0; first < count; first += group) {
+        const int k = (int)std::min<uint32_t>(group, count - first);
+        std::vector<ProofState> ps;
+        for (int i = 0; i < k; i++) ps.push_back(std::move(all[first + i]));
+        dg_prove_stats_t st;
+        memset(&st, 0, sizeof st);
+        run_group(first, k, ps, &st);
+        if (stats) add_stats(stats, st);
+        for (int i = 0; i < k; i++) {
+            status[first + i] = ps[i].status;
+            messages[first + i] = ps[i].message;
+            if (ps[i].status == DG_OK) proofs_out[first + i] = ps[i].proof.release();
+        }
+    }
+    release.done = true;
+}
+
+}  // namespace
 
 Proof *prove_device(Context &c, const fe *d_regs, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
                     const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
                     dg_prove_stats_t *stats, float) {
-    return prove_core(c, const_cast<fe *>(d_regs), nullptr, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs, opt, stats);
+    return prove_one(c, const_cast<fe *>(d_regs), nullptr, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs, opt, stats);
 }
 
 Proof *prove_host(Context &c, const dg_trace_t &trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16,
@@ -751,8 +1058,40 @@ Proof *prove_host(Context &c, const dg_trace_t &trace, const uint8_t *inputs16, 
     DG_REQUIRE(trace.length >= 16 && (trace.length & (trace.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
     for (uint32_t j = 0; j < trace.width; j++) DG_REQUIRE(trace.columns[j] != nullptr, "null register column");
     c.upload_buf.ensure((size_t)trace.length * 16 * trace.width, true);
-    return prove_core(c, c.upload_buf.as<fe>(), trace.columns, trace.width, trace.length, trace.ctx_depth, trace.loop_depth, inputs16, n_inputs,
-                      outputs16, n_outputs, opt, stats);
+    return prove_one(c, c.upload_buf.as<fe>(), trace.columns, trace.width, trace.length, trace.ctx_depth, trace.loop_depth, inputs16, n_inputs,
+                     outputs16, n_outputs, opt, stats);
+}
+
+void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                      const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, Proof **proofs_out, int *status,
+                      std::vector<std::string> &messages, dg_prove_stats_t *stats) {
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    const dg_trace_t &t0 = traces[0];
+    for (uint32_t i = 0; i < count; i++) {
+        const dg_trace_t &t = traces[i];
+        DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
+                   "all traces of a batch must have the same width, length, context depth and loop depth");
+        DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
+        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
+    }
+    DG_REQUIRE(t0.length >= 16 && (t0.length & (t0.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
+    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
+    prove_groups(c, count, t0.width, t0.length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st) {
+        std::vector<const uint8_t *> cols;
+        for (int i = 0; i < k; i++) cols.insert(cols.end(), traces[first + i].columns, traces[first + i].columns + t0.width);
+        c.upload_buf.ensure((size_t)t0.length * 16 * t0.width * k, true);
+        prove_core(c, c.upload_buf.as<fe>(), cols.data(), k, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, ps, opt, st);
+    });
+}
+
+void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                        const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats) {
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
+    prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st) {
+        prove_core(c, const_cast<fe *>(d_regs) + (size_t)first * width * length, nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st);
+    });
 }
 
 }  // namespace dg

@@ -17,5 +17,13 @@ Proof *prove_host(Context &c, const dg_trace_t &trace, const uint8_t *inputs16, 
 Proof *prove_device(Context &c, const fe *d_registers, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
                     const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
                     dg_prove_stats_t *stats, float h2d_ms);
+// batched proving (dg_prove_batch / dg_prove_batch_device): proofs_out[i] / status[i] / messages[i] (why trace i failed, else empty) per
+// trace, one GPU only; when the call throws, no proof is left in proofs_out
+void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                      const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, Proof **proofs_out, int *status,
+                      std::vector<std::string> &messages, dg_prove_stats_t *stats);
+void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                        const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
 
 }  // namespace dg

@@ -58,11 +58,14 @@ void interleave_roots(Context &c, const void *gathered, void *upper, unsigned lo
 }
 
 // items[k * (nc/4) + c4] = H(ev[4c4][k], ev[4c4+1][k], ev[4c4+2][k], ev[4c4+3][k]) over the local cosets (prover.rs:84-86,180-187)
+// blockIdx.y = slab of a batch: evaluations n << log_nc elements apart, items `total` digests apart
 __global__ void __launch_bounds__(256) constraint_items_kernel(const fe *__restrict__ ev, int log_n, int log_nc, uint4 *__restrict__ items) {
     const unsigned long long n = 1ULL << log_n;
     const unsigned long long total = n << (log_nc - 2);
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= total) return;
+    ev += blockIdx.y * (n << log_nc);
+    items += blockIdx.y * 2 * total;
     const unsigned long long c4 = t >> log_n, k = t & (n - 1);
     const unsigned long long j = (k << (log_nc - 2)) + c4;
     uint32_t m[16], cv[8];
@@ -75,9 +78,11 @@ __global__ void __launch_bounds__(256) constraint_items_kernel(const fe *__restr
     items[2 * j] = make_uint4(cv[0], cv[1], cv[2], cv[3]);
     items[2 * j + 1] = make_uint4(cv[4], cv[5], cv[6], cv[7]);
 }
-void constraint_items_local(Context &c, const fe *evals_local, int log_n, int log_nc, void *items) {
+void constraint_items_local(Context &c, const fe *evals_local, int log_n, int log_nc, void *items, int batch) {
     const unsigned long long total = (1ULL << log_n) << (log_nc - 2);
-    constraint_items_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.stream>>>(evals_local, log_n, log_nc, (uint4 *)items); c.launches++;
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "constraint item batch out of range");
+    constraint_items_kernel<<<dim3((unsigned)((total + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(evals_local, log_n, log_nc, (uint4 *)items);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -93,7 +98,7 @@ void ShardedTree::build(Context &c, const void *items_local_dev, uint64_t n, int
         DG_REQUIRE(local_items >= 2, "tree needs at least 2 items");
         local_nodes.alloc(local_items * 32);
         merkle_build(c, items_local_dev, local_nodes.p, local_items);
-        mid_p = top_p = local_nodes.p;
+        mid_p = top_p = local_p = local_nodes.p;
     } else {
         DG_REQUIRE(n >= G && n % G == 0, "sharded tree needs at least one block per rank and k-range");
         const void *roots = items_local_dev;
@@ -116,11 +121,20 @@ void ShardedTree::build(Context &c, const void *items_local_dev, uint64_t n, int
         merkle_finish(c, top.p, G);
         if (c.mark) c.mark("tree.mid+top");
         mid_p = mid.p; top_p = top.p;
+        local_p = local_nodes.p;
     }
     if (fetch_root) {
         DG_CUDA(cudaMemcpyAsync(root.data(), (const uint8_t *)top_p + 32, 32, cudaMemcpyDeviceToHost, c.stream));
         DG_CUDA(cudaStreamSynchronize(c.stream));
     }
+}
+
+void ShardedTree::attach(Context &c, const void *items_dev, const void *nodes_dev, uint64_t n, int log_blk) {
+    DG_REQUIRE(c.world == 1, "a tree built in a batch lives on one GPU");
+    geom.n = n; geom.log_blk = log_blk; geom.log_g = 0;
+    items_local = items_dev;
+    local_nodes.release();
+    mid_p = top_p = local_p = nodes_dev;
 }
 
 // out[t] = base_t ? ((const uint4 *)base_t)[unit_t] : 0

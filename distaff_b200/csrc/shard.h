@@ -69,10 +69,13 @@ struct ShardedTree {
     DevBuf local_nodes;                  // heap over the local items (valid for levels with >= n nodes)
     DevBuf mid, top;                     // mid: heap over this rank's n nodes of the level n*G (2n digests); top: replicated heap of 2G digests
     const void *mid_p = nullptr, *top_p = nullptr;     // one rank: both alias the local heap (global heap indices)
+    const void *local_p = nullptr;                     // the local heap (local_nodes, or a heap owned by the caller: attach)
     Digest root;
 
     // fetch_root = false leaves the root on the device (upper_p + 32): no host synchronisation
     void build(Context &c, const void *items_local_dev, uint64_t n, int log_blk, bool fetch_root = true);
+    // one GPU: the tree over items_dev whose heap (n << log_blk digests) the caller has built (merkle_build_batch) and owns
+    void attach(Context &c, const void *items_dev, const void *nodes_dev, uint64_t n, int log_blk);
     const void *root_dev() const { return (const uint8_t *)top_p + 32; }
     // locations as references for a FetchBatch
     FetchRef item_ref(uint64_t item_index) const { ShardLocation l = geom.item(item_index); return FetchRef{items_local, l.index, l.owner}; }
@@ -80,7 +83,7 @@ struct ShardedTree {
         ShardLocation l = geom.node(heap_index);
         if (l.kind == SHARD_TOP) return FetchRef{top_p, l.index, -1};
         if (l.kind == SHARD_MID) return FetchRef{mid_p, l.index, l.owner};
-        return FetchRef{local_nodes.p, l.index, l.owner};
+        return FetchRef{local_p, l.index, l.owner};
     }
 };
 
@@ -88,6 +91,7 @@ void merkle_build_partial(Context &c, const void *leaves, void *nodes, unsigned 
 void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L);
 void merkle_finish(Context &c, void *nodes, unsigned long long m);
 void interleave_roots(Context &c, const void *gathered, void *upper, unsigned long long n, int log_g);
-void constraint_items_local(Context &c, const fe *evals_local, int log_n, int log_nc, void *items);   // [k][c4_local] digests
+// [k][c4_local] digests; batch > 1: `batch` slabs of n << log_nc evaluations, their items (n << log_nc) / 4 digests apart
+void constraint_items_local(Context &c, const fe *evals_local, int log_n, int log_nc, void *items, int batch = 1);
 
 }  // namespace dg

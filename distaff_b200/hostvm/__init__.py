@@ -121,9 +121,10 @@ def merkle_program(depth, index):
     return f"begin read.ab dup.2 smpath.{depth} swap.2 push.{index} roll.4 swap swap.2 pmpath.{depth} end"
 
 
-def merkle_paths(depth, count):
+def merkle_paths(depth, count, seed=0):
     """`count` Merkle authentication paths of length `depth` verified back to back with the program of examples/merkle.rs:41-57 (paths
-    drawn from field::prng_vector with the example's seeds, path number in byte 3).  The example itself is capped at depth 64 = 2^12
+    drawn from field::prng_vector with the example's seeds, path number in byte 3, `seed` in bytes 4-5: different seeds give different
+    traces of one shape).  The example itself is capped at depth 64 = 2^12
     steps by its own index arithmetic (examples/merkle.rs:75,106); four paths give BASELINE's 2^14-step Rescue-dominated trace."""
     import ctypes
     from .. import backend
@@ -136,8 +137,8 @@ def merkle_paths(depth, count):
 
     a_all, b_all, blocks = [], [], []
     for c in range(count):
-        p0 = prng_vector(bytes([1, 2, 3, c] + [0] * 28), depth)
-        p1 = prng_vector(bytes([4, 5, 6, c] + [0] * 28), depth)
+        p0 = prng_vector(bytes([1, 2, 3, c, seed & 255, seed >> 8] + [0] * 26), depth)
+        p1 = prng_vector(bytes([4, 5, 6, c, seed & 255, seed >> 8] + [0] * 26), depth)
         leaf_index = p0[0] % (2 ** (depth - 1))
         a, b = [p0[0]], [p1[0]]
         index = leaf_index + 2 ** (depth - 1)

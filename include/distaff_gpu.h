@@ -72,6 +72,25 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
                     const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
                     const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats);
 
+/* Batched proving: `count` traces of ONE shape (same width, length, ctx_depth, loop_depth) proven with the same options in one call; every
+ * stage runs once over the whole batch, and every host round trip carries the values of all its proofs.  Public inputs / outputs are
+ * per trace (inputs16[i] holds n_inputs[i] elements; the arrays may be NULL when every count is 0).  Per trace: status[i] = DG_OK and
+ * proofs_out[i] a proof byte-identical to dg_prove of that trace, or a per-trace failure (DG_ERR_UNSATISFIED, DG_ERR_EXHAUSTED) with
+ * proofs_out[i] = NULL; a failing trace does not change any other trace's proof.  Returns DG_OK when the batch ran (even if some traces
+ * failed), otherwise the error of the whole call (DG_ERR_INVALID for count == 0, mixed shapes, bad options or a context that spans
+ * several GPUs; DG_ERR_CUDA; DG_ERR_NO_DEVICE); on such an error every proofs_out[i] is NULL (nothing to free).  The library splits the
+ * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
+ * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) why trace i of the calling
+ * thread's last batched call failed -- the message dg_prove gives for that trace -- or "" if it was proven. */
+int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                   int *status, dg_prove_stats_t *stats);
+/* same, registers already in device memory: one allocation, proof-major [count][width][length] elements */
+int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                          const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                          const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats);
+int dg_batch_message(uint32_t index, char *message, size_t message_cap);
+
 /* Optional: randomness supplied by the host.  The prover derives all of its Fiat-Shamir challenges from two reference functions,
  *   field::prng_vector(seed, n)                            (math/field.rs:264-275: StdRng::from_seed + Uniform(0..M))
  *   utils::compute_query_positions(seed, domain, options)  (stark/utils/mod.rs:25-44: StdRng + Uniform(0..domain), rejections)
