@@ -47,11 +47,7 @@ __device__ __forceinline__ fe tw_pow(const TwiddleRef &t, unsigned long long e) 
 
 // DG_STEP() is a block barrier every few hundred instructions: the warps of a block walk the code together, so that an instruction
 // line is fetched once per block instead of once per warp.
-#ifdef DG_AIR_NOSYNC
-#define DG_STEP()
-#else
 #define DG_STEP() __syncthreads()
-#endif
 
 template <int W>
 __device__ __forceinline__ void matvec(const fe *m, fe *s) {
@@ -491,13 +487,13 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_kernel(cons
     if (live) P.t_ev[out_idx] = t_res;
 }
 
-// Shared-memory variant (n >= BLOCK): the rows of a block's BLOCK consecutive steps of one coset are staged once in shared memory,
+// Shared-memory kernel (n >= BLOCK): the rows of a block's BLOCK consecutive steps of one coset are staged once in shared memory,
 // column-major with pitch BLOCK + 1 -- slot t holds the row of thread t, slot t + 1 is its "next" row (the row of thread t + 1, or the
 // extra row BLOCK for the last thread).  Context / loop / user-stack registers are then addressed dynamically in shared memory instead
 // of in per-thread arrays, which the runtime loop bounds used to force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
-// STAGE_DEC: the 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
+// The 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
 // BATCH: blockIdx.y is the proof of a batch (AirParams strides); a separate instantiation, so that one proof compiles as before.
-template <int BLOCK, int MIN_BLOCKS, bool STAGE_DEC, bool WIDE_SLOTS, bool BATCH = false>
+template <int BLOCK, int MIN_BLOCKS, bool BATCH = false>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel(const AirParams P) {
     extern __shared__ __align__(16) unsigned char air_smem[];
     fe *s_rows = reinterpret_cast<fe *>(air_smem);
@@ -516,7 +512,6 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     const unsigned long long lde_index = s * (unsigned long long)stride;   // = k*blowup + c8*stride
     const fe *const ext = BATCH ? P.ext + blockIdx.y * P.ext_stride : P.ext;
     const fe *cur_p = ext + (c8_local * stride) * n + k;              // the slab starts at coset c8_base*stride
-    const fe *nxt_p = ext + (c8_local * stride) * n + ((k + 1) & (n - 1));
     const unsigned long long out_idx = (c8_local << P.log_n) + k;
 
     const int cl = P.cl, ll = P.ll, sl = P.sl;
@@ -524,26 +519,20 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 
     // ---- the two rows.  Boundary constraints are not evaluated here: their numerators are assembled in coefficient form from the
     //      trace polynomials (poly.cu: boundary_coeffs), which is 8x less work than evaluating them on this domain.
-    constexpr int S0 = STAGE_DEC ? 0 : 15;            // first staged column
     {
-        const int staged = P.w - S0;
-        for (int j = 0; j < staged; j++) s_rows[j * PITCH + tid] = cur_p[(unsigned long long)(S0 + j) * N];
+        const int w = P.w;
+        for (int j = 0; j < w; j++) s_rows[j * PITCH + tid] = cur_p[(unsigned long long)j * N];
         // the extra row: "next" of the block's last thread (k + 1 wraps to 0 of the same coset at the end of the coset)
-        if (tid < staged) {
+        if (tid < w) {
             const unsigned long long gl = (unsigned long long)blockIdx.x * BLOCK + (BLOCK - 1);
             const unsigned long long cl8 = gl >> P.log_n, kl = gl & (n - 1);
-            s_rows[tid * PITCH + BLOCK] = ext[(unsigned long long)(S0 + tid) * N + (cl8 * stride) * n + ((kl + 1) & (n - 1))];
+            s_rows[tid * PITCH + BLOCK] = ext[(unsigned long long)tid * N + (cl8 * stride) * n + ((kl + 1) & (n - 1))];
         }
     }
-    fe cur_dec[STAGE_DEC ? 1 : 15], nxt_dec[STAGE_DEC ? 1 : 15];
-    if constexpr (!STAGE_DEC) {
-#pragma unroll
-        for (int j = 0; j < 15; j++) { cur_dec[j] = cur_p[(unsigned long long)j * N]; nxt_dec[j] = nxt_p[(unsigned long long)j * N]; }
-    }
     __syncthreads();
-#define DCUR(j) (STAGE_DEC ? s_rows[(j) * PITCH + tid] : cur_dec[STAGE_DEC ? 0 : (j)])
-#define DNXT(j) (STAGE_DEC ? s_rows[(j) * PITCH + tid + 1] : nxt_dec[STAGE_DEC ? 0 : (j)])
-#define SCOL(col, nx) s_rows[((col) - S0) * PITCH + tid + (nx)]
+#define SCOL(col, nx) s_rows[(col) * PITCH + tid + (nx)]
+#define DCUR(j) s_rows[(j) * PITCH + tid]
+#define DNXT(j) s_rows[(j) * PITCH + tid + 1]
 #define C_CTX(i) (((i) < P.ctx_depth) ? SCOL(ctx_off + (i), 0) : ZERO)
 #define N_CTX(i) (((i) < P.ctx_depth) ? SCOL(ctx_off + (i), 1) : ZERO)
 #define C_LOOP(i) (((i) < P.loop_depth) ? SCOL(loop_off + (i), 0) : ZERO)
@@ -775,27 +764,17 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         // generic part of slot i; fc / fl1 / fl2 / fl4 are the copy and left-shift flag sums that apply to this slot
         auto slot_value = [&](const int i, const fe fc, const fe fl1, const fe fl2, const fe fl4) -> fe {
             const fe nwi = NW(i);
-            if (WIDE_SLOTS) {
-                // the seven products of a slot are accumulated unreduced (288 bits) and reduced once: 7 x (product + 9-limb add) + 1 reduction
-                // instead of 7 x (modular product + modular add)
-                fe_wide acc7;
-                wide_set(acc7, DG_MUL_WIDE(fc, fe_sub(O(i), nwi)));
-                if (i >= 1) wide_add(acc7, DG_MUL_WIDE(f_rs1, fe_sub(O(i - 1), nwi)));
-                if (i >= 2) wide_add(acc7, DG_MUL_WIDE(f_rs2, fe_sub(O(i - 2), nwi)));
-                if (i >= 4) wide_add(acc7, DG_MUL_WIDE(f_rs4, fe_sub(O(i - 4), nwi)));
-                wide_add(acc7, DG_MUL_WIDE(fl1, (i < L - 1) ? fe_sub(O(i + 1), nwi) : nwi));
-                wide_add(acc7, DG_MUL_WIDE(fl2, (i < L - 2) ? fe_sub(O(i + 2), nwi) : nwi));
-                wide_add(acc7, DG_MUL_WIDE(fl4, (i < L - 4) ? fe_sub(O(i + 4), nwi) : nwi));
-                return DG_REDUCE_WIDE(acc7);
-            }
-            fe v = fe_mul(fc, fe_sub(O(i), nwi));
-            if (i >= 1) v = fe_add(v, fe_mul(f_rs1, fe_sub(O(i - 1), nwi)));
-            if (i >= 2) v = fe_add(v, fe_mul(f_rs2, fe_sub(O(i - 2), nwi)));
-            if (i >= 4) v = fe_add(v, fe_mul(f_rs4, fe_sub(O(i - 4), nwi)));
-            v = fe_add(v, fe_mul(fl1, (i < L - 1) ? fe_sub(O(i + 1), nwi) : nwi));
-            v = fe_add(v, fe_mul(fl2, (i < L - 2) ? fe_sub(O(i + 2), nwi) : nwi));
-            v = fe_add(v, fe_mul(fl4, (i < L - 4) ? fe_sub(O(i + 4), nwi) : nwi));
-            return v;
+            // the seven products of a slot are accumulated unreduced (288 bits) and reduced once: 7 x (product + 9-limb add) + 1 reduction
+            // instead of 7 x (modular product + modular add)
+            fe_wide acc7;
+            wide_set(acc7, DG_MUL_WIDE(fc, fe_sub(O(i), nwi)));
+            if (i >= 1) wide_add(acc7, DG_MUL_WIDE(f_rs1, fe_sub(O(i - 1), nwi)));
+            if (i >= 2) wide_add(acc7, DG_MUL_WIDE(f_rs2, fe_sub(O(i - 2), nwi)));
+            if (i >= 4) wide_add(acc7, DG_MUL_WIDE(f_rs4, fe_sub(O(i - 4), nwi)));
+            wide_add(acc7, DG_MUL_WIDE(fl1, (i < L - 1) ? fe_sub(O(i + 1), nwi) : nwi));
+            wide_add(acc7, DG_MUL_WIDE(fl2, (i < L - 2) ? fe_sub(O(i + 2), nwi) : nwi));
+            wide_add(acc7, DG_MUL_WIDE(fl4, (i < L - 4) ? fe_sub(O(i + 4), nwi) : nwi));
+            return DG_REDUCE_WIDE(acc7);
         };
         fe fc_hi, fl1_hi, fl2_hi, fl4_hi;                  // the sums for slots >= 8 (every shape applies)
         {
@@ -954,51 +933,31 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 
 void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     air_upload_constants(c);
-    const unsigned long long E = (unsigned long long)P.num_c8 << P.log_n;
-    static int variant = -1;
-    if (variant < 0) { const char *e = getenv("DG_AIR_CFG"); variant = e ? atoi(e) : 7; }
-#define DG_AIR_LAUNCH(BLOCK, MINB) constraint_eval_kernel<BLOCK, MINB><<<(unsigned)((E + BLOCK - 1) / BLOCK), BLOCK, 0, c.stream>>>(P)
-#define DG_AIR_LAUNCH_SMEM(BLOCK, MINB, DEC, WIDE)                                                                                         \
-    do {                                                                                                                             \
-        const size_t smem = (size_t)(P.w - ((DEC) ? 0 : 15)) * (BLOCK + 1) * sizeof(fe);                                             \
-        auto k = constraint_eval_smem_kernel<BLOCK, MINB, DEC, WIDE>;                                                                      \
-        set_func_smem(c, (const void *)k, smem);                                                                                     \
-        k<<<(unsigned)(E / BLOCK), BLOCK, smem, c.stream>>>(P);                                                                      \
-    } while (0)
     DG_REQUIRE(batch >= 1 && batch <= 65535, "constraint evaluation batch out of range");
-    int v = variant;
+    const unsigned long long E = (unsigned long long)P.num_c8 << P.log_n;
     const unsigned long long n = 1ULL << P.log_n;
-    // the shared-memory variants need whole blocks inside one coset and at most ~200 KB of rows per block
-    if (v < 5 || v > 7) v = 1;
-    if (v >= 5 && (n < 128 || (size_t)P.w * 129 * sizeof(fe) > 200 * 1024)) v = 1;
-    if (batch > 1 && v == 7) {                      // the default variant: all proofs of the batch in one launch
+    // H100 SXM (700 W), stage 3 of the 2^20-step proof x 26 registers: per-thread arrays 24.8 ms; shared-memory rows, stack-like columns
+    // only 23.7; all columns 23.2; all columns + unreduced per-slot sums (constraint_eval_smem_kernel) 22.2.  The other shared-memory forms
+    // were removed after this measurement.
+    // The shared-memory kernel needs whole blocks inside one coset and at most ~200 KB of rows per block; all proofs of a batch run in one launch.
+    if (n >= 128 && (size_t)P.w * 129 * sizeof(fe) <= 200 * 1024) {
         const size_t smem = (size_t)P.w * 129 * sizeof(fe);
-        auto k = constraint_eval_smem_kernel<128, 4, true, true, true>;
+        auto k = batch > 1 ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
         set_func_smem(c, (const void *)k, smem);
         k<<<dim3((unsigned)(E / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
         c.launches++;
         DG_CUDA(cudaGetLastError());
         return;
     }
-    if (batch > 1) {                                // other variants: one launch per proof
-        for (int q = 0; q < batch; q++) {
-            AirParams Q = P;
-            Q.ext += q * P.ext_stride; Q.t_ev += q * P.t_ev_stride;
-            Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride; Q.violation += q;
-            launch_constraint_eval(c, Q, 1);
-        }
-        return;
+    // per-thread arrays: short traces (n < 128) and very wide ones, one launch per proof
+    for (int q = 0; q < batch; q++) {
+        AirParams Q = P;
+        Q.ext += q * P.ext_stride; Q.t_ev += q * P.t_ev_stride;
+        Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride; Q.violation += q;
+        constraint_eval_kernel<128, 4><<<(unsigned)((E + 127) / 128), 128, 0, c.stream>>>(Q);
+        c.launches++;
+        DG_CUDA(cudaGetLastError());
     }
-    // H100 SXM (700 W), stage 3 of the 2^20-step proof x 26 registers (tools/variant_bench.py): per-thread arrays (variant 1) 24.8 ms;
-    // shared-memory rows, stack-like columns only (5) 23.7; all columns (6) 23.2; all columns + unreduced per-slot sums (7) 22.2
-    switch (v) {
-        case 5: DG_AIR_LAUNCH_SMEM(128, 4, false, false); break;     // only the context / loop / stack columns staged
-        case 6: DG_AIR_LAUNCH_SMEM(128, 4, true, false); break;      // all columns staged
-        case 7: DG_AIR_LAUNCH_SMEM(128, 4, true, true); break;       // default: + unreduced accumulation of the seven products of a stack slot
-        default: DG_AIR_LAUNCH(128, 4); break;                 // per-thread arrays: short traces (n < 128) and very wide ones
-    }
-    c.launches++;
-    DG_CUDA(cudaGetLastError());
 }
 
 }  // namespace dg

@@ -27,8 +27,8 @@ struct AirParams {
     unsigned long long ext_stride, t_ev_stride, coef_stride;
 };
 
-// evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P); the default variant runs them in
-// one launch (blockIdx.y = proof), the measurement variants (DG_AIR_CFG != 7) launch once per proof
+// evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P); the shared-memory kernel runs them in
+// one launch (blockIdx.y = proof), the per-thread kernel of short or very wide traces launches once per proof
 void launch_constraint_eval(Context &c, const AirParams &P, int batch = 1);
 
 }  // namespace dg

@@ -112,8 +112,6 @@ __device__ __forceinline__ fe fe_add(fe a, fe b) {
     return r;
 }
 
-
-#ifndef DG_SUB_V1
 // a - b: subtract, then subtract C when the difference borrowed (a - b + M = a - b - C mod 2^128); always canonical
 __device__ __forceinline__ fe fe_sub(fe a, fe b) {
     unsigned int d0, d1, d2, d3, m, c1;
@@ -136,24 +134,6 @@ __device__ __forceinline__ fe fe_sub(fe a, fe b) {
     r.hi = ((unsigned long long)d3 << 32) | d2;
     return r;
 }
-#else
-__device__ __forceinline__ fe fe_sub(fe a, fe b) {
-    unsigned long long d0, d1, t0, t1;
-    unsigned int bw;
-    asm("{\n\t"
-        "sub.cc.u64  %0, %5, %7;\n\t"
-        "subc.cc.u64 %1, %6, %8;\n\t"
-        "subc.u32    %4, 0, 0;\n\t"
-        "sub.cc.u64  %2, %0, %9;\n\t"
-        "subc.u64    %3, %1, 0;\n\t"
-        "}"
-        : "=&l"(d0), "=&l"(d1), "=&l"(t0), "=&l"(t1), "=&r"(bw)
-        : "l"(a.lo), "l"(a.hi), "l"(b.lo), "l"(b.hi), "l"(DG_C_LO));
-    fe r; r.lo = bw ? t0 : d0; r.hi = bw ? t1 : d1;   // a - b + M == a - b - C (mod 2^128)
-    return r;
-}
-
-#endif
 
 __device__ __forceinline__ fe fe_neg(fe a) { return fe_sub(fe_make(0, 0), a); }
 

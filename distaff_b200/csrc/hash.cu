@@ -72,11 +72,9 @@ __global__ void __launch_bounds__(256) hash_rows_kernel(const fe *__restrict__ e
 void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup, int batch, unsigned long long ext_stride) {
     const unsigned long long N = 1ULL << (log_n + log_blowup);
     DG_REQUIRE(batch >= 1 && batch <= 65535, "row hashing batch out of range");
-    static int fma = -1;
-    if (fma < 0) { const char *e = getenv("DG_B3_FMA"); fma = e ? atoi(e) : 1; }      // FMA-pipe additions: trace tree 10.3 -> 8.8 ms at 2^25 rows x 26 columns (H100 SXM, 700 W)
     const dim3 grid((unsigned)((N + 255) / 256), (unsigned)batch);
-    if (fma) hash_rows_kernel<true><<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, N, log_n, log_blowup, 1u, ext_stride);
-    else hash_rows_kernel<false><<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, N, log_n, log_blowup, 1u, ext_stride);
+    // FMA-pipe additions: trace tree 10.3 -> 8.8 ms at 2^25 rows x 26 columns (H100 SXM, 700 W)
+    hash_rows_kernel<true><<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, N, log_n, log_blowup, 1u, ext_stride);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
@@ -265,11 +263,7 @@ std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<s
     if (K > 1) {
         int log_k = 0;
         while ((1u << log_k) < K) log_k++;
-        int lg = std::max(10, std::min(22, std::max((int)grinding - 2, 22 - log_k)));
-        static int forced = -1;                   // DG_POW_WINDOW_LOG: per-proof window of a batch (measurement only)
-        if (forced < 0) { const char *e = getenv("DG_POW_WINDOW_LOG"); forced = e ? std::max(8, std::min(24, atoi(e))) : 0; }
-        if (forced) lg = forced;
-        window = 1ULL << lg;
+        window = 1ULL << std::max(10, std::min(22, std::max((int)grinding - 2, 22 - log_k)));
     }
     std::vector<unsigned> active(K);
     for (unsigned p = 0; p < K; p++) active[p] = p;

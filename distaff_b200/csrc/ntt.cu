@@ -19,14 +19,11 @@
 // (one shared 80-instruction body) the pass kernels are much smaller.  The large transforms use inlined multiplies with small
 // register rounds instead (ntt_inl.cu): the small rounds keep the unrolled code near the instruction-cache size without a call per multiply.
 // Each kernel is specialised at compile time for one pass kind (PassKind, ntt_pass.cuh), so it holds only its own input and output
-// paths; at the default shape (4-element register rounds, 512 threads, 64 registers) the kernels of the 2^20-step proof do not spill.
+// paths; with 4-element register rounds, 512 threads and 64 registers the kernels of the 2^20-step proof do not spill.
 #define DG_MUL_CALL 1
 #include "ntt_pass.cuh"
 
 namespace dg {
-
-// kernel variants (ntt_pass.cuh): RMAX stages per register round, BT threads per block; inline-multiply instantiations live in ntt_inl.cu
-PassKernel pass_kernel_inline(int kind, int log_l, int rmax, int bt);       // nullptr when that combination is not instantiated
 
 // the kernel specialisation of a pass, from the flags run_transform sets
 static int pass_kind(const PassGeom &g) {
@@ -43,60 +40,27 @@ static int pass_kind(const PassGeom &g) {
     return g.has_scale ? PK_LAST_SCALE : PK_LAST;
 }
 
-// Kernel configuration per pass position: A = strided passes (first / middle), B = the contiguous last pass; "f" variants are used by the
-// transforms whose first pass folds 8 coefficient blocks (constraint / composition LDE).  H100 SXM 80 GB (700 W power limit), stage 1 of
-// the 2^20-step proof (26 columns, LDE x32), tools/variant_bench.py, ms:
-//   default: inline multiply, 4-element units (rmax 2), 512 threads for A and B: 52.7 (no spills at the 64-register cap)
+// Pass kernel shape (ntt_pass.cuh: PASS_RMAX, PASS_THREADS, PASS_INLINE_LOG_L) and tile size.  H100 SXM 80 GB (700 W power limit),
+// stage 1 of the 2^20-step proof (26 columns, LDE x32), ms (A = strided first / middle passes, B = contiguous last pass, AF = fold-8
+// first passes):
+//   inline multiply, 4-element units (rmax 2), 512 threads, 4096-element tiles: 52.7 (no spills at the 64-register cap)
 //   A = B = 8-element units (rmax 3), 512 threads: 56.9 (150-570 bytes of spills per kernel at the 64-register cap)
 //   measured before the kernels were specialised per pass kind (every kind's path in one kernel, a call per multiply):
 //   rmax 3 for A and B 60.8 - 61.3;  A = 256 threads 68.0;  A = 1024 threads + 8192-element tiles 71.7;  B = 256 threads 62.5;
 //   AF = 8-element units or 256 threads: no change in stages 5 / 6
-// Environment overrides (read once): DG_NTT_A / DG_NTT_B / DG_NTT_AF = "rmax,threads,inline", DG_NTT_TILE = log2 of the tile size.
-struct PassCfg { int rmax, bt, inl; };
-struct NttConfig { PassCfg a, b, af; int tile_log; };
-static PassCfg parse_cfg(const char *env, PassCfg d) {
-    const char *e = getenv(env);
-    if (e) { int r = 0, t = 0, i = 0; if (sscanf(e, "%d,%d,%d", &r, &t, &i) == 3) d = PassCfg{r, t, i}; }
-    if (d.rmax < 2 || d.rmax > 4) d.rmax = 4;
-    if (d.bt != 512 && d.bt != 1024) d.bt = 256;
-    return d;
-}
-static const NttConfig &ntt_config() {
-    static NttConfig cfg;
-    static bool init = false;
-    if (!init) {
-        cfg.a = parse_cfg("DG_NTT_A", PassCfg{2, 512, 1});
-        cfg.b = parse_cfg("DG_NTT_B", PassCfg{2, 512, 1});
-        cfg.af = parse_cfg("DG_NTT_AF", PassCfg{2, 512, 1});
-        const char *e = getenv("DG_NTT_TILE");
-        cfg.tile_log = e ? atoi(e) : 12;
-        if (cfg.tile_log < 12 || cfg.tile_log > 13) cfg.tile_log = 12;
-        init = true;
-    }
-    return cfg;
-}
+// The other shapes were removed after this measurement.
+static const int TILE = 4096;                    // elements per block = 64 KB
 
 static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *dst, unsigned blocks_x, unsigned by, unsigned bz) {
     const int L = 1 << log_l, T = 1 << g.log_t;
     const size_t data = g.lane_major ? (size_t)T * (L + (L >> 3) + 1) : (size_t)L * T;
     const size_t smem = ((size_t)L + data) * sizeof(fe);
-    const NttConfig &nc = ntt_config();
-    const PassCfg cfg = g.lane_major ? nc.b : ((g.coset_on && !g.coset_fast) ? nc.af : nc.a);
     const int kind = pass_kind(g);
-    int rmax = cfg.rmax, bt = cfg.bt;
-    PassKernel k = nullptr;
-    if (cfg.inl) k = pass_kernel_inline(kind, log_l, rmax, bt);
-    if (!k) {
-        if (bt == 1024) bt = 512;
-        if (rmax == 4) { bt = 256; k = pass_kernel_of<4, 256, 2, 0, 1, MAX_LOG_L>(kind, log_l); }
-        else if (rmax == 3 && bt == 512) k = pass_kernel_of<3, 512, 2, 0, 1, MAX_LOG_L>(kind, log_l);
-        else if (rmax == 3) k = pass_kernel_of<3, 256, 3, 0, 1, MAX_LOG_L>(kind, log_l);
-        else if (bt == 512) k = pass_kernel_of<2, 512, 2, 0, 1, MAX_LOG_L>(kind, log_l);
-        else k = pass_kernel_of<2, 256, 4, 0, 1, MAX_LOG_L>(kind, log_l);
-    }
+    const PassKernel k = log_l >= PASS_INLINE_LOG_L ? pass_kernel_inline(kind, log_l)
+                                                    : pass_kernel_of<PASS_RMAX, PASS_THREADS, PASS_MINB, 0, 1, PASS_INLINE_LOG_L - 1>(kind, log_l);
     DG_REQUIRE(k, "unsupported sub-transform size");
-    int threads = (L * T) >> (log_l < rmax ? log_l : rmax);           // one unit per thread in the largest round
-    if (threads > bt) threads = bt;
+    int threads = (L * T) >> (log_l < PASS_RMAX ? log_l : PASS_RMAX);           // one unit per thread in the largest round
+    if (threads > PASS_THREADS) threads = PASS_THREADS;
     if (threads < 32) threads = 32;
     set_func_smem(c, (const void *)k, 200 * 1024);
     DG_REQUIRE(by <= 65535 && bz <= 65535, "batch too large for one launch");
@@ -108,8 +72,7 @@ static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *ds
 
 static int lanes_log(int log_l, long long available) {
     int lt = 4;                                   // 16 lanes
-    const int tile = 1 << ntt_config().tile_log;
-    while ((1 << (log_l + lt)) > tile && lt > 0) lt--;    // keep tiles at 4096 elements = 64 KB (8192 with DG_NTT_TILE=13)
+    while ((1 << (log_l + lt)) > TILE && lt > 0) lt--;
     while ((1LL << lt) > available && lt > 0) lt--;
     return lt;
 }
@@ -135,10 +98,8 @@ __global__ void lde_twiddle_fill_kernel(fe *table, TwiddleRef cw, int log_n, int
     table[i] = tw_lookup(cw, lane * ((k << log_b) + c));
 }
 static const fe *lde_twiddle_table(Context &c, int log_n, int log_b, int l0) {
-    static long long cap = -1;
-    if (cap < 0) { const char *e = getenv("DG_LDE_TW_MB"); cap = (e ? atoll(e) : 1024) << 20; }    // 0 disables the table
     const size_t bytes = ((size_t)16 << (log_n + log_b));
-    if ((long long)bytes > cap) return nullptr;
+    if (bytes > ((size_t)1 << 30)) return nullptr;         // over 1 GiB (2^22 steps x 32): the pass uses the two-level table instead
     const long long key = ((long long)log_n << 16) | (log_b << 8) | l0;
     auto it = c.lde_twiddles.find(key);
     if (it == c.lde_twiddles.end()) {
@@ -317,9 +278,7 @@ void lde_batch(Context &c, const fe *src, fe *dst, int log_n, int log_blowup, in
     const unsigned b = 1u << log_blowup, cosets = ncosets ? ncosets : b;
     // any sub-range works (blockIdx.y = coset - coset0 indexes the streamed twiddles and dst); a range beyond the domain does not
     DG_REQUIRE(coset0 < b && cosets <= b - coset0, "coset range out of bounds");
-    static int prefold = -1;
-    if (prefold < 0) { const char *e = getenv("DG_LDE_PREFOLD"); prefold = e ? atoi(e) : 1; }
-    if (prefold && fold == 8 && cosets == (1u << log_blowup) && log_blowup >= 3 && log_blowup <= 8 && (batch == 1 || dst_stride == n * cosets) &&
+    if (fold == 8 && cosets == (1u << log_blowup) && log_blowup >= 3 && log_blowup <= 8 && (batch == 1 || dst_stride == n * cosets) &&
         batch <= 65535) {
         // all cosets: input transform for every coset in one kernel, then b plain transforms (H100 SXM, 700 W, 2^20-step proof: stage 5 5.35 -> 3.83 ms, stage 6 5.83 -> 4.30 ms);
         // a batch of vectors whose outputs are contiguous runs both steps once for all of them
@@ -334,10 +293,8 @@ void lde_batch(Context &c, const fe *src, fe *dst, int log_n, int log_blowup, in
         return;
     }
     // scratch of the two-pass transforms: one intermediate of n * cosets elements per vector; more vectors per launch = fewer passes over
-    // the streamed first-pass twiddles (DG_NTT_SCRATCH_MB, default 4096)
-    static size_t scratch_cap = 0;
-    if (!scratch_cap) { const char *e = getenv("DG_NTT_SCRATCH_MB"); scratch_cap = (size_t)(e ? atoll(e) : 4096) << 20; }
-    size_t max_chunk = std::max<size_t>(1, scratch_cap / (n * cosets * sizeof(fe)));
+    // the streamed first-pass twiddles (at most 4 GiB of scratch)
+    size_t max_chunk = std::max<size_t>(1, ((size_t)4 << 30) / (n * cosets * sizeof(fe)));
     if (max_chunk > 65535) max_chunk = 65535;
     for (size_t b0 = 0; b0 < (size_t)batch; b0 += max_chunk) {
         size_t nb = std::min(max_chunk, (size_t)batch - b0);

@@ -69,8 +69,7 @@ __device__ __forceinline__ fe tw_lookup(const TwiddleRef &t, unsigned long long 
 // One block transforms a tile of T lanes x L points.  The log2(L) decimation-in-frequency stages are grouped into rounds of
 // up to RMAX stages that run entirely in registers on 2^rho elements per thread ("unit"); shared memory is touched only
 // between rounds.  The first round reads its operands straight from global memory and the last one writes straight back.
-// RMAX = 4: 16 elements per unit, 3 rounds for 1024 points (fewest shared-memory round trips, ~110 registers);
-// RMAX = 3 / 2: 8 / 4 elements per unit, 4 / 5 rounds (smaller unrolled bodies, fewer registers, more resident warps).
+// RMAX = 2: 4 elements per unit, 5 rounds for 1024 points (small unrolled bodies, few registers, many resident warps).
 // Stage twiddles come from per-stage compact tables W_st[j] = w_L^(j << st) (unit-stride, conflict-free) staged in shared memory.
 template <int LOG_L, int S0, int RHO>
 __device__ __forceinline__ void dif_regs(fe *x, const fe *s_tw, int g_lo) {
@@ -206,6 +205,11 @@ __global__ void __launch_bounds__(BT, MINB) ntt_pass_kernel(const fe *__restrict
 }
 
 typedef void (*PassKernel)(const fe *, fe *, const PassGeom);
+
+// The shape of every pass kernel (ntt.cu gives the measurements): 4-element register rounds, 512 threads, 2 blocks per SM.  Passes of
+// 2^PASS_INLINE_LOG_L points and more run the inline-multiply kernels of ntt_inl.cu, smaller ones the out-of-line kernels of ntt.cu.
+static const int PASS_RMAX = 2, PASS_THREADS = 512, PASS_MINB = 2, PASS_INLINE_LOG_L = 8;
+PassKernel pass_kernel_inline(int kind, int log_l);     // ntt_inl.cu: 2^PASS_INLINE_LOG_L .. 2^MAX_LOG_L points
 
 // the instantiation for (kind, log2 L) with L in [2^LO, 2^HI], nullptr outside
 template <int KIND, int RMAX, int BT, int MINB, int TAG, int LO, int HI> PassKernel pass_kernel_sized(int log_l) {

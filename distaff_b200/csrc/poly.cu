@@ -97,68 +97,11 @@ __device__ __forceinline__ fe block_suffix_inclusive(fe v, fe *s_warp, fe *block
     return fe_add(v, above);
 }
 
-__global__ void __launch_bounds__(SCAN_THREADS) scan_block_sums_kernel(const fe *__restrict__ data, fe *__restrict__ sums, unsigned long long len) {
-    __shared__ fe s_warp[SCAN_THREADS / 32];
-    const unsigned long long base = (unsigned long long)blockIdx.x * SCAN_BLOCK + (unsigned long long)threadIdx.x * SCAN_PER_THREAD;
-    fe v = fe_make(0, 0);
-#pragma unroll
-    for (int u = 0; u < SCAN_PER_THREAD; u++)
-        if (base + u < len) v = fe_add(v, data[base + u]);
-    fe total;
-    block_suffix_inclusive(v, s_warp, &total);
-    if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-// data[i] <- sum_{j>i, j in block} data[j] + carry[block]     (carry may be null)
-__global__ void __launch_bounds__(SCAN_THREADS) scan_apply_kernel(fe *__restrict__ data, const fe *__restrict__ carry, unsigned long long len) {
-    __shared__ fe s_warp[SCAN_THREADS / 32];
-    const unsigned long long base = (unsigned long long)blockIdx.x * SCAN_BLOCK + (unsigned long long)threadIdx.x * SCAN_PER_THREAD;
-    fe x[SCAN_PER_THREAD];
-    fe v = fe_make(0, 0);
-#pragma unroll
-    for (int u = 0; u < SCAN_PER_THREAD; u++) {
-        x[u] = (base + u < len) ? data[base + u] : fe_make(0, 0);
-        v = fe_add(v, x[u]);
-    }
-    fe incl = block_suffix_inclusive(v, s_warp, nullptr);
-    fe run = fe_sub(incl, v);                           // sum over threads strictly above
-    if (carry) run = fe_add(run, carry[blockIdx.x]);
-#pragma unroll
-    for (int u = SCAN_PER_THREAD - 1; u >= 0; u--) {
-        if (base + u < len) data[base + u] = run;
-        run = fe_add(run, x[u]);
-    }
-}
-
-void suffix_scan_exclusive(Context &c, fe *data, unsigned long long len) {
-    const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
-    if (nblk == 1) {
-        scan_apply_kernel<<<1, SCAN_THREADS, 0, c.stream>>>(data, nullptr, len); c.launches++;
-        DG_CUDA(cudaGetLastError());
-        return;
-    }
-    DevBuf sums(nblk * sizeof(fe));
-    scan_block_sums_kernel<<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(data, sums.as<fe>(), len); c.launches++;
-    DG_CUDA(cudaGetLastError());
-    suffix_scan_exclusive(c, sums.as<fe>(), nblk);
-    scan_apply_kernel<<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(data, sums.as<fe>(), len); c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
-
 // ---- synthetic division by (x - b) ----------------------------------------------------------------------------------------------------
-__global__ void scale_by_pow_kernel(const fe *__restrict__ in, fe *__restrict__ out, PowRef t, unsigned long long offset, unsigned long long len,
-                                    fe sub0) {
-    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= len) return;
-    fe v = in[i];
-    if (i == 0) v = fe_sub(v, sub0);
-    out[i] = fe_mul(v, pw(t, i + offset));
-}
-
 // Single-pass form (decoupled look-back, "chained scan"): one kernel reads every coefficient once and writes every quotient once.
 // Blocks take tickets in launch order and work from the top of the vector downwards; a block publishes the sum of its scaled
 // coefficients, then its first warp walks the descriptors of the blocks above it (32 at a time) until it meets one whose inclusive
-// suffix is known.  Replaces scale + block sums + recursive scan + apply + scale (7-9 launches, ~9 passes over the vector).
+// suffix is known.  One launch, where scale + block sums + recursive scan + apply + scale take 7-9 launches and ~9 passes over the vector.
 struct __align__(16) ScanDesc { fe agg; fe incl; int status; int pad[3]; };     // status: 0 nothing, 1 aggregate published, 2 inclusive suffix published
 
 __device__ __forceinline__ fe ld_cg_fe(const fe *p) {
@@ -251,40 +194,23 @@ __global__ void __launch_bounds__(SCAN_THREADS) syn_div_chained_kernel(const fe 
     }
 }
 
-// out[i] = sum_{j>i} (in[j] - [j==0] sub0) b^(j-i-1);   `scratch` holds len elements (used by the multi-pass form only).  in may equal out.
-void syn_div(Context &c, const fe *in, fe *out, fe *scratch, unsigned long long len, const PowRef &b_pows, const PowRef &binv_pows, fe sub0) {
-    static int chained = -1;
-    if (chained < 0) { const char *e = getenv("DG_SCAN_CHAINED"); chained = e ? atoi(e) : 1; }
-    if (chained) {
-        const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
-        DevBuf d((size_t)nblk * sizeof(ScanDesc) + 16);
-        DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
-        ScanDesc *desc = d.as<ScanDesc>();
-        unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk);
-        syn_div_chained_kernel<false><<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, sub0, desc, ticket, (unsigned)nblk,
-                                                                                    SynDivBatch{}); c.launches++;
-        DG_CUDA(cudaGetLastError());
-        return;
-    }
-    const unsigned blocks = (unsigned)((len + 255) / 256);
-    scale_by_pow_kernel<<<blocks, 256, 0, c.stream>>>(in, scratch, b_pows, 0, len, sub0); c.launches++;
-    DG_CUDA(cudaGetLastError());
-    suffix_scan_exclusive(c, scratch, len);
-    scale_by_pow_kernel<<<blocks, 256, 0, c.stream>>>(scratch, out, binv_pows, 1, len, fe_make(0, 0)); c.launches++;
+// out[i] = sum_{j>i} (in[j] - [j==0] sub0) b^(j-i-1).  in may equal out.
+void syn_div(Context &c, const fe *in, fe *out, unsigned long long len, const PowRef &b_pows, const PowRef &binv_pows, fe sub0) {
+    const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
+    DevBuf d((size_t)nblk * sizeof(ScanDesc) + 16);
+    DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
+    ScanDesc *desc = d.as<ScanDesc>();
+    unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk);
+    syn_div_chained_kernel<false><<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, sub0, desc, ticket, (unsigned)nblk,
+                                                                                SynDivBatch{}); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
-void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, fe *scratch,
-                   unsigned long long len, const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
+void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, unsigned long long len,
+                   const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
                    unsigned long long binv_lo_stride, unsigned long long binv_hi_stride, const fe *sub0_dev, const fe *sub0_host) {
-    static int chained = -1;
-    if (chained < 0) { const char *e = getenv("DG_SCAN_CHAINED"); chained = e ? atoi(e) : 1; }
-    if (!chained || batch == 1) {             // the multi-pass form (measurement only), or one vector: one syn_div per vector
-        for (int q = 0; q < batch; q++) {
-            PowRef b = b_pows, bi = binv_pows;
-            b.lo += q * b_lo_stride; b.hi += q * b_hi_stride; bi.lo += q * binv_lo_stride; bi.hi += q * binv_hi_stride;
-            syn_div(c, in + q * in_stride, out + q * out_stride, scratch, len, b, bi, sub0_host[q]);
-        }
+    if (batch == 1) {
+        syn_div(c, in, out, len, b_pows, binv_pows, sub0_host[0]);
         return;
     }
     const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;

@@ -24,12 +24,11 @@ struct PowTables {
     PowRef ref(int q) const { PowRef r; r.lo = lo.as<fe>() + q * lo_n; r.hi = hi.as<fe>() + q * hi_n; r.lo_bits = lo_bits; return r; }
 };
 
-void suffix_scan_exclusive(Context &c, fe *data, unsigned long long len);
-void syn_div(Context &c, const fe *in, fe *out, fe *scratch, unsigned long long len, const PowRef &b_pows, const PowRef &binv_pows, fe sub0);
+void syn_div(Context &c, const fe *in, fe *out, unsigned long long len, const PowRef &b_pows, const PowRef &binv_pows, fe sub0);
 // syn_div of `batch` vectors in one launch: vector q reads in + q in_stride, writes out + q out_stride, uses the power tables moved by
-// q * (lo, hi) strides and sub0_dev[q] (sub0_host[q] on the host: the per-vector fallback of DG_SCAN_CHAINED=0)
-void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, fe *scratch,
-                   unsigned long long len, const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
+// q * (lo, hi) strides and sub0_dev[q] (sub0_host[0] on the host: one vector takes it by value)
+void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, unsigned long long len,
+                   const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
                    unsigned long long binv_lo_stride, unsigned long long binv_hi_stride, const fe *sub0_dev, const fe *sub0_host);
 // batch > 1: a, add0, add1 of vector q at q * in_stride, out at q * out_stride; scratch holds batch * len elements
 void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, const fe *add1, fe *out, unsigned long long n, unsigned long long len, fe e,

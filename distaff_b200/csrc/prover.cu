@@ -149,9 +149,8 @@ public:
         DG_CUDA(cudaEventCreateWithFlags(&ready, cudaEventDisableTiming));
         DG_CUDA(cudaEventRecord(ready, c.stream));
         cudaPointerAttributes attr;
-        bool pinned = cudaPointerGetAttributes(&attr, host_cols[0]) == cudaSuccess && attr.type != cudaMemoryTypeUnregistered;
+        const bool pinned = cudaPointerGetAttributes(&attr, host_cols[0]) == cudaSuccess && attr.type != cudaMemoryTypeUnregistered;
         cudaGetLastError();
-        if (getenv("DG_NO_STAGING")) pinned = true;
         if (pinned) {
             DG_CUDA(cudaStreamWaitEvent(c.copy_stream, ready, 0));
             for (int i = 0; i < nchunks_; i++) {           // enqueue every upload first: the copy engine runs ahead of the compute stream
@@ -537,8 +536,8 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         DevBuf d_zeros((size_t)16 * K);
         DG_CUDA(cudaMemsetAsync(d_zeros.p, 0, d_zeros.bytes, c.stream));
         fe *ic = evals.as<fe>(), *fc = evals.as<fe>() + E, *tc = evals.as<fe>() + 2 * E;          // of proof 0; proof p at + 3 E p
-        syn_div_batch(c, K, ic, 3 * E, ic, 3 * E, scratch.as<fe>(), E, one_t.ref(), 0, 0, one_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - 1)
-        syn_div_batch(c, K, fc, 3 * E, fc, 3 * E, scratch.as<fe>(), E, xl_t.ref(), 0, 0, xli_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - x_last)
+        syn_div_batch(c, K, ic, 3 * E, ic, 3 * E, E, one_t.ref(), 0, 0, one_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - 1)
+        syn_div_batch(c, K, fc, 3 * E, fc, 3 * E, E, xl_t.ref(), 0, 0, xli_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - x_last)
         syn_div_expanded_sum(c, tc, scratch.as<fe>(), ic, fc, combined.as<fe>(), n, E, x_last, K, 3 * E, E);   // / ((x^n - 1)/(x - x_last)), summed
     }
     if (K == 1) debug_dump(c, "constraint_poly", combined.p, E * 16);
@@ -641,11 +640,11 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * w, *d_ks = d_subs + (size_t)3 * K;
         fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
         lincomb2(c, polys.as<fe>(), n, w, d_cc, d_cc + w, t1, t2, K, 2 * w, 2 * n);
-        syn_div_batch(c, K, t1, 2 * n, t1, 2 * n, scratch.as<fe>(), n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs, subs);
+        syn_div_batch(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs, subs);
         //                                                                                                   (T1(x) - T1(z)) / (x - z)
-        syn_div_batch(c, K, t2, 2 * n, t2, 2 * n, scratch.as<fe>(), n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K,
+        syn_div_batch(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K,
                       subs + K);                                                                           // (T2(x) - T2(zg)) / (x - zg)
-        syn_div_batch(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, scratch.as<fe>(), E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n,
+        syn_div_batch(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n,
                       zi_t.hi_n, d_subs + 2 * K, subs + 2 * K);                                            // (C(x) - C(z)) / (x - z)
     sub.mark("6.lincomb+syndiv");
         compose_batch(c, K, t1, t2, 2 * n, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, d_ks, ks);
