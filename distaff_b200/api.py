@@ -173,6 +173,39 @@ def verify(program_hash, public_inputs, outputs, proof):
     backend.check(rc)
 
 
+def verify_batch(items, stats=None):
+    """verify() of many proofs in one dg_verify_batch call, each verifier stage launched once per group of proofs.  items: iterable of
+    (program_hash, public_inputs, outputs, proof), proof a StarkProof or bytes; the proofs may differ in shape, length and options.
+    Returns a list in input order: None (accepted), the reference's error string (rejected), or a backend.DgError instance for bytes
+    that are not a serialized StarkProof -- returned, not raised, as prove_batch does.  Errors of the whole call raise.  A dict passed as
+    `stats` receives total_ms, kernel_launches and groups."""
+    items = list(items)
+    if not items:
+        return []
+    k = len(items)
+    hashes = [bytes(h) for h, _, _, _ in items]
+    data = [p.bytes if isinstance(p, StarkProof) else bytes(p) for _, _, _, p in items]
+    keep, (pin, nin, pout, nout) = _batch_io([i for _, i, _, _ in items], [o for _, _, o, _ in items])
+    status = (ctypes.c_int * k)()
+    st = backend.DgVerifyStats()
+    backend.check(backend.lib().dg_verify_batch(k, (backend.vp * k)(*[ctypes.cast(ctypes.c_char_p(h), backend.vp) for h in hashes]), pin, nin, pout,
+                                                nout, (backend.vp * k)(*[ctypes.cast(ctypes.c_char_p(d), backend.vp) for d in data]),
+                                                (ctypes.c_size_t * k)(*[len(d) for d in data]), status, ctypes.byref(st)))
+    del keep
+    out = []
+    msg = ctypes.create_string_buffer(512)
+    for i, rc in enumerate(status):
+        if rc == 0:
+            out.append(None)
+            continue
+        backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
+        text = msg.value.decode(errors="replace")
+        out.append(text if rc == -6 else backend.DgError(rc, text))
+    if stats is not None:
+        stats.update(total_ms=float(st.total_ms), kernel_launches=int(st.kernel_launches), groups=int(st.groups))
+    return out
+
+
 def execute(source, public_inputs=(), secret_a=(), secret_b=(), num_outputs=1, options=None):
     """distaff::execute (lib.rs:30-65): run the program on the host VM, then prove on the GPU. Returns (outputs, proof)."""
     trace = hostvm.execute(source, public_inputs, secret_a, secret_b, num_outputs)

@@ -35,6 +35,10 @@ class DgStats(ctypes.Structure):
     _fields_ = [("stage_ms", ctypes.c_float * 9), ("h2d_ms", ctypes.c_float), ("total_ms", ctypes.c_float), ("kernel_launches", u64)]
 
 
+class DgVerifyStats(ctypes.Structure):
+    _fields_ = [("total_ms", ctypes.c_float), ("kernel_launches", u64), ("groups", u32)]
+
+
 DRAW_FIELD_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -56,6 +60,8 @@ EXPORTS = {
                               ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
     "dg_verify": [vp, vp, u32, vp, u32, vp, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t],
+    "dg_verify_batch": [u32, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                        ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgVerifyStats)],
     "dg_proof_serialized_len": [vp, ctypes.POINTER(ctypes.c_size_t)],
     "dg_proof_serialize": [vp, vp, ctypes.c_size_t],
     "dg_proof_digest": [vp, ctypes.c_int, vp],

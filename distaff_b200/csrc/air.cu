@@ -576,7 +576,9 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     for (int g = 0; g < 6; g++) acc.adj[g] = ZERO;
     acc.cA = BATCH ? P.coefA + blockIdx.y * P.coef_stride : P.coefA; acc.cB = BATCH ? P.coefB + blockIdx.y * P.coef_stride : P.coefB; acc.nonzero = false;
 
-    const fe *per = P.per_override ? P.per_override : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
+    const fe *per = P.per_override ? (BATCH ? P.per_override + blockIdx.y * P.override_stride : P.per_override)
+                                   : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
+    const fe *const xpow_override = BATCH && P.xpow_override ? P.xpow_override + blockIdx.y * P.override_stride : P.xpow_override;
 
     DG_STEP();
     // ---- decoder: op bits (decoder/op_bits.rs:10-79), constraints 0..14 -------------------------------------------------------
@@ -906,7 +908,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g ------------------------------------------------------------------
     fe t_res = DG_REDUCE_WIDE(acc.res);
 #pragma unroll
-    for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], P.xpow_override ? P.xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
+    for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], xpow_override ? xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
     if (!P.verify_mode && c8 == 0 && k != n - 1) {
         if (acc.nonzero && live) atomicExch(BATCH ? P.violation + blockIdx.y : P.violation, (unsigned)(k + 1));
@@ -953,7 +955,10 @@ void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     for (int q = 0; q < batch; q++) {
         AirParams Q = P;
         Q.ext += q * P.ext_stride; Q.t_ev += q * P.t_ev_stride;
-        Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride; Q.violation += q;
+        Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride;
+        if (Q.violation) Q.violation += q;
+        if (Q.per_override) Q.per_override += q * P.override_stride;
+        if (Q.xpow_override) Q.xpow_override += q * P.override_stride;
         constraint_eval_kernel<128, 4><<<(unsigned)((E + 127) / 128), 128, 0, c.stream>>>(Q);
         c.launches++;
         DG_CUDA(cudaGetLastError());

@@ -25,6 +25,8 @@ struct AirParams {
     // batched proving: proof q of the batch reads ext + q * ext_stride and coefA / coefB + q * coef_stride, writes t_ev + q * t_ev_stride
     // and violation[q]
     unsigned long long ext_stride, t_ev_stride, coef_stride;
+    // batched verification: proof q reads per_override / xpow_override + q * override_stride
+    unsigned long long override_stride;
 };
 
 // evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P); the shared-memory kernel runs them in

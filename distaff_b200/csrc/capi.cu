@@ -15,11 +15,6 @@ void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned 
 }  // namespace dg
 
 namespace dg {
-std::string verify_proof(Context &c, const uint8_t program_hash[32], const std::vector<fe> &inputs, const std::vector<fe> &outputs,
-                         const uint8_t *proof_bytes, size_t proof_len);
-}
-
-namespace dg {
 bool host_plan_verify_batch(const std::vector<uint64_t> &indexes, int depth, size_t n_values, const std::vector<uint32_t> &node_counts,
                             std::vector<uint32_t> &ops, std::vector<uint32_t> &level_start, uint32_t &root_slot);
 }
@@ -27,7 +22,7 @@ bool host_plan_verify_batch(const std::vector<uint64_t> &indexes, int depth, siz
 using namespace dg;
 
 static thread_local std::string t_last_error;
-static thread_local std::vector<std::string> t_batch_messages;     // per trace of the calling thread's last batched call
+static thread_local std::vector<std::string> t_batch_messages;     // per trace / proof of the calling thread's last batched call
 
 template <typename F>
 static int guarded(F &&f) {
@@ -42,25 +37,6 @@ static int guarded(F &&f) {
         return DG_ERR_INVALID;
     }
 }
-
-struct EventTimer {
-    cudaEvent_t a = nullptr, b = nullptr;
-    cudaStream_t s;
-    float *out;
-    EventTimer(cudaStream_t stream, float *ms) : s(stream), out(ms) {
-        if (!out) return;
-        DG_CUDA(cudaEventCreate(&a));
-        DG_CUDA(cudaEventCreate(&b));
-        DG_CUDA(cudaEventRecord(a, s));
-    }
-    void stop() {
-        if (!out) return;
-        DG_CUDA(cudaEventRecord(b, s));
-        DG_CUDA(cudaEventSynchronize(b));
-        DG_CUDA(cudaEventElapsedTime(out, a, b));
-    }
-    ~EventTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
-};
 
 // ---- helper kernels ------------------------------------------------------------------------------------------------------
 __global__ void coset_to_logical_kernel(const fe *__restrict__ in, fe *__restrict__ out, int log_n, int log_blowup) {
@@ -418,7 +394,7 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
     return guarded([&] {
         DG_REQUIRE(message && cap, "null argument");
-        DG_REQUIRE(index < t_batch_messages.size(), "no such trace in this thread's last batched call");
+        DG_REQUIRE(index < t_batch_messages.size(), "no such trace or proof in this thread's last batched call");
         strncpy(message, t_batch_messages[index].c_str(), cap - 1);
         message[cap - 1] = 0;
     });
@@ -438,14 +414,33 @@ int dg_verify(const uint8_t program_hash[32], const uint8_t *inputs16, uint32_t 
         DG_REQUIRE((n_inputs == 0 || inputs16) && (n_outputs == 0 || outputs16), "null public inputs / outputs");
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        std::vector<fe> in(n_inputs), out(n_outputs);
-        if (n_inputs) memcpy(in.data(), inputs16, n_inputs * 16);
-        if (n_outputs) memcpy(out.data(), outputs16, n_outputs * 16);
-        const std::string verdict = dg::verify_proof(c, program_hash, in, out, proof_bytes, proof_len);
-        if (!verdict.empty()) {
-            if (message && message_cap) { strncpy(message, verdict.c_str(), message_cap - 1); message[message_cap - 1] = 0; }
-            throw Error(DG_ERR_REJECTED, verdict);
+        std::vector<int> status;
+        std::vector<std::string> messages;
+        verify_proofs(c, {VerifyRequest{program_hash, inputs16, n_inputs, outputs16, n_outputs, proof_bytes, proof_len}}, status, messages, nullptr);
+        if (status[0] == DG_OK) return;
+        if (status[0] == DG_ERR_REJECTED && message && message_cap) {
+            strncpy(message, messages[0].c_str(), message_cap - 1);
+            message[message_cap - 1] = 0;
         }
+        throw Error(status[0], messages[0]);
+    });
+}
+int dg_verify_batch(uint32_t count, const uint8_t *const *program_hashes, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *const *proof_bytes, const size_t *proof_lens,
+                    int *status, dg_verify_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one proof");
+        DG_REQUIRE(program_hashes && inputs16 && n_inputs && outputs16 && n_outputs && proof_bytes && proof_lens && status, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        std::vector<VerifyRequest> req(count);
+        for (uint32_t i = 0; i < count; i++)
+            req[i] = VerifyRequest{program_hashes[i], inputs16[i], n_inputs[i], outputs16[i], n_outputs[i], proof_bytes[i], proof_lens[i]};
+        std::vector<int> st;
+        std::vector<std::string> messages;
+        verify_proofs(c, req, st, messages, stats);
+        std::copy(st.begin(), st.end(), status);
+        t_batch_messages = std::move(messages);
     });
 }
 int dg_proof_serialized_len(const dg_proof_t *proof, size_t *len) {

@@ -168,6 +168,26 @@ fe host_inv(fe a);
 
 static const int MAX_LOG_L = 10;                 // largest in-shared-memory transform: 1024 points
 
+// device time between construction and stop() on a stream, in ms; does nothing when ms is null
+struct EventTimer {
+    cudaEvent_t a = nullptr, b = nullptr;
+    cudaStream_t s;
+    float *out;
+    EventTimer(cudaStream_t stream, float *ms) : s(stream), out(ms) {
+        if (!out) return;
+        DG_CUDA(cudaEventCreate(&a));
+        DG_CUDA(cudaEventCreate(&b));
+        DG_CUDA(cudaEventRecord(a, s));
+    }
+    void stop() {
+        if (!out) return;
+        DG_CUDA(cudaEventRecord(b, s));
+        DG_CUDA(cudaEventSynchronize(b));
+        DG_CUDA(cudaEventElapsedTime(out, a, b));
+    }
+    ~EventTimer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+};
+
 // ---- NTT engine (ntt.cu) ------------------------------------------------------------------------------------------
 // natural-order DFT over the subgroup of order n = 2^log_n for `batch` vectors laid out with `stride` elements apart;
 // dst may equal src.  inverse: multiplies by n^-1 (polynom::interpolate_fft semantics).

@@ -26,4 +26,17 @@ void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t w
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                         const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
 
+// GPU verification (verifier.cu).  One proof of dg_verify / dg_verify_batch, with its program hash and public inputs / outputs.
+struct VerifyRequest {
+    const uint8_t *program_hash;
+    const uint8_t *inputs16; uint32_t n_inputs;
+    const uint8_t *outputs16; uint32_t n_outputs;
+    const uint8_t *proof; size_t proof_len;
+};
+// Verifies every proof, each stage launched once per group of proofs.  status[i] is what dg_verify returns for proof i alone: DG_OK,
+// DG_ERR_REJECTED with the reference's error string in messages[i], or the per-proof error (DG_ERR_INVALID, ...) with its message.
+// Throws for errors of the whole call (CUDA failures); then status and messages are left as they were.
+void verify_proofs(Context &c, const std::vector<VerifyRequest> &req, std::vector<int> &status, std::vector<std::string> &messages,
+                   dg_verify_stats_t *stats);
+
 }  // namespace dg

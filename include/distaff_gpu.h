@@ -80,8 +80,9 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
  * failed), otherwise the error of the whole call (DG_ERR_INVALID for count == 0, mixed shapes, bad options or a context that spans
  * several GPUs; DG_ERR_CUDA; DG_ERR_NO_DEVICE); on such an error every proofs_out[i] is NULL (nothing to free).  The library splits the
  * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
- * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) why trace i of the calling
- * thread's last batched call failed -- the message dg_prove gives for that trace -- or "" if it was proven. */
+ * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) the message of entry i of the
+ * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device or dg_verify_batch: why trace i failed (the message dg_prove
+ * gives for that trace) or why proof i was not accepted (what dg_verify reports for that proof), and "" if it was proven / accepted. */
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                    int *status, dg_prove_stats_t *stats);
@@ -126,6 +127,25 @@ void dg_proof_free(dg_proof_t *proof);
  * and the FRI row folds run on the device (verifier.cu); the Fiat-Shamir draws use the same generator / callbacks as dg_prove. */
 int dg_verify(const uint8_t program_hash[32], const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
               const uint8_t *proof_bytes, size_t proof_len, char *message, size_t message_cap);
+
+/* Batched verification: `count` proofs checked in one call, each verifier stage launched once for a group of proofs.  The proofs may
+ * differ in anything: register shape, trace length, extension factor, query count, grinding factor.  Entry i is proof_bytes[i]
+ * (proof_lens[i] bytes) against program_hashes[i] (32 bytes) and inputs16[i] / outputs16[i] (n_inputs[i] / n_outputs[i] elements; a
+ * pointer may be NULL when its count is 0).  status[i] is exactly what dg_verify returns for that proof alone: DG_OK, DG_ERR_REJECTED
+ * (the reference's Err string) or DG_ERR_INVALID (bytes that do not deserialize, a bad argument of that entry); dg_batch_message(i, ...)
+ * gives its message, "" for an accepted proof.  A rejected or malformed proof changes no other proof's verdict.  The Fiat-Shamir draws
+ * run on the calling thread, proof by proof in input order, so registered RNG callbacks see the concatenation of the calls dg_verify
+ * makes for each proof.  Returns DG_OK when the batch ran, otherwise the error of the whole call with every status[i] unset:
+ * DG_ERR_INVALID (count == 0, a NULL array), DG_ERR_CUDA, DG_ERR_NO_DEVICE.  Groups are bounded by a device-memory budget and by
+ * $DG_BATCH_GROUP; stats (may be NULL) covers the whole call. */
+typedef struct {
+    float total_ms;                /* device time of the groups (upload to download) */
+    uint64_t kernel_launches;
+    uint32_t groups;               /* groups that ran on the device (proofs decided on the host take part in none) */
+} dg_verify_stats_t;
+int dg_verify_batch(uint32_t count, const uint8_t *const *program_hashes, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *const *proof_bytes, const size_t *proof_lens,
+                    int *status, dg_verify_stats_t *stats);
 
 /* ---- building blocks (micro-benchmarks of BASELINE.json config 5; same kernels the prover uses) ---------------------- */
 /* math::fft / polynom::{eval_fft, interpolate_fft} (polynom.rs:23-28,82-86): natural-order DFT of `batch` vectors of 2^log_n
