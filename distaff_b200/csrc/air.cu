@@ -15,7 +15,9 @@
 //
 // Layout: the extended trace is coset-major ([column][c][k], LDE index = k*blowup + c).  Evaluation-domain step
 // s = 8k + c8 uses LDE index s*(blowup/8) => coset c = c8*(blowup/8), element k; the "next" row (LDE index + blowup) is
-// element k+1 of the same coset, so both rows are unit-stride reads across a warp.
+// element k+1 of the same coset, so both rows are unit-stride reads across a warp.  One kernel, constraint_eval_smem_kernel, serves every
+// trace length (n >= 16), the prover and the verifier: it stages a block's rows in shared memory, where each step's "next" row is the
+// slot after its own.
 // The kernel is tens of thousands of straight-line instructions.  With every field multiplication inlined it is many times the
 // size of the instruction cache and the warps starve on instruction fetch, so it calls one shared out-of-line multiply body.
 #define DG_MUL_CALL 1
@@ -82,423 +84,24 @@ struct Acc {
     }
 };
 
-template <int BLOCK, int MIN_BLOCKS>
-__global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_kernel(const AirParams P) {
-    const unsigned long long n = 1ULL << P.log_n;
-    const unsigned long long total = n * (unsigned long long)P.num_c8;
-    unsigned long long gid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool live = gid < total;            // no early exit: every thread takes part in the barriers
-    if (!live) gid = total - 1;
-    const unsigned long long c8_local = gid >> P.log_n, k = gid & (n - 1);
-    const unsigned long long c8 = c8_local + P.c8_base;
-    const unsigned long long s = (k << 3) + c8;                       // evaluation-domain step
-    const int stride = 1 << (P.log_blowup - 3);
-    const unsigned long long N = P.col_stride;                         // column stride of the local slab
-    const unsigned long long lde_index = s * (unsigned long long)stride;   // = k*blowup + c8*stride
-    const fe *cur_p = P.ext + (c8_local * stride) * n + k;            // the slab starts at coset c8_base*stride
-    const fe *nxt_p = P.ext + (c8_local * stride) * n + ((k + 1) & (n - 1));
-    const unsigned long long out_idx = (c8_local << P.log_n) + k;
-
-    const int cl = P.cl, ll = P.ll, sl = P.sl;
-    const int ctx_off = 15, loop_off = 15 + P.ctx_depth, stk_off = 15 + P.ctx_depth + P.loop_depth;
-
-    // ---- the two rows.  Boundary constraints are not evaluated here: their numerators are assembled in coefficient form from the
-    //      trace polynomials (poly.cu: boundary_coeffs), which is 8x less work than evaluating them on this domain.
-    fe cur_dec[15], nxt_dec[15];
-    fe c_ctx[16], n_ctx[16], c_loop[8], n_loop[8], o[32], nw[32];
-    {
-        for (int j = 0; j < 15; j++) cur_dec[j] = cur_p[(unsigned long long)j * N];
-        for (int j = 0; j < P.ctx_depth; j++) c_ctx[j] = cur_p[(unsigned long long)(ctx_off + j) * N];
-        for (int j = 0; j < P.loop_depth; j++) c_loop[j] = cur_p[(unsigned long long)(loop_off + j) * N];
-        for (int j = 0; j < P.stack_depth; j++) o[j] = cur_p[(unsigned long long)(stk_off + j) * N];
-        for (int j = P.ctx_depth; j < cl; j++) c_ctx[j] = ZERO;
-        for (int j = P.loop_depth; j < ll; j++) c_loop[j] = ZERO;
-        for (int j = P.stack_depth; j < sl; j++) o[j] = ZERO;
-        for (int j = 0; j < 15; j++) nxt_dec[j] = nxt_p[(unsigned long long)j * N];
-        for (int j = 0; j < P.ctx_depth; j++) n_ctx[j] = nxt_p[(unsigned long long)(ctx_off + j) * N];
-        for (int j = P.ctx_depth; j < cl; j++) n_ctx[j] = ZERO;
-        for (int j = 0; j < P.loop_depth; j++) n_loop[j] = nxt_p[(unsigned long long)(loop_off + j) * N];
-        for (int j = P.loop_depth; j < ll; j++) n_loop[j] = ZERO;
-        for (int j = 0; j < P.stack_depth; j++) nw[j] = nxt_p[(unsigned long long)(stk_off + j) * N];
-        for (int j = P.stack_depth; j < sl; j++) nw[j] = ZERO;
-    }
-
-    DG_STEP();
-    // ---- op flags (trace_state.rs:281-350) ----------------------------------------------------------------------------------
-    const fe op_counter = cur_dec[0];
-    const fe *sp = cur_dec + 1, *cf = cur_dec + 5, *ld = cur_dec + 8, *hd = cur_dec + 13;
-    const fe *nsp = nxt_dec + 1, *ncf = nxt_dec + 5;
-    fe cff[8], ldf[32], hdf[4];
-    {
-        // products of bits and negated bits; f*(1 - x) is computed as f - f*x (one multiplication per pair of flags)
-        fe a3 = fe_mul(cf[0], cf[1]);
-        fe a1 = fe_sub(cf[0], a3), a2 = fe_sub(cf[1], a3), a0 = fe_sub(bnot(cf[0]), a2);
-        cff[4] = fe_mul(a0, cf[2]); cff[5] = fe_mul(a1, cf[2]); cff[6] = fe_mul(a2, cf[2]); cff[7] = fe_mul(a3, cf[2]);
-        cff[0] = fe_sub(a0, cff[4]); cff[1] = fe_sub(a1, cff[5]); cff[2] = fe_sub(a2, cff[6]); cff[3] = fe_sub(a3, cff[7]);
-    }
-    fe hdf_raw0;
-    {
-        hdf[3] = fe_mul(hd[0], hd[1]);
-        hdf[1] = fe_sub(hd[0], hdf[3]); hdf[2] = fe_sub(hd[1], hdf[3]); hdf[0] = fe_sub(bnot(hd[0]), hdf[2]);
-        hdf_raw0 = hdf[0];
-        hdf[0] = fe_mul(hdf[0], ld[0]);      // PUSH flag adjustment
-    }
-    fe next_void;
-    {
-        fe a3 = fe_mul(ncf[0], ncf[1]);
-        next_void = fe_mul(a3, ncf[2]);
-    }
-
-    Acc acc;
-    acc.first = true;
-#pragma unroll
-    for (int g = 0; g < 6; g++) acc.adj[g] = ZERO;
-    acc.cA = P.coefA; acc.cB = P.coefB; acc.nonzero = false;
-
-    const fe *per = P.per_override ? P.per_override : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
-
-    DG_STEP();
-    // ---- decoder: op bits (decoder/op_bits.rs:10-79), constraints 0..14 -------------------------------------------------------
-    {
-        fe cf_sum = ZERO, ld_prod = ONE, hd_prod = ONE;
-#pragma unroll
-        for (int i = 0; i < 3; i++) { acc.fold(i, G2, is_bin(cf[i])); cf_sum = fe_add(cf_sum, cf[i]); }
-#pragma unroll
-        for (int i = 0; i < 5; i++) { acc.fold(3 + i, G2, is_bin(ld[i])); ld_prod = fe_mul(ld_prod, ld[i]); }
-#pragma unroll
-        for (int i = 0; i < 2; i++) { acc.fold(8 + i, G2, is_bin(hd[i])); hd_prod = fe_mul(hd_prod, hd[i]); }
-        fe is_hacc = cff[0];
-        fe hacc_t = fe_mul(fe_add(op_counter, ONE), is_hacc);
-        fe rest_t = fe_mul(op_counter, bnot(is_hacc));
-        acc.fold(10, G3, fe_sub(fe_add(hacc_t, rest_t), nxt_dec[0]));
-        acc.fold(11, G8, fe_mul(op_counter, fe_mul(bnot(ld_prod), bnot(hd_prod))));
-        acc.fold(12, G8, fe_mul(cf_sum, bnot(fe_mul(ld_prod, hd_prod))));
-        acc.fold(13, G6, fe_mul(cff[7], bnot(next_void)));
-        fe prefix = fe_add(fe_add(cff[1], cff[4]), fe_add(cff[5], cff[6]));      // BEGIN, LOOP, WRAP, BREAK
-        fe align = fe_mul(prefix, per[8 + 1]);
-        align = fe_add(align, fe_mul(fe_add(cff[2], cff[3]), per[8 + 0]));       // TEND, FEND
-        align = fe_add(align, fe_mul(hdf[0], per[8 + 2]));                        // PUSH
-        acc.fold(14, G4, align);
-    }
-
-    DG_STEP();
-    // ---- decoder: sponge / flow ops (decoder/sponge.rs, flow_ops.rs) --------------------------------------------------------------
-    {
-        fe r_sp[4], r_img;
-        // HACC
-        {
-            fe f = cff[0];
-            fe op_value = fe_mul(nw[0], hdf[0]);
-            fe os[4], ns[4];
-#pragma unroll
-            for (int i = 0; i < 4; i++) os[i] = fe_cube(fe_add(sp[i], per[i]));
-            DG_STEP();
-            matvec<4>(c_sponge_mds, os);
-            // op_code = sum ld[i]*2^i + hd[i]*2^(5+i)
-            fe opc = ld[0];
-            opc = fe_add(opc, fe_mul_small(ld[1], 2)); opc = fe_add(opc, fe_mul_small(ld[2], 4));
-            opc = fe_add(opc, fe_mul_small(ld[3], 8)); opc = fe_add(opc, fe_mul_small(ld[4], 16));
-            opc = fe_add(opc, fe_mul_small(hd[0], 32)); opc = fe_add(opc, fe_mul_small(hd[1], 64));
-            os[0] = fe_add(os[0], opc);
-            os[1] = fe_add(os[1], op_value);
-#pragma unroll
-            for (int i = 0; i < 4; i++) ns[i] = nsp[i];
-            matvec<4>(c_sponge_inv_mds, ns);
-#pragma unroll
-            for (int i = 0; i < 4; i++) ns[i] = fe_sub(fe_cube(ns[i]), per[4 + i]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_mul(f, fe_sub(os[i], ns[i]));
-        }
-        DG_STEP();
-        // BEGIN, LOOP, WRAP clear the sponge: flag sum * new_sponge[i]
-        {
-            fe fclr = fe_add(fe_add(cff[1], cff[4]), cff[5]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_add(r_sp[i], fe_mul(fclr, nsp[i]));
-        }
-        DG_STEP();
-        // TEND / FEND
-        {
-            fe ft = cff[2], ff = cff[3], fb = fe_add(ft, ff);
-            r_sp[0] = fe_add(r_sp[0], fe_mul(fb, fe_sub(c_ctx[0], nsp[0])));
-            r_sp[1] = fe_add(r_sp[1], fe_mul(ft, fe_sub(sp[0], nsp[1])));
-            r_sp[2] = fe_add(r_sp[2], fe_mul(ff, fe_sub(sp[0], nsp[2])));
-            r_sp[3] = fe_add(r_sp[3], fe_mul(fb, nsp[3]));
-        }
-        // BREAK / VOID keep the sponge
-        {
-            fe fk = fe_add(cff[6], cff[7]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_add(r_sp[i], fe_mul(fk, fe_sub(sp[i], nsp[i])));
-        }
-        acc.fold(15, G6, r_sp[0]); acc.fold(16, G7, r_sp[1]); acc.fold(17, G6, r_sp[2]); acc.fold(18, G6, r_sp[3]);
-        // loop image (WRAP, BREAK)
-        r_img = fe_mul(fe_add(cff[5], cff[6]), fe_sub(sp[0], c_loop[0]));
-        acc.fold(19, G4, r_img);
-
-        DG_STEP();
-        // context stack: BEGIN/LOOP push (right shift 1, slot 0 = parent hash), TEND/FEND pop (left shift 1), WRAP/BREAK/VOID copy
-        {
-            fe f_push = fe_add(cff[1], cff[4]), f_pop = fe_add(cff[2], cff[3]), f_copy = fe_add(fe_add(cff[5], cff[6]), cff[7]);
-            for (int i = 0; i < cl; i++) {
-                fe v = fe_mul(f_copy, fe_sub(c_ctx[i], n_ctx[i]));
-                if (i == 0) v = fe_add(v, fe_mul(f_push, fe_sub(sp[0], n_ctx[0])));
-                else v = fe_add(v, fe_mul(f_push, fe_sub(c_ctx[i - 1], n_ctx[i])));
-                if (i < cl - 1) v = fe_add(v, fe_mul(f_pop, fe_sub(c_ctx[i + 1], n_ctx[i])));
-                else v = fe_add(v, fe_mul(f_pop, n_ctx[i]));
-                acc.fold(20 + i, G4, v);
-            }
-        }
-        DG_STEP();
-        // loop stack: BEGIN/TEND/FEND/WRAP/VOID copy, LOOP right shift 1 (slot 0 unconstrained), BREAK left shift 1
-        {
-            fe f_copy = fe_add(fe_add(fe_add(cff[1], cff[2]), fe_add(cff[3], cff[5])), cff[7]);
-            fe f_rs = cff[4], f_ls = cff[6];
-            for (int i = 0; i < ll; i++) {
-                fe v = fe_mul(f_copy, fe_sub(c_loop[i], n_loop[i]));
-                if (i >= 1) v = fe_add(v, fe_mul(f_rs, fe_sub(c_loop[i - 1], n_loop[i])));
-                if (i < ll - 1) v = fe_add(v, fe_mul(f_ls, fe_sub(c_loop[i + 1], n_loop[i])));
-                else v = fe_add(v, fe_mul(f_ls, n_loop[i]));
-                acc.fold(20 + cl + i, G4, v);
-            }
-        }
-    }
-
-    {
-        fe n0 = bnot(ld[0]);
-        ldf[3] = fe_mul(ld[0], ld[1]);
-        ldf[1] = fe_sub(ld[0], ldf[3]);                               // ld0 (1 - ld1)
-        ldf[0] = fe_sub(n0, fe_sub(ld[1], ldf[3]));                   // (1 - ld0)(1 - ld1)
-        ldf[2] = fe_mul(n0, cf[1]);                                   // sic (trace_state.rs:301)
-#pragma unroll
-        for (int i = 0; i < 4; i++) { ldf[4 + i] = fe_mul(ldf[i], ld[2]); ldf[i] = fe_sub(ldf[i], ldf[4 + i]); }
-#pragma unroll
-        for (int i = 0; i < 8; i++) { ldf[8 + i] = fe_mul(ldf[i], ld[3]); ldf[i] = fe_sub(ldf[i], ldf[8 + i]); }
-        DG_STEP();
-#pragma unroll
-        for (int i = 0; i < 16; i++) { ldf[16 + i] = fe_mul(ldf[i], ld[4]); ldf[i] = fe_sub(ldf[i], ldf[16 + i]); }
-        DG_STEP();
-    }
-    DG_STEP();
-    fe begin_flag, noop_flag;
-    {
-        begin_flag = fe_mul(ldf[0], hdf_raw0);
-        noop_flag = fe_mul(ldf[31], hdf[3]);
-        ldf[0] = fe_mul(ldf[0], hd[0]);      // ASSERT flag adjustment
-    }
-    DG_STEP();
-    // ---- stack constraints (stack/mod.rs:117-195) -----------------------------------------------------------------------------------
-    {
-        const int base = 20 + cl + ll;       // aux constraints at base, base+1; stack slots from base+2
-        const int L = sl;
-        // op flags by name (processor/opcodes.rs:46-92: ld index = opcode & 31)
-        const fe f_assert = ldf[0], f_asserteq = ldf[1], f_eq = ldf[2], f_drop = ldf[3], f_drop4 = ldf[4], f_choose = ldf[5],
-                 f_choose2 = ldf[6], f_cswap2 = ldf[7], f_add = ldf[8], f_mul = ldf[9], f_and = ldf[10], f_or = ldf[11], f_inv = ldf[12],
-                 f_neg = ldf[13], f_not = ldf[14], f_read = ldf[16], f_read2 = ldf[17], f_dup = ldf[18], f_dup2 = ldf[19],
-                 f_dup4 = ldf[20], f_pad2 = ldf[21], f_swap = ldf[24], f_swap2 = ldf[25], f_swap4 = ldf[26], f_roll4 = ldf[27],
-                 f_roll8 = ldf[28], f_binacc = ldf[29];
-        const fe f_push = hdf[0], f_cmp = hdf[1], f_rescr = hdf[2];
-
-        DG_STEP();
-        // --- auxiliary constraints
-        fe aux0, aux1;
-        {
-            aux0 = fe_mul(f_assert, fe_sub(ONE, o[0]));
-            aux0 = fe_add(aux0, fe_mul(f_asserteq, fe_sub(o[0], o[1])));
-            fe b0 = is_bin(o[0]), b1 = is_bin(o[1]);
-            fe f_ao = fe_add(f_and, f_or);
-            aux0 = fe_add(aux0, fe_mul(fe_add(f_not, f_ao), b0));
-            aux1 = fe_mul(f_ao, b1);
-            fe diff = fe_sub(o[1], o[2]);
-            aux0 = fe_add(aux0, fe_mul(f_eq, fe_mul(nw[0], diff)));
-            aux0 = fe_add(aux0, fe_mul(f_choose, is_bin(o[2])));
-            aux0 = fe_add(aux0, fe_mul(fe_add(f_choose2, f_cswap2), is_bin(o[4])));
-        }
-        acc.fold(base, G7, aux0);
-        acc.fold(base + 1, G7, aux1);
-
-        DG_STEP();
-        // --- per-slot shift structure.  For slot i the generic contribution of an operation is
-        //        copy:         f * (o[i]   - n[i])                    when i >= from
-        //        right shift s: f * (o[i-s] - n[i])                   when i >= s
-        //        left shift s from slot `from`: f * (o[i+s] - n[i])   when from-s <= i < L-s, and f * n[i] when i >= L-s
-        //     flags with the same shape are summed first.
-        fe ev[32];
-        const fe f_copy0 = fe_add(begin_flag, noop_flag);                                   // from 0
-        const fe f_copy1 = fe_add(fe_add(f_inv, f_neg), f_not);                              // from 1
-        const fe f_copy2 = f_swap;                                                           // from 2
-        const fe f_copy4 = fe_add(fe_add(f_swap2, f_roll4), f_binacc);                       // from 4
-        const fe f_copy6 = f_rescr;                                                          // from 6
-        const fe f_copy8 = fe_add(fe_add(f_swap4, f_roll8), f_cmp);                          // from 8
-        const fe f_rs1 = fe_add(fe_add(f_read, f_dup), f_push);
-        const fe f_rs2 = fe_add(fe_add(f_read2, f_dup2), f_pad2);
-        const fe f_rs4 = f_dup4;
-        const fe f_ls1_0 = fe_add(f_assert, f_drop);                                         // left 1, start slot 0
-        const fe f_ls1_1 = fe_add(fe_add(f_add, f_mul), fe_add(f_and, f_or));                // left 1, start slot 1
-        const fe f_ls2_0 = f_asserteq;                                                       // left 2, start slot 0
-        const fe f_ls2_1 = fe_add(f_eq, f_choose);                                           // left 2, start slot 1
-        const fe f_ls2_4 = f_cswap2;                                                         // left 2, start slot 4
-        const fe f_ls4_0 = f_drop4;                                                          // left 4, start slot 0
-        const fe f_ls4_2 = f_choose2;                                                        // left 4, start slot 2
-        for (int i = 0; i < L; i++) {
-            fe fc = f_copy0;
-            if (i >= 1) fc = fe_add(fc, f_copy1);
-            if (i >= 2) fc = fe_add(fc, f_copy2);
-            if (i >= 4) fc = fe_add(fc, f_copy4);
-            if (i >= 6) fc = fe_add(fc, f_copy6);
-            if (i >= 8) fc = fe_add(fc, f_copy8);
-            fe v = fe_mul(fc, fe_sub(o[i], nw[i]));
-            if (i >= 1) v = fe_add(v, fe_mul(f_rs1, fe_sub(o[i - 1], nw[i])));
-            if (i >= 2) v = fe_add(v, fe_mul(f_rs2, fe_sub(o[i - 2], nw[i])));
-            if (i >= 4) v = fe_add(v, fe_mul(f_rs4, fe_sub(o[i - 4], nw[i])));
-            {
-                fe fl = f_ls1_0;
-                if (i >= 1) fl = fe_add(fl, f_ls1_1);
-                v = fe_add(v, fe_mul(fl, (i < L - 1) ? fe_sub(o[i + 1], nw[i]) : nw[i]));
-            }
-            {
-                fe fl = f_ls2_0;
-                if (i >= 1) fl = fe_add(fl, f_ls2_1);
-                if (i >= 4) fl = fe_add(fl, f_ls2_4);
-                v = fe_add(v, fe_mul(fl, (i < L - 2) ? fe_sub(o[i + 2], nw[i]) : nw[i]));
-            }
-            {
-                fe fl = f_ls4_0;
-                if (i >= 2) fl = fe_add(fl, f_ls4_2);
-                v = fe_add(v, fe_mul(fl, (i < L - 4) ? fe_sub(o[i + 4], nw[i]) : nw[i]));
-            }
-            ev[i] = v;
-        }
-        DG_STEP();
-        // --- operation-specific constraints on the low slots
-        // dup / dup2 / dup4: new[k] == old[k]
-        ev[0] = fe_add(ev[0], fe_mul(fe_add(fe_add(f_dup, f_dup2), f_dup4), fe_sub(nw[0], o[0])));
-        ev[1] = fe_add(ev[1], fe_mul(fe_add(f_dup2, f_dup4), fe_sub(nw[1], o[1])));
-        ev[2] = fe_add(ev[2], fe_mul(f_dup4, fe_sub(nw[2], o[2])));
-        ev[3] = fe_add(ev[3], fe_mul(f_dup4, fe_sub(nw[3], o[3])));
-        // pad2
-        ev[0] = fe_add(ev[0], fe_mul(f_pad2, nw[0]));
-        ev[1] = fe_add(ev[1], fe_mul(f_pad2, nw[1]));
-        // swap: both constraints accumulate into slot 0 (stack/manipulation.rs:63-64)
-        ev[0] = fe_add(ev[0], fe_mul(f_swap, fe_add(fe_sub(nw[0], o[1]), fe_sub(nw[1], o[0]))));
-        DG_STEP();
-        // swap2
-        ev[0] = fe_add(ev[0], fe_mul(f_swap2, fe_sub(nw[0], o[2]))); ev[1] = fe_add(ev[1], fe_mul(f_swap2, fe_sub(nw[1], o[3])));
-        ev[2] = fe_add(ev[2], fe_mul(f_swap2, fe_sub(nw[2], o[0]))); ev[3] = fe_add(ev[3], fe_mul(f_swap2, fe_sub(nw[3], o[1])));
-        // swap4
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            ev[q] = fe_add(ev[q], fe_mul(f_swap4, fe_sub(nw[q], o[4 + q])));
-            ev[4 + q] = fe_add(ev[4 + q], fe_mul(f_swap4, fe_sub(nw[4 + q], o[q])));
-        }
-        DG_STEP();
-        // roll4 / roll8
-        ev[0] = fe_add(ev[0], fe_mul(f_roll4, fe_sub(nw[0], o[3])));
-#pragma unroll
-        for (int q = 1; q < 4; q++) ev[q] = fe_add(ev[q], fe_mul(f_roll4, fe_sub(nw[q], o[q - 1])));
-        ev[0] = fe_add(ev[0], fe_mul(f_roll8, fe_sub(nw[0], o[7])));
-#pragma unroll
-        for (int q = 1; q < 8; q++) ev[q] = fe_add(ev[q], fe_mul(f_roll8, fe_sub(nw[q], o[q - 1])));
-        DG_STEP();
-        // arithmetic / boolean: slot 0
-        {
-            fe prod = fe_mul(o[0], o[1]);
-            fe v = fe_mul(f_add, fe_sub(nw[0], fe_add(o[0], o[1])));
-            v = fe_add(v, fe_mul(fe_add(f_mul, f_and), fe_sub(nw[0], prod)));
-            v = fe_add(v, fe_mul(f_inv, fe_sub(ONE, fe_mul(nw[0], o[0]))));
-            v = fe_add(v, fe_mul(f_neg, fe_add(nw[0], o[0])));
-            v = fe_add(v, fe_mul(f_not, fe_sub(nw[0], bnot(o[0]))));
-            v = fe_add(v, fe_mul(f_or, fe_sub(nw[0], bnot(fe_mul(bnot(o[0]), bnot(o[1]))))));
-            // eq: new[0] == 1 - (o[1]-o[2]) * o[0]
-            v = fe_add(v, fe_mul(f_eq, fe_sub(nw[0], bnot(fe_mul(fe_sub(o[1], o[2]), o[0])))));
-            // choose
-            {
-                fe c = o[2];
-                v = fe_add(v, fe_mul(f_choose, fe_sub(nw[0], fe_add(fe_mul(c, o[0]), fe_mul(bnot(c), o[1])))));
-            }
-            ev[0] = fe_add(ev[0], v);
-        }
-        DG_STEP();
-        // choose2 / cswap2
-        {
-            fe c = o[4], nc = bnot(c);
-            ev[0] = fe_add(ev[0], fe_mul(f_choose2, fe_sub(nw[0], fe_add(fe_mul(c, o[0]), fe_mul(nc, o[2])))));
-            ev[1] = fe_add(ev[1], fe_mul(f_choose2, fe_sub(nw[1], fe_add(fe_mul(c, o[1]), fe_mul(nc, o[3])))));
-            ev[0] = fe_add(ev[0], fe_mul(f_cswap2, fe_sub(nw[0], fe_add(fe_mul(c, o[2]), fe_mul(nc, o[0])))));
-            ev[1] = fe_add(ev[1], fe_mul(f_cswap2, fe_sub(nw[1], fe_add(fe_mul(c, o[3]), fe_mul(nc, o[1])))));
-            ev[2] = fe_add(ev[2], fe_mul(f_cswap2, fe_sub(nw[2], fe_add(fe_mul(c, o[0]), fe_mul(nc, o[2])))));
-            ev[3] = fe_add(ev[3], fe_mul(f_cswap2, fe_sub(nw[3], fe_add(fe_mul(c, o[1]), fe_mul(nc, o[3])))));
-        }
-        DG_STEP();
-        // binacc (comparison.rs:111-133)
-        {
-            fe bit = nw[0];
-            ev[0] = fe_add(ev[0], fe_mul(f_binacc, is_bin(bit)));
-            ev[1] = fe_add(ev[1], fe_mul(f_binacc, nw[1]));
-            ev[2] = fe_add(ev[2], fe_mul(f_binacc, fe_sub(nw[2], fe_mul_small(o[2], 2))));
-            ev[3] = fe_add(ev[3], fe_mul(f_binacc, fe_sub(nw[3], fe_add(o[3], fe_mul(bit, o[2])))));
-        }
-        DG_STEP();
-        // cmp (comparison.rs:71-108): [pow, bit_a, bit_b, not_set, gt, lt, acc_b, acc_a]
-        {
-            fe xb = nw[1], yb = nw[2], not_set = nw[3];
-            fe bit_gt = fe_mul(xb, bnot(yb)), bit_lt = fe_mul(yb, bnot(xb));
-            fe gt = fe_add(o[4], fe_mul(bit_gt, not_set)), lt = fe_add(o[5], fe_mul(bit_lt, not_set));
-            fe p2 = o[0];
-            fe x_acc = fe_add(o[7], fe_mul(xb, p2)), y_acc = fe_add(o[6], fe_mul(yb, p2));
-            fe nsc = fe_mul(bnot(o[5]), bnot(o[4]));
-            ev[0] = fe_add(ev[0], fe_mul(f_cmp, is_bin(xb)));
-            ev[1] = fe_add(ev[1], fe_mul(f_cmp, is_bin(yb)));
-            ev[2] = fe_add(ev[2], fe_mul(f_cmp, fe_sub(nw[4], gt)));
-            ev[3] = fe_add(ev[3], fe_mul(f_cmp, fe_sub(nw[5], lt)));
-            ev[4] = fe_add(ev[4], fe_mul(f_cmp, fe_sub(nw[6], y_acc)));
-            ev[5] = fe_add(ev[5], fe_mul(f_cmp, fe_sub(nw[7], x_acc)));
-            ev[6] = fe_add(ev[6], fe_mul(f_cmp, fe_sub(not_set, nsc)));
-            ev[7] = fe_add(ev[7], fe_mul(f_cmp, fe_sub(fe_mul_small(nw[0], 2), p2)));
-        }
-        DG_STEP();
-        // rescr (stack/hash.rs:9-35)
-        {
-            fe os[6], ns[6];
-#pragma unroll
-            for (int q = 0; q < 6; q++) os[q] = fe_cube(fe_add(o[q], per[11 + q]));
-            matvec<6>(c_hasher_mds, os);
-#pragma unroll
-            for (int q = 0; q < 6; q++) ns[q] = nw[q];
-            matvec<6>(c_hasher_inv_mds, ns);
-#pragma unroll
-            for (int q = 0; q < 6; q++) ns[q] = fe_sub(fe_cube(ns[q]), per[11 + 6 + q]);
-#pragma unroll
-            for (int q = 0; q < 6; q++) ev[q] = fe_add(ev[q], fe_mul(f_rescr, fe_sub(ns[q], os[q])));
-        }
-        for (int i = 0; i < P.stack_depth; i++) acc.fold(base + 2 + i, G7, ev[i]);
-    }
-
-    DG_STEP();
-    // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g ------------------------------------------------------------------
-    fe t_res = DG_REDUCE_WIDE(acc.res);
-#pragma unroll
-    for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], P.xpow_override ? P.xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
-    // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
-    if (!P.verify_mode && c8 == 0 && k != n - 1) {
-        if (acc.nonzero && live) atomicExch(P.violation, (unsigned)(k + 1));
-        t_res = ZERO;
-    }
-    if (live) P.t_ev[out_idx] = t_res;
-}
-
-// Shared-memory kernel (n >= BLOCK): the rows of a block's BLOCK consecutive steps of one coset are staged once in shared memory,
-// column-major with pitch BLOCK + 1 -- slot t holds the row of thread t, slot t + 1 is its "next" row (the row of thread t + 1, or the
-// extra row BLOCK for the last thread).  Context / loop / user-stack registers are then addressed dynamically in shared memory instead
-// of in per-thread arrays, which the runtime loop bounds used to force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
+// The rows of a block's BLOCK consecutive steps are staged once in shared memory, column-major, so that the "next" row of every thread
+// is the slot after its own:
+//   n >= BLOCK: the block lies inside one coset.  Pitch BLOCK + 1; slot t holds the row of thread t, and the extra slot BLOCK the
+//     "next" row of the block's last thread.
+//   n < BLOCK (SHORT, n >= 16): the block covers BLOCK / n whole cosets.  Thread t stores its row at slot t + t / n, which leaves a
+//     spare slot after each coset's n rows; the coset's k = 0 thread stores its row there too, as the wrap-around "next" row of the
+//     coset's last step.  Pitch BLOCK + BLOCK / 16.
+// Context / loop / user-stack registers are then addressed dynamically in shared memory instead of in per-thread arrays, which the
+// runtime loop bounds would force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
 // The 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
 // BATCH: blockIdx.y is the proof of a batch (AirParams strides); a separate instantiation, so that one proof compiles as before.
-template <int BLOCK, int MIN_BLOCKS, bool BATCH = false>
+template <int BLOCK, int MIN_BLOCKS, bool BATCH = false, bool SHORT = false>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel(const AirParams P) {
     extern __shared__ __align__(16) unsigned char air_smem[];
     fe *s_rows = reinterpret_cast<fe *>(air_smem);
-    constexpr int PITCH = BLOCK + 1;
+    constexpr int PITCH = SHORT ? BLOCK + BLOCK / 16 : BLOCK + 1;
     const int tid = threadIdx.x;
+    const int slot = SHORT ? tid + (tid >> P.log_n) : tid;
     const unsigned long long n = 1ULL << P.log_n;
     const unsigned long long total = n * (unsigned long long)P.num_c8;
     unsigned long long gid = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -521,18 +124,24 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     //      trace polynomials (poly.cu: boundary_coeffs), which is 8x less work than evaluating them on this domain.
     {
         const int w = P.w;
-        for (int j = 0; j < w; j++) s_rows[j * PITCH + tid] = cur_p[(unsigned long long)j * N];
+        // the k = 0 test is on tid, so that threads past the end of the domain (clamped to its last step) fill their spare slots too
+        const bool wrap_row = SHORT && (tid & (n - 1)) == 0;
+        for (int j = 0; j < w; j++) {
+            const fe v = cur_p[(unsigned long long)j * N];
+            s_rows[j * PITCH + slot] = v;
+            if (wrap_row) s_rows[j * PITCH + slot + (int)n] = v;
+        }
         // the extra row: "next" of the block's last thread (k + 1 wraps to 0 of the same coset at the end of the coset)
-        if (tid < w) {
+        if (!SHORT && tid < w) {
             const unsigned long long gl = (unsigned long long)blockIdx.x * BLOCK + (BLOCK - 1);
             const unsigned long long cl8 = gl >> P.log_n, kl = gl & (n - 1);
             s_rows[tid * PITCH + BLOCK] = ext[(unsigned long long)tid * N + (cl8 * stride) * n + ((kl + 1) & (n - 1))];
         }
     }
     __syncthreads();
-#define SCOL(col, nx) s_rows[(col) * PITCH + tid + (nx)]
-#define DCUR(j) s_rows[(j) * PITCH + tid]
-#define DNXT(j) s_rows[(j) * PITCH + tid + 1]
+#define SCOL(col, nx) s_rows[(col) * PITCH + slot + (nx)]
+#define DCUR(j) s_rows[(j) * PITCH + slot]
+#define DNXT(j) s_rows[(j) * PITCH + slot + 1]
 #define C_CTX(i) (((i) < P.ctx_depth) ? SCOL(ctx_off + (i), 0) : ZERO)
 #define N_CTX(i) (((i) < P.ctx_depth) ? SCOL(ctx_off + (i), 1) : ZERO)
 #define C_LOOP(i) (((i) < P.loop_depth) ? SCOL(loop_off + (i), 0) : ZERO)
@@ -937,32 +546,21 @@ void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     air_upload_constants(c);
     DG_REQUIRE(batch >= 1 && batch <= 65535, "constraint evaluation batch out of range");
     const unsigned long long E = (unsigned long long)P.num_c8 << P.log_n;
-    const unsigned long long n = 1ULL << P.log_n;
     // H100 SXM (700 W), stage 3 of the 2^20-step proof x 26 registers: per-thread arrays 24.8 ms; shared-memory rows, stack-like columns
-    // only 23.7; all columns 23.2; all columns + unreduced per-slot sums (constraint_eval_smem_kernel) 22.2.  The other shared-memory forms
-    // were removed after this measurement.
-    // The shared-memory kernel needs whole blocks inside one coset and at most ~200 KB of rows per block; all proofs of a batch run in one launch.
-    if (n >= 128 && (size_t)P.w * 129 * sizeof(fe) <= 200 * 1024) {
-        const size_t smem = (size_t)P.w * 129 * sizeof(fe);
-        auto k = batch > 1 ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
-        set_func_smem(c, (const void *)k, smem);
-        k<<<dim3((unsigned)(E / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
-        c.launches++;
-        DG_CUDA(cudaGetLastError());
-        return;
-    }
-    // per-thread arrays: short traces (n < 128) and very wide ones, one launch per proof
-    for (int q = 0; q < batch; q++) {
-        AirParams Q = P;
-        Q.ext += q * P.ext_stride; Q.t_ev += q * P.t_ev_stride;
-        Q.coefA += q * P.coef_stride; Q.coefB += q * P.coef_stride;
-        if (Q.violation) Q.violation += q;
-        if (Q.per_override) Q.per_override += q * P.override_stride;
-        if (Q.xpow_override) Q.xpow_override += q * P.override_stride;
-        constraint_eval_kernel<128, 4><<<(unsigned)((E + 127) / 128), 128, 0, c.stream>>>(Q);
-        c.launches++;
-        DG_CUDA(cudaGetLastError());
-    }
+    // only 23.7; all columns 23.2; all columns + unreduced per-slot sums (constraint_eval_smem_kernel) 22.2.  The other forms were removed
+    // after this measurement.
+    // All proofs of a batch run in one launch.  Traces shorter than a block take the SHORT layout; with several ranks their domain slice
+    // can be shorter than one block, and the clamped threads of the partial block write nothing.
+    const bool short_n = P.log_n < 7;
+    const size_t smem = (size_t)P.w * (short_n ? 128 + 128 / 16 : 128 + 1) * sizeof(fe);
+    // widths are bounded by the prover's and verifier's argument checks (w <= 15 + 16 + 8 + 32 = 71, 154,496 B in the SHORT layout)
+    DG_REQUIRE(P.log_n >= 4 && smem <= 200 * 1024, "constraint evaluation needs at least 16 steps and at most 200 KB of rows per block");
+    auto k = short_n ? constraint_eval_smem_kernel<128, 4, true, true>
+                     : batch > 1 ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
+    set_func_smem(c, (const void *)k, smem);
+    k<<<dim3((unsigned)((E + 127) / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
 }
 
 }  // namespace dg

@@ -29,8 +29,8 @@ struct AirParams {
     unsigned long long override_stride;
 };
 
-// evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P); the shared-memory kernel runs them in
-// one launch (blockIdx.y = proof), the per-thread kernel of short or very wide traces launches once per proof
+// evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P) in one launch (blockIdx.y = proof);
+// traces of at least 16 steps
 void launch_constraint_eval(Context &c, const AirParams &P, int batch = 1);
 
 }  // namespace dg
