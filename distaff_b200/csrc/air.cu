@@ -74,12 +74,11 @@ enum { G2 = 0, G3 = 1, G4 = 2, G6 = 3, G7 = 4, G8 = 5 };
 struct Acc {
     fe_wide res;                        // sum_i v_i * cA_i, unreduced (at most 78 constraints < 128 products)
     fe adj[6];
-    const fe *cA, *cB;
     bool nonzero, first;
-    __device__ __forceinline__ void fold(int idx, int group, fe v) {
-        if (first) { wide_set(res, DG_MUL_WIDE(v, cA[idx])); first = false; }
-        else wide_add(res, DG_MUL_WIDE(v, cA[idx]));
-        adj[group] = fe_add(adj[group], fe_mul(v, cB[idx]));
+    __device__ __forceinline__ void fold(int group, fe v, fe a, fe b) {
+        if (first) { wide_set(res, DG_MUL_WIDE(v, a)); first = false; }
+        else wide_add(res, DG_MUL_WIDE(v, a));
+        adj[group] = fe_add(adj[group], fe_mul(v, b));
         nonzero = nonzero || !fe_is_zero(v);
     }
 };
@@ -94,8 +93,8 @@ struct Acc {
 // Context / loop / user-stack registers are then addressed dynamically in shared memory instead of in per-thread arrays, which the
 // runtime loop bounds would force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
 // The 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
-// BATCH: blockIdx.y is the proof of a batch (AirParams strides); a separate instantiation, so that one proof compiles as before.
-template <int BLOCK, int MIN_BLOCKS, bool BATCH = false, bool SHORT = false>
+// blockIdx.y is the proof of a batch (AirParams strides).
+template <int BLOCK, int MIN_BLOCKS, bool SHORT = false>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel(const AirParams P) {
     extern __shared__ __align__(16) unsigned char air_smem[];
     fe *s_rows = reinterpret_cast<fe *>(air_smem);
@@ -113,7 +112,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     const int stride = 1 << (P.log_blowup - 3);
     const unsigned long long N = P.col_stride;                         // column stride of the local slab
     const unsigned long long lde_index = s * (unsigned long long)stride;   // = k*blowup + c8*stride
-    const fe *const ext = BATCH ? P.ext + blockIdx.y * P.ext_stride : P.ext;
+    const fe *const ext = P.ext + blockIdx.y * P.ext_stride;
     const fe *cur_p = ext + (c8_local * stride) * n + k;              // the slab starts at coset c8_base*stride
     const unsigned long long out_idx = (c8_local << P.log_n) + k;
 
@@ -183,34 +182,38 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     acc.first = true;
 #pragma unroll
     for (int g = 0; g < 6; g++) acc.adj[g] = ZERO;
-    acc.cA = BATCH ? P.coefA + blockIdx.y * P.coef_stride : P.coefA; acc.cB = BATCH ? P.coefB + blockIdx.y * P.coef_stride : P.coefB; acc.nonzero = false;
+    acc.nonzero = false;
+    // the proof's coefficients are read at each use: pointers to them held across the body would add live registers
+    auto fold = [&](int idx, int group, fe v) {
+        const unsigned long long at = idx + blockIdx.y * P.coef_stride;
+        acc.fold(group, v, P.coefA[at], P.coefB[at]);
+    };
 
-    const fe *per = P.per_override ? (BATCH ? P.per_override + blockIdx.y * P.override_stride : P.per_override)
+    const fe *per = P.per_override ? P.per_override + blockIdx.y * P.override_stride
                                    : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
-    const fe *const xpow_override = BATCH && P.xpow_override ? P.xpow_override + blockIdx.y * P.override_stride : P.xpow_override;
 
     DG_STEP();
     // ---- decoder: op bits (decoder/op_bits.rs:10-79), constraints 0..14 -------------------------------------------------------
     {
         fe cf_sum = ZERO, ld_prod = ONE, hd_prod = ONE;
 #pragma unroll
-        for (int i = 0; i < 3; i++) { acc.fold(i, G2, is_bin(cf(i))); cf_sum = fe_add(cf_sum, cf(i)); }
+        for (int i = 0; i < 3; i++) { fold(i, G2, is_bin(cf(i))); cf_sum = fe_add(cf_sum, cf(i)); }
 #pragma unroll
-        for (int i = 0; i < 5; i++) { acc.fold(3 + i, G2, is_bin(ld(i))); ld_prod = fe_mul(ld_prod, ld(i)); }
+        for (int i = 0; i < 5; i++) { fold(3 + i, G2, is_bin(ld(i))); ld_prod = fe_mul(ld_prod, ld(i)); }
 #pragma unroll
-        for (int i = 0; i < 2; i++) { acc.fold(8 + i, G2, is_bin(hd(i))); hd_prod = fe_mul(hd_prod, hd(i)); }
+        for (int i = 0; i < 2; i++) { fold(8 + i, G2, is_bin(hd(i))); hd_prod = fe_mul(hd_prod, hd(i)); }
         fe is_hacc = cff[0];
         fe hacc_t = fe_mul(fe_add(op_counter, ONE), is_hacc);
         fe rest_t = fe_mul(op_counter, bnot(is_hacc));
-        acc.fold(10, G3, fe_sub(fe_add(hacc_t, rest_t), DNXT(0)));
-        acc.fold(11, G8, fe_mul(op_counter, fe_mul(bnot(ld_prod), bnot(hd_prod))));
-        acc.fold(12, G8, fe_mul(cf_sum, bnot(fe_mul(ld_prod, hd_prod))));
-        acc.fold(13, G6, fe_mul(cff[7], bnot(next_void)));
+        fold(10, G3, fe_sub(fe_add(hacc_t, rest_t), DNXT(0)));
+        fold(11, G8, fe_mul(op_counter, fe_mul(bnot(ld_prod), bnot(hd_prod))));
+        fold(12, G8, fe_mul(cf_sum, bnot(fe_mul(ld_prod, hd_prod))));
+        fold(13, G6, fe_mul(cff[7], bnot(next_void)));
         fe prefix = fe_add(fe_add(cff[1], cff[4]), fe_add(cff[5], cff[6]));      // BEGIN, LOOP, WRAP, BREAK
         fe align = fe_mul(prefix, per[8 + 1]);
         align = fe_add(align, fe_mul(fe_add(cff[2], cff[3]), per[8 + 0]));       // TEND, FEND
         align = fe_add(align, fe_mul(hdf[0], per[8 + 2]));                        // PUSH
-        acc.fold(14, G4, align);
+        fold(14, G4, align);
     }
 
     DG_STEP();
@@ -263,10 +266,10 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 #pragma unroll
             for (int i = 0; i < 4; i++) r_sp[i] = fe_add(r_sp[i], fe_mul(fk, fe_sub(sp(i), nsp(i))));
         }
-        acc.fold(15, G6, r_sp[0]); acc.fold(16, G7, r_sp[1]); acc.fold(17, G6, r_sp[2]); acc.fold(18, G6, r_sp[3]);
+        fold(15, G6, r_sp[0]); fold(16, G7, r_sp[1]); fold(17, G6, r_sp[2]); fold(18, G6, r_sp[3]);
         // loop image (WRAP, BREAK)
         r_img = fe_mul(fe_add(cff[5], cff[6]), fe_sub(sp(0), C_LOOP(0)));
-        acc.fold(19, G4, r_img);
+        fold(19, G4, r_img);
 
         DG_STEP();
         // context stack: BEGIN/LOOP push (right shift 1, slot 0 = parent hash), TEND/FEND pop (left shift 1), WRAP/BREAK/VOID copy
@@ -278,7 +281,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
                 else v = fe_add(v, fe_mul(f_push, fe_sub(C_CTX(i - 1), N_CTX(i))));
                 if (i < cl - 1) v = fe_add(v, fe_mul(f_pop, fe_sub(C_CTX(i + 1), N_CTX(i))));
                 else v = fe_add(v, fe_mul(f_pop, N_CTX(i)));
-                acc.fold(20 + i, G4, v);
+                fold(20 + i, G4, v);
             }
         }
         DG_STEP();
@@ -291,7 +294,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
                 if (i >= 1) v = fe_add(v, fe_mul(f_rs, fe_sub(C_LOOP(i - 1), N_LOOP(i))));
                 if (i < ll - 1) v = fe_add(v, fe_mul(f_ls, fe_sub(C_LOOP(i + 1), N_LOOP(i))));
                 else v = fe_add(v, fe_mul(f_ls, N_LOOP(i)));
-                acc.fold(20 + cl + i, G4, v);
+                fold(20 + cl + i, G4, v);
             }
         }
     }
@@ -346,8 +349,8 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
             aux0 = fe_add(aux0, fe_mul(f_choose, is_bin(O(2))));
             aux0 = fe_add(aux0, fe_mul(fe_add(f_choose2, f_cswap2), is_bin(O(4))));
         }
-        acc.fold(base, G7, aux0);
-        acc.fold(base + 1, G7, aux1);
+        fold(base, G7, aux0);
+        fold(base + 1, G7, aux1);
 
         DG_STEP();
         // --- per-slot shift structure.  For slot i the generic contribution of an operation is
@@ -403,7 +406,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         }
         // slots >= 8 carry no operation-specific terms: evaluate and fold them straight away (no per-thread array)
         for (int i = 8; i < L; i++) {
-            acc.fold(base + 2 + i, G7, slot_value(i, fc_hi, fl1_hi, fl2_hi, fl4_hi));
+            fold(base + 2 + i, G7, slot_value(i, fc_hi, fl1_hi, fl2_hi, fl4_hi));
             DG_STEP();
         }
         DG_STEP();
@@ -510,20 +513,21 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         }
 #pragma unroll
         for (int i = 0; i < 8; i++)
-            if (i < P.stack_depth) acc.fold(base + 2 + i, G7, ev[i]);
+            if (i < P.stack_depth) fold(base + 2 + i, G7, ev[i]);
     }
 
     DG_STEP();
     // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g ------------------------------------------------------------------
     fe t_res = DG_REDUCE_WIDE(acc.res);
+    const fe *const xpow_override = P.xpow_override ? P.xpow_override + blockIdx.y * P.override_stride : nullptr;
 #pragma unroll
     for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], xpow_override ? xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
     if (!P.verify_mode && c8 == 0 && k != n - 1) {
-        if (acc.nonzero && live) atomicExch(BATCH ? P.violation + blockIdx.y : P.violation, (unsigned)(k + 1));
+        if (acc.nonzero && live) atomicExch(P.violation + blockIdx.y, (unsigned)(k + 1));
         t_res = ZERO;
     }
-    if (live) (BATCH ? P.t_ev + blockIdx.y * P.t_ev_stride : P.t_ev)[out_idx] = t_res;
+    if (live) P.t_ev[blockIdx.y * P.t_ev_stride + out_idx] = t_res;
 }
 
 #undef DCUR
@@ -555,8 +559,7 @@ void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     const size_t smem = (size_t)P.w * (short_n ? 128 + 128 / 16 : 128 + 1) * sizeof(fe);
     // widths are bounded by the prover's and verifier's argument checks (w <= 15 + 16 + 8 + 32 = 71, 154,496 B in the SHORT layout)
     DG_REQUIRE(P.log_n >= 4 && smem <= 200 * 1024, "constraint evaluation needs at least 16 steps and at most 200 KB of rows per block");
-    auto k = short_n ? constraint_eval_smem_kernel<128, 4, true, true>
-                     : batch > 1 ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
+    auto k = short_n ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
     set_func_smem(c, (const void *)k, smem);
     k<<<dim3((unsigned)((E + 127) / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
     c.launches++;

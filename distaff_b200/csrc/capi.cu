@@ -7,18 +7,6 @@
 #include "poly.h"
 #include <thread>
 
-namespace dg {
-void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L);
-unsigned long long pow_search(Context &c, const uint8_t seed[32], unsigned grinding);
-void pow_hash(const uint8_t seed[32], unsigned long long nonce, uint8_t out[32]);
-void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows);
-}  // namespace dg
-
-namespace dg {
-bool host_plan_verify_batch(const std::vector<uint64_t> &indexes, int depth, size_t n_values, const std::vector<uint32_t> &node_counts,
-                            std::vector<uint32_t> &ops, std::vector<uint32_t> &level_start, uint32_t &root_slot);
-}
-
 using namespace dg;
 
 static thread_local std::string t_last_error;
@@ -311,7 +299,9 @@ int dg_find_pow_nonce(const uint8_t seed[32], uint32_t grinding_factor, uint64_t
         std::lock_guard<std::mutex> lk(c.mu);
         DG_REQUIRE(seed && nonce, "null argument");
         DG_REQUIRE(grinding_factor <= 32, "grinding factor cannot be greater than 32");
-        unsigned long long n = pow_search(c, seed, grinding_factor);
+        std::array<uint8_t, 32> s;
+        memcpy(s.data(), seed, 32);
+        const unsigned long long n = pow_search_batch(c, {s}, grinding_factor)[0];
         *nonce = n;
         if (new_seed) pow_hash(seed, n, new_seed);
     });

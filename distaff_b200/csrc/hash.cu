@@ -16,7 +16,6 @@ namespace dg {
 // ---- trace rows -----------------------------------------------------------------------------------------------------
 // ext: [w][N] coset-major (N = n << log_blowup), leaves: N digests in logical row order; blockIdx.y = matrix of a batch, ext_stride
 // elements / 2 N uint4 apart
-template <bool FMA_ADDS>
 __global__ void __launch_bounds__(256) hash_rows_kernel(const fe *__restrict__ ext, uint4 *__restrict__ leaves, int w, unsigned long long N,
                                                         int log_n, int log_blowup, uint32_t one, unsigned long long ext_stride) {
     const unsigned long long p = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -49,8 +48,7 @@ __global__ void __launch_bounds__(256) hash_rows_kernel(const fe *__restrict__ e
             uint32_t flags = 0;
             if (b == 0) flags |= b3::CHUNK_START;
             if (b == nblocks - 1) { flags |= b3::CHUNK_END; if (!two_chunks) flags |= b3::ROOT; }
-            if (FMA_ADDS) b3::compress_fma(cv, m, (uint64_t)chunk, rem < 64 ? rem : 64, flags, one);
-            else b3::compress(cv, m, (uint64_t)chunk, rem < 64 ? rem : 64, flags);
+            b3::compress_fma(cv, m, (uint64_t)chunk, rem < 64 ? rem : 64, flags, one);
         }
         if (two_chunks && chunk == 0) {
 #pragma unroll
@@ -74,8 +72,14 @@ void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, 
     DG_REQUIRE(batch >= 1 && batch <= 65535, "row hashing batch out of range");
     const dim3 grid((unsigned)((N + 255) / 256), (unsigned)batch);
     // FMA-pipe additions: trace tree 10.3 -> 8.8 ms at 2^25 rows x 26 columns (H100 SXM, 700 W)
-    hash_rows_kernel<true><<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, N, log_n, log_blowup, 1u, ext_stride);
+    hash_rows_kernel<<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, N, log_n, log_blowup, 1u, ext_stride);
     c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
+// rows of a plain column-major matrix (no coset permutation): physical position == logical row
+void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows) {
+    hash_rows_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c.stream>>>(cols, (uint4 *)digests, w, rows, 63, 0, 1u, 0); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -156,20 +160,13 @@ static void tree_levels(Context &c, const uint4 *in, uint4 *nodes, unsigned long
     }
 }
 
-// leaves: L digests (L power of two >= 2); nodes: L digests (heap layout)
-void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L) {
-    DG_REQUIRE(L >= 2 && (L & (L - 1)) == 0, "number of leaves must be a power of 2 and >= 2");
-    uint4 *nd = (uint4 *)nodes;
-    tree_levels(c, (const uint4 *)leaves, nd, L, 1);
-    DG_CUDA(cudaMemsetAsync(nd, 0, 32, c.stream));             // nodes[0] = 0 (merkle.rs:273)
-}
-
-// `batch` trees of L leaves each: leaves and nodes of tree q at q * L digests from the first
-void merkle_build_batch(Context &c, const void *leaves, void *nodes, unsigned long long L, int batch) {
+// `batch` trees of L leaves each (L power of two >= 2), L digests of nodes each (heap layout): leaves and nodes of tree q at q * L digests
+// from the first
+void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L, int batch) {
     DG_REQUIRE(L >= 2 && (L & (L - 1)) == 0, "number of leaves must be a power of 2 and >= 2");
     uint4 *nd = (uint4 *)nodes;
     tree_levels(c, (const uint4 *)leaves, nd, L, 1, batch, 2 * L, 2 * L);
-    DG_CUDA(cudaMemset2DAsync(nd, L * 32, 0, 32, batch, c.stream));
+    DG_CUDA(cudaMemset2DAsync(nd, L * 32, 0, 32, batch, c.stream));     // nodes[0] = 0 (merkle.rs:273)
 }
 
 // completes a tree whose level with m nodes (m a power of two) already sits at nodes[m .. 2m)
@@ -205,14 +202,6 @@ __device__ __forceinline__ bool pow_hit(const uint32_t *__restrict__ seed, unsig
     return tz >= grinding;
 }
 
-__global__ void __launch_bounds__(256) pow_kernel(const uint32_t *__restrict__ seed, unsigned long long start, unsigned long long count,
-                                                  unsigned grinding, unsigned long long *best) {
-    const unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= count) return;
-    const unsigned long long nonce = start + g;
-    if (pow_hit(seed, nonce, grinding)) atomicMin(best, nonce);
-}
-
 // one window [start, start + count) of nonces for each unfinished proof active[blockIdx.y]: seeds [proof][8 words], best [proof]
 __global__ void __launch_bounds__(256) pow_batch_kernel(const uint32_t *__restrict__ seeds, const unsigned *__restrict__ active,
                                                         unsigned long long start, unsigned long long count, unsigned grinding,
@@ -224,29 +213,10 @@ __global__ void __launch_bounds__(256) pow_batch_kernel(const uint32_t *__restri
     if (pow_hit(seeds + 8 * p, nonce, grinding)) atomicMin(best + p, nonce);
 }
 
-// returns the smallest nonce >= 1 whose hash has >= grinding trailing zero bits in its first 8 bytes
-unsigned long long pow_search(Context &c, const uint8_t seed[32], unsigned grinding) {
-    DevBuf d_seed(32), d_best(8);
-    DG_CUDA(cudaMemcpyAsync(d_seed.p, seed, 32, cudaMemcpyHostToDevice, c.stream));
-    const unsigned long long none = ~0ULL;
-    DG_CUDA(cudaMemcpyAsync(d_best.p, &none, 8, cudaMemcpyHostToDevice, c.stream));
-    unsigned long long start = 1;
-    const unsigned long long batch = 1ULL << 22;
-    for (int iter = 0; iter < (1 << 20); iter++) {
-        pow_kernel<<<(unsigned)(batch / 256), 256, 0, c.stream>>>(d_seed.as<uint32_t>(), start, batch, grinding, d_best.as<unsigned long long>()); c.launches++;
-        DG_CUDA(cudaGetLastError());
-        unsigned long long best;
-        DG_CUDA(cudaMemcpyAsync(&best, d_best.p, 8, cudaMemcpyDeviceToHost, c.stream));
-        DG_CUDA(cudaStreamSynchronize(c.stream));
-        if (best != none) return best;
-        start += batch;
-    }
-    throw Error(-4, "proof-of-work search exhausted");
-}
-
-// pow_search for K seeds at once: each round scans the same window of nonces for every proof that has no hit yet (one launch, one copy
-// of the K results back).  A proof finishes in the first window where it has a hit, and the window's smallest hit is its smallest nonce.
-// One proof keeps pow_search's 2^22 window.  A batch scans 2^22 / K nonces per proof and round (one 2^22-nonce round in all), but at least
+// For each of K seeds, the smallest nonce >= 1 whose hash has >= grinding trailing zero bits in its first 8 bytes.  Each round scans the
+// same window of nonces for every proof that has no hit yet (one launch, one copy of the K results back).  A proof finishes in the first
+// window where it has a hit, and the window's smallest hit is its smallest nonce.
+// One proof scans a 2^22 window per round.  A batch scans 2^22 / K nonces per proof and round (one 2^22-nonce round in all), but at least
 // 2^(grinding - 2), a quarter of the expected search (clamped to 2^10 .. 2^22): large batches run more rounds but hash little past each
 // proof's first hit, small ones keep few rounds.  Measured on an H100 at 400 W, grinding 20, PoW
 // stage of a batch of 16 / 64 / 256 proofs: 2^16: 1.17 / 3.02 / 11.7 ms; 2^18: 0.76 / 2.57 / 10.9; 2^19: 0.74 / 2.75 / 12.2; 2^20: 0.86 /
@@ -284,14 +254,6 @@ std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<s
     throw Error(-4, "proof-of-work search exhausted");
 }
 
-}  // namespace dg
-
-namespace dg {
-// rows of a plain column-major matrix (no coset permutation): physical position == logical row
-void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows) {
-    hash_rows_kernel<false><<<(unsigned)((rows + 255) / 256), 256, 0, c.stream>>>(cols, (uint4 *)digests, w, rows, 63, 0, 1u, 0); c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
 // host-side BLAKE3 of the 64-byte proof-of-work input seed || nonce_le || 0^24 (proof_of_work.rs:12-24)
 void pow_hash(const uint8_t seed[32], unsigned long long nonce, uint8_t out[32]) {
     uint32_t m[16], cv[8];

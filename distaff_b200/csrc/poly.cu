@@ -17,13 +17,6 @@ __device__ __forceinline__ fe pw(const PowRef &t, unsigned long long e) {
     return fe_mul(t.lo[e & ((1ULL << t.lo_bits) - 1ULL)], t.hi[e >> t.lo_bits]);
 }
 
-// lo[i] = base^i (i < lo_n) and hi[i] = step^i (i < hi_n) in one launch
-__global__ void pow_fill_kernel(fe *lo, fe base, unsigned long long lo_n, fe *hi, fe step, unsigned long long hi_n) {
-    unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < lo_n) lo[i] = fe_pow_u64(base, i);
-    else if (i < lo_n + hi_n) hi[i - lo_n] = fe_pow_u64(step, i - lo_n);
-}
-
 // table q = blockIdx.y: (base, step) = bs[2q], bs[2q + 1], written to lo + q lo_n and hi + q hi_n
 __global__ void pow_fill_batch_kernel(fe *lo, unsigned long long lo_n, fe *hi, unsigned long long hi_n, const fe *__restrict__ bs) {
     const fe base = bs[2 * blockIdx.y], step = bs[2 * blockIdx.y + 1];
@@ -39,30 +32,23 @@ static int pow_lo_bits(unsigned long long len) {
     while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
     return lo_bits;
 }
+static unsigned long long pow_hi_n(unsigned long long len) {
+    const unsigned long long lo_n = 1ULL << pow_lo_bits(len);
+    return (len + lo_n - 1) / lo_n + 1;
+}
 
 fe PowTables::step(fe base, unsigned long long len) { return fe_pow_u64(base, 1ULL << pow_lo_bits(len)); }
+unsigned long long PowTables::entries(unsigned long long len) { return (1ULL << pow_lo_bits(len)) + pow_hi_n(len); }
 
 PowTables::PowTables(Context &c, const fe *base_step, int batch, unsigned long long len) {
     DG_REQUIRE(batch >= 1 && batch <= 65535, "power table batch out of range");
     lo_bits = pow_lo_bits(len);
     lo_n = 1ULL << lo_bits;
-    hi_n = (len + lo_n - 1) / lo_n + 1;
+    hi_n = pow_hi_n(len);
     lo.alloc(lo_n * batch * sizeof(fe));
     hi.alloc(hi_n * batch * sizeof(fe));
     pow_fill_batch_kernel<<<dim3((unsigned)((lo_n + hi_n + 127) / 128), (unsigned)batch), 128, 0, c.stream>>>(lo.as<fe>(), lo_n, hi.as<fe>(), hi_n, base_step);
     c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
-
-PowTable::PowTable(Context &c, fe base, unsigned long long len) {
-    lo_bits = 1;
-    while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
-    const unsigned long long lo_n = 1ULL << lo_bits;
-    const unsigned long long hi_n = (len + lo_n - 1) / lo_n + 1;
-    lo.alloc(lo_n * sizeof(fe));
-    hi.alloc(hi_n * sizeof(fe));
-    fe step = fe_pow_u64(base, lo_n);
-    pow_fill_kernel<<<(unsigned)((lo_n + hi_n + 127) / 128), 128, 0, c.stream>>>(lo.as<fe>(), base, lo_n, hi.as<fe>(), step, hi_n); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -113,29 +99,25 @@ __device__ __forceinline__ void st_cg_fe(fe *p, fe v) {
     __stcg(reinterpret_cast<uint4 *>(p), make_uint4((unsigned)v.lo, (unsigned)(v.lo >> 32), (unsigned)v.hi, (unsigned)(v.hi >> 32)));
 }
 
-// BATCH: `batch` vectors in one launch (SynDivBatch strides); one ticket counter over all their blocks, ticket t = (vector t / nblocks,
+// `batch` vectors in one launch (SynDivBatch strides); one ticket counter over all their blocks, ticket t = (vector t / nblocks,
 // block nblocks - 1 - t % nblocks): a block only waits on blocks of its own vector with smaller tickets, so the look-back keeps its
-// forward-progress guarantee.  A separate instantiation, so that one vector compiles as before.
+// forward-progress guarantee.
 struct SynDivBatch { unsigned long long in_stride, out_stride, b_stride_lo, b_stride_hi, binv_stride_lo, binv_stride_hi; const fe *sub0; };
-template <bool BATCH>
 __global__ void __launch_bounds__(SCAN_THREADS) syn_div_chained_kernel(const fe *__restrict__ in, fe *__restrict__ out, unsigned long long len, PowRef bp,
-                                                                       PowRef binvp, fe sub0, ScanDesc *desc, unsigned *ticket, unsigned nblocks,
-                                                                       SynDivBatch sb) {
+                                                                       PowRef binvp, ScanDesc *desc, unsigned *ticket, unsigned nblocks, SynDivBatch sb) {
     __shared__ fe s_warp[SCAN_THREADS / 32];
     __shared__ fe s_carry;
     __shared__ unsigned s_ticket;
     if (threadIdx.x == 0) s_ticket = atomicAdd(ticket, 1u);
     __syncthreads();
     unsigned t = s_ticket;
-    if constexpr (BATCH) {
-        const unsigned q = t / nblocks;
-        t -= q * nblocks;
-        in += q * sb.in_stride; out += q * sb.out_stride;
-        bp.lo += q * sb.b_stride_lo; bp.hi += q * sb.b_stride_hi;
-        binvp.lo += q * sb.binv_stride_lo; binvp.hi += q * sb.binv_stride_hi;
-        sub0 = sb.sub0[q];
-        desc += (unsigned long long)q * nblocks;
-    }
+    const unsigned q = t / nblocks;
+    t -= q * nblocks;
+    in += q * sb.in_stride; out += q * sb.out_stride;
+    bp.lo += q * sb.b_stride_lo; bp.hi += q * sb.b_stride_hi;
+    binvp.lo += q * sb.binv_stride_lo; binvp.hi += q * sb.binv_stride_hi;
+    const fe sub0 = sb.sub0[q];
+    desc += (unsigned long long)q * nblocks;
     const unsigned blk = nblocks - 1u - t;
     const unsigned long long base = (unsigned long long)blk * SCAN_BLOCK + (unsigned long long)threadIdx.x * SCAN_PER_THREAD;
     fe x[SCAN_PER_THREAD];
@@ -194,34 +176,19 @@ __global__ void __launch_bounds__(SCAN_THREADS) syn_div_chained_kernel(const fe 
     }
 }
 
-// out[i] = sum_{j>i} (in[j] - [j==0] sub0) b^(j-i-1).  in may equal out.
-void syn_div(Context &c, const fe *in, fe *out, unsigned long long len, const PowRef &b_pows, const PowRef &binv_pows, fe sub0) {
-    const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
-    DevBuf d((size_t)nblk * sizeof(ScanDesc) + 16);
-    DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
-    ScanDesc *desc = d.as<ScanDesc>();
-    unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk);
-    syn_div_chained_kernel<false><<<(unsigned)nblk, SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, sub0, desc, ticket, (unsigned)nblk,
-                                                                                SynDivBatch{}); c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
-
-void syn_div_batch(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, unsigned long long len,
-                   const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
-                   unsigned long long binv_lo_stride, unsigned long long binv_hi_stride, const fe *sub0_dev, const fe *sub0_host) {
-    if (batch == 1) {
-        syn_div(c, in, out, len, b_pows, binv_pows, sub0_host[0]);
-        return;
-    }
+// out[i] = sum_{j>i} (in[j] - [j==0] sub0) b^(j-i-1) for each vector.  in may equal out.
+void syn_div(Context &c, int batch, const fe *in, unsigned long long in_stride, fe *out, unsigned long long out_stride, unsigned long long len,
+             const PowRef &b_pows, unsigned long long b_lo_stride, unsigned long long b_hi_stride, const PowRef &binv_pows,
+             unsigned long long binv_lo_stride, unsigned long long binv_hi_stride, const fe *sub0) {
     const unsigned long long nblk = (len + SCAN_BLOCK - 1) / SCAN_BLOCK;
     DG_REQUIRE(nblk * batch < (1ULL << 31), "division batch too large for one launch");
     DevBuf d((size_t)nblk * batch * sizeof(ScanDesc) + 16);
     DG_CUDA(cudaMemsetAsync(d.p, 0, d.bytes, c.stream));
     ScanDesc *desc = d.as<ScanDesc>();
     unsigned *ticket = reinterpret_cast<unsigned *>(desc + nblk * batch);
-    const SynDivBatch sb{in_stride, out_stride, b_lo_stride, b_hi_stride, binv_lo_stride, binv_hi_stride, sub0_dev};
-    syn_div_chained_kernel<true><<<(unsigned)(nblk * batch), SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, fe_make(0, 0), desc, ticket,
-                                                                                          (unsigned)nblk, sb); c.launches++;
+    const SynDivBatch sb{in_stride, out_stride, b_lo_stride, b_hi_stride, binv_lo_stride, binv_hi_stride, sub0};
+    syn_div_chained_kernel<<<(unsigned)(nblk * batch), SCAN_THREADS, 0, c.stream>>>(in, out, len, b_pows, binv_pows, desc, ticket, (unsigned)nblk, sb);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -365,19 +332,16 @@ void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe
 //   I = (sum_j a_j T_j - Ka) + x^adj (sum_j b_j T_j - Kb),     Ka = sum_j a_j in_j,  Kb = sum_j b_j in_j
 // whose coefficients are two linear combinations of the trace polynomials' coefficients: n*nb multiplications instead of 8n*nb.
 // coef = [a_init | b_init | a_final | b_final], nb entries each; ic / fc receive the 8n coefficients of the first / last step numerators.
-// BATCH: blockIdx.y = proof of a batch: polys poly_stride, coef coef_stride, ic / fc out_stride elements apart, its constants
-// K[4 y .. 4 y + 4) instead of the by-value ones (a separate instantiation, so that one proof compiles as before)
-template <bool BATCH>
-__global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned long long n, int nb, const fe *__restrict__ coef, fe KiA, fe KiB,
-                                       fe KfA, fe KfB, unsigned long long adj, fe *__restrict__ ic, fe *__restrict__ fc, const fe *__restrict__ K,
-                                       unsigned long long poly_stride, unsigned long long coef_stride, unsigned long long out_stride) {
+// blockIdx.y = proof of a batch: polys poly_stride, coef coef_stride, ic / fc out_stride elements apart, its constants
+// KiA, KiB, KfA, KfB = K[4 y .. 4 y + 4)
+__global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned long long n, int nb, const fe *__restrict__ coef, unsigned long long adj,
+                                       fe *__restrict__ ic, fe *__restrict__ fc, const fe *__restrict__ K, unsigned long long poly_stride,
+                                       unsigned long long coef_stride, unsigned long long out_stride) {
     const unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
-    if constexpr (BATCH) {
-        polys += blockIdx.y * poly_stride; coef += blockIdx.y * coef_stride;
-        ic += blockIdx.y * out_stride; fc += blockIdx.y * out_stride;
-        KiA = K[4 * blockIdx.y]; KiB = K[4 * blockIdx.y + 1]; KfA = K[4 * blockIdx.y + 2]; KfB = K[4 * blockIdx.y + 3];
-    }
+    polys += blockIdx.y * poly_stride; coef += blockIdx.y * coef_stride;
+    ic += blockIdx.y * out_stride; fc += blockIdx.y * out_stride;
+    const fe KiA = K[4 * blockIdx.y], KiB = K[4 * blockIdx.y + 1], KfA = K[4 * blockIdx.y + 2], KfB = K[4 * blockIdx.y + 3];
     // nb < 128 products per sum: accumulated unreduced (288 bits), one reduction each
     fe_wide wa, wb, wc, wd;
     for (int j = 0; j < nb; j++) {
@@ -399,19 +363,11 @@ __global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned lo
     for (unsigned long long q = n + k; q < 8 * n; q += n)
         if (q < adj || q >= adj + n) { ic[q] = zero; fc[q] = zero; }
 }
-void boundary_coeffs(Context &c, const fe *polys, unsigned long long n, int nb, const fe *coef, fe KiA, fe KiB, fe KfA, fe KfB, fe *ic, fe *fc) {
-    boundary_coeffs_kernel<false><<<(unsigned)((n + 255) / 256), 256, 0, c.stream>>>(polys, n, nb, coef, KiA, KiB, KfA, KfB, 6 * n + 2, ic, fc, nullptr, 0,
-                                                                                      0, 0);
-    c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
-void boundary_coeffs_batch(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
-                           unsigned long long coef_stride, const fe *K, const fe *K_host, fe *ic, fe *fc, unsigned long long out_stride) {
+void boundary_coeffs(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
+                     unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride) {
     DG_REQUIRE(batch >= 1 && batch <= 65535, "boundary batch out of range");
-    if (batch == 1) { boundary_coeffs(c, polys, n, nb, coef, K_host[0], K_host[1], K_host[2], K_host[3], ic, fc); return; }
-    const fe z = fe_make(0, 0);
-    boundary_coeffs_kernel<true><<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, nb, coef, z, z, z, z, 6 * n + 2, ic, fc, K,
-                                                                                                      poly_stride, coef_stride, out_stride);
+    boundary_coeffs_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, nb, coef, 6 * n + 2, ic, fc, K, poly_stride,
+                                                                                                   coef_stride, out_stride);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
@@ -469,34 +425,23 @@ void coset_interp_finish(Context &c, const fe *b, fe *out, int log_n, int batch,
 
 // composition polynomial (trace_table.rs:241-258, constraint_poly.rs:49):
 //   comp[k] = cq[k]*kc + [k < n] (t1q[k]+t2q[k])*k1 + [inc <= k < inc+n] (t1q[k-inc]+t2q[k-inc])*k2
-// BATCH: blockIdx.y = proof of a batch: t1q / t2q t_stride, cq / comp len elements apart, its k1, k2, kc = ks[3 y ..] instead of the by-value ones
-template <bool BATCH>
+// blockIdx.y = proof of a batch: t1q / t2q t_stride, cq / comp len elements apart, its k1, k2, kc = ks[3 y ..]
 __global__ void compose_kernel(const fe *__restrict__ t1q, const fe *__restrict__ t2q, const fe *__restrict__ cq, fe *__restrict__ comp,
-                               unsigned long long n, unsigned long long len, unsigned long long inc, fe k1, fe k2, fe kc, const fe *__restrict__ ks,
-                               unsigned long long t_stride) {
+                               unsigned long long n, unsigned long long len, unsigned long long inc, const fe *__restrict__ ks, unsigned long long t_stride) {
     unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= len) return;
-    if constexpr (BATCH) {
-        t1q += blockIdx.y * t_stride; t2q += blockIdx.y * t_stride;
-        cq += blockIdx.y * len; comp += blockIdx.y * len;
-        k1 = ks[3 * blockIdx.y]; k2 = ks[3 * blockIdx.y + 1]; kc = ks[3 * blockIdx.y + 2];
-    }
+    t1q += blockIdx.y * t_stride; t2q += blockIdx.y * t_stride;
+    cq += blockIdx.y * len; comp += blockIdx.y * len;
+    const fe k1 = ks[3 * blockIdx.y], k2 = ks[3 * blockIdx.y + 1], kc = ks[3 * blockIdx.y + 2];
     fe v = fe_mul(cq[k], kc);
     if (k < n) v = fe_add(v, fe_mul(fe_add(t1q[k], t2q[k]), k1));
     if (k >= inc && k < inc + n) v = fe_add(v, fe_mul(fe_add(t1q[k - inc], t2q[k - inc]), k2));
     comp[k] = v;
 }
-void compose(Context &c, const fe *t1q, const fe *t2q, const fe *cq, fe *comp, unsigned long long n, unsigned long long len, unsigned long long inc,
-             fe k1, fe k2, fe kc) {
-    compose_kernel<false><<<(unsigned)((len + 255) / 256), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, k1, k2, kc, nullptr, 0); c.launches++;
-    DG_CUDA(cudaGetLastError());
-}
-void compose_batch(Context &c, int batch, const fe *t1q, const fe *t2q, unsigned long long t_stride, const fe *cq, fe *comp, unsigned long long n,
-                   unsigned long long len, unsigned long long inc, const fe *ks, const fe *ks_host) {
+void compose(Context &c, int batch, const fe *t1q, const fe *t2q, unsigned long long t_stride, const fe *cq, fe *comp, unsigned long long n,
+             unsigned long long len, unsigned long long inc, const fe *ks) {
     DG_REQUIRE(batch >= 1 && batch <= 65535, "composition batch out of range");
-    if (batch == 1) { compose(c, t1q, t2q, cq, comp, n, len, inc, ks_host[0], ks_host[1], ks_host[2]); return; }
-    const fe z = fe_make(0, 0);
-    compose_kernel<true><<<dim3((unsigned)((len + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, z, z, z, ks, t_stride);
+    compose_kernel<<<dim3((unsigned)((len + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(t1q, t2q, cq, comp, n, len, inc, ks, t_stride);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }

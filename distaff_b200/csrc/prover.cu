@@ -402,7 +402,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         // one GPU: the K trees level by level in one launch per level; several GPUs (K == 1): the sharded tree
         if (G == 1) {
             t_nodes.alloc((size_t)K * N_loc * 32);
-            merkle_build_batch(c, t_leaves.p, t_nodes.p, N_loc, K);
+            merkle_build(c, t_leaves.p, t_nodes.p, N_loc, K);
         }
         std::vector<const void *> roots;
         for (int p = 0; p < K; p++) {
@@ -442,7 +442,6 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     // carries a boundary constraint, which depends on the number of public inputs / outputs: they are padded with zero coefficients to
     // the largest count nbm (a zero coefficient adds nothing to the boundary numerators).
     size_t coef_stride = 0, T = 0, nbm = 0;
-    std::vector<fe> bconst;                       // the boundary constants on the host, [K][4]
     {
         for (int p = 0; p < K; p++) {
             ProofState &s = ps[p];
@@ -467,7 +466,6 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             const fe consts[4] = {s.cc.KiA, s.cc.KiB, s.cc.KfA, s.cc.KfB};
             std::copy(consts, consts + 4, pack.begin() + coef_stride * K + 4 * p);
         }
-        bconst.assign(pack.begin() + coef_stride * K, pack.end());
         d_coef.alloc(pack.size() * 16);
         h2d(c, d_coef.p, pack.data(), pack.size() * 16);
         DG_CUDA(cudaStreamSynchronize(c.stream));
@@ -515,8 +513,8 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     sub.mark("3.intt+gather");
         coset_interp_finish(c, G > 1 ? gathered.as<fe>() : evals_loc.as<fe>(), evals.as<fe>() + 2 * E, log_n, K, E_loc, 3 * E);
         // boundary constraints (evaluator.rs:181-326), directly as the 8n coefficients the reference obtains by interpolation
-        boundary_coeffs_batch(c, K, polys.as<fe>(), (size_t)w * n, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
-                              bconst.data(), evals.as<fe>(), evals.as<fe>() + E, 3 * E);
+        boundary_coeffs(c, K, polys.as<fe>(), (size_t)w * n, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
+                        evals.as<fe>(), evals.as<fe>() + E, 3 * E);
     }
     if (K == 1) debug_dump(c, "t_coeffs", evals.as<fe>() + 2 * E, E * 16);
 
@@ -531,13 +529,17 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             debug_dump(c, "i_coeffs", evals.as<fe>(), E * 16);
             debug_dump(c, "f_coeffs", evals.as<fe>() + E, E * 16);
         }
-        PowTable one_t(c, fe_make(1, 0), E + 1), xl_t(c, x_last, E + 1), xli_t(c, root_n, E + 1);
-        const std::vector<fe> zeros(K, fe_make(0, 0));
-        DevBuf d_zeros((size_t)16 * K);
-        DG_CUDA(cudaMemsetAsync(d_zeros.p, 0, d_zeros.bytes, c.stream));
+        // one upload: the (base, step) pairs of the power tables of 1, x_last and 1 / x_last (shared by the K proofs), then K zeros (sub0)
+        std::vector<fe> pack(6 + K, fe_make(0, 0));
+        const fe bases[3] = {fe_make(1, 0), x_last, root_n};
+        for (int t = 0; t < 3; t++) { pack[2 * t] = bases[t]; pack[2 * t + 1] = PowTables::step(bases[t], E + 1); }
+        DevBuf d_pack(pack.size() * 16);
+        h2d(c, d_pack.p, pack.data(), pack.size() * 16);
+        PowTables pows(c, d_pack.as<fe>(), 3, E + 1);
+        const fe *zeros = d_pack.as<fe>() + 6;
         fe *ic = evals.as<fe>(), *fc = evals.as<fe>() + E, *tc = evals.as<fe>() + 2 * E;          // of proof 0; proof p at + 3 E p
-        syn_div_batch(c, K, ic, 3 * E, ic, 3 * E, E, one_t.ref(), 0, 0, one_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - 1)
-        syn_div_batch(c, K, fc, 3 * E, fc, 3 * E, E, xl_t.ref(), 0, 0, xli_t.ref(), 0, 0, d_zeros.as<fe>(), zeros.data());   // / (x - x_last)
+        syn_div(c, K, ic, 3 * E, ic, 3 * E, E, pows.ref(0), 0, 0, pows.ref(0), 0, 0, zeros);   // / (x - 1)
+        syn_div(c, K, fc, 3 * E, fc, 3 * E, E, pows.ref(1), 0, 0, pows.ref(2), 0, 0, zeros);   // / (x - x_last)
         syn_div_expanded_sum(c, tc, scratch.as<fe>(), ic, fc, combined.as<fe>(), n, E, x_last, K, 3 * E, E);   // / ((x^n - 1)/(x - x_last)), summed
     }
     if (K == 1) debug_dump(c, "constraint_poly", combined.p, E * 16);
@@ -554,7 +556,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         if (G == 1) {
             c_nodes.alloc((size_t)K * (N_loc / 4) * 32);
-            merkle_build_batch(c, c_items.p, c_nodes.p, N_loc / 4, K);
+            merkle_build(c, c_items.p, c_nodes.p, N_loc / 4, K);
         }
         std::vector<const void *> roots;
         std::vector<int> who;
@@ -640,14 +642,14 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * w, *d_ks = d_subs + (size_t)3 * K;
         fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
         lincomb2(c, polys.as<fe>(), n, w, d_cc, d_cc + w, t1, t2, K, 2 * w, 2 * n);
-        syn_div_batch(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs, subs);
+        syn_div(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs);
         //                                                                                                   (T1(x) - T1(z)) / (x - z)
-        syn_div_batch(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K,
-                      subs + K);                                                                           // (T2(x) - T2(zg)) / (x - zg)
-        syn_div_batch(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n,
-                      zi_t.hi_n, d_subs + 2 * K, subs + 2 * K);                                            // (C(x) - C(z)) / (x - z)
+        syn_div(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K);
+        //                                                                                                   (T2(x) - T2(zg)) / (x - zg)
+        syn_div(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n,
+                d_subs + 2 * K);                                                                           // (C(x) - C(z)) / (x - z)
     sub.mark("6.lincomb+syndiv");
-        compose_batch(c, K, t1, t2, 2 * n, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, d_ks, ks);
+        compose(c, K, t1, t2, 2 * n, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, d_ks);
         if (K == 1) debug_dump(c, "composition_poly", comp.p, E * 16);
         // every rank extends its own cosets; the first FRI layers work on these slabs directly (no all-gather of the N evaluations)
         lde_batch(c, comp.as<fe>(), comp_ext.as<fe>(), log_n, log_b, 8, K, E, N_loc, c0, (unsigned)nc);
@@ -725,7 +727,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             layer_bufs.emplace_back((size_t)K * R * 32);
             const uint8_t *nodes = layer_bufs.back().as<uint8_t>();
             fri_hash_rows(c, cur, lay, rows, (void *)leaves, K, cur_stride);
-            merkle_build_batch(c, leaves, (void *)nodes, R, K);
+            merkle_build(c, leaves, (void *)nodes, R, K);
             for (int p = 0; p < K; p++) {
                 if (!ps[p].live) continue;
                 FriLayerDev &L = ps[p].layers.emplace_back();
@@ -973,11 +975,7 @@ size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b) {
     f += E * fe16 + N * fe16;                 // 6: composition polynomial + its LDE
     f += 2 * n * fe16;                        // 6: the two trace quotients
     size_t pow_n = 0;                         // 6: the four power tables of z, 1/z (E + 1 entries), z g, 1/(z g) (n + 1 entries)
-    for (uint64_t len : {E + 1, E + 1, (uint64_t)n + 1, (uint64_t)n + 1}) {
-        int lo_bits = 1;
-        while ((1ULL << (2 * lo_bits)) < len) lo_bits++;
-        pow_n += (1ULL << lo_bits) + (len + (1ULL << lo_bits) - 1) / (1ULL << lo_bits) + 1;
-    }
+    for (uint64_t len : {E + 1, E + 1, (uint64_t)n + 1, (uint64_t)n + 1}) pow_n += PowTables::entries(len);
     f += pow_n * fe16;
     f += (N / 4) * (2 * dg32 + fe16) * 4 / 3; // 7: FRI layers (R = D / 4 row hashes, tree and folded values per layer, D = N, N / 4, ...)
     f += (size_t)1 << 20;                     // coefficients, DEEP values, scan descriptors, evaluation partials, PoW, openings (< 1 MB)

@@ -38,5 +38,8 @@ struct VerifyRequest {
 // Throws for errors of the whole call (CUDA failures); then status and messages are left as they were.
 void verify_proofs(Context &c, const std::vector<VerifyRequest> &req, std::vector<int> &status, std::vector<std::string> &messages,
                    dg_verify_stats_t *stats);
+// the verifier's batch-Merkle hashing plan of one tree, computed on the host alone (verifier.cu)
+bool host_plan_verify_batch(const std::vector<uint64_t> &indexes, int depth, size_t n_values, const std::vector<uint32_t> &node_counts,
+                            std::vector<uint32_t> &ops, std::vector<uint32_t> &level_start, uint32_t &root_slot);
 
 }  // namespace dg

@@ -36,12 +36,6 @@ ShardLocation ShardGeom::node(uint64_t h) const {
 }
 
 // ---- kernels ------------------------------------------------------------------------------------------------------------------
-// levels of a heap-layout tree from L/2 nodes down to (and including) the level with `stop` nodes (hash.cu)
-void merkle_levels_down_to(Context &c, const void *leaves, void *nodes, unsigned long long L, unsigned long long stop);
-void merkle_build_partial(Context &c, const void *leaves, void *nodes, unsigned long long L, unsigned long long stop) {
-    merkle_levels_down_to(c, leaves, nodes, L, stop);
-}
-
 // upper[(n << log_g) + (k << log_g) + g] = gathered[g][k]
 __global__ void interleave_roots_kernel(const uint4 *__restrict__ gathered, uint4 *__restrict__ upper, unsigned long long n, int log_g) {
     const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -104,7 +98,7 @@ void ShardedTree::build(Context &c, const void *items_local_dev, uint64_t n, int
         const void *roots = items_local_dev;
         if (log_blk > 0) {
             local_nodes.alloc(local_items * 32);
-            merkle_build_partial(c, items_local_dev, local_nodes.p, local_items, n);
+            merkle_levels_down_to(c, items_local_dev, local_nodes.p, local_items, n);
             roots = (const uint8_t *)local_nodes.p + n * 32;           // heap level with n nodes: the subtree roots, by k
         }
         // re-shard the roots by k-range: recv[g'][k'] = root (k = g n/G + k') of rank g'

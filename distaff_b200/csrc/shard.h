@@ -74,7 +74,7 @@ struct ShardedTree {
 
     // fetch_root = false leaves the root on the device (upper_p + 32): no host synchronisation
     void build(Context &c, const void *items_local_dev, uint64_t n, int log_blk, bool fetch_root = true);
-    // one GPU: the tree over items_dev whose heap (n << log_blk digests) the caller has built (merkle_build_batch) and owns
+    // one GPU: the tree over items_dev whose heap (n << log_blk digests) the caller has built (merkle_build) and owns
     void attach(Context &c, const void *items_dev, const void *nodes_dev, uint64_t n, int log_blk);
     const void *root_dev() const { return (const uint8_t *)top_p + 32; }
     // locations as references for a FetchBatch
@@ -87,9 +87,6 @@ struct ShardedTree {
     }
 };
 
-void merkle_build_partial(Context &c, const void *leaves, void *nodes, unsigned long long L, unsigned long long stop);
-void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long long L);
-void merkle_finish(Context &c, void *nodes, unsigned long long m);
 void interleave_roots(Context &c, const void *gathered, void *upper, unsigned long long n, int log_g);
 // [k][c4_local] digests; batch > 1: `batch` slabs of n << log_nc evaluations, their items (n << log_nc) / 4 digests apart
 void constraint_items_local(Context &c, const fe *evals_local, int log_n, int log_nc, void *items, int batch = 1);

@@ -34,10 +34,6 @@
 
 namespace dg {
 
-void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows);
-void hash64_contiguous(Context &c, const void *in, void *out, unsigned long long count);
-void pow_hash(const uint8_t seed[32], unsigned long long nonce, uint8_t out[32]);
-
 namespace {
 
 // ---- bincode reader (proof.rs:10-37, fri/mod.rs:17-30, merkle.rs:14-18) -------------------------------------------------------
