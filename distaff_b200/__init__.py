@@ -9,4 +9,4 @@ Python host-side mirror of the reference interface for the prove hot path:
 The compute path is hand-written CUDA behind the C-ABI of include/distaff_gpu.h; there is no CPU fallback.
 """
 from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
-                  merkle_build, hash_rows, hash64, find_pow_nonce, field_op)
+                  merkle_build, hash_rows, hash64, find_pow_nonce, field_op, field_dot, eval_transitions)

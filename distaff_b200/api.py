@@ -287,3 +287,35 @@ def field_op(op, a, b=None, impl=0):
     out = np.empty_like(fa)
     backend.check(backend.lib().dg_field_op(code, impl, fa.ctypes.data, fb.ctypes.data if fb is not None else None, out.ctypes.data, fa.shape[0]))
     return out[:fa.shape[0] // 6] if op == "dot6" else out
+
+
+def field_dot(a, b, length):
+    """sum of `length` products per group, accumulated unreduced as the kernels do: (groups * length, 2) arrays -> (groups, 2)"""
+    fa = np.ascontiguousarray(a, dtype=np.uint64)
+    fb = np.ascontiguousarray(b, dtype=np.uint64)
+    assert fa.shape == fb.shape and fa.shape[0] % length == 0
+    out = np.empty((fa.shape[0] // length, 2), dtype=np.uint64)
+    backend.check(backend.lib().dg_field_dot(fa.ctypes.data, fb.ctypes.data, out.ctypes.data, out.shape[0], length))
+    return out
+
+
+def eval_transitions(ext, ctx_depth, loop_depth, stack_depth, blowup, seeds=None, coefs=None, check=False):
+    """The prover's constraint kernel on extended traces: ext (count, w, n * blowup, 2) uint64 in LDE order.  Entry i combines its
+    transition constraints with the coefficients drawn from seeds[i] (32 bytes) or, if given, coefs[i] ((2T, 2): coefA then coefB in
+    evaluation order).  Returns (values (count, 8n, 2) in step order, first_violation: per entry 0 or 1 + the lowest violating trace
+    step; only with check, which is the prover's trace-domain check)."""
+    a = np.ascontiguousarray(ext, dtype=np.uint64)
+    count, w, N = a.shape[0], a.shape[1], a.shape[2]
+    assert w == 15 + ctx_depth + loop_depth + stack_depth and N % blowup == 0
+    n = N // blowup
+    assert n & (n - 1) == 0 and blowup & (blowup - 1) == 0, "trace length and extension factor must be powers of 2"
+    T = 20 + max(ctx_depth, 1) + max(loop_depth, 1) + 2 + stack_depth
+    sd = b"".join(bytes(s) for s in seeds) if seeds is not None else None
+    cf = np.ascontiguousarray(coefs, dtype=np.uint64) if coefs is not None else None
+    assert (sd is not None and len(sd) == 32 * count) or (cf is not None and cf.shape == (count, 2 * T, 2))
+    out = np.empty((count, 8 * n, 2), dtype=np.uint64)
+    first = (backend.u32 * count)()
+    backend.check(backend.lib().dg_eval_transitions(a.ctypes.data, count, ctx_depth, loop_depth, stack_depth, n.bit_length() - 1,
+                                                   blowup.bit_length() - 1, sd, cf.ctypes.data if cf is not None else None,
+                                                   1 if check else 0, out.ctypes.data, first))
+    return out, list(first)

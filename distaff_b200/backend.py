@@ -74,6 +74,8 @@ EXPORTS = {
     "dg_merkle_build_with": [ctypes.c_int, vp, u64, vp],
     "dg_find_pow_nonce": [vp, u32, ctypes.POINTER(u64), vp],
     "dg_field_op": [ctypes.c_int, ctypes.c_int, vp, vp, vp, u64],
+    "dg_field_dot": [vp, vp, vp, u64, u32],
+    "dg_eval_transitions": [vp, u32, u32, u32, u32, u32, u32, vp, vp, ctypes.c_int, vp, ctypes.POINTER(u32)],
     "dg_dev_alloc": [ctypes.POINTER(vp), ctypes.c_size_t],
     "dg_dev_free": [vp],
     "dg_dev_upload": [vp, vp, ctypes.c_size_t],

@@ -524,7 +524,7 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], xpow_override ? xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
     if (!P.verify_mode && c8 == 0 && k != n - 1) {
-        if (acc.nonzero && live) atomicExch(P.violation + blockIdx.y, (unsigned)(k + 1));
+        if (acc.nonzero && live) atomicMax(P.violation + blockIdx.y, violation_word(k));
         t_res = ZERO;
     }
     if (live) P.t_ev[blockIdx.y * P.t_ev_stride + out_idx] = t_res;

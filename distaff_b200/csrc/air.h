@@ -16,7 +16,7 @@ struct AirParams {
     const fe *coefA, *coefB;            // per transition constraint (evaluation order): cc[2i], cc[2i+1] of its flattened slot
     TwiddleRef twN;                     // powers of the LDE root w_N
     unsigned long long inc[6];          // incremental degrees of the groups 2,3,4,6,7,8  (evaluator.rs:395-402)
-    unsigned *violation;                // set to step+1 when a trace-domain point violates a transition constraint
+    unsigned *violation;                // the lowest violating trace step, encoded by violation_word (0 = none)
     // verifier mode (verifier.cu): evaluate the transition combination at ONE out-of-domain point z -- the rows are (trace(z), trace(z g)),
     // the periodic values are the cycle polynomials at z^(n/16) and the degree-adjustment powers z^inc_g come from the host
     int verify_mode;
@@ -28,6 +28,11 @@ struct AirParams {
     // batched verification: proof q reads per_override / xpow_override + q * override_stride
     unsigned long long override_stride;
 };
+
+// A trace step k that violates a transition constraint is recorded as atomicMax(violation, 0xFFFFFFFF - k), so the lowest violating
+// step wins, as in the reference's sequential loop (prover.rs:52-64), and a max-reduce over ranks keeps it.  0 means no violation.
+__host__ __device__ inline unsigned violation_word(unsigned long long step) { return 0xFFFFFFFFu - (unsigned)step; }
+inline unsigned long long violation_step(unsigned word) { return 0xFFFFFFFFu - word; }
 
 // evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P) in one launch (blockIdx.y = proof);
 // traces of at least 16 steps

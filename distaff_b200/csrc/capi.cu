@@ -5,6 +5,7 @@
 #include "host_fs.h"
 #include "shard.h"
 #include "poly.h"
+#include "air.h"
 #include <thread>
 
 using namespace dg;
@@ -70,6 +71,18 @@ __global__ void field_op_kernel(int op, int impl, const fe *a, const fe *b, fe *
         }
     }
     out[i] = r;
+}
+
+// out[i] = sum_j a[len i + j] * b[len i + j] for a runtime len (1..128): the 288-bit accumulation of the constraint kernel's Acc and of
+// the per-register linear combinations, reduced once
+__global__ void field_dot_kernel(const fe *a, const fe *b, fe *out, unsigned long long groups, unsigned len) {
+    const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= groups) return;
+    const fe *x = a + i * len, *y = b + i * len;
+    fe_wide w;
+    wide_set(w, DG_MUL_WIDE(x[0], y[0]));
+    for (unsigned j = 1; j < len; j++) wide_add(w, DG_MUL_WIDE(x[j], y[j]));
+    out[i] = DG_REDUCE_WIDE(w);
 }
 
 __global__ void fill_kernel(uint4 *p, size_t n, unsigned v) {
@@ -319,6 +332,95 @@ int dg_field_op(int op, int impl, const uint8_t *a, const uint8_t *b, uint8_t *o
         DG_CUDA(cudaGetLastError());
         DG_CUDA(cudaMemcpyAsync(out, dout.p, n * 16, cudaMemcpyDeviceToHost, c.stream));
         DG_CUDA(cudaStreamSynchronize(c.stream));
+    });
+}
+int dg_field_dot(const uint8_t *a, const uint8_t *b, uint8_t *out, uint64_t groups, uint32_t len) {
+    return guarded([&] {
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DG_REQUIRE(a && b && out && groups >= 1, "invalid argument");
+        DG_REQUIRE(len >= 1 && len <= 128, "group length must be in 1..128");
+        const size_t n = groups * len;
+        DevBuf da(n * 16), db(n * 16), dout(groups * 16);
+        DG_CUDA(cudaMemcpyAsync(da.p, a, n * 16, cudaMemcpyHostToDevice, c.stream));
+        DG_CUDA(cudaMemcpyAsync(db.p, b, n * 16, cudaMemcpyHostToDevice, c.stream));
+        field_dot_kernel<<<(unsigned)((groups + 127) / 128), 128, 0, c.stream>>>(da.as<fe>(), db.as<fe>(), dout.as<fe>(), groups, len); c.launches++;
+        DG_CUDA(cudaGetLastError());
+        DG_CUDA(cudaMemcpyAsync(out, dout.p, groups * 16, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+    });
+}
+int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t log_n,
+                        uint32_t log_blowup, const uint8_t *seeds32, const uint8_t *coefs16, int check, uint8_t *out16, uint32_t *first_violation) {
+    return guarded([&] {
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DG_REQUIRE(ext16 && out16 && first_violation && (seeds32 || coefs16), "null argument");
+        DG_REQUIRE(count >= 1 && count <= 65535, "count must be in 1..65535");
+        DG_REQUIRE(ctx_depth <= 16 && loop_depth <= 8 && stack_depth >= 1 && stack_depth <= 32, "register shape out of range");
+        DG_REQUIRE(log_n >= 4 && log_blowup >= 4 && log_blowup <= 8 && log_n + log_blowup <= 20, "trace length or extension factor out of range");
+        const int w = 15 + ctx_depth + loop_depth + stack_depth;
+        const int T = 20 + std::max<int>(ctx_depth, 1) + std::max<int>(loop_depth, 1) + 2 + stack_depth;
+        const size_t n = (size_t)1 << log_n, b = (size_t)1 << log_blowup, N = n << log_blowup, E = 8 * n;
+
+        // per entry [coefA | coefB] in evaluation order, drawn as the prover draws them (no public inputs or outputs) or given
+        std::vector<fe> coef((size_t)count * 2 * T);
+        if (coefs16) {
+            memcpy(coef.data(), coefs16, coef.size() * 16);
+        } else {
+            const fe no_hash[2] = {fe_make(0, 0), fe_make(0, 0)};
+            for (uint32_t q = 0; q < count; q++) {
+                fs::ConstraintCoefficients cc = fs::draw_constraint_coefficients(seeds32 + 32 * (size_t)q, ctx_depth, loop_depth, stack_depth, {}, {},
+                                                                                 fe_make(0, 0), no_hash);
+                DG_REQUIRE(cc.coefA.size() == (size_t)T, "transition constraint count mismatch");
+                std::copy(cc.coefA.begin(), cc.coefA.end(), coef.begin() + (size_t)q * 2 * T);
+                std::copy(cc.coefB.begin(), cc.coefB.end(), coef.begin() + (size_t)q * 2 * T + T);
+            }
+        }
+        // logical LDE order (index k * b + c) -> the prover's coset-major slab ([c][k])
+        std::vector<fe> slab((size_t)count * w * N);
+        for (size_t col = 0; col < (size_t)count * w; col++)
+            for (size_t k = 0; k < n; k++)
+                for (size_t cs = 0; cs < b; cs++) memcpy(&slab[col * N + cs * n + k], ext16 + (col * N + k * b + cs) * 16, 16);
+
+        if (!c.d_periodic.p) {
+            std::vector<fe> per = fs::periodic_tables();
+            c.d_periodic.alloc(per.size() * 16, true);
+            DG_CUDA(cudaMemcpyAsync(c.d_periodic.p, per.data(), per.size() * 16, cudaMemcpyHostToDevice, c.stream));
+            DG_CUDA(cudaStreamSynchronize(c.stream));
+        }
+        DevBuf d_ext(slab.size() * 16), d_coef(coef.size() * 16), d_out((size_t)count * E * 16), d_violation((size_t)4 * count);
+        DG_CUDA(cudaMemcpyAsync(d_ext.p, slab.data(), slab.size() * 16, cudaMemcpyHostToDevice, c.stream));
+        DG_CUDA(cudaMemcpyAsync(d_coef.p, coef.data(), coef.size() * 16, cudaMemcpyHostToDevice, c.stream));
+        DG_CUDA(cudaMemsetAsync(d_violation.p, 0, (size_t)4 * count, c.stream));
+        AirParams P;
+        memset(&P, 0, sizeof P);
+        P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
+        P.cl = std::max<int>(ctx_depth, 1); P.ll = std::max<int>(loop_depth, 1); P.sl = std::max<int>(stack_depth, 8);
+        P.log_n = log_n; P.log_blowup = log_blowup;
+        P.ext = d_ext.as<fe>(); P.col_stride = N;
+        P.c8_base = 0; P.num_c8 = 8;
+        P.t_ev = d_out.as<fe>();
+        P.periodic = c.d_periodic.as<fe>();
+        P.coefA = d_coef.as<fe>(); P.coefB = d_coef.as<fe>() + T;
+        P.twN = c.twiddle(log_n + log_blowup, false);
+        static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
+        for (int gi = 0; gi < 6; gi++) P.inc[gi] = (8 * n - 1) - (n - 1) * GROUP_DEG[gi];
+        P.violation = d_violation.as<unsigned>();
+        P.verify_mode = check ? 0 : 1;          // verify mode: no trace-domain check, a value at every step
+        P.ext_stride = (size_t)w * N; P.t_ev_stride = E; P.coef_stride = 2 * T;
+        launch_constraint_eval(c, P, (int)count);
+
+        std::vector<fe> t_ev((size_t)count * E);
+        std::vector<unsigned> violation(count);
+        DG_CUDA(cudaMemcpyAsync(t_ev.data(), d_out.p, t_ev.size() * 16, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaMemcpyAsync(violation.data(), d_violation.p, (size_t)4 * count, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+        // coset-major [c8][k] -> step order s = 8 k + c8
+        for (size_t q = 0; q < count; q++)
+            for (size_t c8 = 0; c8 < 8; c8++)
+                for (size_t k = 0; k < n; k++) memcpy(out16 + (q * E + 8 * k + c8) * 16, &t_ev[q * E + c8 * n + k], 16);
+        for (uint32_t q = 0; q < count; q++) first_violation[q] = violation[q] ? (uint32_t)violation_step(violation[q]) + 1 : 0;
     });
 }
 

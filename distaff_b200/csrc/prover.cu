@@ -502,7 +502,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         d2h(c, violation.data(), d_violation.p, (size_t)4 * K);
         for (int p = 0; p < K; p++)
             if (violation[p])
-                ps[p].fail(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation[p] - 1) + " were not satisfied");
+                ps[p].fail(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation_step(violation[p])) + " were not satisfied");
         if (!any_live()) return;
         // interpolation of the transition combination (constraint_table.rs:54-63), coset by coset: size-n inverse transforms of the own
         // cosets (sharded), all-gather, then the 8-point inverse DFT across cosets (poly.cu: coset_interp_finish) -> the 8n coefficients

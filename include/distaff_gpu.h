@@ -171,6 +171,18 @@ int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uin
 /* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b)), for differential tests of the arithmetic;
  * impl: 0 = PTX path used by the kernels, 1 = portable C++ path, 2 / 3 = earlier PTX multiplies (op 2 only) */
 int dg_field_op(int op, int impl, const uint8_t *a, const uint8_t *b, uint8_t *out, uint64_t n);
+/* out[i] = sum_j a[len*i + j] * b[len*i + j], j < len (1..128), accumulated unreduced in 288 bits and reduced once, as the kernels' dot
+ * products and constraint accumulators are; for differential tests of the arithmetic */
+int dg_field_dot(const uint8_t *a, const uint8_t *b, uint8_t *out, uint64_t groups, uint32_t len);
+/* The prover's constraint-evaluation kernel on a supplied extended trace, for differential tests of the AIR.  ext16 holds count entries
+ * of w = 15 + ctx_depth + loop_depth + stack_depth columns of n << log_blowup elements each, in LDE order (what TraceTable::extend gives).
+ * Entry i combines its transition constraints with the coefficients the prover draws from seeds32[32 i] (ConstraintCoefficients
+ * without public inputs or outputs), or, when coefs16 is not NULL, with coefs16[2T i ..] = [coefA | coefB] of its T constraints in
+ * evaluation order.  All entries run in one launch.  out16 receives count x 8n values in step order.  check = 0 evaluates every step
+ * (no trace-domain check); check = 1 is the prover's check: trace-domain steps other than the last give 0, and first_violation[i] is
+ * 1 + the lowest trace step whose constraints do not all vanish, or 0. */
+int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t log_n,
+                        uint32_t log_blowup, const uint8_t *seeds32, const uint8_t *coefs16, int check, uint8_t *out16, uint32_t *first_violation);
 
 /* ---- device-resident variants (timed with CUDA events on the library's stream; *ms may be NULL) ----------------------- */
 int dg_dev_alloc(void **ptr, size_t bytes);

@@ -257,6 +257,43 @@ uint32_t or_eval_transition_raw(const uint8_t *cur_row, const uint8_t *next_row,
     memcpy(out, ev.data(), ev.size() * 16);
     return (uint32_t)ev.size();
 }
+// the prover's stage-3 transition loop (stark.h prove, prover.rs:52-64) over a supplied extended trace: ext = w columns of n * blowup
+// elements in LDE order; the Evaluator's coefficients come from seed32, with no public inputs or outputs.  check = 1: the prover's loop,
+// which returns 1 with its error message (lowest failing step) in err when a trace-domain step does not vanish, else 0 and
+// evaluate_transition at every step; check = 0: combine_transition_constraints at every step, without the trace-domain assertion.
+// out: 8n values in step order.
+int or_eval_transitions(const uint8_t *ext16, uint32_t cd, uint32_t ldp, uint32_t sd, uint64_t n, uint32_t blowup, const uint8_t *seed32,
+                        int check, uint8_t *out16, char *err, uint32_t err_cap) {
+    try {
+        const size_t w = 15 + cd + ldp + sd, N = n * blowup, E = n * MAX_CONSTRAINT_DEGREE, stride = blowup / MAX_CONSTRAINT_DEGREE;
+        std::vector<std::vector<u128>> ext(w, std::vector<u128>(N));
+        for (size_t j = 0; j < w; j++) memcpy(ext[j].data(), ext16 + j * N * 16, N * 16);
+        const u128 no_hash[2] = {0, 0};
+        Evaluator evaluator(n, MAX_CONSTRAINT_DEGREE, E, cd, ldp, sd, seed32, no_hash, 0, {}, {});
+        std::vector<u128> lde_domain = field::get_power_series(field::get_root_of_unity(N), N);
+        TraceState cur(cd, ldp, sd), nxt(cd, ldp, sd);
+        std::vector<u128> ev(evaluator.t_constraint_num);
+        for (size_t step = 0; step < E; step++) {
+            const size_t i = step * stride;
+            cur.from_columns(ext, i);
+            nxt.from_columns(ext, (i + blowup) % N);
+            u128 t;
+            if (check) {
+                t = evaluator.evaluate_transition(cur, nxt, lde_domain[i], step);
+            } else {
+                std::fill(ev.begin(), ev.end(), 0);
+                evaluator.decoder.evaluate(cur, nxt, step, ev.data());
+                evaluator.stack.evaluate(cur, nxt, step, ev.data() + evaluator.decoder.constraint_count());
+                t = evaluator.combine_transition_constraints(ev, lde_domain[i]);
+            }
+            st(out16 + step * 16, t);
+        }
+        return 0;
+    } catch (const std::exception &e) {
+        if (err && err_cap) { strncpy(err, e.what(), err_cap - 1); err[err_cap - 1] = 0; }
+        return 1;
+    }
+}
 // Decoder::evaluate with explicit periodic values (ark[8], masks[3]) instead of a step: what the reference's unit tests of
 // enforce_op_bits / enforce_hacc pass in (decoder/op_bits.rs, decoder/sponge.rs mod tests)
 uint32_t or_decoder_run_raw(const uint8_t *cur_row, const uint8_t *next_row, uint32_t cd, uint32_t ldp, uint32_t sd,

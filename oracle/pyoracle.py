@@ -69,6 +69,9 @@ def lib():
         L.or_eval_transition_raw.restype = ctypes.c_uint32
         L.or_eval_transition_raw.argtypes = [u8p, u8p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_uint64, u8p]
         L.or_op_flags.argtypes = [u8p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, u8p]
+        L.or_eval_transitions.restype = ctypes.c_int
+        L.or_eval_transitions.argtypes = [u8p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_uint32, u8p, ctypes.c_int,
+                                          u8p, ctypes.c_char_p, ctypes.c_uint32]
         L.or_decoder_run_raw.restype = ctypes.c_uint32
         L.or_decoder_run_raw.argtypes = [u8p, u8p, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, u8p, u8p, u8p]
         L.or_enforce_left_shift.restype = None
@@ -235,6 +238,30 @@ def prove(registers, ctx_depth, loop_depth, inputs, outputs, ext=32, num_queries
     h = lib().or_prove(regs.ctypes.data, w, n, ctx_depth, loop_depth, fi.ctypes.data, len(fi), fo.ctypes.data, len(fo),
                        ext, num_queries, grinding, 1 if keep_large else 0)
     return ProveResult(h)
+
+
+def extend(registers, blowup):
+    """TraceTable::extend (trace_table.rs:143-169): (w, n, 2) register traces -> (w, n * blowup, 2) evaluations in LDE order"""
+    regs = np.ascontiguousarray(registers, dtype=np.uint64)
+    w, n = regs.shape[0], regs.shape[1]
+    out = np.zeros((w, n * blowup, 2), dtype=np.uint64)
+    for j in range(w):
+        out[j, :n] = fft(regs[j], inverse=True)
+        out[j] = fft(out[j])
+    return out
+
+
+def eval_transitions(ext, ctx_depth, loop_depth, stack_depth, blowup, seed, check):
+    """The prover's transition loop over an extended trace: ext (w, n * blowup, 2) uint64 in LDE order, coefficients drawn from the
+    32-byte seed.  Returns (values, error): values (8n, 2) in step order; error None, or with check the prover's message for the lowest
+    failing step (values then None)."""
+    a = np.ascontiguousarray(ext, dtype=np.uint64)
+    n = a.shape[1] // blowup
+    out = np.zeros((8 * n, 2), dtype=np.uint64)
+    err = ctypes.create_string_buffer(512)
+    rc = lib().or_eval_transitions(a.ctypes.data, ctx_depth, loop_depth, stack_depth, n, blowup, bytes(seed), 1 if check else 0,
+                                   out.ctypes.data, err, 512)
+    return (None, err.value.decode()) if rc else (out, None)
 
 
 def verify(program_hash, inputs, outputs, proof):

@@ -238,3 +238,30 @@ def test_trace_state_layout_reference_vectors(po):
     base = [101, 1, 2, 3, 4, 1, 1, 1]
     for bits, code in (([0] * 7, 0), ([1] * 7, 127), ([1, 1, 1, 1, 1, 1, 0], 63), ([1, 0, 0, 0, 0, 1, 1], 97)):
         assert fields(1, 0, 2, base + bits + [15, 16, 17])[-1] == code
+
+
+def test_eval_transitions_is_the_provers_transition_loop(po):
+    """or_eval_transitions over the extended trace: with the trace root as seed it gives the prover's t_evals; on a trace corrupted at
+    two separated steps it fails with the prover's message, which names the lowest violating step; without the check it gives a value
+    at every step"""
+    import re
+    from distaff_b200 import hostvm
+    tr = hostvm.fibonacci(13)
+    n, b = tr.length, 16
+    ref = po.prove(tr.registers, tr.ctx_depth, tr.loop_depth, tr.public_inputs, tr.outputs, ext=b, num_queries=8, grinding=0, keep_large=True)
+    assert ref.error is None
+    ext = po.extend(tr.registers, b)
+    assert all(np.array_equal(ext[j], ref.vector("extended", j)) for j in range(tr.width))
+    vals, err = po.eval_transitions(ext, tr.ctx_depth, tr.loop_depth, tr.stack_depth, b, ref.digest("trace_root"), check=True)
+    assert err is None and np.array_equal(vals, ref.vector("t_evals"))
+    assert not vals[0:8 * (n - 1):8].any() and vals[8 * (n - 1)].any()
+
+    regs = tr.registers.copy()
+    regs[tr.width - 1, 201, 0] += 1                 # transitions 200 and 201 break
+    regs[tr.width - 1, 41, 0] += 1                  # transitions 40 and 41 break
+    bad = po.prove(regs, tr.ctx_depth, tr.loop_depth, tr.public_inputs, tr.outputs, ext=b, num_queries=8, grinding=0)
+    assert bad.error is not None and re.search(r"\bstep 40\b", bad.error), bad.error
+    vals, err = po.eval_transitions(po.extend(regs, b), tr.ctx_depth, tr.loop_depth, tr.stack_depth, b, bytes(32), check=True)
+    assert vals is None and err == bad.error
+    vals, err = po.eval_transitions(po.extend(regs, b), tr.ctx_depth, tr.loop_depth, tr.stack_depth, b, bytes(32), check=False)
+    assert err is None and vals[8 * 40].any() and vals[8 * 201].any()
