@@ -71,15 +71,29 @@ __device__ __forceinline__ fe is_bin(fe v) { return fe_sub(fe_sqr(v), v); }
 // degree groups in ascending order of constraint degree: 2, 3, 4, 6, 7, 8  (evaluator.rs:385-406)
 enum { G2 = 0, G3 = 1, G4 = 2, G6 = 3, G7 = 4, G8 = 5 };
 
+// sums of products accumulated unreduced (fe_wide: fewer than 128 products of canonical operands)
+__device__ __forceinline__ void wide_first(fe_wide &w, fe a, fe b) { wide_set(w, DG_MUL_WIDE(a, b)); }
+__device__ __forceinline__ void wide_mac(fe_wide &w, fe a, fe b) { wide_add(w, DG_MUL_WIDE(a, b)); }
+
+// The combination  sum_i v_i * cA_i + sum_g (sum_{i in g} v_i * cB_i) * x^inc_g  (evaluator.rs:335-358).  The constraints are evaluated
+// group by group, so each degree group is one run: its cB side is accumulated unreduced in `run`, reduced once when the run closes and
+// multiplied by x^inc_g into `res`, which is reduced once at the end.  Bounds (products per accumulator, all operands canonical):
+//   res: one per constraint (at most 20 + 16 + 8 + 2 + 32 = 78) + one per group (6) = 84;
+//   run: the longest runs are G7 (sponge 1, 2 aux, at most 32 stack slots: 35) and G4 (align, image, at most 16 context and 8 loop
+//   entries: 26).  launch_constraint_eval checks cl <= 16, ll <= 8, sl <= 32.
 struct Acc {
-    fe_wide res;                        // sum_i v_i * cA_i, unreduced (at most 78 constraints < 128 products)
-    fe adj[6];
-    bool nonzero, first;
-    __device__ __forceinline__ void fold(int group, fe v, fe a, fe b) {
-        if (first) { wide_set(res, DG_MUL_WIDE(v, a)); first = false; }
-        else wide_add(res, DG_MUL_WIDE(v, a));
-        adj[group] = fe_add(adj[group], fe_mul(v, b));
+    fe_wide res, run;
+    bool nonzero, first, run_first;
+    __device__ __forceinline__ void fold(fe v, fe a, fe b) {
+        if (first) { wide_first(res, v, a); first = false; }
+        else wide_mac(res, v, a);
+        if (run_first) { wide_first(run, v, b); run_first = false; }
+        else wide_mac(run, v, b);
         nonzero = nonzero || !fe_is_zero(v);
+    }
+    __device__ __forceinline__ void close(fe xpow) {
+        wide_mac(res, DG_REDUCE_WIDE(run), xpow);
+        run_first = true;
     }
 };
 
@@ -180,46 +194,45 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 
     Acc acc;
     acc.first = true;
-#pragma unroll
-    for (int g = 0; g < 6; g++) acc.adj[g] = ZERO;
+    acc.run_first = true;
     acc.nonzero = false;
     // the proof's coefficients are read at each use: pointers to them held across the body would add live registers
-    auto fold = [&](int idx, int group, fe v) {
+    auto fold = [&](int idx, fe v) {
         const unsigned long long at = idx + blockIdx.y * P.coef_stride;
-        acc.fold(group, v, P.coefA[at], P.coefB[at]);
+        acc.fold(v, P.coefA[at], P.coefB[at]);
+    };
+    // closes the run of degree group g: x^inc_g is the host's value at the verifier's point, else a power of the LDE root
+    auto close = [&](int g) {
+        acc.close(P.xpow_override ? P.xpow_override[blockIdx.y * P.override_stride + g] : tw_pow(P.twN, lde_index * P.inc[g]));
     };
 
     const fe *per = P.per_override ? P.per_override + blockIdx.y * P.override_stride
                                    : P.periodic + (s & 127ULL) * 23;     // [ark_sponge 8][masks 3][ark_hasher 12]
 
     DG_STEP();
-    // ---- decoder: op bits (decoder/op_bits.rs:10-79), constraints 0..14 -------------------------------------------------------
+    // ---- decoder: op bits (decoder/op_bits.rs:10-79), constraints 0..13 -------------------------------------------------------
     {
         fe cf_sum = ZERO, ld_prod = ONE, hd_prod = ONE;
 #pragma unroll
-        for (int i = 0; i < 3; i++) { fold(i, G2, is_bin(cf(i))); cf_sum = fe_add(cf_sum, cf(i)); }
+        for (int i = 0; i < 3; i++) { fold(i, is_bin(cf(i))); cf_sum = fe_add(cf_sum, cf(i)); }
 #pragma unroll
-        for (int i = 0; i < 5; i++) { fold(3 + i, G2, is_bin(ld(i))); ld_prod = fe_mul(ld_prod, ld(i)); }
+        for (int i = 0; i < 5; i++) { fold(3 + i, is_bin(ld(i))); ld_prod = fe_mul(ld_prod, ld(i)); }
 #pragma unroll
-        for (int i = 0; i < 2; i++) { fold(8 + i, G2, is_bin(hd(i))); hd_prod = fe_mul(hd_prod, hd(i)); }
-        fe is_hacc = cff[0];
-        fe hacc_t = fe_mul(fe_add(op_counter, ONE), is_hacc);
-        fe rest_t = fe_mul(op_counter, bnot(is_hacc));
-        fold(10, G3, fe_sub(fe_add(hacc_t, rest_t), DNXT(0)));
-        fold(11, G8, fe_mul(op_counter, fe_mul(bnot(ld_prod), bnot(hd_prod))));
-        fold(12, G8, fe_mul(cf_sum, bnot(fe_mul(ld_prod, hd_prod))));
-        fold(13, G6, fe_mul(cff[7], bnot(next_void)));
-        fe prefix = fe_add(fe_add(cff[1], cff[4]), fe_add(cff[5], cff[6]));      // BEGIN, LOOP, WRAP, BREAK
-        fe align = fe_mul(prefix, per[8 + 1]);
-        align = fe_add(align, fe_mul(fe_add(cff[2], cff[3]), per[8 + 0]));       // TEND, FEND
-        align = fe_add(align, fe_mul(hdf[0], per[8 + 2]));                        // PUSH
-        fold(14, G4, align);
+        for (int i = 0; i < 2; i++) { fold(8 + i, is_bin(hd(i))); hd_prod = fe_mul(hd_prod, hd(i)); }
+        close(G2);
+        // (op_counter + 1) * hacc + op_counter * (1 - hacc) = op_counter + hacc
+        fold(10, fe_sub(fe_add(op_counter, cff[0]), DNXT(0)));
+        close(G3);
+        fold(11, fe_mul(op_counter, fe_mul(bnot(ld_prod), bnot(hd_prod))));
+        fold(12, fe_mul(cf_sum, bnot(fe_mul(ld_prod, hd_prod))));
+        close(G8);
     }
 
     DG_STEP();
     // ---- decoder: sponge / flow ops (decoder/sponge.rs, flow_ops.rs) --------------------------------------------------------------
+    fe r_sp1;                                   // sponge 1 is a degree-7 constraint: folded with the stack's run
     {
-        fe r_sp[4], r_img;
+        fold(13, fe_mul(cff[7], bnot(next_void)));
         // HACC
         {
             fe f = cff[0];
@@ -241,47 +254,53 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
             matvec<4>(c_sponge_inv_mds, ns);
 #pragma unroll
             for (int i = 0; i < 4; i++) ns[i] = fe_sub(fe_cube(ns[i]), per[4 + i]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_mul(f, fe_sub(os[i], ns[i]));
+            DG_STEP();
+            // sponge register i: HACC f * (os[i] - ns[i]); BEGIN, LOOP, WRAP clear the sponge (flag sum * new_sponge[i]); TEND / FEND;
+            // BREAK / VOID keep the sponge.  One unreduced sum of four products per register
+            const fe fclr = fe_add(fe_add(cff[1], cff[4]), cff[5]);
+            const fe ft = cff[2], ff = cff[3], fb = fe_add(ft, ff), fk = fe_add(cff[6], cff[7]);
+            auto sponge = [&](const int i) -> fe {
+                fe_wide w;
+                wide_first(w, f, fe_sub(os[i], ns[i]));
+                wide_mac(w, fclr, nsp(i));
+                if (i == 0) wide_mac(w, fb, fe_sub(C_CTX(0), nsp(0)));
+                if (i == 1) wide_mac(w, ft, fe_sub(sp(0), nsp(1)));
+                if (i == 2) wide_mac(w, ff, fe_sub(sp(0), nsp(2)));
+                if (i == 3) wide_mac(w, fb, nsp(3));
+                wide_mac(w, fk, fe_sub(sp(i), nsp(i)));
+                return DG_REDUCE_WIDE(w);
+            };
+            fold(15, sponge(0));
+            fold(17, sponge(2));
+            fold(18, sponge(3));
+            close(G6);
+            r_sp1 = sponge(1);
         }
-        DG_STEP();
-        // BEGIN, LOOP, WRAP clear the sponge: flag sum * new_sponge[i]
+    }
+
+    DG_STEP();
+    // ---- decoder: alignment, loop image, context and loop stacks: the degree-4 run ------------------------------------------------
+    {
         {
-            fe fclr = fe_add(fe_add(cff[1], cff[4]), cff[5]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_add(r_sp[i], fe_mul(fclr, nsp(i)));
+            fe_wide w;
+            wide_first(w, fe_add(fe_add(cff[1], cff[4]), fe_add(cff[5], cff[6])), per[8 + 1]);     // BEGIN, LOOP, WRAP, BREAK
+            wide_mac(w, fe_add(cff[2], cff[3]), per[8 + 0]);                                       // TEND, FEND
+            wide_mac(w, hdf[0], per[8 + 2]);                                                       // PUSH
+            fold(14, DG_REDUCE_WIDE(w));
         }
-        DG_STEP();
-        // TEND / FEND
-        {
-            fe ft = cff[2], ff = cff[3], fb = fe_add(ft, ff);
-            r_sp[0] = fe_add(r_sp[0], fe_mul(fb, fe_sub(C_CTX(0), nsp(0))));
-            r_sp[1] = fe_add(r_sp[1], fe_mul(ft, fe_sub(sp(0), nsp(1))));
-            r_sp[2] = fe_add(r_sp[2], fe_mul(ff, fe_sub(sp(0), nsp(2))));
-            r_sp[3] = fe_add(r_sp[3], fe_mul(fb, nsp(3)));
-        }
-        // BREAK / VOID keep the sponge
-        {
-            fe fk = fe_add(cff[6], cff[7]);
-#pragma unroll
-            for (int i = 0; i < 4; i++) r_sp[i] = fe_add(r_sp[i], fe_mul(fk, fe_sub(sp(i), nsp(i))));
-        }
-        fold(15, G6, r_sp[0]); fold(16, G7, r_sp[1]); fold(17, G6, r_sp[2]); fold(18, G6, r_sp[3]);
         // loop image (WRAP, BREAK)
-        r_img = fe_mul(fe_add(cff[5], cff[6]), fe_sub(sp(0), C_LOOP(0)));
-        fold(19, G4, r_img);
+        fold(19, fe_mul(fe_add(cff[5], cff[6]), fe_sub(sp(0), C_LOOP(0))));
 
         DG_STEP();
         // context stack: BEGIN/LOOP push (right shift 1, slot 0 = parent hash), TEND/FEND pop (left shift 1), WRAP/BREAK/VOID copy
         {
             fe f_push = fe_add(cff[1], cff[4]), f_pop = fe_add(cff[2], cff[3]), f_copy = fe_add(fe_add(cff[5], cff[6]), cff[7]);
             for (int i = 0; i < cl; i++) {
-                fe v = fe_mul(f_copy, fe_sub(C_CTX(i), N_CTX(i)));
-                if (i == 0) v = fe_add(v, fe_mul(f_push, fe_sub(sp(0), N_CTX(0))));
-                else v = fe_add(v, fe_mul(f_push, fe_sub(C_CTX(i - 1), N_CTX(i))));
-                if (i < cl - 1) v = fe_add(v, fe_mul(f_pop, fe_sub(C_CTX(i + 1), N_CTX(i))));
-                else v = fe_add(v, fe_mul(f_pop, N_CTX(i)));
-                fold(20 + i, G4, v);
+                fe_wide w;
+                wide_first(w, f_copy, fe_sub(C_CTX(i), N_CTX(i)));
+                wide_mac(w, f_push, fe_sub(i == 0 ? sp(0) : C_CTX(i - 1), N_CTX(i)));
+                wide_mac(w, f_pop, i < cl - 1 ? fe_sub(C_CTX(i + 1), N_CTX(i)) : N_CTX(i));
+                fold(20 + i, DG_REDUCE_WIDE(w));
             }
         }
         DG_STEP();
@@ -290,13 +309,14 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
             fe f_copy = fe_add(fe_add(fe_add(cff[1], cff[2]), fe_add(cff[3], cff[5])), cff[7]);
             fe f_rs = cff[4], f_ls = cff[6];
             for (int i = 0; i < ll; i++) {
-                fe v = fe_mul(f_copy, fe_sub(C_LOOP(i), N_LOOP(i)));
-                if (i >= 1) v = fe_add(v, fe_mul(f_rs, fe_sub(C_LOOP(i - 1), N_LOOP(i))));
-                if (i < ll - 1) v = fe_add(v, fe_mul(f_ls, fe_sub(C_LOOP(i + 1), N_LOOP(i))));
-                else v = fe_add(v, fe_mul(f_ls, N_LOOP(i)));
-                fold(20 + cl + i, G4, v);
+                fe_wide w;
+                wide_first(w, f_copy, fe_sub(C_LOOP(i), N_LOOP(i)));
+                if (i >= 1) wide_mac(w, f_rs, fe_sub(C_LOOP(i - 1), N_LOOP(i)));
+                wide_mac(w, f_ls, i < ll - 1 ? fe_sub(C_LOOP(i + 1), N_LOOP(i)) : N_LOOP(i));
+                fold(20 + cl + i, DG_REDUCE_WIDE(w));
             }
         }
+        close(G4);
     }
 
     {
@@ -335,22 +355,21 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         const fe f_push = hdf[0], f_cmp = hdf[1], f_rescr = hdf[2];
 
         DG_STEP();
+        // the degree-7 run: sponge 1, the auxiliary constraints, every stack slot
+        fold(16, r_sp1);
         // --- auxiliary constraints
-        fe aux0, aux1;
         {
-            aux0 = fe_mul(f_assert, fe_sub(ONE, O(0)));
-            aux0 = fe_add(aux0, fe_mul(f_asserteq, fe_sub(O(0), O(1))));
-            fe b0 = is_bin(O(0)), b1 = is_bin(O(1));
-            fe f_ao = fe_add(f_and, f_or);
-            aux0 = fe_add(aux0, fe_mul(fe_add(f_not, f_ao), b0));
-            aux1 = fe_mul(f_ao, b1);
-            fe diff = fe_sub(O(1), O(2));
-            aux0 = fe_add(aux0, fe_mul(f_eq, fe_mul(NW(0), diff)));
-            aux0 = fe_add(aux0, fe_mul(f_choose, is_bin(O(2))));
-            aux0 = fe_add(aux0, fe_mul(fe_add(f_choose2, f_cswap2), is_bin(O(4))));
+            const fe f_ao = fe_add(f_and, f_or);
+            fe_wide w;
+            wide_first(w, f_assert, fe_sub(ONE, O(0)));
+            wide_mac(w, f_asserteq, fe_sub(O(0), O(1)));
+            wide_mac(w, fe_add(f_not, f_ao), is_bin(O(0)));
+            wide_mac(w, f_eq, fe_mul(NW(0), fe_sub(O(1), O(2))));
+            wide_mac(w, f_choose, is_bin(O(2)));
+            wide_mac(w, fe_add(f_choose2, f_cswap2), is_bin(O(4)));
+            fold(base, DG_REDUCE_WIDE(w));
+            fold(base + 1, fe_mul(f_ao, is_bin(O(1))));
         }
-        fold(base, G7, aux0);
-        fold(base + 1, G7, aux1);
 
         DG_STEP();
         // --- per-slot shift structure.  For slot i the generic contribution of an operation is
@@ -358,7 +377,6 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         //        right shift s: f * (O(i-s) - n[i])                   when i >= s
         //        left shift s from slot `from`: f * (O(i+s) - n[i])   when from-s <= i < L-s, and f * n[i] when i >= L-s
         //     flags with the same shape are summed first.
-        fe ev[8];
         const fe f_copy0 = fe_add(begin_flag, noop_flag);                                   // from 0
         const fe f_copy1 = fe_add(fe_add(f_inv, f_neg), f_not);                              // from 1
         const fe f_copy2 = f_swap;                                                           // from 2
@@ -375,129 +393,37 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
         const fe f_ls2_4 = f_cswap2;                                                         // left 2, start slot 4
         const fe f_ls4_0 = f_drop4;                                                          // left 4, start slot 0
         const fe f_ls4_2 = f_choose2;                                                        // left 4, start slot 2
-        // generic part of slot i; fc / fl1 / fl2 / fl4 are the copy and left-shift flag sums that apply to this slot
-        auto slot_value = [&](const int i, const fe fc, const fe fl1, const fe fl2, const fe fl4) -> fe {
+        // slot i's seven shift products open its unreduced sum; fc / fl1 / fl2 / fl4 are the copy and left-shift flag sums that apply
+        // to this slot
+        auto slot_shifts = [&](fe_wide &w, const int i, const fe fc, const fe fl1, const fe fl2, const fe fl4) {
             const fe nwi = NW(i);
-            // the seven products of a slot are accumulated unreduced (288 bits) and reduced once: 7 x (product + 9-limb add) + 1 reduction
-            // instead of 7 x (modular product + modular add)
-            fe_wide acc7;
-            wide_set(acc7, DG_MUL_WIDE(fc, fe_sub(O(i), nwi)));
-            if (i >= 1) wide_add(acc7, DG_MUL_WIDE(f_rs1, fe_sub(O(i - 1), nwi)));
-            if (i >= 2) wide_add(acc7, DG_MUL_WIDE(f_rs2, fe_sub(O(i - 2), nwi)));
-            if (i >= 4) wide_add(acc7, DG_MUL_WIDE(f_rs4, fe_sub(O(i - 4), nwi)));
-            wide_add(acc7, DG_MUL_WIDE(fl1, (i < L - 1) ? fe_sub(O(i + 1), nwi) : nwi));
-            wide_add(acc7, DG_MUL_WIDE(fl2, (i < L - 2) ? fe_sub(O(i + 2), nwi) : nwi));
-            wide_add(acc7, DG_MUL_WIDE(fl4, (i < L - 4) ? fe_sub(O(i + 4), nwi) : nwi));
-            return DG_REDUCE_WIDE(acc7);
+            wide_first(w, fc, fe_sub(O(i), nwi));
+            if (i >= 1) wide_mac(w, f_rs1, fe_sub(O(i - 1), nwi));
+            if (i >= 2) wide_mac(w, f_rs2, fe_sub(O(i - 2), nwi));
+            if (i >= 4) wide_mac(w, f_rs4, fe_sub(O(i - 4), nwi));
+            wide_mac(w, fl1, (i < L - 1) ? fe_sub(O(i + 1), nwi) : nwi);
+            wide_mac(w, fl2, (i < L - 2) ? fe_sub(O(i + 2), nwi) : nwi);
+            wide_mac(w, fl4, (i < L - 4) ? fe_sub(O(i + 4), nwi) : nwi);
         };
-        fe fc_hi, fl1_hi, fl2_hi, fl4_hi;                  // the sums for slots >= 8 (every shape applies)
+        auto slot_fold = [&](const int i, const fe_wide &w) {
+            if (i < P.stack_depth) fold(base + 2 + i, DG_REDUCE_WIDE(w));
+        };
+
+        // slots >= 8 carry no operation-specific terms (every shape applies)
         {
-            fe fc = f_copy0, fl1 = f_ls1_0, fl2 = f_ls2_0, fl4 = f_ls4_0;
-#pragma unroll
-            for (int i = 0; i < 8; i++) {
-                if (i == 1) { fc = fe_add(fc, f_copy1); fl1 = fe_add(fl1, f_ls1_1); fl2 = fe_add(fl2, f_ls2_1); }
-                if (i == 2) { fc = fe_add(fc, f_copy2); fl4 = fe_add(fl4, f_ls4_2); }
-                if (i == 4) { fc = fe_add(fc, f_copy4); fl2 = fe_add(fl2, f_ls2_4); }
-                if (i == 6) fc = fe_add(fc, f_copy6);
-                ev[i] = slot_value(i, fc, fl1, fl2, fl4);
-                if (i & 1) DG_STEP();
+            const fe fc_hi = fe_add(fe_add(fe_add(f_copy0, f_copy1), fe_add(f_copy2, f_copy4)), fe_add(f_copy6, f_copy8));
+            const fe fl1_hi = fe_add(f_ls1_0, f_ls1_1), fl2_hi = fe_add(fe_add(f_ls2_0, f_ls2_1), f_ls2_4), fl4_hi = fe_add(f_ls4_0, f_ls4_2);
+            for (int i = 8; i < L; i++) {
+                fe_wide w;
+                slot_shifts(w, i, fc_hi, fl1_hi, fl2_hi, fl4_hi);
+                slot_fold(i, w);
+                DG_STEP();
             }
-            fc_hi = fe_add(fc, f_copy8); fl1_hi = fl1; fl2_hi = fl2; fl4_hi = fl4;
         }
-        // slots >= 8 carry no operation-specific terms: evaluate and fold them straight away (no per-thread array)
-        for (int i = 8; i < L; i++) {
-            fold(base + 2 + i, G7, slot_value(i, fc_hi, fl1_hi, fl2_hi, fl4_hi));
-            DG_STEP();
-        }
-        DG_STEP();
-        // --- operation-specific constraints on the low slots
-        // dup / dup2 / dup4: new[k] == old[k]
-        ev[0] = fe_add(ev[0], fe_mul(fe_add(fe_add(f_dup, f_dup2), f_dup4), fe_sub(NW(0), O(0))));
-        ev[1] = fe_add(ev[1], fe_mul(fe_add(f_dup2, f_dup4), fe_sub(NW(1), O(1))));
-        ev[2] = fe_add(ev[2], fe_mul(f_dup4, fe_sub(NW(2), O(2))));
-        ev[3] = fe_add(ev[3], fe_mul(f_dup4, fe_sub(NW(3), O(3))));
-        // pad2
-        ev[0] = fe_add(ev[0], fe_mul(f_pad2, NW(0)));
-        ev[1] = fe_add(ev[1], fe_mul(f_pad2, NW(1)));
-        // swap: both constraints accumulate into slot 0 (stack/manipulation.rs:63-64)
-        ev[0] = fe_add(ev[0], fe_mul(f_swap, fe_add(fe_sub(NW(0), O(1)), fe_sub(NW(1), O(0)))));
-        DG_STEP();
-        // swap2
-        ev[0] = fe_add(ev[0], fe_mul(f_swap2, fe_sub(NW(0), O(2)))); ev[1] = fe_add(ev[1], fe_mul(f_swap2, fe_sub(NW(1), O(3))));
-        ev[2] = fe_add(ev[2], fe_mul(f_swap2, fe_sub(NW(2), O(0)))); ev[3] = fe_add(ev[3], fe_mul(f_swap2, fe_sub(NW(3), O(1))));
-        // swap4
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-            ev[q] = fe_add(ev[q], fe_mul(f_swap4, fe_sub(NW(q), O(4 + q))));
-            ev[4 + q] = fe_add(ev[4 + q], fe_mul(f_swap4, fe_sub(NW(4 + q), O(q))));
-        }
-        DG_STEP();
-        // roll4 / roll8
-        ev[0] = fe_add(ev[0], fe_mul(f_roll4, fe_sub(NW(0), O(3))));
-#pragma unroll
-        for (int q = 1; q < 4; q++) ev[q] = fe_add(ev[q], fe_mul(f_roll4, fe_sub(NW(q), O(q - 1))));
-        ev[0] = fe_add(ev[0], fe_mul(f_roll8, fe_sub(NW(0), O(7))));
-#pragma unroll
-        for (int q = 1; q < 8; q++) ev[q] = fe_add(ev[q], fe_mul(f_roll8, fe_sub(NW(q), O(q - 1))));
-        DG_STEP();
-        // arithmetic / boolean: slot 0
-        {
-            fe prod = fe_mul(O(0), O(1));
-            fe v = fe_mul(f_add, fe_sub(NW(0), fe_add(O(0), O(1))));
-            v = fe_add(v, fe_mul(fe_add(f_mul, f_and), fe_sub(NW(0), prod)));
-            v = fe_add(v, fe_mul(f_inv, fe_sub(ONE, fe_mul(NW(0), O(0)))));
-            v = fe_add(v, fe_mul(f_neg, fe_add(NW(0), O(0))));
-            v = fe_add(v, fe_mul(f_not, fe_sub(NW(0), bnot(O(0)))));
-            v = fe_add(v, fe_mul(f_or, fe_sub(NW(0), bnot(fe_mul(bnot(O(0)), bnot(O(1)))))));
-            // eq: new[0] == 1 - (O(1)-O(2)) * O(0)
-            v = fe_add(v, fe_mul(f_eq, fe_sub(NW(0), bnot(fe_mul(fe_sub(O(1), O(2)), O(0))))));
-            // choose
-            {
-                fe c = O(2);
-                v = fe_add(v, fe_mul(f_choose, fe_sub(NW(0), fe_add(fe_mul(c, O(0)), fe_mul(bnot(c), O(1))))));
-            }
-            ev[0] = fe_add(ev[0], v);
-        }
-        DG_STEP();
-        // choose2 / cswap2
-        {
-            fe c = O(4), nc = bnot(c);
-            ev[0] = fe_add(ev[0], fe_mul(f_choose2, fe_sub(NW(0), fe_add(fe_mul(c, O(0)), fe_mul(nc, O(2))))));
-            ev[1] = fe_add(ev[1], fe_mul(f_choose2, fe_sub(NW(1), fe_add(fe_mul(c, O(1)), fe_mul(nc, O(3))))));
-            ev[0] = fe_add(ev[0], fe_mul(f_cswap2, fe_sub(NW(0), fe_add(fe_mul(c, O(2)), fe_mul(nc, O(0))))));
-            ev[1] = fe_add(ev[1], fe_mul(f_cswap2, fe_sub(NW(1), fe_add(fe_mul(c, O(3)), fe_mul(nc, O(1))))));
-            ev[2] = fe_add(ev[2], fe_mul(f_cswap2, fe_sub(NW(2), fe_add(fe_mul(c, O(0)), fe_mul(nc, O(2))))));
-            ev[3] = fe_add(ev[3], fe_mul(f_cswap2, fe_sub(NW(3), fe_add(fe_mul(c, O(1)), fe_mul(nc, O(3))))));
-        }
-        DG_STEP();
-        // binacc (comparison.rs:111-133)
-        {
-            fe bit = NW(0);
-            ev[0] = fe_add(ev[0], fe_mul(f_binacc, is_bin(bit)));
-            ev[1] = fe_add(ev[1], fe_mul(f_binacc, NW(1)));
-            ev[2] = fe_add(ev[2], fe_mul(f_binacc, fe_sub(NW(2), fe_mul_small(O(2), 2))));
-            ev[3] = fe_add(ev[3], fe_mul(f_binacc, fe_sub(NW(3), fe_add(O(3), fe_mul(bit, O(2))))));
-        }
-        DG_STEP();
-        // cmp (comparison.rs:71-108): [pow, bit_a, bit_b, not_set, gt, lt, acc_b, acc_a]
-        {
-            fe xb = NW(1), yb = NW(2), not_set = NW(3);
-            fe bit_gt = fe_mul(xb, bnot(yb)), bit_lt = fe_mul(yb, bnot(xb));
-            fe gt = fe_add(O(4), fe_mul(bit_gt, not_set)), lt = fe_add(O(5), fe_mul(bit_lt, not_set));
-            fe p2 = O(0);
-            fe x_acc = fe_add(O(7), fe_mul(xb, p2)), y_acc = fe_add(O(6), fe_mul(yb, p2));
-            fe nsc = fe_mul(bnot(O(5)), bnot(O(4)));
-            ev[0] = fe_add(ev[0], fe_mul(f_cmp, is_bin(xb)));
-            ev[1] = fe_add(ev[1], fe_mul(f_cmp, is_bin(yb)));
-            ev[2] = fe_add(ev[2], fe_mul(f_cmp, fe_sub(NW(4), gt)));
-            ev[3] = fe_add(ev[3], fe_mul(f_cmp, fe_sub(NW(5), lt)));
-            ev[4] = fe_add(ev[4], fe_mul(f_cmp, fe_sub(NW(6), y_acc)));
-            ev[5] = fe_add(ev[5], fe_mul(f_cmp, fe_sub(NW(7), x_acc)));
-            ev[6] = fe_add(ev[6], fe_mul(f_cmp, fe_sub(not_set, nsc)));
-            ev[7] = fe_add(ev[7], fe_mul(f_cmp, fe_sub(fe_mul_small(NW(0), 2), p2)));
-        }
-        DG_STEP();
-        // rescr (stack/hash.rs:9-35)
+        // --- low slots 0..7, slot by slot: the shift products, then every operation-specific product of the slot, in one unreduced sum
+        //     (slot 0: 7 + 20 products).  Terms shared between slots are computed once, in reduced form.
+        // rescr (stack/hash.rs:9-35): slot q gets f_rescr * (ns[q] - os[q])
+        fe rs[6];
         {
             fe os[6], ns[6];
 #pragma unroll
@@ -507,21 +433,120 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
             for (int q = 0; q < 6; q++) ns[q] = NW(q);
             matvec<6>(c_hasher_inv_mds, ns);
 #pragma unroll
-            for (int q = 0; q < 6; q++) ns[q] = fe_sub(fe_cube(ns[q]), per[11 + 6 + q]);
-#pragma unroll
-            for (int q = 0; q < 6; q++) ev[q] = fe_add(ev[q], fe_mul(f_rescr, fe_sub(ns[q], os[q])));
+            for (int q = 0; q < 6; q++) rs[q] = fe_sub(fe_sub(fe_cube(ns[q]), per[11 + 6 + q]), os[q]);
         }
+        DG_STEP();
+        // choose2 / cswap2 with c = O(4): c O(j) + (1 - c) O(j+2) = O(j+2) + c (O(j) - O(j+2)); the swapped selection
+        // c O(j+2) + (1 - c) O(j) is O(j) + O(j+2) minus it
+        auto sel = [&](const int j) { return fe_add(O(j + 2), fe_mul(O(4), fe_sub(O(j), O(j + 2)))); };
+        // roll4 and roll8 shift slots 1..3 alike
+        const fe f_roll48 = fe_add(f_roll4, f_roll8);
+        fe fc = f_copy0, fl1 = f_ls1_0, fl2 = f_ls2_0, fl4 = f_ls4_0;
+        {
+            fe_wide w;
+            slot_shifts(w, 0, fc, fl1, fl2, fl4);
+            wide_mac(w, fe_add(fe_add(f_dup, f_dup2), f_dup4), fe_sub(NW(0), O(0)));        // dup / dup2 / dup4: new[k] == old[k]
+            wide_mac(w, f_pad2, NW(0));
+            wide_mac(w, f_swap, fe_add(fe_sub(NW(0), O(1)), fe_sub(NW(1), O(0))));          // swap: both constraints in slot 0
+                                                                                            // (stack/manipulation.rs:63-64)
+            wide_mac(w, f_swap2, fe_sub(NW(0), O(2)));
+            wide_mac(w, f_swap4, fe_sub(NW(0), O(4)));
+            wide_mac(w, f_roll4, fe_sub(NW(0), O(3)));
+            wide_mac(w, f_roll8, fe_sub(NW(0), O(7)));
+            // arithmetic / boolean
+            const fe prod = fe_mul(O(0), O(1));
+            wide_mac(w, f_add, fe_sub(NW(0), fe_add(O(0), O(1))));
+            wide_mac(w, fe_add(f_mul, f_and), fe_sub(NW(0), prod));
+            wide_mac(w, f_inv, fe_sub(ONE, fe_mul(NW(0), O(0))));
+            wide_mac(w, f_neg, fe_add(NW(0), O(0)));
+            wide_mac(w, f_not, fe_sub(NW(0), bnot(O(0))));
+            wide_mac(w, f_or, fe_sub(NW(0), fe_sub(fe_add(O(0), O(1)), prod)));             // 1 - (1 - O(0)) (1 - O(1))
+            wide_mac(w, f_eq, fe_sub(NW(0), bnot(fe_mul(fe_sub(O(1), O(2)), O(0)))));       // eq: new[0] == 1 - (O(1)-O(2)) * O(0)
+            wide_mac(w, f_choose, fe_sub(NW(0), fe_add(O(1), fe_mul(O(2), fe_sub(O(0), O(1))))));   // c O(0) + (1 - c) O(1), c = O(2)
+            {
+                const fe s0 = sel(0);
+                wide_mac(w, f_choose2, fe_sub(NW(0), s0));
+                wide_mac(w, f_cswap2, fe_sub(NW(0), fe_sub(fe_add(O(0), O(2)), s0)));
+            }
+            wide_mac(w, f_binacc, is_bin(NW(0)));                                            // binacc (comparison.rs:111-133)
+            wide_mac(w, f_cmp, is_bin(NW(1)));      // cmp (comparison.rs:71-108): [pow, bit_a, bit_b, not_set, gt, lt, acc_b, acc_a]
+            wide_mac(w, f_rescr, rs[0]);
+            slot_fold(0, w);
+        }
+        DG_STEP();
+        fc = fe_add(fc, f_copy1); fl1 = fe_add(fl1, f_ls1_1); fl2 = fe_add(fl2, f_ls2_1);
+        {
+            fe_wide w;
+            slot_shifts(w, 1, fc, fl1, fl2, fl4);
+            wide_mac(w, fe_add(f_dup2, f_dup4), fe_sub(NW(1), O(1)));
+            wide_mac(w, f_pad2, NW(1));
+            wide_mac(w, f_swap2, fe_sub(NW(1), O(3)));
+            wide_mac(w, f_swap4, fe_sub(NW(1), O(5)));
+            wide_mac(w, f_roll48, fe_sub(NW(1), O(0)));
+            {
+                const fe s1 = sel(1);
+                wide_mac(w, f_choose2, fe_sub(NW(1), s1));
+                wide_mac(w, f_cswap2, fe_sub(NW(1), fe_sub(fe_add(O(1), O(3)), s1)));
+            }
+            wide_mac(w, f_binacc, NW(1));
+            wide_mac(w, f_cmp, is_bin(NW(2)));
+            wide_mac(w, f_rescr, rs[1]);
+            slot_fold(1, w);
+        }
+        DG_STEP();
+        fc = fe_add(fc, f_copy2); fl4 = fe_add(fl4, f_ls4_2);
+        // cmp: gt = O(4) + bit_a (1 - bit_b) not_set, lt = O(5) + bit_b (1 - bit_a) not_set
+        const fe xy = fe_mul(NW(1), NW(2));
+        {
+            fe_wide w;
+            slot_shifts(w, 2, fc, fl1, fl2, fl4);
+            wide_mac(w, f_dup4, fe_sub(NW(2), O(2)));
+            wide_mac(w, f_swap2, fe_sub(NW(2), O(0)));
+            wide_mac(w, f_swap4, fe_sub(NW(2), O(6)));
+            wide_mac(w, f_roll48, fe_sub(NW(2), O(1)));
+            wide_mac(w, f_cswap2, fe_sub(NW(2), sel(0)));
+            wide_mac(w, f_binacc, fe_sub(NW(2), fe_mul_small(O(2), 2)));
+            wide_mac(w, f_cmp, fe_sub(NW(4), fe_add(O(4), fe_mul(fe_sub(NW(1), xy), NW(3)))));
+            wide_mac(w, f_rescr, rs[2]);
+            slot_fold(2, w);
+        }
+        DG_STEP();
+        {
+            fe_wide w;
+            slot_shifts(w, 3, fc, fl1, fl2, fl4);
+            wide_mac(w, f_dup4, fe_sub(NW(3), O(3)));
+            wide_mac(w, f_swap2, fe_sub(NW(3), O(1)));
+            wide_mac(w, f_swap4, fe_sub(NW(3), O(7)));
+            wide_mac(w, f_roll48, fe_sub(NW(3), O(2)));
+            wide_mac(w, f_cswap2, fe_sub(NW(3), sel(1)));
+            wide_mac(w, f_binacc, fe_sub(NW(3), fe_add(O(3), fe_mul(NW(0), O(2)))));
+            wide_mac(w, f_cmp, fe_sub(NW(5), fe_add(O(5), fe_mul(fe_sub(NW(2), xy), NW(3)))));
+            wide_mac(w, f_rescr, rs[3]);
+            slot_fold(3, w);
+        }
+        DG_STEP();
+        fc = fe_add(fc, f_copy4); fl2 = fe_add(fl2, f_ls2_4);
 #pragma unroll
-        for (int i = 0; i < 8; i++)
-            if (i < P.stack_depth) fold(base + 2 + i, G7, ev[i]);
+        for (int q = 4; q < 8; q++) {
+            if (q == 6) fc = fe_add(fc, f_copy6);
+            fe_wide w;
+            slot_shifts(w, q, fc, fl1, fl2, fl4);
+            wide_mac(w, f_swap4, fe_sub(NW(q), O(q - 4)));
+            wide_mac(w, f_roll8, fe_sub(NW(q), O(q - 1)));
+            if (q == 4) wide_mac(w, f_cmp, fe_sub(NW(6), fe_add(O(6), fe_mul(NW(2), O(0)))));     // acc_b
+            if (q == 5) wide_mac(w, f_cmp, fe_sub(NW(7), fe_add(O(7), fe_mul(NW(1), O(0)))));     // acc_a
+            if (q == 6) wide_mac(w, f_cmp, fe_sub(NW(3), fe_mul(bnot(O(5)), bnot(O(4)))));        // not_set
+            if (q == 7) wide_mac(w, f_cmp, fe_sub(fe_mul_small(NW(0), 2), O(0)));                 // pow
+            if (q < 6) wide_mac(w, f_rescr, rs[q]);
+            slot_fold(q, w);
+            if (q & 1) DG_STEP();
+        }
+        close(G7);
     }
 
     DG_STEP();
-    // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g ------------------------------------------------------------------
+    // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g, every group already closed into acc.res ---------------------------
     fe t_res = DG_REDUCE_WIDE(acc.res);
-    const fe *const xpow_override = P.xpow_override ? P.xpow_override + blockIdx.y * P.override_stride : nullptr;
-#pragma unroll
-    for (int g = 0; g < 6; g++) t_res = fe_add(t_res, fe_mul(acc.adj[g], xpow_override ? xpow_override[g] : tw_pow(P.twN, lde_index * P.inc[g])));
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
     if (!P.verify_mode && c8 == 0 && k != n - 1) {
         if (acc.nonzero && live) atomicMax(P.violation + blockIdx.y, violation_word(k));
@@ -549,10 +574,14 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
 void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     air_upload_constants(c);
     DG_REQUIRE(batch >= 1 && batch <= 65535, "constraint evaluation batch out of range");
+    // the kernel's unreduced sums are bounded for at most 16 context, 8 loop and 32 stack registers (Acc)
+    DG_REQUIRE(P.cl >= 1 && P.cl <= 16 && P.ll >= 1 && P.ll <= 8 && P.sl >= 8 && P.sl <= 32, "constraint evaluation register shape out of range");
     const unsigned long long E = (unsigned long long)P.num_c8 << P.log_n;
     // H100 SXM (700 W), stage 3 of the 2^20-step proof x 26 registers: per-thread arrays 24.8 ms; shared-memory rows, stack-like columns
     // only 23.7; all columns 23.2; all columns + unreduced per-slot sums (constraint_eval_smem_kernel) 22.2.  The other forms were removed
     // after this measurement.
+    // H100 80GB HBM3 (700 W), same proof: constraint_eval_smem_kernel with one unreduced sum per constraint and per degree group 18.27 ms,
+    // 21.08 ms with one reduction per product outside the per-slot shift sums (mean of 4 alternating runs each).
     // All proofs of a batch run in one launch.  Traces shorter than a block take the SHORT layout; with several ranks their domain slice
     // can be shorter than one block, and the clamped threads of the partial block write nothing.
     const bool short_n = P.log_n < 7;
