@@ -1,6 +1,7 @@
 """Host-side mirror of the reference's public interface for the prove path (names and argument meaning follow
 /root/reference/src/lib.rs:30-75, /root/reference/src/stark/options.rs:16-91, /root/reference/src/stark/proof.rs:10-77)."""
 import ctypes
+import functools
 
 import numpy as np
 
@@ -204,6 +205,163 @@ def verify_batch(items, stats=None):
     if stats is not None:
         stats.update(total_ms=float(st.total_ms), kernel_launches=int(st.kernel_launches), groups=int(st.groups))
     return out
+
+
+# ---- checking a trace before proving it ---------------------------------------------------------------------------------------------
+_NO_STEP = 2**64 - 1
+MIN_OP_COUNT = 16           # lib.rs:48-52 (MIN_TRACE_LENGTH)
+
+
+def constraint_name(ctx_depth, loop_depth, stack_depth, index):
+    """name of transition constraint `index` (evaluation order) of a register shape: "op bit 3 binary", "sponge 1", "stack slot 5", ..."""
+    buf = ctypes.create_string_buffer(64)
+    backend.check(backend.lib().dg_host_constraint_name(ctx_depth, loop_depth, stack_depth, index, buf, len(buf)))
+    return buf.value.decode()
+
+
+def register_name(r, ctx_depth, loop_depth):
+    """name of register r of the trace layout (trace_state.rs:115-118)"""
+    if r == 0:
+        return "op counter"
+    for base, count, name in ((1, 4, "sponge"), (5, 3, "cf op bit"), (8, 5, "ld op bit"), (13, 2, "hd op bit"), (15, ctx_depth, "ctx stack"),
+                              (15 + ctx_depth, loop_depth, "loop stack")):
+        if r < base + count:
+            return "%s %d" % (name, r - base)
+    return "user stack %d" % (r - 15 - ctx_depth - loop_depth)
+
+
+class TraceReport:
+    """What check_trace finds in one trace, before any proving.
+      ok                    no transition or boundary constraint fails, the op count is >= 16 and the program hash (if given) matches
+      first_step            lowest trace step at which a transition constraint fails, or None (the last step, n - 1 -> 0, is exempt)
+      violating_steps       number of such steps
+      transitions           {constraint name: (steps at which it fails, its lowest such step)}, only the constraints that fail
+      boundary              readable strings, one per register of the first or last row that breaks a boundary assertion
+      first_row_registers / last_row_registers   those registers' indexes
+      op_count              op counter of the last row; program_hash_matches 1, 0, or -1 when no hash was given
+      masks                 (n, 3) uint32: bit j of word j // 32 at step k = constraint j fails at k (None unless asked for)"""
+
+    def __init__(self, raw, shape, length, value_of, inputs, outputs, masks=None):
+        ctx_depth, loop_depth, stack_depth = shape
+        self.length = length
+        self.n_constraints = int(raw.n_constraints)
+        self.violating_steps = int(raw.violating_steps)
+        self.first_step = None if raw.first_step == _NO_STEP else int(raw.first_step)
+        self.transitions = {}
+        for j in (range(self.n_constraints) if self.first_step is not None else ()):
+            if raw.constraint_steps[j]:
+                self.transitions[constraint_name(ctx_depth, loop_depth, stack_depth, j)] = (int(raw.constraint_steps[j]), int(raw.constraint_first[j]))
+        stk = 15 + ctx_depth + loop_depth
+        def registers(words):
+            bits = int(words[0]) | (int(words[1]) << 64)
+            return [r for r in range(128) if (bits >> r) & 1] if bits else []
+        self.first_row_registers = registers(raw.first_row_registers)
+        self.last_row_registers = registers(raw.last_row_registers)
+        self.boundary = []
+        for row, regs, claimed, what in (("first row", self.first_row_registers, inputs, "input"), ("last row", self.last_row_registers, outputs, "output")):
+            for r in regs:
+                if r >= stk:
+                    expected = "%s %d" % (what, claimed[r - stk])
+                else:
+                    expected = "1" if row == "last row" and 5 <= r < 15 else "0"
+                self.boundary.append("%s: %s (register %d) is %d, expected %s" % (
+                    row, register_name(r, ctx_depth, loop_depth), r, value_of(row == "last row", r), expected))
+        self.op_count = int(raw.op_count)
+        self.op_count_ok = bool(raw.op_count_ok)
+        self.program_hash_matches = int(raw.program_hash_matches)
+        self.masks = masks
+
+    @property
+    def ok(self):
+        return self.first_step is None and not self.boundary and self.op_count_ok and self.program_hash_matches != 0
+
+    def __str__(self):
+        if self.ok:
+            return "trace ok: %d steps, %d operations" % (self.length, self.op_count)
+        lines = []
+        if self.first_step is not None:
+            lines.append("transition constraints fail at %d of %d steps, first at step %d:" % (self.violating_steps, self.length - 1, self.first_step))
+            lines += ["  %s: %d steps, first at step %d" % (name, s, f) for name, (s, f) in sorted(self.transitions.items(), key=lambda e: e[1][1])]
+        if self.boundary:
+            lines.append("boundary constraints fail:")
+            lines += ["  " + b for b in self.boundary]
+        if not self.op_count_ok:
+            lines.append("the trace executes %d operations; a proof needs at least %d" % (self.op_count, MIN_OP_COUNT))
+        if self.program_hash_matches == 0:
+            lines.append("the program hash in the last row's sponge does not match the expected hash")
+        return "\n".join(lines)
+
+    __repr__ = __str__
+
+
+def _hashes(program_hashes, count):
+    if program_hashes is None:
+        return None
+    hs = [bytes(h) for h in program_hashes]
+    assert len(hs) == count and all(len(h) == 32 for h in hs), "one 32-byte program hash per trace"
+    return b"".join(hs)
+
+
+def check_traces(traces, program_hashes=None, masks=False):
+    """Checks hostvm.ExecutionTraces without proving them: one GPU pass per group of same-shape traces (dg_check_traces) evaluates every
+    transition constraint at every step, and the first and last rows are compared with the boundary assertions for the trace's public
+    inputs and outputs.  program_hashes: None, or one 32-byte hash per trace.  Returns a TraceReport per trace, in input order."""
+    traces = list(traces)
+    if program_hashes is not None:
+        program_hashes = list(program_hashes)
+    groups = {}
+    for i, tr in enumerate(traces):
+        groups.setdefault((tr.registers.shape[0], tr.registers.shape[1], tr.ctx_depth, tr.loop_depth), []).append(i)
+    result = [None] * len(traces)
+    for (w, n, ctx_depth, loop_depth), idx in groups.items():
+        k = len(idx)
+        regs = [np.ascontiguousarray(traces[i].registers, dtype=np.uint64) for i in idx]
+        cols = [(backend.vp * w)(*[r[j].ctypes.data for j in range(w)]) for r in regs]
+        ts = (backend.DgTrace * k)(*[backend.DgTrace(cols[m], w, n, ctx_depth, loop_depth) for m in range(k)])
+        keep, (pin, nin, pout, nout) = _batch_io([traces[i].public_inputs for i in idx], [traces[i].outputs for i in idx])
+        hashes = _hashes([program_hashes[i] for i in idx], k) if program_hashes is not None else None
+        reports = (backend.DgTraceReport * k)()
+        step_masks = np.zeros((k, n, 3), dtype=np.uint32) if masks else None
+        backend.check(backend.lib().dg_check_traces(ts, k, pin, nin, pout, nout, hashes, reports,
+                                                    step_masks.ctypes.data if masks else None))
+        shape = (ctx_depth, loop_depth, w - 15 - ctx_depth - loop_depth)
+        for m, i in enumerate(idx):
+            tr = traces[i]
+            value_of = (lambda last, r, a=regs[m]: felt.to_ints(a[r, n - 1 if last else 0])[0])
+            result[i] = TraceReport(reports[m], shape, n, value_of, list(tr.public_inputs), list(tr.outputs),
+                                    step_masks[m] if masks else None)
+        del keep, cols
+    return result
+
+
+def check_trace(trace, program_hash=None, masks=False):
+    """check_traces of one trace: a TraceReport.  program_hash (32 bytes) is compared with the last row's sponge; masks=True also returns
+    the per-step masks of failing constraints (report.masks, (n, 3) uint32)."""
+    return check_traces([trace], None if program_hash is None else [program_hash], masks=masks)[0]
+
+
+def check_traces_device(d_registers, count, width, length, ctx_depth, loop_depth, public_inputs_list, outputs_list, program_hashes=None,
+                        d_masks=None):
+    """check_traces for `count` traces of one shape already in device memory, proof-major [count][width][length] elements
+    (backend.DeviceBuffer or raw pointer), used in place.  d_masks: None, or device memory of count * length * 3 uint32 that receives
+    the per-step masks.  Returns a TraceReport per trace."""
+    assert len(public_inputs_list) == count and len(outputs_list) == count, "one list of public inputs and outputs per trace"
+    ptr = d_registers.ptr if isinstance(d_registers, backend.DeviceBuffer) else int(d_registers)
+    mptr = None if d_masks is None else (d_masks.ptr if isinstance(d_masks, backend.DeviceBuffer) else int(d_masks))
+    keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
+    reports = (backend.DgTraceReport * max(count, 1))()
+    backend.check(backend.lib().dg_check_traces_device(ptr, count, width, length, ctx_depth, loop_depth, pin, nin, pout, nout,
+                                                       _hashes(program_hashes, count), reports, mptr))
+    del keep
+
+    def value_of(q, last, r):
+        v = np.zeros(2, dtype=np.uint64)
+        offset = ((q * width + r) * length + (length - 1 if last else 0)) * 16
+        backend.check(backend.lib().dg_dev_download(v.ctypes.data, ptr + offset, 16))
+        return felt.to_ints(v)[0]
+    shape = (ctx_depth, loop_depth, width - 15 - ctx_depth - loop_depth)
+    return [TraceReport(reports[q], shape, length, functools.partial(value_of, q), list(public_inputs_list[q]), list(outputs_list[q]))
+            for q in range(count)]
 
 
 def execute(source, public_inputs=(), secret_a=(), secret_b=(), num_outputs=1, options=None):

@@ -39,7 +39,13 @@ class DgVerifyStats(ctypes.Structure):
     _fields_ = [("total_ms", ctypes.c_float), ("kernel_launches", u64), ("groups", u32)]
 
 
-DRAW_FIELD_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
+class DgTraceReport(ctypes.Structure):
+    _fields_ = [("n_constraints", u32), ("violating_steps", u64), ("first_step", u64), ("constraint_steps", u64 * 128),
+                ("constraint_first", u64 * 128), ("first_row_registers", u64 * 2), ("last_row_registers", u64 * 2), ("op_count", u64),
+                ("op_count_ok", ctypes.c_int32), ("program_hash_matches", ctypes.c_int32)]
+
+
+DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
 
@@ -59,6 +65,10 @@ EXPORTS = {
     "dg_prove_batch_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
                               ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
+    "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
+                        ctypes.POINTER(DgTraceReport), vp],
+    "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                               vp, ctypes.POINTER(DgTraceReport), vp],
     "dg_verify": [vp, vp, u32, vp, u32, vp, ctypes.c_size_t, ctypes.c_char_p, ctypes.c_size_t],
     "dg_verify_batch": [u32, ctypes.POINTER(vp), ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
                         ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgVerifyStats)],
@@ -97,6 +107,7 @@ EXPORTS = {
     "dg_host_plan_batch": [vp, u32, u64, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
     "dg_host_merkle_verify_plan": [vp, u32, u32, u32, vp, u32, vp, ctypes.c_size_t, vp, vp, ctypes.c_size_t, vp, vp],
     "dg_host_periodic_tables": [vp],
+    "dg_host_constraint_name": [u32, u32, u32, u32, ctypes.c_char_p, ctypes.c_size_t],
 }
 VOID_EXPORTS = {"dg_proof_free": [vp]}
 

@@ -108,7 +108,9 @@ struct Acc {
 // runtime loop bounds would force into local memory; stack slots >= 8 are folded into the accumulators as soon as they are evaluated.
 // The 15 decoder registers are staged as well (read from shared memory at every use) instead of being held in registers.
 // blockIdx.y is the proof of a batch (AirParams strides).
-template <int BLOCK, int MIN_BLOCKS, bool SHORT = false>
+// CHECK: the trace check (launch_constraint_check).  fold records which constraints are nonzero in three mask words instead of combining
+// them, close does nothing, and each step writes its mask words.
+template <int BLOCK, int MIN_BLOCKS, bool SHORT = false, bool CHECK = false>
 __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel(const AirParams P) {
     extern __shared__ __align__(16) unsigned char air_smem[];
     fe *s_rows = reinterpret_cast<fe *>(air_smem);
@@ -196,14 +198,25 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     acc.first = true;
     acc.run_first = true;
     acc.nonzero = false;
+    // CHECK: bit idx of (m2 m1 m0) is set when constraint idx is nonzero (T <= 78); scalars, since a runtime-indexed array would live in
+    // local memory
+    unsigned m0 = 0, m1 = 0, m2 = 0;
     // the proof's coefficients are read at each use: pointers to them held across the body would add live registers
     auto fold = [&](int idx, fe v) {
-        const unsigned long long at = idx + blockIdx.y * P.coef_stride;
-        acc.fold(v, P.coefA[at], P.coefB[at]);
+        if constexpr (CHECK) {
+            const unsigned bit = fe_is_zero(v) ? 0u : 1u;
+            if (idx < 32) m0 |= bit << idx;
+            else if (idx < 64) m1 |= bit << (idx - 32);
+            else m2 |= bit << (idx - 64);
+        } else {
+            const unsigned long long at = idx + blockIdx.y * P.coef_stride;
+            acc.fold(v, P.coefA[at], P.coefB[at]);
+        }
     };
     // closes the run of degree group g: x^inc_g is the host's value at the verifier's point, else a power of the LDE root
     auto close = [&](int g) {
-        acc.close(P.xpow_override ? P.xpow_override[blockIdx.y * P.override_stride + g] : tw_pow(P.twN, lde_index * P.inc[g]));
+        if constexpr (!CHECK)
+            acc.close(P.xpow_override ? P.xpow_override[blockIdx.y * P.override_stride + g] : tw_pow(P.twN, lde_index * P.inc[g]));
     };
 
     const fe *per = P.per_override ? P.per_override + blockIdx.y * P.override_stride
@@ -545,6 +558,17 @@ __global__ void __launch_bounds__(BLOCK, MIN_BLOCKS) constraint_eval_smem_kernel
     }
 
     DG_STEP();
+    if constexpr (CHECK) {
+        // the wrap-around transition n - 1 -> 0 is exempt (evaluator.rs:330-333: should_evaluate_to_zero_at)
+        if (live) {
+            unsigned *m = P.masks + (blockIdx.y * n + k) * 3;
+            const bool exempt = k == n - 1;
+            m[0] = exempt ? 0u : m0;
+            m[1] = exempt ? 0u : m1;
+            m[2] = exempt ? 0u : m2;
+        }
+        return;
+    }
     // ---- combine (evaluator.rs:335-358): result + sum_g adj_g * x^inc_g, every group already closed into acc.res ---------------------------
     fe t_res = DG_REDUCE_WIDE(acc.res);
     // on the trace domain (except its last step) every constraint must vanish (evaluator.rs:149-158)
@@ -591,6 +615,76 @@ void launch_constraint_eval(Context &c, const AirParams &P, int batch) {
     auto k = short_n ? constraint_eval_smem_kernel<128, 4, true> : constraint_eval_smem_kernel<128, 4>;
     set_func_smem(c, (const void *)k, smem);
     k<<<dim3((unsigned)((E + 127) / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
+void launch_constraint_check(Context &c, const AirParams &P, int batch) {
+    air_upload_constants(c);
+    DG_REQUIRE(batch >= 1 && batch <= 65535, "trace check batch out of range");
+    DG_REQUIRE(P.cl >= 1 && P.cl <= 16 && P.ll >= 1 && P.ll <= 8 && P.sl >= 8 && P.sl <= 32, "trace check register shape out of range");
+    DG_REQUIRE(P.num_c8 == 1 && P.c8_base == 0 && P.log_blowup == 3 && P.masks, "the trace check runs on the trace domain");
+    const bool short_n = P.log_n < 7;
+    const size_t smem = (size_t)P.w * (short_n ? 128 + 128 / 16 : 128 + 1) * sizeof(fe);
+    DG_REQUIRE(P.log_n >= 4 && smem <= 200 * 1024, "the trace check needs at least 16 steps and at most 200 KB of rows per block");
+    auto k = short_n ? constraint_eval_smem_kernel<128, 4, true, true> : constraint_eval_smem_kernel<128, 4, false, true>;
+    set_func_smem(c, (const void *)k, smem);
+    k<<<dim3((unsigned)(((1ULL << P.log_n) + 127) / 128), (unsigned)batch), 128, smem, c.stream>>>(P);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
+// One atomic per block and constraint: each warp turns a constraint's bits into a ballot (popc = violating steps, ffs = the lowest), the
+// warps of a block combine in shared memory, and the block adds its counts to the trace's totals.  Random rows violate every constraint at
+// every step, where one atomic per step and constraint would serialise.
+__global__ void check_reduce_kernel(const unsigned *__restrict__ masks, unsigned long long n, int T, unsigned long long *stats) {
+    __shared__ unsigned s_cnt[CHECK_SLOTS];
+    __shared__ unsigned long long s_first[CHECK_SLOTS];
+    for (int i = threadIdx.x; i < CHECK_SLOTS; i += blockDim.x) { s_cnt[i] = 0; s_first[i] = ~0ULL; }
+    __syncthreads();
+    const unsigned *m = masks + (unsigned long long)blockIdx.y * n * 3;
+    const int lane = threadIdx.x & 31;
+    for (unsigned long long base = (unsigned long long)blockIdx.x * blockDim.x; base < n; base += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long k = base + threadIdx.x;
+        const unsigned long long warp0 = k - lane;
+        unsigned w[3] = {0, 0, 0};
+        if (k < n) { w[0] = m[k * 3]; w[1] = m[k * 3 + 1]; w[2] = m[k * 3 + 2]; }
+        const unsigned any = __ballot_sync(0xFFFFFFFFu, (w[0] | w[1] | w[2]) != 0);
+        if (!any) continue;                                                     // warp-uniform
+        if (lane == 0) {
+            atomicAdd(&s_cnt[CHECK_SLOTS - 1], __popc(any));
+            atomicMin(&s_first[CHECK_SLOTS - 1], warp0 + __ffs(any) - 1);
+        }
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            if (!__any_sync(0xFFFFFFFFu, w[j] != 0)) continue;
+            for (int b = 0; b < 32 && 32 * j + b < T; b++) {
+                const unsigned ballot = __ballot_sync(0xFFFFFFFFu, (w[j] >> b) & 1u);
+                if (lane == 0 && ballot) {
+                    atomicAdd(&s_cnt[32 * j + b], __popc(ballot));
+                    atomicMin(&s_first[32 * j + b], warp0 + __ffs(ballot) - 1);
+                }
+            }
+        }
+    }
+    __syncthreads();
+    unsigned long long *st = stats + (unsigned long long)blockIdx.y * CHECK_STATS;
+    for (int i = threadIdx.x; i < CHECK_SLOTS; i += blockDim.x)
+        if (s_cnt[i]) {
+            atomicAdd(&st[i], (unsigned long long)s_cnt[i]);
+            atomicMin(&st[CHECK_SLOTS + i], s_first[i]);
+        }
+}
+
+void launch_check_reduce(Context &c, const unsigned *masks, unsigned long long n, int T, int batch, unsigned long long *stats) {
+    DG_REQUIRE(batch >= 1 && batch <= 65535 && T >= 1 && T < CHECK_SLOTS, "trace check reduction out of range");
+    // counts 0, lowest steps UINT64_MAX
+    DG_CUDA(cudaMemsetAsync(stats, 0, (size_t)batch * CHECK_STATS * 8, c.stream));
+    DG_CUDA(cudaMemset2DAsync(stats + CHECK_SLOTS, CHECK_STATS * 8, 0xFF, CHECK_SLOTS * 8, batch, c.stream));
+    // enough blocks to fill the GPU, each walking several 256-step tiles: fewer blocks, fewer global atomics
+    const unsigned long long tiles = (n + 255) / 256;
+    const unsigned gx = (unsigned)std::max<unsigned long long>(1, std::min<unsigned long long>(tiles, (unsigned long long)(4 * c.num_sms + batch - 1) / batch));
+    check_reduce_kernel<<<dim3(gx, (unsigned)batch), 256, 0, c.stream>>>(masks, n, T, stats);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }

@@ -27,6 +27,8 @@ struct AirParams {
     unsigned long long ext_stride, t_ev_stride, coef_stride;
     // batched verification: proof q reads per_override / xpow_override + q * override_stride
     unsigned long long override_stride;
+    // trace check (launch_constraint_check): per trace step k of proof q, masks[(q n + k) * 3 + j] bit i = constraint 32 j + i is nonzero
+    unsigned *masks;
 };
 
 // A trace step k that violates a transition constraint is recorded as atomicMax(violation, 0xFFFFFFFF - k), so the lowest violating
@@ -37,5 +39,14 @@ inline unsigned long long violation_step(unsigned word) { return 0xFFFFFFFFu - w
 // evaluates the transition constraints of `batch` proofs of one shape (proof q at the strides of P) in one launch (blockIdx.y = proof);
 // traces of at least 16 steps
 void launch_constraint_eval(Context &c, const AirParams &P, int batch = 1);
+
+// the trace check: the same kernel on the register traces themselves (coset 0 of the extension is the trace: num_c8 = 1, log_blowup = 3,
+// col_stride = n, ext_stride = w n), recording per trace step which constraints do not vanish (P.masks, 3 words per step; the exempt
+// last step n - 1 gets 0) instead of combining them.  No coefficient, power of x or violation word is read or written.
+void launch_constraint_check(Context &c, const AirParams &P, int batch);
+// masks of `batch` traces of n steps -> per trace q, at stats + q * CHECK_STATS: [0, 96) violating steps per constraint, [96] steps with
+// any violation, then at + 97 the lowest such step (UINT64_MAX if none), in the same order
+constexpr int CHECK_SLOTS = 97, CHECK_STATS = 2 * CHECK_SLOTS;
+void launch_check_reduce(Context &c, const unsigned *masks, unsigned long long n, int T, int batch, unsigned long long *stats);
 
 }  // namespace dg

@@ -483,6 +483,40 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
                            *options, (Proof **)proofs_out, status, t_batch_messages, stats);
     });
 }
+int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
+                    uint32_t *step_masks) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one trace must be checked");
+        DG_REQUIRE(traces && reports, "null argument");
+        const dg_trace_t &t0 = traces[0];
+        std::vector<const uint8_t *> cols;
+        for (uint32_t i = 0; i < count; i++) {
+            const dg_trace_t &t = traces[i];
+            DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
+                       "all traces of a call must have the same width, length, context depth and loop depth");
+            DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
+            for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
+            cols.insert(cols.end(), t.columns, t.columns + t.width);
+        }
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        check_traces(c, nullptr, cols.data(), count, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+                     program_hashes32, reports, step_masks, nullptr);
+    });
+}
+int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                           const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                           const uint8_t *program_hashes32, dg_trace_report_t *reports, uint32_t *d_step_masks) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one trace must be checked");
+        DG_REQUIRE(d_registers && reports, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        check_traces(c, (const fe *)d_registers, nullptr, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+                     program_hashes32, reports, nullptr, d_step_masks);
+    });
+}
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
     return guarded([&] {
         DG_REQUIRE(message && cap, "null argument");
@@ -621,6 +655,14 @@ int dg_host_merkle_verify_plan(const uint64_t *indexes, uint32_t n_indexes, uint
 }
 int dg_host_periodic_tables(uint8_t *out16) {
     return guarded([&] { std::vector<fe> t = fs::periodic_tables(); memcpy(out16, t.data(), t.size() * 16); });
+}
+int dg_host_constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t index, char *name, size_t cap) {
+    return guarded([&] {
+        DG_REQUIRE(name && cap, "null argument");
+        const std::string s = constraint_name(ctx_depth, loop_depth, stack_depth, index);
+        strncpy(name, s.c_str(), cap - 1);
+        name[cap - 1] = 0;
+    });
 }
 
 }  // extern "C"

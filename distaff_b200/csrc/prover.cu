@@ -218,6 +218,14 @@ private:
     std::vector<std::thread> workers_;
 };
 
+void upload_trace_columns(Context &c, fe *d_regs, const uint8_t *const *host_cols, int cols, uint64_t n) {
+    const int chunk = (int)std::max<uint64_t>(1, std::min<uint64_t>(cols, ((uint64_t)1 << 26) / (n * 16)));     // ~64 MB per chunk
+    std::vector<int> bounds = {0};
+    while (bounds.back() < cols) bounds.push_back(std::min(cols, bounds.back() + chunk));
+    TraceUploader up(c, d_regs, host_cols, cols, n, bounds);
+    for (int i = 0; i < up.chunks(); i++) up.wait_chunk(i);
+}
+
 namespace {
 
 typedef std::vector<std::vector<size_t>> Offsets;

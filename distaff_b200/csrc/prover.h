@@ -26,6 +26,20 @@ void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t w
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                         const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
 
+// copies `cols` host register columns of n elements each to d_regs (column stride n) by the prover's upload path (pinned columns DMA'd
+// directly, pageable ones staged through the library's pinned slots) and orders c.stream after the copies
+void upload_trace_columns(Context &c, fe *d_regs, const uint8_t *const *host_cols, int cols, uint64_t n);
+
+// the trace check (check.cu): per trace, which transition constraints fail at which steps and which boundary registers are wrong.
+// d_regs: [count][width][length] on the device, or null with host_cols (count * width column pointers) to upload; program_hashes32
+// (count * 32 bytes) and step_masks (host, count * length * 3 words) / d_step_masks (device, same size) may be null
+void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
+                  uint32_t *step_masks, uint32_t *d_step_masks);
+// name of transition constraint `index` (evaluation order) of a register shape, as the trace check reports it
+std::string constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t index);
+
 // GPU verification (verifier.cu).  One proof of dg_verify / dg_verify_batch, with its program hash and public inputs / outputs.
 struct VerifyRequest {
     const uint8_t *program_hash;

@@ -92,6 +92,41 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
                           const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats);
 int dg_batch_message(uint32_t index, char *message, size_t message_cap);
 
+/* ---- checking a trace before proving it ------------------------------------------------------------------------------------------
+ * dg_prove reports an unsatisfied trace late (after the trace LDE and commitment) and only with its lowest failing step; it does not check
+ * the boundary constraints at all (a trace whose first or last row disagrees with the claimed inputs / outputs is proven, and the proof is
+ * then rejected by the verifier).  dg_check_traces evaluates every transition constraint at every trace step in one GPU pass over the
+ * registers and compares the first and last rows with the boundary assertions (evaluator.rs:181-326):
+ *   first row: op counter, sponge, cf / ld / hd op bits, context and loop stacks all 0; user stack[i] = input i;
+ *   last row:  cf / ld / hd op bits all 1, context and loop stacks 0; user stack[i] = output i.
+ * It also reports what execute (lib.rs:48-60) asserts before proving: the last row's op counter (>= 16) and whether its sponge[0..2]
+ * equals the program hash, when one is given.  Transition constraints are numbered in evaluation order, the order of
+ * dg_eval_transitions' coefficients; dg_host_constraint_name names them.  The last step (n - 1 -> 0) is exempt, as in the prover.
+ * No Fiat-Shamir value is drawn and the RNG callbacks are never called.  Same-shape traces only (as dg_prove_batch; same shape checks as
+ * dg_prove), split into groups bounded by device memory, 65535 traces and $DG_BATCH_GROUP; one GPU (DG_ERR_INVALID for a context that
+ * spans several). */
+typedef struct {
+    uint32_t n_constraints;                 /* T, evaluation order = dg_eval_transitions' coefficient order */
+    uint64_t violating_steps, first_step;   /* transition violations over steps 0..n-2; first_step = UINT64_MAX if none */
+    uint64_t constraint_steps[128];         /* per constraint: steps at which it does not vanish */
+    uint64_t constraint_first[128];         /* per constraint: the lowest such step, UINT64_MAX if none */
+    uint64_t first_row_registers[2];        /* bit r (of word r / 64): register r of the first row breaks a boundary assertion */
+    uint64_t last_row_registers[2];         /* same, last row */
+    uint64_t op_count;                      /* op counter of the last row (UINT64_MAX if it does not fit) */
+    int32_t op_count_ok;                    /* 1 if that op counter is >= 16 (lib.rs:48-52), else 0 */
+    int32_t program_hash_matches;           /* 1, 0, or -1 when no hash was given */
+} dg_trace_report_t;
+/* traces[i], inputs / outputs as in dg_prove_batch; program_hashes32: NULL or count * 32 bytes; reports: count entries; step_masks: NULL
+ * or count * length * 3 words, bit j of word 3 k + j / 32 of trace i = constraint j does not vanish at step k.  Returns DG_OK when every
+ * trace was checked, whatever the reports say. */
+int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
+                    uint32_t *step_masks);
+/* same, registers already in device memory: proof-major [count][width][length] elements; d_step_masks: NULL or device memory */
+int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                           const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                           const uint8_t *program_hashes32, dg_trace_report_t *reports, uint32_t *d_step_masks);
+
 /* Optional: randomness supplied by the host.  The prover derives all of its Fiat-Shamir challenges from two reference functions,
  *   field::prng_vector(seed, n)                            (math/field.rs:264-275: StdRng::from_seed + Uniform(0..M))
  *   utils::compute_query_positions(seed, domain, options)  (stark/utils/mod.rs:25-44: StdRng + Uniform(0..domain), rejections)
@@ -230,6 +265,9 @@ int dg_host_merkle_verify_plan(const uint64_t *indexes, uint32_t n_indexes, uint
                                uint32_t *n_levels, uint32_t *root_slot);
 /* extend_constants tables (constraints/utils.rs:87-113): 128 rows x 23 columns = sponge ARK 8 | masks 3 | hasher ARK 12 */
 int dg_host_periodic_tables(uint8_t *out16 /* 128*23 elements */);
+/* name of transition constraint `index` (evaluation order) of a register shape: "op bit 3 binary", "op counter", "sponge 1", "ctx stack 0",
+ * "stack aux 1", "stack slot 5", ... (NUL-terminated, truncated to cap); DG_ERR_INVALID for a shape dg_prove rejects or index >= T */
+int dg_host_constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t index, char *name, size_t cap);
 
 #ifdef __cplusplus
 }
