@@ -7,8 +7,9 @@ Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.verify(hash, inputs, outputs, p) <->  distaff::verify     (/root/reference/src/lib.rs:68-75, stark/verifier.rs:11-75)
     distaff_b200.verify_batch(items)              <->  distaff::verify of every proof, all checked together on the GPU
     distaff_b200.check_trace(trace, hash)         <->  the named transition / boundary constraints a trace breaks, before proving it
+    distaff_b200.set_memory_limit(bytes)          <->  the most device memory the library may hold (plan_prove, memory_usage)
 The compute path is hand-written CUDA behind the C-ABI of include/distaff_gpu.h; there is no CPU fallback.
 """
 from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
                   merkle_build, hash_rows, hash64, find_pow_nonce, field_op, field_dot, eval_transitions, TraceReport, check_trace, check_traces,
-                  check_traces_device, constraint_name)
+                  check_traces_device, constraint_name, set_memory_limit, memory_usage, plan_prove)

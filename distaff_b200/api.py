@@ -91,6 +91,41 @@ def prove_device(d_registers, width, length, ctx_depth, loop_depth, public_input
     return _collect(handle, stats)
 
 
+def set_memory_limit(nbytes):
+    """dg_set_memory_limit: the most device memory (bytes) the library may hold on the current device; 0 or None removes the limit.
+    Shapes whose trace extension does not fit under it are proven in the evaluation-coset layout, with the same proof bytes."""
+    nbytes = 0 if nbytes is None else int(nbytes)
+    if nbytes < 0:
+        raise ValueError("memory limit must be a non-negative number of bytes")
+    backend.check(backend.lib().dg_set_memory_limit(nbytes))
+
+
+def memory_usage():
+    """dg_memory_usage: {"held": bytes the library holds now, "peak": the most it has held since the limit was last set}."""
+    held, peak = ctypes.c_size_t(0), ctypes.c_size_t(0)
+    backend.check(backend.lib().dg_memory_usage(ctypes.byref(held), ctypes.byref(peak)))
+    return {"held": held.value, "peak": peak.value}
+
+
+def plan_prove(width, length, count=1, options=None):
+    """dg_plan_prove: what proving `count` traces of width x length would do, without running it: the layout ("full" or "eval_cosets"),
+    the group size, the cosets extended per chunk and kept, bytes per proof and the fixed bytes beside them."""
+    options = options or ProofOptions()
+    width, length, count = int(width), int(length), int(count)
+    if not 1 <= width < 128:
+        raise ValueError("width must be in 1..127")
+    if length < 16 or length & (length - 1):
+        raise ValueError("length must be a power of 2 and at least 16")
+    if count < 1:
+        raise ValueError("count must be at least 1")
+    opt = options._c()
+    plan = backend.DgProvePlan()
+    backend.check(backend.lib().dg_plan_prove(width, length, count, ctypes.byref(opt), ctypes.byref(plan)))
+    return {"layout": "full" if plan.layout == 0 else "eval_cosets", "group": plan.group, "coset_chunk": plan.coset_chunk,
+            "retained_cosets": plan.retained_cosets, "bytes_per_proof": plan.bytes_per_proof, "fixed_bytes": plan.fixed_bytes,
+            "available_bytes": plan.available_bytes}
+
+
 def _batch_io(public_inputs_list, outputs_list):
     """per-trace public inputs / outputs as the pointer and count arrays of dg_prove_batch (the arrays are kept alive by the caller)"""
     ins = [felt.from_ints(x) for x in public_inputs_list]

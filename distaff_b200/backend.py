@@ -45,6 +45,11 @@ class DgTraceReport(ctypes.Structure):
                 ("op_count_ok", ctypes.c_int32), ("program_hash_matches", ctypes.c_int32)]
 
 
+class DgProvePlan(ctypes.Structure):
+    _fields_ = [("layout", ctypes.c_int32), ("group", u32), ("coset_chunk", u32), ("retained_cosets", u32), ("bytes_per_proof", u64),
+                ("fixed_bytes", u64), ("available_bytes", u64)]
+
+
 DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -108,6 +113,9 @@ EXPORTS = {
     "dg_host_merkle_verify_plan": [vp, u32, u32, u32, vp, u32, vp, ctypes.c_size_t, vp, vp, ctypes.c_size_t, vp, vp],
     "dg_host_periodic_tables": [vp],
     "dg_host_constraint_name": [u32, u32, u32, u32, ctypes.c_char_p, ctypes.c_size_t],
+    "dg_set_memory_limit": [ctypes.c_size_t],
+    "dg_memory_usage": [ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)],
+    "dg_plan_prove": [u32, u64, u32, ctypes.POINTER(DgOptions), ctypes.POINTER(DgProvePlan)],
 }
 VOID_EXPORTS = {"dg_proof_free": [vp]}
 

@@ -127,7 +127,12 @@ static Proof *prove_on_all_devices(F &&prove_rank, dg_prove_stats_t *stats) {
 extern "C" {
 
 int dg_init(int device) { return guarded([&] { ctx_init(device); }); }
-int dg_init_devices(int n_devices) { return guarded([&] { ctx_init_devices(n_devices); }); }
+int dg_init_devices(int n_devices) {
+    return guarded([&] {
+        DG_REQUIRE(n_devices == 1 || ctx().mem_limit == 0, "a memory limit applies to one GPU: clear it (dg_set_memory_limit(0)) before spanning several");
+        ctx_init_devices(n_devices);
+    });
+}
 const char *dg_last_error(void) { return t_last_error.c_str(); }
 
 int dg_device_info(char *name, size_t cap, int *sm_count, size_t *total_mem) {
@@ -525,6 +530,43 @@ int dg_batch_message(uint32_t index, char *message, size_t cap) {
         message[cap - 1] = 0;
     });
 }
+// ---- device memory ------------------------------------------------------------------------------------------------------------
+static void require_one_gpu(const Context &c) {
+    DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "memory limits and plans apply to one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
+}
+int dg_set_memory_limit(size_t bytes) {
+    return guarded([&] {
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        if (bytes) require_one_gpu(c);
+        memory_set_limit(c, bytes);
+    });
+}
+int dg_memory_usage(size_t *held, size_t *peak) {
+    return guarded([&] {
+        DG_REQUIRE(held || peak, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        memory_usage(c, held, peak);
+    });
+}
+int dg_plan_prove(uint32_t width, uint64_t length, uint32_t count, const dg_options_t *options, dg_prove_plan_t *plan) {
+    return guarded([&] {
+        DG_REQUIRE(options && plan, "null argument");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        require_one_gpu(c);
+        const ProvePlan P = plan_prove(c, width, length, options->extension_factor, count);
+        plan->layout = P.full ? DG_LAYOUT_FULL : DG_LAYOUT_EVAL_COSETS;
+        plan->group = (uint32_t)P.group;
+        plan->coset_chunk = P.chunk;
+        plan->retained_cosets = P.full ? options->extension_factor : 8;
+        plan->bytes_per_proof = P.per_proof;
+        plan->fixed_bytes = P.fixed;
+        plan->available_bytes = P.available;
+    });
+}
+
 int dg_set_rng_callbacks(const dg_rng_callbacks_t *callbacks) {
     return guarded([&] {
         if (!callbacks) { fs::set_rng_hooks(nullptr); return; }
@@ -595,7 +637,12 @@ void dg_proof_free(dg_proof_t *proof) { delete (Proof *)proof; }
 // ---- multi-GPU ---------------------------------------------------------------------------------------------------------------------
 int dg_comm_unique_id(uint8_t id128[128]) { return guarded([&] { comm_unique_id(id128); }); }
 int dg_comm_init(int rank, int world, const uint8_t id128[128]) {
-    return guarded([&] { Context &c = ctx(); std::lock_guard<std::mutex> lk(c.mu); comm_init(c, rank, world, id128); });
+    return guarded([&] {
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DG_REQUIRE(world == 1 || c.mem_limit == 0, "a memory limit applies to one GPU: clear it (dg_set_memory_limit(0)) before spanning several");
+        comm_init(c, rank, world, id128);
+    });
 }
 int dg_comm_finalize(void) { return guarded([&] { Context &c = ctx(); std::lock_guard<std::mutex> lk(c.mu); comm_finalize(c); }); }
 int dg_host_shard_locate(uint64_t n, int log_blk, int log_g, int is_node, uint64_t index, int64_t out[3]) {

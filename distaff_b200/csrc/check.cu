@@ -29,9 +29,10 @@ size_t check_footprint(uint32_t w, uint64_t n, bool upload, bool own_masks) {
 
 int check_group_size(uint32_t w, uint64_t n, bool upload, bool own_masks, uint32_t count) {
     long long k = std::min<long long>(count, 65535);
-    size_t free_b = 0, total_b = 0;
-    DG_CUDA(cudaMemGetInfo(&free_b, &total_b));
-    k = std::min<long long>(k, (long long)std::max<size_t>(1, free_b / 10 * 8 / check_footprint(w, n, upload, own_masks)));
+    const size_t per = check_footprint(w, n, upload, own_masks), avail = memory_budget(ctx(), Budget::FREE, per);
+    DG_REQUIRE(!ctx().mem_limit || per <= avail, "a trace check of " + std::to_string(w) + " x " + std::to_string(n) + " needs " + std::to_string(per) +
+                                                     " bytes of device memory beyond what the memory limit leaves");
+    k = std::min<long long>(k, (long long)std::max<size_t>(1, avail / per));
     if (const char *e = getenv("DG_BATCH_GROUP")) {
         const long long cap = atoll(e);
         DG_REQUIRE(cap >= 1, "DG_BATCH_GROUP must be a positive integer");

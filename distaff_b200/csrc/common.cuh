@@ -142,6 +142,8 @@ struct Context {
     std::string last_error;
     unsigned long long launches = 0;        // kernels launched by this library (bench.py's gpu_launches)
     int rank = 0, world = 1;                // multi-GPU sharding (comm.cu); world == 1: no communication
+    size_t mem_limit = 0;                   // most device bytes the library may hold (arena + pool), 0 = no limit (dg_set_memory_limit)
+    size_t mem_peak = 0;                    // most held since the limit was set, up to the last change of the arena (memory_usage)
 
     TwiddleRef twiddle(int log_order, bool inverse);
     std::map<int, DevBuf> single_tables;    // full power tables w^e, e < 2^log_order (small orders only)
@@ -160,6 +162,17 @@ Context &ctx_of(int index);
 void ctx_bind(Context *c);                  // makes c the calling thread's current context (and its device current)
 // raises the dynamic shared-memory limit of a kernel on c's device once
 void set_func_smem(Context &c, const void *func, size_t bytes);
+
+// ---- device-memory budget (context.cu) -------------------------------------------------------------------------------------
+// The one budget of every grouped call (prover, trace check, batched verification).  ARENA (prover): the arena when `need` fits in it,
+// else 80 % of the free memory plus the arena, which the group replaces; FREE: 80 % of the free memory; FIXED: `need` itself.  With a
+// memory limit the result is capped by the limit less what the library holds outside the arena and the `scratch` bytes the call adds.
+enum class Budget { ARENA, FREE, FIXED };
+size_t memory_budget(Context &c, Budget kind, size_t need, size_t scratch = 0);
+size_t memory_held_outside_arena(Context &c);      // pool memory in use: persistent tables, transform scratch, upload buffer
+void arena_release(Context &c);                   // frees the arena (the next proofs run on the pool until it is sized again)
+void memory_set_limit(Context &c, size_t bytes);  // 0 = no limit; resets the peak
+void memory_usage(Context &c, size_t *held, size_t *peak);
 
 // host-side field helpers (portable path of fp128.cuh)
 fe host_root_of_unity(int log_order);            // w of order 2^log_order  (field::get_root_of_unity)

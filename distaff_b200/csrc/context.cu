@@ -33,24 +33,102 @@ ArenaScope::ArenaScope() {
     a.counting = true;
     a.active = a.base != nullptr && !getenv("DG_NO_ARENA");
 }
+static cudaMemPool_t device_pool(const Context &c) {
+    cudaMemPool_t pool = nullptr;
+    if (cudaDeviceGetDefaultMemPool(&pool, c.device) != cudaSuccess) cudaGetLastError();
+    return pool;
+}
+static size_t pool_attr(const Context &c, cudaMemPoolAttr attr) {
+    unsigned long long v = 0;
+    if (cudaMemPoolGetAttribute(device_pool(c), attr, &v) != cudaSuccess) cudaGetLastError();
+    return (size_t)v;
+}
+// folds what was held since the last fold (the arena + the pool's high-water mark) into the peak, and restarts the pool's mark; called
+// whenever the arena changes size (no error is raised: it runs in destructors)
+static void reset_pool_high(Context &c) {
+    unsigned long long zero = 0;       // restarts the mark at the current reservation
+    if (cudaMemPoolSetAttribute(device_pool(c), cudaMemPoolAttrReservedMemHigh, &zero) != cudaSuccess) cudaGetLastError();
+}
+static void fold_peak(Context &c) {
+    c.mem_peak = std::max(c.mem_peak, c.arena.cap + pool_attr(c, cudaMemPoolAttrReservedMemHigh));
+    reset_pool_high(c);
+}
+
+// the pool keeps what it frees up to what the limit leaves beside the arena (everything without a limit)
+static void apply_release_threshold(Context &c) {
+    unsigned long long threshold = ~(unsigned long long)0;
+    if (c.mem_limit) threshold = c.mem_limit > c.arena.cap ? c.mem_limit - c.arena.cap : 0;
+    if (cudaMemPoolSetAttribute(device_pool(c), cudaMemPoolAttrReleaseThreshold, &threshold) != cudaSuccess) cudaGetLastError();
+}
+
 ArenaScope::~ArenaScope() {
     Arena &a = arena();
     a.counting = false;
     const bool overflowed = a.counted > a.cap;
     a.active = false;
     if (overflowed && !getenv("DG_NO_ARENA")) {          // grow for the next proof of this size (driver call, outside the timed path)
+        Context &c = ctx();
         cudaStreamSynchronize(alloc_stream());
+        fold_peak(c);
         if (a.base) cudaFree(a.base);
         a.base = nullptr;
         a.cap = 0;
         const size_t want = a.counted + (a.counted >> 4) + (64 << 20);
-        cudaMemPool_t pool;                               // hand the measuring proof's pool memory back before taking the arena
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) cudaMemPoolTrimTo(pool, 0);
-        if (cudaMalloc(&a.base, want) == cudaSuccess) a.cap = want;
+        // hand the measuring proof's pool memory back before taking the arena
+        cudaMemPoolTrimTo(device_pool(c), 0);
+        reset_pool_high(c);
+        // under a memory limit an arena that does not fit beside what the pool holds is not taken: the proofs keep running on the pool
+        const bool fits = !c.mem_limit || want + pool_attr(c, cudaMemPoolAttrReservedMemCurrent) <= c.mem_limit;
+        if (fits && cudaMalloc(&a.base, want) == cudaSuccess) a.cap = want;
         else { a.base = nullptr; cudaGetLastError(); }
+        apply_release_threshold(c);
+        fold_peak(c);
     }
+}
+
+void arena_release(Context &c) {
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+    fold_peak(c);
+    if (c.arena.base) cudaFree(c.arena.base);
+    c.arena.base = nullptr;
+    c.arena.cap = 0;
+    apply_release_threshold(c);
+}
+
+size_t memory_held_outside_arena(Context &c) { return pool_attr(c, cudaMemPoolAttrUsedMemCurrent); }
+
+size_t memory_budget(Context &c, Budget kind, size_t need, size_t scratch) {
+    size_t avail = need;
+    if (kind == Budget::ARENA && need <= c.arena.cap) {
+        avail = c.arena.cap;
+    } else if (kind != Budget::FIXED) {                  // does not fit in the arena the library already holds: ask the driver
+        size_t free_b = 0, total_b = 0;
+        DG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+        avail = (free_b + (kind == Budget::ARENA ? c.arena.cap : 0)) / 10 * 8;
+    }
+    if (c.mem_limit) {
+        const size_t held = memory_held_outside_arena(c) + scratch;
+        avail = std::min(avail, c.mem_limit > held ? c.mem_limit - held : 0);
+    }
+    return avail;
+}
+
+void memory_set_limit(Context &c, size_t bytes) {
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+    c.mem_limit = bytes;
+    apply_release_threshold(c);
+    if (bytes) {
+        if (c.arena.cap + memory_held_outside_arena(c) > bytes) arena_release(c);
+        DG_CUDA(cudaMemPoolTrimTo(device_pool(c), bytes > c.arena.cap ? bytes - c.arena.cap : 0));
+    }
+    fold_peak(c);
+    c.mem_peak = c.arena.cap + pool_attr(c, cudaMemPoolAttrReservedMemCurrent);
+}
+
+void memory_usage(Context &c, size_t *held, size_t *peak) {
+    const size_t now = c.arena.cap + pool_attr(c, cudaMemPoolAttrReservedMemCurrent);
+    if (held) *held = now;
+    if (peak) *peak = std::max(c.mem_peak, c.arena.cap + pool_attr(c, cudaMemPoolAttrReservedMemHigh));
 }
 
 static std::mutex g_ctx_mu;

@@ -299,6 +299,61 @@ void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, 
     DG_CUDA(cudaGetLastError());
 }
 
+// ---- trace rows at LDE positions (openings outside the retained cosets) -------------------------------------------------------------------
+// Row `pos` of the trace extension is (P_0(x), ..., P_{w-1}(x)) at x = w_N^pos.  Block (m, y) evaluates the w columns of point m's proof
+// on the tiles y, y + gridDim.y, ... of ROW_TILE coefficients: the tile's powers x^k = w_N^(pos k mod N) go to shared memory once (two-level
+// table, one product each) and are shared by all w columns; warp v sums columns v, v + 8, ..., each lane ROW_TILE / 32 = 64 products
+// accumulated unreduced (288 bits, < 128 products) and reduced once, then the warp's lanes are added into the column's shared sum.
+// partial[(m w + j) * gridDim.y + y] = the block's sum for column j.
+static const int ROW_TILE = 2048, ROW_MAX_BLOCKS = 64;
+__global__ void __launch_bounds__(256) eval_rows_partial_kernel(const fe *__restrict__ polys, unsigned long long n, int w, const ulonglong2 *__restrict__ pts,
+                                                                TwiddleRef twN, fe *__restrict__ partial) {
+    __shared__ fe s_pw[ROW_TILE];
+    __shared__ fe s_acc[128];
+    const ulonglong2 pt = pts[blockIdx.x];                           // (proof, LDE position)
+    const fe *p = polys + pt.x * (unsigned long long)w * n;
+    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int j = threadIdx.x; j < w; j += blockDim.x) s_acc[j] = fe_make(0, 0);
+    const unsigned long long tile = n < (unsigned long long)ROW_TILE ? n : (unsigned long long)ROW_TILE;
+    for (unsigned long long k0 = (unsigned long long)blockIdx.y * tile; k0 < n; k0 += (unsigned long long)gridDim.y * tile) {
+        __syncthreads();                                             // the previous tile's powers are no longer read
+        for (unsigned i = threadIdx.x; i < tile; i += blockDim.x) {
+            const unsigned e = (unsigned)((pt.y * (k0 + i)) & twN.mask);
+            s_pw[i] = fe_mul(twN.lo[e & ((1u << twN.lo_bits) - 1u)], twN.hi[e >> twN.lo_bits]);
+        }
+        __syncthreads();
+        for (int j = warp; j < w; j += 8) {
+            const fe *col = p + (unsigned long long)j * n + k0;
+            fe v = fe_make(0, 0);
+            if (lane < tile) {
+                fe_wide acc;
+                wide_set(acc, DG_MUL_WIDE(col[lane], s_pw[lane]));
+                for (unsigned i = lane + 32; i < tile; i += 32) wide_add(acc, DG_MUL_WIDE(col[i], s_pw[i]));
+                v = DG_REDUCE_WIDE(acc);
+            }
+#pragma unroll
+            for (int d = 16; d >= 1; d >>= 1) v = fe_add(v, shfl_down_fe(v, d));
+            if (lane == 0) s_acc[j] = fe_add(s_acc[j], v);
+        }
+    }
+    __syncthreads();
+    for (int j = threadIdx.x; j < w; j += blockDim.x) partial[((unsigned long long)blockIdx.x * w + j) * gridDim.y + blockIdx.y] = s_acc[j];
+}
+void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, int w, const std::vector<std::pair<uint32_t, uint64_t>> &points, int log_N, fe *out) {
+    DG_REQUIRE(w >= 1 && w <= 128 && !points.empty() && points.size() < (1ULL << 31), "opened-row evaluation out of range");
+    std::vector<ulonglong2> host(points.size());
+    for (size_t m = 0; m < points.size(); m++) host[m] = make_ulonglong2(points[m].first, points[m].second);
+    DevBuf d_pts(host.size() * sizeof(ulonglong2));
+    DG_CUDA(cudaMemcpyAsync(d_pts.p, host.data(), d_pts.bytes, cudaMemcpyHostToDevice, c.stream));
+    const unsigned tiles = (unsigned)((n + ROW_TILE - 1) / ROW_TILE), by = std::min<unsigned>(tiles, ROW_MAX_BLOCKS);
+    DevBuf partial(host.size() * w * by * sizeof(fe));
+    // the points run on x, so the blocks of one tile and many points are resident together and share its coefficients through L2
+    eval_rows_partial_kernel<<<dim3((unsigned)host.size(), by), 256, 0, c.stream>>>(polys, n, w, d_pts.as<ulonglong2>(), c.twiddle(log_N, false),
+                                                                                  partial.as<fe>()); c.launches++;
+    reduce_partials_kernel<<<(unsigned)(host.size() * w), 32, 0, c.stream>>>(partial.as<fe>(), out, by); c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
 // ---- linear combinations ------------------------------------------------------------------------------------------------------------------
 // t1[k] = sum_i cc1[i] P_i[k],  t2[k] = sum_i cc2[i] P_i[k]
 // blockIdx.y = proof of a batch: polys w n, cc1 / cc2 cc_stride, t1 / t2 t_stride elements apart

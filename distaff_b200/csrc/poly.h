@@ -29,6 +29,9 @@ void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, 
 // cols_per_proof < cols: the columns of several proofs, proof q's powers of z at zt moved by q * (lo, hi) strides
 void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, const PowRef &zt, const TwiddleRef &gt, bool two_points, fe *out,
                    int cols_per_proof = 1 << 30, unsigned long long zt_stride_lo = 0, unsigned long long zt_stride_hi = 0);
+// rows of the trace extension computed from the trace polynomials: out[m w + j] = P_j(w_N^pos) of proof q for points[m] = (q, pos), with
+// proof q's w polynomials of n coefficients at polys + q w n; one launch for all points (plus the reduction of the tile sums)
+void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, int w, const std::vector<std::pair<uint32_t, uint64_t>> &points, int log_N, fe *out);
 // `batch` proofs: polys, coef, ic / fc of proof q at q * the strides, its constants KiA, KiB, KfA, KfB = K[4q .. 4q + 4) on the device
 void boundary_coeffs(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
                      unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride);
@@ -43,8 +46,10 @@ void compose(Context &c, int batch, const fe *t1q, const fe *t2q, unsigned long 
              unsigned long long len, unsigned long long inc, const fe *ks);
 
 // ---- hashing (hash.cu) ----
-// batch > 1: `batch` matrices ext_stride elements apart, their leaves N = n << log_blowup digests apart
-void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup, int batch = 1, unsigned long long ext_stride = 0);
+// ext: the cosets [c0, c0 + nc) of every column ([w][nc][n], column stride nc n; nc = 0: all 2^log_blowup); the row of coset c at step k
+// is leaf (k << log_blowup) + c.  batch > 1: `batch` matrices ext_stride elements apart, their leaves leaf_stride digests apart (0: N)
+void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup, int batch = 1, unsigned long long ext_stride = 0,
+                     unsigned c0 = 0, unsigned nc = 0, unsigned long long leaf_stride = 0);
 // digests of the rows of a plain column-major [w][rows] matrix
 void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows);
 void hash64_contiguous(Context &c, const void *in, void *out, unsigned long long count);

@@ -112,8 +112,7 @@ void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, 
         lde_batch(c, polys, ext, log_n, log_b, 1, cols, n, N_loc, c0, nc);
         return;
     }
-    DG_REQUIRE(nc >= 2, "coset range too small");
-    lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
+    if (nc > 1) lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
     DG_CUDA(cudaMemcpy2DAsync(ext, N_loc * sizeof(fe), regs, n * sizeof(fe), n * sizeof(fe), cols, cudaMemcpyDeviceToDevice, c.stream));
 }
 
@@ -280,8 +279,10 @@ struct OpenPlan {
 // FRI roots, PoW, openings) moves the values of all K proofs at once.
 // d_regs: register traces in device memory, [K][w][n]; when `host_cols` (K * w column pointers) is given they are not there yet: column
 // chunks are uploaded on the copy stream while the previous chunk is being interpolated and extended (the upload hides behind the LDE).
+// chunk (one GPU): cosets of the trace extension held at a time (ProvePlan).  The full layout (chunk = b) keeps the whole extension; the
+// evaluation-coset layout (chunk < b) extends and hashes chunk cosets at a time and keeps only the 8 cosets stage 3 reads.
 static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, int K, uint32_t width, uint64_t length, uint32_t ctx_depth,
-                       uint32_t loop_depth, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats) {
+                       uint32_t loop_depth, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats, unsigned chunk) {
     // ---- argument checks (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) -----------------------------------------------
     const uint64_t n = length, b = opt.extension_factor;
     DG_REQUIRE(K >= 1 && (int)ps.size() == K, "batch must hold at least one trace");
@@ -336,24 +337,51 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     const int cpr = (w + G - 1) / G;                           // slot size of the gather = largest share
     auto col_count = [&](int r) { return w / G + (r < w % G ? 1 : 0); };
     auto col_start = [&](int r) { return r * (w / G) + std::min(r, w % G); };
-    DevBuf polys(W * n * 16), ext(W * N_loc * 16);
+    // Layout of the extension.  ext holds `chunk` cosets of every column at a time ([K][w][chunk][n]).  The retained slab holds the cosets
+    // stage 3 reads: in the full layout the whole extension (slab = ext), in the evaluation-coset layout the 8 cosets c = 0 (mod b / 8),
+    // [K][w][8][n].  An opened row outside the retained cosets is computed from the trace polynomials in stage 9.
+    if (G > 1 || chunk == 0 || chunk > nc) chunk = (unsigned)nc;
+    DG_REQUIRE((chunk & (chunk - 1)) == 0, "coset chunk must be a power of 2");
+    const bool full = chunk == nc;
+    const int log_ret = full ? log_nc : 3;                     // retained cosets: all of this rank's, or the 8 evaluation cosets
+    const uint64_t slab_col = n << log_ret, rstep = nc >> log_ret;      // slab column stride; retained cosets are c = 0 (mod rstep)
+    const uint64_t ext_col = n * chunk;                        // column stride of ext (N_loc in the full layout)
+    DevBuf polys(W * n * 16), ext(W * ext_col * 16), slab_own;
+    if (!full) slab_own.alloc(W * slab_col * 16);
+    const fe *slab = full ? ext.as<fe>() : slab_own.as<fe>();
+    DevBuf t_leaves((size_t)K * N_loc * 32), t_nodes;
+    // rows of the chunk at cc: leaves (k << log_b) + c of every proof; then its retained cosets into the slab
+    auto hash_chunk = [&](unsigned cc) {
+        hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, (size_t)w * ext_col, cc, chunk, N_loc);   // local rows, [k][c - c0], per proof
+        if (full) return;
+        for (unsigned cs = cc; cs < cc + chunk; cs++)
+            if (cs % rstep == 0)
+                DG_CUDA(cudaMemcpy2DAsync(slab_own.as<fe>() + (cs / rstep) * n, slab_col * 16, ext.as<fe>() + (size_t)(cs - cc) * n, ext_col * 16, n * 16, W,
+                                          cudaMemcpyDeviceToDevice, c.stream));
+    };
     if (G == 1) {
-        // the K proofs' registers are K * w columns of one batch
-        if (!host_cols) {
-            ntt_batch(c, d_regs, polys.as<fe>(), log_n, (int)W, n, n, true);
-            extend_trace_columns(c, polys.as<fe>(), d_regs, ext.as<fe>(), (int)W, log_n, log_b, N_loc, c0, (unsigned)nc);
+        // the K proofs' registers are K * w columns of one batch, interpolated in column chunks: a host trace is uploaded in chunks of
+        // ~64 MB, but a short ramp first (1, 2 columns), so that the first transform starts after one column's worth of copying; every
+        // column chunk is extended on the first coset chunk as soon as it has been interpolated
+        std::vector<int> bounds = {0};
+        std::unique_ptr<TraceUploader> up;
+        if (host_cols) {
+            const int step_max = (int)std::max<uint64_t>(1, std::min<uint64_t>(W, ((uint64_t)1 << 26) / (n * 16)));
+            for (int step = 1; bounds.back() < (int)W; step = std::min(step_max, step * 2)) bounds.push_back(std::min((int)W, bounds.back() + step));
+            up.reset(new TraceUploader(c, d_regs, host_cols, (int)W, n, bounds));
         } else {
-            // chunks of ~64 MB, but a short ramp first (1, 2 columns): the first transform starts after one column's worth of copying
-            const int chunk = (int)std::max<uint64_t>(1, std::min<uint64_t>(W, ((uint64_t)1 << 26) / (n * 16)));
-            std::vector<int> bounds = {0};
-            for (int step = 1; bounds.back() < (int)W; step = std::min(chunk, step * 2)) bounds.push_back(std::min((int)W, bounds.back() + step));
-            TraceUploader up(c, d_regs, host_cols, (int)W, n, bounds);
-            for (int i = 0; i < up.chunks(); i++) {
+            bounds.push_back((int)W);
+        }
+        for (unsigned cc = 0; cc < nc; cc += chunk) {
+            if (cc > 0) hash_chunk(cc - chunk);                // the last chunk is hashed in stage 2
+            for (size_t i = 0; i + 1 < bounds.size(); i++) {
                 const int j0 = bounds[i], cols = bounds[i + 1] - j0;
-                up.wait_chunk(i);
-                ntt_batch(c, d_regs + (size_t)j0 * n, polys.as<fe>() + (size_t)j0 * n, log_n, cols, n, n, true);
-                extend_trace_columns(c, polys.as<fe>() + (size_t)j0 * n, d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * N_loc, cols, log_n, log_b, N_loc,
-                                     c0, (unsigned)nc);
+                if (cc == 0) {
+                    if (up) up->wait_chunk((int)i);
+                    ntt_batch(c, d_regs + (size_t)j0 * n, polys.as<fe>() + (size_t)j0 * n, log_n, cols, n, n, true);
+                }
+                extend_trace_columns(c, polys.as<fe>() + (size_t)j0 * n, d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * ext_col, cols, log_n, log_b,
+                                     ext_col, cc, chunk);
             }
         }
     } else {
@@ -398,13 +426,12 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         cudaEventDestroy(ev_own);
         cudaEventDestroy(ev_all);
     }
-    auto ext_of = [&](int p) { return ext.as<fe>() + (size_t)p * w * N_loc; };
+    auto slab_of = [&](int p) { return slab + (size_t)p * w * slab_col; };
 
     // ---- 2: trace Merkle tree ----------------------------------------------------------------------------------------------------------
     clk.mark(1);
     sub.mark("1.lde");
-    DevBuf t_leaves((size_t)K * N_loc * 32), t_nodes;
-    hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, (size_t)w * N_loc);      // local rows, [k][c - c0], per proof
+    hash_chunk((unsigned)(nc - chunk));
     sub.mark("2.hash_rows");
     {
         // one GPU: the K trees level by level in one launch per level; several GPUs (K == 1): the sharded tree
@@ -490,18 +517,20 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         memset(&P, 0, sizeof P);
         P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
         P.cl = std::max<int>(ctx_depth, 1); P.ll = std::max<int>(loop_depth, 1); P.sl = std::max(stack_depth, 8);
-        P.log_n = log_n; P.log_blowup = log_b;
-        P.ext = ext.as<fe>(); P.col_stride = N_loc;
+        // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
+        // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
+        P.log_n = log_n; P.log_blowup = full ? log_b : 3;
+        P.ext = slab; P.col_stride = slab_col;
         P.c8_base = g * num_c8; P.num_c8 = num_c8;
         P.t_ev = evals_loc.as<fe>();
         P.periodic = d_periodic.as<fe>();
         const fe *base = d_coef.as<fe>();
         P.coefA = base; P.coefB = base + T;
-        P.twN = c.twiddle(log_N, false);
+        P.twN = c.twiddle(full ? log_N : log_n + 3, false);
         static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
         for (int gi = 0; gi < 6; gi++) P.inc[gi] = (8 * n - 1) - (n - 1) * GROUP_DEG[gi];
         P.violation = d_violation.as<unsigned>();
-        P.ext_stride = (size_t)w * N_loc; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
+        P.ext_stride = (size_t)w * slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
     sub.mark("3.setup");
         launch_constraint_eval(c, P, K);
     sub.mark("3.eval");
@@ -807,18 +836,43 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             for (size_t off : o[i]) v[i].push_back(fb.digest(off));
         return v;
     };
-    auto plan_openings = [&](ProofState &s, const fe *ext_p, const fe *c_ext_p) {
+    // opened trace rows outside the retained cosets (evaluation-coset layout): the trace polynomials at w_N^pos, all proofs in one launch,
+    // into d_rows ([m][w], m = computed row of the batch in proof and query order)
+    auto retained = [&](uint64_t pos) { return ((pos & (b - 1)) & (rstep - 1)) == 0; };
+    DevBuf d_rows;
+    std::vector<size_t> first_row(K, 0);
+    {
+        std::vector<std::pair<uint32_t, uint64_t>> points;
+        for (int p = 0; p < K; p++) {
+            first_row[p] = points.size();
+            if (ps[p].live)
+                for (uint64_t pos : ps[p].positions)
+                    if (!retained(pos)) points.emplace_back((uint32_t)p, pos);
+        }
+        if (!points.empty()) {
+            d_rows.alloc(points.size() * w * 16);
+            eval_trace_rows(c, polys.as<fe>(), n, w, points, log_N, d_rows.as<fe>());
+        }
+    }
+    auto plan_openings = [&](ProofState &s, const fe *slab_p, const fe *c_ext_p, size_t row0) {
         OpenPlan O;
         const std::vector<uint64_t> &positions = s.positions;
         const int nq = (int)positions.size();
-        // trace rows at the queried positions (trace_table.rs:127-134): the rank owning the position's coset reads the row
+        // trace rows at the queried positions (trace_table.rs:127-134): the rank owning the position's coset reads the row from the retained
+        // slab, or it was computed into d_rows
         O.row_off.resize(nq);
         for (int q = 0; q < nq; q++) {
             const uint64_t cpos = positions[q] & (b - 1), k = positions[q] >> log_b;
+            if (!retained(positions[q])) {
+                O.row_off[q] = fb.add16(FetchRef{d_rows.p, row0 * w, -1});
+                for (int j = 1; j < w; j++) fb.add16(FetchRef{d_rows.p, row0 * w + j, -1});
+                row0++;
+                continue;
+            }
             const int owner = (int)(cpos >> log_nc);
-            const uint64_t phys = ((cpos - (uint64_t)owner * nc) << log_n) + k;
+            const uint64_t phys = (((cpos - (uint64_t)owner * nc) / rstep) << log_n) + k;
             for (int j = 0; j < w; j++) {
-                const size_t off = fb.add16(FetchRef{ext_p + (size_t)j * N_loc, phys, owner});
+                const size_t off = fb.add16(FetchRef{slab_p + (size_t)j * slab_col, phys, owner});
                 if (j == 0) O.row_off[q] = off;
             }
         }
@@ -923,7 +977,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         std::vector<OpenPlan> plans(K);
         for (int p = 0; p < K; p++)
-            if (ps[p].live) plans[p] = plan_openings(ps[p], ext_of(p), c_ext_of(p));
+            if (ps[p].live) plans[p] = plan_openings(ps[p], slab_of(p), c_ext_of(p), first_row[p]);
         fb.run();
         for (int p = 0; p < K; p++)
             if (ps[p].live) serialise(ps[p], plans[p]);
@@ -957,24 +1011,23 @@ std::vector<ProofState> make_states(uint32_t count, const uint8_t *const *inputs
     return ps;
 }
 
-// the single-trace entry points: a batch of one whose failure is the call's error
-Proof *prove_one(Context &c, fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                 const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
-                 dg_prove_stats_t *stats) {
-    std::vector<ProofState> ps = make_states(1, &inputs16, &n_inputs, &outputs16, &n_outputs);
-    prove_core(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, ps, opt, stats);
-    if (ps[0].status != DG_OK) throw Error(ps[0].status, ps[0].message);
-    return ps[0].proof.release();
-}
+}  // namespace
 
 // Device bytes one proof of this shape takes in a batch on one GPU: the buffers prove_core allocates per proof, stage by stage (every
-// one stays in the bump arena until the group ends), plus its register columns (the upload buffer of a host batch).
-size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b) {
+// one stays in the bump arena until the group ends), plus its register columns (the upload buffer of a host batch).  chunk: cosets of
+// the trace extension held at a time; b is the full layout, fewer the evaluation-coset layout (a chunk and the 8 retained cosets).
+size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b, uint32_t chunk) {
     const size_t N = (size_t)n * b, E = (size_t)n * 8, fe16 = 16, dg32 = 32;
     size_t f = 0;
     f += (size_t)w * n * fe16;                // registers (host batch: upload buffer)
     f += (size_t)w * n * fe16;                // 1: polynomials
-    f += (size_t)w * N * fe16;                // 1: trace LDE
+    if (chunk >= b) {
+        f += (size_t)w * N * fe16;            // 1: trace LDE
+    } else {
+        f += (size_t)w * n * (chunk + 8) * fe16;      // 1: a coset chunk of the trace LDE + the 8 retained cosets
+        const size_t tiles = std::min<size_t>(64, (n + 2047) / 2048);
+        f += (size_t)128 * (w * (tiles + 1) + 1) * fe16;   // 9: computed opened rows (<= 128 queries), their tile sums and points
+    }
     f += 2 * N * dg32;                        // 2: row hashes + tree
     f += 3 * E * fe16 + E * fe16;             // 3: i / f / t coefficients, coset-local transition evaluations
     f += 3 * E * fe16;                        // 4: combined polynomial + the two division scratch vectors
@@ -994,21 +1047,89 @@ size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b) {
 // dimension, which holds at most 65535 blocks.
 int max_group_for_grid(uint32_t w) { return (int)(65535 / std::max<uint32_t>(w, 1)); }
 
-int batch_group_size(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count) {
-    const size_t per = proof_footprint(w, n, b);
-    long long k = std::min<long long>(count, max_group_for_grid(w));
-    if ((size_t)count * per > c.arena.cap) {                 // does not fit in the arena the library already holds: ask the driver
-        size_t free_b = 0, total_b = 0;
-        DG_CUDA(cudaMemGetInfo(&free_b, &total_b));
-        const size_t avail = (free_b + c.arena.cap) / 10 * 8;
-        k = std::min<long long>(k, (long long)std::max<size_t>(1, avail / per));
-    }
+int batch_group_cap(long long k) {
     if (const char *e = getenv("DG_BATCH_GROUP")) {
         const long long cap = atoll(e);
         DG_REQUIRE(cap >= 1, "DG_BATCH_GROUP must be a positive integer");
         k = std::min(k, cap);
     }
     return (int)k;
+}
+
+// Transform scratch and tables a prove call adds outside the arena (persistent, from the pool): the multi-pass LDE of a coset chunk
+// (<= 4 GiB), the other multi-pass transforms (<= 1 GiB) and the merged first-pass twiddles of the trace LDE (<= 1 GiB), less what the
+// library holds already
+static size_t prove_scratch(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t chunk, long long k) {
+    const size_t four = (size_t)4 << 30, one = (size_t)1 << 30;
+    const size_t ntt = std::max(std::min(four, (size_t)(16 * n * chunk * w * k)), std::min(one, (size_t)(16 * n * b * k)));
+    size_t add = ntt > c.ntt_tmp.bytes ? ntt - c.ntt_tmp.bytes : 0;
+    const size_t table = (size_t)16 * n * b;
+    int log_n = 0, log_b = 0;
+    while ((1ULL << log_n) < n) log_n++;
+    while ((1u << log_b) < b) log_b++;
+    bool have = false;
+    for (auto &t : c.lde_twiddles) have |= (t.first >> 8) == (((long long)log_n << 8) | log_b);
+    if (table <= one && !have) add += table;
+    return add;
+}
+
+ProvePlan plan_prove(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count) {
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
+    DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0 && n <= (1ULL << 30), "execution trace length must be a power of 2 and at least 16");
+    DG_REQUIRE(w >= 1 && w < 128, "execution trace cannot have more than 128 registers");
+    const long long k_max = std::min<long long>(count, max_group_for_grid(w));
+    // the largest group of the layout that keeps `ch` cosets at a time (0 if not even one proof fits); the scratch grows with the group
+    auto group_of = [&](uint32_t ch, size_t &avail) {
+        const size_t per = proof_footprint(w, n, b, ch);
+        avail = memory_budget(c, Budget::ARENA, (size_t)k_max * per, prove_scratch(c, w, n, b, ch, 1));
+        long long g = std::min<long long>(k_max, (long long)(avail / per));
+        while (g > 1 && (size_t)g * per > memory_budget(c, Budget::ARENA, (size_t)g * per, prove_scratch(c, w, n, b, ch, g))) g = g * 3 / 4;
+        return g;
+    };
+    // the full layout when a group of one proof fits; else the evaluation-coset layout with the largest coset chunk that fits
+    for (uint32_t ch = b; ch >= 1; ch = ch == b ? b / 2 : ch / 2) {
+        size_t avail = 0;
+        const long long g = group_of(ch, avail);
+        if (g < 1) continue;
+        ProvePlan P;
+        P.full = ch == b;
+        P.chunk = ch;
+        P.per_proof = proof_footprint(w, n, b, ch);
+        P.fixed = memory_held_outside_arena(c) + prove_scratch(c, w, n, b, ch, g);
+        P.group = batch_group_cap(g);
+        P.available = avail;
+        return P;
+    }
+    const size_t need = proof_footprint(w, n, b, 1) + memory_held_outside_arena(c) + prove_scratch(c, w, n, b, 1, 1);
+    throw Error(DG_ERR_INVALID, "a proof of " + std::to_string(w) + " x " + std::to_string(n) + " at extension factor " + std::to_string(b) + " needs " +
+                                    std::to_string(need) + " bytes of device memory; the memory limit is " + std::to_string(c.mem_limit) + " bytes");
+}
+
+namespace {
+
+// before a group runs under a memory limit: an arena too small for it is released, so that the group runs on the pool alone and what the
+// library holds stays within the limit (the arena is sized again, within the limit, after the group)
+void prepare_arena(Context &c, const ProvePlan &P) {
+    if (c.mem_limit && c.arena.base && (size_t)P.group * P.per_proof > c.arena.cap) arena_release(c);
+}
+
+// the single-trace entry points: a batch of one whose failure is the call's error
+Proof *prove_one(Context &c, fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                 const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
+                 dg_prove_stats_t *stats) {
+    std::vector<ProofState> ps = make_states(1, &inputs16, &n_inputs, &outputs16, &n_outputs);
+    unsigned chunk = 0;
+    if (c.world == 1) {
+        DG_REQUIRE(opt.extension_factor >= 16 && opt.extension_factor <= 256 && (opt.extension_factor & (opt.extension_factor - 1)) == 0,
+                   "extension_factor must be a power of 2 between 16 and 256");
+        const ProvePlan P = plan_prove(c, width, length, opt.extension_factor, 1);
+        prepare_arena(c, P);
+        chunk = P.chunk;
+    }
+    prove_core(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, ps, opt, stats, chunk);
+    if (ps[0].status != DG_OK) throw Error(ps[0].status, ps[0].message);
+    return ps[0].proof.release();
 }
 
 void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
@@ -1018,12 +1139,15 @@ void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
     sum->kernel_launches += s.kernel_launches;
 }
 
-// runs the batch group by group; run_group(first, k, states, stats) proves traces [first, first + k)
+// runs the batch group by group; run_group(first, k, states, stats, chunk) proves traces [first, first + k) with the plan's coset chunk
 template <typename F>
 void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_options_t &opt, std::vector<ProofState> &all, Proof **proofs_out,
                   int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, F &&run_group) {
     DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
-    const int group = batch_group_size(c, w, n, opt.extension_factor, count);
+    DG_REQUIRE(opt.extension_factor >= 16 && opt.extension_factor <= 256 && (opt.extension_factor & (opt.extension_factor - 1)) == 0,
+               "extension_factor must be a power of 2 between 16 and 256");
+    const ProvePlan plan = plan_prove(c, w, n, opt.extension_factor, count);
+    const int group = plan.group;
     if (stats) memset(stats, 0, sizeof *stats);
     for (uint32_t i = 0; i < count; i++) { proofs_out[i] = nullptr; status[i] = DG_OK; }
     messages.assign(count, std::string());
@@ -1038,7 +1162,8 @@ void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_o
         for (int i = 0; i < k; i++) ps.push_back(std::move(all[first + i]));
         dg_prove_stats_t st;
         memset(&st, 0, sizeof st);
-        run_group(first, k, ps, &st);
+        prepare_arena(c, plan);
+        run_group(first, k, ps, &st, plan.chunk);
         if (stats) add_stats(stats, st);
         for (int i = 0; i < k; i++) {
             status[first + i] = ps[i].status;
@@ -1081,11 +1206,11 @@ void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, cons
     }
     DG_REQUIRE(t0.length >= 16 && (t0.length & (t0.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
-    prove_groups(c, count, t0.width, t0.length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st) {
+    prove_groups(c, count, t0.width, t0.length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
         std::vector<const uint8_t *> cols;
         for (int i = 0; i < k; i++) cols.insert(cols.end(), traces[first + i].columns, traces[first + i].columns + t0.width);
         c.upload_buf.ensure((size_t)t0.length * 16 * t0.width * k, true);
-        prove_core(c, c.upload_buf.as<fe>(), cols.data(), k, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, ps, opt, st);
+        prove_core(c, c.upload_buf.as<fe>(), cols.data(), k, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, ps, opt, st, chunk);
     });
 }
 
@@ -1094,8 +1219,8 @@ void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t w
                         const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats) {
     DG_REQUIRE(count >= 1, "batch must hold at least one trace");
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
-    prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st) {
-        prove_core(c, const_cast<fe *>(d_regs) + (size_t)first * width * length, nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st);
+    prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
+        prove_core(c, const_cast<fe *>(d_regs) + (size_t)first * width * length, nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st, chunk);
     });
 }
 

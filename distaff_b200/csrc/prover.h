@@ -26,6 +26,20 @@ void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t w
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                         const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
 
+// What a prove call of one shape does on one GPU (dg_plan_prove): the full layout keeps the whole trace extension; the evaluation-coset
+// layout extends and hashes `chunk` cosets at a time, keeps the 8 cosets the constraint evaluation reads and computes the other opened
+// rows from the trace polynomials.  Proofs run in groups of `group`; per_proof bytes each (arena) on top of `fixed` bytes outside the
+// arena (persistent tables, transform scratch); `available` is the budget the group was fitted into.  Throws DG_ERR_INVALID with the
+// bytes needed when not even one proof fits.
+struct ProvePlan {
+    bool full = true;
+    unsigned chunk = 0;
+    int group = 1;
+    size_t per_proof = 0, fixed = 0, available = 0;
+};
+ProvePlan plan_prove(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count);
+size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b, uint32_t chunk);
+
 // copies `cols` host register columns of n elements each to d_regs (column stride n) by the prover's upload path (pinned columns DMA'd
 // directly, pageable ones staged through the library's pinned slots) and orders c.stream after the copies
 void upload_trace_columns(Context &c, fe *d_regs, const uint8_t *const *host_cols, int cols, uint64_t n);

@@ -842,7 +842,7 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     }
 }
 
-// Proofs per group: a fixed device-memory budget, at most 65535 proofs of one shape (the constraint launch puts them on the grid's y
+// Proofs per group: a fixed device-memory budget (capped by the memory limit), at most 65535 proofs of one shape (the constraint launch puts them on the grid's y
 // dimension) and $DG_BATCH_GROUP.
 const size_t GROUP_BYTES = (size_t)512 << 20;
 
@@ -881,11 +881,12 @@ void verify_proofs(Context &c, const std::vector<VerifyRequest> &req, std::vecto
         groups++;
         g.clear(); per_shape.clear(); bytes = 0;
     };
+    const size_t group_bytes = memory_budget(c, Budget::FIXED, GROUP_BYTES);
     for (Item &it : items) {
         if (it.decided) continue;
         const size_t b = item_bytes(it);
         const std::array<int, 3> shape{it.P.ctx_depth, it.P.loop_depth, it.P.stack_depth};
-        if (!g.empty() && (bytes + b > GROUP_BYTES || g.size() >= cap || per_shape[shape] >= 65535)) flush();
+        if (!g.empty() && (bytes + b > group_bytes || g.size() >= cap || per_shape[shape] >= 65535)) flush();
         g.push_back(&it);
         per_shape[shape]++;
         bytes += b;

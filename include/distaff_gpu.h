@@ -127,6 +127,34 @@ int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t wid
                            const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                            const uint8_t *program_hashes32, dg_trace_report_t *reports, uint32_t *d_step_masks);
 
+/* ---- device memory ----------------------------------------------------------------------------------------------------------------
+ * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
+ * allocates from otherwise, and its persistent tables.  0 (the default) means no limit.  The arena is never sized above the limit and the
+ * pool keeps no more freed memory than the limit leaves beside the arena.  Every prove call is planned against the limit: a shape whose
+ * whole trace extension (16 w n b bytes per proof) fits is proven as without a limit (the full layout); otherwise the prover extends and
+ * hashes the extension a chunk of cosets at a time and keeps only the 8 cosets the constraint evaluation reads (the evaluation-coset
+ * layout), computing the other opened rows from the trace polynomials.  Both layouts give the same proof bytes.  A call that does not fit
+ * in either way fails with DG_ERR_INVALID and a message giving the bytes it needs.  dg_check_traces and dg_verify_batch size their groups
+ * within the limit too.  The limit applies to one GPU: a context that spans several (dg_init_devices(n > 1), dg_comm_init) rejects it with
+ * DG_ERR_INVALID.
+ * dg_memory_usage: device bytes the library holds now (arena + the pool's reservation) and the most it has held since the limit was last
+ * set.  dg_plan_prove: what a prove call of `count` traces of this shape would do, without running it.  All three return DG_ERR_NO_DEVICE
+ * without a device. */
+#define DG_LAYOUT_FULL 0            /* the whole trace extension is kept */
+#define DG_LAYOUT_EVAL_COSETS 1     /* a chunk of cosets at a time; the 8 evaluation cosets are kept */
+typedef struct {
+    int32_t layout;                /* DG_LAYOUT_FULL or DG_LAYOUT_EVAL_COSETS */
+    uint32_t group;                /* proofs per group of a batched call (1 for dg_prove) */
+    uint32_t coset_chunk;          /* cosets of the trace extension extended at a time (= extension_factor in the full layout) */
+    uint32_t retained_cosets;      /* cosets kept for the constraint evaluation and the openings: extension_factor or 8 */
+    uint64_t bytes_per_proof;      /* device bytes of one proof of the group */
+    uint64_t fixed_bytes;          /* bytes held outside the per-proof buffers: persistent tables, transform scratch, upload buffer */
+    uint64_t available_bytes;      /* the budget the group was fitted into */
+} dg_prove_plan_t;
+int dg_set_memory_limit(size_t bytes);
+int dg_memory_usage(size_t *held, size_t *peak);
+int dg_plan_prove(uint32_t width, uint64_t length, uint32_t count, const dg_options_t *options, dg_prove_plan_t *plan);
+
 /* Optional: randomness supplied by the host.  The prover derives all of its Fiat-Shamir challenges from two reference functions,
  *   field::prng_vector(seed, n)                            (math/field.rs:264-275: StdRng::from_seed + Uniform(0..M))
  *   utils::compute_query_positions(seed, domain, options)  (stark/utils/mod.rs:25-44: StdRng + Uniform(0..domain), rejections)
