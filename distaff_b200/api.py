@@ -405,6 +405,117 @@ def execute(source, public_inputs=(), secret_a=(), secret_b=(), num_outputs=1, o
     return trace.outputs, prove(trace, options)
 
 
+# ---- one program, many inputs, executed on the GPU ---------------------------------------------------------------------------------
+MAX_STEPS = 2**22           # the longest trace the project plans for
+
+
+class ProgramInputs:
+    """ProgramInputs::new (programs/inputs.rs:12): public inputs (at most 8, else that execution fails) and the secret tapes A and B."""
+
+    def __init__(self, public=(), secret_a=(), secret_b=()):
+        self.public = [int(x) for x in public]
+        self.secret_a = [int(x) for x in secret_a]
+        self.secret_b = [int(x) for x in secret_b]
+
+
+def _encoded(program):
+    return hostvm.compile_program(program) if isinstance(program, str) else program
+
+
+def _execution_args(program, inputs):
+    """the dg_program_t and dg_program_inputs_t array of a call (plus the arrays they point into, to keep alive)"""
+    prog = _encoded(program)
+    cprog = prog.c_struct()
+    keep = [prog, cprog]
+    arr = (backend.DgProgramInputs * max(len(inputs), 1))()
+    for i, x in enumerate(inputs):
+        vals = [felt.from_ints(v) for v in (x.public, x.secret_a, x.secret_b)]
+        keep += vals
+        arr[i] = backend.DgProgramInputs(vals[0].ctypes.data, len(vals[0]), vals[1].ctypes.data, len(vals[1]), vals[2].ctypes.data, len(vals[2]))
+    return prog, cprog, arr, keep
+
+
+def _messages(status):
+    msg = ctypes.create_string_buffer(512)
+    out = []
+    for i, rc in enumerate(status):
+        if rc == 0:
+            out.append(None)
+            continue
+        backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
+        out.append(backend.DgError(rc, msg.value.decode(errors="replace")))
+    return out
+
+
+def trace_shapes(program, inputs, max_steps=MAX_STEPS):
+    """The shape pass of dg_trace_batch alone: per input, a dict (width, length, steps, ctx_depth, loop_depth, stack_depth) or the
+    DgError of an execution that failed."""
+    inputs = list(inputs)
+    if not inputs:
+        return []
+    _, cprog, arr, keep = _execution_args(program, inputs)
+    k = len(inputs)
+    info = (backend.DgExecutionInfo * k)()
+    status = (ctypes.c_int * k)()
+    backend.check(backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, None, status))
+    errors = _messages(list(status))
+    del keep
+    return [e if e is not None else {f: int(getattr(info[i], f)) for f, _ in backend.DgExecutionInfo._fields_} for i, e in enumerate(errors)]
+
+
+def trace_batch(program, inputs, max_steps=MAX_STEPS, num_outputs=1):
+    """processor::execute of one program (a hostvm.Program or assembly source) for every ProgramInputs, on the GPU, one thread per
+    execution.  Returns a list in input order: a hostvm.ExecutionTrace (what hostvm.execute gives for the same inputs, byte for byte)
+    or the DgError of an execution that failed, with the host VM's message ("execution exceeds N steps" past max_steps).  The buffers
+    are sized by a shapes-only call first, so the shape pass runs twice."""
+    inputs = list(inputs)
+    if not inputs:
+        return []
+    prog, cprog, arr, keep = _execution_args(program, inputs)
+    k = len(inputs)
+    shapes = trace_shapes(prog, inputs, max_steps)
+    regs = [None if isinstance(s, backend.DgError) else np.empty((s["width"], s["length"], 2), dtype=np.uint64) for s in shapes]
+    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
+    info = (backend.DgExecutionInfo * k)()
+    status = (ctypes.c_int * k)()
+    backend.check(backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, outs, status))
+    errors = _messages(list(status))
+    del keep
+    result = []
+    for i, (x, e) in enumerate(zip(inputs, errors)):
+        if e is not None:
+            result.append(e)
+            continue
+        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
+        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, prog.hash, list(x.public), last[:num_outputs]))
+    return result
+
+
+def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_STEPS):
+    """distaff::execute (lib.rs:30-65) for every ProgramInputs: the program runs on the GPU, one thread per execution, and every trace is
+    proven from the device memory it was generated in.  Returns a list in input order: (outputs, StarkProof) -- what execute() returns
+    for the same inputs, byte for byte -- or the DgError of an execution that failed (in the VM or in the prover)."""
+    options = options or ProofOptions()
+    assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
+    inputs = list(inputs)
+    if not inputs:
+        return []
+    _, cprog, arr, keep = _execution_args(program, inputs)
+    k = len(inputs)
+    opt = options._c()
+    handles = (backend.vp * k)()
+    outputs = np.zeros((k, max(num_outputs, 1), 2), dtype=np.uint64)
+    status = (ctypes.c_int * k)()
+    stats = backend.DgStats()
+    backend.check(backend.lib().dg_execute_batch(ctypes.byref(cprog), k, arr, num_outputs, int(max_steps), ctypes.byref(opt), handles,
+                                                outputs.ctypes.data, status, ctypes.byref(stats)))
+    errors = _messages(list(status))
+    del keep
+    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs]) if num_outputs else [], _collect(handles[i], stats))
+            for i, e in enumerate(errors)]
+
+
 # ---- building blocks ------------------------------------------------------------------------------------------------------
 def ntt(values, inverse=False):
     """polynom::eval_fft / interpolate_fft on (batch, n, 2) or (n, 2) uint64 arrays; returns a new array"""

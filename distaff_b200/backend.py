@@ -50,6 +50,29 @@ class DgProvePlan(ctypes.Structure):
                 ("fixed_bytes", u64), ("available_bytes", u64)]
 
 
+class DgOpHint(ctypes.Structure):
+    _fields_ = [("kind", u32), ("n", u32), ("value16", ctypes.c_uint8 * 16)]
+
+
+class DgBlock(ctypes.Structure):
+    _fields_ = [("kind", u32), ("first", u32), ("count", u32), ("alt_first", u32), ("alt_count", u32), ("hash0", ctypes.c_uint8 * 16),
+                ("hash1", ctypes.c_uint8 * 16), ("hash2", ctypes.c_uint8 * 16)]
+
+
+class DgProgram(ctypes.Structure):
+    _fields_ = [("ops", vp), ("hints", ctypes.POINTER(DgOpHint)), ("n_ops", u64), ("blocks", ctypes.POINTER(DgBlock)), ("n_blocks", u32),
+                ("children", ctypes.POINTER(u32)), ("n_children", u32), ("root_first", u32), ("root_count", u32),
+                ("hash32", ctypes.c_uint8 * 32)]
+
+
+class DgProgramInputs(ctypes.Structure):
+    _fields_ = [("public16", vp), ("n_public", u32), ("secret_a16", vp), ("n_secret_a", u64), ("secret_b16", vp), ("n_secret_b", u64)]
+
+
+class DgExecutionInfo(ctypes.Structure):
+    _fields_ = [("width", u32), ("length", u64), ("steps", u64), ("ctx_depth", u32), ("loop_depth", u32), ("stack_depth", u32)]
+
+
 DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -70,6 +93,10 @@ EXPORTS = {
     "dg_prove_batch_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
                               ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
+    "dg_trace_batch": [ctypes.POINTER(DgProgram), u32, ctypes.POINTER(DgProgramInputs), u64, ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp),
+                       ctypes.POINTER(ctypes.c_int)],
+    "dg_execute_batch": [ctypes.POINTER(DgProgram), u32, ctypes.POINTER(DgProgramInputs), u32, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp),
+                         vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),

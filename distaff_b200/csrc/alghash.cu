@@ -17,6 +17,7 @@
 #include "common.cuh"
 #include "air_constants.h"
 #include "blake3.cuh"
+#include "alg_sbox.cuh"
 
 namespace dg {
 
@@ -49,20 +50,6 @@ __device__ __forceinline__ void alg_mds(fe st[6]) {
 #pragma unroll
     for (int i = 0; i < 6; i++) st[i] = r[i];
 }
-// x^INV_ALPHA, hex digits of the exponent from the most significant: 20 x 'a', '8', 'c', 9 x 'a', 'b'
-__device__ __noinline__ fe alg_inv_sbox(fe x) {
-    const fe x2 = fe_sqr(x), x4 = fe_sqr(x2), x8 = fe_sqr(x4);
-    const fe xa = fe_mul(x8, x2), xb = fe_mul(xa, x), xc = fe_mul(x8, x4);
-    fe acc = xa;
-#pragma unroll 1
-    for (int d = 1; d < 32; d++) {
-        acc = fe_sqr(acc); acc = fe_sqr(acc); acc = fe_sqr(acc); acc = fe_sqr(acc);
-        const fe m = d == 20 ? x8 : (d == 21 ? xc : (d == 31 ? xb : xa));
-        acc = fe_mul(acc, m);
-    }
-    return acc;
-}
-
 __device__ __forceinline__ void rescue_permute(fe st[6]) {          // hash.rs:160-173
     alg_add_constants(st, 0);
 #pragma unroll 1

@@ -522,6 +522,30 @@ int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t wid
                      program_hashes32, reports, nullptr, d_step_masks);
     });
 }
+int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
+                   dg_execution_info_t *info, uint8_t *const *registers_out, int *status) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(program && inputs && status, "null argument");
+        check_execution_call(program, count, inputs, max_steps);      // a bad encoding is rejected before the device is touched
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        trace_batch(c, program, count, inputs, max_steps, info, registers_out, status, t_batch_messages);
+    });
+}
+int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
+                     const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(program && inputs && options && proofs_out && status, "null argument");
+        check_execution_call(program, count, inputs, max_steps);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        execute_batch(c, program, count, inputs, num_outputs, max_steps, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, stats);
+    });
+}
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
     return guarded([&] {
         DG_REQUIRE(message && cap, "null argument");

@@ -113,7 +113,7 @@ struct Context {
     Arena arena;                            // per-proof bump arena of this device
     void *nccl_comm = nullptr;              // this rank's NCCL communicator (comm.cu), one per context
     DevBuf d_periodic;                      // periodic AIR tables on this device (prover.cu stage 3)
-    bool air_consts = false, alghash_consts = false;     // __constant__ tables uploaded to this device
+    bool air_consts = false, alghash_consts = false, vm_consts = false;     // __constant__ tables uploaded to this device
     std::map<const void *, size_t> func_smem;            // per-device cudaFuncSetAttribute(MaxDynamicSharedMemorySize) already applied
     DevBuf l2_scratch;
     int num_sms = 132;                      // H100 SXM; set from the device properties

@@ -26,6 +26,24 @@ void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t w
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                         const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
 
+// Batched proving of `count` traces of one shape that are generated on the device group by group: generate(first, k, d_regs, failed)
+// writes traces [first, first + k) into d_regs ([k][width][length], the buffer the prover then reads) and sets failed[i] to the status and
+// message of a trace it could not generate (failed holds k entries of DG_OK on entry).  Otherwise as prove_batch_device.
+void prove_batch_generated(Context &c, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                           const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                           const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
+                           const std::function<void(uint32_t, int, fe *, std::vector<std::pair<int, std::string>> &)> &generate);
+// dg_trace_batch / dg_execute_batch (execute.cu): status / messages per execution.  check_execution_call validates the arguments and the
+// program encoding on the host alone (DG_ERR_INVALID); both calls run it again.
+void check_execution_call(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps);
+void trace_batch(Context &c, const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
+                 dg_execution_info_t *info, uint8_t *const *registers_out, int *status, std::vector<std::string> &messages);
+void execute_batch(Context &c, const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs,
+                   uint64_t max_steps, const dg_options_t &opt, Proof **proofs_out, uint8_t *outputs16, int *status,
+                   std::vector<std::string> &messages, dg_prove_stats_t *stats);
+// the largest group of a batched call, after $DG_BATCH_GROUP
+int batch_group_cap(long long k);
+
 // What a prove call of one shape does on one GPU (dg_plan_prove): the full layout keeps the whole trace extension; the evaluation-coset
 // layout extends and hashes `chunk` cosets at a time, keeps the 8 cosets the constraint evaluation reads and computes the other opened
 // rows from the trace polynomials.  Proofs run in groups of `group`; per_proof bytes each (arena) on top of `fixed` bytes outside the

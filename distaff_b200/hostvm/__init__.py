@@ -32,6 +32,16 @@ def _lib():
         lib.vm_program_hash.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         lib.vm_copy_trace.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
         lib.vm_free.argtypes = [ctypes.c_void_p]
+        lib.vm_compile.restype = ctypes.c_void_p
+        lib.vm_compile.argtypes = [ctypes.c_char_p]
+        lib.vm_compile_error.restype = ctypes.c_char_p
+        lib.vm_compile_error.argtypes = [ctypes.c_void_p]
+        lib.vm_compile_sizes.argtypes = [ctypes.c_void_p, ctypes.c_void_p]
+        lib.vm_compile_copy.argtypes = [ctypes.c_void_p] * 6
+        lib.vm_compile_free.argtypes = [ctypes.c_void_p]
+        lib.vm_execute_program.restype = ctypes.c_void_p
+        lib.vm_execute_program.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint32, ctypes.c_void_p,
+                                           ctypes.c_uint32]
         _LIB = lib
     return _LIB
 
@@ -57,12 +67,74 @@ class ExecutionTrace:
         return self.registers.shape[1]
 
 
+class Program:
+    """A compiled program in the flat encoding of include/distaff_gpu.h (dg_program_t): the op codes with one hint per op, the blocks,
+    the child lists, the root body and Program::hash() -- what the GPU interpreter (dg_trace_batch / dg_execute_batch) runs.  The
+    arrays are ctypes arrays, so tests can alter an encoding before passing it on."""
+
+    def __init__(self, ops, hints, blocks, children, root_first, root_count, hash32):
+        from .. import backend
+        self.ops = (ctypes.c_uint8 * max(len(ops), 1))(*ops)
+        self.hints = (backend.DgOpHint * max(len(hints), 1))(*hints)
+        self.n_ops = len(ops)
+        self.blocks = (backend.DgBlock * max(len(blocks), 1))(*blocks)
+        self.n_blocks = len(blocks)
+        self.children = (ctypes.c_uint32 * max(len(children), 1))(*children)
+        self.n_children = len(children)
+        self.root_first, self.root_count = root_first, root_count
+        self.hash = bytes(hash32)
+
+    def c_struct(self):
+        """the dg_program_t of this encoding (it points into this object's arrays)"""
+        from .. import backend
+        return backend.DgProgram(ctypes.cast(self.ops, ctypes.c_void_p), self.hints, self.n_ops, self.blocks, self.n_blocks, self.children,
+                                 self.n_children, self.root_first, self.root_count, (ctypes.c_uint8 * 32)(*self.hash))
+
+
+def compile_program(source):
+    """Compiles assembly (programs::assembly::compile) into the program encoding: a Program, whose .hash is Program::hash()."""
+    from .. import backend
+    lib = _lib()
+    h = lib.vm_compile(source.encode())
+    try:
+        err = lib.vm_compile_error(h)
+        if err:
+            raise RuntimeError("vm: " + err.decode())
+        sizes = (ctypes.c_uint64 * 5)()
+        lib.vm_compile_sizes(h, sizes)
+        n_ops, n_blocks, n_children, root_first, root_count = (int(x) for x in sizes)
+        ops = (ctypes.c_uint8 * max(n_ops, 1))()
+        hints = (backend.DgOpHint * max(n_ops, 1))()
+        blocks = (backend.DgBlock * n_blocks)()
+        children = (ctypes.c_uint32 * n_children)()
+        hash32 = ctypes.create_string_buffer(32)
+        lib.vm_compile_copy(h, ops, hints, blocks, children, hash32)
+    finally:
+        lib.vm_compile_free(h)
+    return Program(list(ops)[:n_ops], list(hints)[:n_ops], list(blocks), list(children), root_first, root_count, hash32.raw)
+
+
+def execute_program(program, public_inputs=(), secret_a=(), secret_b=(), num_outputs=1):
+    """execute() of a compiled Program: the encoding is decoded back into its block tree and run by the same VM, with the hashes the
+    encoding carries.  Same result and errors as execute() of the source."""
+    lib = _lib()
+    prog = program.c_struct()
+    return _run(lambda pub, sa, sb: lib.vm_execute_program(ctypes.byref(prog), pub.ctypes.data, len(pub), sa.ctypes.data, len(sa),
+                                                          sb.ctypes.data, len(sb)), public_inputs, secret_a, secret_b, num_outputs)
+
+
 def execute(source, public_inputs=(), secret_a=(), secret_b=(), num_outputs=1):
+    lib = _lib()
+    return _run(lambda pub, sa, sb: lib.vm_execute(source.encode(), pub.ctypes.data, len(pub), sa.ctypes.data, len(sa), sb.ctypes.data, len(sb)),
+                public_inputs, secret_a, secret_b, num_outputs)
+
+
+def _run(start, public_inputs, secret_a, secret_b, num_outputs):
     lib = _lib()
     pub = felt.from_ints(public_inputs)
     sa = felt.from_ints(secret_a)
     sb = felt.from_ints(secret_b)
-    h = lib.vm_execute(source.encode(), pub.ctypes.data, len(pub), sa.ctypes.data, len(sa), sb.ctypes.data, len(sb))
+    h = start(pub, sa, sb)
     try:
         err = lib.vm_error(h)
         if err:

@@ -16,6 +16,7 @@
 #include <stdexcept>
 #include <algorithm>
 #include "../csrc/air_constants.h"
+#include "../../include/distaff_gpu.h"
 
 namespace vm {
 
@@ -109,6 +110,10 @@ struct Block {
     Span span;
     std::vector<Block> body;      // group body / switch true branch / loop body
     std::vector<Block> alt;       // switch false branch / loop skip
+    // hashes carried by a decoded program encoding (dg_block_t): switch true / false branch, loop image / body / skip; when absent the
+    // VM hashes the blocks itself
+    bool has_hashes = false;
+    u128 hashes[3] = {0, 0, 0};
 };
 
 static void check_span(const Span &s) {
@@ -761,16 +766,16 @@ struct Machine {
             case B_SWITCH: {
                 start_block();
                 u128 c = top();
-                if (c == 0) { run_blocks(b.alt); close_block(hash_seq(b.body, BLOCK_SUFFIX, 15), false); }
-                else if (c == 1) { run_blocks(b.body); close_block(hash_seq(b.alt, BLOCK_SUFFIX, 15), true); }
+                if (c == 0) { run_blocks(b.alt); close_block(b.has_hashes ? b.hashes[0] : hash_seq(b.body, BLOCK_SUFFIX, 15), false); }
+                else if (c == 1) { run_blocks(b.body); close_block(b.has_hashes ? b.hashes[1] : hash_seq(b.alt, BLOCK_SUFFIX, 15), true); }
                 else fail("cannot select a branch based on a non-binary condition");
                 break; }
             case B_LOOP: {
                 u128 c = top();
-                if (c == 0) { start_block(); run_blocks(b.alt); close_block(hash_seq(b.body, loop_suffix(), 0), false); }
+                if (c == 0) { start_block(); run_blocks(b.alt); close_block(b.has_hashes ? b.hashes[1] : hash_seq(b.body, loop_suffix(), 0), false); }
                 else if (c == 1) {
-                    u128 image = hash_seq(b.body, {}, 0);
-                    u128 skip_hash = hash_seq(b.alt, BLOCK_SUFFIX, 15);
+                    u128 image = b.has_hashes ? b.hashes[0] : hash_seq(b.body, {}, 0);
+                    u128 skip_hash = b.has_hashes ? b.hashes[2] : hash_seq(b.alt, BLOCK_SUFFIX, 15);
                     start_loop(image);
                     for (;;) {
                         run_blocks(b.body);
@@ -807,14 +812,16 @@ struct Execution {
     std::string error;
 };
 
-static Execution *execute(const std::string &source, const std::vector<u128> &pub, const std::vector<u128> &sa, const std::vector<u128> &sb) {
+static Execution *run(const Program *prog, const std::string *source, const std::vector<u128> &pub, const std::vector<u128> &sa,
+                      const std::vector<u128> &sb) {
     Execution *e = new Execution();
     try {
         if (pub.size() > 8) throw std::runtime_error("expected no more than 8 public inputs");
         if (sa.size() < sb.size()) throw std::runtime_error("tape A cannot be shorter than tape B");
-        Program prog = compile(source);
+        Program compiled;
+        if (!prog) { compiled = compile(*source); prog = &compiled; }
         Machine m(pub, sa, sb);
-        m.run_blocks(prog.root.body);
+        m.run_blocks(prog->root.body);
         m.close_block(0, true);
         m.finalize();
         e->ctx_depth = m.ctx_stack.size() - 1;
@@ -830,13 +837,137 @@ static Execution *execute(const std::string &source, const std::vector<u128> &pu
         for (auto &x : m.ctx_stack) r.push_back(std::move(x));
         for (auto &x : m.loop_stack) r.push_back(std::move(x));
         for (size_t i = 0; i < m.max_depth; i++) r.push_back(std::move(m.regs[i]));
-        e->program_hash[0] = prog.hash[0]; e->program_hash[1] = prog.hash[1];
+        e->program_hash[0] = prog->hash[0]; e->program_hash[1] = prog->hash[1];
         // lib.rs:49-59
         size_t n = r[0].size();
         if (r[0][n - 1] < 16) throw std::runtime_error("a program must consist of at least 16 operations");
-        if (r[1][n - 1] != prog.hash[0] || r[2][n - 1] != prog.hash[1]) throw std::runtime_error("program hash does not match trace hash");
+        if (r[1][n - 1] != prog->hash[0] || r[2][n - 1] != prog->hash[1]) throw std::runtime_error("program hash does not match trace hash");
     } catch (std::exception &ex) { e->error = ex.what(); }
     return e;
+}
+static Execution *execute(const std::string &source, const std::vector<u128> &pub, const std::vector<u128> &sa, const std::vector<u128> &sb) {
+    return run(nullptr, &source, pub, sa, sb);
+}
+
+// ---- the flat program encoding of include/distaff_gpu.h (dg_program_t) ----------------------------------------------------------------
+struct Encoded {
+    std::vector<uint8_t> ops;
+    std::vector<dg_op_hint_t> hints;
+    std::vector<dg_block_t> blocks;
+    std::vector<uint32_t> children;
+    uint32_t root_first = 0, root_count = 0;
+    uint8_t hash32[32];
+    std::string error;
+};
+static void put128(uint8_t out[16], u128 v) { memcpy(out, &v, 16); }
+static u128 get128(const uint8_t in[16]) { u128 v; memcpy(&v, in, 16); return v; }
+
+static uint32_t encode_block(Encoded &e, const Block &b);
+// encodes the blocks of a list (their own child lists first), then appends the list itself: returns its first index in `children`
+static uint32_t encode_list(Encoded &e, const std::vector<Block> &list) {
+    std::vector<uint32_t> idx;
+    for (const Block &b : list) idx.push_back(encode_block(e, b));
+    const uint32_t first = (uint32_t)e.children.size();
+    e.children.insert(e.children.end(), idx.begin(), idx.end());
+    return first;
+}
+static uint32_t encode_block(Encoded &e, const Block &b) {
+    dg_block_t d;
+    memset(&d, 0, sizeof d);
+    switch (b.kind) {
+    case B_SPAN:
+        d.kind = DG_BLOCK_SPAN;
+        d.first = (uint32_t)e.ops.size(); d.count = (uint32_t)b.span.ops.size();
+        for (size_t i = 0; i < b.span.ops.size(); i++) {
+            const Hint h = b.span.hint(i);
+            dg_op_hint_t eh;
+            memset(&eh, 0, sizeof eh);
+            eh.kind = h.kind == H_NONE ? DG_HINT_NONE : h.kind == H_PUSH ? DG_HINT_PUSH : h.kind == H_EQSTART ? DG_HINT_EQ_START
+                    : h.kind == H_RCSTART ? DG_HINT_RC_START : h.kind == H_CMPSTART ? DG_HINT_CMP_START : DG_HINT_PMPATH_START;
+            eh.n = h.n;
+            put128(eh.value16, h.value);
+            e.ops.push_back(b.span.ops[i]);
+            e.hints.push_back(eh);
+        }
+        break;
+    case B_GROUP:
+        d.kind = DG_BLOCK_GROUP;
+        d.first = encode_list(e, b.body); d.count = (uint32_t)b.body.size();
+        break;
+    case B_SWITCH:
+        d.kind = DG_BLOCK_SWITCH;
+        d.first = encode_list(e, b.body); d.count = (uint32_t)b.body.size();
+        d.alt_first = encode_list(e, b.alt); d.alt_count = (uint32_t)b.alt.size();
+        put128(d.hash0, hash_seq(b.body, BLOCK_SUFFIX, 15));       // Switch::true_branch_hash
+        put128(d.hash1, hash_seq(b.alt, BLOCK_SUFFIX, 15));        // Switch::false_branch_hash
+        break;
+    case B_LOOP:
+        d.kind = DG_BLOCK_LOOP;
+        d.first = encode_list(e, b.body); d.count = (uint32_t)b.body.size();
+        d.alt_first = encode_list(e, b.alt); d.alt_count = (uint32_t)b.alt.size();
+        put128(d.hash0, hash_seq(b.body, {}, 0));                  // Loop::image
+        put128(d.hash1, hash_seq(b.body, loop_suffix(), 0));       // Loop::body_hash
+        put128(d.hash2, hash_seq(b.alt, BLOCK_SUFFIX, 15));        // Loop::skip_hash
+        break;
+    }
+    e.blocks.push_back(d);
+    return (uint32_t)e.blocks.size() - 1;
+}
+static Encoded *encode(const std::string &source) {
+    Encoded *e = new Encoded();
+    try {
+        Program p = compile(source);
+        e->root_first = encode_list(*e, p.root.body);
+        e->root_count = (uint32_t)p.root.body.size();
+        put128(e->hash32, p.hash[0]);
+        put128(e->hash32 + 16, p.hash[1]);
+    } catch (std::exception &ex) { e->error = ex.what(); }
+    return e;
+}
+
+// the block tree of an encoding, with its hashes; ranges are checked, nothing else (the VM reports what does not run)
+static std::vector<Block> decode_list(const dg_program_t &p, uint32_t first, uint32_t count, int depth);
+static Block decode_block(const dg_program_t &p, uint32_t index, int depth) {
+    if (index >= p.n_blocks) throw std::runtime_error("block index out of range");
+    if (depth > 64) throw std::runtime_error("blocks nested too deeply");
+    const dg_block_t &d = p.blocks[index];
+    Block b;
+    switch (d.kind) {
+    case DG_BLOCK_SPAN:
+        b.kind = B_SPAN;
+        if ((uint64_t)d.first + d.count > p.n_ops) throw std::runtime_error("span op range out of range");
+        for (uint32_t i = 0; i < d.count; i++) {
+            b.span.ops.push_back(p.ops[d.first + i]);
+            const dg_op_hint_t &eh = p.hints[d.first + i];
+            if (eh.kind == DG_HINT_NONE) continue;
+            Hint h;
+            h.kind = eh.kind == DG_HINT_PUSH ? H_PUSH : eh.kind == DG_HINT_EQ_START ? H_EQSTART : eh.kind == DG_HINT_RC_START ? H_RCSTART
+                   : eh.kind == DG_HINT_CMP_START ? H_CMPSTART : H_PMPATH;
+            h.n = eh.n;
+            h.value = get128(eh.value16);
+            b.span.hints[i] = h;
+        }
+        break;
+    case DG_BLOCK_GROUP:
+        b.kind = B_GROUP;
+        b.body = decode_list(p, d.first, d.count, depth + 1);
+        break;
+    case DG_BLOCK_SWITCH: case DG_BLOCK_LOOP:
+        b.kind = d.kind == DG_BLOCK_SWITCH ? B_SWITCH : B_LOOP;
+        b.body = decode_list(p, d.first, d.count, depth + 1);
+        b.alt = decode_list(p, d.alt_first, d.alt_count, depth + 1);
+        b.has_hashes = true;
+        b.hashes[0] = get128(d.hash0); b.hashes[1] = get128(d.hash1); b.hashes[2] = get128(d.hash2);
+        break;
+    default: throw std::runtime_error("unknown block kind");
+    }
+    return b;
+}
+static std::vector<Block> decode_list(const dg_program_t &p, uint32_t first, uint32_t count, int depth) {
+    if (count == 0 || (uint64_t)first + count > p.n_children) throw std::runtime_error("child list out of range");
+    std::vector<Block> list;
+    for (uint32_t i = 0; i < count; i++) list.push_back(decode_block(p, p.children[first + i], depth));
+    return list;
 }
 
 } // namespace vm
@@ -862,4 +993,37 @@ void vm_copy_trace(void *h, uint8_t *out) {
     for (size_t j = 0; j < e->registers.size(); j++) memcpy(out + j * n * 16, e->registers[j].data(), n * 16);
 }
 void vm_free(void *h) { delete (vm::Execution *)h; }
+
+// compiles assembly into the program encoding of include/distaff_gpu.h; sizes = {n_ops, n_blocks, n_children, root_first, root_count}
+void *vm_compile(const char *source) { return vm::encode(source); }
+const char *vm_compile_error(void *h) { auto *e = (vm::Encoded *)h; return e->error.empty() ? nullptr : e->error.c_str(); }
+void vm_compile_sizes(void *h, uint64_t sizes[5]) {
+    auto *e = (vm::Encoded *)h;
+    sizes[0] = e->ops.size(); sizes[1] = e->blocks.size(); sizes[2] = e->children.size(); sizes[3] = e->root_first; sizes[4] = e->root_count;
+}
+void vm_compile_copy(void *h, uint8_t *ops, dg_op_hint_t *hints, dg_block_t *blocks, uint32_t *children, uint8_t *hash32) {
+    auto *e = (vm::Encoded *)h;
+    if (!e->ops.empty()) { memcpy(ops, e->ops.data(), e->ops.size()); memcpy(hints, e->hints.data(), e->hints.size() * sizeof(dg_op_hint_t)); }
+    memcpy(blocks, e->blocks.data(), e->blocks.size() * sizeof(dg_block_t));
+    memcpy(children, e->children.data(), e->children.size() * 4);
+    memcpy(hash32, e->hash32, 32);
+}
+void vm_compile_free(void *h) { delete (vm::Encoded *)h; }
+// runs the VM on a program encoding decoded back into its block tree (the hashes the encoding carries close switches and loops)
+void *vm_execute_program(const dg_program_t *program, const uint8_t *pub16, uint32_t n_pub, const uint8_t *a16, uint32_t n_a, const uint8_t *b16,
+                         uint32_t n_b) {
+    auto rd = [](const uint8_t *p, uint32_t n) { std::vector<vm::u128> v(n); if (n) memcpy(v.data(), p, (size_t)n * 16); return v; };
+    vm::Program prog;
+    try {
+        prog.root.kind = vm::B_GROUP;
+        prog.root.body = vm::decode_list(*program, program->root_first, program->root_count, 0);
+    } catch (std::exception &ex) {
+        auto *e = new vm::Execution();
+        e->error = ex.what();
+        return e;
+    }
+    prog.hash[0] = vm::get128(program->hash32);
+    prog.hash[1] = vm::get128(program->hash32 + 16);
+    return vm::run(&prog, nullptr, rd(pub16, n_pub), rd(a16, n_a), rd(b16, n_b));
+}
 }

@@ -81,8 +81,9 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
  * several GPUs; DG_ERR_CUDA; DG_ERR_NO_DEVICE); on such an error every proofs_out[i] is NULL (nothing to free).  The library splits the
  * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
  * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) the message of entry i of the
- * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device or dg_verify_batch: why trace i failed (the message dg_prove
- * gives for that trace) or why proof i was not accepted (what dg_verify reports for that proof), and "" if it was proven / accepted. */
+ * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device, dg_verify_batch, dg_trace_batch or dg_execute_batch: why
+ * trace i failed (the message dg_prove gives for that trace), why proof i was not accepted (what dg_verify reports for that proof) or
+ * why execution i failed, and "" if it was proven / accepted / executed. */
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                    int *status, dg_prove_stats_t *stats);
@@ -126,6 +127,85 @@ int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *con
 int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
                            const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
                            const uint8_t *program_hashes32, dg_trace_report_t *reports, uint32_t *d_step_masks);
+
+/* ---- executing one program on many inputs --------------------------------------------------------------------------------------------
+ * processor::execute (processor/mod.rs:23-182) of one compiled program for many ProgramInputs, one GPU thread per execution, and
+ * distaff::execute (lib.rs:30-65) on top of it: every trace is proven from device memory where it was generated.  The library has no
+ * assembler: the caller passes the compiled block tree of programs/blocks/mod.rs:30-60 in the flat encoding below, hashes included, so
+ * the library never hashes program blocks on the host.  Every field can be read from the crate's public Program API (INTEGRATION.md
+ * walks program.root() into a dg_program_t).  The encoding is validated on the host before any launch (indices in range, every span as
+ * Span::new checks it, every block list as validate_block_list checks it, at most 15 nested blocks and 8 nested loops); a bad encoding
+ * fails the call with DG_ERR_INVALID.  Hashes that do not match the blocks are not detected there: the execution then ends with
+ * "program hash does not match trace hash" (or a loop image mismatch), as the host VM's does. */
+#define DG_HINT_NONE 0           /* OpHint::None                                                    (processor/opcodes.rs:173-180) */
+#define DG_HINT_PUSH 1           /* OpHint::PushValue(value16)                                                                       */
+#define DG_HINT_EQ_START 2       /* OpHint::EqStart                                                                                  */
+#define DG_HINT_RC_START 3       /* OpHint::RcStart(n)                                                                               */
+#define DG_HINT_CMP_START 4      /* OpHint::CmpStart(n)                                                                              */
+#define DG_HINT_PMPATH_START 5   /* OpHint::PmpathStart(n)                                                                           */
+typedef struct {
+    uint32_t kind;               /* DG_HINT_* */
+    uint32_t n;                  /* RcStart / CmpStart / PmpathStart parameter, else 0 */
+    uint8_t value16[16];         /* PushValue, else zero */
+} dg_op_hint_t;
+
+#define DG_BLOCK_SPAN 0          /* ProgramBlock::Span:   ops[first .. first + count), one hint per op (Span::op_codes / op_hints)       */
+#define DG_BLOCK_GROUP 1         /* ProgramBlock::Group:  body = children[first .. first + count)  (Group::body)                         */
+#define DG_BLOCK_SWITCH 2        /* ProgramBlock::Switch: true branch = children[first ..), false branch = children[alt_first ..)         */
+#define DG_BLOCK_LOOP 3          /* ProgramBlock::Loop:   body = children[first ..), skip = children[alt_first ..)  (Loop::body / skip)   */
+typedef struct {
+    uint32_t kind;               /* DG_BLOCK_* */
+    uint32_t first, count;       /* span: op range; group / switch / loop: child-list range (true branch, loop body) */
+    uint32_t alt_first, alt_count;   /* switch: false branch; loop: skip; else 0 */
+    /* hashes the VM needs when it closes the block (blocks/mod.rs:252-318); zero where not listed:
+     *   switch: hash0 = true_branch_hash(), hash1 = false_branch_hash()
+     *   loop:   hash0 = image(), hash1 = body_hash(), hash2 = skip_hash() */
+    uint8_t hash0[16], hash1[16], hash2[16];
+} dg_block_t;
+
+typedef struct {                 /* Program (programs/mod.rs) */
+    const uint8_t *ops;          /* op codes of every span, n_ops of them (OpCode as u8) */
+    const dg_op_hint_t *hints;   /* one hint per op */
+    uint64_t n_ops;
+    const dg_block_t *blocks;
+    uint32_t n_blocks;
+    const uint32_t *children;    /* block indices; the child lists of groups, switches and loops and the root body are ranges of it */
+    uint32_t n_children;
+    uint32_t root_first, root_count;     /* the root Group's body: children[root_first .. root_first + root_count) */
+    uint8_t hash32[32];          /* Program::hash() */
+} dg_program_t;
+
+typedef struct {                 /* ProgramInputs::new(public, secret_a, secret_b) (programs/inputs.rs:12) */
+    const uint8_t *public16; uint32_t n_public;      /* at most 8 (lib.rs:32), else the execution fails */
+    const uint8_t *secret_a16; uint64_t n_secret_a;  /* tape A, read first to last */
+    const uint8_t *secret_b16; uint64_t n_secret_b;  /* tape B, not longer than tape A, else the execution fails */
+} dg_program_inputs_t;
+
+typedef struct {                 /* the shape of one execution's trace, what execute reports beside it */
+    uint32_t width;              /* 15 + ctx_depth + loop_depth + stack_depth */
+    uint64_t length;             /* next power of two above the last step, at least 16 */
+    uint64_t steps;              /* last step (operations executed) */
+    uint32_t ctx_depth, loop_depth, stack_depth;
+} dg_execution_info_t;
+
+#define DG_ERR_EXECUTION (-7)    /* the program failed on these inputs (processor::execute / lib.rs:48-60 panic); message as the host VM's */
+
+/* dg_trace_batch: executes the program for inputs[0 .. count) in one launch per pass.  Per execution: status[i] = DG_OK and info[i], or
+ * DG_ERR_EXECUTION with dg_batch_message(i) = the VM's message ("ASSERT failed at step 17", ...; "execution exceeds N steps" when the
+ * last step would reach max_steps, which bounds how long a program that never stops keeps the GPU busy).  registers_out: NULL (only the
+ * shape pass runs, so that a caller can size its buffers first), or count pointers, each to info[i].width * info[i].length * 16 bytes
+ * that receive the column-major registers of a successful execution (entries of failed executions may be NULL).  Returns DG_OK when the
+ * batch ran, whatever the executions did; DG_ERR_INVALID for a bad encoding or a context that spans several GPUs. */
+int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
+                   dg_execution_info_t *info, uint8_t *const *registers_out, int *status);
+/* dg_execute_batch: dg_trace_batch, then every successful trace proven from the device memory it was generated in, with the same
+ * options, grouped by shape and then by device memory ($DG_BATCH_GROUP and dg_set_memory_limit apply).  Per execution: status[i] =
+ * DG_OK, proofs_out[i] byte-identical to dg_prove of the trace with the execution's public inputs and outputs, and the num_outputs
+ * (<= 8) elements at outputs16 + 16 * num_outputs * i = the top of the last row's stack, zero below its depth (lib.rs:45-46); or a per-execution
+ * failure (DG_ERR_EXECUTION, DG_ERR_UNSATISFIED, DG_ERR_EXHAUSTED) with its message in dg_batch_message(i) and proofs_out[i] = NULL.
+ * A failing execution changes no other result.  stats (may be NULL) covers the proofs. */
+int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
+                     const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats);
 
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
