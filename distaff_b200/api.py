@@ -516,6 +516,109 @@ def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_ST
             for i, e in enumerate(errors)]
 
 
+# ---- many programs, many inputs, executed on the GPU in one call ----------------------------------------------------------------------
+def pack_jobs(jobs, compile=None):
+    """The program table of a dg_trace_programs / dg_execute_programs call.  jobs: (program, ProgramInputs) or (program, ProgramInputs,
+    num_outputs), the program an assembly source or a hostvm.Program.  Each distinct source is compiled once (by `compile`, default
+    hostvm.compile_program) and each distinct program -- the same source, or the same Program object -- goes into the table once.
+    Returns (programs, program_of, inputs, num_outputs), the last three in job order."""
+    compile = compile or hostvm.compile_program
+    programs, program_of, inputs, num_outputs = [], [], [], []
+    index = {}
+    for job in jobs:
+        if len(job) not in (2, 3):
+            raise ValueError("a job is (program, ProgramInputs) or (program, ProgramInputs, num_outputs)")
+        program, x = job[0], job[1]
+        no = int(job[2]) if len(job) == 3 else 1
+        if not 0 <= no <= 8:
+            raise ValueError("cannot have more than 8 outputs")
+        key = ("source", program) if isinstance(program, str) else ("program", id(program))
+        if key not in index:
+            index[key] = len(programs)
+            programs.append(compile(program) if isinstance(program, str) else program)
+        program_of.append(index[key])
+        inputs.append(x)
+        num_outputs.append(no)
+    return programs, program_of, inputs, num_outputs
+
+
+def _programs_args(jobs):
+    """the dg_program_t table, program_of, dg_program_inputs_t array and num_outputs of a call (plus what they point into)"""
+    programs, program_of, inputs, num_outputs = pack_jobs(jobs)
+    k = len(inputs)
+    cprogs = (backend.DgProgram * len(programs))(*[p.c_struct() for p in programs])
+    arr = (backend.DgProgramInputs * k)()
+    keep = [programs, cprogs]
+    for i, x in enumerate(inputs):
+        vals = [felt.from_ints(v) for v in (x.public, x.secret_a, x.secret_b)]
+        keep += vals
+        arr[i] = backend.DgProgramInputs(vals[0].ctypes.data, len(vals[0]), vals[1].ctypes.data, len(vals[1]), vals[2].ctypes.data, len(vals[2]))
+    return programs, cprogs, (backend.u32 * k)(*program_of), arr, num_outputs, keep
+
+
+def _vm_stats(stats, st):
+    if stats is not None:
+        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgExecutionStats._fields_})
+
+
+def trace_programs(jobs, max_steps=MAX_STEPS, stats=None):
+    """trace_batch for executions of different programs in one call (dg_trace_programs): each program's executions run in warps of
+    their own, and one write launch per wave covers every trace shape.  Returns a list in job order: a hostvm.ExecutionTrace (with the
+    job's num_outputs outputs, default 1) or the DgError of an execution that failed.  A dict passed as `stats` receives the VM passes'
+    figures (shape_launches, write_launches, waves, prove_groups, lanes, shape_ms, write_ms) of the call that writes the traces; a
+    shapes-only call sizes the buffers first."""
+    jobs = list(jobs)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    k, L = len(jobs), backend.lib()
+    info = (backend.DgExecutionInfo * k)()
+    status = (ctypes.c_int * k)()
+    st = backend.DgExecutionStats()
+    backend.check(L.dg_trace_programs(cprogs, len(programs), k, program_of, arr, int(max_steps), info, None, status, ctypes.byref(st)))
+    regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
+    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
+    backend.check(L.dg_trace_programs(cprogs, len(programs), k, program_of, arr, int(max_steps), info, outs, status, ctypes.byref(st)))
+    errors = _messages(list(status))
+    _vm_stats(stats, st)
+    result = []
+    for i, (job, e) in enumerate(zip(jobs, errors)):
+        if e is not None:
+            result.append(e)
+            continue
+        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
+        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
+                                            list(job[1].public), last[:num_outputs[i]]))
+    del keep
+    return result
+
+
+def execute_programs(jobs, options=None, max_steps=MAX_STEPS, stats=None):
+    """execute_batch for executions of different programs in one call (dg_execute_programs): the VM runs every job on the GPU, and each
+    trace shape's traces are proven together, whichever programs they came from, in the device memory they were written to.  Returns a
+    list in job order: (outputs, StarkProof) -- what execute_batch of that program alone returns, byte for byte -- or the DgError of an
+    execution that failed.  `stats` as in trace_programs, prove_groups included."""
+    options = options or ProofOptions()
+    jobs = list(jobs)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    k = len(jobs)
+    opt = options._c()
+    handles = (backend.vp * k)()
+    outputs = np.zeros((k, 8, 2), dtype=np.uint64)
+    status = (ctypes.c_int * k)()
+    pst, st = backend.DgStats(), backend.DgExecutionStats()
+    backend.check(backend.lib().dg_execute_programs(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), int(max_steps),
+                                                   ctypes.byref(opt), handles, outputs.ctypes.data, status, ctypes.byref(pst), ctypes.byref(st)))
+    errors = _messages(list(status))
+    _vm_stats(stats, st)
+    del keep
+    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs[i]]) if num_outputs[i] else [], _collect(handles[i], pst))
+            for i, e in enumerate(errors)]
+
+
 # ---- building blocks ------------------------------------------------------------------------------------------------------
 def ntt(values, inverse=False):
     """polynom::eval_fft / interpolate_fft on (batch, n, 2) or (n, 2) uint64 arrays; returns a new array"""

@@ -73,6 +73,11 @@ class DgExecutionInfo(ctypes.Structure):
     _fields_ = [("width", u32), ("length", u64), ("steps", u64), ("ctx_depth", u32), ("loop_depth", u32), ("stack_depth", u32)]
 
 
+class DgExecutionStats(ctypes.Structure):
+    _fields_ = [("shape_launches", u32), ("write_launches", u32), ("waves", u32), ("prove_groups", u32), ("lanes", u64),
+                ("shape_ms", ctypes.c_float), ("write_ms", ctypes.c_float)]
+
+
 DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -97,6 +102,11 @@ EXPORTS = {
                        ctypes.POINTER(ctypes.c_int)],
     "dg_execute_batch": [ctypes.POINTER(DgProgram), u32, ctypes.POINTER(DgProgramInputs), u32, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp),
                          vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_trace_programs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), u64,
+                          ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgExecutionStats)],
+    "dg_execute_programs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32), u64,
+                            ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
+                            ctypes.POINTER(DgExecutionStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),

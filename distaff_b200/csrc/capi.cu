@@ -522,16 +522,48 @@ int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t wid
                      program_hashes32, reports, nullptr, d_step_masks);
     });
 }
+int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                      const dg_program_inputs_t *inputs, uint64_t max_steps, dg_execution_info_t *info, uint8_t *const *registers_out,
+                      int *status, dg_execution_stats_t *vm_stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(programs && program_of && inputs && status, "null argument");
+        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        trace_programs(c, x, info, registers_out, status, t_batch_messages, vm_stats);
+    });
+}
+int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                        const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                        dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
+        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+        check_execution_call(x);
+        check_output_counts(count, num_outputs, outputs16);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        execute_programs(c, x, num_outputs, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, stats, vm_stats);
+    });
+}
+// the one-program case: program_of all 0
 int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
                    dg_execution_info_t *info, uint8_t *const *registers_out, int *status) {
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(program && inputs && status, "null argument");
-        check_execution_call(program, count, inputs, max_steps);      // a bad encoding is rejected before the device is touched
+        const std::vector<uint32_t> of(count, 0);
+        const ExecutionCall x{program, 1, count, of.data(), inputs, max_steps};
+        check_execution_call(x);      // a bad encoding is rejected before the device is touched
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        trace_batch(c, program, count, inputs, max_steps, info, registers_out, status, t_batch_messages);
+        trace_programs(c, x, info, registers_out, status, t_batch_messages, nullptr);
     });
 }
 int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
@@ -539,11 +571,19 @@ int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_progr
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(program && inputs && options && proofs_out && status, "null argument");
-        check_execution_call(program, count, inputs, max_steps);
+        const std::vector<uint32_t> of(count, 0);
+        const ExecutionCall x{program, 1, count, of.data(), inputs, max_steps};
+        check_execution_call(x);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        execute_batch(c, program, count, inputs, num_outputs, max_steps, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, stats);
+        DG_REQUIRE(num_outputs <= 8, "cannot have more than 8 outputs");
+        DG_REQUIRE(num_outputs == 0 || outputs16, "null outputs");
+        const std::vector<uint32_t> n_out(count, num_outputs);
+        std::vector<uint8_t> outs((size_t)count * 8 * 16);
+        execute_programs(c, x, n_out.data(), *options, (Proof **)proofs_out, outs.data(), status, t_batch_messages, stats, nullptr);
+        if (num_outputs)     // num_outputs elements per execution
+            for (uint32_t i = 0; i < count; i++) memcpy(outputs16 + (size_t)16 * num_outputs * i, outs.data() + (size_t)128 * i, (size_t)16 * num_outputs);
     });
 }
 int dg_batch_message(uint32_t index, char *message, size_t cap) {

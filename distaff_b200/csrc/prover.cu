@@ -1214,30 +1214,16 @@ void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, cons
     });
 }
 
-void prove_batch_generated(Context &c, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                           const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                           const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
-                           const std::function<void(uint32_t, int, fe *, std::vector<std::pair<int, std::string>> &)> &generate) {
-    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
-    prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
-        // the traces are generated where a host batch is uploaded to, which the plan counts per proof
-        c.upload_buf.ensure((size_t)length * 16 * width * k, true);
-        std::vector<std::pair<int, std::string>> failed(k, std::make_pair(DG_OK, std::string()));
-        generate(first, k, c.upload_buf.as<fe>(), failed);
-        for (int i = 0; i < k; i++) if (failed[i].first != DG_OK) ps[i].fail(failed[i].first, failed[i].second);
-        prove_core(c, c.upload_buf.as<fe>(), nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st, chunk);
-        for (int i = 0; i < k; i++) if (failed[i].first != DG_OK) ps[i].fail(failed[i].first, failed[i].second);     // not the constraint check's
-    });
-}
-
 void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats) {
+                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
+                        uint32_t *groups) {
     DG_REQUIRE(count >= 1, "batch must hold at least one trace");
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
+    if (groups) *groups = 0;
     prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
         prove_core(c, const_cast<fe *>(d_regs) + (size_t)first * width * length, nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st, chunk);
+        if (groups) ++*groups;
     });
 }
 

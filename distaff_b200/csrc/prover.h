@@ -22,25 +22,29 @@ Proof *prove_device(Context &c, const fe *d_registers, uint32_t width, uint64_t 
 void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                       const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, Proof **proofs_out, int *status,
                       std::vector<std::string> &messages, dg_prove_stats_t *stats);
+// groups (may be null) receives the number of prove groups the batch ran in
 void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
                         const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats);
+                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
+                        uint32_t *groups = nullptr);
 
-// Batched proving of `count` traces of one shape that are generated on the device group by group: generate(first, k, d_regs, failed)
-// writes traces [first, first + k) into d_regs ([k][width][length], the buffer the prover then reads) and sets failed[i] to the status and
-// message of a trace it could not generate (failed holds k entries of DG_OK on entry).  Otherwise as prove_batch_device.
-void prove_batch_generated(Context &c, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                           const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                           const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
-                           const std::function<void(uint32_t, int, fe *, std::vector<std::pair<int, std::string>> &)> &generate);
-// dg_trace_batch / dg_execute_batch (execute.cu): status / messages per execution.  check_execution_call validates the arguments and the
-// program encoding on the host alone (DG_ERR_INVALID); both calls run it again.
-void check_execution_call(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps);
-void trace_batch(Context &c, const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
-                 dg_execution_info_t *info, uint8_t *const *registers_out, int *status, std::vector<std::string> &messages);
-void execute_batch(Context &c, const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs,
-                   uint64_t max_steps, const dg_options_t &opt, Proof **proofs_out, uint8_t *outputs16, int *status,
-                   std::vector<std::string> &messages, dg_prove_stats_t *stats);
+// dg_trace_programs / dg_execute_programs (execute.cu; dg_trace_batch / dg_execute_batch with one program): execution i runs
+// programs[program_of[i]] on inputs[i]; status / messages per execution.  check_execution_call validates the arguments and every
+// program's encoding on the host alone (DG_ERR_INVALID), as does check_output_counts the per-execution output counts; the calls run
+// them again.  execute_programs writes 8 output elements per execution (zero past its num_outputs).
+struct ExecutionCall {
+    const dg_program_t *programs;
+    uint32_t n_programs, count;
+    const uint32_t *program_of;
+    const dg_program_inputs_t *inputs;
+    uint64_t max_steps;
+};
+void check_execution_call(const ExecutionCall &x);
+void check_output_counts(uint32_t count, const uint32_t *num_outputs, const uint8_t *outputs16);
+void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                    std::vector<std::string> &messages, dg_execution_stats_t *vm_stats);
+void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
+                      uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP
 int batch_group_cap(long long k);
 

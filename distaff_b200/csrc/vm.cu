@@ -1,13 +1,14 @@
-// The Distaff VM on the GPU: processor::execute (processor/mod.rs:23-182, decoder/mod.rs, stack/mod.rs) of one program for many inputs,
-// one thread per execution.  It restates the Machine of the host VM (hostvm/vm.cpp) as a loop: run_blocks / close_block / run_span
-// become an explicit frame stack, and the decoder and stack operations keep their order, checks and messages.
+// The Distaff VM on the GPU: processor::execute (processor/mod.rs:23-182, decoder/mod.rs, stack/mod.rs) of many programs for many
+// inputs, one thread per execution.  It restates the Machine of the host VM (hostvm/vm.cpp) as a loop: run_blocks / close_block /
+// run_span become an explicit frame stack, and the decoder and stack operations keep their order, checks and messages.  The programs of
+// a call share one set of tables; each program's executions start on a warp boundary, so that a warp runs one instruction stream.
 //
-// Two passes, each one launch for all executions of a call:
+// Two passes, each one launch for many executions:
 //   shape pass  no sponge and no register writes: the step count, the ctx / loop / stack depths, the peak tape lengths, the final stack
 //               and the first failure.  Control flow and the stack never read the sponge, so this is the whole execution but the hash.
-//   write pass  the same execution with the sponge, writing every register of every row up to the last step into [count][width][length]
-//               buffers of one shape; it also checks the loop images and the program hash, which need the sponge.  A second, coalesced
-//               kernel writes the padding rows of Machine::finalize.
+//   write pass  the same execution with the sponge, writing every register of every row up to the last step into its own place and
+//               shape (one launch covers executions of any mix of shapes); it also checks the loop images and the program hash, which
+//               need the sponge.  A second, coalesced kernel writes the padding rows of Machine::finalize, one launch per shape.
 // The per-thread stack, context stack, loop stack and frame stack are indexed at run time and live in local memory by design.
 #define DG_MUL_CALL 1
 #include "common.cuh"
@@ -134,7 +135,9 @@ struct Machine {
     fe ctx[16], lp[8], S[32];
     fe *ta, *tb;
     unsigned long long na, nb, cap_a, cap_b, peak_a, peak_b;
-    fe *out;                      // write pass: this execution's registers, column stride L.length
+    fe *out;                      // write pass: this execution's registers, column stride `length`
+    unsigned long long length;
+    unsigned ctx_out, loop_out, stack_out;
 
     __device__ Machine(const VmLaunch &l) : L(l), max_steps(l.max_steps) {}
 
@@ -142,16 +145,16 @@ struct Machine {
     __device__ __forceinline__ bool failed() const { return code != VM_OK; }
 
     // ---- registers of the write pass
-    __device__ __forceinline__ void put(unsigned col, unsigned long long row, fe v) { out[(size_t)col * L.length + row] = v; }
+    __device__ __forceinline__ void put(unsigned col, unsigned long long row, fe v) { out[(size_t)col * length + row] = v; }
     __device__ void commit_state() {
         if (!WRITE) return;
         const unsigned long long s = step;
         put(0, s, fe_small(opc));
         for (int i = 0; i < 4; i++) put(1 + i, s, sponge[i]);
         unsigned col = 15;
-        for (unsigned i = 0; i < L.ctx_out; i++) put(col++, s, ctx[i]);
-        for (unsigned i = 0; i < L.loop_out; i++) put(col++, s, lp[i]);
-        for (unsigned i = 0; i < L.stack_out; i++) put(col++, s, i < 32 ? S[i] : fe_small(0));
+        for (unsigned i = 0; i < ctx_out; i++) put(col++, s, ctx[i]);
+        for (unsigned i = 0; i < loop_out; i++) put(col++, s, lp[i]);
+        for (unsigned i = 0; i < stack_out; i++) put(col++, s, i < 32 ? S[i] : fe_small(0));
     }
     __device__ void commit_bits(unsigned flow, unsigned user) {    // the op bits of the step that led to row `step` sit in row step - 1
         if (!WRITE) return;
@@ -177,7 +180,7 @@ struct Machine {
 
     __device__ bool advance(bool user_op) {
         if (step + 1 >= max_steps) { code = VM_CAP; fail_step = step; return false; }
-        if (WRITE && step + 1 >= L.length) return fail(VM_DIVERGED);      // never past the rows the shape pass measured
+        if (WRITE && step + 1 >= length) return fail(VM_DIVERGED);        // never past the rows the shape pass measured
         step += 1;
         if (user_op) opc += 1;
         return true;
@@ -443,10 +446,10 @@ struct Machine {
     }
     // run_blocks(root body), then close_block(0, true), with the recursion as a frame stack: a frame is a block list being run, `k` the
     // next block of it, `cont` what its block does when the list ends.  The host checked that lists nest at most 15 deep.
-    __device__ void run() {
+    __device__ void run(unsigned root_first, unsigned root_count) {
         Frame fr[16];
         int top = 0;
-        fr[0] = Frame{L.root_first, L.root_count, 0, 0, C_ROOT};
+        fr[0] = Frame{root_first, root_count, 0, 0, C_ROOT};
         const fe z = fe_small(0);
         for (;;) {
             Frame &f = fr[top];
@@ -504,7 +507,9 @@ __global__ void __launch_bounds__(32) vm_kernel(const VmLaunch L) {
     const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= L.count) return;
     const unsigned e = L.ids[q];
+    if (e == VM_NO_EXECUTION) return;
     const VmInput in = L.in[e];
+    const VmProgram &P = L.programs[in.program];
     Machine<WRITE> m(L);
     m.ta = L.tapes + L.tape_off[e];
     m.cap_a = L.cap[2 * e];
@@ -521,14 +526,17 @@ __global__ void __launch_bounds__(32) vm_kernel(const VmLaunch L) {
     for (int i = 0; i < 32; i++) m.S[i] = (unsigned)i < in.n_pub ? L.data[in.pub + i] : z;
     m.depth = m.max_depth = in.n_pub;
     if (WRITE) {
-        m.out = L.out + (size_t)q * L.width * L.length;
+        const VmOut o = L.outs[e];
+        m.out = L.out + o.offset;
+        m.length = o.length;
+        m.ctx_out = o.ctx_out; m.loop_out = o.loop_out; m.stack_out = o.stack_out;
         m.commit_state();
     }
-    m.run();
+    m.run(P.root_first, P.root_count);
     VmResult &r = L.res[e];
     if (!m.failed()) {
         if (m.opc < 16) m.fail(VM_MIN_OPS);                                      // lib.rs:48-52
-        else if (WRITE && !(fe_eq(m.sponge[0], L.hash[0]) && fe_eq(m.sponge[1], L.hash[1]))) m.fail(VM_HASH);    // lib.rs:55-59
+        else if (WRITE && !(fe_eq(m.sponge[0], P.hash[0]) && fe_eq(m.sponge[1], P.hash[1]))) m.fail(VM_HASH);    // lib.rs:55-59
     }
     // the write pass must retrace the shape pass (control flow never reads the sponge); anything else would mean the shape is wrong
     if (WRITE && !m.failed() && (m.step != r.steps || m.ctx_cols != r.ctx_cols || m.loop_cols != r.loop_cols || m.max_depth != r.max_depth))
@@ -575,8 +583,12 @@ void vm_write_pass(Context &c, const VmLaunch &L) {
     vm_kernel<true><<<(L.count + 31) / 32, 32, 0, c.stream>>>(L);
     c.launches++;
     DG_CUDA(cudaGetLastError());
-    DG_REQUIRE(L.count <= 65535 && L.width <= 65535, "too many executions or registers for one padding launch");
-    vm_pad_kernel<<<dim3((unsigned)((L.length + 255) / 256), L.width, L.count), 256, 0, c.stream>>>(L.out, L.res, L.ids, L.width, L.length);
+}
+
+void vm_pad_rows(Context &c, fe *out, const VmResult *res, const unsigned *ids, unsigned count, unsigned width, unsigned long long length) {
+    if (count == 0) return;
+    DG_REQUIRE(count <= 65535 && width <= 65535, "too many executions or registers for one padding launch");
+    vm_pad_kernel<<<dim3((unsigned)((length + 255) / 256), width, count), 256, 0, c.stream>>>(out, res, ids, width, length);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }

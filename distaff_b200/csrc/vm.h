@@ -1,4 +1,4 @@
-// The VM interpreter (vm.cu) and what the host orchestration of dg_trace_batch / dg_execute_batch (execute.cu) passes to it.
+// The VM interpreter (vm.cu) and what the host orchestration of dg_trace_programs / dg_execute_programs (execute.cu) passes to it.
 #pragma once
 #include "../../include/distaff_gpu.h"
 #include "common.cuh"
@@ -9,8 +9,20 @@ namespace dg {
 struct VmHint { unsigned kind, n; fe value; };
 struct VmBlock { unsigned kind, first, count, alt_first, alt_count, pad[3]; fe hash[3]; };
 
-// per execution: public inputs at data[pub], tape A (reversed: its first element last) at data[a], tape B (reversed) at data[b]
-struct VmInput { unsigned long long pub, a, b, n_a, n_b; unsigned n_pub, pad; };
+// The programs of a call share the ops / hints / blocks / children tables (their ranges rebased on the host); per program only the root
+// body and Program::hash() differ
+struct VmProgram { unsigned root_first, root_count; fe hash[2]; };
+
+// per execution: public inputs at data[pub], tape A (reversed: its first element last) at data[a], tape B (reversed) at data[b], and the
+// index of its program in VmLaunch::programs
+struct VmInput { unsigned long long pub, a, b, n_a, n_b; unsigned n_pub, program; };
+
+// write pass, per execution: its registers at VmLaunch::out + offset, `width` columns of `length` rows, of which the context, loop and
+// stack columns number ctx_out, loop_out and stack_out
+struct VmOut { unsigned long long offset, length; unsigned width, ctx_out, loop_out, stack_out; };
+
+// launch slots that run no execution (the lanes after a program's last execution in its last warp)
+constexpr unsigned VM_NO_EXECUTION = 0xffffffffu;
 
 // Why an execution stopped.  Codes below VM_NO_STEP are the VM's own failures, reported as "<message> at step <fail_step>" (hostvm's
 // Machine::fail); the others carry no step.  VM_TAPE_SCRATCH is internal: the shape pass ran out of tape scratch and is repeated with more.
@@ -33,24 +45,24 @@ struct VmResult {
 
 struct VmLaunch {
     const uint8_t *ops; const VmHint *hints; const VmBlock *blocks; const unsigned *children;
-    unsigned root_first, root_count;
-    fe hash[2];                           // Program::hash()
+    const VmProgram *programs;
     const VmInput *in; const fe *data;
     fe *tapes;                            // per execution: tape A at tapes + tape_off[e] (cap[2e] elements), tape B after it (cap[2e + 1])
     const unsigned long long *tape_off, *cap;
-    const unsigned *ids;                  // the executions of this launch
+    const unsigned *ids;                  // the executions of this launch: each program's from a multiple of 32, VM_NO_EXECUTION between
     unsigned count;
     unsigned long long max_steps;
     VmResult *res;
-    // write pass: execution ids[q] into out + q * width * length, columns of one shape
+    // write pass: execution e into out + outs[e].offset, with its own shape
     fe *out;
-    unsigned long long length;
-    unsigned width, ctx_out, loop_out, stack_out;
+    const VmOut *outs;
 };
 
 void vm_upload_constants(Context &c);
 void vm_shape_pass(Context &c, const VmLaunch &L);
-void vm_write_pass(Context &c, const VmLaunch &L);     // the write pass, then the padding rows
+void vm_write_pass(Context &c, const VmLaunch &L);
+// the padding rows of `count` executions of one shape, ids[q]'s registers at out + q * width * length (after the write pass)
+void vm_pad_rows(Context &c, fe *out, const VmResult *res, const unsigned *ids, unsigned count, unsigned width, unsigned long long length);
 std::string vm_message(unsigned code, unsigned long long step, unsigned long long max_steps);
 
 }  // namespace dg

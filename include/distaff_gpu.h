@@ -81,7 +81,8 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
  * several GPUs; DG_ERR_CUDA; DG_ERR_NO_DEVICE); on such an error every proofs_out[i] is NULL (nothing to free).  The library splits the
  * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
  * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) the message of entry i of the
- * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device, dg_verify_batch, dg_trace_batch or dg_execute_batch: why
+ * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device, dg_verify_batch, dg_trace_batch, dg_execute_batch,
+ * dg_trace_programs or dg_execute_programs: why
  * trace i failed (the message dg_prove gives for that trace), why proof i was not accepted (what dg_verify reports for that proof) or
  * why execution i failed, and "" if it was proven / accepted / executed. */
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -190,7 +191,8 @@ typedef struct {                 /* the shape of one execution's trace, what exe
 
 #define DG_ERR_EXECUTION (-7)    /* the program failed on these inputs (processor::execute / lib.rs:48-60 panic); message as the host VM's */
 
-/* dg_trace_batch: executes the program for inputs[0 .. count) in one launch per pass.  Per execution: status[i] = DG_OK and info[i], or
+/* dg_trace_batch: executes the program for inputs[0 .. count): the shape pass, then the write pass in waves (as dg_trace_programs,
+ * below).  Per execution: status[i] = DG_OK and info[i], or
  * DG_ERR_EXECUTION with dg_batch_message(i) = the VM's message ("ASSERT failed at step 17", ...; "execution exceeds N steps" when the
  * last step would reach max_steps, which bounds how long a program that never stops keeps the GPU busy).  registers_out: NULL (only the
  * shape pass runs, so that a caller can size its buffers first), or count pointers, each to info[i].width * info[i].length * 16 bytes
@@ -206,6 +208,34 @@ int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program
  * A failing execution changes no other result.  stats (may be NULL) covers the proofs. */
 int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
                      const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats);
+
+/* ---- executing many programs -------------------------------------------------------------------------------------------------------
+ * dg_trace_programs / dg_execute_programs: dg_trace_batch / dg_execute_batch for executions of different programs in one call (those two
+ * are the one-program case).  Execution i runs programs[program_of[i]] on inputs[i]; each program of the table is validated once, and a
+ * bad one fails the call with DG_ERR_INVALID and "program p: " before the message when the table holds more than one.  Each program's
+ * executions run in warps of their own.  After the shape pass the successful executions are written in waves: one write launch per
+ * wave covers every trace shape in it; a wave's traces take at most half of the device memory the library may use (dg_set_memory_limit)
+ * and leave room for one proof of the wave's largest shape; $DG_BATCH_GROUP caps the executions of a wave.  dg_execute_programs proves
+ * each shape's traces of a wave together, whichever programs they came from, where they were written; the RNG callbacks run shape by
+ * shape, in input order inside a shape.  Per execution, results and failures are as in dg_trace_batch / dg_execute_batch, with the
+ * messages in dg_batch_message; num_outputs[i] (<= 8) is per execution and outputs16 holds 8 elements per execution (zero past
+ * num_outputs[i]; it may be NULL when every num_outputs[i] is 0).  Bad arguments (n_programs == 0, program_of[i] >= n_programs, more than
+ * 2^32 ops in all, num_outputs[i] > 8, a bad encoding) are rejected before the device is touched; a context that spans several GPUs is
+ * rejected.  vm_stats (may be NULL) describes the VM passes. */
+typedef struct {
+    uint32_t shape_launches;     /* shape-pass launches (more than one when an execution outgrows its tape scratch) */
+    uint32_t write_launches;     /* write-pass launches, one per wave (each followed by one padding launch per shape) */
+    uint32_t waves;
+    uint32_t prove_groups;       /* prove groups of dg_execute_programs (0 for dg_trace_programs) */
+    uint64_t lanes;              /* threads of the write launches, idle lanes included */
+    float shape_ms, write_ms;    /* device time of the shape and write passes (padding included) */
+} dg_execution_stats_t;
+int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                      const dg_program_inputs_t *inputs, uint64_t max_steps, dg_execution_info_t *info, uint8_t *const *registers_out,
+                      int *status, dg_execution_stats_t *vm_stats);
+int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                        const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                        dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
 
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
