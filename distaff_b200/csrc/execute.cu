@@ -120,6 +120,15 @@ struct Executions {
     ~Executions() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 
     void fail(uint32_t i, int code, const std::string &m) { status[i] = code; messages[i] = m; }
+    // "<what> <j> is not a field element" for the first of n values at or above M, else ""
+    static std::string first_non_element(const uint8_t *p, uint64_t n, const char *what) {
+        for (uint64_t j = 0; j < n; j++) {
+            fe e;
+            memcpy(&e, p + 16 * j, 16);
+            if (e.hi == DG_M_HI && e.lo >= DG_M_LO) return std::string(what) + " " + std::to_string(j) + " is not a field element";
+        }
+        return "";
+    }
 
     template <typename T> void upload(DevBuf &d, const std::vector<T> &v) {
         d.alloc(std::max<size_t>(v.size(), 1) * sizeof(T));
@@ -183,6 +192,11 @@ struct Executions {
             in[i].program = x.program_of[i];
             if (v.n_public > 8) { fail(i, DG_ERR_EXECUTION, "expected no more than 8 public inputs"); continue; }      // lib.rs:32
             if (v.n_secret_a < v.n_secret_b) { fail(i, DG_ERR_EXECUTION, "tape A cannot be shorter than tape B"); continue; }   // inputs.rs:17
+            // the VM's arithmetic assumes canonical operands: a value in [M, 2^128) fails its execution (the reference does not check)
+            std::string bad = first_non_element(v.public16, v.n_public, "public input");
+            if (bad.empty()) bad = first_non_element(v.secret_a16, v.n_secret_a, "tape A value");
+            if (bad.empty()) bad = first_non_element(v.secret_b16, v.n_secret_b, "tape B value");
+            if (!bad.empty()) { fail(i, DG_ERR_EXECUTION, bad); continue; }
             auto put = [&](const uint8_t *p, uint64_t n, bool reverse) {
                 const size_t at = data.size();
                 for (uint64_t j = 0; j < n; j++) { fe e; memcpy(&e, p + 16 * (reverse ? n - 1 - j : j), 16); data.push_back(e); }
@@ -442,11 +456,15 @@ void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_ou
         if (X.status[i] == DG_OK) for (uint32_t j = 0; j < num_outputs[i]; j++) outs[(size_t)i * 8 + j] = X.res[i].top[j];
     X.write_waves(&opt, nullptr, [&](const std::vector<Slab> &slabs) {
         for (const Slab &s : slabs) {
-            // executions the write pass failed are left out: the traces after them move down over them
+            // executions the write pass failed are left out: the traces after them move down over them, and their outputs are zero, as
+            // those of executions the shape pass failed
             const size_t per = (size_t)s.shape.width * s.shape.length;
             std::vector<unsigned> ok;
             for (size_t q = 0; q < s.ids.size(); q++) {
-                if (X.status[s.ids[q]] != DG_OK) continue;
+                if (X.status[s.ids[q]] != DG_OK) {
+                    std::fill(outs.begin() + (size_t)s.ids[q] * 8, outs.begin() + (size_t)s.ids[q] * 8 + 8, fe_make(0, 0));
+                    continue;
+                }
                 if (ok.size() != q)
                     DG_CUDA(cudaMemcpyAsync(s.regs + ok.size() * per, s.regs + q * per, per * 16, cudaMemcpyDeviceToDevice, c.stream));
                 ok.push_back(s.ids[q]);

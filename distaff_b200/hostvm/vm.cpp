@@ -647,7 +647,12 @@ struct Machine {
                 u128 idx = R(2);
                 std::vector<u128> va(tape_a.end() - n, tape_a.end());
                 tape_a.resize(tape_a.size() - n);
-                for (size_t i = 0; i < n; i++) { tape_a.push_back((idx >> (n - i - 1)) & 1); tape_a.push_back(va[i]); }
+                // bit k of the index, 0 from bit 128 on (a shift by 128 or more is undefined in C++; the GPU VM's bit_of does the same)
+                for (size_t i = 0; i < n; i++) {
+                    const size_t k = n - i - 1;
+                    tape_a.push_back(k < 128 ? (idx >> k) & 1 : 0);
+                    tape_a.push_back(va[i]);
+                }
             } else if (hint.kind == H_NONE) { if (tape_a.empty() || tape_b.empty()) fail("attempt to read from empty tape"); }
             else fail("invalid hint for READ2");
             shift_right(0, 2);
@@ -818,6 +823,14 @@ static Execution *run(const Program *prog, const std::string *source, const std:
     try {
         if (pub.size() > 8) throw std::runtime_error("expected no more than 8 public inputs");
         if (sa.size() < sb.size()) throw std::runtime_error("tape A cannot be shorter than tape B");
+        // the field arithmetic assumes canonical operands (the reference does not check; see include/distaff_gpu.h)
+        auto check = [](const std::vector<u128> &v, const char *what) {
+            for (size_t i = 0; i < v.size(); i++)
+                if (v[i] >= M) throw std::runtime_error(std::string(what) + " " + std::to_string(i) + " is not a field element");
+        };
+        check(pub, "public input");
+        check(sa, "tape A value");
+        check(sb, "tape B value");
         Program compiled;
         if (!prog) { compiled = compile(*source); prog = &compiled; }
         Machine m(pub, sa, sb);

@@ -176,7 +176,11 @@ typedef struct {                 /* Program (programs/mod.rs) */
     uint8_t hash32[32];          /* Program::hash() */
 } dg_program_t;
 
-typedef struct {                 /* ProgramInputs::new(public, secret_a, secret_b) (programs/inputs.rs:12) */
+/* ProgramInputs::new(public, secret_a, secret_b) (programs/inputs.rs:12).  Every value must be a field element, below M: a public input or
+ * tape value in [M, 2^128) fails that execution (DG_ERR_EXECUTION, "public input 2 is not a field element", "tape A value 0 is not a
+ * field element", "tape B value 5 ..."; the first one in that order), before it runs, and no other.  The reference accepts such values
+ * and leaves what a program computes from them undefined (its field arithmetic assumes canonical operands). */
+typedef struct {
     const uint8_t *public16; uint32_t n_public;      /* at most 8 (lib.rs:32), else the execution fails */
     const uint8_t *secret_a16; uint64_t n_secret_a;  /* tape A, read first to last */
     const uint8_t *secret_b16; uint64_t n_secret_b;  /* tape B, not longer than tape A, else the execution fails */
@@ -196,7 +200,11 @@ typedef struct {                 /* the shape of one execution's trace, what exe
  * DG_ERR_EXECUTION with dg_batch_message(i) = the VM's message ("ASSERT failed at step 17", ...; "execution exceeds N steps" when the
  * last step would reach max_steps, which bounds how long a program that never stops keeps the GPU busy).  registers_out: NULL (only the
  * shape pass runs, so that a caller can size its buffers first), or count pointers, each to info[i].width * info[i].length * 16 bytes
- * that receive the column-major registers of a successful execution (entries of failed executions may be NULL).  Returns DG_OK when the
+ * that receive the column-major registers of a successful execution (entries of failed executions may be NULL).  The shape pass does
+ * not compute the sponge, so a shapes-only call reports DG_OK and the shape for the two failures that need it: "program hash does not
+ * match trace hash" and "hash of the last iteration doesn't match loop image"; only a call with registers_out reports them.  The trace
+ * length is the smallest power of two above the last step (16 at least: a last step of 2^k - 1 gives 2^k), and a last step that would
+ * reach max_steps fails the execution: it succeeds with max_steps = last step + 1.  Returns DG_OK when the
  * batch ran, whatever the executions did; DG_ERR_INVALID for a bad encoding or a context that spans several GPUs. */
 int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program_inputs_t *inputs, uint64_t max_steps,
                    dg_execution_info_t *info, uint8_t *const *registers_out, int *status);
@@ -219,8 +227,8 @@ int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_progr
  * each shape's traces of a wave together, whichever programs they came from, where they were written; the RNG callbacks run shape by
  * shape, in input order inside a shape.  Per execution, results and failures are as in dg_trace_batch / dg_execute_batch, with the
  * messages in dg_batch_message; num_outputs[i] (<= 8) is per execution and outputs16 holds 8 elements per execution (zero past
- * num_outputs[i]; it may be NULL when every num_outputs[i] is 0).  Bad arguments (n_programs == 0, program_of[i] >= n_programs, more than
- * 2^32 ops in all, num_outputs[i] > 8, a bad encoding) are rejected before the device is touched; a context that spans several GPUs is
+ * num_outputs[i], and all zero for an execution the VM failed; it may be NULL when every num_outputs[i] is 0).  Bad arguments
+ * (n_programs == 0, program_of[i] >= n_programs, more than 2^32 ops in all, num_outputs[i] > 8, a bad encoding) are rejected before the device is touched; a context that spans several GPUs is
  * rejected.  vm_stats (may be NULL) describes the VM passes. */
 typedef struct {
     uint32_t shape_launches;     /* shape-pass launches (more than one when an execution outgrows its tape scratch) */
