@@ -23,6 +23,7 @@
 #define DG_MUL_CALL 1
 #include "air.h"
 #include "air_constants.h"
+#include "host_fs.h"
 
 namespace dg {
 
@@ -687,6 +688,53 @@ void launch_check_reduce(Context &c, const unsigned *masks, unsigned long long n
     check_reduce_kernel<<<dim3(gx, (unsigned)batch), 256, 0, c.stream>>>(masks, n, T, stats);
     c.launches++;
     DG_CUDA(cudaGetLastError());
+}
+
+// ---- host side: the register shape ---------------------------------------------------------------------------------------------
+
+static int first_stack_register(uint32_t ctx_depth, uint32_t loop_depth) { return 15 + (int)ctx_depth + (int)loop_depth; }
+
+TraceShape::TraceShape(int ctx, int loop, int stack)
+    : w(first_stack_register(ctx, loop) + stack), ctx_depth(ctx), loop_depth(loop), stack_depth(stack), cl(std::max(ctx, 1)),
+      ll(std::max(loop, 1)), sl(std::max(stack, 8)), T(20 + cl + ll + 2 + stack), stack_reg(first_stack_register(ctx, loop)) {}
+
+bool TraceShape::in_range(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth) {
+    return ctx_depth <= 16 && loop_depth <= 8 && stack_depth >= 1 && stack_depth <= 32;
+}
+
+TraceShape TraceShape::of_trace(uint32_t width, uint32_t ctx_depth, uint32_t loop_depth) {
+    DG_REQUIRE(ctx_depth <= 16, "context depth cannot be greater than 16");
+    DG_REQUIRE(loop_depth <= 8, "loop depth cannot be greater than 8");
+    DG_REQUIRE(width < 128, "execution trace cannot have more than 128 registers");
+    const int stack_depth = (int)width - first_stack_register(ctx_depth, loop_depth);
+    DG_REQUIRE(stack_depth >= 1, "user stack must consist of at least one register");
+    DG_REQUIRE(stack_depth <= 32, "stack depth cannot be greater than 32");
+    return TraceShape((int)ctx_depth, (int)loop_depth, stack_depth);
+}
+
+AirParams TraceShape::air_params(uint64_t n) const {
+    AirParams P;
+    memset(&P, 0, sizeof P);
+    P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
+    P.cl = cl; P.ll = ll; P.sl = sl;
+    P.log_n = ceil_log2(n);
+    for (int g = 0; g < 6; g++) P.inc[g] = group_increment(g, n);
+    return P;
+}
+
+unsigned long long group_increment(int g, uint64_t n) {
+    static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
+    return (8 * n - 1) - (n - 1) * GROUP_DEG[g];
+}
+
+const fe *periodic_table(Context &c) {
+    if (!c.d_periodic.p) {
+        const std::vector<fe> per = fs::periodic_tables();
+        c.d_periodic.alloc(per.size() * 16, true);
+        DG_CUDA(cudaMemcpyAsync(c.d_periodic.p, per.data(), per.size() * 16, cudaMemcpyHostToDevice, c.stream));
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    return c.d_periodic.as<fe>();
 }
 
 }  // namespace dg

@@ -31,6 +31,28 @@ struct AirParams {
     unsigned *masks;
 };
 
+// The register layout of a trace (trace_state.rs:58-60): 15 decoder registers, the context stack, the loop stack, then the user stack.
+struct TraceShape {
+    int w, ctx_depth, loop_depth, stack_depth;
+    int cl, ll, sl;                     // padded stack lengths: max(depth, 1 / 1 / 8)
+    int T;                              // transition constraints: 20 decoder, cl context, ll loop, 2 stack auxiliary, stack_depth stack
+    int stack_reg;                      // first user-stack register
+    // the layout of depths known to be in range
+    TraceShape(int ctx_depth, int loop_depth, int stack_depth);
+    // what dg_prove accepts: at most 16 context, 8 loop and 32 user-stack registers, at least one of the last
+    static bool in_range(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth);
+    // the shape of a trace of `width` registers (trace_table.rs:23-58); throws DG_ERR_INVALID with the prover's message when out of range
+    static TraceShape of_trace(uint32_t width, uint32_t ctx_depth, uint32_t loop_depth);
+    // AirParams with this shape's part filled in for traces of n steps (depths, padded lengths, log_n, inc[]), every other field zero
+    AirParams air_params(uint64_t n) const;
+};
+
+// exponent of the degree adjustment of degree group g (degrees 2, 3, 4, 6, 7, 8) for traces of n steps (evaluator.rs:395-402)
+unsigned long long group_increment(int g, uint64_t n);
+
+// the periodic AIR tables on c's device, uploaded the first time
+const fe *periodic_table(Context &c);
+
 // A trace step k that violates a transition constraint is recorded as atomicMax(violation, 0xFFFFFFFF - k), so the lowest violating
 // step wins, as in the reference's sequential loop (prover.rs:52-64), and a max-reduce over ranks keeps it.  0 means no violation.
 __host__ __device__ inline unsigned violation_word(unsigned long long step) { return 0xFFFFFFFFu - (unsigned)step; }

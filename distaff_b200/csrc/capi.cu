@@ -362,10 +362,10 @@ int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth
         std::lock_guard<std::mutex> lk(c.mu);
         DG_REQUIRE(ext16 && out16 && first_violation && (seeds32 || coefs16), "null argument");
         DG_REQUIRE(count >= 1 && count <= 65535, "count must be in 1..65535");
-        DG_REQUIRE(ctx_depth <= 16 && loop_depth <= 8 && stack_depth >= 1 && stack_depth <= 32, "register shape out of range");
+        DG_REQUIRE(TraceShape::in_range(ctx_depth, loop_depth, stack_depth), "register shape out of range");
         DG_REQUIRE(log_n >= 4 && log_blowup >= 4 && log_blowup <= 8 && log_n + log_blowup <= 20, "trace length or extension factor out of range");
-        const int w = 15 + ctx_depth + loop_depth + stack_depth;
-        const int T = 20 + std::max<int>(ctx_depth, 1) + std::max<int>(loop_depth, 1) + 2 + stack_depth;
+        const TraceShape shape(ctx_depth, loop_depth, stack_depth);
+        const int w = shape.w, T = shape.T;
         const size_t n = (size_t)1 << log_n, b = (size_t)1 << log_blowup, N = n << log_blowup, E = 8 * n;
 
         // per entry [coefA | coefB] in evaluation order, drawn as the prover draws them (no public inputs or outputs) or given
@@ -375,9 +375,7 @@ int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth
         } else {
             const fe no_hash[2] = {fe_make(0, 0), fe_make(0, 0)};
             for (uint32_t q = 0; q < count; q++) {
-                fs::ConstraintCoefficients cc = fs::draw_constraint_coefficients(seeds32 + 32 * (size_t)q, ctx_depth, loop_depth, stack_depth, {}, {},
-                                                                                 fe_make(0, 0), no_hash);
-                DG_REQUIRE(cc.coefA.size() == (size_t)T, "transition constraint count mismatch");
+                fs::ConstraintCoefficients cc = fs::draw_constraint_coefficients(seeds32 + 32 * (size_t)q, shape, {}, {}, fe_make(0, 0), no_hash);
                 std::copy(cc.coefA.begin(), cc.coefA.end(), coef.begin() + (size_t)q * 2 * T);
                 std::copy(cc.coefB.begin(), cc.coefB.end(), coef.begin() + (size_t)q * 2 * T + T);
             }
@@ -388,29 +386,19 @@ int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth
             for (size_t k = 0; k < n; k++)
                 for (size_t cs = 0; cs < b; cs++) memcpy(&slab[col * N + cs * n + k], ext16 + (col * N + k * b + cs) * 16, 16);
 
-        if (!c.d_periodic.p) {
-            std::vector<fe> per = fs::periodic_tables();
-            c.d_periodic.alloc(per.size() * 16, true);
-            DG_CUDA(cudaMemcpyAsync(c.d_periodic.p, per.data(), per.size() * 16, cudaMemcpyHostToDevice, c.stream));
-            DG_CUDA(cudaStreamSynchronize(c.stream));
-        }
+        const fe *periodic = periodic_table(c);
         DevBuf d_ext(slab.size() * 16), d_coef(coef.size() * 16), d_out((size_t)count * E * 16), d_violation((size_t)4 * count);
         DG_CUDA(cudaMemcpyAsync(d_ext.p, slab.data(), slab.size() * 16, cudaMemcpyHostToDevice, c.stream));
         DG_CUDA(cudaMemcpyAsync(d_coef.p, coef.data(), coef.size() * 16, cudaMemcpyHostToDevice, c.stream));
         DG_CUDA(cudaMemsetAsync(d_violation.p, 0, (size_t)4 * count, c.stream));
-        AirParams P;
-        memset(&P, 0, sizeof P);
-        P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
-        P.cl = std::max<int>(ctx_depth, 1); P.ll = std::max<int>(loop_depth, 1); P.sl = std::max<int>(stack_depth, 8);
-        P.log_n = log_n; P.log_blowup = log_blowup;
+        AirParams P = shape.air_params(n);
+        P.log_blowup = log_blowup;
         P.ext = d_ext.as<fe>(); P.col_stride = N;
         P.c8_base = 0; P.num_c8 = 8;
         P.t_ev = d_out.as<fe>();
-        P.periodic = c.d_periodic.as<fe>();
+        P.periodic = periodic;
         P.coefA = d_coef.as<fe>(); P.coefB = d_coef.as<fe>() + T;
         P.twN = c.twiddle(log_n + log_blowup, false);
-        static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
-        for (int gi = 0; gi < 6; gi++) P.inc[gi] = (8 * n - 1) - (n - 1) * GROUP_DEG[gi];
         P.violation = d_violation.as<unsigned>();
         P.verify_mode = check ? 0 : 1;          // verify mode: no trace-domain check, a value at every step
         P.ext_stride = (size_t)w * N; P.t_ev_stride = E; P.coef_stride = 2 * T;
@@ -430,6 +418,19 @@ int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth
 }
 
 // ---- prover ------------------------------------------------------------------------------------------------------------------------
+// dg_prove / dg_prove_device: a batch of one whose failure is the call's error
+static Proof *prove_single(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth,
+                           uint32_t loop_depth, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
+                           const dg_options_t &opt, dg_prove_stats_t *stats) {
+    Proof *proof = nullptr;
+    int status = DG_OK;
+    std::vector<std::string> messages;
+    prove_traces(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, &inputs16, &n_inputs, &outputs16, &n_outputs, opt, false, &proof,
+                 &status, messages, stats);
+    if (status != DG_OK) throw Error(status, messages[0]);
+    return proof;
+}
+
 int dg_prove(const dg_trace_t *trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
              const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats) {
     return guarded([&] {
@@ -437,12 +438,12 @@ int dg_prove(const dg_trace_t *trace, const uint8_t *inputs16, uint32_t n_inputs
         DG_REQUIRE((n_inputs == 0 || inputs16) && (n_outputs == 0 || outputs16), "null public inputs / outputs");
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        if (ctx_device_count() > 1) {
-            *proof_out = (dg_proof_t *)prove_on_all_devices([&](Context &cg, dg_prove_stats_t *st) {
-                return prove_host(cg, *trace, inputs16, n_inputs, outputs16, n_outputs, *options, st); }, stats);
-            return;
-        }
-        *proof_out = (dg_proof_t *)prove_host(c, *trace, inputs16, n_inputs, outputs16, n_outputs, *options, stats);
+        auto prove = [&](Context &cg, dg_prove_stats_t *st) {
+            const std::vector<const uint8_t *> cols = trace_columns(trace, 1, "call", true);
+            return prove_single(cg, nullptr, cols.data(), trace->width, trace->length, trace->ctx_depth, trace->loop_depth, inputs16, n_inputs,
+                                outputs16, n_outputs, *options, st);
+        };
+        *proof_out = (dg_proof_t *)(ctx_device_count() > 1 ? prove_on_all_devices(prove, stats) : prove(c, stats));
     });
 }
 int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
@@ -453,14 +454,12 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
         DG_REQUIRE((n_inputs == 0 || inputs16) && (n_outputs == 0 || outputs16), "null public inputs / outputs");
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        if (ctx_device_count() > 1) {          // the trace lives on device 0; the other devices read their columns over NVLink (peer access)
-            *proof_out = (dg_proof_t *)prove_on_all_devices([&](Context &cg, dg_prove_stats_t *st) {
-                return prove_device(cg, (const fe *)d_registers, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs, *options,
-                                    st, 0.0f); }, stats);
-            return;
-        }
-        *proof_out = (dg_proof_t *)prove_device(c, (const fe *)d_registers, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16,
-                                                n_outputs, *options, stats, 0.0f);
+        // several devices: the trace lives on device 0; the other devices read their columns over NVLink (peer access)
+        auto prove = [&](Context &cg, dg_prove_stats_t *st) {
+            return prove_single(cg, (const fe *)d_registers, nullptr, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16,
+                                n_outputs, *options, st);
+        };
+        *proof_out = (dg_proof_t *)(ctx_device_count() > 1 ? prove_on_all_devices(prove, stats) : prove(c, stats));
     });
 }
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -472,7 +471,10 @@ int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *cons
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        prove_batch_host(c, traces, count, inputs16, n_inputs, outputs16, n_outputs, *options, (Proof **)proofs_out, status, t_batch_messages, stats);
+        const std::vector<const uint8_t *> cols = trace_columns(traces, count, "batch", false);
+        const dg_trace_t &t = traces[0];
+        prove_traces(c, nullptr, cols.data(), count, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+                     *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
     });
 }
 int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
@@ -484,8 +486,8 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        prove_batch_device(c, (const fe *)d_registers, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
-                           *options, (Proof **)proofs_out, status, t_batch_messages, stats);
+        prove_traces(c, (const fe *)d_registers, nullptr, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+                     *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
     });
 }
 int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -494,19 +496,11 @@ int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *con
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one trace must be checked");
         DG_REQUIRE(traces && reports, "null argument");
-        const dg_trace_t &t0 = traces[0];
-        std::vector<const uint8_t *> cols;
-        for (uint32_t i = 0; i < count; i++) {
-            const dg_trace_t &t = traces[i];
-            DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
-                       "all traces of a call must have the same width, length, context depth and loop depth");
-            DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
-            for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
-            cols.insert(cols.end(), t.columns, t.columns + t.width);
-        }
+        const std::vector<const uint8_t *> cols = trace_columns(traces, count, "call", false);
+        const dg_trace_t &t = traces[0];
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        check_traces(c, nullptr, cols.data(), count, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
+        check_traces(c, nullptr, cols.data(), count, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
                      program_hashes32, reports, step_masks, nullptr);
     });
 }

@@ -7,13 +7,10 @@
 // assertions (evaluator.rs:181-326) are compared on the host with the first and last rows, 2 w elements per trace.
 #include "prover.h"
 #include "air.h"
-#include "host_fs.h"
 
 namespace dg {
 
 namespace {
-
-int log2_exact(uint64_t v) { int l = 0; while ((1ULL << l) < v) l++; return l; }
 
 const char *const DECODER_NAMES[20] = {
     "op bit 0 binary", "op bit 1 binary", "op bit 2 binary", "op bit 3 binary", "op bit 4 binary", "op bit 5 binary", "op bit 6 binary",
@@ -33,26 +30,21 @@ int check_group_size(uint32_t w, uint64_t n, bool upload, bool own_masks, uint32
     DG_REQUIRE(!ctx().mem_limit || per <= avail, "a trace check of " + std::to_string(w) + " x " + std::to_string(n) + " needs " + std::to_string(per) +
                                                      " bytes of device memory beyond what the memory limit leaves");
     k = std::min<long long>(k, (long long)std::max<size_t>(1, avail / per));
-    if (const char *e = getenv("DG_BATCH_GROUP")) {
-        const long long cap = atoll(e);
-        DG_REQUIRE(cap >= 1, "DG_BATCH_GROUP must be a positive integer");
-        k = std::min(k, cap);
-    }
-    return (int)k;
+    return (int)batch_group_cap(k);
 }
 
 }  // namespace
 
 std::string constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t index) {
-    DG_REQUIRE(ctx_depth <= 16 && loop_depth <= 8 && stack_depth >= 1 && stack_depth <= 32, "register shape out of range");
-    const uint32_t cl = std::max<uint32_t>(ctx_depth, 1), ll = std::max<uint32_t>(loop_depth, 1);
-    DG_REQUIRE(index < 20 + cl + ll + 2 + stack_depth, "constraint index out of range");
+    DG_REQUIRE(TraceShape::in_range(ctx_depth, loop_depth, stack_depth), "register shape out of range");
+    const TraceShape shape(ctx_depth, loop_depth, stack_depth);
+    DG_REQUIRE(index < (uint32_t)shape.T, "constraint index out of range");
     if (index < 20) return DECODER_NAMES[index];
     index -= 20;
-    if (index < cl) return "ctx stack " + std::to_string(index);
-    index -= cl;
-    if (index < ll) return "loop stack " + std::to_string(index);
-    index -= ll;
+    if (index < (uint32_t)shape.cl) return "ctx stack " + std::to_string(index);
+    index -= shape.cl;
+    if (index < (uint32_t)shape.ll) return "loop stack " + std::to_string(index);
+    index -= shape.ll;
     if (index < 2) return "stack aux " + std::to_string(index);
     return "stack slot " + std::to_string(index - 2);
 }
@@ -66,13 +58,9 @@ void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols,
     DG_REQUIRE(count >= 1, "at least one trace must be checked");
     DG_REQUIRE(reports && (d_regs || host_cols), "null argument");
     DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    DG_REQUIRE(ctx_depth <= 16, "context depth cannot be greater than 16");
-    DG_REQUIRE(loop_depth <= 8, "loop depth cannot be greater than 8");
-    DG_REQUIRE(width < 128, "execution trace cannot have more than 128 registers");
-    DG_REQUIRE(width > 15 + ctx_depth + loop_depth, "user stack must consist of at least one register");
-    const int w = (int)width, stack_depth = w - 15 - (int)ctx_depth - (int)loop_depth;
-    DG_REQUIRE(stack_depth <= 32, "stack depth cannot be greater than 32");
-    DG_REQUIRE(log2_exact(n) <= 32, "execution trace too long");
+    const TraceShape shape = TraceShape::of_trace(width, ctx_depth, loop_depth);
+    const int w = shape.w, stack_depth = shape.stack_depth, T = shape.T, stk = shape.stack_reg;
+    DG_REQUIRE(ceil_log2(n) <= 32, "execution trace too long");
     for (uint32_t i = 0; i < count; i++) {
         const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
         DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
@@ -80,15 +68,7 @@ void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols,
     }
     DG_REQUIRE(c.world == 1 && ctx_device_count() == 1,
                "the trace check runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
-    const int cl = std::max<int>(ctx_depth, 1), ll = std::max<int>(loop_depth, 1);
-    const int T = 20 + cl + ll + 2 + stack_depth;
-    const int stk = 15 + (int)ctx_depth + (int)loop_depth;      // first user-stack register
-
-    if (!c.d_periodic.p) {
-        std::vector<fe> per = fs::periodic_tables();
-        c.d_periodic.alloc(per.size() * 16, true);
-        DG_CUDA(cudaMemcpyAsync(c.d_periodic.p, per.data(), per.size() * 16, cudaMemcpyHostToDevice, c.stream));
-    }
+    const fe *periodic = periodic_table(c);
     const int group = check_group_size(width, n, host_cols != nullptr, d_step_masks == nullptr, count);
     DevBuf d_masks, d_stats;
     std::vector<unsigned long long> stats;
@@ -106,14 +86,11 @@ void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols,
         else { d_masks.ensure((size_t)k * n * 12); masks = d_masks.as<unsigned>(); }
         d_stats.ensure((size_t)k * CHECK_STATS * 8);
 
-        AirParams P;
-        memset(&P, 0, sizeof P);
-        P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
-        P.cl = cl; P.ll = ll; P.sl = std::max(stack_depth, 8);
-        P.log_n = log2_exact(n); P.log_blowup = 3;
+        AirParams P = shape.air_params(n);
+        P.log_blowup = 3;
         P.ext = regs; P.col_stride = n; P.ext_stride = (size_t)w * n;
         P.c8_base = 0; P.num_c8 = 1;
-        P.periodic = c.d_periodic.as<fe>();
+        P.periodic = periodic;
         P.masks = masks;
         launch_constraint_check(c, P, k);
         launch_check_reduce(c, masks, n, T, k, d_stats.as<unsigned long long>());

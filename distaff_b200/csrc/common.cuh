@@ -179,6 +179,9 @@ fe host_root_of_unity(int log_order);            // w of order 2^log_order  (fie
 fe host_pow(fe b, unsigned long long e);
 fe host_inv(fe a);
 
+// the least l with 2^l >= v
+inline int ceil_log2(uint64_t v) { int l = 0; while ((1ULL << l) < v) l++; return l; }
+
 static const int MAX_LOG_L = 10;                 // largest in-shared-memory transform: 1024 points
 
 // device time between construction and stop() on a stream, in ms; does nothing when ms is null

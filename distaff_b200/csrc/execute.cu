@@ -2,8 +2,9 @@
 // and dg_execute_batch are the one-program case): validate each program's encoding, put every program into one set of tables and upload
 // them and the inputs once, run the shape pass for every execution, and write the successful executions in waves -- one write launch
 // (vm.cu) per wave for every shape in it -- into one slab per shape, which is copied to the caller's buffers (dg_trace_programs) or
-// proven in place (dg_execute_programs, through prove_batch_device).
+// proven in place (dg_execute_programs, through prove_traces).
 #include "vm.h"
+#include "air.h"
 #include "prover.h"
 #include <algorithm>
 #include <map>
@@ -275,7 +276,7 @@ struct Executions {
         memset(&v, 0, sizeof v);
         const VmResult &r = res[i];
         v.ctx_depth = r.ctx_cols - 1; v.loop_depth = r.loop_cols; v.stack_depth = r.max_depth;
-        v.width = 15 + v.ctx_depth + v.loop_depth + v.stack_depth;
+        v.width = TraceShape(v.ctx_depth, v.loop_depth, v.stack_depth).w;
         v.steps = r.steps;
         v.length = 16;
         while (v.length <= r.steps) v.length *= 2;
@@ -483,8 +484,8 @@ void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_ou
             dg_prove_stats_t gs;
             memset(&gs, 0, sizeof gs);
             uint32_t groups = 0;
-            prove_batch_device(c, s.regs, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth, in16.data(), n_in.data(),
-                               out16.data(), n_out.data(), opt, proofs.data(), st.data(), msg, &gs, &groups);
+            prove_traces(c, s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth, in16.data(), n_in.data(),
+                         out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &groups);
             for (uint32_t q = 0; q < k; q++) {
                 proofs_out[ok[q]] = proofs[q];
                 if (st[q] != DG_OK) X.fail(ok[q], st[q], msg[q]);

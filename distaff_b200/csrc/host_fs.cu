@@ -1,5 +1,6 @@
 // Host-side Fiat-Shamir glue (see host_fs.h for the reference lines each piece follows).
 #include "host_fs.h"
+#include "air.h"
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -102,20 +103,19 @@ void blake3_short(const uint8_t *data, size_t len, uint8_t out[32]) {
 // ---- coefficients ----------------------------------------------------------------------------------------------------------
 static const int DEG_STATIC[20] = {2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 8, 8, 6, 4, 6, 7, 6, 6, 4};
 
-ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32], int ctx_depth, int loop_depth, int stack_depth,
-                                                    const std::vector<fe> &inputs, const std::vector<fe> &outputs, fe op_count,
-                                                    const fe program_hash[2]) {
+ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32], const TraceShape &shape, const std::vector<fe> &inputs,
+                                                    const std::vector<fe> &outputs, fe op_count, const fe program_hash[2]) {
     const int NUM_BOUNDARY = 47, NUM_TRANSITION = 78;
     std::vector<fe> c = prng_vector(trace_root, 2 * (NUM_TRANSITION + 2 * NUM_BOUNDARY));
     const fe *bi = c.data(), *bf = c.data() + 2 * NUM_BOUNDARY, *tr = c.data() + 4 * NUM_BOUNDARY;
-    const int cl = std::max(ctx_depth, 1), ll = std::max(loop_depth, 1), sl = std::max(stack_depth, 8);
+    const int ctx_depth = shape.ctx_depth, loop_depth = shape.loop_depth, stack_depth = shape.stack_depth;
+    const int cl = shape.cl, ll = shape.ll, sl = shape.sl, T = shape.T;
 
     ConstraintCoefficients r;
     // ---- transition: compact the MAX-depth layout, then hand each constraint the pair of its flattened slot
     std::vector<fe> compact;
     auto take = [&](int src, int count) { for (int k = 0; k < count; k++) compact.push_back(tr[src + k]); };
     take(0, 40); take(40, 2 * cl); take(40 + 32, 2 * ll); take(40 + 32 + 16, 4); take(40 + 32 + 16 + 4, 2 * sl);
-    const int T = 20 + cl + ll + 2 + stack_depth;
     std::vector<int> degree(T);
     for (int j = 0; j < 20; j++) degree[j] = DEG_STATIC[j];
     for (int j = 20; j < 20 + cl + ll; j++) degree[j] = 4;
@@ -130,7 +130,7 @@ ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32]
     // ---- boundary: per-register coefficient vectors + constants
     const int io = (int)std::max(inputs.size(), outputs.size());
     const int stack_regs = std::min(stack_depth, io);
-    r.n_boundary_regs = 15 + ctx_depth + loop_depth + stack_regs;
+    r.n_boundary_regs = shape.stack_reg + stack_regs;
     const fe Z = fe_make(0, 0), ONEv = fe_make(1, 0);
     r.bAi.assign(r.n_boundary_regs, Z); r.bBi.assign(r.n_boundary_regs, Z);
     r.bAf.assign(r.n_boundary_regs, Z); r.bBf.assign(r.n_boundary_regs, Z);
@@ -152,7 +152,7 @@ ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32]
     for (int i = 0; i < ctx_depth; i++) set(15 + i, 30 + 2 * i, true, true, Z, Z);
     for (int i = 0; i < loop_depth; i++) set(15 + ctx_depth + i, 62 + 2 * i, true, true, Z, Z);
     for (int i = 0; i < io; i++) {
-        const int reg = i < stack_depth ? 15 + ctx_depth + loop_depth + i : -1;
+        const int reg = i < stack_depth ? shape.stack_reg + i : -1;
         set(reg, 78 + 2 * i, i < (int)inputs.size(), i < (int)outputs.size(), i < (int)inputs.size() ? inputs[i] : Z,
             i < (int)outputs.size() ? outputs[i] : Z);
     }

@@ -15,6 +15,7 @@
 #include "fp128.cuh"
 
 namespace dg {
+struct TraceShape;      // air.h
 namespace fs {
 
 // ---- StdRng ---------------------------------------------------------------------------------------------------------
@@ -54,8 +55,7 @@ struct ConstraintCoefficients {
     fe KiA, KiB, KfA, KfB;
     int n_boundary_regs;
 };
-ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32], int ctx_depth, int loop_depth, int stack_depth,
-                                                    const std::vector<fe> &inputs, const std::vector<fe> &outputs, fe op_count,
+ConstraintCoefficients draw_constraint_coefficients(const uint8_t trace_root[32], const TraceShape &shape, const std::vector<fe> &inputs, const std::vector<fe> &outputs, fe op_count,
                                                     const fe program_hash[2]);
 struct CompositionCoefficients {
     fe z;

@@ -100,8 +100,6 @@ void write_felt_vec(fs::ByteWriter &w, const std::vector<fe> &v) {
     for (auto &x : v) w.felt(x);
 }
 
-int ilog2(uint64_t v) { int l = 0; while ((1ULL << l) < v) l++; return l; }
-
 // Trace LDE of `cols` columns (polynomials `polys`, stride n) onto the cosets [c0, c0 + nc), written to ext (column stride N_loc).
 // Coset 0 is P(w_n^k), which is register row k itself (polys = iNTT(regs) exactly): when the range starts at coset 0 and the registers
 // are on the device (`regs`, stride n; null if not), slab 0 is copied from them and only the other cosets are transformed.
@@ -114,6 +112,10 @@ void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, 
     }
     if (nc > 1) lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
     DG_CUDA(cudaMemcpy2DAsync(ext, N_loc * sizeof(fe), regs, n * sizeof(fe), n * sizeof(fe), cols, cudaMemcpyDeviceToDevice, c.stream));
+}
+
+void require_extension_factor(uint64_t b) {
+    DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
 }
 
 struct FriLayerDev {
@@ -288,20 +290,14 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     DG_REQUIRE(K >= 1 && (int)ps.size() == K, "batch must hold at least one trace");
     DG_REQUIRE((uint64_t)K * width <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
     DG_REQUIRE(opt.hash_id == 0, "unsupported hash function (only blake3 is serialisable, options.rs:107)");
-    DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
+    require_extension_factor(b);
     DG_REQUIRE(opt.num_queries > 0 && opt.num_queries <= 128, "num_queries must be in 1..128");
     DG_REQUIRE(opt.grinding_factor <= 32, "grinding factor cannot be greater than 32");
     DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    DG_REQUIRE(ctx_depth <= 16, "context depth cannot be greater than 16");
-    DG_REQUIRE(loop_depth <= 8, "loop depth cannot be greater than 8");
-    DG_REQUIRE(width < 128, "execution trace cannot have more than 128 registers");
-    DG_REQUIRE(width > 15 + ctx_depth + loop_depth, "user stack must consist of at least one register");
-    for (auto &s : ps) DG_REQUIRE(s.inputs.size() <= 8 && s.outputs.size() <= 8, "cannot have more than 8 public inputs / outputs");
-    const int w = (int)width, log_n = ilog2(n), log_b = ilog2(b), log_N = log_n + log_b;
+    const TraceShape shape = TraceShape::of_trace(width, ctx_depth, loop_depth);
+    const int w = shape.w, log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
     DG_REQUIRE(log_N <= 30, "LDE domain too large");
     const uint64_t N = n * b, E = n * 8;
-    const int stack_depth = w - 15 - (int)ctx_depth - (int)loop_depth;
-    DG_REQUIRE(stack_depth <= 32, "stack depth cannot be greater than 32");
     auto any_live = [&] { for (auto &s : ps) if (s.live) return true; return false; };
 
     ArenaScope arena_scope;                   // all DevBufs below come from the per-proof arena (no driver allocation inside a proof)
@@ -319,8 +315,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     // ---- sharding: rank g owns the LDE cosets [c0, c0 + nc) of every column (world == 1: all of them) ------------------------------
     const int G = c.world, g = c.rank;
     DG_REQUIRE(G == 1 || K == 1, "a batch of proofs runs on one GPU (the context spans several)");
-    int log_g = 0;
-    while ((1 << log_g) < G) log_g++;
+    const int log_g = ceil_log2(G);
     DG_REQUIRE((b >> log_g) >= 4 && G <= 8, "extension factor too small for this many GPUs (need >= 4 cosets per rank)");
     const int log_nc = log_b - log_g;
     const uint64_t nc = 1ULL << log_nc, N_loc = n * nc;
@@ -464,28 +459,19 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
                                       cudaMemcpyDeviceToDevice, c.stream));
         d2h(c, last_rows.data(), d_last.p, (size_t)48 * K);
     }
-    DevBuf &d_periodic = c.d_periodic;
-    if (!d_periodic.p) {
-        std::vector<fe> per = fs::periodic_tables();
-        d_periodic.alloc(per.size() * 16, true);
-        h2d(c, d_periodic.p, per.data(), per.size() * 16);
-        DG_CUDA(cudaStreamSynchronize(c.stream));
-    }
     DevBuf d_coef, d_violation((size_t)4 * K);
     // per proof [coefA | coefB | bAi | bBi | bAf | bBf], coef_stride elements apart, then the boundary constants [K][KiA, KiB, KfA, KfB].
-    // The transition coefficients have the same count for every proof of a shape; the boundary vectors have one entry per register that
+    // The transition coefficients have the same count T for every proof of a shape; the boundary vectors have one entry per register that
     // carries a boundary constraint, which depends on the number of public inputs / outputs: they are padded with zero coefficients to
     // the largest count nbm (a zero coefficient adds nothing to the boundary numerators).
-    size_t coef_stride = 0, T = 0, nbm = 0;
+    const size_t T = shape.T;
+    size_t coef_stride = 0, nbm = 0;
     {
         for (int p = 0; p < K; p++) {
             ProofState &s = ps[p];
             s.op_count = last_rows[3 * p];
             const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
-            s.cc = fs::draw_constraint_coefficients(s.proof->trace_root, ctx_depth, loop_depth, stack_depth, s.inputs, s.outputs, s.op_count,
-                                                    program_hash);
-            DG_REQUIRE(s.cc.coefA.size() == ps[0].cc.coefA.size(), "transition constraint counts differ inside a batch");
-            T = s.cc.coefA.size();
+            s.cc = fs::draw_constraint_coefficients(s.proof->trace_root, shape, s.inputs, s.outputs, s.op_count, program_hash);
             nbm = std::max(nbm, s.cc.bAi.size());
         }
         DG_REQUIRE(nbm <= (size_t)w, "more boundary registers than registers");
@@ -513,22 +499,17 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         const uint64_t E_loc = n * num_c8;
         DevBuf evals_loc((size_t)K * E_loc * 16), gathered;
         if (G > 1) gathered.alloc(E * 16);
-        AirParams P;
-        memset(&P, 0, sizeof P);
-        P.w = w; P.ctx_depth = ctx_depth; P.loop_depth = loop_depth; P.stack_depth = stack_depth;
-        P.cl = std::max<int>(ctx_depth, 1); P.ll = std::max<int>(loop_depth, 1); P.sl = std::max(stack_depth, 8);
+        AirParams P = shape.air_params(n);
         // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
         // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
-        P.log_n = log_n; P.log_blowup = full ? log_b : 3;
+        P.log_blowup = full ? log_b : 3;
         P.ext = slab; P.col_stride = slab_col;
         P.c8_base = g * num_c8; P.num_c8 = num_c8;
         P.t_ev = evals_loc.as<fe>();
-        P.periodic = d_periodic.as<fe>();
+        P.periodic = periodic_table(c);
         const fe *base = d_coef.as<fe>();
         P.coefA = base; P.coefB = base + T;
         P.twN = c.twiddle(full ? log_N : log_n + 3, false);
-        static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
-        for (int gi = 0; gi < 6; gi++) P.inc[gi] = (8 * n - 1) - (n - 1) * GROUP_DEG[gi];
         P.violation = d_violation.as<unsigned>();
         P.ext_stride = (size_t)w * slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
     sub.mark("3.setup");
@@ -941,7 +922,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         Proof *proof = s.proof.get();
         const int nq = (int)s.positions.size();
         out.raw(proof->trace_root, 32);
-        out.u8(O.tplan.depth); out.u8((uint8_t)ctx_depth); out.u8((uint8_t)loop_depth); out.u8((uint8_t)stack_depth);
+        out.u8(O.tplan.depth); out.u8((uint8_t)ctx_depth); out.u8((uint8_t)loop_depth); out.u8((uint8_t)shape.stack_depth);
         out.u32((uint32_t)s.op_count.lo);                                             // op_count as u32 (proof.rs:62)
         write_digest_vv(out, digests_at(O.t_off));
         out.u64(nq);
@@ -1047,13 +1028,13 @@ size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b, uint32_t chunk) {
 // dimension, which holds at most 65535 blocks.
 int max_group_for_grid(uint32_t w) { return (int)(65535 / std::max<uint32_t>(w, 1)); }
 
-int batch_group_cap(long long k) {
+long long batch_group_cap(long long k) {
     if (const char *e = getenv("DG_BATCH_GROUP")) {
         const long long cap = atoll(e);
         DG_REQUIRE(cap >= 1, "DG_BATCH_GROUP must be a positive integer");
         k = std::min(k, cap);
     }
-    return (int)k;
+    return k;
 }
 
 // Transform scratch and tables a prove call adds outside the arena (persistent, from the pool): the multi-pass LDE of a coset chunk
@@ -1064,18 +1045,15 @@ static size_t prove_scratch(Context &c, uint32_t w, uint64_t n, uint32_t b, uint
     const size_t ntt = std::max(std::min(four, (size_t)(16 * n * chunk * w * k)), std::min(one, (size_t)(16 * n * b * k)));
     size_t add = ntt > c.ntt_tmp.bytes ? ntt - c.ntt_tmp.bytes : 0;
     const size_t table = (size_t)16 * n * b;
-    int log_n = 0, log_b = 0;
-    while ((1ULL << log_n) < n) log_n++;
-    while ((1u << log_b) < b) log_b++;
     bool have = false;
-    for (auto &t : c.lde_twiddles) have |= (t.first >> 8) == (((long long)log_n << 8) | log_b);
+    for (auto &t : c.lde_twiddles) have |= (t.first >> 8) == (((long long)ceil_log2(n) << 8) | ceil_log2(b));
     if (table <= one && !have) add += table;
     return add;
 }
 
 ProvePlan plan_prove(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count) {
     DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
+    require_extension_factor(b);
     DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0 && n <= (1ULL << 30), "execution trace length must be a power of 2 and at least 16");
     DG_REQUIRE(w >= 1 && w < 128, "execution trace cannot have more than 128 registers");
     const long long k_max = std::min<long long>(count, max_group_for_grid(w));
@@ -1097,7 +1075,7 @@ ProvePlan plan_prove(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t co
         P.chunk = ch;
         P.per_proof = proof_footprint(w, n, b, ch);
         P.fixed = memory_held_outside_arena(c) + prove_scratch(c, w, n, b, ch, g);
-        P.group = batch_group_cap(g);
+        P.group = (int)batch_group_cap(g);
         P.available = avail;
         return P;
     }
@@ -1114,24 +1092,6 @@ void prepare_arena(Context &c, const ProvePlan &P) {
     if (c.mem_limit && c.arena.base && (size_t)P.group * P.per_proof > c.arena.cap) arena_release(c);
 }
 
-// the single-trace entry points: a batch of one whose failure is the call's error
-Proof *prove_one(Context &c, fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                 const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
-                 dg_prove_stats_t *stats) {
-    std::vector<ProofState> ps = make_states(1, &inputs16, &n_inputs, &outputs16, &n_outputs);
-    unsigned chunk = 0;
-    if (c.world == 1) {
-        DG_REQUIRE(opt.extension_factor >= 16 && opt.extension_factor <= 256 && (opt.extension_factor & (opt.extension_factor - 1)) == 0,
-                   "extension_factor must be a power of 2 between 16 and 256");
-        const ProvePlan P = plan_prove(c, width, length, opt.extension_factor, 1);
-        prepare_arena(c, P);
-        chunk = P.chunk;
-    }
-    prove_core(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, ps, opt, stats, chunk);
-    if (ps[0].status != DG_OK) throw Error(ps[0].status, ps[0].message);
-    return ps[0].proof.release();
-}
-
 void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
     for (int i = 0; i < 9; i++) sum->stage_ms[i] += s.stage_ms[i];
     sum->h2d_ms += s.h2d_ms;
@@ -1139,16 +1099,35 @@ void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
     sum->kernel_launches += s.kernel_launches;
 }
 
-// runs the batch group by group; run_group(first, k, states, stats, chunk) proves traces [first, first + k) with the plan's coset chunk
-template <typename F>
-void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_options_t &opt, std::vector<ProofState> &all, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, F &&run_group) {
-    DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
-    DG_REQUIRE(opt.extension_factor >= 16 && opt.extension_factor <= 256 && (opt.extension_factor & (opt.extension_factor - 1)) == 0,
-               "extension_factor must be a power of 2 between 16 and 256");
-    const ProvePlan plan = plan_prove(c, w, n, opt.extension_factor, count);
-    const int group = plan.group;
+}  // namespace
+
+std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first) {
+    const dg_trace_t &t0 = traces[0];
+    std::vector<const uint8_t *> cols;
+    for (uint32_t i = 0; i < count; i++) {
+        const dg_trace_t &t = traces[i];
+        DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
+                   std::string("all traces of a ") + call + " must have the same width, length, context depth and loop depth");
+        DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
+        if (length_first) DG_REQUIRE(t.length >= 16 && (t.length & (t.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
+        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
+        cols.insert(cols.end(), t.columns, t.columns + t.width);
+    }
+    return cols;
+}
+
+void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
+    if (host_cols) DG_REQUIRE(length >= 16 && (length & (length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
+    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
+    if (batch)
+        DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
+    ProvePlan plan;                                // several GPUs (one trace): one group, and prove_core shards the full layout
+    if (c.world == 1) plan = plan_prove(c, width, length, opt.extension_factor, count);
     if (stats) memset(stats, 0, sizeof *stats);
+    if (groups) *groups = 0;
     for (uint32_t i = 0; i < count; i++) { proofs_out[i] = nullptr; status[i] = DG_OK; }
     messages.assign(count, std::string());
     // a group that fails as a whole fails the call: the proofs of the earlier groups are freed, nothing is returned
@@ -1156,15 +1135,22 @@ void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_o
         Proof **out; uint32_t count; bool done = false;
         ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
     } release{proofs_out, count};
-    for (uint32_t first = 0; first < count; first += group) {
-        const int k = (int)std::min<uint32_t>(group, count - first);
+    for (uint32_t first = 0; first < count; first += plan.group) {
+        const int k = (int)std::min<uint32_t>(plan.group, count - first);
         std::vector<ProofState> ps;
         for (int i = 0; i < k; i++) ps.push_back(std::move(all[first + i]));
         dg_prove_stats_t st;
         memset(&st, 0, sizeof st);
         prepare_arena(c, plan);
-        run_group(first, k, ps, &st, plan.chunk);
+        fe *regs = const_cast<fe *>(d_regs) + (size_t)first * width * length;
+        if (host_cols) {
+            c.upload_buf.ensure((size_t)length * 16 * width * k, true);
+            regs = c.upload_buf.as<fe>();
+        }
+        prove_core(c, regs, host_cols ? host_cols + (size_t)first * width : nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, &st,
+                   plan.chunk);
         if (stats) add_stats(stats, st);
+        if (groups) ++*groups;
         for (int i = 0; i < k; i++) {
             status[first + i] = ps[i].status;
             messages[first + i] = ps[i].message;
@@ -1172,59 +1158,6 @@ void prove_groups(Context &c, uint32_t count, uint32_t w, uint64_t n, const dg_o
         }
     }
     release.done = true;
-}
-
-}  // namespace
-
-Proof *prove_device(Context &c, const fe *d_regs, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                    const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
-                    dg_prove_stats_t *stats, float) {
-    return prove_one(c, const_cast<fe *>(d_regs), nullptr, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs, opt, stats);
-}
-
-Proof *prove_host(Context &c, const dg_trace_t &trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16,
-                  uint32_t n_outputs, const dg_options_t &opt, dg_prove_stats_t *stats) {
-    DG_REQUIRE(trace.columns && trace.width >= 16 && trace.width < 128, "invalid trace");
-    DG_REQUIRE(trace.length >= 16 && (trace.length & (trace.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    for (uint32_t j = 0; j < trace.width; j++) DG_REQUIRE(trace.columns[j] != nullptr, "null register column");
-    c.upload_buf.ensure((size_t)trace.length * 16 * trace.width, true);
-    return prove_one(c, c.upload_buf.as<fe>(), trace.columns, trace.width, trace.length, trace.ctx_depth, trace.loop_depth, inputs16, n_inputs,
-                     outputs16, n_outputs, opt, stats);
-}
-
-void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                      const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, Proof **proofs_out, int *status,
-                      std::vector<std::string> &messages, dg_prove_stats_t *stats) {
-    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    const dg_trace_t &t0 = traces[0];
-    for (uint32_t i = 0; i < count; i++) {
-        const dg_trace_t &t = traces[i];
-        DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
-                   "all traces of a batch must have the same width, length, context depth and loop depth");
-        DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
-        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
-    }
-    DG_REQUIRE(t0.length >= 16 && (t0.length & (t0.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
-    prove_groups(c, count, t0.width, t0.length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
-        std::vector<const uint8_t *> cols;
-        for (int i = 0; i < k; i++) cols.insert(cols.end(), traces[first + i].columns, traces[first + i].columns + t0.width);
-        c.upload_buf.ensure((size_t)t0.length * 16 * t0.width * k, true);
-        prove_core(c, c.upload_buf.as<fe>(), cols.data(), k, t0.width, t0.length, t0.ctx_depth, t0.loop_depth, ps, opt, st, chunk);
-    });
-}
-
-void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                        const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
-                        uint32_t *groups) {
-    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
-    if (groups) *groups = 0;
-    prove_groups(c, count, width, length, opt, all, proofs_out, status, messages, stats, [&](uint32_t first, int k, std::vector<ProofState> &ps, dg_prove_stats_t *st, unsigned chunk) {
-        prove_core(c, const_cast<fe *>(d_regs) + (size_t)first * width * length, nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, st, chunk);
-        if (groups) ++*groups;
-    });
 }
 
 }  // namespace dg

@@ -12,21 +12,18 @@ struct Proof {
     unsigned long long pow_nonce = 0;
 };
 
-Proof *prove_host(Context &c, const dg_trace_t &trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16,
-                  uint32_t n_outputs, const dg_options_t &opt, dg_prove_stats_t *stats);
-Proof *prove_device(Context &c, const fe *d_registers, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                    const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs, const dg_options_t &opt,
-                    dg_prove_stats_t *stats, float h2d_ms);
-// batched proving (dg_prove_batch / dg_prove_batch_device): proofs_out[i] / status[i] / messages[i] (why trace i failed, else empty) per
-// trace, one GPU only; when the call throws, no proof is left in proofs_out
-void prove_batch_host(Context &c, const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                      const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, Proof **proofs_out, int *status,
-                      std::vector<std::string> &messages, dg_prove_stats_t *stats);
-// groups (may be null) receives the number of prove groups the batch ran in
-void prove_batch_device(Context &c, const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                        const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                        const dg_options_t &opt, Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats,
-                        uint32_t *groups = nullptr);
+// Proves `count` traces of one shape: registers on the device ([count][width][length] at d_regs), or host columns (host_cols: count * width
+// pointers) uploaded group by group into c.upload_buf.  On one GPU the call is planned (plan_prove) and runs in groups; on several
+// (dg_prove on every rank) it proves one trace, sharded.  batch: a batched call, which runs on one GPU only.  proofs_out[i] / status[i] /
+// messages[i] (why trace i failed, else empty) per trace; when the call throws, no proof is left in proofs_out.  groups (may be null)
+// receives the number of groups the traces ran in.
+void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
+// The register columns of `count` host traces, trace after trace.  Every trace must have the shape of the first ("all traces of a
+// <call> must ..."), 16..127 registers and no null column; length_first also checks each length before its columns (dg_prove).
+std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first);
 
 // dg_trace_programs / dg_execute_programs (execute.cu; dg_trace_batch / dg_execute_batch with one program): execution i runs
 // programs[program_of[i]] on inputs[i]; status / messages per execution.  check_execution_call validates the arguments and every
@@ -46,7 +43,7 @@ void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *inf
 void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP
-int batch_group_cap(long long k);
+long long batch_group_cap(long long k);
 
 // What a prove call of one shape does on one GPU (dg_plan_prove): the full layout keeps the whole trace extension; the evaluation-coset
 // layout extends and hashes `chunk` cosets at a time, keeps the 8 cosets the constraint evaluation reads and computes the other opened

@@ -418,8 +418,9 @@ void prepare(Item &it) {
     const uint64_t b = 1ULL << P.log_ext, N = 1ULL << P.domain_depth, n = N >> P.log_ext;
     it.n = n;
     it.log_N = P.domain_depth;
-    const int w = it.w = 15 + P.ctx_depth + P.loop_depth + P.stack_depth;
-    DG_REQUIRE(P.ctx_depth <= 16 && P.loop_depth <= 8 && P.stack_depth >= 1 && P.stack_depth <= 32 && w < 128, "invalid register counts in the proof");
+    DG_REQUIRE(TraceShape::in_range(P.ctx_depth, P.loop_depth, P.stack_depth), "invalid register counts in the proof");
+    const TraceShape shape(P.ctx_depth, P.loop_depth, P.stack_depth);
+    const int w = it.w = shape.w;
 
     // ---- 1: PoW, query positions (verifier.rs:19-31)
     std::vector<uint8_t> fri_roots;
@@ -484,11 +485,9 @@ void prepare(Item &it) {
     it.z = fs::prng_vector(P.constraint_root.data(), 1)[0];
     fe program_hash_fe[2];
     memcpy(program_hash_fe, it.in.program_hash, 32);
-    it.cc = fs::draw_constraint_coefficients(P.trace_root.data(), P.ctx_depth, P.loop_depth, P.stack_depth, it.inputs, it.outputs,
-                                             fe_make(P.op_count, 0), program_hash_fe);
-    static const int GROUP_DEG[6] = {2, 3, 4, 6, 7, 8};
+    it.cc = fs::draw_constraint_coefficients(P.trace_root.data(), shape, it.inputs, it.outputs, fe_make(P.op_count, 0), program_hash_fe);
     it.per_xpow = fs::periodic_at(fe_pow_u64(it.z, n / 16));
-    for (int gi = 0; gi < 6; gi++) it.per_xpow.push_back(fe_pow_u64(it.z, (8 * n - 1) - (n - 1) * GROUP_DEG[gi]));
+    for (int g = 0; g < 6; g++) it.per_xpow.push_back(fe_pow_u64(it.z, group_increment(g, n)));
 
     // ---- 5: DEEP composition coefficients and the constraint evaluation opened at each trace position (verifier.rs:54-69)
     it.dc = fs::draw_composition_coefficients(P.constraint_root.data(), w);
@@ -596,6 +595,7 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     // register shapes (ctx, loop, stack depth) and widths, in order of first appearance
     std::vector<std::array<int, 3>> shapes;
     std::vector<int> shape_of(K), widths;
+    auto shape_at = [&](size_t s) { return TraceShape(shapes[s][0], shapes[s][1], shapes[s][2]); };
     for (int i = 0; i < K; i++) {
         const std::array<int, 3> s{g[i]->P.ctx_depth, g[i]->P.loop_depth, g[i]->P.stack_depth};
         shape_of[i] = (int)(std::find(shapes.begin(), shapes.end(), s) - shapes.begin());
@@ -719,7 +719,7 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     const size_t down_bytes = (size_t)n_trees * 32 + (size_t)Q * 16 + (size_t)F * 16;
     size_t slab_elems = 0;
     std::vector<size_t> slab0(shapes.size()), tev0(shapes.size());
-    for (size_t s = 0; s < shapes.size(); s++) { slab0[s] = slab_elems; slab_elems += (size_t)shape_count[s] * 128 * (15 + shapes[s][0] + shapes[s][1] + shapes[s][2]); }
+    for (size_t s = 0; s < shapes.size(); s++) { slab0[s] = slab_elems; slab_elems += (size_t)shape_count[s] * 128 * shape_at(s).w; }
     for (size_t s = 0, e = 0; s < shapes.size(); s++) { tev0[s] = e; e += (size_t)shape_count[s] * 128; }
     const size_t work_off = aligned(up_bytes + down_bytes);
     const size_t slab_off = work_off, tev_off = aligned(slab_off + slab_elems * 16), cz_off = aligned(tev_off + (size_t)K * 128 * 16);
@@ -790,14 +790,12 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     deep_rows_to_slab_kernel<<<K, 128, 0, c.stream>>>(atz_dev); c.launches++;
     DG_CUDA(cudaGetLastError());
     for (size_t s = 0; s < shapes.size(); s++) {
-        const int ctx_depth = shapes[s][0], loop_depth = shapes[s][1], stack_depth = shapes[s][2], w = 15 + ctx_depth + loop_depth + stack_depth;
-        const int i0 = (int)(std::find(shape_of.begin(), shape_of.end(), (int)s) - shape_of.begin());
-        const size_t T = g[i0]->cc.coefA.size();
-        AirParams A;
-        memset(&A, 0, sizeof A);
-        A.w = w; A.ctx_depth = ctx_depth; A.loop_depth = loop_depth; A.stack_depth = stack_depth;
-        A.cl = std::max(ctx_depth, 1); A.ll = std::max(loop_depth, 1); A.sl = std::max(stack_depth, 8);
-        A.log_n = 7; A.log_blowup = 3;
+        const TraceShape shape = shape_at(s);
+        const int w = shape.w;
+        const size_t T = shape.T;
+        // the inc[] of 128 steps are not read: the powers of z come from the host (xpow_override)
+        AirParams A = shape.air_params(128);
+        A.log_blowup = 3;
         A.ext = slab + slab0[s]; A.col_stride = 128; A.ext_stride = 128ULL * w;
         A.c8_base = 0; A.num_c8 = 1;
         A.t_ev = tev + tev0[s]; A.t_ev_stride = 128;
@@ -805,7 +803,6 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
         A.periodic = px;                                            // unused in verify mode (per_override is set)
         A.coefA = coef; A.coefB = coef + T; A.coef_stride = 2 * T;
         A.twN = c.twiddle(10, false);
-        A.violation = nullptr;
         A.verify_mode = 1;
         A.per_override = px; A.xpow_override = px + 23; A.override_stride = 29;
         launch_constraint_eval(c, A, shape_count[s]);
@@ -851,12 +848,7 @@ const size_t GROUP_BYTES = (size_t)512 << 20;
 void verify_proofs(Context &c, const std::vector<VerifyRequest> &req, std::vector<int> &status, std::vector<std::string> &messages,
                    dg_verify_stats_t *stats) {
     const unsigned long long launches0 = c.launches;
-    size_t cap = (size_t)-1;
-    if (const char *e = getenv("DG_BATCH_GROUP")) {
-        const long long v = atoll(e);
-        DG_REQUIRE(v >= 1, "DG_BATCH_GROUP must be a positive integer");
-        cap = (size_t)v;
-    }
+    const size_t cap = (size_t)batch_group_cap((long long)req.size());
     std::vector<Item> items(req.size());
     // ---- prepare, proof by proof in input order (the Fiat-Shamir callbacks see the proofs one after the other)
     for (size_t i = 0; i < req.size(); i++) {
