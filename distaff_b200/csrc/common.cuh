@@ -1,6 +1,7 @@
 // Shared host-side plumbing for the CUDA prover: error handling, device buffers, the per-process context.
 #pragma once
 #include <cuda_runtime.h>
+#include <array>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -13,6 +14,8 @@
 #include "fp128.cuh"
 
 namespace dg {
+
+typedef std::array<uint8_t, 32> Digest;
 
 struct Error : public std::runtime_error {
     int code;

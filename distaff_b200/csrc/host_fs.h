@@ -6,9 +6,8 @@
 //   MerkleTree::prove_batch index planning                       /root/reference/src/crypto/merkle.rs:64-124
 //   fri::utils::get_augmented_positions                          /root/reference/src/stark/fri/utils.rs:4-14
 //   periodic constant tables (extend_constants)                  /root/reference/src/stark/constraints/utils.rs:87-113
-//   bincode encoding of StarkProof                               /root/reference/src/stark/proof.rs:10-37
-// The rand 0.7.3 / bincode 1.3.1 crates are not vendored with the reference; their semantics are restated from the
-// crates' documented algorithms (see DESIGN.md, "unpinned third-party semantics").
+// The rand 0.7.3 crate is not vendored with the reference; its semantics are restated from the crate's documented algorithms
+// (see DESIGN.md, "unpinned third-party semantics").
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -80,16 +79,6 @@ struct BatchPlan {
     uint8_t depth;
 };
 BatchPlan plan_batch_proof(const std::vector<uint64_t> &indexes, uint64_t n_leaves);
-
-// ---- bincode ------------------------------------------------------------------------------------------------------------
-struct ByteWriter {
-    std::vector<uint8_t> b;
-    void u8(uint8_t v) { b.push_back(v); }
-    void u32(uint32_t v) { for (int i = 0; i < 4; i++) b.push_back((uint8_t)(v >> (8 * i))); }
-    void u64(uint64_t v) { for (int i = 0; i < 8; i++) b.push_back((uint8_t)(v >> (8 * i))); }
-    void felt(fe v) { u64(v.lo); u64(v.hi); }
-    void raw(const uint8_t *p, size_t n) { b.insert(b.end(), p, p + n); }
-};
 
 }  // namespace fs
 }  // namespace dg

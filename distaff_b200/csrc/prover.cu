@@ -86,20 +86,6 @@ void debug_dump_host(const char *name, const void *host, size_t bytes) {
     fclose(f);
 }
 
-
-void write_digest_vec(fs::ByteWriter &w, const std::vector<Digest> &v) {
-    w.u64(v.size());
-    for (auto &d : v) w.raw(d.data(), 32);
-}
-void write_digest_vv(fs::ByteWriter &w, const std::vector<std::vector<Digest>> &v) {
-    w.u64(v.size());
-    for (auto &x : v) write_digest_vec(w, x);
-}
-void write_felt_vec(fs::ByteWriter &w, const std::vector<fe> &v) {
-    w.u64(v.size());
-    for (auto &x : v) w.felt(x);
-}
-
 // Trace LDE of `cols` columns (polynomials `polys`, stride n) onto the cosets [c0, c0 + nc), written to ext (column stride N_loc).
 // Coset 0 is P(w_n^k), which is register row k itself (polys = iNTT(regs) exactly): when the range starts at coset 0 and the registers
 // are on the device (`regs`, stride n; null if not), slab 0 is copied from them and only the other cosets are transformed.
@@ -125,7 +111,6 @@ struct FriLayerDev {
     Layout layout;                    // layout of the (whole) layer (domain size 2^layout.log_d)
     bool sharded = false;             // multi-GPU: rows hashed / folded per coset range, tree = ShardedTree over [k'][c - c0] items
     ShardedTree tree;
-    Digest root;
 };
 
 }  // namespace
@@ -238,11 +223,10 @@ struct ProofState {
     int status = DG_OK;
     std::string message;
     std::unique_ptr<Proof> proof{new Proof()};
+    StarkProof stark;                     // filled by the stages that produce each field, written out in stage 9
     std::vector<fe> inputs, outputs;
-    fe op_count;
     fs::ConstraintCoefficients cc;
     fs::CompositionCoefficients dc;
-    std::vector<fe> state1, state2;
     ShardedTree t_tree, c_tree;
     std::vector<FriLayerDev> layers;
     std::vector<uint64_t> positions;
@@ -265,7 +249,7 @@ std::vector<Digest> fetch_roots(Context &c, const std::vector<const void *> &roo
 }
 
 // everything a proof opens, as offsets into the batch's FetchBatch (stage 9)
-struct LayerOpen { std::vector<uint64_t> pos; std::vector<size_t> val_off; Offsets node_off; uint8_t depth; };
+struct LayerOpen { std::vector<size_t> val_off; Offsets node_off; uint8_t depth; };
 struct OpenPlan {
     std::vector<size_t> row_off;
     fs::BatchPlan tplan, cplan;
@@ -298,6 +282,11 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     const int w = shape.w, log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
     DG_REQUIRE(log_N <= 30, "LDE domain too large");
     const uint64_t N = n * b, E = n * 8;
+    for (auto &s : ps) {                      // what the call fixes in every proof: the register shape and the options (blake3)
+        TraceInfo &t = s.stark.trace_info;
+        t.ctx_depth = (uint8_t)ctx_depth; t.loop_depth = (uint8_t)loop_depth; t.stack_depth = (uint8_t)shape.stack_depth;
+        s.stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opt.num_queries, (uint8_t)opt.grinding_factor, 0};
+    }
     auto any_live = [&] { for (auto &s : ps) if (s.live) return true; return false; };
 
     ArenaScope arena_scope;                   // all DevBufs below come from the per-proof arena (no driver allocation inside a proof)
@@ -442,7 +431,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             roots.push_back(ps[p].t_tree.root_dev());
         }
         std::vector<Digest> r = fetch_roots(c, roots);
-        for (int p = 0; p < K; p++) memcpy(ps[p].proof->trace_root, r[p].data(), 32);
+        for (int p = 0; p < K; p++) ps[p].stark.trace_root = r[p];
     }
 
     // ---- 3: evaluate constraints --------------------------------------------------------------------------------------------------------
@@ -469,9 +458,9 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         for (int p = 0; p < K; p++) {
             ProofState &s = ps[p];
-            s.op_count = last_rows[3 * p];
+            s.stark.trace_info.op_count = (uint32_t)last_rows[3 * p].lo;       // op_count as u32 (proof.rs:62)
             const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
-            s.cc = fs::draw_constraint_coefficients(s.proof->trace_root, shape, s.inputs, s.outputs, s.op_count, program_hash);
+            s.cc = fs::draw_constraint_coefficients(s.stark.trace_root.data(), shape, s.inputs, s.outputs, last_rows[3 * p], program_hash);
             nbm = std::max(nbm, s.cc.bAi.size());
         }
         DG_REQUIRE(nbm <= (size_t)w, "more boundary registers than registers");
@@ -587,7 +576,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             who.push_back(p);
         }
         std::vector<Digest> r = fetch_roots(c, roots);
-        for (size_t i = 0; i < who.size(); i++) memcpy(ps[who[i]].proof->constraint_root, r[i].data(), 32);
+        for (size_t i = 0; i < who.size(); i++) ps[who[i]].stark.constraint_root = r[i];
     }
 
     // ---- 6: DEEP composition polynomial ---------------------------------------------------------------------------------------------------------
@@ -607,7 +596,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         for (int p = 0; p < K; p++) {
             ProofState &s = ps[p];
             if (!s.live) continue;
-            s.dc = fs::draw_composition_coefficients(s.proof->constraint_root, w);
+            s.dc = fs::draw_composition_coefficients(s.stark.constraint_root.data(), w);
             const fe z = s.dc.z, zg = fe_mul(z, root_n);
             const fe bases[4] = {z, host_inv(z), zg, host_inv(zg)};
             for (int t = 0; t < 4; t++) {
@@ -643,12 +632,13 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
                     deep[2 * (col_start(r) + o)] = slots[2 * (r * cpr + o)];
                     deep[2 * (col_start(r) + o) + 1] = slots[2 * (r * cpr + o) + 1];
                 }
-            s.state1.resize(w); s.state2.resize(w);
+            std::vector<fe> &z1 = s.stark.trace_at_z1, &z2 = s.stark.trace_at_z2;
+            z1.resize(w); z2.resize(w);
             fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
             for (int i = 0; i < w; i++) {
-                s.state1[i] = deep[2 * i]; s.state2[i] = deep[2 * i + 1];
-                sub1 = fe_add(sub1, fe_mul(s.state1[i], s.dc.trace1[i]));
-                sub2 = fe_add(sub2, fe_mul(s.state2[i], s.dc.trace2[i]));
+                z1[i] = deep[2 * i]; z2[i] = deep[2 * i + 1];
+                sub1 = fe_add(sub1, fe_mul(z1[i], s.dc.trace1[i]));
+                sub2 = fe_add(sub2, fe_mul(z2[i], s.dc.trace2[i]));
             }
             subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[(size_t)K * 2 * wp + 2 * p];
             std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + w, ccs + (size_t)p * 2 * w);
@@ -766,9 +756,15 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         }
         std::vector<uint8_t> roots(32 * n_layers * K);
         d2h(c, roots.data(), d_roots.p, roots.size());
-        for (int p = 0; p < K; p++)
-            if (ps[p].live)
-                for (size_t i = 0; i < n_layers; i++) memcpy(ps[p].layers[i].root.data(), roots.data() + 32 * (i * K + p), 32);
+        // the last layer is the remainder: its root is the FRI proof's rem_root
+        for (int p = 0; p < K; p++) {
+            if (!ps[p].live) continue;
+            FriProof &f = ps[p].stark.degree_proof;
+            auto root = [&](size_t i) { return roots.data() + 32 * (i * K + p); };
+            f.layers.resize(n_layers - 1);
+            for (size_t i = 0; i + 1 < n_layers; i++) memcpy(f.layers[i].root.data(), root(i), 32);
+            memcpy(f.rem_root.data(), root(n_layers - 1), 32);
+        }
     }
 
     // ---- 8: query positions ------------------------------------------------------------------------------------------------------------------------
@@ -779,8 +775,10 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         std::vector<int> who;
         for (int p = 0; p < K; p++) {
             if (!ps[p].live) continue;
+            const FriProof &f = ps[p].stark.degree_proof;
             std::vector<uint8_t> roots;
-            for (auto &L : ps[p].layers) roots.insert(roots.end(), L.root.begin(), L.root.end());
+            for (auto &l : f.layers) roots.insert(roots.end(), l.root.begin(), l.root.end());
+            roots.insert(roots.end(), f.rem_root.begin(), f.rem_root.end());
             if (K == 1) debug_dump_host("fri_roots", roots.data(), roots.size());
             seeds.emplace_back();
             fs::blake3_short(roots.data(), roots.size(), seeds.back().data());
@@ -789,8 +787,8 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, opt.grinding_factor);
         for (size_t i = 0; i < who.size(); i++) {
             ProofState &s = ps[who[i]];
-            s.proof->pow_nonce = nonces[i];
-            pow_hash(seeds[i].data(), s.proof->pow_nonce, s.proof->pow_seed);
+            s.stark.pow_nonce = nonces[i];
+            pow_hash(seeds[i].data(), s.stark.pow_nonce, s.proof->pow_seed);
             try {
                 s.positions = fs::query_positions(s.proof->pow_seed, N, b, opt.num_queries);
             } catch (const std::exception &e) { s.fail(DG_ERR_EXHAUSTED, e.what()); continue; }
@@ -802,7 +800,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     // ---- 9: build proof objects --------------------------------------------------------------------------------------------------------------------------
     clk.mark(8);
     sub.mark("8.pow");
-    // Plan every opening of every proof on the host, fetch all opened values / digests in one batched pass (FetchBatch), then serialise.
+    // Plan every opening of every proof on the host, fetch all opened values / digests in one batched pass (FetchBatch), then write each proof.
     FetchBatch fb(c);
     // registers the nodes of a batch-proof plan; leaf_ref / node_ref map leaf indices / heap indices to fetch references
     auto plan_offsets = [&](const fs::BatchPlan &plan, auto leaf_ref, auto node_ref) {
@@ -891,7 +889,6 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             LayerOpen &lo = O.fri_open[d];
             const uint64_t D = 1ULL << L.layout.log_d, R = D / 4;
             fpos = fs::augmented_positions(fpos, D);
-            lo.pos = fpos;
             fs::BatchPlan plan = fs::plan_batch_proof(fpos, R);
             lo.depth = plan.depth;
             for (uint64_t p : fpos)
@@ -916,44 +913,30 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         }
         return O;
     };
-    // serialise (proof.rs:10-37; bincode: u64 length prefixes, arrays raw, little endian)
-    auto serialise = [&](ProofState &s, const OpenPlan &O) {
-        fs::ByteWriter out;
-        Proof *proof = s.proof.get();
-        const int nq = (int)s.positions.size();
-        out.raw(proof->trace_root, 32);
-        out.u8(O.tplan.depth); out.u8((uint8_t)ctx_depth); out.u8((uint8_t)loop_depth); out.u8((uint8_t)shape.stack_depth);
-        out.u32((uint32_t)s.op_count.lo);                                             // op_count as u32 (proof.rs:62)
-        write_digest_vv(out, digests_at(O.t_off));
-        out.u64(nq);
-        for (int q = 0; q < nq; q++) {
-            out.u64(w);
-            for (int j = 0; j < w; j++) out.felt(fb.value(O.row_off[q] + j));
-        }
-        out.raw(proof->constraint_root, 32);
-        out.u64(O.cval_off.size());
-        for (size_t off : O.cval_off) { Digest dgt = fb.digest(off); out.raw(dgt.data(), 32); }
-        write_digest_vv(out, digests_at(O.c_off));
-        out.u8(O.cplan.depth);
-        write_felt_vec(out, s.state1);
-        write_felt_vec(out, s.state2);
-
-        out.u64(s.layers.size() - 1);
-        for (size_t d = 0; d + 1 < s.layers.size(); d++) {
+    // the opened values and digests into the proof, which is then written out
+    auto fill_openings = [&](ProofState &s, const OpenPlan &O) {
+        StarkProof &P = s.stark;
+        P.trace_info.domain_depth = O.tplan.depth;
+        P.trace_nodes = digests_at(O.t_off);
+        P.trace_evaluations.assign(O.row_off.size(), std::vector<fe>(w));
+        for (size_t q = 0; q < O.row_off.size(); q++)
+            for (int j = 0; j < w; j++) P.trace_evaluations[q][j] = fb.value(O.row_off[q] + j);
+        for (size_t off : O.cval_off) P.constraint_proof.values.push_back(fb.digest(off));
+        P.constraint_proof.nodes = digests_at(O.c_off);
+        P.constraint_proof.depth = O.cplan.depth;
+        for (size_t d = 0; d < O.fri_open.size(); d++) {
             const LayerOpen &lo = O.fri_open[d];
-            out.raw(s.layers[d].root.data(), 32);
-            out.u64(lo.pos.size());
-            for (size_t off : lo.val_off)
-                for (int j = 0; j < 4; j++) out.felt(fb.value(off + j));
-            write_digest_vv(out, digests_at(lo.node_off));
-            out.u8(lo.depth);
+            FriLayer &l = P.degree_proof.layers[d];
+            for (size_t off : lo.val_off) l.values.push_back({fb.value(off), fb.value(off + 1), fb.value(off + 2), fb.value(off + 3)});
+            l.nodes = digests_at(lo.node_off);
+            l.depth = lo.depth;
         }
-        out.raw(s.layers.back().root.data(), 32);
-        out.u64(O.rem_off.size());
-        for (size_t off : O.rem_off) out.felt(fb.value(off));
-        out.u64(proof->pow_nonce);
-        out.u8((uint8_t)log_b); out.u8((uint8_t)opt.num_queries); out.u8((uint8_t)opt.grinding_factor); out.u8(0);
-        proof->bytes = std::move(out.b);
+        for (size_t off : O.rem_off) P.degree_proof.rem_values.push_back(fb.value(off));
+        Proof &h = *s.proof;
+        h.bytes = write_proof(P);
+        memcpy(h.trace_root, P.trace_root.data(), 32);
+        memcpy(h.constraint_root, P.constraint_root.data(), 32);
+        h.pow_nonce = P.pow_nonce;
     };
     {
         std::vector<OpenPlan> plans(K);
@@ -961,7 +944,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             if (ps[p].live) plans[p] = plan_openings(ps[p], slab_of(p), c_ext_of(p), first_row[p]);
         fb.run();
         for (int p = 0; p < K; p++)
-            if (ps[p].live) serialise(ps[p], plans[p]);
+            if (ps[p].live) fill_openings(ps[p], plans[p]);
     }
     clk.mark(9);
     sub.mark("9.openings");

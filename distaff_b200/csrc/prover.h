@@ -3,14 +3,9 @@
 #pragma once
 #include "../../include/distaff_gpu.h"
 #include "common.cuh"
+#include "proof.h"
 
 namespace dg {
-
-struct Proof {
-    std::vector<uint8_t> bytes;          // bincode encoding of StarkProof
-    uint8_t trace_root[32], constraint_root[32], pow_seed[32];
-    unsigned long long pow_nonce = 0;
-};
 
 // Proves `count` traces of one shape: registers on the device ([count][width][length] at d_regs), or host columns (host_cols: count * width
 // pointers) uploaded group by group into c.upload_buf.  On one GPU the call is planned (plan_prove) and runs in groups; on several

@@ -12,12 +12,9 @@
 // redundantly.  With G == 1 the same code runs without
 // communication and the three heaps are one.
 #pragma once
-#include <array>
 #include "common.cuh"
 
 namespace dg {
-
-typedef std::array<uint8_t, 32> Digest;
 
 enum { SHARD_LOCAL = 0, SHARD_TOP = 1, SHARD_MID = 2 };
 struct ShardLocation { int owner; int kind; uint64_t index; };   // kind: which heap `index` points into (SHARD_TOP: replicated, owner = -1)

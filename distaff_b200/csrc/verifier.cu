@@ -29,73 +29,13 @@
 #include "blake3.cuh"
 #include "host_fs.h"
 #include "poly.h"
+#include "proof.h"
 #include "prover.h"
 #include "shard.h"
 
 namespace dg {
 
 namespace {
-
-// ---- bincode reader (proof.rs:10-37, fri/mod.rs:17-30, merkle.rs:14-18) -------------------------------------------------------
-struct Reader {
-    const uint8_t *p, *end;
-    bool ok = true;
-    Reader(const uint8_t *b, size_t n) : p(b), end(b + n) {}
-    bool need(size_t n) { if (!ok || (size_t)(end - p) < n) { ok = false; return false; } return true; }
-    uint8_t u8() { if (!need(1)) return 0; return *p++; }
-    uint32_t u32() { if (!need(4)) return 0; uint32_t v; memcpy(&v, p, 4); p += 4; return v; }
-    uint64_t u64() { if (!need(8)) return 0; uint64_t v; memcpy(&v, p, 8); p += 8; return v; }
-    fe felt() { fe v = fe_make(0, 0); if (!need(16)) return v; memcpy(&v, p, 16); p += 16; return v; }
-    Digest digest() { Digest d; d.fill(0); if (!need(32)) return d; memcpy(d.data(), p, 32); p += 32; return d; }
-    size_t len(size_t elem_bytes) {                              // a Vec length that the remaining bytes can actually hold
-        uint64_t n = u64();
-        if (!ok || n > (uint64_t)(end - p) / (elem_bytes ? elem_bytes : 1)) { ok = false; return 0; }
-        return (size_t)n;
-    }
-    std::vector<Digest> dvec() { size_t n = len(32); std::vector<Digest> v(n); for (auto &x : v) x = digest(); return v; }
-    std::vector<std::vector<Digest>> dvv() { size_t n = len(8); std::vector<std::vector<Digest>> v(n); for (auto &x : v) x = dvec(); return v; }
-    std::vector<fe> fvec() { size_t n = len(16); std::vector<fe> v(n); for (auto &x : v) x = felt(); return v; }
-};
-
-struct FriLayerProof { Digest root; std::vector<std::array<fe, 4>> values; std::vector<std::vector<Digest>> nodes; uint8_t depth; };
-struct ParsedProof {
-    Digest trace_root, constraint_root, rem_root;
-    uint8_t domain_depth, ctx_depth, loop_depth, stack_depth, c_depth;
-    uint32_t op_count;
-    std::vector<std::vector<Digest>> trace_nodes, c_nodes;
-    std::vector<std::vector<fe>> trace_evaluations;
-    std::vector<Digest> c_values;
-    std::vector<fe> z1, z2, rem_values;
-    std::vector<FriLayerProof> layers;
-    uint64_t pow_nonce;
-    uint8_t log_ext, num_queries, grinding, hash_id;
-};
-
-bool parse_proof(const uint8_t *bytes, size_t n, ParsedProof &P) {
-    Reader r(bytes, n);
-    P.trace_root = r.digest();
-    P.domain_depth = r.u8(); P.ctx_depth = r.u8(); P.loop_depth = r.u8(); P.stack_depth = r.u8();
-    P.op_count = r.u32();
-    P.trace_nodes = r.dvv();
-    { size_t k = r.len(8); P.trace_evaluations.resize(k); for (auto &row : P.trace_evaluations) row = r.fvec(); }
-    P.constraint_root = r.digest();
-    P.c_values = r.dvec(); P.c_nodes = r.dvv(); P.c_depth = r.u8();
-    P.z1 = r.fvec(); P.z2 = r.fvec();
-    { size_t k = r.len(41); P.layers.resize(k); }
-    for (auto &l : P.layers) {
-        l.root = r.digest();
-        size_t k = r.len(64);
-        l.values.resize(k);
-        for (auto &q : l.values) for (int j = 0; j < 4; j++) q[j] = r.felt();
-        l.nodes = r.dvv();
-        l.depth = r.u8();
-    }
-    P.rem_root = r.digest();
-    P.rem_values = r.fvec();
-    P.pow_nonce = r.u64();
-    P.log_ext = r.u8(); P.num_queries = r.u8(); P.grinding = r.u8(); P.hash_id = r.u8();
-    return r.ok && r.p == r.end;
-}
 
 // ---- batch Merkle verification as a hashing plan (merkle.rs:154-263) -------------------------------------------------------------
 // pool slots: the caller lays out the proof's values and nodes in a pool of 32-byte digests; computed parents get fresh slots
@@ -380,7 +320,7 @@ struct Item {
     int status = DG_OK;
     std::string message;
     // ---- prepare
-    ParsedProof P;
+    StarkProof P;
     int w = 0, log_N = 0, nq = 0;
     uint64_t n = 0;
     std::vector<uint64_t> t_positions;
@@ -409,23 +349,27 @@ void prepare(Item &it) {
     it.outputs.resize(it.in.n_outputs);
     if (it.in.n_inputs) memcpy(it.inputs.data(), it.in.inputs16, (size_t)it.in.n_inputs * 16);
     if (it.in.n_outputs) memcpy(it.outputs.data(), it.in.outputs16, (size_t)it.in.n_outputs * 16);
-    ParsedProof &P = it.P;
-    if (!parse_proof(it.in.proof, it.in.proof_len, P)) throw Error(DG_ERR_INVALID, "malformed proof bytes (bincode layout of StarkProof, proof.rs:10-37)");
-    if (P.hash_id != 0) return reject(it, "unsupported hash function");
-    DG_REQUIRE(P.log_ext >= 4 && P.log_ext <= 8, "invalid extension factor in proof options");
-    DG_REQUIRE(P.domain_depth >= P.log_ext + 4 && P.domain_depth <= 30, "invalid domain depth");
+    StarkProof &P = it.P;
+    if (!read_proof(it.in.proof, it.in.proof_len, P)) throw Error(DG_ERR_INVALID, "malformed proof bytes (bincode layout of StarkProof, proof.rs:10-37)");
+    const TraceInfo &info = P.trace_info;
+    const BatchMerkleProof &cp = P.constraint_proof;
+    const std::vector<FriLayer> &layers = P.degree_proof.layers;
+    const int log_ext = P.options.log_extension_factor;
+    if (P.options.hash_fn != 0) return reject(it, "unsupported hash function");
+    DG_REQUIRE(log_ext >= 4 && log_ext <= 8, "invalid extension factor in proof options");
+    DG_REQUIRE(info.domain_depth >= log_ext + 4 && info.domain_depth <= 30, "invalid domain depth");
     DG_REQUIRE(it.inputs.size() <= 8 && it.outputs.size() <= 8, "cannot have more than 8 public inputs / outputs");
-    const uint64_t b = 1ULL << P.log_ext, N = 1ULL << P.domain_depth, n = N >> P.log_ext;
+    const uint64_t b = 1ULL << log_ext, N = 1ULL << info.domain_depth, n = N >> log_ext;
     it.n = n;
-    it.log_N = P.domain_depth;
-    DG_REQUIRE(TraceShape::in_range(P.ctx_depth, P.loop_depth, P.stack_depth), "invalid register counts in the proof");
-    const TraceShape shape(P.ctx_depth, P.loop_depth, P.stack_depth);
+    it.log_N = info.domain_depth;
+    DG_REQUIRE(TraceShape::in_range(info.ctx_depth, info.loop_depth, info.stack_depth), "invalid register counts in the proof");
+    const TraceShape shape(info.ctx_depth, info.loop_depth, info.stack_depth);
     const int w = it.w = shape.w;
 
     // ---- 1: PoW, query positions (verifier.rs:19-31)
     std::vector<uint8_t> fri_roots;
-    for (auto &l : P.layers) fri_roots.insert(fri_roots.end(), l.root.begin(), l.root.end());
-    fri_roots.insert(fri_roots.end(), P.rem_root.begin(), P.rem_root.end());
+    for (auto &l : layers) fri_roots.insert(fri_roots.end(), l.root.begin(), l.root.end());
+    fri_roots.insert(fri_roots.end(), P.degree_proof.rem_root.begin(), P.degree_proof.rem_root.end());
     DG_REQUIRE(fri_roots.size() <= 1024, "too many FRI layers");
     uint8_t seed[32], pseed[32];
     fs::blake3_short(fri_roots.data(), fri_roots.size(), seed);
@@ -434,17 +378,17 @@ void prepare(Item &it) {
         uint64_t o0;
         memcpy(&o0, pseed, 8);
         const unsigned tz = o0 == 0 ? 64u : (unsigned)__builtin_ctzll(o0);
-        if (tz < P.grinding) return reject(it, "seed proof-of-work verification failed");
+        if (tz < P.options.grinding_factor) return reject(it, "seed proof-of-work verification failed");
     }
-    try { it.t_positions = fs::query_positions(pseed, N, b, P.num_queries); }
+    try { it.t_positions = fs::query_positions(pseed, N, b, P.options.num_queries); }
     catch (const std::exception &e) { return reject(it, e.what()); }
     const std::vector<uint64_t> c_positions = fs::constraint_positions(it.t_positions);
     const int nq = it.nq = (int)it.t_positions.size();
     // ---- 2: minimum op count (verifier.rs:34-37; MIN_TRACE_LENGTH = 16)
-    if (P.op_count < 16) return reject(it, "Verification of minimum operation count failed");
+    if (info.op_count < 16) return reject(it, "Verification of minimum operation count failed");
     if ((int)P.trace_evaluations.size() != nq) return reject(it, "verification of trace Merkle proof failed");
     for (auto &row : P.trace_evaluations) DG_REQUIRE((int)row.size() == w, "trace evaluation row has wrong width");
-    DG_REQUIRE((int)P.z1.size() == w && (int)P.z2.size() == w, "deep value vector has wrong width");
+    DG_REQUIRE((int)P.trace_at_z1.size() == w && (int)P.trace_at_z2.size() == w, "deep value vector has wrong width");
 
     // ---- the Merkle plans over the proof's local pool of digests
     std::vector<Digest> &pool = it.pool;
@@ -456,36 +400,36 @@ void prepare(Item &it) {
     };
     const uint32_t tv_base = reserve(nq);
     std::vector<uint32_t> fv_base;
-    for (auto &l : P.layers) { it.fri_off.push_back(it.n_fri); fv_base.push_back(reserve(l.values.size())); it.n_fri += (uint32_t)l.values.size(); }
+    for (auto &l : layers) { it.fri_off.push_back(it.n_fri); fv_base.push_back(reserve(l.values.size())); it.n_fri += (uint32_t)l.values.size(); }
     const uint32_t cv_base = (uint32_t)pool.size();
-    pool.insert(pool.end(), P.c_values.begin(), P.c_values.end());
-    const std::vector<uint32_t> tn_bases = put_nodes(P.trace_nodes), cn_bases = put_nodes(P.c_nodes);
+    pool.insert(pool.end(), cp.values.begin(), cp.values.end());
+    const std::vector<uint32_t> tn_bases = put_nodes(P.trace_nodes), cn_bases = put_nodes(cp.nodes);
     std::vector<std::vector<uint32_t>> fn_bases;
-    for (auto &l : P.layers) fn_bases.push_back(put_nodes(l.nodes));
+    for (auto &l : layers) fn_bases.push_back(put_nodes(l.nodes));
     uint32_t next_slot = (uint32_t)pool.size();
 
     // FRI positions per layer (fri/verifier.rs:24-31)
-    it.layer_aug.resize(P.layers.size());
+    it.layer_aug.resize(layers.size());
     {
         std::vector<uint64_t> pos = it.t_positions;
         uint64_t domain = N;
-        for (size_t d = 0; d < P.layers.size(); d++) {
+        for (size_t d = 0; d < layers.size(); d++) {
             it.layer_aug[d] = fs::augmented_positions(pos, domain);
             pos = it.layer_aug[d];
             domain /= 4;
         }
     }
-    it.plans.push_back(plan_verify_batch(it.t_positions, P.domain_depth, nq, tv_base, P.trace_nodes, tn_bases, next_slot));
-    it.plans.push_back(plan_verify_batch(c_positions, P.c_depth, P.c_values.size(), cv_base, P.c_nodes, cn_bases, next_slot));
-    for (size_t d = 0; d < P.layers.size(); d++)
-        it.plans.push_back(plan_verify_batch(it.layer_aug[d], P.layers[d].depth, P.layers[d].values.size(), fv_base[d], P.layers[d].nodes, fn_bases[d], next_slot));
+    it.plans.push_back(plan_verify_batch(it.t_positions, info.domain_depth, nq, tv_base, P.trace_nodes, tn_bases, next_slot));
+    it.plans.push_back(plan_verify_batch(c_positions, cp.depth, cp.values.size(), cv_base, cp.nodes, cn_bases, next_slot));
+    for (size_t d = 0; d < layers.size(); d++)
+        it.plans.push_back(plan_verify_batch(it.layer_aug[d], layers[d].depth, layers[d].values.size(), fv_base[d], layers[d].nodes, fn_bases[d], next_slot));
     pool.resize(next_slot);
 
     // ---- 4: constraints at z (verifier.rs:47-52, 79-97)
     it.z = fs::prng_vector(P.constraint_root.data(), 1)[0];
     fe program_hash_fe[2];
     memcpy(program_hash_fe, it.in.program_hash, 32);
-    it.cc = fs::draw_constraint_coefficients(P.trace_root.data(), shape, it.inputs, it.outputs, fe_make(P.op_count, 0), program_hash_fe);
+    it.cc = fs::draw_constraint_coefficients(P.trace_root.data(), shape, it.inputs, it.outputs, fe_make(info.op_count, 0), program_hash_fe);
     it.per_xpow = fs::periodic_at(fe_pow_u64(it.z, n / 16));
     for (int g = 0; g < 6; g++) it.per_xpow.push_back(fe_pow_u64(it.z, group_increment(g, n)));
 
@@ -496,32 +440,33 @@ void prepare(Item &it) {
         const uint64_t position = it.t_positions[q];
         const size_t leaf_idx = std::find(c_positions.begin(), c_positions.end(), position / 2) - c_positions.begin();
         // the reference fails here, before any root is compared: this verdict wins over every later check
-        if (leaf_idx >= P.c_values.size()) return reject(it, "verification of constraint Merkle proof failed");
-        memcpy(&it.c_evals[q], P.c_values[leaf_idx].data() + (position % 2) * 16, 16);
+        if (leaf_idx >= cp.values.size()) return reject(it, "verification of constraint Merkle proof failed");
+        memcpy(&it.c_evals[q], cp.values[leaf_idx].data() + (position % 2) * 16, 16);
     }
 
     // ---- 6: FRI folding points (fri/verifier.rs:33-75)
-    for (auto &l : P.layers) it.alphas.push_back(fs::prng_vector(l.root.data(), 1)[0]);
+    for (auto &l : layers) it.alphas.push_back(fs::prng_vector(l.root.data(), 1)[0]);
 }
 
 // the reference's checks in its order, on the device results; returns "" when the proof is accepted
 std::string finish(const Item &it) {
-    const ParsedProof &P = it.P;
-    const uint64_t b = 1ULL << P.log_ext;
+    const StarkProof &P = it.P;
+    const std::vector<FriLayer> &layers = P.degree_proof.layers;
+    const uint64_t b = 1ULL << P.options.log_extension_factor;
     auto root_ok = [&](size_t t, const Digest &root) { return it.plans[t].ok && it.roots[t] == root; };
     if (!root_ok(0, P.trace_root)) return "verification of trace Merkle proof failed";
     if (!root_ok(1, P.constraint_root)) return "verification of constraint Merkle proof failed";
 
     std::string fri_err;
     {
-        if (P.layers.empty()) return "verification of low-degree proof failed: no FRI layers";
+        if (layers.empty()) return "verification of low-degree proof failed: no FRI layers";
         std::vector<fe> evaluations = it.comp;
         std::vector<uint64_t> positions = it.t_positions;
-        uint64_t domain_size = (1ULL << P.layers[0].depth) * 4;
+        uint64_t domain_size = (1ULL << layers[0].depth) * 4;
         uint64_t max_degree_plus_1 = (7 * it.n - 1) + 1;          // get_composition_degree(n) + 1
-        fe domain_root = host_root_of_unity(P.layers[0].depth + 2);
-        for (size_t d = 0; d < P.layers.size() && fri_err.empty(); d++) {
-            const FriLayerProof &layer = P.layers[d];
+        fe domain_root = host_root_of_unity(layers[0].depth + 2);
+        for (size_t d = 0; d < layers.size() && fri_err.empty(); d++) {
+            const FriLayer &layer = layers[d];
             const std::vector<uint64_t> aug = fs::augmented_positions(positions, domain_size);
             const uint64_t row_length = domain_size / 4;
             std::vector<fe> column_values;
@@ -544,13 +489,13 @@ std::string finish(const Item &it) {
         }
         if (fri_err.empty()) {
             for (size_t i = 0; i < positions.size(); i++)
-                if (positions[i] >= P.rem_values.size() || !fe_eq(P.rem_values[positions[i]], evaluations[i])) {
+                if (positions[i] >= P.degree_proof.rem_values.size() || !fe_eq(P.degree_proof.rem_values[positions[i]], evaluations[i])) {
                     fri_err = "remainder values are inconsistent with values of the last column";
                     break;
                 }
         }
         if (fri_err.empty()) {                                      // verify_remainder (fri/verifier.rs:97-131)
-            const std::vector<fe> &rem = P.rem_values;
+            const std::vector<fe> &rem = P.degree_proof.rem_values;
             if (max_degree_plus_1 > rem.size()) fri_err = "remainder degree is greater than number of remainder values";
             else {
                 std::vector<fe> xs, ys;
@@ -597,7 +542,7 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     std::vector<int> shape_of(K), widths;
     auto shape_at = [&](size_t s) { return TraceShape(shapes[s][0], shapes[s][1], shapes[s][2]); };
     for (int i = 0; i < K; i++) {
-        const std::array<int, 3> s{g[i]->P.ctx_depth, g[i]->P.loop_depth, g[i]->P.stack_depth};
+        const std::array<int, 3> s{g[i]->P.trace_info.ctx_depth, g[i]->P.trace_info.loop_depth, g[i]->P.trace_info.stack_depth};
         shape_of[i] = (int)(std::find(shapes.begin(), shapes.end(), s) - shapes.begin());
         if (shape_of[i] == (int)shapes.size()) shapes.push_back(s);
         if (std::find(widths.begin(), widths.end(), g[i]->w) == widths.end()) widths.push_back(g[i]->w);
@@ -640,9 +585,10 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
         unsigned *layer = (unsigned *)(up.b.data() + fri_layer_off), *proof = (unsigned *)(up.b.data() + fri_proof_off);
         for (int i = 0; i < K; i++) {
             size_t t = ffirst[i];
-            for (size_t d = 0; d < g[i]->P.layers.size(); d++)
-                for (size_t j = 0; j < g[i]->P.layers[d].values.size(); j++, t++) {
-                    for (int k = 0; k < 4; k++) rows[4 * t + k] = g[i]->P.layers[d].values[j][k];
+            const std::vector<FriLayer> &layers = g[i]->P.degree_proof.layers;
+            for (size_t d = 0; d < layers.size(); d++)
+                for (size_t j = 0; j < layers[d].values.size(); j++, t++) {
+                    for (int k = 0; k < 4; k++) rows[4 * t + k] = layers[d].values[j][k];
                     pos[t] = j < g[i]->layer_aug[d].size() ? g[i]->layer_aug[d][j] : 0;
                     layer[t] = (unsigned)d;
                     proof[t] = (unsigned)i;
@@ -662,8 +608,8 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
     const size_t pos_off = up.put(positions), qproof_off = up.put(qproof), cev_off = up.put(c_evals);
     for (int i = 0; i < K; i++) {
         const Item &it = *g[i];
-        std::vector<fe> v(it.P.z1);
-        v.insert(v.end(), it.P.z2.begin(), it.P.z2.end());
+        std::vector<fe> v(it.P.trace_at_z1);
+        v.insert(v.end(), it.P.trace_at_z2.begin(), it.P.trace_at_z2.end());
         v.insert(v.end(), it.dc.trace1.begin(), it.dc.trace1.end());
         v.insert(v.end(), it.dc.trace2.begin(), it.dc.trace2.end());
         zs_off[i] = up.put(v);
@@ -739,7 +685,7 @@ void run_group(Context &c, const std::vector<Item *> &g, float *ms) {
             const int s = shape_of[i];
             const size_t v = std::find(widths.begin(), widths.end(), it.w) - widths.begin();
             const fe *zs = (const fe *)(base + zs_off[i]);
-            const fe root_n = host_root_of_unity(it.log_N - it.P.log_ext);
+            const fe root_n = host_root_of_unity(it.log_N - it.P.options.log_extension_factor);
             AtZDesc &a = atz[i];
             a.z1 = zs; a.bcoef = (const fe *)(base + bc_off[i]);
             a.t_at_z = tev + tev0[s] + (size_t)shape_pos[i] * 128;
@@ -877,7 +823,7 @@ void verify_proofs(Context &c, const std::vector<VerifyRequest> &req, std::vecto
     for (Item &it : items) {
         if (it.decided) continue;
         const size_t b = item_bytes(it);
-        const std::array<int, 3> shape{it.P.ctx_depth, it.P.loop_depth, it.P.stack_depth};
+        const std::array<int, 3> shape{it.P.trace_info.ctx_depth, it.P.trace_info.loop_depth, it.P.trace_info.stack_depth};
         if (!g.empty() && (bytes + b > group_bytes || g.size() >= cap || per_shape[shape] >= 65535)) flush();
         g.push_back(&it);
         per_shape[shape]++;
