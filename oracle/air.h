@@ -613,13 +613,15 @@ struct Evaluator {
         }
         return result;
     }
-    // :139-162 ; `raw` (optional) receives the individual constraint evaluations
-    u128 evaluate_transition(const TraceState &cur, const TraceState &nxt, u128 x, size_t step, std::vector<u128> *raw = nullptr) const {
+    // :139-162 ; `raw` (optional) receives the individual constraint evaluations.  check = false (forged proofs only) skips the
+    // assertion and combines the constraints at trace steps as at every other step.
+    u128 evaluate_transition(const TraceState &cur, const TraceState &nxt, u128 x, size_t step, std::vector<u128> *raw = nullptr,
+                             bool check = true) const {
         std::vector<u128> ev(t_constraint_num, 0);
         decoder.evaluate(cur, nxt, step, ev.data());
         stack.evaluate(cur, nxt, step, ev.data() + decoder.constraint_count());
         if (raw) *raw = ev;
-        if (should_evaluate_to_zero_at(step)) {
+        if (check && should_evaluate_to_zero_at(step)) {
             for (size_t i = 0; i < ev.size(); i++)
                 if (ev[i] != 0) throw std::runtime_error("transition constraint at step " + std::to_string(step / extension_factor) + " were not satisfied (constraint " + std::to_string(i) + ")");
             return 0;

@@ -181,11 +181,25 @@ void or_hasher_digest(const uint8_t *values, uint32_t n, uint8_t *out32) {
 
 // ---- prover / verifier ---------------------------------------------------------------------------------------------------
 // cols: column-major w x n field elements.  Returns a handle (never null); query with or_result_*.
+void *or_prove_forged(const uint8_t *cols, uint32_t w, uint64_t n, uint32_t ctx_depth, uint32_t loop_depth,
+                      const uint8_t *inputs, uint32_t n_in, const uint8_t *outputs, uint32_t n_out,
+                      uint32_t ext, uint32_t num_queries, uint32_t grinding, int keep_large, int forge_kind, int64_t forge_a, int64_t forge_b);
 void *or_prove(const uint8_t *cols, uint32_t w, uint64_t n, uint32_t ctx_depth, uint32_t loop_depth,
                const uint8_t *inputs, uint32_t n_in, const uint8_t *outputs, uint32_t n_out,
                uint32_t ext, uint32_t num_queries, uint32_t grinding, int keep_large) {
+    return or_prove_forged(cols, w, n, ctx_depth, loop_depth, inputs, n_in, outputs, n_out, ext, num_queries, grinding, keep_large,
+                           Forgery::none, 0, 0);
+}
+// or_prove with one value changed before it is committed (stark.h Forgery: kind, a, b); a proof of a false statement whose
+// commitments are all consistent, for testing what the verifiers reject
+void *or_prove_forged(const uint8_t *cols, uint32_t w, uint64_t n, uint32_t ctx_depth, uint32_t loop_depth,
+                      const uint8_t *inputs, uint32_t n_in, const uint8_t *outputs, uint32_t n_out,
+                      uint32_t ext, uint32_t num_queries, uint32_t grinding, int keep_large, int forge_kind, int64_t forge_a, int64_t forge_b) {
     ProveResult *r = new ProveResult();
     try {
+        Forgery forge;
+        if (forge_kind < Forgery::none || forge_kind > Forgery::remainder_cut) throw std::runtime_error("unknown forgery");
+        forge.kind = (Forgery::Kind)forge_kind; forge.a = forge_a; forge.b = forge_b;
         std::vector<std::vector<u128>> regs(w, std::vector<u128>(n));
         for (uint32_t j = 0; j < w; j++) memcpy(regs[j].data(), cols + (size_t)j * n * 16, n * 16);
         std::vector<u128> in(n_in), out(n_out);
@@ -193,7 +207,7 @@ void *or_prove(const uint8_t *cols, uint32_t w, uint64_t n, uint32_t ctx_depth, 
         if (n_out) memcpy(out.data(), outputs, n_out * 16);
         ProofOptions opt; opt.extension_factor = ext; opt.num_queries = num_queries; opt.grinding_factor = grinding;
         r->trace.keep_large = keep_large != 0;
-        StarkProof p = prove(regs, ctx_depth, loop_depth, in, out, opt, &r->trace);
+        StarkProof p = prove(regs, ctx_depth, loop_depth, in, out, opt, &r->trace, forge);
         r->bytes = serialize(p);
     } catch (std::exception &e) { r->error = e.what(); }
     return r;

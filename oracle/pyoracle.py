@@ -22,6 +22,8 @@ def lib():
         L.or_prove.restype = ctypes.c_void_p
         L.or_prove.argtypes = [u8p, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_uint32, ctypes.c_uint32, u8p, ctypes.c_uint32, u8p,
                                ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, ctypes.c_int]
+        L.or_prove_forged.restype = ctypes.c_void_p
+        L.or_prove_forged.argtypes = L.or_prove.argtypes + [ctypes.c_int, ctypes.c_int64, ctypes.c_int64]
         L.or_result_error.restype = ctypes.c_char_p
         L.or_result_error.argtypes = [ctypes.c_void_p]
         L.or_result_proof_len.restype = ctypes.c_uint64
@@ -230,14 +232,23 @@ class ProveResult:
             pass
 
 
-def prove(registers, ctx_depth, loop_depth, inputs, outputs, ext=32, num_queries=50, grinding=20, keep_large=False):
-    """registers: (w, n, 2) uint64 column-major.  Returns ProveResult (check .error)."""
+# stark.h Forgery::Kind: what or_prove_forged changes before it is committed
+FORGERIES = {"transition": 1, "op_count": 2, "constraint_offset": 3, "deep_value": 4, "fri_offset": 5, "fri_alpha": 6,
+             "remainder_point": 7, "layers": 8, "remainder_cut": 9}
+
+
+def prove(registers, ctx_depth, loop_depth, inputs, outputs, ext=32, num_queries=50, grinding=20, keep_large=False, forge=None):
+    """registers: (w, n, 2) uint64 column-major.  Returns ProveResult (check .error).  forge: None for an honest proof, or
+    (kind, a[, b]) with kind a key of FORGERIES: a proof of a false statement whose commitments are all consistent (stark.h Forgery)."""
     regs = np.ascontiguousarray(registers, dtype=np.uint64)
     w, n = regs.shape[0], regs.shape[1]
     fi, fo = fvec(list(inputs)), fvec(list(outputs))
-    h = lib().or_prove(regs.ctypes.data, w, n, ctx_depth, loop_depth, fi.ctypes.data, len(fi), fo.ctypes.data, len(fo),
-                       ext, num_queries, grinding, 1 if keep_large else 0)
-    return ProveResult(h)
+    args = (regs.ctypes.data, w, n, ctx_depth, loop_depth, fi.ctypes.data, len(fi), fo.ctypes.data, len(fo), ext, num_queries, grinding,
+            1 if keep_large else 0)
+    if forge is None:
+        return ProveResult(lib().or_prove(*args))
+    kind, a, b = (tuple(forge) + (0, 0))[:3]
+    return ProveResult(lib().or_prove_forged(*args, FORGERIES[kind], a, b))
 
 
 def extend(registers, blowup):

@@ -140,12 +140,12 @@ static inline std::vector<size_t> map_trace_to_constraint_positions(const std::v
     for (size_t p : positions) { size_t cp = p / 2; if (std::find(r.begin(), r.end(), cp) == r.end()) r.push_back(cp); }
     return r;
 }
-// proof_of_work.rs:4-32
-static inline uint64_t find_pow_nonce(const uint8_t seed[32], uint32_t grinding, HashFn hash, uint8_t out_seed[32]) {
+// proof_of_work.rs:4-32 ; `after` > 0 (forged proofs only) returns the first valid nonce above it
+static inline uint64_t find_pow_nonce(const uint8_t seed[32], uint32_t grinding, HashFn hash, uint8_t out_seed[32], uint64_t after = 0) {
     uint8_t in[64];
     memset(in, 0, 64);
     memcpy(in, seed, 32);
-    uint64_t nonce = 0;
+    uint64_t nonce = after;
     for (;;) {
         nonce += 1;
         for (int i = 0; i < 8; i++) in[32 + i] = (uint8_t)(nonce >> (8 * i));
@@ -170,6 +170,27 @@ static inline bool verify_pow_nonce(const uint8_t seed[32], uint64_t nonce, uint
     return tz >= grinding;
 }
 
+// ---- forged proofs (tests only; the reference has no such switch) ----------------------------------------------
+// One value is changed before it is committed.  Every root, Fiat-Shamir draw, PoW nonce, query position and opening after it is
+// derived from the changed value, so the proof passes the Merkle and PoW checks and only the verifier's algebraic checks can reject it.
+struct Forgery {
+    enum Kind {
+        none = 0,
+        transition,         // a: trace row whose top user-stack value gets +1, breaking the transitions into and out of it; stage 3's
+                            //    assertion and stage 4's degree check are skipped
+        op_count,           // a: the op count in the proof and in the boundary constraint at the last step (stage 4 check skipped)
+        constraint_offset,  // a: added to the combined constraint polynomial before its LDE and tree
+        deep_value,         // a: register, b: 0 = its value at z, 1 = at z * g; gets +1 and is used so in the DEEP composition
+        fri_offset,         // a: FRI layer whose values all get +1 before its tree; a = number of layers: the remainder
+        fri_alpha,          // a: FRI layer folded at prng(root) + 1
+        remainder_point,    // +1 on the last non-skipped remainder value that no query opens (retried downwards until one is found)
+        layers,             // a: folds beyond (> 0) or short of (< 0) the prover's count; everything stays honest
+        remainder_cut,      // only the first (degree bound + a) remainder values are sent; the nonce is the first valid one whose
+                            //    queries open none of the cut values (the verifier hashes the remainder root only into the PoW seed)
+    } kind = none;
+    int64_t a = 0, b = 0;
+};
+
 // ---- FRI (fri/prover.rs, fri/utils.rs) -----------------------------------------------------------------------
 static const size_t MAX_REMAINDER_LENGTH = 256;
 
@@ -186,23 +207,35 @@ static inline std::vector<size_t> get_augmented_positions(const std::vector<size
     for (size_t p : positions) { size_t ap = p % row_length; if (std::find(r.begin(), r.end(), ap) == r.end()) r.push_back(ap); }
     return r;
 }
+// number of folds fri_reduce makes on a domain of this size: while (p_tree.leaves().len() * 4 > MAX_REMAINDER_LENGTH)
+static inline size_t fri_fold_count(size_t domain_size) {
+    size_t k = 0;
+    for (; domain_size > MAX_REMAINDER_LENGTH; domain_size /= 4) k++;
+    return k;
+}
 static inline void fri_reduce(const std::vector<u128> &evaluations, const std::vector<u128> &domain, HashFn hash,
-                              std::vector<MerkleTree> &trees, std::vector<std::vector<quartic::Q>> &values) {
+                              std::vector<MerkleTree> &trees, std::vector<std::vector<quartic::Q>> &values,
+                              const Forgery &forge = Forgery()) {
+    const size_t folds = fri_fold_count(evaluations.size()) + (forge.kind == Forgery::layers ? forge.a : 0);
+    auto commit = [&](std::vector<quartic::Q> &v) {         // the tree of layer trees.size() (the remainder after the last fold)
+        if (forge.kind == Forgery::fri_offset && (size_t)forge.a == trees.size())
+            for (auto &q : v) for (auto &x : q.v) x = field::add(x, 1);
+        return MerkleTree(hash_values(v, hash), hash);
+    };
     std::vector<quartic::Q> p_values = quartic::transpose(evaluations.data(), evaluations.size(), 1);
-    MerkleTree p_tree(hash_values(p_values, hash), hash);
-    while (p_tree.values.size() * 4 > MAX_REMAINDER_LENGTH) {
+    MerkleTree p_tree = commit(p_values);
+    while (trees.size() < folds) {
         size_t depth = trees.size();
         size_t stride = (size_t)1 << (2 * depth);
         std::vector<quartic::Q> xs = quartic::transpose(domain.data(), domain.size(), stride);
         std::vector<quartic::Q> polys = quartic::interpolate_batch(xs, p_values);
         u128 special_x = prng(p_tree.root().data());
+        if (forge.kind == Forgery::fri_alpha && (size_t)forge.a == depth) special_x = field::add(special_x, 1);
         std::vector<u128> column = quartic::evaluate_batch(polys, special_x);
-        std::vector<quartic::Q> c_values = quartic::transpose(column.data(), column.size(), 1);
-        MerkleTree c_tree(hash_values(c_values, hash), hash);
         trees.push_back(std::move(p_tree));
         values.push_back(std::move(p_values));
-        p_tree = std::move(c_tree);
-        p_values = std::move(c_values);
+        p_values = quartic::transpose(column.data(), column.size(), 1);
+        p_tree = commit(p_values);
     }
     trees.push_back(std::move(p_tree));
     values.push_back(std::move(p_values));
@@ -256,7 +289,7 @@ static inline double now_ms();
 
 static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, size_t ctx_depth, size_t loop_depth,
                                const std::vector<u128> &inputs, const std::vector<u128> &outputs,
-                               const ProofOptions &opt, ProverTrace *dbg = nullptr) {
+                               const ProofOptions &opt, ProverTrace *dbg = nullptr, const Forgery &forge = Forgery()) {
     const size_t w = registers.size();
     const size_t n = registers[0].size();
     const size_t b = opt.extension_factor;
@@ -267,6 +300,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     const size_t decoder_width = 15 + ctx_depth + loop_depth;
     if (w <= decoder_width || w >= MAX_REGISTER_COUNT) throw std::runtime_error("invalid register count");
     const size_t stack_depth = w - decoder_width;
+    const bool lax = forge.kind == Forgery::transition || forge.kind == Forgery::op_count;   // a false statement: skip the prover's checks
     double t0 = now_ms();
 
     // 1 ----- extend execution trace (prover.rs:22-27, trace_table.rs:143-169) --------------------
@@ -278,6 +312,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     u128 trace_root_w = field::get_root_of_unity(n);
     std::vector<u128> inv_twiddles = fft::get_inv_twiddles(trace_root_w, n);
     std::vector<std::vector<u128>> polys(registers);
+    if (forge.kind == Forgery::transition) polys.at(decoder_width).at(forge.a) = field::add(polys[decoder_width][forge.a], 1);
     std::vector<std::vector<u128>> ext(w);
     const int T = fft::host_threads();
     if (T <= 1 || (size_t)T >= 2 * w) {                  // many more threads than columns: parallelism inside each transform instead
@@ -320,8 +355,9 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     TraceState last_state(ctx_depth, loop_depth, stack_depth);
     last_state.from_columns(ext, N - b);
     const size_t E = n * MAX_CONSTRAINT_DEGREE;
+    const u128 op_count = forge.kind == Forgery::op_count ? (u128)forge.a : last_state.op_counter;
     Evaluator evaluator(n, MAX_CONSTRAINT_DEGREE, E, ctx_depth, loop_depth, stack_depth, trace_tree.root().data(),
-                        last_state.sponge, last_state.op_counter, inputs, outputs);
+                        last_state.sponge, op_count, inputs, outputs);
     std::vector<u128> i_ev(E), f_ev(E), t_ev(E);
     {
         const size_t stride = b / MAX_CONSTRAINT_DEGREE;
@@ -337,7 +373,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
                     cur.from_columns(ext, i);
                     nxt.from_columns(ext, (i + b) % N);
                     evaluator.evaluate_boundaries(cur, lde_domain[i], i_ev[step], f_ev[step]);
-                    t_ev[step] = evaluator.evaluate_transition(cur, nxt, lde_domain[i], step);
+                    t_ev[step] = evaluator.evaluate_transition(cur, nxt, lde_domain[i], step, nullptr, !lax);
                 } catch (const std::exception &e) {
                     #pragma omp critical
                     if (step < failure_step) { failure_step = step; failure = e.what(); }
@@ -365,9 +401,10 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
         polynom::syn_div_expanded_in_place(t_ev.data(), E, n, &x_last, 1);
         for (size_t k = 0; k < E; k++) combined[k] = field::add(combined[k], t_ev[k]);
         // constraint_poly.rs:16-19 (debug assertion in the reference; a hard check here)
-        if (polynom::degree_of(combined.data(), E) != E - n)
+        if (!lax && polynom::degree_of(combined.data(), E) != E - n)
             throw std::runtime_error("combined constraint polynomial has unexpected degree");
     }
+    if (forge.kind == Forgery::constraint_offset) combined[0] = field::add(combined[0], (u128)forge.a);
     if (dbg) dbg->constraint_poly = combined;
     double t4 = now_ms(); if (dbg) dbg->stage_ms[3] = t4 - t3;
 
@@ -389,6 +426,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     std::vector<u128> state1(w), state2(w);
     for (size_t j = 0; j < w; j++) { state1[j] = polynom::eval(polys[j], z); }
     for (size_t j = 0; j < w; j++) { state2[j] = polynom::eval(polys[j], next_z); }
+    if (forge.kind == Forgery::deep_value) { u128 &v = (forge.b ? state2 : state1).at(forge.a); v = field::add(v, 1); }
     std::vector<u128> t1c(n, 0), t2c(n, 0);
     for (size_t j = 0; j < w; j++) {
         field::mul_acc(t1c.data(), polys[j].data(), cc.trace1[j], n);
@@ -421,16 +459,54 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     // 7 ----- FRI layers (prover.rs:109-114) ------------------------------------------------------
     std::vector<MerkleTree> fri_trees;
     std::vector<std::vector<quartic::Q>> fri_values;
-    fri_reduce(composed, lde_domain, hash, fri_trees, fri_values);
+    fri_reduce(composed, lde_domain, hash, fri_trees, fri_values, forge);
     double t7 = now_ms(); if (dbg) dbg->stage_ms[6] = t7 - t6;
 
     // 8 ----- query positions (prover.rs:119-133) -------------------------------------------------
-    std::vector<uint8_t> fri_roots;
-    for (auto &t : fri_trees) fri_roots.insert(fri_roots.end(), t.root().begin(), t.root().end());
     uint8_t seed[32], pow_seed[32];
-    hash(fri_roots.data(), fri_roots.size(), seed);
-    uint64_t pow_nonce = find_pow_nonce(seed, opt.grinding_factor, hash, pow_seed);
-    std::vector<size_t> positions = compute_query_positions(pow_seed, N, b, opt.num_queries);
+    uint64_t pow_nonce = 0;
+    std::vector<size_t> positions;
+    auto draw_positions = [&]() {
+        std::vector<uint8_t> fri_roots;
+        for (auto &t : fri_trees) fri_roots.insert(fri_roots.end(), t.root().begin(), t.root().end());
+        hash(fri_roots.data(), fri_roots.size(), seed);
+        pow_nonce = find_pow_nonce(seed, opt.grinding_factor, hash, pow_seed);
+        positions = compute_query_positions(pow_seed, N, b, opt.num_queries);
+    };
+    draw_positions();
+    // forged remainders: the remainder positions the queries open (fri/verifier.rs:33-80) and the degree bound the verifier applies
+    const size_t n_layers = fri_trees.size() - 1;
+    auto remainder_positions = [&]() {
+        std::vector<size_t> p = positions;
+        for (size_t d = 0, D = N; d < n_layers; d++, D /= 4) p = get_augmented_positions(p, D);
+        return p;
+    };
+    size_t rem_bound = get_composition_degree(n) + 1;
+    for (size_t d = 0; d < n_layers; d++) rem_bound /= 4;
+    if (forge.kind == Forgery::remainder_point) {
+        std::vector<quartic::Q> &last = fri_values.back();
+        const std::vector<quartic::Q> honest = last;
+        const size_t rows = last.size();
+        for (size_t r = rows * 4; ; ) {
+            do { if (r-- == 0) throw std::runtime_error("every remainder value is opened"); } while (r % b == 0);
+            last = honest;
+            last[r % rows].v[r / rows] = field::add(last[r % rows].v[r / rows], 1);
+            fri_trees.back() = MerkleTree(hash_values(last, hash), hash);
+            draw_positions();
+            std::vector<size_t> opened = remainder_positions();
+            if (std::find(opened.begin(), opened.end(), r) == opened.end()) break;
+        }
+    }
+    if (forge.kind == Forgery::remainder_cut) {
+        const size_t kept = (size_t)((int64_t)rem_bound + forge.a);
+        for (int t = 0;; t++) {
+            std::vector<size_t> opened = remainder_positions();
+            if (*std::max_element(opened.begin(), opened.end()) < kept) break;
+            if (t == 100000) throw std::runtime_error("no nonce opens only the kept remainder values");
+            pow_nonce = find_pow_nonce(seed, opt.grinding_factor, hash, pow_seed, pow_nonce);
+            positions = compute_query_positions(pow_seed, N, b, opt.num_queries);
+        }
+    }
     if (dbg) {
         for (auto &t : fri_trees) dbg->fri_roots.push_back(t.root());
         dbg->pow_nonce = pow_nonce; memcpy(dbg->pow_seed.data(), pow_seed, 32); dbg->positions = positions;
@@ -441,6 +517,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     // 9 ----- proof object (prover.rs:143-165) ----------------------------------------------------
     StarkProof proof;
     proof.degree_proof = fri_build_proof(fri_trees, fri_values, positions);
+    if (forge.kind == Forgery::remainder_cut) proof.degree_proof.rem_values.resize((size_t)((int64_t)rem_bound + forge.a));
     for (size_t p : positions) {
         std::vector<u128> row(w);
         for (size_t j = 0; j < w; j++) row[j] = ext[j][p];
@@ -451,7 +528,7 @@ static inline StarkProof prove(const std::vector<std::vector<u128>> &registers, 
     proof.trace_root = trace_tree.root();
     proof.domain_depth = tproof.depth;
     proof.ctx_depth = (uint8_t)ctx_depth; proof.loop_depth = (uint8_t)loop_depth; proof.stack_depth = (uint8_t)stack_depth;
-    proof.op_count = (uint32_t)last_state.op_counter;
+    proof.op_count = (uint32_t)op_count;
     proof.trace_nodes = tproof.nodes;
     proof.constraint_root = constraint_tree.root();
     proof.constraint_proof = constraint_tree.prove_batch(c_positions);
@@ -519,6 +596,9 @@ static inline std::string fri_verify(const FriProof &proof, std::vector<u128> ev
     for (size_t i = 0; i < rem.size(); i++) if (i % opt.extension_factor != 0) pos.push_back(i);
     std::vector<u128> domain = field::get_power_series(domain_root, rem.size());
     std::vector<u128> xs, ys;
+    // fri/verifier.rs:108-110 indexes positions[i] past its end when the bound exceeds the non-skipped points, and panics
+    if (max_degree_plus_1 > pos.size())
+        throw std::runtime_error("index out of bounds: the len is " + std::to_string(pos.size()) + " but the index is " + std::to_string(pos.size()));
     for (size_t i = 0; i < max_degree_plus_1; i++) { xs.push_back(domain[pos[i]]); ys.push_back(rem[pos[i]]); }
     std::vector<u128> poly = polynom::interpolate(xs, ys);
     for (size_t i = max_degree_plus_1; i < pos.size(); i++)
