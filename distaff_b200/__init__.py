@@ -3,6 +3,7 @@
 Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.prove(trace, options)            <->  stark::prove        (/root/reference/src/stark/prover.rs:17)
     distaff_b200.prove_batch(traces, options)     <->  stark::prove of every trace, same-shape traces proven together
+    distaff_b200.prove_traces(traces, options)    <->  stark::prove of every trace, traces of any shapes in one call
     distaff_b200.execute(source, inputs, ...)     <->  distaff::execute    (/root/reference/src/lib.rs:30-65), VM = host stand-in
     distaff_b200.verify(hash, inputs, outputs, p) <->  distaff::verify     (/root/reference/src/lib.rs:68-75, stark/verifier.rs:11-75)
     distaff_b200.verify_batch(items)              <->  distaff::verify of every proof, all checked together on the GPU
@@ -13,7 +14,7 @@ Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.execute_programs(jobs)           <->  execute_batch for jobs of many programs in one call (trace_programs: the traces)
 The compute path is hand-written CUDA behind the C-ABI of include/distaff_gpu.h; there is no CPU fallback.
 """
-from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
+from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, prove_traces, prove_traces_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
                   merkle_build, hash_rows, hash64, find_pow_nonce, field_op, field_dot, eval_transitions, TraceReport, check_trace, check_traces,
                   check_traces_device, constraint_name, set_memory_limit, memory_usage, plan_prove, ProgramInputs, trace_batch, trace_shapes,
-                  execute_batch, trace_programs, execute_programs)
+                  execute_batch, trace_programs, execute_programs, group_traces)

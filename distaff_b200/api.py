@@ -195,6 +195,65 @@ def prove_batch_device(d_registers, count, width, length, ctx_depth, loop_depth,
     return _collect_batch(list(handles)[:count], list(status)[:count], stats)
 
 
+def prove_traces(traces, options=None):
+    """Proves many hostvm.ExecutionTraces of any register shapes and lengths in one dg_prove_traces call: every stage is launched once
+    per group of traces of one length, whatever their shapes (the constraint evaluation once per shape).  Returns what prove_batch
+    returns, in input order: a StarkProof byte-identical to prove() of the same trace (its stats: the whole call's), or the
+    backend.DgError of a trace that failed."""
+    options = options or ProofOptions()
+    opt = options._c()
+    traces = list(traces)
+    k = len(traces)
+    regs = [np.ascontiguousarray(tr.registers, dtype=np.uint64) for tr in traces]
+    cols = [(backend.vp * r.shape[0])(*[r[j].ctypes.data for j in range(r.shape[0])]) for r in regs]
+    ts = (backend.DgTrace * max(k, 1))(*[backend.DgTrace(cols[i], r.shape[0], r.shape[1], tr.ctx_depth, tr.loop_depth)
+                                        for i, (r, tr) in enumerate(zip(regs, traces))])
+    keep, (pin, nin, pout, nout) = _batch_io([tr.public_inputs for tr in traces], [tr.outputs for tr in traces])
+    handles = (backend.vp * max(k, 1))()
+    status = (ctypes.c_int * max(k, 1))()
+    st = backend.DgStats()
+    backend.check(backend.lib().dg_prove_traces(ts, k, pin, nin, pout, nout, ctypes.byref(opt), handles, status, ctypes.byref(st)))
+    del keep, regs, cols
+    return _collect_batch(list(handles)[:k], list(status)[:k], st)
+
+
+def prove_traces_device(d_registers, widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list, options=None):
+    """prove_traces for traces already in device memory: trace i's widths[i] x lengths[i] registers (column-major) at d_registers[i]
+    (backend.DeviceBuffer or raw pointer); the other arguments hold one entry per trace."""
+    options = options or ProofOptions()
+    k = len(d_registers)
+    assert all(len(a) == k for a in (widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list)), "one entry per trace"
+    ptrs = (backend.vp * max(k, 1))(*[d.ptr if isinstance(d, backend.DeviceBuffer) else int(d) for d in d_registers])
+    arr = lambda t, xs: (t * max(k, 1))(*[int(x) for x in xs])
+    opt = options._c()
+    keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
+    handles = (backend.vp * max(k, 1))()
+    status = (ctypes.c_int * max(k, 1))()
+    st = backend.DgStats()
+    backend.check(backend.lib().dg_prove_traces_device(ptrs, arr(backend.u32, widths), arr(backend.u64, lengths), arr(backend.u32, ctx_depths),
+                                                      arr(backend.u32, loop_depths), k, pin, nin, pout, nout, ctypes.byref(opt), handles, status,
+                                                      ctypes.byref(st)))
+    del keep
+    return _collect_batch(list(handles)[:k], list(status)[:k], st)
+
+
+def group_traces(lengths, widths, ctx_depths, loop_depths, footprints, budget, cap):
+    """dg_host_group_traces (no device): the groups prove_traces runs, as lists of trace indices in device order."""
+    k = len(lengths)
+    arr = lambda t, xs: (t * max(k, 1))(*[int(x) for x in xs])
+    order = (backend.u32 * max(k, 1))()
+    sizes = (backend.u32 * max(k, 1))()
+    n = backend.u32(0)
+    backend.check(backend.lib().dg_host_group_traces(k, arr(backend.u64, lengths), arr(backend.u32, widths), arr(backend.u32, ctx_depths),
+                                                    arr(backend.u32, loop_depths), arr(backend.u64, footprints), int(budget), int(cap), order,
+                                                    sizes, ctypes.byref(n)))
+    out, at = [], 0
+    for s in list(sizes)[:n.value]:
+        out.append(list(order)[at:at + s])
+        at += s
+    return out
+
+
 def verify(program_hash, public_inputs, outputs, proof):
     """distaff::verify (lib.rs:68-75 -> stark/verifier.rs:11-75) on the GPU.  Returns None when the proof is accepted, otherwise the
     reference's error string (what `Err(msg)` carries); raises DgError for bytes that are not a serialized StarkProof."""

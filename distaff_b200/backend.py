@@ -97,6 +97,11 @@ EXPORTS = {
                        ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_prove_batch_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
                               ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_prove_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                        ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_prove_traces_device": [ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32), u32,
+                               ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(DgOptions),
+                               ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
     "dg_trace_batch": [ctypes.POINTER(DgProgram), u32, ctypes.POINTER(DgProgramInputs), u64, ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp),
                        ctypes.POINTER(ctypes.c_int)],
@@ -143,6 +148,8 @@ EXPORTS = {
     "dg_comm_init": [ctypes.c_int, ctypes.c_int, vp],
     "dg_comm_finalize": [],
     "dg_host_shard_locate": [u64, ctypes.c_int, ctypes.c_int, ctypes.c_int, u64, ctypes.POINTER(ctypes.c_int64)],
+    "dg_host_group_traces": [u32, ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u64), u64, u32,
+                             ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32)],
     "dg_host_prng_vector": [vp, u64, vp],
     "dg_host_query_positions": [vp, u64, u32, u32, vp],
     "dg_host_blake3": [vp, ctypes.c_size_t, vp],

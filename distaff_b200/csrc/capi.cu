@@ -490,6 +490,62 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
                      *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
     });
 }
+// the checks dg_prove makes of a trace's shape, length and public inputs / outputs, on the host alone; a failure names the entry
+static void check_trace_entry(uint32_t i, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16,
+                              const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs) {
+    try {
+        DG_REQUIRE(width >= 16 && width < 128, "invalid trace");
+        DG_REQUIRE(length >= 16 && (length & (length - 1)) == 0 && length <= (1ULL << 30),
+                   "execution trace length must be a power of 2 and at least 16");
+        TraceShape::of_trace(width, ctx_depth, loop_depth);
+        const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
+        DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
+        DG_REQUIRE((ni == 0 || (inputs16 && inputs16[i])) && (no == 0 || (outputs16 && outputs16[i])), "null public inputs / outputs");
+    } catch (const Error &e) {
+        throw Error(e.code, "trace " + std::to_string(i) + ": " + e.what());
+    }
+}
+int dg_prove_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                    int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+        std::vector<TraceRef> refs(count);
+        for (uint32_t i = 0; i < count; i++) {
+            const dg_trace_t &t = traces[i];
+            check_trace_entry(i, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs);
+            DG_REQUIRE(t.columns, "trace " + std::to_string(i) + ": null register columns");
+            for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "trace " + std::to_string(i) + ": null register column");
+            refs[i].width = t.width; refs[i].length = t.length; refs[i].ctx_depth = t.ctx_depth; refs[i].loop_depth = t.loop_depth;
+            refs[i].host_cols = t.columns;
+        }
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+    });
+}
+int dg_prove_traces_device(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                           const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                           const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                           int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
+        std::vector<TraceRef> refs(count);
+        for (uint32_t i = 0; i < count; i++) {
+            check_trace_entry(i, width[i], length[i], ctx_depth[i], loop_depth[i], inputs16, n_inputs, outputs16, n_outputs);
+            DG_REQUIRE(d_registers[i], "trace " + std::to_string(i) + ": null registers");
+            refs[i].width = width[i]; refs[i].length = length[i]; refs[i].ctx_depth = ctx_depth[i]; refs[i].loop_depth = loop_depth[i];
+            refs[i].d_regs = (const fe *)d_registers[i];
+        }
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+    });
+}
 int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                     const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
                     uint32_t *step_masks) {
@@ -708,6 +764,30 @@ int dg_host_shard_locate(uint64_t n, int log_blk, int log_g, int is_node, uint64
         ShardGeom geo; geo.n = n; geo.log_blk = log_blk; geo.log_g = log_g;
         ShardLocation l = is_node ? geo.node(index) : geo.item(index);
         out[0] = l.owner; out[1] = l.kind; out[2] = (int64_t)l.index;
+    });
+}
+
+int dg_host_group_traces(uint32_t count, const uint64_t *lengths, const uint32_t *widths, const uint32_t *ctx_depths, const uint32_t *loop_depths,
+                         const uint64_t *footprints, uint64_t budget, uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out,
+                         uint32_t *n_groups) {
+    return guarded([&] {
+        DG_REQUIRE(lengths && widths && ctx_depths && loop_depths && footprints && order_out && group_sizes_out && n_groups, "null argument");
+        DG_REQUIRE(cap >= 1, "a group holds at least one trace");
+        uint32_t at = 0, groups = 0;
+        for (const std::vector<uint32_t> &idx : partition_by_length(std::vector<uint64_t>(lengths, lengths + count))) {
+            std::vector<uint32_t> w;
+            std::vector<size_t> foot;
+            for (uint32_t i : idx) { w.push_back(widths[i]); foot.push_back(footprints[i]); }
+            size_t first = 0;
+            for (uint32_t k : cut_groups(w, foot, budget, cap)) {
+                std::vector<RegisterShape> keys;
+                for (size_t m = first; m < first + k; m++) keys.push_back(RegisterShape{widths[idx[m]], ctx_depths[idx[m]], loop_depths[idx[m]]});
+                for (uint32_t m : shape_order(keys)) order_out[at++] = idx[first + m];
+                group_sizes_out[groups++] = k;
+                first += k;
+            }
+        }
+        *n_groups = groups;
     });
 }
 

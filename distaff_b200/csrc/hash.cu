@@ -15,13 +15,20 @@ namespace dg {
 
 // ---- trace rows -----------------------------------------------------------------------------------------------------
 // ext: [w][N] coset-major (N = rows of the slab: its cosets c0, c0 + 1, ... of n = 2^log_n rows each), leaves in logical row order: the row
-// of coset c at step k is leaf (k << log_blowup) + c; blockIdx.y = matrix of a batch, ext_stride elements / 2 leaf_stride uint4 apart
+// of coset c at step k is leaf (k << log_blowup) + c; blockIdx.y = matrix of a batch, ext_stride elements / 2 leaf_stride uint4 apart, or,
+// with a column table, matrix q = the cols[q].y columns from column cols[q].x on (a batch of several widths)
 __global__ void __launch_bounds__(256) hash_rows_kernel(const fe *__restrict__ ext, uint4 *__restrict__ leaves, int w, unsigned long long N,
                                                         int log_n, int log_blowup, uint32_t one, unsigned long long ext_stride, unsigned c0,
-                                                        unsigned long long leaf_stride) {
+                                                        unsigned long long leaf_stride, const uint2 *__restrict__ cols) {
     const unsigned long long p = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= N) return;
-    ext += blockIdx.y * ext_stride;
+    if (cols) {
+        const uint2 t = cols[blockIdx.y];
+        ext += (unsigned long long)t.x * N;
+        w = (int)t.y;
+    } else {
+        ext += blockIdx.y * ext_stride;
+    }
     leaves += blockIdx.y * 2 * leaf_stride;
     const unsigned long long n_mask = (1ULL << log_n) - 1ULL;
     const unsigned long long k = p & n_mask, c = (p >> log_n) + c0;
@@ -69,21 +76,23 @@ __global__ void __launch_bounds__(256) hash_rows_kernel(const fe *__restrict__ e
 }
 
 void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup, int batch, unsigned long long ext_stride, unsigned c0,
-                     unsigned nc, unsigned long long leaf_stride) {
+                     unsigned nc, unsigned long long leaf_stride, const uint2 *cols) {
     const unsigned long long all = 1ULL << (log_n + log_blowup);
     const unsigned long long rows = nc ? (unsigned long long)nc << log_n : all;
     DG_REQUIRE(batch >= 1 && batch <= 65535, "row hashing batch out of range");
     DG_REQUIRE(c0 + (rows >> log_n) <= (1ULL << log_blowup), "coset range out of bounds");
     const dim3 grid((unsigned)((rows + 255) / 256), (unsigned)batch);
     // FMA-pipe additions: trace tree 10.3 -> 8.8 ms at 2^25 rows x 26 columns (H100 SXM, 700 W)
-    hash_rows_kernel<<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, rows, log_n, log_blowup, 1u, ext_stride, c0, leaf_stride ? leaf_stride : all);
+    hash_rows_kernel<<<grid, 256, 0, c.stream>>>(ext, (uint4 *)leaves, w, rows, log_n, log_blowup, 1u, ext_stride, c0, leaf_stride ? leaf_stride : all,
+                                                 cols);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
 // rows of a plain column-major matrix (no coset permutation): physical position == logical row
 void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows) {
-    hash_rows_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c.stream>>>(cols, (uint4 *)digests, w, rows, 63, 0, 1u, 0, 0u, 0); c.launches++;
+    hash_rows_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, c.stream>>>(cols, (uint4 *)digests, w, rows, 63, 0, 1u, 0, 0u, 0, nullptr);
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 

@@ -241,14 +241,15 @@ void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, 
 // ---- evaluation of many polynomials at two points (DEEP values) -----------------------------------------------------------------------------
 // partial[(col*2 + p) * chunks + chunk] = sum_{k in chunk} poly[col][k] * x_p^k,  x_0 = z (table zt), x_1 = z*g (zt * gt)
 static const int EVAL_CHUNK = 4096;
-// columns of a batch: column col uses the table of its proof col / cols_per_proof, zt_stride_lo / zt_stride_hi elements apart
+// columns of a batch: column col uses the table of its proof col / cols_per_proof, or col_proof[col] (a batch of several widths),
+// zt_stride_lo / zt_stride_hi elements apart
 __global__ void __launch_bounds__(256) eval2_partial_kernel(const fe *__restrict__ polys, unsigned long long n, PowRef zt, TwiddleRef gt, fe *__restrict__ partial,
                                                             int two_points, unsigned cols_per_proof, unsigned long long zt_stride_lo,
-                                                            unsigned long long zt_stride_hi) {
+                                                            unsigned long long zt_stride_hi, const unsigned *__restrict__ col_proof) {
     __shared__ fe s_warp[2][8];
     const unsigned long long col = blockIdx.y, chunk = blockIdx.x, chunks = gridDim.x;
     const fe *p = polys + col * n;
-    const unsigned q = blockIdx.y / cols_per_proof;
+    const unsigned q = col_proof ? col_proof[blockIdx.y] : blockIdx.y / cols_per_proof;
     zt.lo += q * zt_stride_lo;
     zt.hi += q * zt_stride_hi;
     fe a0 = fe_make(0, 0), a1 = fe_make(0, 0);
@@ -289,12 +290,12 @@ __global__ void reduce_partials_kernel(const fe *__restrict__ partial, fe *__res
 }
 // out[col*2 + p] = poly_col(x_p)
 void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, const PowRef &zt, const TwiddleRef &gt, bool two_points, fe *out,
-                   int cols_per_proof, unsigned long long zt_stride_lo, unsigned long long zt_stride_hi) {
+                   int cols_per_proof, unsigned long long zt_stride_lo, unsigned long long zt_stride_hi, const unsigned *col_proof) {
     const unsigned chunks = (unsigned)((n + EVAL_CHUNK - 1) / EVAL_CHUNK);
     DG_REQUIRE(cols >= 1 && cols <= 65535 && cols_per_proof >= 1, "too many polynomials for one launch");
     DevBuf partial((size_t)cols * 2 * chunks * sizeof(fe));
     eval2_partial_kernel<<<dim3(chunks, cols), 256, 0, c.stream>>>(polys, n, zt, gt, partial.as<fe>(), two_points ? 1 : 0, (unsigned)cols_per_proof,
-                                                                   zt_stride_lo, zt_stride_hi); c.launches++;
+                                                                   zt_stride_lo, zt_stride_hi, col_proof); c.launches++;
     reduce_partials_kernel<<<cols * 2, 32, 0, c.stream>>>(partial.as<fe>(), out, chunks); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
@@ -304,21 +305,22 @@ void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, 
 // on the tiles y, y + gridDim.y, ... of ROW_TILE coefficients: the tile's powers x^k = w_N^(pos k mod N) go to shared memory once (two-level
 // table, one product each) and are shared by all w columns; warp v sums columns v, v + 8, ..., each lane ROW_TILE / 32 = 64 products
 // accumulated unreduced (288 bits, < 128 products) and reduced once, then the warp's lanes are added into the column's shared sum.
-// partial[(m w + j) * gridDim.y + y] = the block's sum for column j.
+// partial[(out + j) * gridDim.y + y] = the block's sum for column j, out = point m's first output (the widths of the points before it).
 static const int ROW_TILE = 2048, ROW_MAX_BLOCKS = 64;
-__global__ void __launch_bounds__(256) eval_rows_partial_kernel(const fe *__restrict__ polys, unsigned long long n, int w, const ulonglong2 *__restrict__ pts,
+__global__ void __launch_bounds__(256) eval_rows_partial_kernel(const fe *__restrict__ polys, unsigned long long n, const TraceRow *__restrict__ pts,
                                                                 TwiddleRef twN, fe *__restrict__ partial) {
     __shared__ fe s_pw[ROW_TILE];
     __shared__ fe s_acc[128];
-    const ulonglong2 pt = pts[blockIdx.x];                           // (proof, LDE position)
-    const fe *p = polys + pt.x * (unsigned long long)w * n;
+    const TraceRow pt = pts[blockIdx.x];
+    const int w = (int)pt.w;
+    const fe *p = polys + (unsigned long long)pt.col * n;
     const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int j = threadIdx.x; j < w; j += blockDim.x) s_acc[j] = fe_make(0, 0);
     const unsigned long long tile = n < (unsigned long long)ROW_TILE ? n : (unsigned long long)ROW_TILE;
     for (unsigned long long k0 = (unsigned long long)blockIdx.y * tile; k0 < n; k0 += (unsigned long long)gridDim.y * tile) {
         __syncthreads();                                             // the previous tile's powers are no longer read
         for (unsigned i = threadIdx.x; i < tile; i += blockDim.x) {
-            const unsigned e = (unsigned)((pt.y * (k0 + i)) & twN.mask);
+            const unsigned e = (unsigned)((pt.pos * (k0 + i)) & twN.mask);
             s_pw[i] = fe_mul(twN.lo[e & ((1u << twN.lo_bits) - 1u)], twN.hi[e >> twN.lo_bits]);
         }
         __syncthreads();
@@ -337,31 +339,43 @@ __global__ void __launch_bounds__(256) eval_rows_partial_kernel(const fe *__rest
         }
     }
     __syncthreads();
-    for (int j = threadIdx.x; j < w; j += blockDim.x) partial[((unsigned long long)blockIdx.x * w + j) * gridDim.y + blockIdx.y] = s_acc[j];
+    for (int j = threadIdx.x; j < w; j += blockDim.x) partial[(pt.out + j) * gridDim.y + blockIdx.y] = s_acc[j];
 }
-void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, int w, const std::vector<std::pair<uint32_t, uint64_t>> &points, int log_N, fe *out) {
-    DG_REQUIRE(w >= 1 && w <= 128 && !points.empty() && points.size() < (1ULL << 31), "opened-row evaluation out of range");
-    std::vector<ulonglong2> host(points.size());
-    for (size_t m = 0; m < points.size(); m++) host[m] = make_ulonglong2(points[m].first, points[m].second);
-    DevBuf d_pts(host.size() * sizeof(ulonglong2));
-    DG_CUDA(cudaMemcpyAsync(d_pts.p, host.data(), d_pts.bytes, cudaMemcpyHostToDevice, c.stream));
+void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, std::vector<TraceRow> points, int log_N, fe *out) {
+    DG_REQUIRE(!points.empty() && points.size() < (1ULL << 31), "opened-row evaluation out of range");
+    unsigned long long values = 0;
+    for (TraceRow &pt : points) {
+        DG_REQUIRE(pt.w >= 1 && pt.w <= 128, "opened-row evaluation out of range");
+        pt.out = values;
+        values += pt.w;
+    }
+    DevBuf d_pts(points.size() * sizeof(TraceRow));
+    DG_CUDA(cudaMemcpyAsync(d_pts.p, points.data(), d_pts.bytes, cudaMemcpyHostToDevice, c.stream));
     const unsigned tiles = (unsigned)((n + ROW_TILE - 1) / ROW_TILE), by = std::min<unsigned>(tiles, ROW_MAX_BLOCKS);
-    DevBuf partial(host.size() * w * by * sizeof(fe));
+    DevBuf partial(values * by * sizeof(fe));
     // the points run on x, so the blocks of one tile and many points are resident together and share its coefficients through L2
-    eval_rows_partial_kernel<<<dim3((unsigned)host.size(), by), 256, 0, c.stream>>>(polys, n, w, d_pts.as<ulonglong2>(), c.twiddle(log_N, false),
-                                                                                  partial.as<fe>()); c.launches++;
-    reduce_partials_kernel<<<(unsigned)(host.size() * w), 32, 0, c.stream>>>(partial.as<fe>(), out, by); c.launches++;
+    eval_rows_partial_kernel<<<dim3((unsigned)points.size(), by), 256, 0, c.stream>>>(polys, n, d_pts.as<TraceRow>(), c.twiddle(log_N, false),
+                                                                                    partial.as<fe>()); c.launches++;
+    reduce_partials_kernel<<<(unsigned)values, 32, 0, c.stream>>>(partial.as<fe>(), out, by); c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
 // ---- linear combinations ------------------------------------------------------------------------------------------------------------------
 // t1[k] = sum_i cc1[i] P_i[k],  t2[k] = sum_i cc2[i] P_i[k]
-// blockIdx.y = proof of a batch: polys w n, cc1 / cc2 cc_stride, t1 / t2 t_stride elements apart
+// blockIdx.y = proof of a batch: polys w n, cc1 / cc2 cc_stride, t1 / t2 t_stride elements apart; with a column table, proof q's
+// polynomials are the cols[q].y columns from column cols[q].x on
 __global__ void lincomb2_kernel(const fe *__restrict__ polys, unsigned long long n, int w, const fe *__restrict__ cc1, const fe *__restrict__ cc2,
-                                fe *__restrict__ t1, fe *__restrict__ t2, unsigned long long cc_stride, unsigned long long t_stride) {
+                                fe *__restrict__ t1, fe *__restrict__ t2, unsigned long long cc_stride, unsigned long long t_stride,
+                                const uint2 *__restrict__ cols) {
     unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
-    polys += blockIdx.y * (unsigned long long)w * n;
+    if (cols) {
+        const uint2 t = cols[blockIdx.y];
+        polys += (unsigned long long)t.x * n;
+        w = (int)t.y;
+    } else {
+        polys += blockIdx.y * (unsigned long long)w * n;
+    }
     cc1 += blockIdx.y * cc_stride; cc2 += blockIdx.y * cc_stride;
     t1 += blockIdx.y * t_stride; t2 += blockIdx.y * t_stride;
     // w < 128 products per sum: accumulated unreduced (288 bits), one reduction each (fp128.cuh: fe_wide)
@@ -374,9 +388,10 @@ __global__ void lincomb2_kernel(const fe *__restrict__ polys, unsigned long long
     t1[k] = DG_REDUCE_WIDE(a); t2[k] = DG_REDUCE_WIDE(b);
 }
 void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe *cc1, const fe *cc2, fe *t1, fe *t2, int batch,
-              unsigned long long cc_stride, unsigned long long t_stride) {
+              unsigned long long cc_stride, unsigned long long t_stride, const uint2 *cols) {
     DG_REQUIRE(batch >= 1 && batch <= 65535, "linear combination batch out of range");
-    lincomb2_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, w, cc1, cc2, t1, t2, cc_stride, t_stride);
+    lincomb2_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, w, cc1, cc2, t1, t2, cc_stride, t_stride,
+                                                                                             cols);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
@@ -388,18 +403,28 @@ void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe
 // whose coefficients are two linear combinations of the trace polynomials' coefficients: n*nb multiplications instead of 8n*nb.
 // coef = [a_init | b_init | a_final | b_final], nb entries each; ic / fc receive the 8n coefficients of the first / last step numerators.
 // blockIdx.y = proof of a batch: polys poly_stride, coef coef_stride, ic / fc out_stride elements apart, its constants
-// KiA, KiB, KfA, KfB = K[4 y .. 4 y + 4)
+// KiA, KiB, KfA, KfB = K[4 y .. 4 y + 4).  With a column table, proof q's polynomials are the cols[q].y columns from column cols[q].x on,
+// and only the first min(nb, cols[q].y) coefficients of each vector are read: the vectors are padded with zeros to the batch's largest
+// count nb, which a narrower proof's registers do not reach (a zero coefficient adds nothing to the unreduced sums)
 __global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned long long n, int nb, const fe *__restrict__ coef, unsigned long long adj,
                                        fe *__restrict__ ic, fe *__restrict__ fc, const fe *__restrict__ K, unsigned long long poly_stride,
-                                       unsigned long long coef_stride, unsigned long long out_stride) {
+                                       unsigned long long coef_stride, unsigned long long out_stride, const uint2 *__restrict__ cols) {
     const unsigned long long k = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n) return;
-    polys += blockIdx.y * poly_stride; coef += blockIdx.y * coef_stride;
+    int regs = nb;
+    if (cols) {
+        const uint2 t = cols[blockIdx.y];
+        polys += (unsigned long long)t.x * n;
+        regs = min(nb, (int)t.y);
+    } else {
+        polys += blockIdx.y * poly_stride;
+    }
+    coef += blockIdx.y * coef_stride;
     ic += blockIdx.y * out_stride; fc += blockIdx.y * out_stride;
     const fe KiA = K[4 * blockIdx.y], KiB = K[4 * blockIdx.y + 1], KfA = K[4 * blockIdx.y + 2], KfB = K[4 * blockIdx.y + 3];
     // nb < 128 products per sum: accumulated unreduced (288 bits), one reduction each
     fe_wide wa, wb, wc, wd;
-    for (int j = 0; j < nb; j++) {
+    for (int j = 0; j < regs; j++) {
         const fe v = polys[(unsigned long long)j * n + k];
         if (j == 0) {
             wide_set(wa, DG_MUL_WIDE(v, coef[0])); wide_set(wb, DG_MUL_WIDE(v, coef[nb])); wide_set(wc, DG_MUL_WIDE(v, coef[2 * nb]));
@@ -419,10 +444,10 @@ __global__ void boundary_coeffs_kernel(const fe *__restrict__ polys, unsigned lo
         if (q < adj || q >= adj + n) { ic[q] = zero; fc[q] = zero; }
 }
 void boundary_coeffs(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
-                     unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride) {
+                     unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride, const uint2 *cols) {
     DG_REQUIRE(batch >= 1 && batch <= 65535, "boundary batch out of range");
     boundary_coeffs_kernel<<<dim3((unsigned)((n + 255) / 256), (unsigned)batch), 256, 0, c.stream>>>(polys, n, nb, coef, 6 * n + 2, ic, fc, K, poly_stride,
-                                                                                                   coef_stride, out_stride);
+                                                                                                   coef_stride, out_stride, cols);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }

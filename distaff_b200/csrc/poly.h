@@ -26,30 +26,37 @@ void syn_div(Context &c, int batch, const fe *in, unsigned long long in_stride, 
 // batch > 1: a, add0, add1 of vector q at q * in_stride, out at q * out_stride; scratch holds batch * len elements
 void syn_div_expanded_sum(Context &c, const fe *a, fe *scratch, const fe *add0, const fe *add1, fe *out, unsigned long long n, unsigned long long len, fe e,
                           int batch = 1, unsigned long long in_stride = 0, unsigned long long out_stride = 0);
-// cols_per_proof < cols: the columns of several proofs, proof q's powers of z at zt moved by q * (lo, hi) strides
+// cols_per_proof < cols: the columns of several proofs, proof q's powers of z at zt moved by q * (lo, hi) strides; col_proof (device, one
+// entry per column, may be null) names each column's proof instead, for proofs of several widths
 void eval_polys_at(Context &c, const fe *polys, unsigned long long n, int cols, const PowRef &zt, const TwiddleRef &gt, bool two_points, fe *out,
-                   int cols_per_proof = 1 << 30, unsigned long long zt_stride_lo = 0, unsigned long long zt_stride_hi = 0);
-// rows of the trace extension computed from the trace polynomials: out[m w + j] = P_j(w_N^pos) of proof q for points[m] = (q, pos), with
-// proof q's w polynomials of n coefficients at polys + q w n; one launch for all points (plus the reduction of the tile sums)
-void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, int w, const std::vector<std::pair<uint32_t, uint64_t>> &points, int log_N, fe *out);
-// `batch` proofs: polys, coef, ic / fc of proof q at q * the strides, its constants KiA, KiB, KfA, KfB = K[4q .. 4q + 4) on the device
+                   int cols_per_proof = 1 << 30, unsigned long long zt_stride_lo = 0, unsigned long long zt_stride_hi = 0,
+                   const unsigned *col_proof = nullptr);
+// one opened row computed from the trace polynomials: the w columns from column `col` on, at LDE position pos (out: set by eval_trace_rows)
+struct TraceRow { unsigned long long pos, out; unsigned col, w; };
+// rows of the trace extension computed from the trace polynomials (column stride n): point m's values P_j(w_N^pos), j < w, at out + the
+// widths of the points before it; one launch for all points (plus the reduction of the tile sums)
+void eval_trace_rows(Context &c, const fe *polys, unsigned long long n, std::vector<TraceRow> points, int log_N, fe *out);
+// `batch` proofs: polys, coef, ic / fc of proof q at q * the strides, its constants KiA, KiB, KfA, KfB = K[4q .. 4q + 4) on the device.
+// cols (device, may be null): proofs of several widths, proof q's polynomials the cols[q].y columns from column cols[q].x on
 void boundary_coeffs(Context &c, int batch, const fe *polys, unsigned long long poly_stride, unsigned long long n, int nb, const fe *coef,
-                     unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride);
+                     unsigned long long coef_stride, const fe *K, fe *ic, fe *fc, unsigned long long out_stride, const uint2 *cols = nullptr);
 // finishes the coset-by-coset interpolation of 8n evaluations: b = [8][n] size-n inverse transforms of the cosets -> 8n coefficients;
 // batch > 1: vector q at b + q b_stride, out + q out_stride
 void coset_interp_finish(Context &c, const fe *b, fe *out, int log_n, int batch = 1, unsigned long long b_stride = 0, unsigned long long out_stride = 0);
-// batch > 1: proof q's polynomials w n elements after proof q - 1's, its coefficients at q cc_stride, outputs at q t_stride
+// batch > 1: proof q's polynomials w n elements after proof q - 1's (or, with cols, the cols[q].y columns from column cols[q].x on), its
+// coefficients at q cc_stride, outputs at q t_stride
 void lincomb2(Context &c, const fe *polys, unsigned long long n, int w, const fe *cc1, const fe *cc2, fe *t1, fe *t2, int batch = 1,
-              unsigned long long cc_stride = 0, unsigned long long t_stride = 0);
+              unsigned long long cc_stride = 0, unsigned long long t_stride = 0, const uint2 *cols = nullptr);
 // `batch` proofs: t1q / t2q at q t_stride, cq / comp at q len, k1, k2, kc = ks[3q .. 3q + 3) on the device
 void compose(Context &c, int batch, const fe *t1q, const fe *t2q, unsigned long long t_stride, const fe *cq, fe *comp, unsigned long long n,
              unsigned long long len, unsigned long long inc, const fe *ks);
 
 // ---- hashing (hash.cu) ----
 // ext: the cosets [c0, c0 + nc) of every column ([w][nc][n], column stride nc n; nc = 0: all 2^log_blowup); the row of coset c at step k
-// is leaf (k << log_blowup) + c.  batch > 1: `batch` matrices ext_stride elements apart, their leaves leaf_stride digests apart (0: N)
+// is leaf (k << log_blowup) + c.  batch > 1: `batch` matrices ext_stride elements apart, their leaves leaf_stride digests apart (0: N);
+// cols (device, may be null): matrices of several widths, matrix q the cols[q].y columns from column cols[q].x on (w, ext_stride unused)
 void hash_trace_rows(Context &c, const fe *ext, void *leaves, int w, int log_n, int log_blowup, int batch = 1, unsigned long long ext_stride = 0,
-                     unsigned c0 = 0, unsigned nc = 0, unsigned long long leaf_stride = 0);
+                     unsigned c0 = 0, unsigned nc = 0, unsigned long long leaf_stride = 0, const uint2 *cols = nullptr);
 // digests of the rows of a plain column-major [w][rows] matrix
 void hash_rows_plain(Context &c, const fe *cols, void *digests, int w, unsigned long long rows);
 void hash64_contiguous(Context &c, const void *in, void *out, unsigned long long count);

@@ -7,6 +7,7 @@
 #include "host_fs.h"
 #include "poly.h"
 #include "shard.h"
+#include <algorithm>
 #include <array>
 #include <atomic>
 #include <memory>
@@ -260,33 +261,54 @@ struct OpenPlan {
 
 }  // namespace
 
-// Proves K traces of one shape (K == 1: dg_prove / dg_prove_device).  Every device buffer is proof-major ([K][...] with the single-proof
-// layout inside), so the transforms run once over the K proofs' columns, and each host round trip (violation flags, roots, DEEP values,
-// FRI roots, PoW, openings) moves the values of all K proofs at once.
-// d_regs: register traces in device memory, [K][w][n]; when `host_cols` (K * w column pointers) is given they are not there yet: column
-// chunks are uploaded on the copy stream while the previous chunk is being interpolated and extended (the upload hides behind the LDE).
-// chunk (one GPU): cosets of the trace extension held at a time (ProvePlan).  The full layout (chunk = b) keeps the whole extension; the
-// evaluation-coset layout (chunk < b) extends and hashes chunk cosets at a time and keeps only the 8 cosets stage 3 reads.
-static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, int K, uint32_t width, uint64_t length, uint32_t ctx_depth,
-                       uint32_t loop_depth, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats, unsigned chunk) {
+// Proves K traces of one length (K == 1: dg_prove / dg_prove_device).  Every device buffer is proof-major: the registers, polynomials and
+// trace extension are sum(w_p) columns, proof p's w_p columns from column col0[p] on, and every per-proof vector ([K][...]) has the
+// single-proof layout inside.  So the transforms run once over all the proofs' columns, and each host round trip (violation flags, roots,
+// DEEP values, FRI roots, PoW, openings) moves the values of all K proofs at once.  shapes[p] is proof p's register shape; proofs of one
+// shape are adjacent, so that the constraint kernel runs once per shape over proofs at a uniform stride (a one-shape batch: one launch).
+// order: the proofs in the order their Fiat-Shamir draws are made (the RNG callbacks see them in that order, stage by stage).
+// d_regs: register traces in device memory, [sum w_p][n]; when `host_cols` (sum w_p column pointers) is given they are not there yet:
+// column chunks are uploaded on the copy stream while the previous chunk is being interpolated and extended (the upload hides behind the
+// LDE).  chunk (one GPU): cosets of the trace extension held at a time (ProvePlan).  The full layout (chunk = b) keeps the whole extension;
+// the evaluation-coset layout (chunk < b) extends and hashes chunk cosets at a time and keeps only the 8 cosets stage 3 reads.
+static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, const std::vector<RegisterShape> &regs_shape, uint64_t length,
+                       const std::vector<int> &order, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats,
+                       unsigned chunk) {
     // ---- argument checks (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) -----------------------------------------------
     const uint64_t n = length, b = opt.extension_factor;
-    DG_REQUIRE(K >= 1 && (int)ps.size() == K, "batch must hold at least one trace");
-    DG_REQUIRE((uint64_t)K * width <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
+    const int K = (int)ps.size();
+    DG_REQUIRE(K >= 1 && regs_shape.size() == ps.size() && order.size() == ps.size(), "batch must hold at least one trace");
+    size_t W = 0;                                              // columns of the whole batch
+    for (const RegisterShape &r : regs_shape) W += r.width;
+    DG_REQUIRE(W <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
     DG_REQUIRE(opt.hash_id == 0, "unsupported hash function (only blake3 is serialisable, options.rs:107)");
     require_extension_factor(b);
     DG_REQUIRE(opt.num_queries > 0 && opt.num_queries <= 128, "num_queries must be in 1..128");
     DG_REQUIRE(opt.grinding_factor <= 32, "grinding factor cannot be greater than 32");
     DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    const TraceShape shape = TraceShape::of_trace(width, ctx_depth, loop_depth);
-    const int w = shape.w, log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
+    std::vector<TraceShape> shapes;
+    for (const RegisterShape &r : regs_shape) shapes.push_back(TraceShape::of_trace(r.width, r.ctx_depth, r.loop_depth));
+    // the column table: proof p's registers are the columns [col0[p], col0[p] + w_p) of the batch
+    std::vector<uint32_t> col0(K + 1, 0);
+    int wmax = 0, Tmax = 0;
+    for (int p = 0; p < K; p++) {
+        col0[p + 1] = col0[p] + shapes[p].w;
+        wmax = std::max(wmax, shapes[p].w);
+        Tmax = std::max(Tmax, shapes[p].T);
+    }
+    const int log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
     DG_REQUIRE(log_N <= 30, "LDE domain too large");
     const uint64_t N = n * b, E = n * 8;
-    for (auto &s : ps) {                      // what the call fixes in every proof: the register shape and the options (blake3)
-        TraceInfo &t = s.stark.trace_info;
-        t.ctx_depth = (uint8_t)ctx_depth; t.loop_depth = (uint8_t)loop_depth; t.stack_depth = (uint8_t)shape.stack_depth;
-        s.stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opt.num_queries, (uint8_t)opt.grinding_factor, 0};
+    for (int p = 0; p < K; p++) {             // what the call fixes in every proof: the register shape and the options (blake3)
+        TraceInfo &t = ps[p].stark.trace_info;
+        t.ctx_depth = (uint8_t)shapes[p].ctx_depth; t.loop_depth = (uint8_t)shapes[p].loop_depth; t.stack_depth = (uint8_t)shapes[p].stack_depth;
+        ps[p].stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opt.num_queries, (uint8_t)opt.grinding_factor, 0};
     }
+    // runs of proofs of one shape: [shape_first[s], shape_first[s + 1])
+    std::vector<int> shape_first = {0};
+    for (int p = 1; p < K; p++)
+        if (!(regs_shape[p] == regs_shape[p - 1])) shape_first.push_back(p);
+    shape_first.push_back(K);
     auto any_live = [&] { for (auto &s : ps) if (s.live) return true; return false; };
 
     ArenaScope arena_scope;                   // all DevBufs below come from the per-proof arena (no driver allocation inside a proof)
@@ -300,6 +322,19 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         ~DeviceStateReset() { for (auto &s : ps) { s.t_tree = ShardedTree(); s.c_tree = ShardedTree(); s.layers.clear(); } }
     } state_reset{ps};
     const unsigned long long launches0 = c.launches;
+    // the column table on the device: [K] (first column, width) of every proof, then [W] the proof of every column
+    DevBuf d_table((2 * K + W) * 4);
+    {
+        std::vector<uint32_t> table(2 * K + W);
+        for (int p = 0; p < K; p++) {
+            table[2 * p] = col0[p];
+            table[2 * p + 1] = (uint32_t)shapes[p].w;
+            for (uint32_t j = col0[p]; j < col0[p + 1]; j++) table[2 * K + j] = (uint32_t)p;
+        }
+        h2d(c, d_table.p, table.data(), table.size() * 4);
+    }
+    const uint2 *d_cols = d_table.as<uint2>();
+    const unsigned *d_col_proof = d_table.as<unsigned>() + 2 * K;
 
     // ---- sharding: rank g owns the LDE cosets [c0, c0 + nc) of every column (world == 1: all of them) ------------------------------
     const int G = c.world, g = c.rank;
@@ -309,7 +344,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     const int log_nc = log_b - log_g;
     const uint64_t nc = 1ULL << log_nc, N_loc = n * nc;
     const unsigned c0 = (unsigned)(g * nc);
-    const size_t W = (size_t)K * w;                            // columns of the whole batch
+    const int w = shapes[0].w;                                 // several GPUs: the width of the one proof
 
     // ---- 1: extend execution trace ---------------------------------------------------------------------------------------------------
     clk.mark(0);
@@ -321,9 +356,9 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     const int cpr = (w + G - 1) / G;                           // slot size of the gather = largest share
     auto col_count = [&](int r) { return w / G + (r < w % G ? 1 : 0); };
     auto col_start = [&](int r) { return r * (w / G) + std::min(r, w % G); };
-    // Layout of the extension.  ext holds `chunk` cosets of every column at a time ([K][w][chunk][n]).  The retained slab holds the cosets
+    // Layout of the extension.  ext holds `chunk` cosets of every column at a time ([W][chunk][n]).  The retained slab holds the cosets
     // stage 3 reads: in the full layout the whole extension (slab = ext), in the evaluation-coset layout the 8 cosets c = 0 (mod b / 8),
-    // [K][w][8][n].  An opened row outside the retained cosets is computed from the trace polynomials in stage 9.
+    // [W][8][n].  An opened row outside the retained cosets is computed from the trace polynomials in stage 9.
     if (G > 1 || chunk == 0 || chunk > nc) chunk = (unsigned)nc;
     DG_REQUIRE((chunk & (chunk - 1)) == 0, "coset chunk must be a power of 2");
     const bool full = chunk == nc;
@@ -336,7 +371,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     DevBuf t_leaves((size_t)K * N_loc * 32), t_nodes;
     // rows of the chunk at cc: leaves (k << log_b) + c of every proof; then its retained cosets into the slab
     auto hash_chunk = [&](unsigned cc) {
-        hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, (size_t)w * ext_col, cc, chunk, N_loc);   // local rows, [k][c - c0], per proof
+        hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, 0, cc, chunk, N_loc, d_cols);   // local rows, [k][c - c0], per proof
         if (full) return;
         for (unsigned cs = cc; cs < cc + chunk; cs++)
             if (cs % rstep == 0)
@@ -344,7 +379,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
                                           cudaMemcpyDeviceToDevice, c.stream));
     };
     if (G == 1) {
-        // the K proofs' registers are K * w columns of one batch, interpolated in column chunks: a host trace is uploaded in chunks of
+        // the K proofs' registers are the W columns of one batch, interpolated in column chunks: a host trace is uploaded in chunks of
         // ~64 MB, but a short ramp first (1, 2 columns), so that the first transform starts after one column's worth of copying; every
         // column chunk is extended on the first coset chunk as soon as it has been interpolated
         std::vector<int> bounds = {0};
@@ -410,7 +445,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         cudaEventDestroy(ev_own);
         cudaEventDestroy(ev_all);
     }
-    auto slab_of = [&](int p) { return slab + (size_t)p * w * slab_col; };
+    auto slab_of = [&](int p) { return slab + (size_t)col0[p] * slab_col; };
 
     // ---- 2: trace Merkle tree ----------------------------------------------------------------------------------------------------------
     clk.mark(1);
@@ -440,30 +475,34 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     std::vector<fe> last_rows((size_t)3 * K);      // op_counter and program hash of the last trace step of every proof (evaluator.rs:73-74)
     if (host_cols) {
         for (int p = 0; p < K; p++)
-            for (int j = 0; j < 3; j++) memcpy(&last_rows[3 * p + j], host_cols[(size_t)p * w + j] + (n - 1) * 16, 16);
+            for (int j = 0; j < 3; j++) memcpy(&last_rows[3 * p + j], host_cols[col0[p] + j] + (n - 1) * 16, 16);
     } else {
         DevBuf d_last((size_t)48 * K);
-        for (int j = 0; j < 3; j++)
-            DG_CUDA(cudaMemcpy2DAsync((uint8_t *)d_last.p + 16 * j, 48, d_regs + (size_t)j * n + (n - 1), (size_t)w * n * 16, 16, K,
-                                      cudaMemcpyDeviceToDevice, c.stream));
+        for (size_t s = 0; s + 1 < shape_first.size(); s++) {          // the proofs of one shape are w n elements apart
+            const int p0 = shape_first[s], k = shape_first[s + 1] - p0;
+            for (int j = 0; j < 3; j++)
+                DG_CUDA(cudaMemcpy2DAsync((uint8_t *)d_last.p + 48 * p0 + 16 * j, 48, d_regs + (size_t)(col0[p0] + j) * n + (n - 1),
+                                          (size_t)shapes[p0].w * n * 16, 16, k, cudaMemcpyDeviceToDevice, c.stream));
+        }
         d2h(c, last_rows.data(), d_last.p, (size_t)48 * K);
     }
     DevBuf d_coef, d_violation((size_t)4 * K);
     // per proof [coefA | coefB | bAi | bBi | bAf | bBf], coef_stride elements apart, then the boundary constants [K][KiA, KiB, KfA, KfB].
-    // The transition coefficients have the same count T for every proof of a shape; the boundary vectors have one entry per register that
-    // carries a boundary constraint, which depends on the number of public inputs / outputs: they are padded with zero coefficients to
-    // the largest count nbm (a zero coefficient adds nothing to the boundary numerators).
-    const size_t T = shape.T;
+    // The transition coefficients of a proof are T of its shape: coefA and coefB are padded to the batch's largest count Tmax.  The
+    // boundary vectors have one entry per register that carries a boundary constraint, which depends on the shape and on the number of
+    // public inputs / outputs: they are padded with zero coefficients to the largest count nbm (a zero coefficient adds nothing to the
+    // boundary numerators).
+    const size_t T = Tmax;
     size_t coef_stride = 0, nbm = 0;
     {
-        for (int p = 0; p < K; p++) {
+        for (int p : order) {
             ProofState &s = ps[p];
             s.stark.trace_info.op_count = (uint32_t)last_rows[3 * p].lo;       // op_count as u32 (proof.rs:62)
             const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
-            s.cc = fs::draw_constraint_coefficients(s.stark.trace_root.data(), shape, s.inputs, s.outputs, last_rows[3 * p], program_hash);
+            s.cc = fs::draw_constraint_coefficients(s.stark.trace_root.data(), shapes[p], s.inputs, s.outputs, last_rows[3 * p], program_hash);
+            DG_REQUIRE(s.cc.bAi.size() <= (size_t)shapes[p].w, "more boundary registers than registers");
             nbm = std::max(nbm, s.cc.bAi.size());
         }
-        DG_REQUIRE(nbm <= (size_t)w, "more boundary registers than registers");
         coef_stride = 2 * T + 4 * nbm;
         std::vector<fe> pack(coef_stride * K + 4 * K, fe_make(0, 0));
         for (int p = 0; p < K; p++) {
@@ -488,21 +527,25 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         const uint64_t E_loc = n * num_c8;
         DevBuf evals_loc((size_t)K * E_loc * 16), gathered;
         if (G > 1) gathered.alloc(E * 16);
-        AirParams P = shape.air_params(n);
-        // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
-        // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
-        P.log_blowup = full ? log_b : 3;
-        P.ext = slab; P.col_stride = slab_col;
-        P.c8_base = g * num_c8; P.num_c8 = num_c8;
-        P.t_ev = evals_loc.as<fe>();
-        P.periodic = periodic_table(c);
-        const fe *base = d_coef.as<fe>();
-        P.coefA = base; P.coefB = base + T;
-        P.twN = c.twiddle(full ? log_N : log_n + 3, false);
-        P.violation = d_violation.as<unsigned>();
-        P.ext_stride = (size_t)w * slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
-    sub.mark("3.setup");
-        launch_constraint_eval(c, P, K);
+        // one launch per register shape, over that shape's proofs (adjacent, so at uniform strides)
+        for (size_t s = 0; s + 1 < shape_first.size(); s++) {
+            const int p0 = shape_first[s], k = shape_first[s + 1] - p0;
+            AirParams P = shapes[p0].air_params(n);
+            // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
+            // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
+            P.log_blowup = full ? log_b : 3;
+            P.ext = slab_of(p0); P.col_stride = slab_col;
+            P.c8_base = g * num_c8; P.num_c8 = num_c8;
+            P.t_ev = evals_loc.as<fe>() + (size_t)p0 * E_loc;
+            P.periodic = periodic_table(c);
+            const fe *base = d_coef.as<fe>() + (size_t)p0 * coef_stride;
+            P.coefA = base; P.coefB = base + T;
+            P.twN = c.twiddle(full ? log_N : log_n + 3, false);
+            P.violation = d_violation.as<unsigned>() + p0;
+            P.ext_stride = (size_t)shapes[p0].w * slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
+            if (s == 0) sub.mark("3.setup");
+            launch_constraint_eval(c, P, k);
+        }
     sub.mark("3.eval");
         comm_all_reduce_max_u32(c, d_violation.as<unsigned>(), 1);
         std::vector<unsigned> violation(K);
@@ -520,8 +563,8 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     sub.mark("3.intt+gather");
         coset_interp_finish(c, G > 1 ? gathered.as<fe>() : evals_loc.as<fe>(), evals.as<fe>() + 2 * E, log_n, K, E_loc, 3 * E);
         // boundary constraints (evaluator.rs:181-326), directly as the 8n coefficients the reference obtains by interpolation
-        boundary_coeffs(c, K, polys.as<fe>(), (size_t)w * n, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
-                        evals.as<fe>(), evals.as<fe>() + E, 3 * E);
+        boundary_coeffs(c, K, polys.as<fe>(), 0, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
+                        evals.as<fe>(), evals.as<fe>() + E, 3 * E, d_cols);
     }
     if (K == 1) debug_dump(c, "t_coeffs", evals.as<fe>() + 2 * E, E * 16);
 
@@ -586,17 +629,18 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         TwiddleRef g_t = c.twiddle(log_n, false);
         // trace polynomials at z and z*g: every rank evaluates its own columns (the split of stage 1); slots of 2 cpr values are gathered.
-        // d_deep = [K][2 wp] trace values, then [K][2] values of the constraint polynomial at z
-        const int wp = cpr * G;
-        DevBuf d_deep((size_t)K * (2 * wp + 2) * 16);
-        fe *deep_c = d_deep.as<fe>() + (size_t)K * 2 * wp;
+        // d_deep = 2 trace values per column (one GPU: proof p's from column col0[p] on; several: G slots of cpr columns), then [K][2]
+        // values of the constraint polynomial at z
+        const size_t deep_cols = G == 1 ? W : (size_t)cpr * G;
+        DevBuf d_deep((2 * deep_cols + 2 * K) * 16);
+        fe *deep_c = d_deep.as<fe>() + 2 * deep_cols;
         DG_CUDA(cudaMemsetAsync(d_deep.p, 0, d_deep.bytes, c.stream));
         // powers of z, 1/z, z g, 1/(z g) of every proof: four batched tables from one upload of the (base, step) pairs, [table][proof][2]
         std::vector<fe> base_step((size_t)8 * K, fe_make(0, 0));
-        for (int p = 0; p < K; p++) {
+        for (int p : order) {
             ProofState &s = ps[p];
             if (!s.live) continue;
-            s.dc = fs::draw_composition_coefficients(s.stark.constraint_root.data(), w);
+            s.dc = fs::draw_composition_coefficients(s.stark.constraint_root.data(), shapes[p].w);
             const fe z = s.dc.z, zg = fe_mul(z, root_n);
             const fe bases[4] = {z, host_inv(z), zg, host_inv(zg)};
             for (int t = 0; t < 4; t++) {
@@ -609,47 +653,50 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         const fe *bs = d_base_step.as<fe>();
         PowTables z_t(c, bs, K, E + 1), zi_t(c, bs + 2 * K, K, E + 1), zg_t(c, bs + 4 * K, K, n + 1), zgi_t(c, bs + 6 * K, K, n + 1);
         if (G == 1) {
-            eval_polys_at(c, polys.as<fe>(), n, K * w, z_t.ref(0), g_t, true, d_deep.as<fe>(), w, z_t.lo_n, z_t.hi_n);
+            eval_polys_at(c, polys.as<fe>(), n, (int)W, z_t.ref(0), g_t, true, d_deep.as<fe>(), 1 << 30, z_t.lo_n, z_t.hi_n, d_col_proof);
         } else {
             const int j0 = col_start(g), mine = col_count(g);
             if (mine > 0) eval_polys_at(c, polys.as<fe>() + (size_t)j0 * n, n, mine, z_t.ref(0), g_t, true, d_deep.as<fe>() + (size_t)2 * g * cpr);
             comm_all_gather(c, d_deep.as<fe>() + (size_t)2 * g * cpr, d_deep.p, (size_t)2 * cpr * 16);
         }
         eval_polys_at(c, combined.as<fe>(), E, K, z_t.ref(0), g_t, false, deep_c, 1, z_t.lo_n, z_t.hi_n);
-        std::vector<fe> deep_slots((size_t)K * (2 * wp + 2));
+        std::vector<fe> deep_slots(2 * deep_cols + 2 * K);
         d2h(c, deep_slots.data(), d_deep.p, deep_slots.size() * 16);
     sub.mark("6.deep_values");
-        // one upload: [K][2w] coefficients of the trace combinations | sub0 of the three divisions [3][K] | compose's k1, k2, kc [K][3]
-        std::vector<fe> pack((size_t)K * (2 * w + 6), fe_make(0, 0));
-        fe *ccs = pack.data(), *subs = ccs + (size_t)K * 2 * w, *ks = subs + (size_t)3 * K;
+        // one upload: [K][2 wmax] coefficients of the trace combinations (proof p's trace1 | trace2 at p 2 wmax, p 2 wmax + wmax) | sub0
+        // of the three divisions [3][K] | compose's k1, k2, kc [K][3]
+        std::vector<fe> pack((size_t)K * (2 * wmax + 6), fe_make(0, 0));
+        fe *ccs = pack.data(), *subs = ccs + (size_t)K * 2 * wmax, *ks = subs + (size_t)3 * K;
         for (int p = 0; p < K; p++) {
             ProofState &s = ps[p];
             if (!s.live) continue;
-            const fe *slots = deep_slots.data() + (size_t)p * 2 * wp;
-            std::vector<fe> deep(2 * w);
+            const int wq = shapes[p].w;
+            const fe *slots = deep_slots.data() + 2 * (size_t)col0[p];           // several GPUs: K == 1, col0[0] == 0
+            std::vector<fe> deep(2 * wq);
             for (int r = 0; r < G; r++)
-                for (int o = 0; o < col_count(r); o++) {
-                    deep[2 * (col_start(r) + o)] = slots[2 * (r * cpr + o)];
-                    deep[2 * (col_start(r) + o) + 1] = slots[2 * (r * cpr + o) + 1];
+                for (int o = 0; o < (G == 1 ? wq : col_count(r)); o++) {
+                    const int from = G == 1 ? o : r * cpr + o, to = G == 1 ? o : col_start(r) + o;
+                    deep[2 * to] = slots[2 * from];
+                    deep[2 * to + 1] = slots[2 * from + 1];
                 }
             std::vector<fe> &z1 = s.stark.trace_at_z1, &z2 = s.stark.trace_at_z2;
-            z1.resize(w); z2.resize(w);
+            z1.resize(wq); z2.resize(wq);
             fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
-            for (int i = 0; i < w; i++) {
+            for (int i = 0; i < wq; i++) {
                 z1[i] = deep[2 * i]; z2[i] = deep[2 * i + 1];
                 sub1 = fe_add(sub1, fe_mul(z1[i], s.dc.trace1[i]));
                 sub2 = fe_add(sub2, fe_mul(z2[i], s.dc.trace2[i]));
             }
-            subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[(size_t)K * 2 * wp + 2 * p];
-            std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + w, ccs + (size_t)p * 2 * w);
-            std::copy(s.dc.trace2.begin(), s.dc.trace2.begin() + w, ccs + (size_t)p * 2 * w + w);
+            subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[2 * deep_cols + 2 * p];
+            std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + wq, ccs + (size_t)p * 2 * wmax);
+            std::copy(s.dc.trace2.begin(), s.dc.trace2.begin() + wq, ccs + (size_t)p * 2 * wmax + wmax);
             ks[3 * p] = s.dc.t1_degree; ks[3 * p + 1] = s.dc.t2_degree; ks[3 * p + 2] = s.dc.constraints;
         }
         DevBuf d_pack(pack.size() * 16), t12((size_t)K * 2 * n * 16);
         h2d(c, d_pack.p, pack.data(), pack.size() * 16);
-        const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * w, *d_ks = d_subs + (size_t)3 * K;
+        const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * wmax, *d_ks = d_subs + (size_t)3 * K;
         fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
-        lincomb2(c, polys.as<fe>(), n, w, d_cc, d_cc + w, t1, t2, K, 2 * w, 2 * n);
+        lincomb2(c, polys.as<fe>(), n, wmax, d_cc, d_cc + wmax, t1, t2, K, 2 * wmax, 2 * n, d_cols);
         syn_div(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs);
         //                                                                                                   (T1(x) - T1(z)) / (x - z)
         syn_div(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K);
@@ -698,7 +745,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             std::vector<uint8_t> r((size_t)32 * K);
             d2h(c, r.data(), root_slots(li), r.size());
             std::vector<fe> alphas(K, fe_make(0, 0));
-            for (int p = 0; p < K; p++)
+            for (int p : order)
                 if (ps[p].live) alphas[p] = fs::prng_vector(r.data() + 32 * p, 1)[0];   // field::prng(seed) = first draw of the generator (field.rs:264-269)
             DG_CUDA(cudaMemcpyAsync(alpha_dev(li), alphas.data(), (size_t)16 * K, cudaMemcpyHostToDevice, c.stream));
             DG_CUDA(cudaStreamSynchronize(c.stream));
@@ -773,7 +820,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         std::vector<std::array<uint8_t, 32>> seeds;
         std::vector<int> who;
-        for (int p = 0; p < K; p++) {
+        for (int p : order) {
             if (!ps[p].live) continue;
             const FriProof &f = ps[p].stark.degree_proof;
             std::vector<uint8_t> roots;
@@ -816,24 +863,28 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         return v;
     };
     // opened trace rows outside the retained cosets (evaluation-coset layout): the trace polynomials at w_N^pos, all proofs in one launch,
-    // into d_rows ([m][w], m = computed row of the batch in proof and query order)
+    // into d_rows (the w_p values of each computed row of the batch, rows in proof and query order)
     auto retained = [&](uint64_t pos) { return ((pos & (b - 1)) & (rstep - 1)) == 0; };
     DevBuf d_rows;
-    std::vector<size_t> first_row(K, 0);
+    std::vector<size_t> first_row(K, 0);                       // proof p's first value in d_rows
     {
-        std::vector<std::pair<uint32_t, uint64_t>> points;
+        std::vector<TraceRow> points;
+        size_t values = 0;
         for (int p = 0; p < K; p++) {
-            first_row[p] = points.size();
+            first_row[p] = values;
             if (ps[p].live)
                 for (uint64_t pos : ps[p].positions)
-                    if (!retained(pos)) points.emplace_back((uint32_t)p, pos);
+                    if (!retained(pos)) {
+                        points.push_back(TraceRow{pos, 0, col0[p], (unsigned)shapes[p].w});
+                        values += shapes[p].w;
+                    }
         }
         if (!points.empty()) {
-            d_rows.alloc(points.size() * w * 16);
-            eval_trace_rows(c, polys.as<fe>(), n, w, points, log_N, d_rows.as<fe>());
+            d_rows.alloc(values * 16);
+            eval_trace_rows(c, polys.as<fe>(), n, points, log_N, d_rows.as<fe>());
         }
     }
-    auto plan_openings = [&](ProofState &s, const fe *slab_p, const fe *c_ext_p, size_t row0) {
+    auto plan_openings = [&](ProofState &s, const fe *slab_p, const fe *c_ext_p, size_t row0, int w) {
         OpenPlan O;
         const std::vector<uint64_t> &positions = s.positions;
         const int nq = (int)positions.size();
@@ -843,9 +894,9 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         for (int q = 0; q < nq; q++) {
             const uint64_t cpos = positions[q] & (b - 1), k = positions[q] >> log_b;
             if (!retained(positions[q])) {
-                O.row_off[q] = fb.add16(FetchRef{d_rows.p, row0 * w, -1});
-                for (int j = 1; j < w; j++) fb.add16(FetchRef{d_rows.p, row0 * w + j, -1});
-                row0++;
+                O.row_off[q] = fb.add16(FetchRef{d_rows.p, row0, -1});
+                for (int j = 1; j < w; j++) fb.add16(FetchRef{d_rows.p, row0 + j, -1});
+                row0 += w;
                 continue;
             }
             const int owner = (int)(cpos >> log_nc);
@@ -914,7 +965,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         return O;
     };
     // the opened values and digests into the proof, which is then written out
-    auto fill_openings = [&](ProofState &s, const OpenPlan &O) {
+    auto fill_openings = [&](ProofState &s, const OpenPlan &O, int w) {
         StarkProof &P = s.stark;
         P.trace_info.domain_depth = O.tplan.depth;
         P.trace_nodes = digests_at(O.t_off);
@@ -941,10 +992,10 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     {
         std::vector<OpenPlan> plans(K);
         for (int p = 0; p < K; p++)
-            if (ps[p].live) plans[p] = plan_openings(ps[p], slab_of(p), c_ext_of(p), first_row[p]);
+            if (ps[p].live) plans[p] = plan_openings(ps[p], slab_of(p), c_ext_of(p), first_row[p], shapes[p].w);
         fb.run();
         for (int p = 0; p < K; p++)
-            if (ps[p].live) fill_openings(ps[p], plans[p]);
+            if (ps[p].live) fill_openings(ps[p], plans[p], shapes[p].w);
     }
     clk.mark(9);
     sub.mark("9.openings");
@@ -1099,16 +1150,80 @@ std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t co
     return cols;
 }
 
-void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+std::vector<std::vector<uint32_t>> partition_by_length(const std::vector<uint64_t> &length) {
+    std::vector<std::vector<uint32_t>> parts;
+    std::vector<uint64_t> seen;
+    for (uint32_t i = 0; i < length.size(); i++) {
+        const size_t at = std::find(seen.begin(), seen.end(), length[i]) - seen.begin();
+        if (at == seen.size()) { seen.push_back(length[i]); parts.emplace_back(); }
+        parts[at].push_back(i);
+    }
+    return parts;
+}
+
+std::vector<uint32_t> cut_groups(const std::vector<uint32_t> &width, const std::vector<size_t> &footprint, size_t budget, uint32_t cap) {
+    std::vector<uint32_t> sizes;
+    uint32_t k = 0;
+    size_t bytes = 0, cols = 0;
+    for (size_t i = 0; i < width.size(); i++) {
+        if (k > 0 && (k == cap || bytes + footprint[i] > budget || cols + width[i] > 65535)) {
+            sizes.push_back(k);
+            k = 0; bytes = 0; cols = 0;
+        }
+        k++; bytes += footprint[i]; cols += width[i];
+    }
+    if (k > 0) sizes.push_back(k);
+    return sizes;
+}
+
+std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape) {
+    std::vector<uint32_t> out;
+    std::vector<bool> done(shape.size(), false);
+    for (size_t i = 0; i < shape.size(); i++) {
+        if (done[i]) continue;
+        for (size_t j = i; j < shape.size(); j++)
+            if (!done[j] && shape[j] == shape[i]) { out.push_back((uint32_t)j); done[j] = true; }
+    }
+    return out;
+}
+
+void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
                   int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
-    if (host_cols) DG_REQUIRE(length >= 16 && (length & (length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
+    const uint32_t count = (uint32_t)traces.size();
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    const bool host = traces[0].host_cols != nullptr;
+    if (host)
+        for (const TraceRef &t : traces)
+            DG_REQUIRE(t.length >= 16 && (t.length & (t.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
     if (batch)
         DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
-    ProvePlan plan;                                // several GPUs (one trace): one group, and prove_core shards the full layout
-    if (c.world == 1) plan = plan_prove(c, width, length, opt.extension_factor, count);
+    // every length's plan and groups before any proof runs: a length that fits in no way fails the call before the device computes
+    std::vector<uint64_t> lengths;
+    for (const TraceRef &t : traces) lengths.push_back(t.length);
+    struct LengthRun { std::vector<uint32_t> idx; ProvePlan plan; std::vector<uint32_t> sizes; };
+    std::vector<LengthRun> runs;
+    for (std::vector<uint32_t> &idx : partition_by_length(lengths)) {
+        LengthRun r;
+        r.idx = std::move(idx);
+        r.sizes.assign(r.idx.size(), 1);           // several GPUs (one trace): one group, and prove_core shards the full layout
+        if (c.world == 1) {
+            // planned for the widest shape of the length: its group's bytes are the budget the groups of mixed widths are cut to
+            uint32_t wmax = 0;
+            for (uint32_t i : r.idx) wmax = std::max(wmax, traces[i].width);
+            const uint64_t n = traces[r.idx[0]].length;
+            r.plan = plan_prove(c, wmax, n, opt.extension_factor, (uint32_t)r.idx.size());
+            std::vector<uint32_t> width;
+            std::vector<size_t> foot;
+            for (uint32_t i : r.idx) {
+                width.push_back(traces[i].width);
+                foot.push_back(proof_footprint(traces[i].width, n, opt.extension_factor, r.plan.chunk));
+            }
+            r.sizes = cut_groups(width, foot, (size_t)r.plan.group * r.plan.per_proof, (uint32_t)r.plan.group);
+        }
+        runs.push_back(std::move(r));
+    }
     if (stats) memset(stats, 0, sizeof *stats);
     if (groups) *groups = 0;
     for (uint32_t i = 0; i < count; i++) { proofs_out[i] = nullptr; status[i] = DG_OK; }
@@ -1118,29 +1233,76 @@ void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols,
         Proof **out; uint32_t count; bool done = false;
         ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
     } release{proofs_out, count};
-    for (uint32_t first = 0; first < count; first += plan.group) {
-        const int k = (int)std::min<uint32_t>(plan.group, count - first);
-        std::vector<ProofState> ps;
-        for (int i = 0; i < k; i++) ps.push_back(std::move(all[first + i]));
-        dg_prove_stats_t st;
-        memset(&st, 0, sizeof st);
-        prepare_arena(c, plan);
-        fe *regs = const_cast<fe *>(d_regs) + (size_t)first * width * length;
-        if (host_cols) {
-            c.upload_buf.ensure((size_t)length * 16 * width * k, true);
-            regs = c.upload_buf.as<fe>();
-        }
-        prove_core(c, regs, host_cols ? host_cols + (size_t)first * width : nullptr, k, width, length, ctx_depth, loop_depth, ps, opt, &st,
-                   plan.chunk);
-        if (stats) add_stats(stats, st);
-        if (groups) ++*groups;
-        for (int i = 0; i < k; i++) {
-            status[first + i] = ps[i].status;
-            messages[first + i] = ps[i].message;
-            if (ps[i].status == DG_OK) proofs_out[first + i] = ps[i].proof.release();
+    for (const LengthRun &r : runs) {
+        const uint64_t n = traces[r.idx[0]].length;
+        size_t first = 0;
+        for (uint32_t k : r.sizes) {
+            // the group's traces in input order, and on the device grouped by shape (shapes in order of first appearance)
+            const std::vector<uint32_t> members(r.idx.begin() + first, r.idx.begin() + first + k);
+            first += k;
+            std::vector<RegisterShape> keys;
+            for (uint32_t i : members) keys.push_back(traces[i].shape());
+            std::vector<uint32_t> dev;                                   // trace of device slot p
+            for (uint32_t m : shape_order(keys)) dev.push_back(members[m]);
+            std::vector<int> order(k);                                   // device slot of the group's m-th trace in input order
+            for (uint32_t p = 0; p < k; p++) order[std::find(members.begin(), members.end(), dev[p]) - members.begin()] = (int)p;
+            std::vector<ProofState> ps;
+            std::vector<RegisterShape> shapes;
+            std::vector<const uint8_t *> cols;
+            size_t W = 0;
+            for (uint32_t i : dev) {
+                const TraceRef &t = traces[i];
+                ps.push_back(std::move(all[i]));
+                shapes.push_back(t.shape());
+                if (host) cols.insert(cols.end(), t.host_cols, t.host_cols + t.width);
+                W += t.width;
+            }
+            dg_prove_stats_t st;
+            memset(&st, 0, sizeof st);
+            prepare_arena(c, r.plan);
+            // the group's registers as W columns: host traces are uploaded into the upload buffer by prove_core; device traces are read in
+            // place when they are adjacent in device memory (a one-shape batch), else copied there
+            fe *regs = const_cast<fe *>(traces[dev[0]].d_regs);
+            bool adjacent = !host;
+            for (uint32_t p = 1; p < k && adjacent; p++)
+                adjacent = traces[dev[p]].d_regs == traces[dev[p - 1]].d_regs + (size_t)traces[dev[p - 1]].width * n;
+            if (!adjacent) {
+                c.upload_buf.ensure((size_t)n * 16 * W, true);
+                regs = c.upload_buf.as<fe>();
+                if (!host) {
+                    size_t col = 0;
+                    for (uint32_t i : dev) {
+                        DG_CUDA(cudaMemcpyAsync(regs + col * n, traces[i].d_regs, (size_t)traces[i].width * n * 16, cudaMemcpyDeviceToDevice, c.stream));
+                        col += traces[i].width;
+                    }
+                }
+            }
+            prove_core(c, regs, host ? cols.data() : nullptr, shapes, n, order, ps, opt, &st, r.plan.chunk);
+            if (stats) add_stats(stats, st);
+            if (groups) ++*groups;
+            for (uint32_t p = 0; p < k; p++) {
+                const uint32_t i = dev[p];
+                status[i] = ps[p].status;
+                messages[i] = ps[p].message;
+                if (ps[p].status == DG_OK) proofs_out[i] = ps[p].proof.release();
+            }
         }
     }
     release.done = true;
+}
+
+void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
+    std::vector<TraceRef> traces(count);
+    for (uint32_t i = 0; i < count; i++) {
+        TraceRef &t = traces[i];
+        t.width = width; t.length = length; t.ctx_depth = ctx_depth; t.loop_depth = loop_depth;
+        if (host_cols) t.host_cols = host_cols + (size_t)i * width;
+        else t.d_regs = d_regs + (size_t)i * width * length;
+    }
+    prove_traces(c, traces, inputs16, n_inputs, outputs16, n_outputs, opt, batch, proofs_out, status, messages, stats, groups);
 }
 
 }  // namespace dg

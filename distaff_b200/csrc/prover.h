@@ -16,6 +16,35 @@ void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols,
                   uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
                   int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
+
+// what the caller gives of a trace's register shape (TraceShape::of_trace checks it and derives the rest)
+struct RegisterShape {
+    uint32_t width, ctx_depth, loop_depth;
+    bool operator==(const RegisterShape &o) const { return width == o.width && ctx_depth == o.ctx_depth && loop_depth == o.loop_depth; }
+};
+// one trace of a prove call: its shape and length, and its registers, either host columns (width pointers) or device memory ([width][length])
+struct TraceRef {
+    uint32_t width = 0;
+    uint64_t length = 0;
+    uint32_t ctx_depth = 0, loop_depth = 0;
+    const uint8_t *const *host_cols = nullptr;
+    const fe *d_regs = nullptr;
+    RegisterShape shape() const { return RegisterShape{width, ctx_depth, loop_depth}; }
+};
+// The same for traces of any shapes and lengths (every trace host, or every trace on the device).  The call is partitioned by length
+// (partition_by_length); each length is planned for its widest shape (plan_prove) and cut into groups (cut_groups) of at most that plan's
+// bytes; inside a group the traces are laid out on the device by shape (shape_order).  The Fiat-Shamir draws run length by length, group
+// by group, stage by stage, and within a stage in input order.  Per trace, the result is the one-shape call's.
+void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
+// the traces of each length, lengths in order of first appearance, traces in input order
+std::vector<std::vector<uint32_t>> partition_by_length(const std::vector<uint64_t> &length);
+// sizes of the consecutive groups the traces (in this order) are cut into: a group holds at most `cap` traces, footprints summing to at
+// most `budget` bytes and widths summing to at most 65535 (one launch); a trace that exceeds the budget alone is a group of its own
+std::vector<uint32_t> cut_groups(const std::vector<uint32_t> &width, const std::vector<size_t> &footprint, size_t budget, uint32_t cap);
+// the device order of a group: positions of the traces grouped by shape, shapes in order of first appearance, input order inside a shape
+std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape);
 // The register columns of `count` host traces, trace after trace.  Every trace must have the shape of the first ("all traces of a
 // <call> must ..."), 16..127 registers and no null column; length_first also checks each length before its columns (dg_prove).
 std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first);

@@ -94,6 +94,25 @@ int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t widt
                           const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats);
 int dg_batch_message(uint32_t index, char *message, size_t message_cap);
 
+/* Batched proving across register shapes: `count` traces of any widths, context / loop depths and lengths, proven with the same options in
+ * one call.  Per trace the result is exactly dg_prove_batch's: status[i] = DG_OK and proofs_out[i] byte-identical to dg_prove of that
+ * trace, or a per-trace DG_ERR_UNSATISFIED / DG_ERR_EXHAUSTED with its message in dg_batch_message(i); a failing trace changes no other
+ * proof.  Every trace is checked on the host before the device is touched: a shape, length or public input / output count dg_prove would
+ * reject fails the whole call with DG_ERR_INVALID and a message that starts with "trace i: ".  The call is partitioned by trace length;
+ * the traces of one length run in groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps them further), and every
+ * stage of a group is launched once for all its traces, whatever their shapes, except the constraint evaluation, which is launched once
+ * per register shape of the group.  RNG callbacks (dg_set_rng_callbacks) are called length by length, lengths in order of first
+ * appearance; inside a length group by group and, in every group, stage by stage in input order.  A context that spans several GPUs is
+ * rejected.  Returns and stats as dg_prove_batch. */
+int dg_prove_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                    int *status, dg_prove_stats_t *stats);
+/* same, registers already in device memory: trace i's width[i] x length[i] elements, column-major, at d_registers[i] */
+int dg_prove_traces_device(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                           const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                           const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                           int *status, dg_prove_stats_t *stats);
+
 /* ---- checking a trace before proving it ------------------------------------------------------------------------------------------
  * dg_prove reports an unsatisfied trace late (after the trace LDE and commitment) and only with its lowest failing step; it does not check
  * the boundary constraints at all (a trace whose first or last row disagrees with the claimed inputs / outputs is proven, and the proof is
@@ -391,6 +410,14 @@ int dg_comm_finalize(void);
  * node with global heap index `index` (is_node = 1) of a tree with n blocks of 2^log_blk items per rank over 2^log_g ranks;
  * out = {owner rank or -1 if replicated, 1 if in the replicated upper heap else 0, local index} */
 int dg_host_shard_locate(uint64_t n, int log_blk, int log_g, int is_node, uint64_t index, int64_t out[3]);
+/* the grouping of dg_prove_traces, exported for CPU tests: the traces partitioned by length (lengths in order of first appearance, input
+ * order inside a length), each length's traces cut into consecutive groups of at most `cap` traces whose footprints[i] sum to at most
+ * `budget` (the call uses a budget per length) and whose widths sum to at most 65535.  order_out (count entries) receives the traces in
+ * the order the groups run, each group in its device order: grouped by register shape, shapes in order of first appearance, input order
+ * inside a shape; group_sizes_out (up to count entries) the sizes of the groups, n_groups their number. */
+int dg_host_group_traces(uint32_t count, const uint64_t *lengths, const uint32_t *widths, const uint32_t *ctx_depths, const uint32_t *loop_depths,
+                         const uint64_t *footprints, uint64_t budget, uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out,
+                         uint32_t *n_groups);
 
 /* ---- host-side Fiat-Shamir glue, exported so that it can be unit-tested without a GPU (none of these touch the device) ---- */
 /* field::prng_vector (field.rs:271-275): count draws of StdRng::from_seed(seed) through Uniform(0..M) */
