@@ -575,6 +575,56 @@ def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_ST
             for i, e in enumerate(errors)]
 
 
+# ---- one long execution, split across GPU threads ------------------------------------------------------------------------------------
+def _one_stats(stats, st):
+    if stats is not None:
+        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgTraceOneStats._fields_})
+
+
+def trace_one(program, inputs=None, max_steps=MAX_STEPS, num_outputs=1, segment_steps=0, stats=None):
+    """processor::execute of one program (a hostvm.Program or assembly source) for one ProgramInputs on the GPU, split across threads
+    (dg_trace_one): the sponge from a per-program table, one sequential pass that records checkpoints, and one thread per segment writing
+    the rows.  Returns a hostvm.ExecutionTrace (what hostvm.execute gives, byte for byte); raises DgError when the execution fails, with
+    the host VM's message.  segment_steps: 0 (the library chooses) or a power of two >= 16.  The buffer is sized by a call without
+    registers first, so the table and the sequential pass run twice.  A dict passed as `stats` receives the full call's figures."""
+    assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
+    x = inputs or ProgramInputs()
+    prog, cprog, arr, keep = _execution_args(program, [x])
+    L, info, st = backend.lib(), backend.DgExecutionInfo(), backend.DgTraceOneStats()
+
+    def call(out):
+        rc = L.dg_trace_one(ctypes.byref(cprog), arr, int(max_steps), int(segment_steps), ctypes.byref(info), out, ctypes.byref(st))
+        _one_stats(stats, st)
+        backend.check(rc)
+
+    call(None)
+    regs = np.empty((info.width, info.length, 2), dtype=np.uint64)
+    call(regs.ctypes.data)
+    del keep
+    sd, start, n = info.stack_depth, 15 + info.ctx_depth + info.loop_depth, info.length
+    last = [felt.to_ints(regs[start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+    return hostvm.ExecutionTrace(regs, info.ctx_depth, info.loop_depth, sd, prog.hash, list(x.public), last[:num_outputs])
+
+
+def execute_one(program, inputs=None, num_outputs=1, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
+    """distaff::execute (lib.rs:30-65) of one program for one ProgramInputs, the execution split across GPU threads as in trace_one and
+    the trace proven where it was written (dg_execute_one).  Returns (outputs, StarkProof) -- what execute() returns, byte for byte --
+    and raises DgError when the execution or the proof fails.  `stats` as in trace_one."""
+    options = options or ProofOptions()
+    assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
+    _, cprog, arr, keep = _execution_args(program, [inputs or ProgramInputs()])
+    opt = options._c()
+    handle = backend.vp()
+    outputs = np.zeros((max(num_outputs, 1), 2), dtype=np.uint64)
+    pst, st = backend.DgStats(), backend.DgTraceOneStats()
+    rc = backend.lib().dg_execute_one(ctypes.byref(cprog), arr, num_outputs, int(max_steps), int(segment_steps), ctypes.byref(opt),
+                                      ctypes.byref(handle), outputs.ctypes.data, None, ctypes.byref(pst), ctypes.byref(st))
+    del keep
+    _one_stats(stats, st)
+    backend.check(rc)
+    return (felt.to_ints(outputs[:num_outputs]) if num_outputs else []), _collect(handle.value, pst)
+
+
 # ---- many programs, many inputs, executed on the GPU in one call ----------------------------------------------------------------------
 def pack_jobs(jobs, compile=None):
     """The program table of a dg_trace_programs / dg_execute_programs call.  jobs: (program, ProgramInputs) or (program, ProgramInputs,

@@ -78,6 +78,12 @@ class DgExecutionStats(ctypes.Structure):
                 ("shape_ms", ctypes.c_float), ("write_ms", ctypes.c_float)]
 
 
+class DgTraceOneStats(ctypes.Structure):
+    _fields_ = [("table_ms", ctypes.c_float), ("sequential_ms", ctypes.c_float), ("segment_ms", ctypes.c_float), ("table_rounds", u64),
+                ("table_entries", u64), ("table_levels", u32), ("sequential_launches", u32), ("checkpoints", u64), ("segments", u64),
+                ("logged", u64), ("segment_steps", u64), ("fallback", ctypes.c_int32)]
+
+
 DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -112,6 +118,10 @@ EXPORTS = {
     "dg_execute_programs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32), u64,
                             ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
                             ctypes.POINTER(DgExecutionStats)],
+    "dg_trace_one": [ctypes.POINTER(DgProgram), ctypes.POINTER(DgProgramInputs), u64, u64, ctypes.POINTER(DgExecutionInfo), vp,
+                     ctypes.POINTER(DgTraceOneStats)],
+    "dg_execute_one": [ctypes.POINTER(DgProgram), ctypes.POINTER(DgProgramInputs), u32, u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp,
+                       ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(DgStats), ctypes.POINTER(DgTraceOneStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),

@@ -636,6 +636,35 @@ int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_progr
             for (uint32_t i = 0; i < count; i++) memcpy(outputs16 + (size_t)16 * num_outputs * i, outs.data() + (size_t)128 * i, (size_t)16 * num_outputs);
     });
 }
+int dg_trace_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps,
+                 dg_execution_info_t *info, uint8_t *registers_out, dg_trace_one_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(program && inputs, "null argument");
+        const uint32_t of = 0;
+        const ExecutionCall x{program, 1, 1, &of, inputs, max_steps};
+        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
+        check_segment_steps(segment_steps);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        trace_one(c, x, segment_steps, info, registers_out, stats);
+    });
+}
+int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
+                   uint64_t segment_steps, const dg_options_t *options, dg_proof_t **proof_out, uint8_t *outputs16, dg_execution_info_t *info,
+                   dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(program && inputs && options && proof_out, "null argument");
+        *proof_out = nullptr;
+        const uint32_t of = 0;
+        const ExecutionCall x{program, 1, 1, &of, inputs, max_steps};
+        check_execution_call(x);
+        check_output_counts(1, &num_outputs, outputs16);
+        check_segment_steps(segment_steps);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        *proof_out = (dg_proof_t *)execute_one(c, x, num_outputs, segment_steps, *options, outputs16, info, prove_stats, stats);
+    });
+}
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
     return guarded([&] {
         DG_REQUIRE(message && cap, "null argument");

@@ -2,11 +2,13 @@
 // and dg_execute_batch are the one-program case): validate each program's encoding, put every program into one set of tables and upload
 // them and the inputs once, run the shape pass for every execution, and write the successful executions in waves -- one write launch
 // (vm.cu) per wave for every shape in it -- into one slab per shape, which is copied to the caller's buffers (dg_trace_programs) or
-// proven in place (dg_execute_programs, through prove_traces).
+// proven in place (dg_execute_programs, through prove_traces).  dg_trace_one / dg_execute_one run one execution from the sponge table:
+// the table level by level, the sequential pass, the segment pass (vm.cu), with the batch path as the fallback for inconsistent hashes.
 #include "vm.h"
 #include "air.h"
 #include "prover.h"
 #include <algorithm>
+#include <functional>
 #include <map>
 #include <set>
 #include <tuple>
@@ -371,6 +373,270 @@ void finish(const Executions &X, int *status, std::vector<std::string> &messages
     if (vm_stats) *vm_stats = X.stats;
 }
 
+// ---- one execution from the sponge table ------------------------------------------------------------------------------------------------
+// The chains of a program (vm.h): every block list reachable from the root once (lists may be shared: a list is its child range) and, per
+// loop, the chain after BREAK.  A chain's level is one above every chain it reads -- a list reads its group, switch and loop children's
+// closing states, the break chains of its loops and its loops' skips; a break chain reads the body's last state -- so one launch per
+// level computes them in order.  Nothing is hashed here: the host only counts each chain's entries and lays the table out by level.
+struct ChainPlan {
+    std::vector<VmChainRef> refs;                 // per block
+    std::vector<VmChainItem> items;               // level by level
+    std::vector<size_t> level_start;              // the items of level l (from 1) are [level_start[l - 1], level_start[l])
+    unsigned long long root = 0, entries = 0, rounds = 0;
+};
+
+ChainPlan plan_chains(const dg_program_t &p) {
+    struct List { uint32_t first, count; unsigned level; unsigned long long len, ends; };      // ends: child end_block entries
+    std::map<std::pair<uint32_t, uint32_t>, unsigned> ids;
+    std::vector<List> lists;
+    std::vector<unsigned> brk_level(p.n_blocks, 0);
+    std::function<unsigned(uint32_t, uint32_t)> list = [&](uint32_t first, uint32_t count) -> unsigned {
+        const auto it = ids.find({first, count});
+        if (it != ids.end()) return it->second;
+        unsigned level = 0;
+        unsigned long long len = 1, ends = 0;                                  // the closing NOOP
+        for (uint32_t k = 0; k < count; k++) {
+            const uint32_t bi = p.children[first + k];
+            const dg_block_t &b = p.blocks[bi];
+            if (b.kind == DG_BLOCK_SPAN) { len += b.count + (k > 0); continue; }
+            len += 15;                                                         // end_block and 14 NOOPs
+            ends++;
+            const unsigned main = lists[list(b.first, b.count)].level;
+            unsigned m = main;
+            if (b.kind != DG_BLOCK_GROUP) m = std::max(m, lists[list(b.alt_first, b.alt_count)].level);
+            if (b.kind == DG_BLOCK_LOOP) { brk_level[bi] = main + 1; m = std::max(m, main + 1); }
+            level = std::max(level, m);
+        }
+        lists.push_back(List{first, count, level + 1, len, ends});
+        return ids[{first, count}] = (unsigned)lists.size() - 1;
+    };
+    const unsigned root = list(p.root_first, p.root_count);
+    unsigned levels = 0;
+    for (const List &l : lists) levels = std::max(levels, l.level);
+    ChainPlan P;
+    P.refs.assign(p.n_blocks, VmChainRef{0, 0, 0, 0, 0, 0});
+    std::vector<unsigned long long> out(lists.size());
+    P.level_start.push_back(0);
+    for (unsigned level = 1; level <= levels; level++) {
+        for (size_t i = 0; i < lists.size(); i++) {
+            const List &l = lists[i];
+            if (l.level != level) continue;
+            out[i] = P.entries;
+            const bool tail = i == root;
+            P.items.push_back(VmChainItem{VM_CHAIN_LIST, l.first, l.count, 0, tail ? 1u : 0u, 0, P.entries});
+            P.entries += l.len + (tail ? 15 : 0);
+            P.rounds += l.len - l.ends + (tail ? 14 : 0);
+        }
+        for (uint32_t bi = 0; bi < p.n_blocks; bi++) {
+            if (brk_level[bi] != level) continue;
+            const dg_block_t &b = p.blocks[bi];
+            const unsigned long long len = p.blocks[p.children[b.alt_first]].count + 1;    // the skip's first span and a NOOP
+            P.refs[bi].brk = P.entries;
+            P.refs[bi].brk_close = P.entries + len - 1;
+            P.items.push_back(VmChainItem{VM_CHAIN_BREAK, 0, 0, bi, 0, 0, P.entries});
+            P.entries += len;
+            P.rounds += len;
+        }
+        P.level_start.push_back(P.items.size());
+    }
+    for (uint32_t bi = 0; bi < p.n_blocks; bi++) {
+        const dg_block_t &b = p.blocks[bi];
+        if (b.kind == DG_BLOCK_SPAN) continue;
+        const auto at = [&](uint32_t first, uint32_t count, unsigned long long &start, unsigned long long &close) {
+            const auto it = ids.find({first, count});
+            if (it == ids.end()) return;                                     // a block the root does not reach
+            start = out[it->second];
+            close = start + lists[it->second].len - 1;
+        };
+        at(b.first, b.count, P.refs[bi].main, P.refs[bi].main_close);
+        if (b.kind != DG_BLOCK_GROUP) at(b.alt_first, b.alt_count, P.refs[bi].alt, P.refs[bi].alt_close);
+    }
+    P.root = out[root];
+    return P;
+}
+
+// S when the caller leaves it to the library: at most 4096 segments for an execution of max_steps steps
+uint64_t default_segment_steps(uint64_t max_steps) {
+    uint64_t s = 16;
+    while (s < (1ULL << 40) && s * 4096 < max_steps) s *= 2;
+    return s;
+}
+
+// One execution from the sponge table.  table() returns whether the encoding's hashes are consistent; sequential() runs the execution
+// (again with more room when the tape scratch, the read log or the checkpoint buffer were too small) and throws its failure; segments()
+// writes the rows into regs ([width][length]) and pads them.
+struct OneExecution {
+    Context &c;
+    Executions X;
+    uint64_t S;
+    dg_trace_one_stats_t st;
+    DevBuf d_refs, d_items, d_tab, d_bad, d_log, d_cp, d_seq, d_codes;
+    VmTabled T;
+    VmSequential seq{0, 0};
+
+    OneExecution(Context &ctx_, const ExecutionCall &x, uint64_t segment_steps)
+        : c(ctx_), X(ctx_, x), S(segment_steps ? segment_steps : default_segment_steps(x.max_steps)) {
+        memset(&st, 0, sizeof st);
+        memset(&T, 0, sizeof T);
+        st.segment_steps = S;
+        X.setup();
+    }
+
+    bool table() {
+        if (X.status[0] != DG_OK) throw Error(X.status[0], X.messages[0]);        // inputs that fail before the execution runs
+        const ChainPlan P = plan_chains(X.x.programs[0]);
+        X.upload(d_refs, P.refs);
+        X.upload(d_items, P.items);
+        d_tab.alloc(P.entries * sizeof(VmSponge));
+        const std::vector<unsigned> zero(1, 0);
+        X.upload(d_bad, zero);
+        st.table_ms = X.timed([&] {
+            for (size_t l = 0; l + 1 < P.level_start.size(); l++)
+                vm_table_level(c, X.L, d_items.as<VmChainItem>() + P.level_start[l], (unsigned)(P.level_start[l + 1] - P.level_start[l]),
+                               d_refs.as<VmChainRef>(), d_tab.as<VmSponge>(), d_bad.as<unsigned>());
+        });
+        st.table_levels = (uint32_t)P.level_start.size() - 1;
+        st.table_rounds = P.rounds;
+        st.table_entries = P.entries;
+        unsigned bad = 0;
+        DG_CUDA(cudaMemcpy(&bad, d_bad.p, sizeof bad, cudaMemcpyDeviceToHost));
+        T.tab = d_tab.as<VmSponge>();
+        T.chains = d_refs.as<VmChainRef>();
+        T.root = P.root;
+        T.segment_steps = S;
+        return bad == 0;
+    }
+
+    void sequential() {
+        const ExecutionCall &x = X.x;
+        const uint64_t max_steps = x.max_steps;
+        unsigned long long extra = 256, log_cap = std::min<uint64_t>(2 * max_steps, 1ULL << 21);
+        unsigned long long cp_cap = std::min<uint64_t>(max_steps / S + 2, 4096);
+        d_seq.alloc(sizeof(VmSequential));
+        for (;;) {
+            X.cap[0] = x.inputs[0].n_secret_a + extra;
+            X.cap[1] = x.inputs[0].n_secret_b + extra;
+            X.place_tapes({0});
+            X.launch_ids({0});
+            d_log.alloc(std::max<unsigned long long>(log_cap, 1) * sizeof(fe));
+            d_cp.alloc(cp_cap * vm_checkpoint_bytes());
+            T.log = d_log.as<fe>(); T.log_cap = log_cap;
+            T.checkpoints = d_cp.p; T.cp_cap = cp_cap;
+            st.sequential_ms += X.timed([&] { vm_sequential_pass(c, X.L, T, d_seq.as<VmSequential>()); });
+            st.sequential_launches++;
+            X.download_results();
+            DG_CUDA(cudaMemcpy(&seq, d_seq.p, sizeof seq, cudaMemcpyDeviceToHost));
+            const VmResult &r = X.res[0];
+            if (r.code == VM_TAPE_SCRATCH) { extra *= 16; continue; }
+            if (r.code != VM_OK) throw Error(DG_ERR_EXECUTION, vm_message(r.code, r.fail_step, max_steps));
+            if (seq.checkpoints + 1 <= cp_cap && seq.logged <= log_cap) break;
+            cp_cap = std::max(cp_cap, seq.checkpoints + 1);                   // the sizes this execution needs
+            log_cap = std::max(log_cap, seq.logged);
+        }
+        st.checkpoints = seq.checkpoints + 1;
+        st.segments = seq.checkpoints;
+        st.logged = seq.logged;
+    }
+
+    dg_execution_info_t shape() const { return X.info(0); }
+
+    void segments(fe *regs) {
+        const dg_execution_info_t s = shape();
+        X.upload(X.d_outs, std::vector<VmOut>{VmOut{0, s.length, s.width, s.ctx_depth, s.loop_depth, s.stack_depth}});
+        X.L.out = regs;
+        X.L.outs = X.d_outs.as<VmOut>();
+        d_codes.alloc(2 * seq.checkpoints * sizeof(unsigned long long));
+        st.segment_ms = X.timed([&] {
+            vm_segment_pass(c, X.L, T, seq.checkpoints, d_codes.as<unsigned long long>());
+            vm_pad_rows(c, regs, X.L.res, X.L.ids, 1, s.width, s.length);
+        });
+        std::vector<unsigned long long> codes(2 * seq.checkpoints);
+        DG_CUDA(cudaMemcpy(codes.data(), d_codes.p, codes.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        for (unsigned long long q = 0; q < seq.checkpoints; q++) {
+            const unsigned code = (unsigned)codes[2 * q];
+            if (code == VM_OK) continue;
+            const std::string m = vm_message(code, codes[2 * q + 1], X.x.max_steps);
+            throw Error(DG_ERR_EXECUTION, code == VM_SEGMENT ? m : "internal error: trace segment " + std::to_string(q) +
+                                                                      " failed where the sequential pass did not: " + m);
+        }
+    }
+    // the buffers the rows no longer need, before a proof
+    void release() { for (DevBuf *d : {&d_refs, &d_items, &d_tab, &d_bad, &d_log, &d_cp, &d_seq, &d_codes, &X.d_tapes}) d->release(); }
+};
+
+void one_stats(dg_trace_one_stats_t *stats, const dg_trace_one_stats_t &st) { if (stats) *stats = st; }
+
+void trace_one_path(OneExecution &E, Context &c, dg_execution_info_t *info, uint8_t *registers_out) {
+    if (!E.table()) {
+        // the batch path, with its write pass even without registers_out, so that a shapes-only call reports what a full one reports
+        Executions &X = E.X;
+        E.st.fallback = 1;
+        X.shapes();
+        uint8_t *const outs[1] = {registers_out};
+        X.write_waves(nullptr, registers_out ? outs : nullptr, [&](const std::vector<Slab> &slabs) {
+            if (registers_out && X.status[0] == DG_OK)
+                DG_CUDA(cudaMemcpy(registers_out, slabs[0].regs, (size_t)slabs[0].shape.width * slabs[0].shape.length * 16, cudaMemcpyDeviceToHost));
+        });
+        E.st.sequential_ms = X.stats.shape_ms;
+        E.st.segment_ms = X.stats.write_ms;
+        if (X.status[0] != DG_OK) throw Error(X.status[0], X.messages[0]);
+        if (info) *info = X.info(0);
+        return;
+    }
+    E.sequential();
+    const dg_execution_info_t s = E.shape();
+    if (registers_out) {
+        DevBuf regs((size_t)s.width * s.length * 16);
+        E.segments(regs.as<fe>());
+        DG_CUDA(cudaMemcpy(registers_out, regs.p, (size_t)s.width * s.length * 16, cudaMemcpyDeviceToHost));
+    }
+    if (info) *info = s;
+}
+
+Proof *execute_one_path(OneExecution &E, Context &c, const ExecutionCall &x, uint32_t num_outputs, const dg_options_t &opt, uint8_t *outputs16,
+                        dg_execution_info_t *info, dg_prove_stats_t *prove_stats) {
+    if (!E.table()) {
+        E.release();
+        dg_execution_info_t shape;                   // the batch path's shape pass gives the shape it proves
+        memset(&shape, 0, sizeof shape);
+        if (info) {
+            E.X.shapes();
+            if (E.X.status[0] == DG_OK) shape = E.X.info(0);
+        }
+        Proof *proof = nullptr;
+        int status = DG_OK;
+        std::vector<std::string> messages;
+        dg_execution_stats_t vm;
+        std::vector<uint8_t> outs(8 * 16);
+        execute_programs(c, x, &num_outputs, opt, &proof, outs.data(), &status, messages, prove_stats, &vm);
+        E.st.fallback = 1;
+        E.st.sequential_ms = vm.shape_ms;
+        E.st.segment_ms = vm.write_ms;
+        if (status != DG_OK) throw Error(status, messages[0]);
+        if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
+        if (info) *info = shape;
+        return proof;
+    }
+    E.sequential();
+    const dg_execution_info_t s = E.shape();
+    DevBuf regs((size_t)s.width * s.length * 16);
+    E.segments(regs.as<fe>());
+    E.release();
+    std::vector<fe> outs(8, fe_make(0, 0));
+    for (uint32_t j = 0; j < num_outputs; j++) outs[j] = E.X.res[0].top[j];
+    const uint8_t *in16 = x.inputs[0].public16, *out16 = (const uint8_t *)outs.data();
+    const uint32_t n_in = x.inputs[0].n_public;
+    Proof *proof = nullptr;
+    int status = DG_OK;
+    std::vector<std::string> messages;
+    prove_traces(c, regs.as<fe>(), nullptr, 1, s.width, s.length, s.ctx_depth, s.loop_depth, &in16, &n_in, &out16, &num_outputs, opt, true,
+                 &proof, &status, messages, prove_stats);
+    if (status != DG_OK) throw Error(status, messages[0]);
+    if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
+    if (info) *info = s;
+    return proof;
+}
+
 }  // namespace
 
 void check_execution_call(const ExecutionCall &x) {
@@ -409,6 +675,45 @@ void check_output_counts(uint32_t count, const uint32_t *num_outputs, const uint
         any |= num_outputs[i] > 0;
     }
     DG_REQUIRE(!any || outputs16, "null outputs");
+}
+
+void check_segment_steps(uint64_t s) {
+    DG_REQUIRE(s == 0 || (s >= 16 && (s & (s - 1)) == 0), "segment_steps must be 0 or a power of two of at least 16");
+}
+
+void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *registers_out,
+               dg_trace_one_stats_t *stats) {
+    DG_REQUIRE(x.count == 1, "one execution");
+    check_execution_call(x);
+    check_segment_steps(segment_steps);
+    check_one_gpu(c);
+    OneExecution E(c, x, segment_steps);
+    try {
+        trace_one_path(E, c, info, registers_out);
+    } catch (...) {
+        one_stats(stats, E.st);
+        throw;
+    }
+    one_stats(stats, E.st);
+}
+
+Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
+                   dg_execution_info_t *info, dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats) {
+    DG_REQUIRE(x.count == 1, "one execution");
+    check_execution_call(x);
+    check_output_counts(1, &num_outputs, outputs16);
+    check_segment_steps(segment_steps);
+    check_one_gpu(c);
+    if (prove_stats) memset(prove_stats, 0, sizeof *prove_stats);
+    OneExecution E(c, x, segment_steps);
+    try {
+        Proof *proof = execute_one_path(E, c, x, num_outputs, opt, outputs16, info, prove_stats);
+        one_stats(stats, E.st);
+        return proof;
+    } catch (...) {
+        one_stats(stats, E.st);
+        throw;
+    }
 }
 
 void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,

@@ -66,6 +66,13 @@ void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *inf
                     std::vector<std::string> &messages, dg_execution_stats_t *vm_stats);
 void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
+// dg_trace_one / dg_execute_one (execute.cu): one execution (x.count == 1) from the sponge table; a failed execution throws
+// DG_ERR_EXECUTION with its message.  check_segment_steps rejects an S that is neither 0 nor a power of two >= 16.
+void check_segment_steps(uint64_t segment_steps);
+void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *registers_out,
+               dg_trace_one_stats_t *stats);
+Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
+                   dg_execution_info_t *info, dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP
 long long batch_group_cap(long long k);
 

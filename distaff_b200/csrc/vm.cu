@@ -9,6 +9,14 @@
 //   write pass  the same execution with the sponge, writing every register of every row up to the last step into its own place and
 //               shape (one launch covers executions of any mix of shapes); it also checks the loop images and the program hash, which
 //               need the sponge.  A second, coalesced kernel writes the padding rows of Machine::finalize, one launch per shape.
+// One long execution (dg_trace_one / dg_execute_one) runs three more kernels instead:
+//   table       the sponge chain of every block list, level by level (vm.h); the sponge never reads data, so with consistent hashes
+//               the state after every step is a table lookup
+//   sequential  the execution on one thread, as the write pass but with the sponge from the table and no register writes: it records a
+//               checkpoint (the whole machine state) at the first top of the frame loop at or after every S steps, and logs every value
+//               popped from the tapes (hints push onto them mid-execution, so a segment cannot read the tapes itself)
+//   segment     one thread per checkpoint: replays from it to the next one with the sponge from the table and the tape values from the
+//               log, writes those rows, and checks that it ends in the state the next checkpoint holds
 // The per-thread stack, context stack, loop stack and frame stack are indexed at run time and live in local memory by design.
 #define DG_MUL_CALL 1
 #include "common.cuh"
@@ -52,6 +60,7 @@ std::string vm_message(unsigned code, unsigned long long step, unsigned long lon
         "cannot enter loop based on a non-binary condition"};
     if (code < VM_NO_STEP) return std::string(MSG[code]) + " at step " + std::to_string(step);
     switch (code) {
+        case VM_SEGMENT: return "internal error: a trace segment did not end in the state the sequential pass recorded, at step " + std::to_string(step);
         case VM_CAP: return "execution exceeds " + std::to_string(max_steps) + " steps";
         case VM_MIN_OPS: return "a program must consist of at least 16 operations";
         case VM_HASH: return "program hash does not match trace hash";
@@ -122,10 +131,41 @@ __device__ void hasher_round(fe s[6], unsigned long long step) {
 
 struct Frame { unsigned first, count, k, block, cont; };
 
+// what a Machine runs: the shape and write passes, or the sequential and segment passes of one execution, which take the sponge from the
+// table (vm.h)
+enum : int { M_SHAPE, M_WRITE, M_SEQUENTIAL, M_SEGMENT };
+
+// the whole state of an execution at the top of the frame loop: what the sequential pass records and a segment starts from
+struct VmCheckpoint {
+    unsigned long long step, opc, na, nb, lpos, at, tpos[16];
+    unsigned depth, max_depth, ctx_depth, loop_depth, ctx_cols, loop_cols;
+    int top;
+    unsigned pad;
+    Frame fr[16];
+    fe sponge[4], S[32], ctx[16], lp[8];
+};
+
+// the members only the tabled passes have (an empty base of the shape and write passes)
+template <bool TABLED> struct TableState {};
+template <> struct TableState<true> {
+    const VmSponge *tab;
+    const VmChainRef *chains;
+    unsigned long long at, parent_at;                 // the next entry of the running frame's chain; the entry end_block resumes at
+    fe *log;
+    unsigned long long lpos, lcap;                    // values popped so far (the next one to log or read)
+    VmCheckpoint *cp;                                 // sequential pass: checkpoints recorded and room for them, where the next is due
+    unsigned long long ncp, cp_cap, next_cp, seg;
+    const VmCheckpoint *expect;                       // segment pass: the state it must end in, at the first boundary at or after `stop`
+    unsigned long long stop;
+};
+
 // One execution.  The decoder and the stack advance in lock-step, so `step` serves both; the registers of row `step` are the fields
 // below (S[i] = 0 at and above the stack depth, ctx / lp = 0 at and above their depths, as the host VM's columns are).
-template <bool WRITE>
-struct Machine {
+template <int MODE>
+struct Machine : TableState<(MODE >= M_SEQUENTIAL)> {
+    static constexpr bool WRITE = MODE == M_WRITE || MODE == M_SEGMENT;       // writes registers
+    static constexpr bool SPONGE = MODE != M_SHAPE;                           // knows the sponge (rounds or the table)
+    static constexpr bool TABLED = MODE >= M_SEQUENTIAL;
     const VmLaunch &L;
     unsigned long long step = 0, opc = 0, max_steps;
     unsigned code = VM_OK;
@@ -166,16 +206,39 @@ struct Machine {
 
     // ---- tapes (stacks: the next value to read is the last one)
     __device__ __forceinline__ bool push_a(fe v) {
+        if constexpr (MODE == M_SEGMENT) { na++; return true; }          // a segment counts the tapes and reads popped values from the log
         if (na == cap_a) return fail(VM_TAPE_SCRATCH);
         ta[na++] = v;
         peak_a = max(peak_a, na);
         return true;
     }
     __device__ __forceinline__ bool push_b(fe v) {
+        if constexpr (MODE == M_SEGMENT) { nb++; return true; }
         if (nb == cap_b) return fail(VM_TAPE_SCRATCH);
         tb[nb++] = v;
         peak_b = max(peak_b, nb);
         return true;
+    }
+    __device__ __forceinline__ fe pop_a() {
+        if constexpr (MODE == M_SEGMENT) { --na; return this->log[this->lpos++]; }
+        const fe v = ta[--na];
+        if constexpr (MODE == M_SEQUENTIAL) logged(v);
+        return v;
+    }
+    __device__ __forceinline__ fe pop_b() {
+        if constexpr (MODE == M_SEGMENT) { --nb; return this->log[this->lpos++]; }
+        const fe v = tb[--nb];
+        if constexpr (MODE == M_SEQUENTIAL) logged(v);
+        return v;
+    }
+    __device__ __forceinline__ void logged(fe v) {     // a log too small for the execution is counted on; the host runs it again
+        if (this->lpos < this->lcap) this->log[this->lpos] = v;
+        this->lpos++;
+    }
+    // the tabled passes: the state after this step is the running frame's next chain entry
+    __device__ __forceinline__ void take() {
+        const VmSponge &e = this->tab[this->at++];
+        for (int i = 0; i < 4; i++) sponge[i] = e.s[i];
     }
 
     __device__ bool advance(bool user_op) {
@@ -234,6 +297,7 @@ struct Machine {
         if (!advance(false) || !pop_context(h)) return false;
         const fe bh = sponge[0], z = fe_small(0);
         if (true_branch) set_sponge(h, bh, sibling, z); else set_sponge(h, sibling, bh, z);
+        if constexpr (TABLED) this->at++;               // computed as the write pass does; the table holds the same state
         commit_bits(true_branch ? F_TEND : F_FEND, OP_NOOP); commit_state();
         return true;
     }
@@ -249,7 +313,7 @@ struct Machine {
         if (step % 16 != 15) return fail(VM_WRAP_ALIGN);
         if (!advance(false)) return false;
         if (loop_depth == 0) return fail(VM_LOOP_UNDERFLOW);
-        if (WRITE && !fe_eq(sponge[0], lp[0])) return fail(VM_LOOP_IMAGE);
+        if (SPONGE && !fe_eq(sponge[0], lp[0])) return fail(VM_LOOP_IMAGE);
         const fe z = fe_small(0);
         set_sponge(z, z, z, z);
         commit_bits(F_WRAP, OP_NOOP); commit_state();
@@ -259,7 +323,7 @@ struct Machine {
         if (step % 16 != 15) return fail(VM_BREAK_ALIGN);
         fe img;
         if (!advance(false) || !pop_loop_image(img)) return false;
-        if (WRITE && !fe_eq(sponge[0], img)) return fail(VM_LOOP_IMAGE);
+        if (SPONGE && !fe_eq(sponge[0], img)) return fail(VM_LOOP_IMAGE);
         commit_bits(F_BREAK, OP_NOOP); commit_state();
         return true;
     }
@@ -270,7 +334,8 @@ struct Machine {
             if (step % 8 != 0) return fail(VM_PUSH_ALIGN);
         }
         if (!advance(true)) return false;
-        if (WRITE) sponge_round(sponge, op, op_value, step - 1);
+        if constexpr (TABLED) take();
+        else if (WRITE) sponge_round(sponge, op, op_value, step - 1);
         if (!stack_op(op, hint)) return false;
         commit_bits(F_HACC, op); commit_state();
         return true;
@@ -311,7 +376,7 @@ struct Machine {
             } else if (hint.kind == H_NONE) { if (na == 0) return fail(VM_EMPTY_TAPE_A); }
             else return fail(VM_HINT_READ);
             if (!shift_right(1)) return false;
-            S[0] = ta[--na];
+            S[0] = pop_a();
             return true;
         case OP_READ2:
             if (hint.kind == H_PMPATH) {
@@ -322,18 +387,19 @@ struct Machine {
                 // the last n values of A become (bit, value) pairs; backwards, so that no value is overwritten before it is read
                 const fe idx = S[2];
                 const unsigned long long base = na - n;
-                for (int i = (int)n - 1; i >= 0; i--) {
-                    const fe v = ta[base + i];
-                    ta[base + 2 * i] = fe_small(bit_of(idx, n - i - 1));
-                    ta[base + 2 * i + 1] = v;
-                }
+                if constexpr (MODE != M_SEGMENT)
+                    for (int i = (int)n - 1; i >= 0; i--) {
+                        const fe v = ta[base + i];
+                        ta[base + 2 * i] = fe_small(bit_of(idx, n - i - 1));
+                        ta[base + 2 * i + 1] = v;
+                    }
                 na += n;
                 peak_a = max(peak_a, na);
             } else if (hint.kind == H_NONE) { if (na == 0 || nb == 0) return fail(VM_EMPTY_TAPE); }
             else return fail(VM_HINT_READ2);
             if (!shift_right(2)) return false;
-            S[1] = ta[--na];
-            S[0] = tb[--nb];
+            S[1] = pop_a();
+            S[0] = pop_b();
             return true;
         case OP_DUP: return need(1) && shift_right(1);
         case OP_DUP2: return need(2) && shift_right(2);
@@ -394,7 +460,8 @@ struct Machine {
                     if (!push_a(fe_small(bit_of(a, i))) || !push_b(fe_small(bit_of(b, i)))) return false;
             } else if (hint.kind == H_NONE) { if (!need(8)) return false; if (na == 0 || nb == 0) return fail(VM_EMPTY_TAPE); }
             else return fail(VM_HINT_CMP);
-            const fe a_bit = ta[--na], b_bit = tb[--nb];
+            // (spelt so that the shape and write passes compile exactly as they did before the tabled passes)
+            const fe a_bit = TABLED ? pop_a() : ta[--na], b_bit = TABLED ? pop_b() : tb[--nb];
             if (!is_bin(a_bit) || !is_bin(b_bit)) return fail(VM_BINARY);
             const fe p2 = S[0];
             if (!is_pow2(p2)) return fail(VM_CMP_POW2);
@@ -415,7 +482,7 @@ struct Machine {
                 for (unsigned i = 0; i < hint.n; i++) if (!push_a(fe_small(bit_of(v, hint.n - i - 1)))) return false;
             } else if (hint.kind == H_NONE) { if (!need(4)) return false; if (na == 0) return fail(VM_EMPTY_TAPE_A); }
             else return fail(VM_HINT_BINACC);
-            const fe bit = ta[--na];
+            const fe bit = pop_a();
             if (!is_bin(bit)) return fail(VM_BINARY);
             const fe p2 = S[2];
             if (!is_pow2(p2)) return fail(VM_BINACC_POW2);
@@ -435,7 +502,9 @@ struct Machine {
 
     // ---- processor/mod.rs:50-182
     __device__ bool close_block(fe sibling, bool true_branch) {
-        if (!noop() || !end_block(sibling, true_branch)) return false;
+        if (!noop()) return false;                      // the last step of the closed list's frame
+        if constexpr (TABLED) this->at = this->parent_at;
+        if (!end_block(sibling, true_branch)) return false;
         for (int i = 0; i < 14; i++) if (!noop()) return false;
         return true;
     }
@@ -444,14 +513,84 @@ struct Machine {
         for (unsigned i = 0; i < b.count; i++) if (!exec(L.ops[b.first + i], L.hints[b.first + i])) return false;
         return true;
     }
+    // ---- checkpoints of the tabled passes: the state at the top of the frame loop, the frames and where each resumes in its chain
+    __device__ void save(VmCheckpoint &c, const Frame *fr, int top, const unsigned long long *tpos) const {
+        c.step = step; c.opc = opc; c.na = na; c.nb = nb; c.lpos = this->lpos; c.at = this->at;
+        c.depth = depth; c.max_depth = max_depth; c.ctx_depth = ctx_depth; c.loop_depth = loop_depth; c.ctx_cols = ctx_cols;
+        c.loop_cols = loop_cols; c.top = top; c.pad = 0;
+        for (int i = 0; i < 16; i++) {
+            c.tpos[i] = i < top ? tpos[i] : 0;
+            c.fr[i] = i <= top ? fr[i] : Frame{0, 0, 0, 0, 0};
+            c.ctx[i] = ctx[i];
+        }
+        for (int i = 0; i < 4; i++) c.sponge[i] = sponge[i];
+        for (int i = 0; i < 32; i++) c.S[i] = S[i];
+        for (int i = 0; i < 8; i++) c.lp[i] = lp[i];
+    }
+    __device__ void load(const VmCheckpoint &c) {
+        step = c.step; opc = c.opc; na = c.na; nb = c.nb; this->lpos = c.lpos; this->at = c.at;
+        depth = c.depth; max_depth = c.max_depth; ctx_depth = c.ctx_depth; loop_depth = c.loop_depth; ctx_cols = c.ctx_cols;
+        loop_cols = c.loop_cols;
+        for (int i = 0; i < 4; i++) sponge[i] = c.sponge[i];
+        for (int i = 0; i < 32; i++) S[i] = c.S[i];
+        for (int i = 0; i < 16; i++) ctx[i] = c.ctx[i];
+        for (int i = 0; i < 8; i++) lp[i] = c.lp[i];
+    }
+    __device__ bool same(const VmCheckpoint &c, const Frame *fr, int top, const unsigned long long *tpos) const {
+        bool ok = c.step == step && c.opc == opc && c.na == na && c.nb == nb && c.lpos == this->lpos && c.at == this->at && c.depth == depth &&
+                  c.max_depth == max_depth && c.ctx_depth == ctx_depth && c.loop_depth == loop_depth && c.ctx_cols == ctx_cols &&
+                  c.loop_cols == loop_cols && c.top == top;
+        for (int i = 0; ok && i <= top; i++)
+            ok = c.fr[i].first == fr[i].first && c.fr[i].count == fr[i].count && c.fr[i].k == fr[i].k && c.fr[i].block == fr[i].block &&
+                 c.fr[i].cont == fr[i].cont && (i == top || c.tpos[i] == tpos[i]);
+        for (int i = 0; i < 4; i++) ok = ok && fe_eq(c.sponge[i], sponge[i]);
+        for (int i = 0; i < 32; i++) ok = ok && fe_eq(c.S[i], S[i]);
+        for (int i = 0; i < 16; i++) ok = ok && fe_eq(c.ctx[i], ctx[i]);
+        for (int i = 0; i < 8; i++) ok = ok && fe_eq(c.lp[i], lp[i]);
+        return ok;
+    }
+    // the top of the frame loop: the sequential pass records a checkpoint at the first one at or after every `seg` steps (a buffer too
+    // small is counted on, as the log); a segment stops at the first one at or after `stop`, which must hold the next checkpoint's state
+    __device__ bool boundary(const Frame *fr, int top, const unsigned long long *tpos) {
+        if constexpr (MODE == M_SEQUENTIAL) {
+            if (step >= this->next_cp) {
+                if (this->ncp < this->cp_cap) save(this->cp[this->ncp], fr, top, tpos);
+                this->ncp++;
+                this->next_cp = (step / this->seg + 1) * this->seg;
+            }
+            return false;
+        } else {
+            if (step < this->stop) return false;
+            if (!same(*this->expect, fr, top, tpos)) fail(VM_SEGMENT);
+            return true;
+        }
+    }
+    // the root is closed: the final state goes after the checkpoints (sequential pass), and the last segment must end in it
+    __device__ void ended(const Frame *fr, int top, const unsigned long long *tpos) {
+        if constexpr (MODE == M_SEQUENTIAL) {
+            if (this->ncp < this->cp_cap) save(this->cp[this->ncp], fr, top, tpos);
+        } else if (!same(*this->expect, fr, top, tpos)) {
+            fail(VM_SEGMENT);
+        }
+    }
+
     // run_blocks(root body), then close_block(0, true), with the recursion as a frame stack: a frame is a block list being run, `k` the
-    // next block of it, `cont` what its block does when the list ends.  The host checked that lists nest at most 15 deep.
+    // next block of it, `cont` what its block does when the list ends.  The host checked that lists nest at most 15 deep.  The tabled
+    // passes also keep where each frame below the top resumes in its own chain; a segment starts from the frames of its checkpoint.
     __device__ void run(unsigned root_first, unsigned root_count) {
         Frame fr[16];
+        unsigned long long tpos[TABLED ? 16 : 1];
         int top = 0;
-        fr[0] = Frame{root_first, root_count, 0, 0, C_ROOT};
+        if constexpr (MODE == M_SEGMENT) {
+            const VmCheckpoint &c = *(this->expect - 1);
+            top = c.top;
+            for (int i = 0; i <= top; i++) { fr[i] = c.fr[i]; tpos[i] = c.tpos[i]; }
+        } else {
+            fr[0] = Frame{root_first, root_count, 0, 0, C_ROOT};
+        }
         const fe z = fe_small(0);
         for (;;) {
+            if constexpr (TABLED) { if (boundary(fr, top, tpos)) return; }
             Frame &f = fr[top];
             if (f.k < f.count) {
                 const unsigned bi = L.children[f.first + f.k];
@@ -478,11 +617,19 @@ struct Machine {
                     }
                 }
                 fr[++top] = nf;
+                if constexpr (TABLED) {
+                    tpos[top - 1] = this->at;
+                    this->at = nf.cont == C_SWITCH_FALSE || nf.cont == C_LOOP_SKIP ? this->chains[bi].alt : this->chains[bi].main;
+                }
                 continue;
             }
             const VmBlock &b = L.blocks[f.block];
+            if constexpr (TABLED) this->parent_at = top > 0 ? tpos[top - 1] : this->at + 1;    // the root's end follows its closing NOOP
             switch (f.cont) {
-            case C_ROOT: close_block(z, true); return;
+            case C_ROOT:
+                if (!close_block(z, true)) return;
+                if constexpr (TABLED) ended(fr, top, tpos);
+                return;
             case C_GROUP: if (!close_block(z, true)) return; break;
             case C_SWITCH_TRUE: if (!close_block(b.hash[1], true)) return; break;
             case C_SWITCH_FALSE: if (!close_block(b.hash[0], false)) return; break;
@@ -491,9 +638,11 @@ struct Machine {
                 if (!is_bin(S[0])) { fail(VM_LOOP_EXIT_COND); return; }
                 if (S[0].lo == 1) {
                     if (!wrap_loop()) return;
+                    if constexpr (TABLED) this->at = this->chains[f.block].main;
                     f.k = 0;
                     continue;
                 }
+                if constexpr (TABLED) this->at = this->chains[f.block].brk;
                 if (!break_loop() || !run_span(L.blocks[L.children[b.alt_first]], true) || !close_block(b.hash[2], true)) return;
                 break;
             }
@@ -510,7 +659,7 @@ __global__ void __launch_bounds__(32) vm_kernel(const VmLaunch L) {
     if (e == VM_NO_EXECUTION) return;
     const VmInput in = L.in[e];
     const VmProgram &P = L.programs[in.program];
-    Machine<WRITE> m(L);
+    Machine<WRITE ? M_WRITE : M_SHAPE> m(L);
     m.ta = L.tapes + L.tape_off[e];
     m.cap_a = L.cap[2 * e];
     m.tb = m.ta + m.cap_a;
@@ -567,7 +716,183 @@ __global__ void vm_pad_kernel(fe *out, const VmResult *res, const unsigned *ids,
     c[row] = op_bit ? fe_small(1) : c[r.steps];
 }
 
+// ---- one execution from the sponge table ------------------------------------------------------------------------------------------------
+// One thread per chain of a level (vm.h): the rounds of Machine<M_WRITE>, each at the cycle position its step has (every flow op is aligned
+// to the 16-step cycle, so a step's round constants depend only on its place in its frame).  A child's end_block state is [h, x, y, 0]
+// with h the state before the child: a group's x is its body's result; a switch's (x, y) are its two branch hashes and a loop's its body
+// and skip hashes, which every path through the block must reproduce -- *bad is set where one does not, or where a loop body does not
+// end on its image.
+__global__ void __launch_bounds__(64) vm_table_kernel(const VmLaunch L, const VmChainItem *items, unsigned count, const VmChainRef *chains,
+                                                      VmSponge *tab, unsigned *bad) {
+    const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= count) return;
+    const VmChainItem it = items[q];
+    const fe z = fe_small(0);
+    unsigned long long pos = it.out;
+    fe s[4];
+    auto put = [&] {
+        for (int i = 0; i < 4; i++) tab[pos].s[i] = s[i];
+        pos++;
+    };
+    auto span = [&](const VmBlock &b) {
+        for (unsigned i = 0; i < b.count; i++) {
+            const VmHint &h = L.hints[b.first + i];
+            sponge_round(s, L.ops[b.first + i], h.kind == H_PUSH ? h.value : z, i);
+            put();
+        }
+    };
+    auto noop = [&](unsigned cycle) { sponge_round(s, OP_NOOP, z, cycle); put(); };
+    if (it.kind == VM_CHAIN_BREAK) {                 // from the body's last state: the skip's first span, then close_block's NOOP
+        const VmBlock &b = L.blocks[it.block];
+        const VmSponge &last = tab[chains[it.block].main_close - 1];
+        for (int i = 0; i < 4; i++) s[i] = last.s[i];
+        span(L.blocks[L.children[b.alt_first]]);
+        noop(15);
+        return;
+    }
+    for (int i = 0; i < 4; i++) s[i] = z;
+    bool ok = true;
+    for (unsigned k = 0; k < it.count; k++) {
+        const unsigned bi = L.children[it.first + k];
+        const VmBlock &b = L.blocks[bi];
+        if (b.kind == DG_BLOCK_SPAN) {
+            if (k > 0) noop(15);
+            span(b);
+            continue;
+        }
+        const VmChainRef r = chains[bi];
+        if (b.kind == DG_BLOCK_GROUP) {
+            s[1] = tab[r.main_close].s[0];
+            s[2] = z;
+        } else if (b.kind == DG_BLOCK_SWITCH) {
+            ok = ok && fe_eq(tab[r.main_close].s[0], b.hash[0]) && fe_eq(tab[r.alt_close].s[0], b.hash[1]);
+            s[1] = b.hash[0];
+            s[2] = b.hash[1];
+        } else {
+            ok = ok && fe_eq(tab[r.main_close - 1].s[0], b.hash[0]) && fe_eq(tab[r.brk_close].s[0], b.hash[1]) &&
+                 fe_eq(tab[r.alt_close].s[0], b.hash[2]);
+            s[1] = b.hash[1];
+            s[2] = b.hash[2];
+        }
+        s[3] = z;
+        put();
+        for (unsigned i = 1; i <= 14; i++) noop(i);
+    }
+    noop(15);
+    if (it.tail) {                                   // the root's close_block(0, true): [ctx 0 = 0, root result, 0, 0], then 14 NOOPs
+        s[1] = s[0];
+        s[0] = s[2] = s[3] = z;
+        put();
+        for (unsigned i = 1; i <= 14; i++) noop(i);
+    }
+    if (!ok) atomicOr(bad, 1u);
+}
+
+// the start of execution e, as vm_kernel sets it up
+template <int MODE>
+__device__ void start(Machine<MODE> &m, const VmLaunch &L, const VmInput &in, unsigned e) {
+    m.ta = L.tapes + L.tape_off[e];
+    m.cap_a = L.cap[2 * e];
+    m.tb = m.ta + m.cap_a;
+    m.cap_b = L.cap[2 * e + 1];
+    m.na = m.peak_a = in.n_a;
+    m.nb = m.peak_b = in.n_b;
+    for (unsigned long long i = 0; i < in.n_a; i++) m.ta[i] = L.data[in.a + i];
+    for (unsigned long long i = 0; i < in.n_b; i++) m.tb[i] = L.data[in.b + i];
+    const fe z = fe_small(0);
+    m.set_sponge(z, z, z, z);
+    for (int i = 0; i < 16; i++) m.ctx[i] = z;
+    for (int i = 0; i < 8; i++) m.lp[i] = z;
+    for (int i = 0; i < 32; i++) m.S[i] = (unsigned)i < in.n_pub ? L.data[in.pub + i] : z;
+    m.depth = m.max_depth = in.n_pub;
+}
+
+// The sequential pass of execution L.ids[0] on one thread: the write pass's checks, codes and steps, the sponge from the table, no
+// register writes; VmResult as the shape pass fills it, the checkpoints and the read log
+__global__ void __launch_bounds__(32) vm_sequential_kernel(const VmLaunch L, const VmTabled T, VmSequential *out) {
+    const unsigned e = L.ids[0];
+    const VmInput in = L.in[e];
+    const VmProgram &P = L.programs[in.program];
+    Machine<M_SEQUENTIAL> m(L);
+    start(m, L, in, e);
+    m.tab = T.tab; m.chains = T.chains; m.at = T.root; m.parent_at = 0;
+    m.log = T.log; m.lpos = 0; m.lcap = T.log_cap;
+    m.cp = (VmCheckpoint *)T.checkpoints; m.ncp = 0; m.cp_cap = T.cp_cap; m.next_cp = 0; m.seg = T.segment_steps;
+    m.run(P.root_first, P.root_count);
+    if (!m.failed()) {
+        if (m.opc < 16) m.fail(VM_MIN_OPS);
+        else if (!(fe_eq(m.sponge[0], P.hash[0]) && fe_eq(m.sponge[1], P.hash[1]))) m.fail(VM_HASH);
+    }
+    VmResult &r = L.res[e];
+    r.code = m.code;
+    r.fail_step = m.fail_step;
+    r.steps = m.step;
+    r.op_count = m.opc;
+    r.peak_a = m.peak_a;
+    r.peak_b = m.peak_b;
+    r.ctx_cols = m.ctx_cols;
+    r.loop_cols = m.loop_cols;
+    r.max_depth = m.max_depth;
+    for (int i = 0; i < 8; i++) r.top[i] = m.S[i];
+    out->checkpoints = m.ncp;
+    out->logged = m.lpos;
+}
+
+// Segment q of execution L.ids[0]: from checkpoint q to the first frame-loop boundary at or after checkpoint q + 1's step (the last
+// segment to the end), rows written as the write pass writes them (segment 0 also row 0); codes[2q] = VM_OK, VM_SEGMENT when it does not
+// end in the recorded state, or the failure it met (both internal errors: the sequential pass ran the same execution to the end), and
+// codes[2q + 1] the step it stopped at
+__global__ void __launch_bounds__(32) vm_segment_kernel(const VmLaunch L, const VmTabled T, unsigned long long segments,
+                                                        unsigned long long *codes) {
+    const unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= segments) return;
+    const unsigned e = L.ids[0];
+    const VmCheckpoint *cp = (const VmCheckpoint *)T.checkpoints;
+    Machine<M_SEGMENT> m(L);
+    m.ta = m.tb = nullptr;
+    m.cap_a = m.cap_b = ~0ULL;
+    m.peak_a = m.peak_b = 0;
+    m.tab = T.tab; m.chains = T.chains; m.log = T.log;
+    m.expect = cp + q + 1;
+    m.stop = q + 1 < segments ? cp[q + 1].step : ~0ULL;
+    m.load(cp[q]);
+    const VmOut o = L.outs[e];
+    m.out = L.out + o.offset;
+    m.length = o.length;
+    m.ctx_out = o.ctx_out; m.loop_out = o.loop_out; m.stack_out = o.stack_out;
+    if (q == 0) m.commit_state();
+    m.run(0, 0);
+    codes[2 * q] = m.code;
+    codes[2 * q + 1] = m.fail_step;
+}
+
 }  // namespace
+
+size_t vm_checkpoint_bytes() { return sizeof(VmCheckpoint); }
+
+void vm_table_level(Context &c, const VmLaunch &L, const VmChainItem *items, unsigned count, const VmChainRef *chains, VmSponge *tab,
+                    unsigned *bad) {
+    if (count == 0) return;
+    vm_upload_constants(c);
+    vm_table_kernel<<<(count + 63) / 64, 64, 0, c.stream>>>(L, items, count, chains, tab, bad);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
+void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTabled &T, VmSequential *out) {
+    vm_upload_constants(c);            // RESCR's hasher round
+    vm_sequential_kernel<<<1, 1, 0, c.stream>>>(L, T, out);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
+
+void vm_segment_pass(Context &c, const VmLaunch &L, const VmTabled &T, unsigned long long segments, unsigned long long *codes) {
+    if (segments == 0) return;
+    vm_upload_constants(c);
+    vm_segment_kernel<<<(unsigned)((segments + 31) / 32), 32, 0, c.stream>>>(L, T, segments, codes);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+}
 
 void vm_shape_pass(Context &c, const VmLaunch &L) {
     if (L.count == 0) return;

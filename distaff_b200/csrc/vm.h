@@ -35,6 +35,8 @@ enum VmCode : unsigned {
     VM_NO_STEP, VM_CAP = VM_NO_STEP, VM_MIN_OPS, VM_HASH, VM_TAPE_SCRATCH,
     VM_DIVERGED,                          // the write pass did not retrace the shape pass (a guard: control flow never reads the sponge)
 };
+// the segment pass's guard, beside the VM's codes: a trace segment did not end in the state the sequential pass recorded
+constexpr unsigned VM_SEGMENT = VM_DIVERGED + 1;
 
 // what a pass reports per execution (indexed by execution)
 struct VmResult {
@@ -57,6 +59,44 @@ struct VmLaunch {
     fe *out;
     const VmOut *outs;
 };
+
+// ---- one execution from a sponge table (dg_trace_one / dg_execute_one) ------------------------------------------------------------------
+// The sponge never reads data: with hashes that match their blocks, the state after every step of a block list's frame is a function of
+// the program.  The table holds, per block list, its chain -- the state after each step its frame owns: the span ops, the NOOP before a
+// non-first span, per child block end_block and the 14 NOOPs after it, then the NOOP close_block runs inside the list -- and, per loop,
+// the chain after BREAK (the skip's first span and its closing NOOP, from the body's last state).  The root list's chain continues with
+// the root's end_block and 14 NOOPs.
+struct VmSponge { fe s[4]; };
+// where the chains of a group / switch / loop block start (main: body or true branch; alt: false branch or skip; brk: after BREAK), and the
+// index of their closing entries
+struct VmChainRef { unsigned long long main, alt, brk, main_close, alt_close, brk_close; };
+// one chain to compute: a block list (children[first .. first + count), `tail`: the root's end_block and NOOPs follow its closing NOOP) or
+// the chain after BREAK of loop `block`; written from table index `out` on
+enum : unsigned { VM_CHAIN_LIST, VM_CHAIN_BREAK };
+struct VmChainItem { unsigned kind, first, count, block, tail, pad; unsigned long long out; };
+
+struct VmTabled {
+    VmSponge *tab;
+    const VmChainRef *chains;             // per block (spans unused)
+    unsigned long long root;              // where the root list's chain starts
+    fe *log;                              // every value popped from tape A or B, in order
+    unsigned long long log_cap;
+    void *checkpoints;                    // vm_checkpoint_bytes() each
+    unsigned long long cp_cap, segment_steps;
+};
+// what the sequential pass reports beside VmResult: the checkpoints it recorded (the final state after them: cp_cap must exceed this
+// count) and the values it logged (log_cap must reach it); a pass whose buffers were too small reports the sizes it needed
+struct VmSequential { unsigned long long checkpoints, logged; };
+
+// one launch per level: every item of a level reads only chains of lower levels; inconsistent hashes set *bad
+void vm_table_level(Context &c, const VmLaunch &L, const VmChainItem *items, unsigned count, const VmChainRef *chains, VmSponge *tab,
+                    unsigned *bad);
+// the execution L.ids[0] on one thread, sponge from the table: VmResult as the write pass reports it, plus checkpoints and the read log
+void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTabled &T, VmSequential *out);
+// one thread per segment, one segment per checkpoint: segment q replays from checkpoint q to checkpoint q + 1 (the last one to the final
+// state) and writes its rows of execution L.ids[0] as the write pass does; codes[2q] = VM_OK or why segment q stopped, codes[2q + 1] where
+void vm_segment_pass(Context &c, const VmLaunch &L, const VmTabled &T, unsigned long long segments, unsigned long long *codes);
+size_t vm_checkpoint_bytes();
 
 void vm_upload_constants(Context &c);
 void vm_shape_pass(Context &c, const VmLaunch &L);

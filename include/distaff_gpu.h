@@ -264,6 +264,41 @@ int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint3
                         const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
                         dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
 
+/* ---- executing one long program -------------------------------------------------------------------------------------------------
+ * dg_trace_one / dg_execute_one: one execution of one program, split across GPU threads.  The batch calls above run an execution on one
+ * thread with the sponge, which costs one sponge round per step.  These calls use that the sponge never reads data: when the encoding's
+ * switch and loop hashes match their bodies, the sponge state after every step of a block list is a function of the program, computed
+ * once per call into a table (one launch per nesting level).  The execution then runs once on one thread with the sponge looked up
+ * (every check, code and step of the batch path's write pass; at the first frame-loop boundary at or after every segment_steps steps it
+ * records a checkpoint, and it logs every value read from the tapes), and one thread per checkpoint writes the rows up to the next one.
+ * A straight-line program's table is as long as its trace, so it gains nothing.  An encoding whose hashes do not match on some path
+ * through a switch or loop runs the batch path instead (dg_trace_batch with one input), so results are identical either way; stats say
+ * which path ran.  segment_steps: 0 (the library chooses) or a power of two >= 16.  Arguments are validated as dg_trace_batch /
+ * dg_execute_batch validate them (the encoding, num_outputs <= 8, one GPU) before any launch.  A failed execution returns
+ * DG_ERR_EXECUTION with the message dg_batch_message would give (dg_last_error).
+ * dg_trace_one: info receives the shape; registers_out: NULL (no rows are written) or info->width * info->length * 16 bytes, column-major.
+ * Unlike dg_trace_batch's, a call without registers_out also reports the failures that need the sponge (program hash, loop image).
+ * dg_execute_one: the trace is proven where it was written (dg_prove's bytes for the trace with the execution's public inputs and the
+ * num_outputs elements of the last row's stack top, written to outputs16); prove_stats and info may be NULL. */
+typedef struct {
+    float table_ms, sequential_ms, segment_ms;   /* device time of the table, the sequential pass and the segment pass (with padding);
+                                                    after the fallback, the batch path's shape and write passes */
+    uint64_t table_rounds;       /* sponge rounds of the table */
+    uint64_t table_entries;      /* states in the table */
+    uint32_t table_levels;       /* table launches */
+    uint32_t sequential_launches;/* more than one when the tape scratch, the read log or the checkpoint buffer needed more room */
+    uint64_t checkpoints;        /* checkpoints recorded (one per segment) */
+    uint64_t segments;
+    uint64_t logged;             /* tape values logged */
+    uint64_t segment_steps;      /* S used */
+    int32_t fallback;            /* 1: the encoding's hashes are inconsistent and the batch path ran */
+} dg_trace_one_stats_t;
+int dg_trace_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps,
+                 dg_execution_info_t *info, uint8_t *registers_out, dg_trace_one_stats_t *stats);
+int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
+                   uint64_t segment_steps, const dg_options_t *options, dg_proof_t **proof_out, uint8_t *outputs16, dg_execution_info_t *info,
+                   dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats);
+
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
  * allocates from otherwise, and its persistent tables.  0 (the default) means no limit.  The arena is never sized above the limit and the
