@@ -797,7 +797,7 @@ def find_pow_nonce(seed, grinding_factor=20):
 
 
 def field_op(op, a, b=None, impl=0):
-    code = {"add": 0, "sub": 1, "mul": 2, "inv": 3, "exp": 4, "dot6": 5}[op]
+    code = {"add": 0, "sub": 1, "mul": 2, "inv": 3, "exp": 4, "dot6": 5, "mul_tw": 6}[op]
     fa = np.ascontiguousarray(a, dtype=np.uint64)
     fb = np.ascontiguousarray(b, dtype=np.uint64) if b is not None else None
     out = np.empty_like(fa)

@@ -49,6 +49,10 @@ __global__ void field_op_kernel(int op, int impl, const fe *a, const fe *b, fe *
         return;
     }
     fe x = a[i], y = b ? b[i] : fe_make(0, 0), r;
+    if (op == 6) {                    // a * b through fe_mul_tw, the companion of b computed as the twiddle tables compute it
+        out[i] = impl == 0 ? fe_mul_tw(x, y, fe_tw_companion(y)) : portable::fe_mul_tw(x, y, portable::fe_tw_companion(y));
+        return;
+    }
     if ((impl == 2 || impl == 3) && op == 2) {
 #ifdef __CUDA_ARCH__
         r = impl == 2 ? ptx::fe_mul_v1(x, y) : ptx::fe_mul_v3(x, y);      // earlier multiplies, kept for differential tests
@@ -328,7 +332,7 @@ int dg_field_op(int op, int impl, const uint8_t *a, const uint8_t *b, uint8_t *o
     return guarded([&] {
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        DG_REQUIRE(a && out && n >= 1 && op >= 0 && op <= 5, "invalid argument");
+        DG_REQUIRE(a && out && n >= 1 && op >= 0 && op <= 6, "invalid argument");
         DG_REQUIRE(b || op == 3, "second operand missing");
         DevBuf da(n * 16), db(n * 16), dout(n * 16);
         DG_CUDA(cudaMemcpyAsync(da.p, a, n * 16, cudaMemcpyHostToDevice, c.stream));

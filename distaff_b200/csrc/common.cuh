@@ -125,7 +125,8 @@ struct Context {
     std::function<void(const char *)> mark;     // optional sub-stage marker of the running proof (DG_SUBSTAGE), else empty
     cudaStream_t comm_stream = nullptr;     // collectives that overlap compute (the all-gather of the trace polynomials)
     std::mutex mu;
-    // small root tables for the in-shared-memory transforms: roots[inv][l] = w_{2^l}^m, m < 2^(l-1), l = 1..MAX_LOG_L
+    // small root tables for the in-shared-memory transforms: per size 2^l (l = 1..MAX_LOG_L) the per-stage roots, then their fe_mul_tw
+    // companions (context.cu)
     DevBuf small_roots[2];
     size_t small_root_offset[16];
     std::map<int, TwiddleTable> twiddles;   // key = log_order * 2 + inverse
@@ -151,6 +152,8 @@ struct Context {
     TwiddleRef twiddle(int log_order, bool inverse);
     std::map<int, DevBuf> single_tables;    // full power tables w^e, e < 2^log_order (small orders only)
     const fe *single_table(int log_order);
+    std::map<int, DevBuf> single_tables_tw; // the same powers interleaved with their fe_mul_tw companions: (w^e, w^e * 2^64)
+    const fe *single_table_tw(int log_order);
     std::map<long long, DevBuf> lde_twiddles;   // per (log_n, log_blowup, first pass size): merged lane/coset twiddles of the LDE's first pass (ntt.cu)
     const fe *roots(int log_l, bool inverse) const { return small_roots[inverse ? 1 : 0].as<fe>() + small_root_offset[log_l]; }
 };

@@ -21,6 +21,19 @@ __global__ void power_table_kernel(fe *out, fe step, unsigned count) {
     unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count) out[i] = fe_pow_u64(step, i);
 }
+// companions of fixed twiddles for fe_mul_tw: out[i] = in[i] * 2^64
+__global__ void companion_table_kernel(fe *out, const fe *in, unsigned count) {
+    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < count) out[i] = fe_tw_companion(in[i]);
+}
+// (w^e, w^e * 2^64) pairs, e < count, interleaved
+__global__ void power_pair_table_kernel(fe *out, fe step, unsigned count) {
+    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const fe w = fe_pow_u64(step, i);
+    out[2 * i] = w;
+    out[2 * i + 1] = fe_tw_companion(w);
+}
 
 static thread_local Context *tl_ctx = nullptr;
 cudaStream_t &alloc_stream() { return ctx().stream; }
@@ -159,9 +172,10 @@ static Context *build_context(int device) {
     }
     // small root tables
     // per-stage tables of every sub-transform size L = 2^l: stage st occupies [L - (L >> st), L - (L >> (st+1))) with
-    // W_st[j] = w_L^(j << st), j < L >> (st+1); L entries reserved per size (the last one is unused)
+    // W_st[j] = w_L^(j << st), j < L >> (st+1); L entries reserved per size (the last one is unused), followed by the L companions
+    // W_st[j] * 2^64 of fe_mul_tw at the same positions + L
     size_t total = 0;
-    for (int l = 1; l <= MAX_LOG_L; l++) { c->small_root_offset[l] = total; total += (size_t)1 << l; }
+    for (int l = 1; l <= MAX_LOG_L; l++) { c->small_root_offset[l] = total; total += (size_t)2 << l; }
     c->small_root_offset[0] = 0;
     for (int inv = 0; inv < 2; inv++) {
         c->small_roots[inv].alloc(total * sizeof(fe), true);
@@ -177,6 +191,9 @@ static Context *build_context(int device) {
                 DG_CUDA(cudaGetLastError());
                 w = fe_sqr(w);
             }
+            fe *roots = c->small_roots[inv].as<fe>() + c->small_root_offset[l];
+            companion_table_kernel<<<(L + 127) / 128, 128, 0, c->stream>>>(roots + L, roots, L);
+            DG_CUDA(cudaGetLastError());
         }
     }
     DG_CUDA(cudaStreamSynchronize(c->stream));
@@ -258,6 +275,20 @@ const fe *Context::single_table(int log_order) {
         power_table_kernel<<<(cnt + 127) / 128, 128, 0, stream>>>(t.as<fe>(), host_root_of_unity(log_order), cnt); launches++;
         DG_CUDA(cudaGetLastError());
         it = single_tables.emplace(log_order, std::move(t)).first;
+    }
+    return it->second.as<fe>();
+}
+
+const fe *Context::single_table_tw(int log_order) {
+    DG_REQUIRE(log_order <= 20, "single-level table too large");
+    auto it = single_tables_tw.find(log_order);
+    if (it == single_tables_tw.end()) {
+        DevBuf t;
+        t.alloc(((size_t)2 << log_order) * sizeof(fe), true);
+        const unsigned cnt = 1u << log_order;
+        power_pair_table_kernel<<<(cnt + 127) / 128, 128, 0, stream>>>(t.as<fe>(), host_root_of_unity(log_order), cnt); launches++;
+        DG_CUDA(cudaGetLastError());
+        it = single_tables_tw.emplace(log_order, std::move(t)).first;
     }
     return it->second.as<fe>();
 }

@@ -81,6 +81,12 @@ __host__ __device__ inline fe fe_pow_u128(fe a, unsigned long long e_lo, unsigne
 }
 __host__ __device__ inline fe fe_pow_u64(fe a, unsigned long long e) { return fe_pow_u128(a, e, 0); }
 __host__ __device__ inline fe fe_inv(fe a) { return fe_pow_u128(a, DG_M_LO - 2ULL, DG_M_HI); }
+// the companion of a twiddle for fe_mul_tw: w * 2^64 mod M
+__host__ __device__ inline fe fe_tw_companion(fe w) { return fe_mul(w, fe_make(0, 1)); }
+// a0*w + a1*w_c mod M for a = a1*2^64 + a0: a*w when w_c is w's companion
+__host__ __device__ inline fe fe_mul_tw(fe a, fe w, fe w_c) {
+    return fe_add(fe_mul(fe_make(a.lo, 0), w), fe_mul(fe_make(a.hi, 0), w_c));
+}
 
 
 }  // namespace portable
@@ -428,6 +434,84 @@ __device__ __forceinline__ fe fe_mul_v4t(fe a, fe b) {
     return fe_reduce_v4<NESTED_CALL>(r);
 }
 __device__ __forceinline__ fe fe_mul_v4(fe a, fe b) { return fe_mul_v4t<true>(a, b); }
+// ---- product with a fixed twiddle w and its companion w_c = w * 2^64 mod M (fe_tw_companion) -----------------------------------------
+// For a = a1*2^64 + a0:  a*w == a0*w + a1*w_c (mod M).  Both products are 64 x 128 bits, so the 16 IMAD.WIDE of a full product sum
+// into columns 0..6 only (a0*w + a1*w_c < 2^193), and the reduction is v4's second fold alone, widened to a 65-bit top.
+// tools/model_mul_tw.py restates every chain below and checks its bounds against Python integers.
+template <bool NESTED_CALL>
+__device__ __forceinline__ fe fe_mul_twt(fe a, fe w, fe w_c) {
+    const unsigned int x0 = (unsigned int)a.lo, x1 = (unsigned int)(a.lo >> 32), x2 = (unsigned int)a.hi, x3 = (unsigned int)(a.hi >> 32);
+    const unsigned int y0 = (unsigned int)w.lo, y1 = (unsigned int)(w.lo >> 32), y2 = (unsigned int)w.hi, y3 = (unsigned int)(w.hi >> 32);
+    const unsigned int z0 = (unsigned int)w_c.lo, z1 = (unsigned int)(w_c.lo >> 32), z2 = (unsigned int)w_c.hi, z3 = (unsigned int)(w_c.hi >> 32);
+    // E = even columns 0, 2, 4, 6 ; O = odd columns 1, 3, 5 (64-bit accumulators as in mul_wide_eo)
+    unsigned int e0, e1, e2, e3, e4, e5, e6, o1, o2, o3, o4, o5;
+    // x0 * w at column 0: E0 = x0 y0, E2 = x0 y2, O1 = x0 y1, O3 = x0 y3
+    asm("mul.lo.u32 %0, %8, %9;\n\t"  "mul.hi.u32 %1, %8, %9;\n\t"
+        "mul.lo.u32 %2, %8, %11;\n\t" "mul.hi.u32 %3, %8, %11;\n\t"
+        "mul.lo.u32 %4, %8, %10;\n\t" "mul.hi.u32 %5, %8, %10;\n\t"
+        "mul.lo.u32 %6, %8, %12;\n\t" "mul.hi.u32 %7, %8, %12;"
+        : "=&r"(e0), "=&r"(e1), "=&r"(e2), "=&r"(e3), "=&r"(o1), "=&r"(o2), "=&r"(o3), "=&r"(o4)
+        : "r"(x0), "r"(y0), "r"(y1), "r"(y2), "r"(y3));
+    // x2 * w_c at column 0: E0 += x2 z0 ; E2 += x2 z2 + c ; E4 = c        O1 += x2 z1 ; O3 += x2 z3 + c ; O5 = c
+    asm("mad.lo.cc.u32  %0, %10, %11, %0;\n\t" "madc.hi.cc.u32 %1, %10, %11, %1;\n\t"
+        "madc.lo.cc.u32 %2, %10, %13, %2;\n\t" "madc.hi.cc.u32 %3, %10, %13, %3;\n\t"
+        "addc.u32       %4, 0, 0;\n\t"
+        "mad.lo.cc.u32  %5, %10, %12, %5;\n\t" "madc.hi.cc.u32 %6, %10, %12, %6;\n\t"
+        "madc.lo.cc.u32 %7, %10, %14, %7;\n\t" "madc.hi.cc.u32 %8, %10, %14, %8;\n\t"
+        "addc.u32       %9, 0, 0;"
+        : "+r"(e0), "+r"(e1), "+r"(e2), "+r"(e3), "=&r"(e4), "+r"(o1), "+r"(o2), "+r"(o3), "+r"(o4), "=&r"(o5)
+        : "r"(x2), "r"(z0), "r"(z1), "r"(z2), "r"(z3));
+    // x1 * w at column 1: O1 += x1 y0 ; O3 += x1 y2 + c ; O5 += c         E2 += x1 y1 ; E4:E5 = x1 y3 + E4 + c
+    asm("mad.lo.cc.u32  %0, %9, %10, %0;\n\t" "madc.hi.cc.u32 %1, %9, %10, %1;\n\t"
+        "madc.lo.cc.u32 %2, %9, %12, %2;\n\t" "madc.hi.cc.u32 %3, %9, %12, %3;\n\t"
+        "addc.u32       %4, %4, 0;\n\t"
+        "mad.lo.cc.u32  %5, %9, %11, %5;\n\t" "madc.hi.cc.u32 %6, %9, %11, %6;\n\t"
+        "madc.lo.cc.u32 %7, %9, %13, %7;\n\t" "madc.hi.u32    %8, %9, %13, 0;"
+        : "+r"(o1), "+r"(o2), "+r"(o3), "+r"(o4), "+r"(o5), "+r"(e2), "+r"(e3), "+r"(e4), "=&r"(e5)
+        : "r"(x1), "r"(y0), "r"(y1), "r"(y2), "r"(y3));
+    // x3 * w_c at column 1: O1 += x3 z0 ; O3 += x3 z2 + c ; O5 += c       E2 += x3 z1 ; E4 += x3 z3 + c ; E6 = c
+    asm("mad.lo.cc.u32  %0, %10, %11, %0;\n\t" "madc.hi.cc.u32 %1, %10, %11, %1;\n\t"
+        "madc.lo.cc.u32 %2, %10, %13, %2;\n\t" "madc.hi.cc.u32 %3, %10, %13, %3;\n\t"
+        "addc.u32       %4, %4, 0;\n\t"
+        "mad.lo.cc.u32  %5, %10, %12, %5;\n\t" "madc.hi.cc.u32 %6, %10, %12, %6;\n\t"
+        "madc.lo.cc.u32 %7, %10, %14, %7;\n\t" "madc.hi.cc.u32 %8, %10, %14, %8;\n\t"
+        "addc.u32       %9, 0, 0;"
+        : "+r"(o1), "+r"(o2), "+r"(o3), "+r"(o4), "+r"(o5), "+r"(e2), "+r"(e3), "+r"(e4), "+r"(e5), "=&r"(e6)
+        : "r"(x3), "r"(z0), "r"(z1), "r"(z2), "r"(z3));
+    // r = E + (O << 32): columns 0..6, r6 <= 1 because the sum is < 2^193
+    unsigned int r1, r2, r3, r4, r5, r6;
+    asm("add.cc.u32  %0, %6, %12;\n\t"
+        "addc.cc.u32 %1, %7, %13;\n\t"
+        "addc.cc.u32 %2, %8, %14;\n\t"
+        "addc.cc.u32 %3, %9, %15;\n\t"
+        "addc.cc.u32 %4, %10, %16;\n\t"
+        "addc.u32    %5, %11, 0;"
+        : "=&r"(r1), "=&r"(r2), "=&r"(r3), "=&r"(r4), "=&r"(r5), "=&r"(r6)
+        : "r"(e1), "r"(e2), "r"(e3), "r"(e4), "r"(e5), "r"(e6), "r"(o1), "r"(o2), "r"(o3), "r"(o4), "r"(o5));
+    // fold the 65-bit top T = r6:r5:r4:  + (T*K) << 32 on a multiply-add chain (T*K < 2^79), then - T.  The result is non-negative and
+    // < 2^128 + 2^111: cy below is carry - borrow in {0, 1}
+    const unsigned int K = 11520u, one = 1u;
+    unsigned int v0 = e0;
+    unsigned long long u1 = wmad(r4, K, (unsigned long long)r1);
+    unsigned long long u2 = wmad(r2, one, wmad(r5, K, u1 >> 32));
+    unsigned long long u3 = wmad(r3, one, wmad(r6, K, u2 >> 32));
+    unsigned int v1 = (unsigned int)u1, v2 = (unsigned int)u2, v3 = (unsigned int)u3, cy = (unsigned int)(u3 >> 32);
+    asm("sub.cc.u32  %0, %0, %5;\n\t"
+        "subc.cc.u32 %1, %1, %6;\n\t"
+        "subc.cc.u32 %2, %2, %7;\n\t"
+        "subc.cc.u32 %3, %3, 0;\n\t"
+        "subc.u32    %4, %4, 0;"
+        : "+r"(v0), "+r"(v1), "+r"(v2), "+r"(v3), "+r"(cy) : "r"(r4), "r"(r5), "r"(r6));
+    // canonical unless it overflowed 2^128 or lies in [2^128 - 2^96, 2^128): the same rare path as fe_reduce_v4
+    if (__builtin_expect((cy != 0u) | (v3 == 0xffffffffu), 0)) {
+        if (NESTED_CALL) return fe_canon_slow(v0, v1, v2, v3, cy);
+        return fe_canon_inline(v0, v1, v2, v3, cy);
+    }
+    fe out;
+    out.lo = ((unsigned long long)v1 << 32) | v0;
+    out.hi = ((unsigned long long)v3 << 32) | v2;
+    return out;
+}
 // ---- unreduced accumulation: sums of up to 128 products are kept as 288-bit integers and reduced once ------------------------------
 // A dot product sum_j a_j b_j costs, per term, one 256-bit product (16 IMAD.WIDE + 13 ALU) and one 9-limb addition (9 ALU) instead of a
 // full modular multiplication and a modular addition (31 + 13 ALU); the single reduction at the end is the v4 fold extended by one limb
@@ -493,7 +577,8 @@ __device__ __forceinline__ fe fe_reduce_wide(const fe_wide &w) {
     out.hi = ((unsigned long long)v3 << 32) | v2;
     return out;
 }
-// the multiply used by every kernel (tools/bench_modmul.cu on an H100 SXM, 700 W: v1 204, v3 249, v4 266 G modmul/s; butterfly mix 163 / 183 / 200 G/s)
+// the multiply used by every kernel (tools/bench_modmul.cu on an H100 SXM, 700 W: v1 204, v3 249, v4 266 G modmul/s; butterfly mix 163 / 183 / 200 G/s;
+// fe_mul_tw above, for fixed twiddles with companions: 340 G modmul/s, 244 G butterflies/s)
 #ifdef DG_MUL_CALL
 // out-of-line variant for kernels whose fully inlined code would not fit the instruction caches
 static __device__ __noinline__ fe fe_mul_call(fe a, fe b) { return fe_mul_v4t<false>(a, b); }
@@ -557,6 +642,14 @@ __host__ __device__ __forceinline__ fe fe_pow_u64(fe a, unsigned long long e) { 
 __host__ __device__ __forceinline__ fe fe_pow_u128(fe a, unsigned long long lo, unsigned long long hi) { return DG_IMPL::fe_pow_u128(a, lo, hi); }
 __host__ __device__ __forceinline__ fe fe_inv(fe a) { return DG_IMPL::fe_inv(a); }
 __host__ __device__ __forceinline__ fe fe_cube(fe a) { return fe_mul(fe_sqr(a), a); }
+__host__ __device__ __forceinline__ fe fe_tw_companion(fe w) { return portable::fe_tw_companion(w); }
+__host__ __device__ __forceinline__ fe fe_mul_tw(fe a, fe w, fe w_c) {
+#ifdef __CUDA_ARCH__
+    return ptx::fe_mul_twt<true>(a, w, w_c);
+#else
+    return portable::fe_mul_tw(a, w, w_c);
+#endif
+}
 __host__ __device__ __forceinline__ fe fe_mul_small(fe a, unsigned int k) {
 #ifdef __CUDA_ARCH__
     return ptx::fe_mul_small(a, k);

@@ -48,13 +48,15 @@ static int pass_kind(const PassGeom &g) {
 //   measured before the kernels were specialised per pass kind (every kind's path in one kernel, a call per multiply):
 //   rmax 3 for A and B 60.8 - 61.3;  A = 256 threads 68.0;  A = 1024 threads + 8192-element tiles 71.7;  B = 256 threads 62.5;
 //   AF = 8-element units or 256 threads: no change in stages 5 / 6
-// The other shapes were removed after this measurement.
+// The other shapes were removed after this measurement.  With the butterflies through fe_mul_tw (the companions double s_tw to 2L entries:
+// 96 KiB per strided and 104 KiB per lane-major 1024-point block, still two blocks per SM) the same shape measured stage 1 at 49.4 - 49.5 ms
+// against 52.4 - 52.7 ms, four runs each, alternating, H100 80GB HBM3 at 700 W; with tw_full stored as (w, w_c) pairs as well, 51.9 ms.
 static const int TILE = 4096;                    // elements per block = 64 KB
 
 static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *dst, unsigned blocks_x, unsigned by, unsigned bz) {
     const int L = 1 << log_l, T = 1 << g.log_t;
     const size_t data = g.lane_major ? (size_t)T * (L + (L >> 3) + 1) : (size_t)L * T;
-    const size_t smem = ((size_t)L + data) * sizeof(fe);
+    const size_t smem = ((size_t)2 * L + data) * sizeof(fe);      // stage roots and their companions, then the data
     const int kind = pass_kind(g);
     const PassKernel k = log_l >= PASS_INLINE_LOG_L ? pass_kernel_inline(kind, log_l)
                                                     : pass_kernel_of<PASS_RMAX, PASS_THREADS, PASS_MINB, 0, 1, PASS_INLINE_LOG_L - 1>(kind, log_l);
@@ -137,7 +139,7 @@ static void run_transform(Context &c, const fe *src, fe *dst, int log_n, bool in
             // order of w_N^in_point where in_point = n / N1 (first pass) : N / in_point = N1 << log_blowup
             const int log_order = l[0] + cs.log_blowup;
             base.coset_fast = 1;
-            base.cw_point = c.single_table(log_order);
+            base.cw_point = c.single_table_tw(log_order);
             base.cw_point_mask = (1u << log_order) - 1u;
         }
     }

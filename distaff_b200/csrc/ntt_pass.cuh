@@ -21,6 +21,9 @@ enum PassKind {
 __host__ __device__ constexpr bool pk_lane_major(int k) { return k >= PK_LAST; }
 __host__ __device__ constexpr bool pk_coset_in(int k) { return k == PK_COSET_TWFULL || k == PK_COSET_TW || k == PK_COSET_ONE; }
 __host__ __device__ constexpr bool pk_fold_in(int k) { return k == PK_FOLD_TW || k == PK_FOLD_ONE; }
+// butterflies through fe_mul_tw with the stage roots' companions.  The kinds whose output factor comes from the two-level table keep fe_mul:
+// with the companions they spill at the 64-register cap.
+__host__ __device__ constexpr bool pk_mul_tw(int k) { return k != PK_TW && k != PK_COSET_TW && k != PK_FOLD_TW; }
 
 struct PassGeom {
     int log_t;                          // lanes per block (power of two)
@@ -39,13 +42,14 @@ struct PassGeom {
     int fold;
     long long fold_stride;
     TwiddleRef cw;
-    const fe *cw_point;                 // cw_point[e] = (w_N^in_point)^e, e < cw_point_mask + 1
+    const fe *cw_point;                 // (cw_point[2e], cw_point[2e + 1]) = ((w_N^in_point)^e, its fe_mul_tw companion), e < cw_point_mask + 1
     unsigned cw_point_mask;
     const fe *tw_full;                  // coset_fast: tw_full[coset][k * out_point + lane] = cw^(lane * (k * blowup + coset)), or null
     long long tw_full_stride;           // elements per coset (= transform size n)
     int log_blowup;
     unsigned coset0;                    // first coset handled by this launch (blockIdx.y = coset - coset0)
-    const fe *roots;                    // per-stage twiddle tables of the L-point transform: W_st[j] = w_L^(j << st), back to back
+    const fe *roots;                    // per-stage twiddle tables of the L-point transform: W_st[j] = w_L^(j << st), back to back (L entries),
+                                        // then their fe_mul_tw companions (L entries)
 };
 
 // The pass kernels' multiply.  ntt.cu: the shared out-of-line body.  ntt_inl.cu: v4 inlined with its rare canonicalisation as a plain
@@ -55,6 +59,17 @@ __device__ __forceinline__ fe ntt_mul(fe a, fe b) {
     return ptx::fe_mul_v4t<false>(a, b);
 #else
     return fe_mul(a, b);
+#endif
+}
+
+// a product with a fixed twiddle w and its companion w_c = w * 2^64 (fe_mul_tw): inlined in ntt_inl.cu; ntt.cu keeps its one shared
+// out-of-line multiply and ignores the companion
+__device__ __forceinline__ fe ntt_mul_tw(fe a, fe w, fe w_c) {
+#if defined(__CUDA_ARCH__) && !defined(DG_MUL_CALL)
+    return ptx::fe_mul_twt<false>(a, w, w_c);
+#else
+    (void)w_c;
+    return fe_mul(a, w);
 #endif
 }
 
@@ -70,8 +85,9 @@ __device__ __forceinline__ fe tw_lookup(const TwiddleRef &t, unsigned long long 
 // up to RMAX stages that run entirely in registers on 2^rho elements per thread ("unit"); shared memory is touched only
 // between rounds.  The first round reads its operands straight from global memory and the last one writes straight back.
 // RMAX = 2: 4 elements per unit, 5 rounds for 1024 points (small unrolled bodies, few registers, many resident warps).
-// Stage twiddles come from per-stage compact tables W_st[j] = w_L^(j << st) (unit-stride, conflict-free) staged in shared memory.
-template <int LOG_L, int S0, int RHO>
+// Stage twiddles come from per-stage compact tables W_st[j] = w_L^(j << st) (unit-stride, conflict-free) staged in shared memory, their
+// companions L entries further on.
+template <int LOG_L, int S0, int RHO, bool TWC>
 __device__ __forceinline__ void dif_regs(fe *x, const fe *s_tw, int g_lo) {
     constexpr int L = 1 << LOG_L, R = 1 << RHO;
     constexpr int LOG_SP = LOG_L - S0 - RHO;
@@ -87,7 +103,10 @@ __device__ __forceinline__ void dif_regs(fe *x, const fe *s_tw, int g_lo) {
                 x[i] = fe_add(a, b);
                 fe d = fe_sub(a, b);
                 // in the last round (LOG_SP == 0, g_lo == 0) the twiddle index is a compile-time constant: index 0 is w^0 = 1
-                if (st != LOG_L - 1 && !(LOG_SP == 0 && (i & (hr - 1)) == 0)) d = ntt_mul(d, W[g_lo + ((i & (hr - 1)) << LOG_SP)]);
+                if (st != LOG_L - 1 && !(LOG_SP == 0 && (i & (hr - 1)) == 0)) {
+                    const int e = g_lo + ((i & (hr - 1)) << LOG_SP);
+                    d = TWC ? ntt_mul_tw(d, W[e], W[L + e]) : ntt_mul(d, W[e]);
+                }
                 x[i + hr] = d;
             }
         }
@@ -132,7 +151,9 @@ __device__ __forceinline__ void ntt_round(const fe *__restrict__ src, fe *__rest
                 const long long j = in_base + (long long)t * g.in_lane + (long long)pos * g.in_point;
                 if (pk_coset_in(KIND)) {
                     // p[j] * w_N^(c*pos*in_point); the lane part w_N^(c*lane) rides on the output twiddle
-                    x[m] = ntt_mul(src[j], g.cw_point[((g.coset0 + (unsigned)blockIdx.y) * (unsigned)pos) & g.cw_point_mask]);
+                    const fe *cw = g.cw_point + 2 * (((g.coset0 + (unsigned)blockIdx.y) * (unsigned)pos) & g.cw_point_mask);
+                    // fe_mul_tw only in the one-pass kind: next to the tw_full product's fe_mul (and in PK_COSET_TW) it spills
+                    x[m] = KIND == PK_COSET_ONE ? ntt_mul_tw(src[j], cw[0], cw[1]) : ntt_mul(src[j], cw[0]);
                 } else if (pk_fold_in(KIND)) {
                     // sum_f src[j + f n] w_N^(c (j + f n)) = w_N^(c j) * Horner_f(src[j + f n]; u),  u = w_N^(c n) (constant per coset)
                     const unsigned long long c = g.coset0 + blockIdx.y;
@@ -147,14 +168,16 @@ __device__ __forceinline__ void ntt_round(const fe *__restrict__ src, fe *__rest
                 x[m] = s_data[sidx<LOG_L, LANE_MAJOR>(pos, t, T)];
             }
         }
-        dif_regs<LOG_L, S0, RHO>(x, s_tw, g_lo);
+        dif_regs<LOG_L, S0, RHO, pk_mul_tw(KIND)>(x, s_tw, g_lo);
 #pragma unroll
         for (int m = 0; m < R; m++) {
             const int pos = gbase + (m << LOG_SP);
             if (LAST) {                        // position q holds X[bitrev(q)]
                 const unsigned k = __brev((unsigned)pos) >> (32 - LOG_L);
                 fe v = x[m];
-                if (KIND == PK_COSET_TWFULL)   // streamed table in the layout of the output: one 16-byte load instead of two loads and a multiplication
+                // streamed table in the layout of the output: one 16-byte load instead of two loads and a multiplication.  It keeps fe_mul:
+                // every column streams the whole table again, and companions beside it would double that traffic
+                if (KIND == PK_COSET_TWFULL)
                     v = ntt_mul(v, g.tw_full[(long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)(tile * T + t) * g.out_lane + (long long)k * g.out_point]);
                 else if (KIND == PK_COSET_TW)
                     v = ntt_mul(v, tw_lookup(g.cw, (unsigned long long)(tile * T + t) * (((unsigned long long)k << g.log_blowup) + g.coset0 + blockIdx.y)));
@@ -185,15 +208,15 @@ template <int LOG_L, int KIND, int RMAX, int BT, int MINB, int TAG>
 __global__ void __launch_bounds__(BT, MINB) ntt_pass_kernel(const fe *__restrict__ src, fe *__restrict__ dst, const PassGeom g) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     constexpr int L = 1 << LOG_L;
-    fe *s_tw = reinterpret_cast<fe *>(smem_raw);          // L entries: per-stage tables back to back
-    fe *s_data = s_tw + L;
+    fe *s_tw = reinterpret_cast<fe *>(smem_raw);          // 2L entries: per-stage tables back to back, then their companions
+    fe *s_data = s_tw + 2 * L;
     const int T = 1 << g.log_t;
     const unsigned tile = blockIdx.x % g.num_tiles, outer = blockIdx.x / g.num_tiles;
     const long long in_base = (long long)outer * g.in_outer + (long long)tile * T * g.in_lane;   // index inside the vector
     src += (long long)blockIdx.y * g.in_batch_y + (long long)blockIdx.z * g.in_batch_z;
     dst += (long long)blockIdx.y * g.out_batch_y + (long long)blockIdx.z * g.out_batch_z + (long long)outer * g.out_outer +
            (long long)tile * T * g.out_lane;
-    for (int i = threadIdx.x; i < L - 1; i += blockDim.x) s_tw[i] = g.roots[i];
+    for (int i = threadIdx.x; i < 2 * L; i += blockDim.x) s_tw[i] = g.roots[i];
     if (KIND == PK_COSET_TWFULL) {
         // the streamed twiddles are consumed in the last round: start pulling this block's T*16-byte segments (one per output k) into L2 now
         const fe *tb = g.tw_full + (long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)tile * T * g.out_lane;

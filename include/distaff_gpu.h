@@ -403,7 +403,8 @@ int dg_find_pow_nonce(const uint8_t seed[32], uint32_t grinding_factor, uint64_t
 #define DG_HASH_POSEIDON 2
 int dg_hash64(int hash, const uint8_t *messages64, uint64_t n, uint8_t *digests32);
 int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uint8_t *nodes);
-/* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b)), for differential tests of the arithmetic;
+/* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b), 6 mul with b as a fixed twiddle: the NTT pass
+ * kernels' product with a precomputed companion b * 2^64), for differential tests of the arithmetic;
  * impl: 0 = PTX path used by the kernels, 1 = portable C++ path, 2 / 3 = earlier PTX multiplies (op 2 only) */
 int dg_field_op(int op, int impl, const uint8_t *a, const uint8_t *b, uint8_t *out, uint64_t n);
 /* out[i] = sum_j a[len*i + j] * b[len*i + j], j < len (1..128), accumulated unreduced in 288 bits and reduced once, as the kernels' dot

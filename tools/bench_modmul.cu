@@ -7,31 +7,34 @@
 using namespace dg;
 
 #define DG_HAVE_V3 1
-template <int V> __device__ __forceinline__ fe mulv(fe a, fe b) {
+// V = 5: fe_mul_tw, b a fixed twiddle with its companion bc = b * 2^64 mod M
+template <int V> __device__ __forceinline__ fe mulv(fe a, fe b, fe bc) {
 #ifdef __CUDA_ARCH__
+    if (V == 5) return ptx::fe_mul_twt<false>(a, b, bc);
     if (V == 1) return ptx::fe_mul_v1(a, b);
     if (V == 2) return ptx::fe_mul_v3(a, b);
     if (V == 3) return ptx::fe_mul_v4(a, b);
     if (V == 4) return ptx::fe_mul_v4t<false>(a, b);      // the NTT pass kernels' multiply: rare canonicalisation inline, no call
 #endif
+    (void)bc;
     return portable::fe_mul(a, b);
 }
 
 template <int V>
-__global__ void __launch_bounds__(256) tput(const fe *in, fe *out, int iters) {
+__global__ void __launch_bounds__(256) tput(const fe *in, const fe *inc, fe *out, int iters) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    fe x0 = in[i], x1 = in[i + 1], x2 = in[i + 2], x3 = in[i + 3], m = in[i + 4];
-    for (int k = 0; k < iters; k++) { x0 = mulv<V>(x0, m); x1 = mulv<V>(x1, m); x2 = mulv<V>(x2, m); x3 = mulv<V>(x3, m); }
+    fe x0 = in[i], x1 = in[i + 1], x2 = in[i + 2], x3 = in[i + 3], m = in[i + 4], mc = inc[i + 4];
+    for (int k = 0; k < iters; k++) { x0 = mulv<V>(x0, m, mc); x1 = mulv<V>(x1, m, mc); x2 = mulv<V>(x2, m, mc); x3 = mulv<V>(x3, m, mc); }
     out[i] = fe_add(fe_add(x0, x1), fe_add(x2, x3));
 }
 // butterfly-like mix: add, sub, mul
 template <int V>
-__global__ void __launch_bounds__(256) tput_bfly(const fe *in, fe *out, int iters) {
+__global__ void __launch_bounds__(256) tput_bfly(const fe *in, const fe *inc, fe *out, int iters) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
-    fe a = in[i], b = in[i + 1], c = in[i + 2], d = in[i + 3], w = in[i + 4];
+    fe a = in[i], b = in[i + 1], c = in[i + 2], d = in[i + 3], w = in[i + 4], wc = inc[i + 4];
     for (int k = 0; k < iters; k++) {
-        fe s = fe_add(a, b), t = mulv<V>(fe_sub(a, b), w); a = s; b = t;
-        fe s2 = fe_add(c, d), t2 = mulv<V>(fe_sub(c, d), w); c = s2; d = t2;
+        fe s = fe_add(a, b), t = mulv<V>(fe_sub(a, b), w, wc); a = s; b = t;
+        fe s2 = fe_add(c, d), t2 = mulv<V>(fe_sub(c, d), w, wc); c = s2; d = t2;
     }
     out[i] = fe_add(fe_add(a, b), fe_add(c, d));
 }
@@ -87,15 +90,15 @@ template <int MODE> void run_call(const char *name, fe *d_in, fe *d_out, int blo
     printf("%-22s %8.3f ms  %7.1f Gbfly/s (16 warps/SM)\n", name, best, (double)blocks * 256 * iters * 4 / best / 1e6);
 }
 
-template <int V> __global__ void check(const fe *a, const fe *b, fe *o, int n) { int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) o[i] = mulv<V>(a[i], b[i]); }
+template <int V> __global__ void check(const fe *a, const fe *b, const fe *bc, fe *o, int n) { int i = blockIdx.x * blockDim.x + threadIdx.x; if (i < n) o[i] = mulv<V>(a[i], b[i], bc[i]); }
 
-template <int V> void run(const char *name, fe *d_in, fe *d_out, int blocks, int iters) {
+template <int V> void run(const char *name, fe *d_in, fe *d_inc, fe *d_out, int blocks, int iters) {
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
     for (int kind = 0; kind < 2; kind++) {
         float best = 1e9;
         for (int rep = 0; rep < 3; rep++) {
             cudaEventRecord(e0);
-            if (kind == 0) tput<V><<<blocks, 256>>>(d_in, d_out, iters); else tput_bfly<V><<<blocks, 256>>>(d_in, d_out, iters);
+            if (kind == 0) tput<V><<<blocks, 256>>>(d_in, d_inc, d_out, iters); else tput_bfly<V><<<blocks, 256>>>(d_in, d_inc, d_out, iters);
             cudaEventRecord(e1); cudaEventSynchronize(e1);
             float ms; cudaEventElapsedTime(&ms, e0, e1); if (ms < best) best = ms;
         }
@@ -123,28 +126,35 @@ int main() {
         if (f) { fe ab[2]; int cnt = 0; while (fread(ab, 16, 2, f) == 2) { ea.push_back(ab[0]); eb.push_back(ab[1]); cnt++; } fclose(f); printf("%d crafted pairs\n", cnt); }
         else printf("tools/_bin/mul_vectors.bin not found: crafted pairs skipped\n");
     }
-    fe *d_in, *d_out, *da, *db, *d0, *d1;
-    cudaMalloc(&d_in, n * 16); cudaMalloc(&d_out, n * 16);
-    cudaMemcpy(d_in, h.data(), n * 16, cudaMemcpyHostToDevice);
+    // companions w * 2^64 mod M of the fixed operands (fe_mul_tw), computed on the host
+    std::vector<fe> hc(n), ebc;
+    for (int i = 0; i < n; i++) hc[i] = portable::fe_tw_companion(h[i]);
+    for (const fe &b : eb) ebc.push_back(portable::fe_tw_companion(b));
+    fe *d_in, *d_inc, *d_out, *da, *db, *dbc, *d0, *d1;
+    cudaMalloc(&d_in, n * 16); cudaMalloc(&d_inc, n * 16); cudaMalloc(&d_out, n * 16);
+    cudaMemcpy(d_in, h.data(), n * 16, cudaMemcpyHostToDevice); cudaMemcpy(d_inc, hc.data(), n * 16, cudaMemcpyHostToDevice);
     int m = ea.size();
-    cudaMalloc(&da, m * 16); cudaMalloc(&db, m * 16); cudaMalloc(&d0, m * 16); cudaMalloc(&d1, m * 16);
+    cudaMalloc(&da, m * 16); cudaMalloc(&db, m * 16); cudaMalloc(&dbc, m * 16); cudaMalloc(&d0, m * 16); cudaMalloc(&d1, m * 16);
     cudaMemcpy(da, ea.data(), m * 16, cudaMemcpyHostToDevice); cudaMemcpy(db, eb.data(), m * 16, cudaMemcpyHostToDevice);
+    cudaMemcpy(dbc, ebc.data(), m * 16, cudaMemcpyHostToDevice);
     std::vector<fe> r0(m), r1(m);
-    check<0><<<(m + 255) / 256, 256>>>(da, db, d0, m); cudaMemcpy(r0.data(), d0, m * 16, cudaMemcpyDeviceToHost);
+    check<0><<<(m + 255) / 256, 256>>>(da, db, dbc, d0, m); cudaMemcpy(r0.data(), d0, m * 16, cudaMemcpyDeviceToHost);
     auto cmp = [&](const char *nm) { cudaMemcpy(r1.data(), d1, m * 16, cudaMemcpyDeviceToHost); int bad = 0; for (int i = 0; i < m; i++) if (r0[i].lo != r1[i].lo || r0[i].hi != r1[i].hi) { if (bad < 3) printf("  %s mismatch at %d\n", nm, i); bad++; } printf("%s vs portable: %d mismatches of %d\n", nm, bad, m); };
-    check<1><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("ptx");
+    check<1><<<(m + 255) / 256, 256>>>(da, db, dbc, d1, m); cmp("ptx");
 #ifdef DG_HAVE_V3
-    check<2><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v3");
+    check<2><<<(m + 255) / 256, 256>>>(da, db, dbc, d1, m); cmp("v3");
 #endif
-    check<3><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v4");
-    check<4><<<(m + 255) / 256, 256>>>(da, db, d1, m); cmp("v4 inline");
-    run<0>("portable", d_in, d_out, blocks, iters);
-    run<1>("ptx", d_in, d_out, blocks, iters);
+    check<3><<<(m + 255) / 256, 256>>>(da, db, dbc, d1, m); cmp("v4");
+    check<4><<<(m + 255) / 256, 256>>>(da, db, dbc, d1, m); cmp("v4 inline");
+    check<5><<<(m + 255) / 256, 256>>>(da, db, dbc, d1, m); cmp("tw");
+    run<0>("portable", d_in, d_inc, d_out, blocks, iters);
+    run<1>("ptx", d_in, d_inc, d_out, blocks, iters);
 #ifdef DG_HAVE_V3
-    run<2>("v3", d_in, d_out, blocks, iters);
+    run<2>("v3", d_in, d_inc, d_out, blocks, iters);
 #endif
-    run<3>("v4", d_in, d_out, blocks, iters);
-    run<4>("v4 inline", d_in, d_out, blocks, iters);
+    run<3>("v4", d_in, d_inc, d_out, blocks, iters);
+    run<4>("v4 inline", d_in, d_inc, d_out, blocks, iters);
+    run<5>("tw", d_in, d_inc, d_out, blocks, iters);
     run_call<0>("bfly inline", d_in, d_out, blocks, iters / 2);
     run_call<1>("bfly 1 mul per call", d_in, d_out, blocks, iters / 2);
     run_call<2>("bfly 2 muls per call", d_in, d_out, blocks, iters / 2);
