@@ -13,9 +13,11 @@ Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.trace_batch(program, inputs)     <->  processor::execute for many ProgramInputs on the GPU (trace_shapes: shapes only)
     distaff_b200.execute_programs(jobs)           <->  execute_batch for jobs of many programs in one call (trace_programs: the traces)
     distaff_b200.execute_one(program, inputs)     <->  distaff::execute of one long execution, split across GPU threads (trace_one)
+    distaff_b200.execute_many(jobs)               <->  execute_programs with every execution split as execute_one splits one (trace_many)
 The compute path is hand-written CUDA behind the C-ABI of include/distaff_gpu.h; there is no CPU fallback.
 """
 from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, prove_traces, prove_traces_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
                   merkle_build, hash_rows, hash64, find_pow_nonce, field_op, field_dot, eval_transitions, TraceReport, check_trace, check_traces,
                   check_traces_device, constraint_name, set_memory_limit, memory_usage, plan_prove, ProgramInputs, trace_batch, trace_shapes,
-                  execute_batch, trace_programs, execute_programs, group_traces, trace_one, execute_one)
+                  execute_batch, trace_programs, execute_programs, group_traces, trace_one, execute_one,
+                  trace_many, execute_many)

@@ -728,6 +728,82 @@ def execute_programs(jobs, options=None, max_steps=MAX_STEPS, stats=None):
             for i, e in enumerate(errors)]
 
 
+# ---- many long executions, each split across GPU threads, in one call ------------------------------------------------------------------
+def _many_stats(stats, st):
+    if stats is not None:
+        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgManyStats._fields_ if f != "fallback"})
+        fb = {}
+        _vm_stats(fb, st.fallback)
+        stats["fallback"] = fb
+
+
+def _segment_steps(segment_steps):
+    s = int(segment_steps)
+    if s != 0 and (s < 16 or s & (s - 1)):
+        raise ValueError("segment_steps must be 0 or a power of two of at least 16")
+    return s
+
+
+def trace_many(jobs, max_steps=MAX_STEPS, segment_steps=0, stats=None):
+    """trace_programs with every execution run as trace_one runs one (dg_trace_many): the programs' sponge tables, one sequential pass
+    for every execution and the rows written by one thread per checkpoint.  jobs as in trace_programs (pack_jobs).  Returns a list in job
+    order: a hostvm.ExecutionTrace (what trace_programs returns, byte for byte) or the DgError of an execution that failed.
+    segment_steps: 0 (the library chooses) or a power of two >= 16.  The buffers are sized by a call without registers first, so the
+    tables and the sequential pass run twice.  A dict passed as `stats` receives the full call's figures, the batch path's for the
+    fallback executions under "fallback"."""
+    jobs = list(jobs)
+    s = _segment_steps(segment_steps)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    k, L = len(jobs), backend.lib()
+    info = (backend.DgExecutionInfo * k)()
+    status = (ctypes.c_int * k)()
+    st = backend.DgManyStats()
+    backend.check(L.dg_trace_many(cprogs, len(programs), k, program_of, arr, int(max_steps), s, info, None, status, ctypes.byref(st)))
+    regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
+    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
+    backend.check(L.dg_trace_many(cprogs, len(programs), k, program_of, arr, int(max_steps), s, info, outs, status, ctypes.byref(st)))
+    errors = _messages(list(status))
+    _many_stats(stats, st)
+    result = []
+    for i, (job, e) in enumerate(zip(jobs, errors)):
+        if e is not None:
+            result.append(e)
+            continue
+        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
+        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
+                                            list(job[1].public), last[:num_outputs[i]]))
+    del keep
+    return result
+
+
+def execute_many(jobs, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
+    """execute_programs with every execution run as execute_one runs one (dg_execute_many): every trace is proven where it was written.
+    Returns a list in job order: (outputs, StarkProof) -- what execute_programs returns, byte for byte -- or the DgError of an execution
+    that failed.  segment_steps and `stats` as in trace_many."""
+    options = options or ProofOptions()
+    jobs = list(jobs)
+    s = _segment_steps(segment_steps)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    k = len(jobs)
+    opt = options._c()
+    handles = (backend.vp * k)()
+    outputs = np.zeros((k, 8, 2), dtype=np.uint64)
+    status = (ctypes.c_int * k)()
+    pst, st = backend.DgStats(), backend.DgManyStats()
+    backend.check(backend.lib().dg_execute_many(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), int(max_steps), s,
+                                               ctypes.byref(opt), handles, outputs.ctypes.data, status, ctypes.byref(pst), ctypes.byref(st)))
+    errors = _messages(list(status))
+    _many_stats(stats, st)
+    del keep
+    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs[i]]) if num_outputs[i] else [], _collect(handles[i], pst))
+            for i, e in enumerate(errors)]
+
+
 # ---- building blocks ------------------------------------------------------------------------------------------------------
 def ntt(values, inverse=False):
     """polynom::eval_fft / interpolate_fft on (batch, n, 2) or (n, 2) uint64 arrays; returns a new array"""

@@ -84,6 +84,13 @@ class DgTraceOneStats(ctypes.Structure):
                 ("logged", u64), ("segment_steps", u64), ("fallback", ctypes.c_int32)]
 
 
+class DgManyStats(ctypes.Structure):
+    _fields_ = [("table_ms", ctypes.c_float), ("sequential_ms", ctypes.c_float), ("segment_ms", ctypes.c_float), ("table_rounds", u64),
+                ("table_entries", u64), ("table_levels", u32), ("tabled_programs", u32), ("fallback_programs", u32),
+                ("sequential_launches", u32), ("checkpoints", u64), ("segments", u64), ("logged", u64), ("segment_steps", u64),
+                ("waves", u32), ("prove_groups", u32), ("fallback", DgExecutionStats)]
+
+
 DRAW_FIELD_FN =ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, vp)
 DRAW_POSITIONS_FN = ctypes.CFUNCTYPE(ctypes.c_int, vp, vp, u64, u32, u32, vp)
 
@@ -122,6 +129,11 @@ EXPORTS = {
                      ctypes.POINTER(DgTraceOneStats)],
     "dg_execute_one": [ctypes.POINTER(DgProgram), ctypes.POINTER(DgProgramInputs), u32, u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp,
                        ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(DgStats), ctypes.POINTER(DgTraceOneStats)],
+    "dg_trace_many": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), u64, u64,
+                      ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgManyStats)],
+    "dg_execute_many": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32), u64, u64,
+                        ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
+                        ctypes.POINTER(DgManyStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),

@@ -669,6 +669,38 @@ int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *input
         *proof_out = (dg_proof_t *)execute_one(c, x, num_outputs, segment_steps, *options, outputs16, info, prove_stats, stats);
     });
 }
+int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                  const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps, dg_execution_info_t *info,
+                  uint8_t *const *registers_out, int *status, dg_many_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(programs && program_of && inputs && status, "null argument");
+        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
+        check_segment_steps(segment_steps);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        trace_many(c, x, segment_steps, info, registers_out, status, t_batch_messages, stats);
+    });
+}
+int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                    const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                    const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
+                    dg_many_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "at least one execution is needed");
+        DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
+        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+        check_execution_call(x);
+        check_output_counts(count, num_outputs, outputs16);
+        check_segment_steps(segment_steps);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        t_batch_messages.clear();
+        execute_many(c, x, num_outputs, segment_steps, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, prove_stats, stats);
+    });
+}
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
     return guarded([&] {
         DG_REQUIRE(message && cap, "null argument");

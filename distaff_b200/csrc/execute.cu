@@ -2,12 +2,14 @@
 // and dg_execute_batch are the one-program case): validate each program's encoding, put every program into one set of tables and upload
 // them and the inputs once, run the shape pass for every execution, and write the successful executions in waves -- one write launch
 // (vm.cu) per wave for every shape in it -- into one slab per shape, which is copied to the caller's buffers (dg_trace_programs) or
-// proven in place (dg_execute_programs, through prove_traces).  dg_trace_one / dg_execute_one run one execution from the sponge table:
-// the table level by level, the sequential pass, the segment pass (vm.cu), with the batch path as the fallback for inconsistent hashes.
+// proven in place (dg_execute_programs, through prove_traces).  dg_trace_many / dg_execute_many (and dg_trace_one / dg_execute_one, their
+// one-execution case) run the executions from the sponge tables: every program's table level by level, one sequential pass for every
+// execution, and the segment pass (vm.cu) in the same waves, with the batch path for the programs whose hashes are inconsistent.
 #include "vm.h"
 #include "air.h"
 #include "prover.h"
 #include <algorithm>
+#include <deque>
 #include <functional>
 #include <map>
 #include <set>
@@ -248,11 +250,11 @@ struct Executions {
         DG_CUDA(cudaStreamSynchronize(c.stream));
     }
 
-    // the shape pass; an execution whose hints outgrow its tape scratch (256 elements beyond its inputs at first; what the assembler's
-    // macros need) runs again with 16 times more
-    void shapes() {
+    // the shape pass of the executions `ids` (those the inputs did not fail); an execution whose hints outgrow its tape scratch (256
+    // elements beyond its inputs at first; what the assembler's macros need) runs again with 16 times more
+    void shapes(const std::vector<unsigned> &ids) {
         std::vector<unsigned> pending;
-        for (uint32_t i = 0; i < x.count; i++) if (status[i] == DG_OK) pending.push_back(i);
+        for (unsigned i : ids) if (status[i] == DG_OK) pending.push_back(i);
         for (unsigned long long extra = 256; !pending.empty(); extra *= 16) {
             for (unsigned e : pending) { cap[2 * e] = x.inputs[e].n_secret_a + extra; cap[2 * e + 1] = x.inputs[e].n_secret_b + extra; }
             place_tapes(pending);
@@ -264,11 +266,11 @@ struct Executions {
             for (unsigned e : pending) if (res[e].code == VM_TAPE_SCRATCH) again.push_back(e);
             pending.swap(again);
         }
-        for (uint32_t i = 0; i < x.count; i++)
+        for (unsigned i : ids)
             if (status[i] == DG_OK && res[i].code != VM_OK) fail(i, DG_ERR_EXECUTION, vm_message(res[i].code, res[i].fail_step, x.max_steps));
         // the write pass runs with the tape scratch each execution needed
         std::vector<unsigned> ok;
-        for (uint32_t i = 0; i < x.count; i++)
+        for (unsigned i : ids)
             if (status[i] == DG_OK) { ok.push_back(i); cap[2 * i] = res[i].peak_a; cap[2 * i + 1] = res[i].peak_b; }
         place_tapes(ok);
     }
@@ -285,21 +287,21 @@ struct Executions {
         return v;
     }
     static ShapeKey key(const dg_execution_info_t &v) { return std::make_tuple(v.width, v.length, v.ctx_depth, v.loop_depth); }
-    // the successful executions by shape, shapes in order and input order inside a shape
-    std::vector<unsigned> shape_order() const {
+    // the successful executions of `ids` by shape, shapes in order and input order inside a shape
+    std::vector<unsigned> shape_order(const std::vector<unsigned> &ids) const {
         std::map<ShapeKey, std::vector<unsigned>> g;
-        for (uint32_t i = 0; i < x.count; i++) if (status[i] == DG_OK) g[key(info(i))].push_back(i);
+        for (unsigned i : ids) if (status[i] == DG_OK) g[key(info(i))].push_back(i);
         std::vector<unsigned> order;
         for (auto &kv : g) order.insert(order.end(), kv.second.begin(), kv.second.end());
         return order;
     }
 
-    // The write pass of every successful execution, in waves.  A wave is a run of the executions in shape order, written by one launch
-    // into one slab per shape and handed to done(slabs) while its traces are on the device; waves follow each other, so the executions
-    // reach done in shape order, input order inside a shape.  A wave's traces take at most half of the device memory the library may
-    // use, and with `opt` they leave room beside them for one proof of the wave's largest shape.  $DG_BATCH_GROUP caps its executions.
-    template <typename F> void write_waves(const dg_options_t *opt, uint8_t *const *registers_out, F &&done) {
-        const std::vector<unsigned> order = shape_order();
+    // The executions `order` (in shape order) in waves: a wave is a run of them, given one slab per shape in a fresh register buffer and
+    // handed to write(wave, slabs, last) while its traces are on the device; waves follow each other, so the executions reach write in
+    // shape order, input order inside a shape.  A wave's traces take at most half of the device memory the library may use, and with
+    // `opt` they leave room beside them for one proof of the wave's largest shape.  $DG_BATCH_GROUP caps its executions.  L.out / L.outs
+    // and d_pad_ids (the wave, in slab order) are set for the wave.
+    template <typename F> void cut_waves(const std::vector<unsigned> &order, const dg_options_t *opt, uint8_t *const *registers_out, F &&write) {
         const size_t most = (size_t)batch_group_cap(65535);         // one padding launch holds 65535 executions
         std::map<ShapeKey, size_t> room;                           // bytes one proof of a shape needs beside the traces
         std::vector<VmOut> outs(x.count);
@@ -340,17 +342,30 @@ struct Executions {
                 at += (size_t)s.width * s.length;
             }
             upload(d_outs, outs);
-            upload(d_pad_ids, wave);                               // the wave is in slab order
+            upload(d_pad_ids, wave);
             L.out = regs.as<fe>();
             L.outs = d_outs.as<VmOut>();
+            write(wave, slabs, end == order.size());
+            first = end;
+        }
+    }
+    // the padding rows of a wave's slabs (after its rows are written)
+    void pad(const std::vector<Slab> &slabs) {
+        size_t q = 0;
+        for (const Slab &s : slabs) {
+            vm_pad_rows(c, s.regs, L.res, d_pad_ids.as<unsigned>() + q, (unsigned)s.ids.size(), s.shape.width, s.shape.length);
+            q += s.ids.size();
+        }
+    }
+
+    // The write pass of the successful executions of `ids`, in waves (cut_waves): one launch per wave for every shape in it, then
+    // done(slabs).
+    template <typename F> void write_waves(const std::vector<unsigned> &ids, const dg_options_t *opt, uint8_t *const *registers_out, F &&done) {
+        cut_waves(shape_order(ids), opt, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool) {
             stats.lanes += launch_ids(wave);
             stats.write_ms += timed([&] {
                 vm_write_pass(c, L);
-                size_t q = 0;
-                for (const Slab &s : slabs) {
-                    vm_pad_rows(c, s.regs, L.res, d_pad_ids.as<unsigned>() + q, (unsigned)s.ids.size(), s.shape.width, s.shape.length);
-                    q += s.ids.size();
-                }
+                pad(slabs);
             });
             stats.write_launches++;
             stats.waves++;
@@ -358,13 +373,95 @@ struct Executions {
             for (unsigned e : wave)
                 if (res[e].code != VM_OK) fail(e, DG_ERR_EXECUTION, vm_message(res[e].code, res[e].fail_step, x.max_steps));
             done(slabs);
-            first = end;
-        }
+        });
     }
 };
 
 void check_one_gpu(Context &c) {
     DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched execution runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
+}
+
+// the registers of a wave's successful executions to the caller's buffers
+void copy_slabs(Context &c, const Executions &X, const std::vector<Slab> &slabs, uint8_t *const *registers_out) {
+    for (const Slab &s : slabs) {
+        const size_t per = (size_t)s.shape.width * s.shape.length * 16;
+        for (size_t q = 0; q < s.ids.size(); q++)
+            if (X.status[s.ids[q]] == DG_OK) {
+                DG_REQUIRE(registers_out[s.ids[q]], "null register buffer of execution " + std::to_string(s.ids[q]));
+                DG_CUDA(cudaMemcpyAsync(registers_out[s.ids[q]], (const uint8_t *)s.regs + q * per, per, cudaMemcpyDeviceToHost, c.stream));
+            }
+    }
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+}
+
+// Each shape's successful traces of a wave proven together where they were written (prove_traces), RNG callbacks shape by shape and
+// in input order inside a shape.  Executions the rows failed are left out: the traces after them move down over them, and their outputs
+// (8 per execution in outs) are zeroed, as those of executions the VM failed earlier.  Adds the prove groups to `groups`.
+void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, const uint32_t *num_outputs, const dg_options_t &opt,
+                 std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats, uint32_t &groups) {
+    const ExecutionCall &x = X.x;
+    for (const Slab &s : slabs) {
+        const size_t per = (size_t)s.shape.width * s.shape.length;
+        std::vector<unsigned> ok;
+        for (size_t q = 0; q < s.ids.size(); q++) {
+            if (X.status[s.ids[q]] != DG_OK) {
+                std::fill(outs.begin() + (size_t)s.ids[q] * 8, outs.begin() + (size_t)s.ids[q] * 8 + 8, fe_make(0, 0));
+                continue;
+            }
+            if (ok.size() != q)
+                DG_CUDA(cudaMemcpyAsync(s.regs + ok.size() * per, s.regs + q * per, per * 16, cudaMemcpyDeviceToDevice, c.stream));
+            ok.push_back(s.ids[q]);
+        }
+        if (ok.empty()) continue;
+        const uint32_t k = (uint32_t)ok.size();
+        std::vector<const uint8_t *> in16(k), out16(k);
+        std::vector<uint32_t> n_in(k), n_out(k);
+        for (uint32_t q = 0; q < k; q++) {
+            in16[q] = x.inputs[ok[q]].public16; n_in[q] = x.inputs[ok[q]].n_public;
+            out16[q] = (const uint8_t *)&outs[(size_t)ok[q] * 8]; n_out[q] = num_outputs[ok[q]];
+        }
+        std::vector<Proof *> proofs(k, nullptr);
+        std::vector<int> st(k, DG_OK);
+        std::vector<std::string> msg;
+        dg_prove_stats_t gs;
+        memset(&gs, 0, sizeof gs);
+        uint32_t g = 0;
+        prove_traces(c, s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth, in16.data(), n_in.data(),
+                     out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &g);
+        for (uint32_t q = 0; q < k; q++) {
+            proofs_out[ok[q]] = proofs[q];
+            if (st[q] != DG_OK) X.fail(ok[q], st[q], msg[q]);
+        }
+        groups += g;
+        if (stats) {
+            for (int i = 0; i < 9; i++) stats->stage_ms[i] += gs.stage_ms[i];
+            stats->h2d_ms += gs.h2d_ms; stats->total_ms += gs.total_ms; stats->kernel_launches += gs.kernel_launches;
+        }
+    }
+}
+
+// The batch path for the executions `ids`: the shape pass, then (with `write`) the write pass in waves, the registers copied to
+// registers_out when it is given.  Without `write` the failures that need the sponge (program hash, loop image) go unreported.  With
+// `precheck` every buffer of an execution the shape pass let through must be there before the write pass; without, only those of the
+// executions the write pass lets through (a caller that learned of a write-pass failure from an earlier call may pass NULL for it).
+void batch_trace(Context &c, Executions &X, const std::vector<unsigned> &ids, uint8_t *const *registers_out, bool write, bool precheck) {
+    X.shapes(ids);
+    if (write)
+        X.write_waves(ids, nullptr, precheck ? registers_out : nullptr, [&](const std::vector<Slab> &slabs) {
+            if (registers_out) copy_slabs(c, X, slabs, registers_out);
+        });
+}
+
+// The batch path for the executions `ids`, proven: the shape pass, outputs from the final stacks, the write pass in waves and each wave
+// proven in place
+void batch_execute(Context &c, Executions &X, const std::vector<unsigned> &ids, const uint32_t *num_outputs, const dg_options_t &opt,
+                   std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats) {
+    X.shapes(ids);
+    for (unsigned i : ids)
+        if (X.status[i] == DG_OK) for (uint32_t j = 0; j < num_outputs[i]; j++) outs[(size_t)i * 8 + j] = X.res[i].top[j];
+    X.write_waves(ids, &opt, nullptr, [&](const std::vector<Slab> &slabs) {
+        prove_slabs(c, X, slabs, num_outputs, opt, outs, proofs_out, stats, X.stats.prove_groups);
+    });
 }
 
 void finish(const Executions &X, int *status, std::vector<std::string> &messages, dg_execution_stats_t *vm_stats) {
@@ -373,7 +470,13 @@ void finish(const Executions &X, int *status, std::vector<std::string> &messages
     if (vm_stats) *vm_stats = X.stats;
 }
 
-// ---- one execution from the sponge table ------------------------------------------------------------------------------------------------
+// the proofs of the waves done so far are freed when a later wave fails the call
+struct ReleaseOnError {
+    Proof **out; uint32_t count; bool done = false;
+    ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
+};
+
+// ---- executions from the sponge tables --------------------------------------------------------------------------------------------------
 // The chains of a program (vm.h): every block list reachable from the root once (lists may be shared: a list is its child range) and, per
 // loop, the chain after BREAK.  A chain's level is one above every chain it reads -- a list reads its group, switch and loop children's
 // closing states, the break chains of its loops and its loops' skips; a break chain reads the body's last state -- so one launch per
@@ -455,186 +558,241 @@ ChainPlan plan_chains(const dg_program_t &p) {
     return P;
 }
 
-// S when the caller leaves it to the library: at most 4096 segments for an execution of max_steps steps
+// S when the caller leaves it to the library: at most 4096 segments for an execution of max_steps steps (DESIGN.md section 7i measures it
+// against the executions a call holds)
 uint64_t default_segment_steps(uint64_t max_steps) {
     uint64_t s = 16;
     while (s < (1ULL << 40) && s * 4096 < max_steps) s *= 2;
     return s;
 }
 
-// One execution from the sponge table.  table() returns whether the encoding's hashes are consistent; sequential() runs the execution
-// (again with more room when the tape scratch, the read log or the checkpoint buffer were too small) and throws its failure; segments()
-// writes the rows into regs ([width][length]) and pads them.
-struct OneExecution {
+// The executions of a call from the sponge tables.  tables() computes every program's chains in one table (one launch per level for all
+// programs) and sorts the executions the inputs did not fail into `run` (their program's hashes are consistent) and `fallback` (they are
+// not: the batch path runs them, in X, so results are identical either way).  sequential() runs every execution of `run` in one launch,
+// one warp each (again, for the executions that outgrew their tape scratch, read log or checkpoint buffer, with the room they reported),
+// and waves() writes the rows of its successful executions in waves, one segment launch per wave for all their checkpoints.
+struct TabledExecutions {
     Context &c;
     Executions X;
     uint64_t S;
-    dg_trace_one_stats_t st;
-    DevBuf d_refs, d_items, d_tab, d_bad, d_log, d_cp, d_seq, d_codes;
-    VmTabled T;
-    VmSequential seq{0, 0};
+    dg_many_stats_t st;
+    std::vector<char> tabled;                     // per program
+    std::vector<unsigned> run, fallback;          // in input order
+    std::vector<VmTabled> T;                      // per execution
+    std::vector<VmSequential> seq;                // per execution
+    std::deque<DevBuf> logs;                      // the read logs and checkpoints of each sequential launch
+    DevBuf d_refs, d_tab, d_T, d_seq, d_codes, d_execs, d_first;
+    VmTables G;
 
-    OneExecution(Context &ctx_, const ExecutionCall &x, uint64_t segment_steps)
-        : c(ctx_), X(ctx_, x), S(segment_steps ? segment_steps : default_segment_steps(x.max_steps)) {
+    TabledExecutions(Context &ctx_, const ExecutionCall &x, uint64_t segment_steps)
+        : c(ctx_), X(ctx_, x), S(segment_steps ? segment_steps : default_segment_steps(x.max_steps)), tabled(x.n_programs, 0), T(x.count),
+          seq(x.count) {
         memset(&st, 0, sizeof st);
-        memset(&T, 0, sizeof T);
+        memset(T.data(), 0, T.size() * sizeof(VmTabled));
+        memset(seq.data(), 0, seq.size() * sizeof(VmSequential));
         st.segment_steps = S;
+        G = VmTables{nullptr, nullptr, S};
         X.setup();
     }
 
-    bool table() {
-        if (X.status[0] != DG_OK) throw Error(X.status[0], X.messages[0]);        // inputs that fail before the execution runs
-        const ChainPlan P = plan_chains(X.x.programs[0]);
-        X.upload(d_refs, P.refs);
-        X.upload(d_items, P.items);
-        d_tab.alloc(P.entries * sizeof(VmSponge));
-        const std::vector<unsigned> zero(1, 0);
-        X.upload(d_bad, zero);
+    // the chains of every program with an execution to run, rebased as X.setup() rebased the programs: child ranges by the child entries
+    // before the program, block indices by the blocks before it, table indices by the entries before it
+    void tables() {
+        const ExecutionCall &x = X.x;
+        std::vector<char> used(x.n_programs, 0);
+        for (uint32_t i = 0; i < x.count; i++) if (X.status[i] == DG_OK) used[x.program_of[i]] = 1;
+        std::vector<VmChainRef> refs;
+        std::vector<std::vector<VmChainItem>> levels;
+        std::vector<unsigned long long> root(x.n_programs, 0);
+        unsigned long long entries = 0;
+        unsigned b0 = 0, c0 = 0;
+        for (uint32_t p = 0; p < x.n_programs; p++) {
+            const dg_program_t &g = x.programs[p];
+            refs.resize(b0 + g.n_blocks, VmChainRef{0, 0, 0, 0, 0, 0});
+            if (used[p]) {
+                const ChainPlan P = plan_chains(g);
+                for (uint32_t bi = 0; bi < g.n_blocks; bi++) {
+                    const VmChainRef &r = P.refs[bi];
+                    refs[b0 + bi] = VmChainRef{r.main + entries, r.alt + entries, r.brk + entries, r.main_close + entries,
+                                               r.alt_close + entries, r.brk_close + entries};
+                }
+                if (levels.size() + 1 < P.level_start.size()) levels.resize(P.level_start.size() - 1);
+                for (size_t l = 0; l + 1 < P.level_start.size(); l++)
+                    for (size_t k = P.level_start[l]; k < P.level_start[l + 1]; k++) {
+                        VmChainItem it = P.items[k];
+                        if (it.kind == VM_CHAIN_LIST) it.first += c0; else it.block += b0;
+                        it.program = p;
+                        it.out += entries;
+                        levels[l].push_back(it);
+                    }
+                root[p] = P.root + entries;
+                entries += P.entries;
+                st.table_rounds += P.rounds;
+            }
+            b0 += g.n_blocks;
+            c0 += g.n_children;
+        }
+        std::vector<VmChainItem> items;
+        std::vector<size_t> level_start{0};
+        for (const auto &l : levels) { items.insert(items.end(), l.begin(), l.end()); level_start.push_back(items.size()); }
+        DevBuf d_items, d_bad;
+        X.upload(d_refs, refs);
+        X.upload(d_items, items);
+        d_tab.alloc(std::max<unsigned long long>(entries, 1) * sizeof(VmSponge));
+        std::vector<unsigned> bad(x.n_programs, 0);
+        X.upload(d_bad, bad);
         st.table_ms = X.timed([&] {
-            for (size_t l = 0; l + 1 < P.level_start.size(); l++)
-                vm_table_level(c, X.L, d_items.as<VmChainItem>() + P.level_start[l], (unsigned)(P.level_start[l + 1] - P.level_start[l]),
+            for (size_t l = 0; l + 1 < level_start.size(); l++)
+                vm_table_level(c, X.L, d_items.as<VmChainItem>() + level_start[l], (unsigned)(level_start[l + 1] - level_start[l]),
                                d_refs.as<VmChainRef>(), d_tab.as<VmSponge>(), d_bad.as<unsigned>());
         });
-        st.table_levels = (uint32_t)P.level_start.size() - 1;
-        st.table_rounds = P.rounds;
-        st.table_entries = P.entries;
-        unsigned bad = 0;
-        DG_CUDA(cudaMemcpy(&bad, d_bad.p, sizeof bad, cudaMemcpyDeviceToHost));
-        T.tab = d_tab.as<VmSponge>();
-        T.chains = d_refs.as<VmChainRef>();
-        T.root = P.root;
-        T.segment_steps = S;
-        return bad == 0;
+        st.table_levels = (uint32_t)levels.size();
+        st.table_entries = entries;
+        DG_CUDA(cudaMemcpy(bad.data(), d_bad.p, bad.size() * sizeof(unsigned), cudaMemcpyDeviceToHost));
+        for (uint32_t p = 0; p < x.n_programs; p++) {
+            tabled[p] = used[p] && !bad[p];
+            st.tabled_programs += tabled[p];
+            st.fallback_programs += used[p] && bad[p];
+        }
+        G.tab = d_tab.as<VmSponge>();
+        G.chains = d_refs.as<VmChainRef>();
+        for (uint32_t i = 0; i < x.count; i++) {
+            if (X.status[i] != DG_OK) continue;
+            (tabled[x.program_of[i]] ? run : fallback).push_back(i);
+            T[i].root = root[x.program_of[i]];
+        }
     }
 
     void sequential() {
+        if (run.empty()) return;
         const ExecutionCall &x = X.x;
-        const uint64_t max_steps = x.max_steps;
-        unsigned long long extra = 256, log_cap = std::min<uint64_t>(2 * max_steps, 1ULL << 21);
-        unsigned long long cp_cap = std::min<uint64_t>(max_steps / S + 2, 4096);
-        d_seq.alloc(sizeof(VmSequential));
-        for (;;) {
-            X.cap[0] = x.inputs[0].n_secret_a + extra;
-            X.cap[1] = x.inputs[0].n_secret_b + extra;
-            X.place_tapes({0});
-            X.launch_ids({0});
-            d_log.alloc(std::max<unsigned long long>(log_cap, 1) * sizeof(fe));
-            d_cp.alloc(cp_cap * vm_checkpoint_bytes());
-            T.log = d_log.as<fe>(); T.log_cap = log_cap;
-            T.checkpoints = d_cp.p; T.cp_cap = cp_cap;
-            st.sequential_ms += X.timed([&] { vm_sequential_pass(c, X.L, T, d_seq.as<VmSequential>()); });
+        const size_t cpb = vm_checkpoint_bytes();
+        // the first logs and checkpoint buffers take at most a quarter of the memory the library may use, shared equally
+        const size_t share = memory_budget(c, Budget::FREE, 0) / 4 / run.size();
+        const unsigned long long cp0 = std::max<unsigned long long>(2, std::min<unsigned long long>(std::min<uint64_t>(x.max_steps / S + 2, 4096), share / 2 / cpb));
+        const unsigned long long log0 = std::max<unsigned long long>(1, std::min<unsigned long long>(std::min<uint64_t>(2 * x.max_steps, 1ULL << 21), share / 2 / 16));
+        std::vector<unsigned long long> extra(x.count, 256), log_cap(x.count, log0), cp_cap(x.count, cp0);
+        X.upload(d_seq, seq);
+        std::vector<unsigned> pending = run;
+        while (!pending.empty()) {
+            for (unsigned e : pending) { X.cap[2 * e] = x.inputs[e].n_secret_a + extra[e]; X.cap[2 * e + 1] = x.inputs[e].n_secret_b + extra[e]; }
+            X.place_tapes(pending);
+            // one warp per execution: the executions of a warp would take different paths through the interpreter (DESIGN.md section 7i)
+            std::vector<unsigned> lanes;
+            for (unsigned e : pending) { lanes.push_back(e); lanes.resize(lanes.size() + 31, VM_NO_EXECUTION); }
+            X.upload(X.d_ids, lanes);
+            X.L.ids = X.d_ids.as<unsigned>();
+            X.L.count = (unsigned)lanes.size();
+            size_t log_n = 0, cp_n = 0;
+            for (unsigned e : pending) { log_n += log_cap[e]; cp_n += cp_cap[e]; }
+            logs.emplace_back(std::max<size_t>(log_n, 1) * sizeof(fe));
+            fe *log = logs.back().as<fe>();
+            logs.emplace_back(cp_n * cpb);
+            uint8_t *cp = (uint8_t *)logs.back().p;
+            for (unsigned e : pending) {
+                T[e].log = log; T[e].log_cap = log_cap[e]; log += log_cap[e];
+                T[e].checkpoints = cp; T[e].cp_cap = cp_cap[e]; cp += cp_cap[e] * cpb;
+            }
+            X.upload(d_T, T);
+            st.sequential_ms += X.timed([&] { vm_sequential_pass(c, X.L, G, d_T.as<VmTabled>(), d_seq.as<VmSequential>()); });
             st.sequential_launches++;
             X.download_results();
-            DG_CUDA(cudaMemcpy(&seq, d_seq.p, sizeof seq, cudaMemcpyDeviceToHost));
-            const VmResult &r = X.res[0];
-            if (r.code == VM_TAPE_SCRATCH) { extra *= 16; continue; }
-            if (r.code != VM_OK) throw Error(DG_ERR_EXECUTION, vm_message(r.code, r.fail_step, max_steps));
-            if (seq.checkpoints + 1 <= cp_cap && seq.logged <= log_cap) break;
-            cp_cap = std::max(cp_cap, seq.checkpoints + 1);                   // the sizes this execution needs
-            log_cap = std::max(log_cap, seq.logged);
+            DG_CUDA(cudaMemcpy(seq.data(), d_seq.p, seq.size() * sizeof(VmSequential), cudaMemcpyDeviceToHost));
+            std::vector<unsigned> again;
+            for (unsigned e : pending) {
+                const VmResult &r = X.res[e];
+                if (r.code == VM_TAPE_SCRATCH) { extra[e] *= 16; again.push_back(e); continue; }
+                if (r.code != VM_OK) { X.fail(e, DG_ERR_EXECUTION, vm_message(r.code, r.fail_step, x.max_steps)); continue; }
+                if (seq[e].checkpoints + 1 <= cp_cap[e] && seq[e].logged <= log_cap[e]) continue;
+                cp_cap[e] = std::max(cp_cap[e], seq[e].checkpoints + 1);                   // the sizes this execution needs
+                log_cap[e] = std::max(log_cap[e], seq[e].logged);
+                again.push_back(e);
+            }
+            pending.swap(again);
         }
-        st.checkpoints = seq.checkpoints + 1;
-        st.segments = seq.checkpoints;
-        st.logged = seq.logged;
+        X.d_tapes.release();                      // the segments read the logs
+        for (unsigned e : run)
+            if (X.status[e] == DG_OK) { st.checkpoints += seq[e].checkpoints + 1; st.segments += seq[e].checkpoints; st.logged += seq[e].logged; }
     }
 
-    dg_execution_info_t shape() const { return X.info(0); }
-
-    void segments(fe *regs) {
-        const dg_execution_info_t s = shape();
-        X.upload(X.d_outs, std::vector<VmOut>{VmOut{0, s.length, s.width, s.ctx_depth, s.loop_depth, s.stack_depth}});
-        X.L.out = regs;
-        X.L.outs = X.d_outs.as<VmOut>();
-        d_codes.alloc(2 * seq.checkpoints * sizeof(unsigned long long));
-        st.segment_ms = X.timed([&] {
-            vm_segment_pass(c, X.L, T, seq.checkpoints, d_codes.as<unsigned long long>());
-            vm_pad_rows(c, regs, X.L.res, X.L.ids, 1, s.width, s.length);
+    // The rows of the successful executions of `run`, in waves as the batch path cuts them: per wave one segment launch for every
+    // checkpoint of its executions and one padding launch per shape, then done(slabs).  A segment that fails is an internal error of its
+    // execution.  The tables, logs and checkpoints are freed before the last wave's done.
+    template <typename F> void waves(const dg_options_t *opt, uint8_t *const *registers_out, F &&done) {
+        X.cut_waves(X.shape_order(run), opt, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool last) {
+            std::vector<unsigned long long> first{0};
+            for (unsigned e : wave) first.push_back(first.back() + seq[e].checkpoints);
+            const unsigned long long segments = first.back();
+            X.upload(d_execs, wave);
+            X.upload(d_first, first);
+            d_codes.alloc(std::max<unsigned long long>(2 * segments, 1) * sizeof(unsigned long long));
+            st.segment_ms += X.timed([&] {
+                vm_segment_pass(c, X.L, G, d_T.as<VmTabled>(), d_execs.as<unsigned>(), d_first.as<unsigned long long>(), (unsigned)wave.size(),
+                                segments, d_codes.as<unsigned long long>());
+                X.pad(slabs);
+            });
+            st.waves++;
+            std::vector<unsigned long long> codes(2 * segments);
+            DG_CUDA(cudaMemcpy(codes.data(), d_codes.p, codes.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+            for (size_t j = 0; j < wave.size(); j++)
+                for (unsigned long long g = first[j]; g < first[j + 1]; g++) {
+                    const unsigned code = (unsigned)codes[2 * g];
+                    if (code == VM_OK) continue;
+                    const std::string m = vm_message(code, codes[2 * g + 1], X.x.max_steps);
+                    X.fail(wave[j], DG_ERR_EXECUTION, code == VM_SEGMENT ? m : "internal error: trace segment " + std::to_string(g - first[j]) +
+                                                                             " failed where the sequential pass did not: " + m);
+                    break;
+                }
+            if (last) release();
+            done(slabs);
         });
-        std::vector<unsigned long long> codes(2 * seq.checkpoints);
-        DG_CUDA(cudaMemcpy(codes.data(), d_codes.p, codes.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-        for (unsigned long long q = 0; q < seq.checkpoints; q++) {
-            const unsigned code = (unsigned)codes[2 * q];
-            if (code == VM_OK) continue;
-            const std::string m = vm_message(code, codes[2 * q + 1], X.x.max_steps);
-            throw Error(DG_ERR_EXECUTION, code == VM_SEGMENT ? m : "internal error: trace segment " + std::to_string(q) +
-                                                                      " failed where the sequential pass did not: " + m);
-        }
     }
     // the buffers the rows no longer need, before a proof
-    void release() { for (DevBuf *d : {&d_refs, &d_items, &d_tab, &d_bad, &d_log, &d_cp, &d_seq, &d_codes, &X.d_tapes}) d->release(); }
+    void release() {
+        for (DevBuf *d : {&d_refs, &d_tab, &d_T, &d_seq, &d_codes, &d_execs, &d_first, &X.d_tapes}) d->release();
+        logs.clear();
+    }
+
+    // dg_trace_many: the fallback executions on the batch path (with the write pass even without registers_out, so that a shapes-only
+    // call reports what a full one reports), then the tabled ones
+    void trace(uint8_t *const *registers_out) {
+        tables();
+        if (run.empty()) release();
+        batch_trace(c, X, fallback, registers_out, true, false);
+        sequential();
+        if (registers_out) waves(nullptr, registers_out, [&](const std::vector<Slab> &slabs) { copy_slabs(c, X, slabs, registers_out); });
+        st.fallback = X.stats;
+    }
+    // dg_execute_many: the same, every trace proven where it was written; outs holds 8 elements per execution
+    void execute(const uint32_t *num_outputs, const dg_options_t &opt, std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats) {
+        tables();
+        if (run.empty()) release();
+        batch_execute(c, X, fallback, num_outputs, opt, outs, proofs_out, stats);
+        sequential();
+        for (unsigned e : run)
+            if (X.status[e] == DG_OK) for (uint32_t j = 0; j < num_outputs[e]; j++) outs[(size_t)e * 8 + j] = X.res[e].top[j];
+        waves(&opt, nullptr, [&](const std::vector<Slab> &slabs) { prove_slabs(c, X, slabs, num_outputs, opt, outs, proofs_out, stats, st.prove_groups); });
+        st.fallback = X.stats;
+    }
 };
 
-void one_stats(dg_trace_one_stats_t *stats, const dg_trace_one_stats_t &st) { if (stats) *stats = st; }
-
-void trace_one_path(OneExecution &E, Context &c, dg_execution_info_t *info, uint8_t *registers_out) {
-    if (!E.table()) {
-        // the batch path, with its write pass even without registers_out, so that a shapes-only call reports what a full one reports
-        Executions &X = E.X;
-        E.st.fallback = 1;
-        X.shapes();
-        uint8_t *const outs[1] = {registers_out};
-        X.write_waves(nullptr, registers_out ? outs : nullptr, [&](const std::vector<Slab> &slabs) {
-            if (registers_out && X.status[0] == DG_OK)
-                DG_CUDA(cudaMemcpy(registers_out, slabs[0].regs, (size_t)slabs[0].shape.width * slabs[0].shape.length * 16, cudaMemcpyDeviceToHost));
-        });
-        E.st.sequential_ms = X.stats.shape_ms;
-        E.st.segment_ms = X.stats.write_ms;
-        if (X.status[0] != DG_OK) throw Error(X.status[0], X.messages[0]);
-        if (info) *info = X.info(0);
-        return;
-    }
-    E.sequential();
-    const dg_execution_info_t s = E.shape();
-    if (registers_out) {
-        DevBuf regs((size_t)s.width * s.length * 16);
-        E.segments(regs.as<fe>());
-        DG_CUDA(cudaMemcpy(registers_out, regs.p, (size_t)s.width * s.length * 16, cudaMemcpyDeviceToHost));
-    }
-    if (info) *info = s;
-}
-
-Proof *execute_one_path(OneExecution &E, Context &c, const ExecutionCall &x, uint32_t num_outputs, const dg_options_t &opt, uint8_t *outputs16,
-                        dg_execution_info_t *info, dg_prove_stats_t *prove_stats) {
-    if (!E.table()) {
-        E.release();
-        dg_execution_info_t shape;                   // the batch path's shape pass gives the shape it proves
-        memset(&shape, 0, sizeof shape);
-        if (info) {
-            E.X.shapes();
-            if (E.X.status[0] == DG_OK) shape = E.X.info(0);
-        }
-        Proof *proof = nullptr;
-        int status = DG_OK;
-        std::vector<std::string> messages;
-        dg_execution_stats_t vm;
-        std::vector<uint8_t> outs(8 * 16);
-        execute_programs(c, x, &num_outputs, opt, &proof, outs.data(), &status, messages, prove_stats, &vm);
-        E.st.fallback = 1;
-        E.st.sequential_ms = vm.shape_ms;
-        E.st.segment_ms = vm.write_ms;
-        if (status != DG_OK) throw Error(status, messages[0]);
-        if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
-        if (info) *info = shape;
-        return proof;
-    }
-    E.sequential();
-    const dg_execution_info_t s = E.shape();
-    DevBuf regs((size_t)s.width * s.length * 16);
-    E.segments(regs.as<fe>());
-    E.release();
-    std::vector<fe> outs(8, fe_make(0, 0));
-    for (uint32_t j = 0; j < num_outputs; j++) outs[j] = E.X.res[0].top[j];
-    const uint8_t *in16 = x.inputs[0].public16, *out16 = (const uint8_t *)outs.data();
-    const uint32_t n_in = x.inputs[0].n_public;
-    Proof *proof = nullptr;
-    int status = DG_OK;
-    std::vector<std::string> messages;
-    prove_traces(c, regs.as<fe>(), nullptr, 1, s.width, s.length, s.ctx_depth, s.loop_depth, &in16, &n_in, &out16, &num_outputs, opt, true,
-                 &proof, &status, messages, prove_stats);
-    if (status != DG_OK) throw Error(status, messages[0]);
-    if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
-    if (info) *info = s;
-    return proof;
+// dg_trace_one's stats from the call's: after the fallback, the batch path's shape and write passes
+void one_stats(dg_trace_one_stats_t *stats, const dg_many_stats_t &m) {
+    if (!stats) return;
+    memset(stats, 0, sizeof *stats);
+    const bool fb = m.fallback_programs > 0;
+    stats->table_ms = m.table_ms;
+    stats->sequential_ms = fb ? m.fallback.shape_ms : m.sequential_ms;
+    stats->segment_ms = fb ? m.fallback.write_ms : m.segment_ms;
+    stats->table_rounds = m.table_rounds;
+    stats->table_entries = m.table_entries;
+    stats->table_levels = m.table_levels;
+    stats->sequential_launches = m.sequential_launches;
+    stats->checkpoints = m.checkpoints;
+    stats->segments = m.segments;
+    stats->logged = m.logged;
+    stats->segment_steps = m.segment_steps;
+    stats->fallback = fb ? 1 : 0;
 }
 
 }  // namespace
@@ -681,20 +839,58 @@ void check_segment_steps(uint64_t s) {
     DG_REQUIRE(s == 0 || (s >= 16 && (s & (s - 1)) == 0), "segment_steps must be 0 or a power of two of at least 16");
 }
 
+void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                std::vector<std::string> &messages, dg_many_stats_t *stats) {
+    check_execution_call(x);
+    check_segment_steps(segment_steps);
+    check_one_gpu(c);
+    TabledExecutions E(c, x, segment_steps);
+    E.trace(registers_out);
+    if (info)
+        for (uint32_t i = 0; i < x.count; i++) {
+            if (E.X.status[i] == DG_OK) info[i] = E.X.info(i);
+            else memset(&info[i], 0, sizeof info[i]);
+        }
+    finish(E.X, status, messages, nullptr);
+    if (stats) *stats = E.st;
+}
+
+void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
+                  Proof **proofs_out, uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *prove_stats,
+                  dg_many_stats_t *stats) {
+    check_execution_call(x);
+    check_output_counts(x.count, num_outputs, outputs16);
+    check_segment_steps(segment_steps);
+    check_one_gpu(c);
+    for (uint32_t i = 0; i < x.count; i++) proofs_out[i] = nullptr;
+    if (prove_stats) memset(prove_stats, 0, sizeof *prove_stats);
+    TabledExecutions E(c, x, segment_steps);
+    ReleaseOnError release{proofs_out, x.count};
+    std::vector<fe> outs((size_t)x.count * 8, fe_make(0, 0));
+    E.execute(num_outputs, opt, outs, proofs_out, prove_stats);
+    release.done = true;
+    if (outputs16) memcpy(outputs16, outs.data(), outs.size() * 16);
+    finish(E.X, status, messages, nullptr);
+    if (stats) *stats = E.st;
+}
+
 void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *registers_out,
                dg_trace_one_stats_t *stats) {
     DG_REQUIRE(x.count == 1, "one execution");
     check_execution_call(x);
     check_segment_steps(segment_steps);
     check_one_gpu(c);
-    OneExecution E(c, x, segment_steps);
+    TabledExecutions E(c, x, segment_steps);
+    uint8_t *const outs[1] = {registers_out};
     try {
-        trace_one_path(E, c, info, registers_out);
+        E.trace(registers_out ? outs : nullptr);
     } catch (...) {
         one_stats(stats, E.st);
         throw;
     }
     one_stats(stats, E.st);
+    if (E.X.status[0] != DG_OK) throw Error(E.X.status[0], E.X.messages[0]);
+    if (info) *info = E.X.info(0);
 }
 
 Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
@@ -705,15 +901,21 @@ Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uin
     check_segment_steps(segment_steps);
     check_one_gpu(c);
     if (prove_stats) memset(prove_stats, 0, sizeof *prove_stats);
-    OneExecution E(c, x, segment_steps);
+    TabledExecutions E(c, x, segment_steps);
+    Proof *proof = nullptr;
+    std::vector<fe> outs(8, fe_make(0, 0));
     try {
-        Proof *proof = execute_one_path(E, c, x, num_outputs, opt, outputs16, info, prove_stats);
-        one_stats(stats, E.st);
-        return proof;
+        E.execute(&num_outputs, opt, outs, &proof, prove_stats);
     } catch (...) {
+        delete proof;
         one_stats(stats, E.st);
         throw;
     }
+    one_stats(stats, E.st);
+    if (E.X.status[0] != DG_OK) throw Error(E.X.status[0], E.X.messages[0]);
+    if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
+    if (info) *info = E.X.info(0);
+    return proof;
 }
 
 void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
@@ -722,18 +924,9 @@ void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *inf
     check_one_gpu(c);
     Executions X(c, x);
     X.setup();
-    X.shapes();
-    if (registers_out) {
-        X.write_waves(nullptr, registers_out, [&](const std::vector<Slab> &slabs) {
-            for (const Slab &s : slabs) {
-                const size_t per = (size_t)s.shape.width * s.shape.length * 16;
-                for (size_t q = 0; q < s.ids.size(); q++)
-                    if (X.status[s.ids[q]] == DG_OK)
-                        DG_CUDA(cudaMemcpyAsync(registers_out[s.ids[q]], (const uint8_t *)s.regs + q * per, per, cudaMemcpyDeviceToHost, c.stream));
-            }
-            DG_CUDA(cudaStreamSynchronize(c.stream));
-        });
-    }
+    std::vector<unsigned> all(x.count);
+    for (uint32_t i = 0; i < x.count; i++) all[i] = i;
+    batch_trace(c, X, all, registers_out, registers_out != nullptr, true);
     if (info)
         for (uint32_t i = 0; i < x.count; i++) {
             if (X.status[i] == DG_OK) info[i] = X.info(i);
@@ -751,57 +944,11 @@ void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_ou
     if (stats) memset(stats, 0, sizeof *stats);
     Executions X(c, x);
     X.setup();
-    X.shapes();
-    // the proofs of the waves done so far are freed when a later wave fails the call
-    struct ReleaseOnError {
-        Proof **out; uint32_t count; bool done = false;
-        ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
-    } release{proofs_out, x.count};
+    ReleaseOnError release{proofs_out, x.count};
     std::vector<fe> outs((size_t)x.count * 8, fe_make(0, 0));
-    for (uint32_t i = 0; i < x.count; i++)
-        if (X.status[i] == DG_OK) for (uint32_t j = 0; j < num_outputs[i]; j++) outs[(size_t)i * 8 + j] = X.res[i].top[j];
-    X.write_waves(&opt, nullptr, [&](const std::vector<Slab> &slabs) {
-        for (const Slab &s : slabs) {
-            // executions the write pass failed are left out: the traces after them move down over them, and their outputs are zero, as
-            // those of executions the shape pass failed
-            const size_t per = (size_t)s.shape.width * s.shape.length;
-            std::vector<unsigned> ok;
-            for (size_t q = 0; q < s.ids.size(); q++) {
-                if (X.status[s.ids[q]] != DG_OK) {
-                    std::fill(outs.begin() + (size_t)s.ids[q] * 8, outs.begin() + (size_t)s.ids[q] * 8 + 8, fe_make(0, 0));
-                    continue;
-                }
-                if (ok.size() != q)
-                    DG_CUDA(cudaMemcpyAsync(s.regs + ok.size() * per, s.regs + q * per, per * 16, cudaMemcpyDeviceToDevice, c.stream));
-                ok.push_back(s.ids[q]);
-            }
-            if (ok.empty()) continue;
-            const uint32_t k = (uint32_t)ok.size();
-            std::vector<const uint8_t *> in16(k), out16(k);
-            std::vector<uint32_t> n_in(k), n_out(k);
-            for (uint32_t q = 0; q < k; q++) {
-                in16[q] = x.inputs[ok[q]].public16; n_in[q] = x.inputs[ok[q]].n_public;
-                out16[q] = (const uint8_t *)&outs[(size_t)ok[q] * 8]; n_out[q] = num_outputs[ok[q]];
-            }
-            std::vector<Proof *> proofs(k, nullptr);
-            std::vector<int> st(k, DG_OK);
-            std::vector<std::string> msg;
-            dg_prove_stats_t gs;
-            memset(&gs, 0, sizeof gs);
-            uint32_t groups = 0;
-            prove_traces(c, s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth, in16.data(), n_in.data(),
-                         out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &groups);
-            for (uint32_t q = 0; q < k; q++) {
-                proofs_out[ok[q]] = proofs[q];
-                if (st[q] != DG_OK) X.fail(ok[q], st[q], msg[q]);
-            }
-            X.stats.prove_groups += groups;
-            if (stats) {
-                for (int i = 0; i < 9; i++) stats->stage_ms[i] += gs.stage_ms[i];
-                stats->h2d_ms += gs.h2d_ms; stats->total_ms += gs.total_ms; stats->kernel_launches += gs.kernel_launches;
-            }
-        }
-    });
+    std::vector<unsigned> all(x.count);
+    for (uint32_t i = 0; i < x.count; i++) all[i] = i;
+    batch_execute(c, X, all, num_outputs, opt, outs, proofs_out, stats);
     release.done = true;
     if (outputs16) memcpy(outputs16, outs.data(), outs.size() * 16);
     finish(X, status, messages, vm_stats);

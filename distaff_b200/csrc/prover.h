@@ -73,6 +73,12 @@ void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_ex
                dg_trace_one_stats_t *stats);
 Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
                    dg_execution_info_t *info, dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats);
+// dg_trace_many / dg_execute_many (execute.cu): trace_programs / execute_programs with the executions run from the sponge tables
+void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                std::vector<std::string> &messages, dg_many_stats_t *stats);
+void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
+                  Proof **proofs_out, uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *prove_stats,
+                  dg_many_stats_t *stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP
 long long batch_group_cap(long long k);
 

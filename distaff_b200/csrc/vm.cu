@@ -9,14 +9,15 @@
 //   write pass  the same execution with the sponge, writing every register of every row up to the last step into its own place and
 //               shape (one launch covers executions of any mix of shapes); it also checks the loop images and the program hash, which
 //               need the sponge.  A second, coalesced kernel writes the padding rows of Machine::finalize, one launch per shape.
-// One long execution (dg_trace_one / dg_execute_one) runs three more kernels instead:
-//   table       the sponge chain of every block list, level by level (vm.h); the sponge never reads data, so with consistent hashes
-//               the state after every step is a table lookup
-//   sequential  the execution on one thread, as the write pass but with the sponge from the table and no register writes: it records a
+// Executions from sponge tables (dg_trace_many / dg_execute_many, and dg_trace_one / dg_execute_one as their one-execution case) run
+// three more kernels instead:
+//   table       the sponge chain of every block list of every program, level by level (vm.h); the sponge never reads data, so with
+//               consistent hashes the state after every step is a table lookup
+//   sequential  each execution on one lane, as the write pass but with the sponge from the table and no register writes: it records a
 //               checkpoint (the whole machine state) at the first top of the frame loop at or after every S steps, and logs every value
 //               popped from the tapes (hints push onto them mid-execution, so a segment cannot read the tapes itself)
-//   segment     one thread per checkpoint: replays from it to the next one with the sponge from the table and the tape values from the
-//               log, writes those rows, and checks that it ends in the state the next checkpoint holds
+//   segment     one thread per checkpoint of every execution of a wave: replays from it to the next one with the sponge from the table
+//               and the tape values from the log, writes those rows, and checks that it ends in the state the next checkpoint holds
 // The per-thread stack, context stack, loop stack and frame stack are indexed at run time and live in local memory by design.
 #define DG_MUL_CALL 1
 #include "common.cuh"
@@ -720,8 +721,8 @@ __global__ void vm_pad_kernel(fe *out, const VmResult *res, const unsigned *ids,
 // One thread per chain of a level (vm.h): the rounds of Machine<M_WRITE>, each at the cycle position its step has (every flow op is aligned
 // to the 16-step cycle, so a step's round constants depend only on its place in its frame).  A child's end_block state is [h, x, y, 0]
 // with h the state before the child: a group's x is its body's result; a switch's (x, y) are its two branch hashes and a loop's its body
-// and skip hashes, which every path through the block must reproduce -- *bad is set where one does not, or where a loop body does not
-// end on its image.
+// and skip hashes, which every path through the block must reproduce -- the item's program's bad word is set where one does not, or
+// where a loop body does not end on its image.  The items of a launch may belong to any programs of the call.
 __global__ void __launch_bounds__(64) vm_table_kernel(const VmLaunch L, const VmChainItem *items, unsigned count, const VmChainRef *chains,
                                                       VmSponge *tab, unsigned *bad) {
     const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
@@ -785,7 +786,7 @@ __global__ void __launch_bounds__(64) vm_table_kernel(const VmLaunch L, const Vm
         put();
         for (unsigned i = 1; i <= 14; i++) noop(i);
     }
-    if (!ok) atomicOr(bad, 1u);
+    if (!ok) atomicOr(bad + it.program, 1u);
 }
 
 // the start of execution e, as vm_kernel sets it up
@@ -807,17 +808,21 @@ __device__ void start(Machine<MODE> &m, const VmLaunch &L, const VmInput &in, un
     m.depth = m.max_depth = in.n_pub;
 }
 
-// The sequential pass of execution L.ids[0] on one thread: the write pass's checks, codes and steps, the sponge from the table, no
-// register writes; VmResult as the shape pass fills it, the checkpoints and the read log
-__global__ void __launch_bounds__(32) vm_sequential_kernel(const VmLaunch L, const VmTabled T, VmSequential *out) {
-    const unsigned e = L.ids[0];
+// The sequential pass of every execution L.ids[q], one per lane: the write pass's checks, codes and steps, the sponge from the tables, no
+// register writes; VmResult as the shape pass fills it, the checkpoints and the read log in T[e], their counts in out[e]
+__global__ void __launch_bounds__(32) vm_sequential_kernel(const VmLaunch L, const VmTables G, const VmTabled *T, VmSequential *out) {
+    const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= L.count) return;
+    const unsigned e = L.ids[q];
+    if (e == VM_NO_EXECUTION) return;
     const VmInput in = L.in[e];
     const VmProgram &P = L.programs[in.program];
+    const VmTabled t = T[e];
     Machine<M_SEQUENTIAL> m(L);
     start(m, L, in, e);
-    m.tab = T.tab; m.chains = T.chains; m.at = T.root; m.parent_at = 0;
-    m.log = T.log; m.lpos = 0; m.lcap = T.log_cap;
-    m.cp = (VmCheckpoint *)T.checkpoints; m.ncp = 0; m.cp_cap = T.cp_cap; m.next_cp = 0; m.seg = T.segment_steps;
+    m.tab = G.tab; m.chains = G.chains; m.at = t.root; m.parent_at = 0;
+    m.log = t.log; m.lpos = 0; m.lcap = t.log_cap;
+    m.cp = (VmCheckpoint *)t.checkpoints; m.ncp = 0; m.cp_cap = t.cp_cap; m.next_cp = 0; m.seg = G.segment_steps;
     m.run(P.root_first, P.root_count);
     if (!m.failed()) {
         if (m.opc < 16) m.fail(VM_MIN_OPS);
@@ -834,27 +839,35 @@ __global__ void __launch_bounds__(32) vm_sequential_kernel(const VmLaunch L, con
     r.loop_cols = m.loop_cols;
     r.max_depth = m.max_depth;
     for (int i = 0; i < 8; i++) r.top[i] = m.S[i];
-    out->checkpoints = m.ncp;
-    out->logged = m.lpos;
+    out[e].checkpoints = m.ncp;
+    out[e].logged = m.lpos;
 }
 
-// Segment q of execution L.ids[0]: from checkpoint q to the first frame-loop boundary at or after checkpoint q + 1's step (the last
-// segment to the end), rows written as the write pass writes them (segment 0 also row 0); codes[2q] = VM_OK, VM_SEGMENT when it does not
-// end in the recorded state, or the failure it met (both internal errors: the sequential pass ran the same execution to the end), and
-// codes[2q + 1] the step it stopped at
-__global__ void __launch_bounds__(32) vm_segment_kernel(const VmLaunch L, const VmTabled T, unsigned long long segments,
+// Global segment g is segment q of execution e = execs[j] (first[j] <= g < first[j + 1]): from its checkpoint q to the first frame-loop
+// boundary at or after checkpoint q + 1's step (its last segment to the end), rows written as the write pass writes them (segment 0 also
+// row 0); codes[2g] = VM_OK, VM_SEGMENT when it does not end in the recorded state, or the failure it met (both internal errors: the
+// sequential pass ran the same execution to the end), and codes[2g + 1] the step it stopped at
+__global__ void __launch_bounds__(32) vm_segment_kernel(const VmLaunch L, const VmTables G, const VmTabled *T, const unsigned *execs,
+                                                        const unsigned long long *first, unsigned n, unsigned long long segments,
                                                         unsigned long long *codes) {
-    const unsigned long long q = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= segments) return;
-    const unsigned e = L.ids[0];
-    const VmCheckpoint *cp = (const VmCheckpoint *)T.checkpoints;
+    const unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= segments) return;
+    unsigned lo = 0, hi = n;                          // the last j with first[j] <= g
+    while (hi - lo > 1) {
+        const unsigned mid = (lo + hi) / 2;
+        if (first[mid] <= g) lo = mid; else hi = mid;
+    }
+    const unsigned e = execs[lo];
+    const unsigned long long q = g - first[lo], count = first[lo + 1] - first[lo];
+    const VmTabled t = T[e];
+    const VmCheckpoint *cp = (const VmCheckpoint *)t.checkpoints;
     Machine<M_SEGMENT> m(L);
     m.ta = m.tb = nullptr;
     m.cap_a = m.cap_b = ~0ULL;
     m.peak_a = m.peak_b = 0;
-    m.tab = T.tab; m.chains = T.chains; m.log = T.log;
+    m.tab = G.tab; m.chains = G.chains; m.log = t.log;
     m.expect = cp + q + 1;
-    m.stop = q + 1 < segments ? cp[q + 1].step : ~0ULL;
+    m.stop = q + 1 < count ? cp[q + 1].step : ~0ULL;
     m.load(cp[q]);
     const VmOut o = L.outs[e];
     m.out = L.out + o.offset;
@@ -862,8 +875,8 @@ __global__ void __launch_bounds__(32) vm_segment_kernel(const VmLaunch L, const 
     m.ctx_out = o.ctx_out; m.loop_out = o.loop_out; m.stack_out = o.stack_out;
     if (q == 0) m.commit_state();
     m.run(0, 0);
-    codes[2 * q] = m.code;
-    codes[2 * q + 1] = m.fail_step;
+    codes[2 * g] = m.code;
+    codes[2 * g + 1] = m.fail_step;
 }
 
 }  // namespace
@@ -879,17 +892,19 @@ void vm_table_level(Context &c, const VmLaunch &L, const VmChainItem *items, uns
     DG_CUDA(cudaGetLastError());
 }
 
-void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTabled &T, VmSequential *out) {
+void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTables &G, const VmTabled *T, VmSequential *out) {
+    if (L.count == 0) return;
     vm_upload_constants(c);            // RESCR's hasher round
-    vm_sequential_kernel<<<1, 1, 0, c.stream>>>(L, T, out);
+    vm_sequential_kernel<<<(L.count + 31) / 32, 32, 0, c.stream>>>(L, G, T, out);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
-void vm_segment_pass(Context &c, const VmLaunch &L, const VmTabled &T, unsigned long long segments, unsigned long long *codes) {
+void vm_segment_pass(Context &c, const VmLaunch &L, const VmTables &G, const VmTabled *T, const unsigned *execs, const unsigned long long *first,
+                     unsigned n, unsigned long long segments, unsigned long long *codes) {
     if (segments == 0) return;
     vm_upload_constants(c);
-    vm_segment_kernel<<<(unsigned)((segments + 31) / 32), 32, 0, c.stream>>>(L, T, segments, codes);
+    vm_segment_kernel<<<(unsigned)((segments + 31) / 32), 32, 0, c.stream>>>(L, G, T, execs, first, n, segments, codes);
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }

@@ -1,4 +1,4 @@
-// The VM interpreter (vm.cu) and what the host orchestration of dg_trace_programs / dg_execute_programs (execute.cu) passes to it.
+// The VM interpreter (vm.cu) and what the host orchestration of the execution calls (execute.cu) passes to it.
 #pragma once
 #include "../../include/distaff_gpu.h"
 #include "common.cuh"
@@ -60,42 +60,51 @@ struct VmLaunch {
     const VmOut *outs;
 };
 
-// ---- one execution from a sponge table (dg_trace_one / dg_execute_one) ------------------------------------------------------------------
+// ---- executions from sponge tables (dg_trace_many / dg_execute_many; dg_trace_one / dg_execute_one) ------------------------------------
 // The sponge never reads data: with hashes that match their blocks, the state after every step of a block list's frame is a function of
 // the program.  The table holds, per block list, its chain -- the state after each step its frame owns: the span ops, the NOOP before a
 // non-first span, per child block end_block and the 14 NOOPs after it, then the NOOP close_block runs inside the list -- and, per loop,
 // the chain after BREAK (the skip's first span and its closing NOOP, from the body's last state).  The root list's chain continues with
-// the root's end_block and 14 NOOPs.
+// the root's end_block and 14 NOOPs.  Every program of a call has its chains in one table, indexed through the rebased block tables.
 struct VmSponge { fe s[4]; };
 // where the chains of a group / switch / loop block start (main: body or true branch; alt: false branch or skip; brk: after BREAK), and the
 // index of their closing entries
 struct VmChainRef { unsigned long long main, alt, brk, main_close, alt_close, brk_close; };
 // one chain to compute: a block list (children[first .. first + count), `tail`: the root's end_block and NOOPs follow its closing NOOP) or
-// the chain after BREAK of loop `block`; written from table index `out` on
+// the chain after BREAK of loop `block`, of program `program`; written from table index `out` on
 enum : unsigned { VM_CHAIN_LIST, VM_CHAIN_BREAK };
-struct VmChainItem { unsigned kind, first, count, block, tail, pad; unsigned long long out; };
+struct VmChainItem { unsigned kind, first, count, block, tail, program; unsigned long long out; };
 
-struct VmTabled {
-    VmSponge *tab;
+// the tables of a call: the chains of every tabled program, the chain references per block, and the segment length S
+struct VmTables {
+    const VmSponge *tab;
     const VmChainRef *chains;             // per block (spans unused)
-    unsigned long long root;              // where the root list's chain starts
+    unsigned long long segment_steps;
+};
+// per execution of the tabled passes
+struct VmTabled {
+    unsigned long long root;              // where its program's root list chain starts
     fe *log;                              // every value popped from tape A or B, in order
     unsigned long long log_cap;
     void *checkpoints;                    // vm_checkpoint_bytes() each
-    unsigned long long cp_cap, segment_steps;
+    unsigned long long cp_cap;
 };
-// what the sequential pass reports beside VmResult: the checkpoints it recorded (the final state after them: cp_cap must exceed this
-// count) and the values it logged (log_cap must reach it); a pass whose buffers were too small reports the sizes it needed
+// what the sequential pass reports per execution beside VmResult: the checkpoints it recorded (the final state after them: cp_cap must
+// exceed this count) and the values it logged (log_cap must reach it); a pass whose buffers were too small reports the sizes it needed
 struct VmSequential { unsigned long long checkpoints, logged; };
 
-// one launch per level: every item of a level reads only chains of lower levels; inconsistent hashes set *bad
+// one launch per level: every item of a level reads only chains of lower levels; inconsistent hashes set bad[item.program]
 void vm_table_level(Context &c, const VmLaunch &L, const VmChainItem *items, unsigned count, const VmChainRef *chains, VmSponge *tab,
                     unsigned *bad);
-// the execution L.ids[0] on one thread, sponge from the table: VmResult as the write pass reports it, plus checkpoints and the read log
-void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTabled &T, VmSequential *out);
-// one thread per segment, one segment per checkpoint: segment q replays from checkpoint q to checkpoint q + 1 (the last one to the final
-// state) and writes its rows of execution L.ids[0] as the write pass does; codes[2q] = VM_OK or why segment q stopped, codes[2q + 1] where
-void vm_segment_pass(Context &c, const VmLaunch &L, const VmTabled &T, unsigned long long segments, unsigned long long *codes);
+// every execution L.ids[q] on its lane, sponge from the tables: VmResult as the write pass reports it, T[e]'s checkpoints and read log,
+// and out[e]
+void vm_sequential_pass(Context &c, const VmLaunch &L, const VmTables &G, const VmTabled *T, VmSequential *out);
+// one thread per segment, one segment per checkpoint, for the executions execs[0 .. n): execs[j]'s segments are the global indices
+// first[j] .. first[j + 1) (first[n] = segments).  Its segment q replays from checkpoint q to checkpoint q + 1 (the last one to the final
+// state) and writes its rows into L.outs[execs[j]] as the write pass does; codes[2g] = VM_OK or why global segment g stopped,
+// codes[2g + 1] where
+void vm_segment_pass(Context &c, const VmLaunch &L, const VmTables &G, const VmTabled *T, const unsigned *execs, const unsigned long long *first,
+                     unsigned n, unsigned long long segments, unsigned long long *codes);
 size_t vm_checkpoint_bytes();
 
 void vm_upload_constants(Context &c);

@@ -82,7 +82,7 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
  * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
  * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) the message of entry i of the
  * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device, dg_verify_batch, dg_trace_batch, dg_execute_batch,
- * dg_trace_programs or dg_execute_programs: why
+ * dg_trace_programs, dg_execute_programs, dg_trace_many or dg_execute_many: why
  * trace i failed (the message dg_prove gives for that trace), why proof i was not accepted (what dg_verify reports for that proof) or
  * why execution i failed, and "" if it was proven / accepted / executed. */
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -298,6 +298,40 @@ int dg_trace_one(const dg_program_t *program, const dg_program_inputs_t *inputs,
 int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
                    uint64_t segment_steps, const dg_options_t *options, dg_proof_t **proof_out, uint8_t *outputs16, dg_execution_info_t *info,
                    dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats);
+
+/* ---- executing many long programs -----------------------------------------------------------------------------------------------
+ * dg_trace_many / dg_execute_many: dg_trace_programs / dg_execute_programs with every execution run as dg_trace_one runs one (those two
+ * are the one-execution case).  The programs' sponge tables are computed in one launch per nesting level for all of them; then one
+ * sequential launch runs every execution, one warp each, and the rows are written in waves (cut as dg_trace_programs cuts them), one
+ * segment launch per wave covering every checkpoint of every execution in it.  The tables live for the call.  A program whose hashes are
+ * inconsistent has all its executions run on the batch path in the same call, before the tabled ones.  Per execution, status[i], info[i],
+ * the message in dg_batch_message(i), the registers, the 8 elements of outputs16 (as dg_execute_programs) and the proof are exactly
+ * those of dg_trace_programs / dg_execute_programs with registers_out; a failing execution changes no other result.
+ * dg_trace_many without registers_out writes no rows, and still reports the failures that need the sponge (program hash, loop image),
+ * as dg_trace_one does.  Bad arguments are rejected before the device is touched, as dg_execute_programs rejects them, and segment_steps
+ * must be 0 (the library chooses) or a power of two >= 16; a context that spans several GPUs is rejected.
+ * RNG callbacks (dg_execute_many): first the fallback executions' proofs, in dg_execute_programs' order; then wave by wave, in every wave
+ * shape by shape (shapes ordered by width, length, context depth, loop depth) and in input order inside a shape. */
+typedef struct {
+    float table_ms, sequential_ms, segment_ms;    /* device time of the tables, the sequential launches and the segment launches (padding
+                                                     included) of the tabled executions, all waves */
+    uint64_t table_rounds, table_entries;         /* summed over the call's tabled programs */
+    uint32_t table_levels;                        /* table launches */
+    uint32_t tabled_programs, fallback_programs;  /* programs run from tables / on the batch path (inconsistent hashes) */
+    uint32_t sequential_launches;                 /* more than one when an execution needed more tape scratch, read log or checkpoints */
+    uint64_t checkpoints, segments, logged;       /* over the successful tabled executions: checkpoints recorded, segments, tape values logged */
+    uint64_t segment_steps;                       /* S used */
+    uint32_t waves;                               /* segment launches */
+    uint32_t prove_groups;                        /* prove groups of the tabled executions (dg_execute_many) */
+    dg_execution_stats_t fallback;                /* the batch path's figures for the fallback executions (zero if none) */
+} dg_many_stats_t;
+int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                  const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps, dg_execution_info_t *info,
+                  uint8_t *const *registers_out, int *status, dg_many_stats_t *stats);
+int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                    const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                    const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
+                    dg_many_stats_t *stats);
 
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
