@@ -831,11 +831,13 @@ def lde(values, blowup=32):
     return out
 
 
-HASH_IDS = {"blake3": 0, "rescue": 1, "poseidon": 2}
+HASH_IDS = {"blake3": 0, "rescue": 1, "poseidon": 2, "hasher": 3}
 
 
 def merkle_build(leaves, hash="blake3"):
-    """crypto::build_merkle_nodes (merkle.rs:269-294): bytes (n*32) -> bytes (n*32), heap layout; hash in blake3 | rescue | poseidon"""
+    """crypto::build_merkle_nodes (merkle.rs:269-294): bytes (n*32) -> bytes (n*32), heap layout; hash in blake3 | rescue | poseidon |
+    hasher (utils::hasher::digest, the VM's hash: a leaf is 2 field elements, and a tree of 2^d leaves is one smpath.n / pmpath.n verify,
+    n = d + 1)"""
     leaves = bytes(leaves)
     n = len(leaves) // 32
     out = ctypes.create_string_buffer(n * 32)
@@ -847,13 +849,134 @@ def merkle_build(leaves, hash="blake3"):
 
 
 def hash64(messages, hash="rescue"):
-    """crypto::hash::{blake3, rescue, poseidon} of n independent 64-byte messages: bytes (n*64) -> bytes (n*32)"""
+    """crypto::hash::{blake3, rescue, poseidon} or utils::hasher::digest ("hasher") of n independent 64-byte messages: bytes (n*64) ->
+    bytes (n*32)"""
     messages = bytes(messages)
     assert len(messages) % 64 == 0
     n = len(messages) // 64
     out = ctypes.create_string_buffer(max(1, n * 32))
     backend.check(backend.lib().dg_hash64(HASH_IDS[hash], messages, n, out))
     return out.raw[:n * 32]
+
+
+# ---- Merkle trees of the VM's hash, and programs that prove membership of their leaves -----------------------------------------------
+def _le_pairs(pairs):
+    return b"".join(int(v).to_bytes(16, "little") for p in pairs for v in p)
+
+
+def _int_pairs(raw):
+    v = [int.from_bytes(raw[16 * k:16 * k + 16], "little") for k in range(len(raw) // 16)]
+    return [(v[2 * k], v[2 * k + 1]) for k in range(len(v) // 2)]
+
+
+def smpath_program(n):
+    """Membership in a tree of 2^(n-1) leaves with the index private: the leaf and the path on the tapes, the index bits beside the path
+    (HasherTree.smpath_inputs).  Outputs the root in stack order, [root[1], root[0]]."""
+    _check_path_length(n)
+    return f"begin read.ab smpath.{n} end"
+
+
+def pmpath_program(n):
+    """Membership in a tree of 2^(n-1) leaves with the index public: the index is the public input, the leaf and the path are on the tapes
+    (HasherTree.pmpath_inputs).  Outputs the root in stack order, [root[1], root[0]]."""
+    _check_path_length(n)
+    return f"begin read.ab pmpath.{n} end"
+
+
+def _check_path_length(n):
+    if not 2 <= n <= 256:
+        raise ValueError(f"a Merkle path has 2 to 256 entries (smpath.n / pmpath.n), not {n}")
+
+
+class HasherTree:
+    """A Merkle tree of utils::hasher::digest over L = 2^d leaves, each a pair of field elements, in the heap layout of
+    merkle_build(..., "hasher"): nodes[L/2 + i] = digest(leaf[2i] | leaf[2i+1]), nodes[1] the root, nodes[0] zero.  Built on the GPU;
+    `nodes` (L pairs) gives the heap instead, so that the path and tape logic runs on any heap.  Its paths are those of smpath.n /
+    pmpath.n with n = depth = d + 1."""
+
+    def __init__(self, leaves, nodes=None):
+        self.leaves = [(int(a), int(b)) for a, b in leaves]
+        L = len(self.leaves)
+        if L < 2 or L & (L - 1) or L > 2**255:
+            raise ValueError(f"a tree has 2^d leaves, 1 <= d <= 255, not {L}")
+        if nodes is None:
+            nodes = _int_pairs(merkle_build(_le_pairs(self.leaves), "hasher"))
+        self.nodes = [(int(a), int(b)) for a, b in nodes]
+        if len(self.nodes) != L:
+            raise ValueError(f"the heap of {L} leaves has {L} nodes, not {len(self.nodes)}")
+
+    @property
+    def root(self):
+        return list(self.nodes[1])
+
+    @property
+    def depth(self):
+        """n of smpath.n / pmpath.n: the number of entries of a path"""
+        return len(self.leaves).bit_length()
+
+    def _index(self, i):
+        i = int(i)
+        if not 0 <= i < len(self.leaves):
+            raise IndexError(f"leaf {i} of a tree of {len(self.leaves)} leaves")
+        return i
+
+    def path(self, i):
+        """the path of examples/merkle.rs: [leaf i, leaf i^1, then the sibling of every node from leaf i's parent up to the root's child]"""
+        i = self._index(i)
+        p, k = [self.leaves[i], self.leaves[i ^ 1]], (len(self.leaves) + i) >> 1
+        while k > 1:
+            p.append(self.nodes[k ^ 1])
+            k >>= 1
+        return p
+
+    def _smpath_tapes(self, i):
+        """tapes A and B of smpath: the leaf, then per later entry (0, index bit) and the entry (merkle.rs:63-85)"""
+        path, bits = self.path(i), i
+        a, b = [path[0][0]], [path[0][1]]
+        for node in path[1:]:
+            a += [0, node[0]]
+            b += [bits & 1, node[1]]
+            bits >>= 1
+        return a, b
+
+    def tapes(self, i):
+        """(tape A, tape B) of the program of examples/merkle.rs (hostvm.merkle_program(depth, i)), as generate_program_inputs
+        (merkle.rs:63-94) lays them out: the smpath tapes, then every entry after the leaf again for pmpath"""
+        a, b = self._smpath_tapes(self._index(i))
+        path = self.path(i)
+        return a + [e[0] for e in path[1:]], b + [e[1] for e in path[1:]]
+
+    def smpath_inputs(self, i):
+        """the ProgramInputs of smpath_program(depth) for leaf i"""
+        a, b = self._smpath_tapes(self._index(i))
+        return ProgramInputs([], a, b)
+
+    def pmpath_inputs(self, i):
+        """the ProgramInputs of pmpath_program(depth) for leaf i: the index public, the leaf and the path on the tapes"""
+        path = self.path(i)
+        return ProgramInputs([int(i)], [e[0] for e in path], [e[1] for e in path])
+
+
+def prove_membership(tree, indexes, program="smpath", options=None):
+    """Proves that leaves of a HasherTree belong to it: one execute_batch call runs smpath_program(tree.depth) (index private) or
+    pmpath_program(tree.depth) (index public) for every index.  Returns a list in index order: (program_hash, public_inputs, outputs,
+    proof), an item of verify_batch whose outputs are the root in stack order, or a DgError for an entry whose execution failed or did not
+    output the root."""
+    if program not in ("smpath", "pmpath"):
+        raise ValueError(f"program is smpath or pmpath, not {program!r}")
+    indexes = [tree._index(i) for i in indexes]
+    prog = hostvm.compile_program(smpath_program(tree.depth) if program == "smpath" else pmpath_program(tree.depth))
+    inputs = [tree.smpath_inputs(i) if program == "smpath" else tree.pmpath_inputs(i) for i in indexes]
+    want = tree.root[::-1]
+    out = []
+    for i, x, r in zip(indexes, inputs, execute_batch(prog, inputs, num_outputs=2, options=options)):
+        if isinstance(r, backend.DgError):
+            out.append(r)
+        elif r[0] != want:
+            out.append(backend.DgError(-7, f"leaf {i}: the {program} program output {r[0]}, not the root"))
+        else:
+            out.append((prog.hash, x.public, r[0], r[1]))
+    return out
 
 
 def hash_rows(columns):

@@ -1,4 +1,5 @@
-// Algebraic hash functions over F_M on the GPU: Rescue and Poseidon, one thread per 64-byte message, and Merkle trees built with them.
+// Algebraic hash functions over F_M on the GPU: Rescue and Poseidon, one thread per 64-byte message, and Merkle trees built with them
+// and with the VM's hasher (hasher.cu, hash 3).
 //
 // Replaces (SURVEY.md section 8 row a10, micro-benchmark config C5)
 //   hash::rescue     /root/reference/src/crypto/hash.rs:151-177
@@ -18,6 +19,7 @@
 #include "air_constants.h"
 #include "blake3.cuh"
 #include "alg_sbox.cuh"
+#include "poly.h"
 
 namespace dg {
 
@@ -106,8 +108,9 @@ __global__ void __launch_bounds__(128) alg_hash64_kernel(const uint4 *__restrict
 }
 
 void alg_hash64(Context &c, int hash_id, const void *in, void *out, unsigned long long n) {
-    DG_REQUIRE(hash_id >= 0 && hash_id <= 2, "hash id must be 0 (blake3), 1 (rescue) or 2 (poseidon)");
+    DG_REQUIRE(hash_id >= 0 && hash_id <= 3, "hash id must be 0 (blake3), 1 (rescue), 2 (poseidon) or 3 (hasher)");
     if (n == 0) return;
+    if (hash_id == 3) return hasher_digest(c, in, out, n);            // DG_HASH_HASHER
     alg_upload_constants(c);
     const unsigned grid = (unsigned)((n + 127) / 128);
     switch (hash_id) {

@@ -275,13 +275,27 @@ int dg_merkle_build(const uint8_t *leaves, uint64_t n_leaves, uint8_t *nodes) {
         DG_CUDA(cudaStreamSynchronize(c.stream));
     });
 }
+// the VM's hasher takes field elements only (a tape value >= M fails its execution): rejects the first of n items of `width` little-endian
+// u128 elements that holds one
+static void require_canonical(const uint8_t *items, uint64_t n, unsigned width, const char *what) {
+    DG_REQUIRE(items, "null buffer");
+    for (uint64_t k = 0; k < n * width; k++) {
+        uint64_t lo, hi;
+        memcpy(&lo, items + 16 * k, 8);
+        memcpy(&hi, items + 16 * k + 8, 8);
+        if (hi == DG_M_HI && lo >= DG_M_LO)
+            throw dg::Error(DG_ERR_INVALID, std::string(what) + " " + std::to_string(k / width) + " element " + std::to_string(k % width) +
+                                                " is not a field element (>= M)");
+    }
+}
 int dg_hash64(int hash, const uint8_t *messages64, uint64_t n, uint8_t *digests32) {
     return guarded([&] {
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        DG_REQUIRE(hash >= 0 && hash <= 2, "hash id must be 0 (blake3), 1 (rescue) or 2 (poseidon)");
+        DG_REQUIRE(hash >= 0 && hash <= 3, "hash id must be 0 (blake3), 1 (rescue), 2 (poseidon) or 3 (hasher)");
         if (n == 0) return;
         DG_REQUIRE(messages64 && digests32, "null buffer");
+        if (hash == DG_HASH_HASHER) require_canonical(messages64, n, 4, "message");
         DevBuf d_in(n * 64), d_out(n * 32);
         DG_CUDA(cudaMemcpyAsync(d_in.p, messages64, n * 64, cudaMemcpyHostToDevice, c.stream));
         alg_hash64(c, hash, d_in.p, d_out.p, n);
@@ -294,6 +308,7 @@ int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uin
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         DG_REQUIRE(n_leaves >= 2 && (n_leaves & (n_leaves - 1)) == 0, "number of leaves must be a power of 2 and >= 2");
+        if (hash == DG_HASH_HASHER) require_canonical(leaves, n_leaves, 2, "leaf");
         DevBuf d_l(n_leaves * 32), d_n(n_leaves * 32);
         DG_CUDA(cudaMemcpyAsync(d_l.p, leaves, n_leaves * 32, cudaMemcpyHostToDevice, c.stream));
         alg_merkle_build(c, hash, d_l.p, d_n.p, n_leaves);

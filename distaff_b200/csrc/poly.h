@@ -65,8 +65,12 @@ void merkle_build(Context &c, const void *leaves, void *nodes, unsigned long lon
 // levels of a heap-layout tree from L/2 nodes down to (and including) the level with `stop` nodes
 void merkle_levels_down_to(Context &c, const void *leaves, void *nodes, unsigned long long L, unsigned long long stop);
 void merkle_finish(Context &c, void *nodes, unsigned long long m);     // level with m nodes already at nodes[m..2m)
-// alghash.cu: blake3 / rescue / poseidon over 64-byte messages, and Merkle trees with them
+// alghash.cu: blake3 / rescue / poseidon / the VM's hasher over 64-byte messages, and Merkle trees with them
 void alg_hash64(Context &c, int hash_id, const void *in, void *out, unsigned long long n);
+// hasher::digest of n messages of 4 elements (64 bytes) into 2 elements (32 bytes) each: fewer than HASHER_WIDE_MIN messages run the
+// narrow layout (8 lanes per message), more the wide one (a thread per message)
+constexpr unsigned long long HASHER_WIDE_MIN = 1ULL << 16;     // measured crossover on an H100 (DESIGN.md section 7j)
+void hasher_digest(Context &c, const void *in, void *out, unsigned long long n);
 void alg_merkle_build(Context &c, int hash_id, const void *leaves, void *nodes, unsigned long long L);
 // the smallest proof-of-work nonce >= 1 of every seed, one kernel per round for all of them; result i belongs to seeds[i]
 std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<std::array<uint8_t, 32>> &seeds, unsigned grinding);

@@ -431,10 +431,20 @@ int dg_hash_rows(const uint8_t *columns, uint32_t width, uint64_t rows, uint8_t 
 int dg_find_pow_nonce(const uint8_t seed[32], uint32_t grinding_factor, uint64_t *nonce, uint8_t new_seed[32]);
 /* crypto::hash::{blake3, rescue, poseidon} (hash.rs:119-177,205-209) over n independent 64-byte messages -> n 32-byte digests
  * (benches/hash.rs), and build_merkle_nodes (merkle.rs:269-294) with any of them.  hash: 0 blake3, 1 rescue, 2 poseidon -- ids of
- * THIS interface; a proof can only carry blake3 (options.rs:97-125).  Messages must hold valid field elements for 1 and 2 (field.rs:25). */
+ * THIS interface; a proof can only carry blake3 (options.rs:97-125).  Messages must hold valid field elements for 1 and 2 (field.rs:25).
+ *
+ * hash 3 is utils::hasher::digest (hasher.rs:12-40), the hash of the VM's RESCR op, so a tree built with it is one that the smpath /
+ * pmpath operations of a program verify.  A message is 4 field elements (64 bytes, each a little-endian u128) and its digest 2 elements
+ * (32 bytes); a message of 1-3 elements hashes as its zero-padded form.  A leaf is 2 elements, and the heap is nodes[L/2 + i] =
+ * digest(leaf[2i] | leaf[2i+1]), nodes[i] = digest(nodes[2i] | nodes[2i+1]), nodes[1] the root, nodes[0] zero.  A tree of L = 2^d
+ * leaves has the authentication paths of smpath.n / pmpath.n with n = d + 1, and 2 <= n <= 256 (so 2 <= L <= 2^255).  dg_hash64 and
+ * dg_merkle_build_with reject a message or leaf element >= M (DG_ERR_INVALID, naming the first such message or leaf and its element);
+ * dg_dev_merkle_build_with expects canonical leaves, as for 1 and 2.  Levels of fewer than 2^16 digests run a kernel that splits each
+ * digest over 8 lanes, wider ones a thread per digest. */
 #define DG_HASH_BLAKE3 0
 #define DG_HASH_RESCUE 1
 #define DG_HASH_POSEIDON 2
+#define DG_HASH_HASHER 3
 int dg_hash64(int hash, const uint8_t *messages64, uint64_t n, uint8_t *digests32);
 int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uint8_t *nodes);
 /* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b), 6 mul with b as a fixed twiddle: the NTT pass
