@@ -958,16 +958,21 @@ class HasherTree:
 
 
 def prove_membership(tree, indexes, program="smpath", options=None):
-    """Proves that leaves of a HasherTree belong to it: one execute_batch call runs smpath_program(tree.depth) (index private) or
+    """Proves that leaves of a HasherTree, or of a MerkleTree of hash "hasher" (its paths from one dg_tree_paths call, laid out as
+    HasherTree.smpath_inputs / pmpath_inputs lay them out), belong to it: one execute_batch call runs smpath_program(tree.depth) (index private) or
     pmpath_program(tree.depth) (index public) for every index.  Returns a list in index order: (program_hash, public_inputs, outputs,
     proof), an item of verify_batch whose outputs are the root in stack order, or a DgError for an entry whose execution failed or did not
     output the root."""
     if program not in ("smpath", "pmpath"):
         raise ValueError(f"program is smpath or pmpath, not {program!r}")
-    indexes = [tree._index(i) for i in indexes]
+    if isinstance(tree, MerkleTree):
+        indexes, inputs, root = tree._membership_inputs(indexes, program)
+    else:
+        indexes = [tree._index(i) for i in indexes]
+        inputs = [tree.smpath_inputs(i) if program == "smpath" else tree.pmpath_inputs(i) for i in indexes]
+        root = tree.root
     prog = hostvm.compile_program(smpath_program(tree.depth) if program == "smpath" else pmpath_program(tree.depth))
-    inputs = [tree.smpath_inputs(i) if program == "smpath" else tree.pmpath_inputs(i) for i in indexes]
-    want = tree.root[::-1]
+    want = root[::-1]
     out = []
     for i, x, r in zip(indexes, inputs, execute_batch(prog, inputs, num_outputs=2, options=options)):
         if isinstance(r, backend.DgError):
@@ -977,6 +982,149 @@ def prove_membership(tree, indexes, program="smpath", options=None):
         else:
             out.append((prog.hash, x.public, r[0], r[1]))
     return out
+
+
+class MerkleTree:
+    """crypto::MerkleTree (merkle.rs:22-62) kept in device memory (dg_tree_*): L = 2^d leaves of 32 bytes and the heap of
+    merkle_build(leaves, hash), built once on the GPU.  paths() gathers the authentication paths of many leaves in one call and copies
+    only those; update() replaces leaves and rehashes only the nodes on their paths.  `leaves` is L x 32 bytes, a contiguous CUDA uint8
+    tensor of L x 32 bytes on the library's device (copied into the tree's own buffer), or, for hash="hasher" only, a sequence of (a, b)
+    field-element pairs as HasherTree takes them.  The tree holds 64 L bytes of the library's device memory until close()."""
+
+    def __init__(self, leaves, hash="blake3"):
+        if hash not in HASH_IDS:
+            raise ValueError(f"hash is one of {', '.join(HASH_IDS)}, not {hash!r}")
+        self.hash = hash
+        self._h = None
+        handle = backend.vp()
+        if getattr(leaves, "is_cuda", False):
+            import torch
+            if leaves.dtype != torch.uint8 or not leaves.is_contiguous() or leaves.numel() % 32:
+                raise ValueError("device leaves are a contiguous uint8 tensor of L x 32 bytes")
+            torch.cuda.synchronize(leaves.device)                # the copy runs on the library's stream
+            backend.check(backend.lib().dg_tree_new_device(HASH_IDS[hash], leaves.data_ptr(), leaves.numel() // 32, ctypes.byref(handle)))
+        else:
+            raw = self._leaf_bytes(leaves)
+            backend.check(backend.lib().dg_tree_new(HASH_IDS[hash], raw, len(raw) // 32, ctypes.byref(handle)))
+        self._h = handle.value
+        n = backend.u64(0)
+        backend.check(backend.lib().dg_tree_info(self._h, None, ctypes.byref(n), None))
+        self._n = n.value
+
+    def _leaf_bytes(self, leaves):
+        if isinstance(leaves, (bytes, bytearray, memoryview, np.ndarray)):
+            raw = leaves.tobytes() if isinstance(leaves, np.ndarray) else bytes(leaves)
+        elif self.hash == "hasher":
+            pairs = [(int(a), int(b)) for a, b in leaves]
+            if any(not 0 <= v < 2**128 for p in pairs for v in p):
+                raise ValueError("a leaf element is an integer in [0, 2^128)")
+            raw = _le_pairs(pairs)
+        else:
+            raise TypeError(f"leaves of a {self.hash} tree are bytes of L x 32")
+        if len(raw) % 32:
+            raise ValueError(f"leaves are 32 bytes each, not {len(raw)} bytes in all")
+        return raw
+
+    def _handle(self):
+        if not self._h:
+            raise ValueError("the tree is closed")
+        return self._h
+
+    @staticmethod
+    def _indexes(indexes):
+        idx = np.asarray(indexes if isinstance(indexes, np.ndarray) else list(indexes), dtype=np.int64).reshape(-1)
+        if (idx < 0).any():
+            raise ValueError("leaf indexes are non-negative")
+        return idx.astype(np.uint64)
+
+    def __len__(self):
+        return self._n
+
+    @property
+    def depth(self):
+        """d + 1 for L = 2^d: the number of entries of a path, n of smpath.n / pmpath.n (HasherTree.depth)"""
+        return self._n.bit_length()
+
+    @property
+    def root(self):
+        """nodes[1], 32 bytes"""
+        out = ctypes.create_string_buffer(32)
+        backend.check(backend.lib().dg_tree_info(self._handle(), None, None, out))
+        return out.raw
+
+    def paths(self, indexes):
+        """one dg_tree_paths call: per index, its depth entries of 32 bytes in MerkleTree::prove order (leaf i, leaf i ^ 1, then the
+        sibling of every node from leaf i's parent up to the root's child).  An index >= len(tree) raises DgError naming it."""
+        idx, e = self._indexes(indexes), self.depth
+        if len(idx) == 0:
+            return []
+        out = ctypes.create_string_buffer(32 * e * len(idx))
+        backend.check(backend.lib().dg_tree_paths(self._handle(), idx.ctypes.data, len(idx), out))
+        raw = out.raw
+        return [[raw[32 * (k * e + j):32 * (k * e + j + 1)] for j in range(e)] for k in range(len(idx))]
+
+    def update(self, indexes, leaves):
+        """the leaf at indexes[k] becomes leaves[k] (a repeated index: its last occurrence); rehashes only the changed paths and returns
+        the new root.  A rejected call (an index out of range, a non-canonical hasher leaf) leaves the tree as it was."""
+        idx, raw = self._indexes(indexes), self._leaf_bytes(leaves)
+        if len(raw) != 32 * len(idx):
+            raise ValueError(f"{len(idx)} indexes and {len(raw) // 32} leaves")
+        root = ctypes.create_string_buffer(32)
+        backend.check(backend.lib().dg_tree_update(self._handle(), idx.ctypes.data if len(idx) else None, raw, len(idx), root))
+        return root.raw
+
+    def leaves(self):
+        out = ctypes.create_string_buffer(32 * self._n)
+        backend.check(backend.lib().dg_tree_read(self._handle(), out, None))
+        return out.raw
+
+    def nodes(self):
+        """the heap of merkle_build: nodes[1] the root, nodes[0] zero"""
+        out = ctypes.create_string_buffer(32 * self._n)
+        backend.check(backend.lib().dg_tree_read(self._handle(), None, out))
+        return out.raw
+
+    def _index(self, i):
+        i = int(i)
+        if not 0 <= i < self._n:
+            raise IndexError(f"leaf {i} of a tree of {self._n} leaves")
+        return i
+
+    def _membership_inputs(self, indexes, program):
+        """prove_membership's indexes, ProgramInputs and root (field elements) from one paths() call"""
+        if self.hash != "hasher":
+            raise ValueError(f"membership proofs verify paths of the VM's hash: a MerkleTree of hash 'hasher', not {self.hash!r}")
+        indexes = [self._index(i) for i in indexes]
+        inputs = []
+        for i, entries in zip(indexes, self.paths(indexes)):
+            path = _int_pairs(b"".join(entries))
+            if program == "smpath":                  # HasherTree.smpath_inputs: the leaf, then per entry (0, index bit) and the entry
+                a, b, bits = [path[0][0]], [path[0][1]], i
+                for node in path[1:]:
+                    a += [0, node[0]]
+                    b += [bits & 1, node[1]]
+                    bits >>= 1
+                inputs.append(ProgramInputs([], a, b))
+            else:                                    # HasherTree.pmpath_inputs: the index public, the path on the tapes
+                inputs.append(ProgramInputs([i], [e[0] for e in path], [e[1] for e in path]))
+        return indexes, inputs, list(_int_pairs(self.root)[0])
+
+    def close(self):
+        if self._h:
+            backend.lib().dg_tree_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def hash_rows(columns):

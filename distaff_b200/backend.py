@@ -151,6 +151,12 @@ EXPORTS = {
     "dg_hash_rows": [vp, u32, u64, vp],
     "dg_hash64": [ctypes.c_int, vp, u64, vp],
     "dg_merkle_build_with": [ctypes.c_int, vp, u64, vp],
+    "dg_tree_new": [ctypes.c_int, vp, u64, ctypes.POINTER(vp)],
+    "dg_tree_new_device": [ctypes.c_int, vp, u64, ctypes.POINTER(vp)],
+    "dg_tree_info": [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(u64), vp],
+    "dg_tree_paths": [vp, vp, u32, vp],
+    "dg_tree_update": [vp, vp, vp, u32, vp],
+    "dg_tree_read": [vp, vp, vp],
     "dg_find_pow_nonce": [vp, u32, ctypes.POINTER(u64), vp],
     "dg_field_op": [ctypes.c_int, ctypes.c_int, vp, vp, vp, u64],
     "dg_field_dot": [vp, vp, vp, u64, u32],
@@ -176,6 +182,7 @@ EXPORTS = {
     "dg_host_query_positions": [vp, u64, u32, u32, vp],
     "dg_host_blake3": [vp, ctypes.c_size_t, vp],
     "dg_host_plan_batch": [vp, u32, u64, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
+    "dg_host_tree_plan": [vp, u32, u64, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
     "dg_host_merkle_verify_plan": [vp, u32, u32, u32, vp, u32, vp, ctypes.c_size_t, vp, vp, ctypes.c_size_t, vp, vp],
     "dg_host_periodic_tables": [vp],
     "dg_host_constraint_name": [u32, u32, u32, u32, ctypes.c_char_p, ctypes.c_size_t],
@@ -183,7 +190,7 @@ EXPORTS = {
     "dg_memory_usage": [ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)],
     "dg_plan_prove": [u32, u64, u32, ctypes.POINTER(DgOptions), ctypes.POINTER(DgProvePlan)],
 }
-VOID_EXPORTS = {"dg_proof_free": [vp]}
+VOID_EXPORTS = {"dg_proof_free": [vp], "dg_tree_free": [vp]}
 
 
 def lib():

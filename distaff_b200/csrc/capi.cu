@@ -6,6 +6,8 @@
 #include "shard.h"
 #include "poly.h"
 #include "air.h"
+#include "tree.h"
+#include <memory>
 #include <thread>
 
 using namespace dg;
@@ -316,6 +318,109 @@ int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uin
         DG_CUDA(cudaStreamSynchronize(c.stream));
     });
 }
+
+// ---- Merkle trees that stay on the GPU (tree.cu) ---------------------------------------------------------------------------------------
+static void require_tree_shape(int hash, uint64_t n_leaves) {
+    DG_REQUIRE(hash >= 0 && hash <= 3, "hash id must be 0 (blake3), 1 (rescue), 2 (poseidon) or 3 (hasher)");
+    DG_REQUIRE(n_leaves >= 2 && (n_leaves & (n_leaves - 1)) == 0, "number of leaves must be a power of 2 and >= 2");
+}
+static void require_tree_indexes(const Tree &t, const uint64_t *indexes, uint32_t count) {
+    for (uint32_t k = 0; k < count; k++)
+        if (indexes[k] >= t.L)
+            throw Error(DG_ERR_INVALID, "index " + std::to_string(indexes[k]) + " (entry " + std::to_string(k) + ") is not a leaf of a tree of " +
+                                            std::to_string(t.L) + " leaves");
+}
+// a new tree on the primary context, its buffers from the pool; `fill` copies the leaves in
+static Tree *new_tree(int hash, uint64_t n_leaves, const std::function<void(Context &, Tree &)> &fill) {
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    std::unique_ptr<Tree> t(new Tree());
+    t->hash = hash;
+    t->L = n_leaves;
+    t->leaves.alloc(n_leaves * 32, true);
+    t->nodes.alloc(n_leaves * 32, true);
+    fill(c, *t);
+    tree_build(c, *t);
+    return t.release();
+}
+int dg_tree_new(int hash, const uint8_t *leaves32, uint64_t n_leaves, dg_tree_t **tree) {
+    return guarded([&] {
+        DG_REQUIRE(tree && leaves32, "null argument");
+        *tree = nullptr;
+        require_tree_shape(hash, n_leaves);
+        if (hash == DG_HASH_HASHER) require_canonical(leaves32, n_leaves, 2, "leaf");
+        *tree = (dg_tree_t *)new_tree(hash, n_leaves, [&](Context &c, Tree &t) {
+            DG_CUDA(cudaMemcpyAsync(t.leaves.p, leaves32, n_leaves * 32, cudaMemcpyHostToDevice, c.stream));
+        });
+    });
+}
+int dg_tree_new_device(int hash, const void *d_leaves32, uint64_t n_leaves, dg_tree_t **tree) {
+    return guarded([&] {
+        DG_REQUIRE(tree && d_leaves32, "null argument");
+        *tree = nullptr;
+        require_tree_shape(hash, n_leaves);
+        *tree = (dg_tree_t *)new_tree(hash, n_leaves, [&](Context &c, Tree &t) {
+            DG_CUDA(cudaMemcpyAsync(t.leaves.p, d_leaves32, n_leaves * 32, cudaMemcpyDeviceToDevice, c.stream));
+        });
+    });
+}
+int dg_tree_info(const dg_tree_t *tree, int *hash, uint64_t *n_leaves, uint8_t root32[32]) {
+    return guarded([&] {
+        DG_REQUIRE(tree, "null tree");
+        const Tree &t = *(const Tree *)tree;
+        if (hash) *hash = t.hash;
+        if (n_leaves) *n_leaves = t.L;
+        if (root32) memcpy(root32, t.root, 32);
+    });
+}
+int dg_tree_paths(const dg_tree_t *tree, const uint64_t *indexes, uint32_t count, uint8_t *paths32) {
+    return guarded([&] {
+        DG_REQUIRE(tree, "null tree");
+        DG_REQUIRE(count == 0 || (indexes && paths32), "null buffer");
+        const Tree &t = *(const Tree *)tree;
+        require_tree_indexes(t, indexes, count);
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        tree_paths(c, t, indexes, count, paths32);
+    });
+}
+int dg_tree_update(dg_tree_t *tree, const uint64_t *indexes, const uint8_t *leaves32, uint32_t count, uint8_t root32[32]) {
+    return guarded([&] {
+        DG_REQUIRE(tree, "null tree");
+        DG_REQUIRE(count == 0 || (indexes && leaves32), "null buffer");
+        Tree &t = *(Tree *)tree;
+        require_tree_indexes(t, indexes, count);
+        if (t.hash == DG_HASH_HASHER && count) require_canonical(leaves32, count, 2, "leaf");
+        if (count) {
+            const TreePlan plan = plan_tree_update(indexes, count, t.L);
+            Context &c = ctx();
+            std::lock_guard<std::mutex> lk(c.mu);
+            tree_update(c, t, plan, leaves32);
+        }
+        if (root32) memcpy(root32, t.root, 32);
+    });
+}
+int dg_tree_read(const dg_tree_t *tree, uint8_t *leaves32, uint8_t *nodes32) {
+    return guarded([&] {
+        DG_REQUIRE(tree, "null tree");
+        const Tree &t = *(const Tree *)tree;
+        if (!leaves32 && !nodes32) return;
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        if (leaves32) DG_CUDA(cudaMemcpyAsync(leaves32, t.leaves.p, t.L * 32, cudaMemcpyDeviceToHost, c.stream));
+        if (nodes32) DG_CUDA(cudaMemcpyAsync(nodes32, t.nodes.p, t.L * 32, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+    });
+}
+void dg_tree_free(dg_tree_t *tree) {
+    if (!tree) return;
+    guarded([&] {                         // a tree exists only on a context, so ctx() does not throw here
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        delete (Tree *)tree;              // the buffers go back to the pool in stream order
+    });
+}
+
 int dg_hash_rows(const uint8_t *columns, uint32_t width, uint64_t rows, uint8_t *digests) {
     return guarded([&] {
         Context &c = ctx();
@@ -894,6 +999,29 @@ int dg_host_plan_batch(const uint64_t *indexes, uint32_t n_indexes, uint64_t n_l
         for (auto &slot : plan.nodes) {
             flat.push_back(slot.size());
             for (auto &r : slot) { flat.push_back(r.leaf ? 1 : 0); flat.push_back(r.index); }
+        }
+        DG_REQUIRE(flat.size() <= cap, "buffer too small");
+        memcpy(out, flat.data(), flat.size() * 8);
+        *written = flat.size();
+    });
+}
+int dg_host_tree_plan(const uint64_t *indexes, uint32_t count, uint64_t n_leaves, uint64_t *out, size_t cap, size_t *written) {
+    return guarded([&] {
+        DG_REQUIRE((indexes || count == 0) && out && written, "null argument");
+        DG_REQUIRE(n_leaves >= 2 && (n_leaves & (n_leaves - 1)) == 0, "number of leaves must be a power of 2 and >= 2");
+        Tree t;
+        t.L = n_leaves;
+        require_tree_indexes(t, indexes, count);
+        const TreePlan p = plan_tree_update(indexes, count, n_leaves);
+        std::vector<uint64_t> flat = {(uint64_t)p.leaves.size(), (uint64_t)p.level_size.size(), (uint64_t)p.ids.size()};
+        flat.insert(flat.end(), p.leaves.begin(), p.leaves.end());
+        flat.insert(flat.end(), p.source.begin(), p.source.end());
+        size_t at = 0;
+        for (uint32_t n : p.level_size) {
+            flat.push_back(n);
+            flat.insert(flat.end(), p.ids.begin() + at, p.ids.begin() + at + n);
+            flat.insert(flat.end(), p.first.begin() + at, p.first.begin() + at + n);
+            at += n;
         }
         DG_REQUIRE(flat.size() <= cap, "buffer too small");
         memcpy(out, flat.data(), flat.size() * 8);

@@ -447,6 +447,35 @@ int dg_find_pow_nonce(const uint8_t seed[32], uint32_t grinding_factor, uint64_t
 #define DG_HASH_HASHER 3
 int dg_hash64(int hash, const uint8_t *messages64, uint64_t n, uint8_t *digests32);
 int dg_merkle_build_with(int hash, const uint8_t *leaves, uint64_t n_leaves, uint8_t *nodes);
+
+/* ---- Merkle trees that stay on the GPU (crypto::MerkleTree, merkle.rs:22-62, kept in device memory) ---------------------------------
+ * A dg_tree_t holds L = 2^d leaves and the heap of dg_merkle_build_with (byte for byte) in device memory, on the library's primary device
+ * and context; it is owned by the library until dg_tree_free().  Its two buffers (64 L bytes) come from the context's stream-ordered pool,
+ * so dg_memory_usage counts a live tree and proofs that run beside it see that memory as taken.  Hash ids as for dg_merkle_build_with.
+ * Without a CUDA device every entry point that takes leaves or a tree returns DG_ERR_NO_DEVICE. */
+typedef struct dg_tree dg_tree_t;
+/* builds a tree of n_leaves x 32 bytes of host leaves.  The checks of dg_merkle_build_with, with its messages, before the device is
+ * touched: a hash id of 0-3, L a power of 2 >= 2, and for hash 3 every leaf element < M (the first bad leaf is named). */
+int dg_tree_new(int hash, const uint8_t *leaves32, uint64_t n_leaves, dg_tree_t **tree);
+/* the same from leaves in device memory, copied into the tree's own buffer; like dg_dev_merkle_build_with it expects canonical leaves */
+int dg_tree_new_device(int hash, const void *d_leaves32, uint64_t n_leaves, dg_tree_t **tree);
+/* the hash id, the number of leaves and the root (nodes[1]); each may be NULL.  Touches no device: the root is kept on the host. */
+int dg_tree_info(const dg_tree_t *tree, int *hash, uint64_t *n_leaves, uint8_t root32[32]);
+/* the authentication paths of count leaves (MerkleTree::prove, merkle.rs:47-62) in one launch: paths32 receives count x (d + 1) entries
+ * of 32 bytes, path k at k (d + 1), each leaf i, leaf i ^ 1, then nodes[((L + i) >> 1 >> j) ^ 1] for j = 0 .. d - 2.  For hash 3 this is
+ * the path of smpath.n / pmpath.n with n = d + 1.  Indexes may repeat and come in any order; one >= L fails the call with DG_ERR_INVALID
+ * naming it.  Only the paths are copied to the host. */
+int dg_tree_paths(const dg_tree_t *tree, const uint64_t *indexes, uint32_t count, uint8_t *paths32);
+/* the leaf at indexes[k] becomes leaves32[k] (a repeated index: its last occurrence), and only the nodes on the changed leaves' paths are
+ * hashed again, one pass per level: at most count x d digests instead of L - 1.  When the changed paths hold at least half of the L - 1
+ * nodes, the call writes the new leaves and builds the tree again instead, which measured faster there.  Every argument is checked before the device changes
+ * (indexes < L, and for hash 3 canonical leaves, named as dg_tree_new names them): a failed call leaves the tree as it was.  root32 (may be
+ * NULL) receives the new root; count == 0 changes nothing and gives the current root. */
+int dg_tree_update(dg_tree_t *tree, const uint64_t *indexes, const uint8_t *leaves32, uint32_t count, uint8_t root32[32]);
+/* copies the L leaves and / or the L heap nodes to the host; either may be NULL */
+int dg_tree_read(const dg_tree_t *tree, uint8_t *leaves32, uint8_t *nodes32);
+void dg_tree_free(dg_tree_t *tree);
+
 /* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b), 6 mul with b as a fixed twiddle: the NTT pass
  * kernels' product with a precomputed companion b * 2^64), for differential tests of the arithmetic;
  * impl: 0 = PTX path used by the kernels, 1 = portable C++ path, 2 / 3 = earlier PTX multiplies (op 2 only) */
@@ -509,6 +538,11 @@ int dg_host_blake3(const uint8_t *data, size_t len, uint8_t out32[32]);
 /* MerkleTree::prove_batch planning (merkle.rs:64-124): writes, per normalised slot, the count and then (is_leaf, index) pairs;
  * out layout: [n_slots][depth] then for each slot [count] (is_leaf, index)*count, all uint64 */
 int dg_host_plan_batch(const uint64_t *indexes, uint32_t n_indexes, uint64_t n_leaves, uint64_t *out, size_t cap, size_t *written);
+/* the plan of dg_tree_update: the indexes deduplicated (last occurrence wins) and sorted, then per level from the leaves' parents in
+ * [L/2, L) up to the root the sorted unique changed nodes, each with the position in the level below of its first changed child.
+ * out layout, all uint64: [K][d][T = digests hashed] [leaf index]*K [position of its last occurrence in the call]*K, then per level
+ * [n] [node id]*n [first changed child]*n */
+int dg_host_tree_plan(const uint64_t *indexes, uint32_t count, uint64_t n_leaves, uint64_t *out, size_t cap, size_t *written);
 /* MerkleTree::verify_batch (merkle.rs:154-263) as the hashing plan dg_verify executes on the device: digests live in a pool -- the proof's
  * values in slots [0, n_values), the nodes of slot i from n_values + node_counts[0..i) on, computed parents after them; ops = (left, right,
  * out) slot triples, level_start[l] .. level_start[l+1] the ops of level l; the tree is accepted iff pool[root_slot] equals the root.
