@@ -152,9 +152,8 @@ struct Context {
     TwiddleRef twiddle(int log_order, bool inverse);
     std::map<int, DevBuf> single_tables;    // full power tables w^e, e < 2^log_order (small orders only)
     const fe *single_table(int log_order);
-    std::map<int, DevBuf> single_tables_tw; // the same powers interleaved with their fe_mul_tw companions: (w^e, w^e * 2^64)
-    const fe *single_table_tw(int log_order);
     std::map<long long, DevBuf> lde_twiddles;   // per (log_n, log_blowup, first pass size): merged lane/coset twiddles of the LDE's first pass (ntt.cu)
+    std::map<long long, DevBuf> coset_roots;    // per (first pass size, log_blowup): butterfly factors of the fold-1 LDE's first pass (ntt.cu)
     const fe *roots(int log_l, bool inverse) const { return small_roots[inverse ? 1 : 0].as<fe>() + small_root_offset[log_l]; }
 };
 
@@ -219,6 +218,8 @@ void ntt_batch(Context &c, const fe *src, fe *dst, int log_n, int batch, size_t 
 // [coset c][k] = P(w_N^c * w_n^k), N = n << log_blowup, i.e. LDE index i = (k << log_blowup) + c lives at c*n + k.
 void lde_batch(Context &c, const fe *src, fe *dst, int log_n, int log_blowup, int fold, int batch, size_t src_stride, size_t dst_stride,
                unsigned coset0 = 0, unsigned ncosets = 0 /* 0 = all 2^log_blowup */);
+// bytes of the per-shape tables a fold-1 LDE of this shape would build that the context does not hold yet
+size_t lde_tables_to_add(Context &c, int log_n, int log_blowup);
 
 // ---- multi-GPU plumbing (comm.cu) -----------------------------------------------------------------------------------------
 void comm_unique_id(uint8_t out[128]);

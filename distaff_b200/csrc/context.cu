@@ -26,14 +26,6 @@ __global__ void companion_table_kernel(fe *out, const fe *in, unsigned count) {
     unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < count) out[i] = fe_tw_companion(in[i]);
 }
-// (w^e, w^e * 2^64) pairs, e < count, interleaved
-__global__ void power_pair_table_kernel(fe *out, fe step, unsigned count) {
-    unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= count) return;
-    const fe w = fe_pow_u64(step, i);
-    out[2 * i] = w;
-    out[2 * i + 1] = fe_tw_companion(w);
-}
 
 static thread_local Context *tl_ctx = nullptr;
 cudaStream_t &alloc_stream() { return ctx().stream; }
@@ -275,20 +267,6 @@ const fe *Context::single_table(int log_order) {
         power_table_kernel<<<(cnt + 127) / 128, 128, 0, stream>>>(t.as<fe>(), host_root_of_unity(log_order), cnt); launches++;
         DG_CUDA(cudaGetLastError());
         it = single_tables.emplace(log_order, std::move(t)).first;
-    }
-    return it->second.as<fe>();
-}
-
-const fe *Context::single_table_tw(int log_order) {
-    DG_REQUIRE(log_order <= 20, "single-level table too large");
-    auto it = single_tables_tw.find(log_order);
-    if (it == single_tables_tw.end()) {
-        DevBuf t;
-        t.alloc(((size_t)2 << log_order) * sizeof(fe), true);
-        const unsigned cnt = 1u << log_order;
-        power_pair_table_kernel<<<(cnt + 127) / 128, 128, 0, stream>>>(t.as<fe>(), host_root_of_unity(log_order), cnt); launches++;
-        DG_CUDA(cudaGetLastError());
-        it = single_tables_tw.emplace(log_order, std::move(t)).first;
     }
     return it->second.as<fe>();
 }

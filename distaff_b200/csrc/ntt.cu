@@ -12,7 +12,8 @@
 // segments.  Inter-pass twiddles w^(lane*k) come from a two-level power table (2 loads + 1 multiply).
 //
 // Low-degree extension does not zero-pad: evaluating P (n coefficients) on the LDE domain of size N = b*n is done as b
-// independent size-n transforms of the coset-scaled coefficients p[m] * w_N^(c*m); the result is stored coset-major
+// independent size-n transforms of the coset-scaled coefficients p[m] * w_N^(c*m) (the scaling folded into the first pass's butterflies,
+// ct_coset_regs); the result is stored coset-major
 // ([c][k] <-> LDE index b*k + c), which is the layout every later kernel (leaf hashing, constraint evaluation, FRI)
 // consumes with unit-stride reads.  This removes log2(b) of the log2(N) butterfly levels and all work on zeros.
 // The fully unrolled rounds are far larger than the 32 KB instruction cache; with the field multiplication out of line
@@ -51,6 +52,9 @@ static int pass_kind(const PassGeom &g) {
 // The other shapes were removed after this measurement.  With the butterflies through fe_mul_tw (the companions double s_tw to 2L entries:
 // 96 KiB per strided and 104 KiB per lane-major 1024-point block, still two blocks per SM) the same shape measured stage 1 at 49.4 - 49.5 ms
 // against 52.4 - 52.7 ms, four runs each, alternating, H100 80GB HBM3 at 700 W; with tw_full stored as (w, w_c) pairs as well, 51.9 ms.
+// With the coset factor folded into the fold-1 first pass's butterflies (coset_roots) as well, same card and power limit, 4 runs each,
+// alternating: stage 1 49.2 - 49.5 ms before, 50.0 ms with the folded butterflies alone, 46.0 ms with tw_full as pairs and the first pass's
+// grid ordered (vector, coset, tile), so that the vectors of a launch share each streamed segment in L2.
 static const int TILE = 4096;                    // elements per block = 64 KB
 
 static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *dst, unsigned blocks_x, unsigned by, unsigned bz) {
@@ -66,9 +70,13 @@ static void launch_pass(Context &c, int log_l, PassGeom g, const fe *src, fe *ds
     if (threads < 32) threads = 32;
     set_func_smem(c, (const void *)k, 200 * 1024);
     DG_REQUIRE(by <= 65535 && bz <= 65535, "batch too large for one launch");
-    // (folding the vector index into blockIdx.x so that all columns of a (tile, coset) share the streamed twiddles in L2 spills at the
-    //  64-register cap: rejected)
-    k<<<dim3(blocks_x, by, bz), threads, smem, c.stream>>>(src, dst, g); c.launches++;
+    if (pk_vector_x(kind)) {                      // (vector, coset, tile): see pk_vector_x
+        DG_REQUIRE(blocks_x <= 65535, "too many tiles for one launch");
+        k<<<dim3(bz, by, blocks_x), threads, smem, c.stream>>>(src, dst, g);
+    } else {
+        k<<<dim3(blocks_x, by, bz), threads, smem, c.stream>>>(src, dst, g);
+    }
+    c.launches++;
     DG_CUDA(cudaGetLastError());
 }
 
@@ -90,28 +98,73 @@ static int split_passes(int log_n, int l[3]) {
 
 struct CosetSpec { bool on; int log_blowup; int fold; unsigned coset0; };
 
-// table[c][k * R1 + lane] = w_N^(lane * (k * b + c)): the twiddle the first LDE pass applies to output k of lane `lane` on coset c.
-// It depends on the shape only (n, b, first pass size), so it is built once per shape and kept: N elements (512 MB for 2^20 x 32).
+// table[c][k * R1 + lane] = w_N^(lane * (k * b + c)) and its fe_mul_tw companion: the twiddle the first LDE pass applies to output k of
+// lane `lane` on coset c.  It depends on the shape only (n, b, first pass size), so it is built once per shape and kept: N pairs (1 GiB for
+// 2^20 x 32).
 __global__ void lde_twiddle_fill_kernel(fe *table, TwiddleRef cw, int log_n, int log_r1, int log_b) {
     const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >> (log_n + log_b)) return;
     const unsigned long long c = i >> log_n, pos = i & ((1ULL << log_n) - 1);
     const unsigned long long lane = pos & ((1ULL << log_r1) - 1), k = pos >> log_r1;
-    table[i] = tw_lookup(cw, lane * ((k << log_b) + c));
+    const fe w = tw_lookup(cw, lane * ((k << log_b) + c));
+    table[2 * i] = w;
+    table[2 * i + 1] = fe_tw_companion(w);
 }
+// Memory of a per-shape table: the stream-ordered pool's cached blocks are handed back to the driver first, so that the table gets a chunk
+// of its own.  Carved out of a cached block, a table that is kept for the life of the context would pin the rest of that block's chunk,
+// which the pool could then not release when a memory limit asks it to.
+static void alloc_table(Context &c, DevBuf &t, size_t bytes) {
+    cudaMemPool_t pool = nullptr;
+    DG_CUDA(cudaDeviceGetDefaultMemPool(&pool, c.device));
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+    DG_CUDA(cudaMemPoolTrimTo(pool, 0));
+    t.alloc(bytes, true);
+}
+
+static const int LDE_TWIDDLE_MAX_LOG = 26;        // streamed table up to 2^26 pairs (2^20 steps x 64); larger shapes use the two-level table
+static long long lde_twiddle_key(int log_n, int log_b, int l0) { return ((long long)log_n << 16) | (log_b << 8) | l0; }
 static const fe *lde_twiddle_table(Context &c, int log_n, int log_b, int l0) {
-    const size_t bytes = ((size_t)16 << (log_n + log_b));
-    if (bytes > ((size_t)1 << 30)) return nullptr;         // over 1 GiB (2^22 steps x 32): the pass uses the two-level table instead
-    const long long key = ((long long)log_n << 16) | (log_b << 8) | l0;
-    auto it = c.lde_twiddles.find(key);
+    if (log_n + log_b > LDE_TWIDDLE_MAX_LOG) return nullptr;
+    auto it = c.lde_twiddles.find(lde_twiddle_key(log_n, log_b, l0));
     if (it == c.lde_twiddles.end()) {
         DevBuf t;
-        t.alloc(bytes, true);
+        alloc_table(c, t, (size_t)32 << (log_n + log_b));
         const unsigned long long cnt = 1ULL << (log_n + log_b);
         lde_twiddle_fill_kernel<<<(unsigned)((cnt + 255) / 256), 256, 0, c.stream>>>(t.as<fe>(), c.twiddle(log_n + log_b, false), log_n, log_n - l0, log_b);
         c.launches++;
         DG_CUDA(cudaGetLastError());
-        it = c.lde_twiddles.emplace(key, std::move(t)).first;
+        it = c.lde_twiddles.emplace(lde_twiddle_key(log_n, log_b, l0), std::move(t)).first;
+    }
+    return it->second.as<fe>();
+}
+
+// The butterfly factors of the fold-1 coset first pass (ct_coset_regs, ntt_pass.cuh) for every coset c < b of an L-point pass:
+// rho_{st,r}(c) = (t_c w_L^rev_st(r))^(L >> (st+1)) at [c][2^st - 1 + r], companions at [c][L + 2^st - 1 + r], entry L - 1 unused.
+// t_c = w_N^(c R1) = w_(L b)^c and w_L = w_(L b)^b, so every factor is a power of w_(L b).  2L entries per coset (1 MiB at L = 1024, b = 32).
+__global__ void coset_roots_fill_kernel(fe *table, fe w, int log_l, int log_b) {
+    const unsigned i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >> (log_l + log_b)) return;
+    const unsigned c = i >> log_l, h = (i & ((1u << log_l) - 1)) + 1;       // heap index + 1 = 2^st + r
+    fe *row = table + ((size_t)c << (log_l + 1));
+    const int st = 31 - __clz(h);
+    if (st == log_l) { row[h - 1] = row[(1u << log_l) + h - 1] = fe_make(0, 0); return; }
+    const unsigned r = h - (1u << st), rev = st ? __brev(r) >> (32 - st) : 0;
+    const unsigned long long e = ((unsigned long long)c + ((unsigned long long)rev << log_b)) << (log_l - st - 1);
+    const fe v = fe_pow_u64(w, e & ((1ULL << (log_l + log_b)) - 1));
+    row[h - 1] = v;
+    row[(1u << log_l) + h - 1] = fe_tw_companion(v);
+}
+static long long coset_roots_key(int log_l, int log_b) { return ((long long)log_l << 8) | log_b; }
+static const fe *coset_roots(Context &c, int log_l, int log_b) {
+    auto it = c.coset_roots.find(coset_roots_key(log_l, log_b));
+    if (it == c.coset_roots.end()) {
+        DevBuf t;
+        alloc_table(c, t, (size_t)32 << (log_l + log_b));
+        const unsigned cnt = 1u << (log_l + log_b);
+        coset_roots_fill_kernel<<<(cnt + 255) / 256, 256, 0, c.stream>>>(t.as<fe>(), host_root_of_unity(log_l + log_b), log_l, log_b);
+        c.launches++;
+        DG_CUDA(cudaGetLastError());
+        it = c.coset_roots.emplace(coset_roots_key(log_l, log_b), std::move(t)).first;
     }
     return it->second.as<fe>();
 }
@@ -136,11 +189,8 @@ static void run_transform(Context &c, const fe *src, fe *dst, int log_n, bool in
         base.log_blowup = cs.log_blowup;
         base.coset0 = cs.coset0;
         if (cs.fold == 1) {
-            // order of w_N^in_point where in_point = n / N1 (first pass) : N / in_point = N1 << log_blowup
-            const int log_order = l[0] + cs.log_blowup;
             base.coset_fast = 1;
-            base.cw_point = c.single_table_tw(log_order);
-            base.cw_point_mask = (1u << log_order) - 1u;
+            base.coset_roots = coset_roots(c, l[0], cs.log_blowup);
         }
     }
 
@@ -206,6 +256,22 @@ static void run_transform(Context &c, const fe *src, fe *dst, int log_n, bool in
         g.roots = c.roots(ll, inverse);
         launch_pass(c, ll, g, tmp, dst, (unsigned)(g.num_tiles * N2), by, bz);
     }
+}
+
+// first-pass size of an n-point transform
+static int first_pass_log(int log_n) {
+    int l[3];
+    split_passes(log_n, l);
+    return l[0];
+}
+
+size_t lde_tables_to_add(Context &c, int log_n, int log_b) {
+    const int l0 = first_pass_log(log_n);
+    size_t add = 0;
+    if (!c.coset_roots.count(coset_roots_key(l0, log_b))) add += (size_t)32 << (l0 + log_b);
+    if (l0 < log_n && log_n + log_b <= LDE_TWIDDLE_MAX_LOG && !c.lde_twiddles.count(lde_twiddle_key(log_n, log_b, l0)))
+        add += (size_t)32 << (log_n + log_b);
+    return add;
 }
 
 void ntt_batch(Context &c, const fe *src, fe *dst, int log_n, int batch, size_t src_stride, size_t dst_stride, bool inverse) {

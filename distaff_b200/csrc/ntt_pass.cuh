@@ -9,21 +9,24 @@ namespace dg {
 // (and its registers are allocated for that path alone).  launch_pass (ntt.cu) picks the kind from the PassGeom flags.
 enum PassKind {
     PK_TW,              // first / middle pass: output k of lane l times tw^(l*k)
-    PK_COSET_TWFULL,    // first pass of a fold-1 LDE: input times cw_point, output times the streamed tw_full table
+    PK_COSET_TWFULL,    // first pass of a fold-1 LDE: coset factor folded into the butterflies, output times the streamed tw_full pairs
     PK_COSET_TW,        // the same, output factor from the two-level table cw (tw_full not built for this shape)
     PK_FOLD_TW,         // first pass of a fold > 1 LDE: Horner fold of the input, output times tw^(l*k)
     PK_LAST,            // last or only pass (lane-major), plain output
     PK_LAST_SCALE,      // last or only pass of an inverse transform: output times n^-1
-    PK_COSET_ONE,       // only pass of a fold-1 LDE: input times cw_point
+    PK_COSET_ONE,       // only pass of a fold-1 LDE: coset factor folded into the butterflies
     PK_FOLD_ONE,        // only pass of a fold > 1 LDE: Horner fold of the input
     PK_COUNT
 };
 __host__ __device__ constexpr bool pk_lane_major(int k) { return k >= PK_LAST; }
 __host__ __device__ constexpr bool pk_coset_in(int k) { return k == PK_COSET_TWFULL || k == PK_COSET_TW || k == PK_COSET_ONE; }
 __host__ __device__ constexpr bool pk_fold_in(int k) { return k == PK_FOLD_TW || k == PK_FOLD_ONE; }
-// butterflies through fe_mul_tw with the stage roots' companions.  The kinds whose output factor comes from the two-level table keep fe_mul:
-// with the companions they spill at the 64-register cap.
-__host__ __device__ constexpr bool pk_mul_tw(int k) { return k != PK_TW && k != PK_COSET_TW && k != PK_FOLD_TW; }
+// butterflies through fe_mul_tw with the stage roots' companions.  The plain and fold first passes, whose output factor comes from the
+// two-level table, keep fe_mul: with the companions they spill at the 64-register cap.
+__host__ __device__ constexpr bool pk_mul_tw(int k) { return k != PK_TW && k != PK_FOLD_TW; }
+// the grid of the streamed-table first pass is (vector, coset, tile): the vectors of a launch read each (coset, tile) segment of tw_full
+// together, from L2
+__host__ __device__ constexpr bool pk_vector_x(int k) { return k == PK_COSET_TWFULL; }
 
 struct PassGeom {
     int log_t;                          // lanes per block (power of two)
@@ -36,16 +39,17 @@ struct PassGeom {
     int tw_on;                          // multiply output k of lane (tile*T+lane) by tw^((tile*T+lane)*k)
     int has_scale;
     int coset_on;                       // input transform of the LDE: sum_f src[j + f*fold_stride] * cw^(c*(j + f*fold_stride))
-    int coset_fast;                     // fold == 1: input factor from a single-level table, lane factor merged into the output twiddle
+    int coset_fast;                     // fold == 1: coset factor in the butterflies (coset_roots), lane factor merged into the output twiddle
     TwiddleRef tw;
     fe scale;
     int fold;
     long long fold_stride;
     TwiddleRef cw;
-    const fe *cw_point;                 // (cw_point[2e], cw_point[2e + 1]) = ((w_N^in_point)^e, its fe_mul_tw companion), e < cw_point_mask + 1
-    unsigned cw_point_mask;
-    const fe *tw_full;                  // coset_fast: tw_full[coset][k * out_point + lane] = cw^(lane * (k * blowup + coset)), or null
-    long long tw_full_stride;           // elements per coset (= transform size n)
+    const fe *coset_roots;              // coset_fast: 2L entries per coset (absolute index), the butterfly factors of ct_coset_regs, then
+                                        // their fe_mul_tw companions
+    const fe *tw_full;                  // coset_fast: tw_full[coset][k * out_point + lane] = cw^(lane * (k * blowup + coset)) and its companion,
+                                        // (w, w_c) pairs; or null
+    long long tw_full_stride;           // pairs per coset (= transform size n)
     int log_blowup;
     unsigned coset0;                    // first coset handled by this launch (blockIdx.y = coset - coset0)
     const fe *roots;                    // per-stage twiddle tables of the L-point transform: W_st[j] = w_L^(j << st), back to back (L entries),
@@ -113,6 +117,30 @@ __device__ __forceinline__ void dif_regs(fe *x, const fe *s_tw, int g_lo) {
     }
 }
 
+// The same data flow for the fold-1 coset kinds, as Cooley-Tukey butterflies (a + rho b, a - rho b) that evaluate sum_j x_j (t w_L^k)^j
+// without scaling x_j by t^j first (t = the coset factor of the pass's points).  Stage st, block r of L >> st points multiplies by
+// rho_{st,r} = (t w_L^rev_st(r))^(L >> (st+1)), kept in heap order at s_tw[2^st - 1 + r] (companion L entries on); position q ends up
+// holding the transform at bitrev(q), as after dif_regs.  The block index comes from g_hi and the element index, so the threads of a warp
+// mostly read the same factor.  tools/model_coset_ct.py restates it.
+template <int LOG_L, int S0, int RHO>
+__device__ __forceinline__ void ct_coset_regs(fe *x, const fe *s_tw, int g_hi) {
+    constexpr int L = 1 << LOG_L, R = 1 << RHO;
+#pragma unroll
+    for (int u = 0; u < RHO; u++) {
+        const int hr = R >> (u + 1);
+        const fe *W = s_tw + (1 << (S0 + u)) - 1 + (g_hi << u);
+#pragma unroll
+        for (int i = 0; i < R; i++) {
+            if ((i & hr) == 0) {
+                const int e = i >> (RHO - u);
+                const fe a = x[i], b = ntt_mul_tw(x[i + hr], W[e], W[L + e]);
+                x[i] = fe_add(a, b);
+                x[i + hr] = fe_sub(a, b);
+            }
+        }
+    }
+}
+
 template <int LOG_L, bool LANE_MAJOR>
 __device__ __forceinline__ int sidx(int pos, int t, int T) {
     constexpr int L = 1 << LOG_L;
@@ -149,12 +177,7 @@ __device__ __forceinline__ void ntt_round(const fe *__restrict__ src, fe *__rest
             const int pos = gbase + (m << LOG_SP);
             if (FIRST) {
                 const long long j = in_base + (long long)t * g.in_lane + (long long)pos * g.in_point;
-                if (pk_coset_in(KIND)) {
-                    // p[j] * w_N^(c*pos*in_point); the lane part w_N^(c*lane) rides on the output twiddle
-                    const fe *cw = g.cw_point + 2 * (((g.coset0 + (unsigned)blockIdx.y) * (unsigned)pos) & g.cw_point_mask);
-                    // fe_mul_tw only in the one-pass kind: next to the tw_full product's fe_mul (and in PK_COSET_TW) it spills
-                    x[m] = KIND == PK_COSET_ONE ? ntt_mul_tw(src[j], cw[0], cw[1]) : ntt_mul(src[j], cw[0]);
-                } else if (pk_fold_in(KIND)) {
+                if (pk_fold_in(KIND)) {
                     // sum_f src[j + f n] w_N^(c (j + f n)) = w_N^(c j) * Horner_f(src[j + f n]; u),  u = w_N^(c n) (constant per coset)
                     const unsigned long long c = g.coset0 + blockIdx.y;
                     const fe u = tw_lookup(g.cw, c * (unsigned long long)g.fold_stride);
@@ -168,18 +191,20 @@ __device__ __forceinline__ void ntt_round(const fe *__restrict__ src, fe *__rest
                 x[m] = s_data[sidx<LOG_L, LANE_MAJOR>(pos, t, T)];
             }
         }
-        dif_regs<LOG_L, S0, RHO, pk_mul_tw(KIND)>(x, s_tw, g_lo);
+        if constexpr (pk_coset_in(KIND)) ct_coset_regs<LOG_L, S0, RHO>(x, s_tw, g_hi);
+        else dif_regs<LOG_L, S0, RHO, pk_mul_tw(KIND)>(x, s_tw, g_lo);
 #pragma unroll
         for (int m = 0; m < R; m++) {
             const int pos = gbase + (m << LOG_SP);
             if (LAST) {                        // position q holds X[bitrev(q)]
                 const unsigned k = __brev((unsigned)pos) >> (32 - LOG_L);
                 fe v = x[m];
-                // streamed table in the layout of the output: one 16-byte load instead of two loads and a multiplication.  It keeps fe_mul:
-                // every column streams the whole table again, and companions beside it would double that traffic
-                if (KIND == PK_COSET_TWFULL)
-                    v = ntt_mul(v, g.tw_full[(long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)(tile * T + t) * g.out_lane + (long long)k * g.out_point]);
-                else if (KIND == PK_COSET_TW)
+                // streamed table in the layout of the output: one 32-byte load instead of two loads and a multiplication
+                if (KIND == PK_COSET_TWFULL) {
+                    const fe *w = g.tw_full + 2 * ((long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)(tile * T + t) * g.out_lane +
+                                                   (long long)k * g.out_point);
+                    v = ntt_mul_tw(v, w[0], w[1]);
+                } else if (KIND == PK_COSET_TW)
                     v = ntt_mul(v, tw_lookup(g.cw, (unsigned long long)(tile * T + t) * (((unsigned long long)k << g.log_blowup) + g.coset0 + blockIdx.y)));
                 else if (KIND == PK_TW || KIND == PK_FOLD_TW)
                     v = ntt_mul(v, tw_lookup(g.tw, (unsigned long long)(tile * T + t) * k));
@@ -211,17 +236,19 @@ __global__ void __launch_bounds__(BT, MINB) ntt_pass_kernel(const fe *__restrict
     fe *s_tw = reinterpret_cast<fe *>(smem_raw);          // 2L entries: per-stage tables back to back, then their companions
     fe *s_data = s_tw + 2 * L;
     const int T = 1 << g.log_t;
-    const unsigned tile = blockIdx.x % g.num_tiles, outer = blockIdx.x / g.num_tiles;
+    const unsigned bx = pk_vector_x(KIND) ? blockIdx.z : blockIdx.x, vec = pk_vector_x(KIND) ? blockIdx.x : blockIdx.z;
+    const unsigned tile = bx % g.num_tiles, outer = bx / g.num_tiles;
     const long long in_base = (long long)outer * g.in_outer + (long long)tile * T * g.in_lane;   // index inside the vector
-    src += (long long)blockIdx.y * g.in_batch_y + (long long)blockIdx.z * g.in_batch_z;
-    dst += (long long)blockIdx.y * g.out_batch_y + (long long)blockIdx.z * g.out_batch_z + (long long)outer * g.out_outer +
+    src += (long long)blockIdx.y * g.in_batch_y + (long long)vec * g.in_batch_z;
+    dst += (long long)blockIdx.y * g.out_batch_y + (long long)vec * g.out_batch_z + (long long)outer * g.out_outer +
            (long long)tile * T * g.out_lane;
-    for (int i = threadIdx.x; i < 2 * L; i += blockDim.x) s_tw[i] = g.roots[i];
+    const fe *roots = pk_coset_in(KIND) ? g.coset_roots + (long long)(g.coset0 + blockIdx.y) * (2 * L) : g.roots;
+    for (int i = threadIdx.x; i < 2 * L; i += blockDim.x) s_tw[i] = roots[i];
     if (KIND == PK_COSET_TWFULL) {
-        // the streamed twiddles are consumed in the last round: start pulling this block's T*16-byte segments (one per output k) into L2 now
-        const fe *tb = g.tw_full + (long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)tile * T * g.out_lane;
+        // the streamed twiddles are consumed in the last round: start pulling this block's T*32-byte segments (one per output k) into L2 now
+        const fe *tb = g.tw_full + 2 * ((long long)(g.coset0 + blockIdx.y) * g.tw_full_stride + (long long)tile * T * g.out_lane);
         for (int k = threadIdx.x; k < L; k += blockDim.x)
-            asm volatile("prefetch.global.L2 [%0];" :: "l"(tb + (long long)k * g.out_point));
+            asm volatile("prefetch.global.L2 [%0];" :: "l"(tb + 2 * (long long)k * g.out_point));
     }
     __syncthreads();
     ntt_rounds<LOG_L, RMAX, 0, KIND>(src, dst, s_data, s_tw, g, tile, in_base);

@@ -1072,17 +1072,13 @@ long long batch_group_cap(long long k) {
 }
 
 // Transform scratch and tables a prove call adds outside the arena (persistent, from the pool): the multi-pass LDE of a coset chunk
-// (<= 4 GiB), the other multi-pass transforms (<= 1 GiB) and the merged first-pass twiddles of the trace LDE (<= 1 GiB), less what the
+// (<= 4 GiB), the other multi-pass transforms (<= 1 GiB) and the first-pass tables of the trace LDE (lde_tables_to_add), less what the
 // library holds already
 static size_t prove_scratch(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t chunk, long long k) {
     const size_t four = (size_t)4 << 30, one = (size_t)1 << 30;
     const size_t ntt = std::max(std::min(four, (size_t)(16 * n * chunk * w * k)), std::min(one, (size_t)(16 * n * b * k)));
     size_t add = ntt > c.ntt_tmp.bytes ? ntt - c.ntt_tmp.bytes : 0;
-    const size_t table = (size_t)16 * n * b;
-    bool have = false;
-    for (auto &t : c.lde_twiddles) have |= (t.first >> 8) == (((long long)ceil_log2(n) << 8) | ceil_log2(b));
-    if (table <= one && !have) add += table;
-    return add;
+    return add + lde_tables_to_add(c, ceil_log2(n), ceil_log2(b));
 }
 
 ProvePlan plan_prove(Context &c, uint32_t w, uint64_t n, uint32_t b, uint32_t count) {
