@@ -136,18 +136,21 @@ def _batch_io(public_inputs_list, outputs_list):
     return ins + outs, arrays
 
 
+def _messages(status, error=backend.DgError):
+    """per entry of the thread's last batched call: None when it succeeded, else error(code, the library's message for it)"""
+    msg = ctypes.create_string_buffer(512)
+    out = []
+    for i, rc in enumerate(status):
+        if rc != 0:
+            backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
+        out.append(None if rc == 0 else error(rc, msg.value.decode(errors="replace")))
+    return out
+
+
 def _collect_batch(handles, status, stats):
     """one entry per trace: a StarkProof, or the DgError of a trace that failed with the library's message for it (stats: the
     whole batch)"""
-    out = []
-    msg = ctypes.create_string_buffer(512)
-    for i, (h, rc) in enumerate(zip(handles, status)):
-        if rc == 0:
-            out.append(_collect(h, stats))
-        else:
-            backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
-            out.append(backend.DgError(rc, msg.value.decode(errors="replace")))
-    return out
+    return [_collect(h, stats) if e is None else e for h, e in zip(handles, _messages(status))]
 
 
 def prove_batch(traces, options=None):
@@ -287,15 +290,7 @@ def verify_batch(items, stats=None):
                                                 nout, (backend.vp * k)(*[ctypes.cast(ctypes.c_char_p(d), backend.vp) for d in data]),
                                                 (ctypes.c_size_t * k)(*[len(d) for d in data]), status, ctypes.byref(st)))
     del keep
-    out = []
-    msg = ctypes.create_string_buffer(512)
-    for i, rc in enumerate(status):
-        if rc == 0:
-            out.append(None)
-            continue
-        backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
-        text = msg.value.decode(errors="replace")
-        out.append(text if rc == -6 else backend.DgError(rc, text))
+    out = _messages(status, lambda rc, text: text if rc == -6 else backend.DgError(rc, text))
     if stats is not None:
         stats.update(total_ms=float(st.total_ms), kernel_launches=int(st.kernel_launches), groups=int(st.groups))
     return out
@@ -477,33 +472,70 @@ class ProgramInputs:
         self.secret_b = [int(x) for x in secret_b]
 
 
-def _encoded(program):
-    return hostvm.compile_program(program) if isinstance(program, str) else program
-
-
-def _execution_args(program, inputs):
-    """the dg_program_t and dg_program_inputs_t array of a call (plus the arrays they point into, to keep alive)"""
-    prog = _encoded(program)
-    cprog = prog.c_struct()
-    keep = [prog, cprog]
-    arr = (backend.DgProgramInputs * max(len(inputs), 1))()
+def _programs_args(jobs):
+    """the dg_program_t table, program_of, dg_program_inputs_t array and num_outputs of a call (plus what they point into)"""
+    programs, program_of, inputs, num_outputs = pack_jobs(jobs)
+    k = len(inputs)
+    cprogs = (backend.DgProgram * len(programs))(*[p.c_struct() for p in programs])
+    arr = (backend.DgProgramInputs * k)()
+    keep = [programs, cprogs]
     for i, x in enumerate(inputs):
         vals = [felt.from_ints(v) for v in (x.public, x.secret_a, x.secret_b)]
         keep += vals
         arr[i] = backend.DgProgramInputs(vals[0].ctypes.data, len(vals[0]), vals[1].ctypes.data, len(vals[1]), vals[2].ctypes.data, len(vals[2]))
-    return prog, cprog, arr, keep
+    return programs, cprogs, (backend.u32 * k)(*program_of), arr, num_outputs, keep
 
 
-def _messages(status):
-    msg = ctypes.create_string_buffer(512)
-    out = []
-    for i, rc in enumerate(status):
-        if rc == 0:
-            out.append(None)
-            continue
-        backend.check(backend.lib().dg_batch_message(i, msg, len(msg)))
-        out.append(backend.DgError(rc, msg.value.decode(errors="replace")))
-    return out
+def _execution_args(program, inputs):
+    """the one-program case of _programs_args: the hostvm.Program, its dg_program_t, the dg_program_inputs_t array (plus what they point
+    into, to keep alive)"""
+    (prog,), cprogs, _, arr, _, keep = _programs_args([(program, x) for x in inputs])
+    return prog, cprogs[0], arr, keep
+
+
+def _fields(st, into=None):
+    """a ctypes structure as a dict, also written into `into` when given: *_ms fields as floats, other numbers as ints, a nested
+    structure as a dict"""
+    d = {}
+    for f, _ in st._fields_:
+        v = getattr(st, f)
+        d[f] = _fields(v) if isinstance(v, ctypes.Structure) else (float if f.endswith("_ms") else int)(v)
+    if into is not None:
+        into.update(d)
+    return d
+
+
+def _traces(call, jobs, programs, program_of, num_outputs):
+    """The trace calls: call(info, registers_out, status) once without registers to size the buffers, then with one buffer per execution
+    that call let through.  Returns a list in job order: a hostvm.ExecutionTrace with num_outputs[i] outputs, or the DgError of an
+    execution that failed."""
+    k = len(jobs)
+    info = (backend.DgExecutionInfo * k)()
+    status = (ctypes.c_int * k)()
+    backend.check(call(info, None, status))
+    regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
+    backend.check(call(info, (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs]), status))
+    result = _messages(status)
+    for i, job in enumerate(jobs):
+        if result[i] is None:
+            sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
+            last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+            result[i] = hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
+                                              list(job[1].public), last[:num_outputs[i]])
+    return result
+
+
+def _proofs(call, num_outputs, per=8):
+    """The execute calls: call(proofs_out, outputs16, status, prove_stats) with room for `per` output elements per execution.  Returns a
+    list in execution order: (outputs, StarkProof), or the DgError of an execution that failed."""
+    k = len(num_outputs)
+    handles = (backend.vp * k)()
+    outputs = np.zeros((k, per, 2), dtype=np.uint64)
+    status = (ctypes.c_int * k)()
+    pst = backend.DgStats()
+    backend.check(call(handles, outputs.ctypes.data, status, ctypes.byref(pst)))
+    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs[i]]) if num_outputs[i] else [], _collect(handles[i], pst))
+            for i, e in enumerate(_messages(status))]
 
 
 def trace_shapes(program, inputs, max_steps=MAX_STEPS):
@@ -517,9 +549,7 @@ def trace_shapes(program, inputs, max_steps=MAX_STEPS):
     info = (backend.DgExecutionInfo * k)()
     status = (ctypes.c_int * k)()
     backend.check(backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, None, status))
-    errors = _messages(list(status))
-    del keep
-    return [e if e is not None else {f: int(getattr(info[i], f)) for f, _ in backend.DgExecutionInfo._fields_} for i, e in enumerate(errors)]
+    return [e if e is not None else _fields(info[i]) for i, e in enumerate(_messages(status))]
 
 
 def trace_batch(program, inputs, max_steps=MAX_STEPS, num_outputs=1):
@@ -527,28 +557,13 @@ def trace_batch(program, inputs, max_steps=MAX_STEPS, num_outputs=1):
     execution.  Returns a list in input order: a hostvm.ExecutionTrace (what hostvm.execute gives for the same inputs, byte for byte)
     or the DgError of an execution that failed, with the host VM's message ("execution exceeds N steps" past max_steps).  The buffers
     are sized by a shapes-only call first, so the shape pass runs twice."""
-    inputs = list(inputs)
-    if not inputs:
+    jobs = [(program, x) for x in inputs]
+    if not jobs:
         return []
-    prog, cprog, arr, keep = _execution_args(program, inputs)
-    k = len(inputs)
-    shapes = trace_shapes(prog, inputs, max_steps)
-    regs = [None if isinstance(s, backend.DgError) else np.empty((s["width"], s["length"], 2), dtype=np.uint64) for s in shapes]
-    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
-    info = (backend.DgExecutionInfo * k)()
-    status = (ctypes.c_int * k)()
-    backend.check(backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, outs, status))
-    errors = _messages(list(status))
-    del keep
-    result = []
-    for i, (x, e) in enumerate(zip(inputs, errors)):
-        if e is not None:
-            result.append(e)
-            continue
-        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
-        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
-        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, prog.hash, list(x.public), last[:num_outputs]))
-    return result
+    prog, cprog, arr, keep = _execution_args(program, [x for _, x in jobs])
+    k = len(jobs)
+    return _traces(lambda info, outs, status: backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, outs, status),
+                   jobs, [prog], [0] * k, [num_outputs] * k)
 
 
 def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_STEPS):
@@ -557,30 +572,17 @@ def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_ST
     for the same inputs, byte for byte -- or the DgError of an execution that failed (in the VM or in the prover)."""
     options = options or ProofOptions()
     assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
-    inputs = list(inputs)
-    if not inputs:
+    jobs = [(program, x) for x in inputs]
+    if not jobs:
         return []
-    _, cprog, arr, keep = _execution_args(program, inputs)
-    k = len(inputs)
-    opt = options._c()
-    handles = (backend.vp * k)()
-    outputs = np.zeros((k, max(num_outputs, 1), 2), dtype=np.uint64)
-    status = (ctypes.c_int * k)()
-    stats = backend.DgStats()
-    backend.check(backend.lib().dg_execute_batch(ctypes.byref(cprog), k, arr, num_outputs, int(max_steps), ctypes.byref(opt), handles,
-                                                outputs.ctypes.data, status, ctypes.byref(stats)))
-    errors = _messages(list(status))
-    del keep
-    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs]) if num_outputs else [], _collect(handles[i], stats))
-            for i, e in enumerate(errors)]
+    _, cprog, arr, keep = _execution_args(program, [x for _, x in jobs])
+    k, opt = len(jobs), options._c()
+    return _proofs(lambda handles, outputs16, status, pst: backend.lib().dg_execute_batch(
+        ctypes.byref(cprog), k, arr, num_outputs, int(max_steps), ctypes.byref(opt), handles, outputs16, status, pst),
+        [num_outputs] * k, max(num_outputs, 1))
 
 
 # ---- one long execution, split across GPU threads ------------------------------------------------------------------------------------
-def _one_stats(stats, st):
-    if stats is not None:
-        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgTraceOneStats._fields_})
-
-
 def trace_one(program, inputs=None, max_steps=MAX_STEPS, num_outputs=1, segment_steps=0, stats=None):
     """processor::execute of one program (a hostvm.Program or assembly source) for one ProgramInputs on the GPU, split across threads
     (dg_trace_one): the sponge from a per-program table, one sequential pass that records checkpoints, and one thread per segment writing
@@ -588,22 +590,16 @@ def trace_one(program, inputs=None, max_steps=MAX_STEPS, num_outputs=1, segment_
     the host VM's message.  segment_steps: 0 (the library chooses) or a power of two >= 16.  The buffer is sized by a call without
     registers first, so the table and the sequential pass run twice.  A dict passed as `stats` receives the full call's figures."""
     assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
-    x = inputs or ProgramInputs()
-    prog, cprog, arr, keep = _execution_args(program, [x])
-    L, info, st = backend.lib(), backend.DgExecutionInfo(), backend.DgTraceOneStats()
+    jobs = [(program, inputs or ProgramInputs())]
+    prog, cprog, arr, keep = _execution_args(program, [jobs[0][1]])
+    st = backend.DgTraceOneStats()
 
-    def call(out):
-        rc = L.dg_trace_one(ctypes.byref(cprog), arr, int(max_steps), int(segment_steps), ctypes.byref(info), out, ctypes.byref(st))
-        _one_stats(stats, st)
-        backend.check(rc)
-
-    call(None)
-    regs = np.empty((info.width, info.length, 2), dtype=np.uint64)
-    call(regs.ctypes.data)
-    del keep
-    sd, start, n = info.stack_depth, 15 + info.ctx_depth + info.loop_depth, info.length
-    last = [felt.to_ints(regs[start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
-    return hostvm.ExecutionTrace(regs, info.ctx_depth, info.loop_depth, sd, prog.hash, list(x.public), last[:num_outputs])
+    def call(info, outs, status):
+        rc = backend.lib().dg_trace_one(ctypes.byref(cprog), arr, int(max_steps), int(segment_steps), info, None if outs is None else outs[0],
+                                        ctypes.byref(st))
+        _fields(st, stats)
+        return rc
+    return _traces(call, jobs, [prog], [0], [num_outputs])[0]
 
 
 def execute_one(program, inputs=None, num_outputs=1, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
@@ -613,16 +609,14 @@ def execute_one(program, inputs=None, num_outputs=1, options=None, max_steps=MAX
     options = options or ProofOptions()
     assert 0 <= num_outputs <= 8, "cannot have more than 8 outputs"
     _, cprog, arr, keep = _execution_args(program, [inputs or ProgramInputs()])
-    opt = options._c()
-    handle = backend.vp()
-    outputs = np.zeros((max(num_outputs, 1), 2), dtype=np.uint64)
-    pst, st = backend.DgStats(), backend.DgTraceOneStats()
-    rc = backend.lib().dg_execute_one(ctypes.byref(cprog), arr, num_outputs, int(max_steps), int(segment_steps), ctypes.byref(opt),
-                                      ctypes.byref(handle), outputs.ctypes.data, None, ctypes.byref(pst), ctypes.byref(st))
-    del keep
-    _one_stats(stats, st)
-    backend.check(rc)
-    return (felt.to_ints(outputs[:num_outputs]) if num_outputs else []), _collect(handle.value, pst)
+    opt, st = options._c(), backend.DgTraceOneStats()
+
+    def call(handles, outputs16, status, pst):
+        rc = backend.lib().dg_execute_one(ctypes.byref(cprog), arr, num_outputs, int(max_steps), int(segment_steps), ctypes.byref(opt), handles,
+                                          outputs16, None, pst, ctypes.byref(st))
+        _fields(st, stats)
+        return rc
+    return _proofs(call, [num_outputs])[0]
 
 
 # ---- many programs, many inputs, executed on the GPU in one call ----------------------------------------------------------------------
@@ -651,23 +645,33 @@ def pack_jobs(jobs, compile=None):
     return programs, program_of, inputs, num_outputs
 
 
-def _programs_args(jobs):
-    """the dg_program_t table, program_of, dg_program_inputs_t array and num_outputs of a call (plus what they point into)"""
-    programs, program_of, inputs, num_outputs = pack_jobs(jobs)
-    k = len(inputs)
-    cprogs = (backend.DgProgram * len(programs))(*[p.c_struct() for p in programs])
-    arr = (backend.DgProgramInputs * k)()
-    keep = [programs, cprogs]
-    for i, x in enumerate(inputs):
-        vals = [felt.from_ints(v) for v in (x.public, x.secret_a, x.secret_b)]
-        keep += vals
-        arr[i] = backend.DgProgramInputs(vals[0].ctypes.data, len(vals[0]), vals[1].ctypes.data, len(vals[1]), vals[2].ctypes.data, len(vals[2]))
-    return programs, cprogs, (backend.u32 * k)(*program_of), arr, num_outputs, keep
+def _trace_jobs(entry, jobs, st, stats, *args):
+    """trace_programs / trace_many: the C entry named `entry` (programs, n_programs, count, program_of, inputs, *args, info, registers_out,
+    status, st) through _traces, its stats structure st into the dict `stats`"""
+    jobs = list(jobs)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    fn = getattr(backend.lib(), entry)
+    result = _traces(lambda info, outs, status: fn(cprogs, len(programs), len(jobs), program_of, arr, *args, info, outs, status, ctypes.byref(st)),
+                     jobs, programs, program_of, num_outputs)
+    _fields(st, stats)
+    return result
 
 
-def _vm_stats(stats, st):
-    if stats is not None:
-        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgExecutionStats._fields_})
+def _execute_jobs(entry, jobs, options, st, stats, *args):
+    """execute_programs / execute_many: the C entry named `entry` (programs, n_programs, count, program_of, inputs, num_outputs, *args,
+    options, proofs_out, outputs16, status, prove_stats, st) through _proofs, its stats structure st into the dict `stats`"""
+    opt = (options or ProofOptions())._c()
+    jobs = list(jobs)
+    if not jobs:
+        return []
+    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
+    k, fn = len(jobs), getattr(backend.lib(), entry)
+    result = _proofs(lambda handles, outputs16, status, pst: fn(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), *args,
+                                                                ctypes.byref(opt), handles, outputs16, status, pst, ctypes.byref(st)), num_outputs)
+    _fields(st, stats)
+    return result
 
 
 def trace_programs(jobs, max_steps=MAX_STEPS, stats=None):
@@ -676,31 +680,7 @@ def trace_programs(jobs, max_steps=MAX_STEPS, stats=None):
     job's num_outputs outputs, default 1) or the DgError of an execution that failed.  A dict passed as `stats` receives the VM passes'
     figures (shape_launches, write_launches, waves, prove_groups, lanes, shape_ms, write_ms) of the call that writes the traces; a
     shapes-only call sizes the buffers first."""
-    jobs = list(jobs)
-    if not jobs:
-        return []
-    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
-    k, L = len(jobs), backend.lib()
-    info = (backend.DgExecutionInfo * k)()
-    status = (ctypes.c_int * k)()
-    st = backend.DgExecutionStats()
-    backend.check(L.dg_trace_programs(cprogs, len(programs), k, program_of, arr, int(max_steps), info, None, status, ctypes.byref(st)))
-    regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
-    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
-    backend.check(L.dg_trace_programs(cprogs, len(programs), k, program_of, arr, int(max_steps), info, outs, status, ctypes.byref(st)))
-    errors = _messages(list(status))
-    _vm_stats(stats, st)
-    result = []
-    for i, (job, e) in enumerate(zip(jobs, errors)):
-        if e is not None:
-            result.append(e)
-            continue
-        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
-        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
-        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
-                                            list(job[1].public), last[:num_outputs[i]]))
-    del keep
-    return result
+    return _trace_jobs("dg_trace_programs", jobs, backend.DgExecutionStats(), stats, int(max_steps))
 
 
 def execute_programs(jobs, options=None, max_steps=MAX_STEPS, stats=None):
@@ -708,35 +688,10 @@ def execute_programs(jobs, options=None, max_steps=MAX_STEPS, stats=None):
     trace shape's traces are proven together, whichever programs they came from, in the device memory they were written to.  Returns a
     list in job order: (outputs, StarkProof) -- what execute_batch of that program alone returns, byte for byte -- or the DgError of an
     execution that failed.  `stats` as in trace_programs, prove_groups included."""
-    options = options or ProofOptions()
-    jobs = list(jobs)
-    if not jobs:
-        return []
-    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
-    k = len(jobs)
-    opt = options._c()
-    handles = (backend.vp * k)()
-    outputs = np.zeros((k, 8, 2), dtype=np.uint64)
-    status = (ctypes.c_int * k)()
-    pst, st = backend.DgStats(), backend.DgExecutionStats()
-    backend.check(backend.lib().dg_execute_programs(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), int(max_steps),
-                                                   ctypes.byref(opt), handles, outputs.ctypes.data, status, ctypes.byref(pst), ctypes.byref(st)))
-    errors = _messages(list(status))
-    _vm_stats(stats, st)
-    del keep
-    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs[i]]) if num_outputs[i] else [], _collect(handles[i], pst))
-            for i, e in enumerate(errors)]
+    return _execute_jobs("dg_execute_programs", jobs, options, backend.DgExecutionStats(), stats, int(max_steps))
 
 
 # ---- many long executions, each split across GPU threads, in one call ------------------------------------------------------------------
-def _many_stats(stats, st):
-    if stats is not None:
-        stats.update({f: (float if f.endswith("_ms") else int)(getattr(st, f)) for f, _ in backend.DgManyStats._fields_ if f != "fallback"})
-        fb = {}
-        _vm_stats(fb, st.fallback)
-        stats["fallback"] = fb
-
-
 def _segment_steps(segment_steps):
     s = int(segment_steps)
     if s != 0 and (s < 16 or s & (s - 1)):
@@ -751,57 +706,14 @@ def trace_many(jobs, max_steps=MAX_STEPS, segment_steps=0, stats=None):
     segment_steps: 0 (the library chooses) or a power of two >= 16.  The buffers are sized by a call without registers first, so the
     tables and the sequential pass run twice.  A dict passed as `stats` receives the full call's figures, the batch path's for the
     fallback executions under "fallback"."""
-    jobs = list(jobs)
-    s = _segment_steps(segment_steps)
-    if not jobs:
-        return []
-    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
-    k, L = len(jobs), backend.lib()
-    info = (backend.DgExecutionInfo * k)()
-    status = (ctypes.c_int * k)()
-    st = backend.DgManyStats()
-    backend.check(L.dg_trace_many(cprogs, len(programs), k, program_of, arr, int(max_steps), s, info, None, status, ctypes.byref(st)))
-    regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
-    outs = (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs])
-    backend.check(L.dg_trace_many(cprogs, len(programs), k, program_of, arr, int(max_steps), s, info, outs, status, ctypes.byref(st)))
-    errors = _messages(list(status))
-    _many_stats(stats, st)
-    result = []
-    for i, (job, e) in enumerate(zip(jobs, errors)):
-        if e is not None:
-            result.append(e)
-            continue
-        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
-        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
-        result.append(hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
-                                            list(job[1].public), last[:num_outputs[i]]))
-    del keep
-    return result
+    return _trace_jobs("dg_trace_many", jobs, backend.DgManyStats(), stats, int(max_steps), _segment_steps(segment_steps))
 
 
 def execute_many(jobs, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
     """execute_programs with every execution run as execute_one runs one (dg_execute_many): every trace is proven where it was written.
     Returns a list in job order: (outputs, StarkProof) -- what execute_programs returns, byte for byte -- or the DgError of an execution
     that failed.  segment_steps and `stats` as in trace_many."""
-    options = options or ProofOptions()
-    jobs = list(jobs)
-    s = _segment_steps(segment_steps)
-    if not jobs:
-        return []
-    programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
-    k = len(jobs)
-    opt = options._c()
-    handles = (backend.vp * k)()
-    outputs = np.zeros((k, 8, 2), dtype=np.uint64)
-    status = (ctypes.c_int * k)()
-    pst, st = backend.DgStats(), backend.DgManyStats()
-    backend.check(backend.lib().dg_execute_many(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), int(max_steps), s,
-                                               ctypes.byref(opt), handles, outputs.ctypes.data, status, ctypes.byref(pst), ctypes.byref(st)))
-    errors = _messages(list(status))
-    _many_stats(stats, st)
-    del keep
-    return [e if e is not None else (felt.to_ints(outputs[i, :num_outputs[i]]) if num_outputs[i] else [], _collect(handles[i], pst))
-            for i, e in enumerate(errors)]
+    return _execute_jobs("dg_execute_many", jobs, options, backend.DgManyStats(), stats, int(max_steps), _segment_steps(segment_steps))
 
 
 # ---- building blocks ------------------------------------------------------------------------------------------------------

@@ -703,7 +703,7 @@ int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(programs && program_of && inputs && status, "null argument");
         const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
+        check_execution_call(x);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
@@ -717,8 +717,7 @@ int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint3
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
         const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x);
-        check_output_counts(count, num_outputs, outputs16);
+        check_execution_call(x, OutputCounts{num_outputs, outputs16});
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
@@ -733,7 +732,7 @@ int dg_trace_batch(const dg_program_t *program, uint32_t count, const dg_program
         DG_REQUIRE(program && inputs && status, "null argument");
         const std::vector<uint32_t> of(count, 0);
         const ExecutionCall x{program, 1, count, of.data(), inputs, max_steps};
-        check_execution_call(x);      // a bad encoding is rejected before the device is touched
+        check_execution_call(x);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
@@ -745,20 +744,52 @@ int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_progr
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(program && inputs && options && proofs_out && status, "null argument");
-        const std::vector<uint32_t> of(count, 0);
+        const std::vector<uint32_t> of(count, 0), n_out(count, num_outputs);
         const ExecutionCall x{program, 1, count, of.data(), inputs, max_steps};
-        check_execution_call(x);
+        check_execution_call(x, OutputCounts{n_out.data(), outputs16});
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        DG_REQUIRE(num_outputs <= 8, "cannot have more than 8 outputs");
-        DG_REQUIRE(num_outputs == 0 || outputs16, "null outputs");
-        const std::vector<uint32_t> n_out(count, num_outputs);
         std::vector<uint8_t> outs((size_t)count * 8 * 16);
         execute_programs(c, x, n_out.data(), *options, (Proof **)proofs_out, outs.data(), status, t_batch_messages, stats, nullptr);
         if (num_outputs)     // num_outputs elements per execution
             for (uint32_t i = 0; i < count; i++) memcpy(outputs16 + (size_t)16 * num_outputs * i, outs.data() + (size_t)128 * i, (size_t)16 * num_outputs);
     });
+}
+// dg_trace_one's stats from its dg_trace_many call's: after the fallback, the batch path's shape and write passes
+static void one_stats(dg_trace_one_stats_t *stats, const dg_many_stats_t &m) {
+    if (!stats) return;
+    memset(stats, 0, sizeof *stats);
+    const bool fb = m.fallback_programs > 0;
+    stats->table_ms = m.table_ms;
+    stats->sequential_ms = fb ? m.fallback.shape_ms : m.sequential_ms;
+    stats->segment_ms = fb ? m.fallback.write_ms : m.segment_ms;
+    stats->table_rounds = m.table_rounds;
+    stats->table_entries = m.table_entries;
+    stats->table_levels = m.table_levels;
+    stats->sequential_launches = m.sequential_launches;
+    stats->checkpoints = m.checkpoints;
+    stats->segments = m.segments;
+    stats->logged = m.logged;
+    stats->segment_steps = m.segment_steps;
+    stats->fallback = fb ? 1 : 0;
+}
+// dg_trace_one / dg_execute_one: many(status, messages, many_stats) runs the execution as dg_trace_many / dg_execute_many with count 1.
+// Its stats reach `stats` also when it throws, and a failed execution throws with its message.  The messages stay local, so that these
+// calls leave the thread's dg_batch_message list as it was.
+static void run_one(dg_trace_one_stats_t *stats, const std::function<void(int *, std::vector<std::string> &, dg_many_stats_t *)> &many) {
+    dg_many_stats_t m;
+    memset(&m, 0, sizeof m);
+    int status = DG_OK;
+    std::vector<std::string> messages;
+    try {
+        many(&status, messages, &m);
+    } catch (...) {
+        one_stats(stats, m);
+        throw;
+    }
+    one_stats(stats, m);
+    if (status != DG_OK) throw Error(status, messages[0]);
 }
 int dg_trace_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps,
                  dg_execution_info_t *info, uint8_t *registers_out, dg_trace_one_stats_t *stats) {
@@ -766,11 +797,15 @@ int dg_trace_one(const dg_program_t *program, const dg_program_inputs_t *inputs,
         DG_REQUIRE(program && inputs, "null argument");
         const uint32_t of = 0;
         const ExecutionCall x{program, 1, 1, &of, inputs, max_steps};
-        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
-        check_segment_steps(segment_steps);
+        check_execution_call(x, std::nullopt, segment_steps);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        trace_one(c, x, segment_steps, info, registers_out, stats);
+        uint8_t *const outs[1] = {registers_out};
+        dg_execution_info_t one;          // reaches info only when the call succeeds
+        run_one(stats, [&](int *status, std::vector<std::string> &messages, dg_many_stats_t *m) {
+            trace_many(c, x, segment_steps, &one, registers_out ? outs : nullptr, status, messages, m);
+        });
+        if (info) *info = one;
     });
 }
 int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *inputs, uint32_t num_outputs, uint64_t max_steps,
@@ -781,12 +816,16 @@ int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *input
         *proof_out = nullptr;
         const uint32_t of = 0;
         const ExecutionCall x{program, 1, 1, &of, inputs, max_steps};
-        check_execution_call(x);
-        check_output_counts(1, &num_outputs, outputs16);
-        check_segment_steps(segment_steps);
+        check_execution_call(x, OutputCounts{&num_outputs, outputs16}, segment_steps);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        *proof_out = (dg_proof_t *)execute_one(c, x, num_outputs, segment_steps, *options, outputs16, info, prove_stats, stats);
+        uint8_t outs[8 * 16];             // execute_many writes 8 elements; the caller's buffer holds num_outputs
+        dg_execution_info_t one;
+        run_one(stats, [&](int *status, std::vector<std::string> &messages, dg_many_stats_t *m) {
+            execute_many(c, x, &num_outputs, segment_steps, *options, (Proof **)proof_out, outs, &one, status, messages, prove_stats, m);
+        });
+        if (num_outputs) memcpy(outputs16, outs, (size_t)16 * num_outputs);
+        if (info) *info = one;
     });
 }
 int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
@@ -796,8 +835,7 @@ int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t co
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(programs && program_of && inputs && status, "null argument");
         const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x);      // bad arguments and encodings are rejected before the device is touched
-        check_segment_steps(segment_steps);
+        check_execution_call(x, std::nullopt, segment_steps);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
@@ -812,13 +850,12 @@ int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t 
         DG_REQUIRE(count >= 1, "at least one execution is needed");
         DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
         const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x);
-        check_output_counts(count, num_outputs, outputs16);
-        check_segment_steps(segment_steps);
+        check_execution_call(x, OutputCounts{num_outputs, outputs16}, segment_steps);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
-        execute_many(c, x, num_outputs, segment_steps, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, prove_stats, stats);
+        execute_many(c, x, num_outputs, segment_steps, *options, (Proof **)proofs_out, outputs16, nullptr, status, t_batch_messages, prove_stats,
+                     stats);
     });
 }
 int dg_batch_message(uint32_t index, char *message, size_t cap) {

@@ -12,6 +12,7 @@
 #include <deque>
 #include <functional>
 #include <map>
+#include <numeric>
 #include <set>
 #include <tuple>
 
@@ -464,17 +465,33 @@ void batch_execute(Context &c, Executions &X, const std::vector<unsigned> &ids, 
     });
 }
 
-void finish(const Executions &X, int *status, std::vector<std::string> &messages, dg_execution_stats_t *vm_stats) {
-    for (uint32_t i = 0; i < X.x.count; i++) status[i] = X.status[i];
+// the per-execution results of a call: info (may be null; zero for a failed execution), status, messages and the VM passes' stats
+void finish(const Executions &X, dg_execution_info_t *info, int *status, std::vector<std::string> &messages, dg_execution_stats_t *vm_stats) {
+    for (uint32_t i = 0; i < X.x.count; i++) {
+        if (info) {
+            if (X.status[i] == DG_OK) info[i] = X.info(i);
+            else memset(&info[i], 0, sizeof info[i]);
+        }
+        status[i] = X.status[i];
+    }
     messages = X.messages;
     if (vm_stats) *vm_stats = X.stats;
 }
 
-// the proofs of the waves done so far are freed when a later wave fails the call
-struct ReleaseOnError {
-    Proof **out; uint32_t count; bool done = false;
-    ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
-};
+// The frame of an execute call around run(outs): proofs_out and stats start null / zero, the proofs of the waves done so far are freed
+// when a later wave fails the call, and the 8 output elements per execution that run leaves in outs go to outputs16 (when given).
+template <typename F> void proven(uint32_t count, Proof **proofs_out, uint8_t *outputs16, dg_prove_stats_t *stats, F &&run) {
+    for (uint32_t i = 0; i < count; i++) proofs_out[i] = nullptr;
+    if (stats) memset(stats, 0, sizeof *stats);
+    try {
+        std::vector<fe> outs((size_t)count * 8, fe_make(0, 0));
+        run(outs);
+        if (outputs16) memcpy(outputs16, outs.data(), outs.size() * 16);
+    } catch (...) {
+        for (uint32_t i = 0; i < count; i++) { delete proofs_out[i]; proofs_out[i] = nullptr; }
+        throw;
+    }
+}
 
 // ---- executions from the sponge tables --------------------------------------------------------------------------------------------------
 // The chains of a program (vm.h): every block list reachable from the root once (lists may be shared: a list is its child range) and, per
@@ -570,12 +587,14 @@ uint64_t default_segment_steps(uint64_t max_steps) {
 // programs) and sorts the executions the inputs did not fail into `run` (their program's hashes are consistent) and `fallback` (they are
 // not: the batch path runs them, in X, so results are identical either way).  sequential() runs every execution of `run` in one launch,
 // one warp each (again, for the executions that outgrew their tape scratch, read log or checkpoint buffer, with the room they reported),
-// and waves() writes the rows of its successful executions in waves, one segment launch per wave for all their checkpoints.
+// and waves() writes the rows of its successful executions in waves, one segment launch per wave for all their checkpoints.  The stats
+// reach `out` (may be null) in the destructor, so also when a pass throws: dg_trace_one reports a failed call's.
 struct TabledExecutions {
     Context &c;
     Executions X;
     uint64_t S;
     dg_many_stats_t st;
+    dg_many_stats_t *out;
     std::vector<char> tabled;                     // per program
     std::vector<unsigned> run, fallback;          // in input order
     std::vector<VmTabled> T;                      // per execution
@@ -584,9 +603,9 @@ struct TabledExecutions {
     DevBuf d_refs, d_tab, d_T, d_seq, d_codes, d_execs, d_first;
     VmTables G;
 
-    TabledExecutions(Context &ctx_, const ExecutionCall &x, uint64_t segment_steps)
-        : c(ctx_), X(ctx_, x), S(segment_steps ? segment_steps : default_segment_steps(x.max_steps)), tabled(x.n_programs, 0), T(x.count),
-          seq(x.count) {
+    TabledExecutions(Context &ctx_, const ExecutionCall &x, uint64_t segment_steps, dg_many_stats_t *stats)
+        : c(ctx_), X(ctx_, x), S(segment_steps ? segment_steps : default_segment_steps(x.max_steps)), out(stats), tabled(x.n_programs, 0),
+          T(x.count), seq(x.count) {
         memset(&st, 0, sizeof st);
         memset(T.data(), 0, T.size() * sizeof(VmTabled));
         memset(seq.data(), 0, seq.size() * sizeof(VmSequential));
@@ -594,6 +613,7 @@ struct TabledExecutions {
         G = VmTables{nullptr, nullptr, S};
         X.setup();
     }
+    ~TabledExecutions() { if (out) *out = st; }
 
     // the chains of every program with an execution to run, rebased as X.setup() rebased the programs: child ranges by the child entries
     // before the program, block indices by the blocks before it, table indices by the entries before it
@@ -776,28 +796,9 @@ struct TabledExecutions {
     }
 };
 
-// dg_trace_one's stats from the call's: after the fallback, the batch path's shape and write passes
-void one_stats(dg_trace_one_stats_t *stats, const dg_many_stats_t &m) {
-    if (!stats) return;
-    memset(stats, 0, sizeof *stats);
-    const bool fb = m.fallback_programs > 0;
-    stats->table_ms = m.table_ms;
-    stats->sequential_ms = fb ? m.fallback.shape_ms : m.sequential_ms;
-    stats->segment_ms = fb ? m.fallback.write_ms : m.segment_ms;
-    stats->table_rounds = m.table_rounds;
-    stats->table_entries = m.table_entries;
-    stats->table_levels = m.table_levels;
-    stats->sequential_launches = m.sequential_launches;
-    stats->checkpoints = m.checkpoints;
-    stats->segments = m.segments;
-    stats->logged = m.logged;
-    stats->segment_steps = m.segment_steps;
-    stats->fallback = fb ? 1 : 0;
-}
-
 }  // namespace
 
-void check_execution_call(const ExecutionCall &x) {
+void check_execution_call(const ExecutionCall &x, const std::optional<OutputCounts> &outputs, std::optional<uint64_t> segment_steps) {
     DG_REQUIRE(x.count >= 1, "at least one execution is needed");
     DG_REQUIRE(x.n_programs >= 1, "at least one program is needed");
     DG_REQUIRE(x.programs && x.program_of, "null program table");
@@ -823,135 +824,62 @@ void check_execution_call(const ExecutionCall &x) {
         DG_REQUIRE((v.n_public == 0 || v.public16) && (v.n_secret_a == 0 || v.secret_a16) && (v.n_secret_b == 0 || v.secret_b16),
                    "null inputs of execution " + std::to_string(i));
     }
-}
-
-void check_output_counts(uint32_t count, const uint32_t *num_outputs, const uint8_t *outputs16) {
-    DG_REQUIRE(num_outputs, "null num_outputs");
-    bool any = false;
-    for (uint32_t i = 0; i < count; i++) {
-        DG_REQUIRE(num_outputs[i] <= 8, "cannot have more than 8 outputs");
-        any |= num_outputs[i] > 0;
-    }
-    DG_REQUIRE(!any || outputs16, "null outputs");
-}
-
-void check_segment_steps(uint64_t s) {
-    DG_REQUIRE(s == 0 || (s >= 16 && (s & (s - 1)) == 0), "segment_steps must be 0 or a power of two of at least 16");
-}
-
-void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
-                std::vector<std::string> &messages, dg_many_stats_t *stats) {
-    check_execution_call(x);
-    check_segment_steps(segment_steps);
-    check_one_gpu(c);
-    TabledExecutions E(c, x, segment_steps);
-    E.trace(registers_out);
-    if (info)
+    if (outputs) {
+        DG_REQUIRE(outputs->num_outputs, "null num_outputs");
+        bool any = false;
         for (uint32_t i = 0; i < x.count; i++) {
-            if (E.X.status[i] == DG_OK) info[i] = E.X.info(i);
-            else memset(&info[i], 0, sizeof info[i]);
+            DG_REQUIRE(outputs->num_outputs[i] <= 8, "cannot have more than 8 outputs");
+            any |= outputs->num_outputs[i] > 0;
         }
-    finish(E.X, status, messages, nullptr);
-    if (stats) *stats = E.st;
-}
-
-void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
-                  Proof **proofs_out, uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *prove_stats,
-                  dg_many_stats_t *stats) {
-    check_execution_call(x);
-    check_output_counts(x.count, num_outputs, outputs16);
-    check_segment_steps(segment_steps);
-    check_one_gpu(c);
-    for (uint32_t i = 0; i < x.count; i++) proofs_out[i] = nullptr;
-    if (prove_stats) memset(prove_stats, 0, sizeof *prove_stats);
-    TabledExecutions E(c, x, segment_steps);
-    ReleaseOnError release{proofs_out, x.count};
-    std::vector<fe> outs((size_t)x.count * 8, fe_make(0, 0));
-    E.execute(num_outputs, opt, outs, proofs_out, prove_stats);
-    release.done = true;
-    if (outputs16) memcpy(outputs16, outs.data(), outs.size() * 16);
-    finish(E.X, status, messages, nullptr);
-    if (stats) *stats = E.st;
-}
-
-void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *registers_out,
-               dg_trace_one_stats_t *stats) {
-    DG_REQUIRE(x.count == 1, "one execution");
-    check_execution_call(x);
-    check_segment_steps(segment_steps);
-    check_one_gpu(c);
-    TabledExecutions E(c, x, segment_steps);
-    uint8_t *const outs[1] = {registers_out};
-    try {
-        E.trace(registers_out ? outs : nullptr);
-    } catch (...) {
-        one_stats(stats, E.st);
-        throw;
+        DG_REQUIRE(!any || outputs->outputs16, "null outputs");
     }
-    one_stats(stats, E.st);
-    if (E.X.status[0] != DG_OK) throw Error(E.X.status[0], E.X.messages[0]);
-    if (info) *info = E.X.info(0);
-}
-
-Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
-                   dg_execution_info_t *info, dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats) {
-    DG_REQUIRE(x.count == 1, "one execution");
-    check_execution_call(x);
-    check_output_counts(1, &num_outputs, outputs16);
-    check_segment_steps(segment_steps);
-    check_one_gpu(c);
-    if (prove_stats) memset(prove_stats, 0, sizeof *prove_stats);
-    TabledExecutions E(c, x, segment_steps);
-    Proof *proof = nullptr;
-    std::vector<fe> outs(8, fe_make(0, 0));
-    try {
-        E.execute(&num_outputs, opt, outs, &proof, prove_stats);
-    } catch (...) {
-        delete proof;
-        one_stats(stats, E.st);
-        throw;
+    if (segment_steps) {
+        const uint64_t s = *segment_steps;
+        DG_REQUIRE(s == 0 || (s >= 16 && (s & (s - 1)) == 0), "segment_steps must be 0 or a power of two of at least 16");
     }
-    one_stats(stats, E.st);
-    if (E.X.status[0] != DG_OK) throw Error(E.X.status[0], E.X.messages[0]);
-    if (num_outputs) memcpy(outputs16, outs.data(), (size_t)16 * num_outputs);
-    if (info) *info = E.X.info(0);
-    return proof;
 }
 
 void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
                     std::vector<std::string> &messages, dg_execution_stats_t *vm_stats) {
-    check_execution_call(x);
     check_one_gpu(c);
     Executions X(c, x);
     X.setup();
     std::vector<unsigned> all(x.count);
-    for (uint32_t i = 0; i < x.count; i++) all[i] = i;
+    std::iota(all.begin(), all.end(), 0u);
     batch_trace(c, X, all, registers_out, registers_out != nullptr, true);
-    if (info)
-        for (uint32_t i = 0; i < x.count; i++) {
-            if (X.status[i] == DG_OK) info[i] = X.info(i);
-            else memset(&info[i], 0, sizeof info[i]);
-        }
-    finish(X, status, messages, vm_stats);
+    finish(X, info, status, messages, vm_stats);
 }
 
 void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
-    check_execution_call(x);
-    check_output_counts(x.count, num_outputs, outputs16);
     check_one_gpu(c);
-    for (uint32_t i = 0; i < x.count; i++) proofs_out[i] = nullptr;
-    if (stats) memset(stats, 0, sizeof *stats);
-    Executions X(c, x);
-    X.setup();
-    ReleaseOnError release{proofs_out, x.count};
-    std::vector<fe> outs((size_t)x.count * 8, fe_make(0, 0));
-    std::vector<unsigned> all(x.count);
-    for (uint32_t i = 0; i < x.count; i++) all[i] = i;
-    batch_execute(c, X, all, num_outputs, opt, outs, proofs_out, stats);
-    release.done = true;
-    if (outputs16) memcpy(outputs16, outs.data(), outs.size() * 16);
-    finish(X, status, messages, vm_stats);
+    proven(x.count, proofs_out, outputs16, stats, [&](std::vector<fe> &outs) {
+        Executions X(c, x);
+        X.setup();
+        std::vector<unsigned> all(x.count);
+        std::iota(all.begin(), all.end(), 0u);
+        batch_execute(c, X, all, num_outputs, opt, outs, proofs_out, stats);
+        finish(X, nullptr, status, messages, vm_stats);
+    });
+}
+
+void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                std::vector<std::string> &messages, dg_many_stats_t *stats) {
+    check_one_gpu(c);
+    TabledExecutions E(c, x, segment_steps, stats);
+    E.trace(registers_out);
+    finish(E.X, info, status, messages, nullptr);
+}
+
+void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
+                  Proof **proofs_out, uint8_t *outputs16, dg_execution_info_t *info, int *status, std::vector<std::string> &messages,
+                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
+    check_one_gpu(c);
+    proven(x.count, proofs_out, outputs16, prove_stats, [&](std::vector<fe> &outs) {
+        TabledExecutions E(c, x, segment_steps, stats);
+        E.execute(num_outputs, opt, outs, proofs_out, prove_stats);
+        finish(E.X, info, status, messages, nullptr);
+    });
 }
 
 }  // namespace dg

@@ -4,6 +4,7 @@
 #include "../../include/distaff_gpu.h"
 #include "common.cuh"
 #include "proof.h"
+#include <optional>
 
 namespace dg {
 
@@ -49,10 +50,7 @@ std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape);
 // <call> must ..."), 16..127 registers and no null column; length_first also checks each length before its columns (dg_prove).
 std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first);
 
-// dg_trace_programs / dg_execute_programs (execute.cu; dg_trace_batch / dg_execute_batch with one program): execution i runs
-// programs[program_of[i]] on inputs[i]; status / messages per execution.  check_execution_call validates the arguments and every
-// program's encoding on the host alone (DG_ERR_INVALID), as does check_output_counts the per-execution output counts; the calls run
-// them again.  execute_programs writes 8 output elements per execution (zero past its num_outputs).
+// The execution calls (execute.cu).  Execution i runs programs[program_of[i]] on inputs[i]; status / messages per execution.
 struct ExecutionCall {
     const dg_program_t *programs;
     uint32_t n_programs, count;
@@ -60,25 +58,30 @@ struct ExecutionCall {
     const dg_program_inputs_t *inputs;
     uint64_t max_steps;
 };
-void check_execution_call(const ExecutionCall &x);
-void check_output_counts(uint32_t count, const uint32_t *num_outputs, const uint8_t *outputs16);
+// the output counts of an execute call: num_outputs[i] <= 8 per execution; outputs16 may be null when every count is 0
+struct OutputCounts {
+    const uint32_t *num_outputs;
+    const uint8_t *outputs16;
+};
+// Every execution entry runs this once before it touches the device: it rejects bad arguments and encodings on the host alone
+// (DG_ERR_INVALID), with the output counts of an execute call and the segment_steps of a tabled call (0 or a power of two >= 16) when
+// given.  The calls below assume it passed.
+void check_execution_call(const ExecutionCall &x, const std::optional<OutputCounts> &outputs = std::nullopt,
+                          std::optional<uint64_t> segment_steps = std::nullopt);
+// dg_trace_programs / dg_execute_programs (dg_trace_batch / dg_execute_batch with one program): the batch path.  info may be null.
+// execute_programs writes 8 output elements per execution (zero past its num_outputs).
 void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
                     std::vector<std::string> &messages, dg_execution_stats_t *vm_stats);
 void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
-// dg_trace_one / dg_execute_one (execute.cu): one execution (x.count == 1) from the sponge table; a failed execution throws
-// DG_ERR_EXECUTION with its message.  check_segment_steps rejects an S that is neither 0 nor a power of two >= 16.
-void check_segment_steps(uint64_t segment_steps);
-void trace_one(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *registers_out,
-               dg_trace_one_stats_t *stats);
-Proof *execute_one(Context &c, const ExecutionCall &x, uint32_t num_outputs, uint64_t segment_steps, const dg_options_t &opt, uint8_t *outputs16,
-                   dg_execution_info_t *info, dg_prove_stats_t *prove_stats, dg_trace_one_stats_t *stats);
-// dg_trace_many / dg_execute_many (execute.cu): trace_programs / execute_programs with the executions run from the sponge tables
+// dg_trace_many / dg_execute_many (dg_trace_one / dg_execute_one with one execution): trace_programs / execute_programs with the
+// executions run from the sponge tables.  info may be null.  stats (may be null) are written also when the tabled passes throw (dg_trace_one
+// reports a failed call's).
 void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
                 std::vector<std::string> &messages, dg_many_stats_t *stats);
 void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
-                  Proof **proofs_out, uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *prove_stats,
-                  dg_many_stats_t *stats);
+                  Proof **proofs_out, uint8_t *outputs16, dg_execution_info_t *info, int *status, std::vector<std::string> &messages,
+                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP
 long long batch_group_cap(long long k);
 

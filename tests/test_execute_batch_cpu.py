@@ -141,3 +141,18 @@ def test_shared_blocks_are_validated_once():
     deeper = cases.shared_block_program(levels=16)
     rc, msg = _call(backend, deeper)
     assert rc == -1 and "nested more than 15 deep" in msg, msg
+
+
+def test_output_count_is_checked_before_the_device():
+    """dg_execute_batch rejects more than 8 outputs on the host, as every execution entry rejects bad arguments, with or without a GPU"""
+    backend = _lib_or_skip()
+    from distaff_b200 import api
+    _, cprog, arr, keep = api._execution_args(hostvm.fibonacci_program(13), [api.ProgramInputs([1, 0])])
+    opt = api.ProofOptions()._c()
+    handles = (backend.vp * 1)()
+    out = np.zeros((9, 2), dtype=np.uint64)
+    status = (ctypes.c_int * 1)()
+    rc = backend.lib().dg_execute_batch(ctypes.byref(cprog), 1, arr, 9, 1 << 10, ctypes.byref(opt), handles, out.ctypes.data, status, None)
+    del keep
+    assert (rc, backend.lib().dg_last_error().decode()) == (-1, "cannot have more than 8 outputs")
+    assert handles[0] is None
