@@ -189,6 +189,14 @@ EXPORTS = {
     "dg_set_memory_limit": [ctypes.c_size_t],
     "dg_memory_usage": [ctypes.POINTER(ctypes.c_size_t), ctypes.POINTER(ctypes.c_size_t)],
     "dg_plan_prove": [u32, u64, u32, ctypes.POINTER(DgOptions), ctypes.POINTER(DgProvePlan)],
+    # test hooks (include/distaff_gpu.h): the stage kernels one at a time, for tests only
+    "dg_test_syn_div": [vp, vp, u32, u64, u64, u64, ctypes.c_int, vp, ctypes.c_int, vp],
+    "dg_test_syn_div_expanded_sum": [vp, vp, vp, vp, u32, u64, u64, u64, vp],
+    "dg_test_eval_polys_at": [vp, u32, u32, vp, u32, vp, vp],
+    "dg_test_eval_trace_rows": [vp, u32, u32, u32, vp, vp, vp, u32, vp],
+    "dg_test_lde_fold8": [vp, vp, u32, u32, u32, u32, u32, u64],
+    "dg_test_coset_interp": [vp, vp, u32, u32, u64],
+    "dg_test_fri_layer": [vp, u32, u64, u32, ctypes.c_int32, u32, vp, u64, vp, vp, vp, vp],
 }
 VOID_EXPORTS = {"dg_proof_free": [vp], "dg_tree_free": [vp]}
 

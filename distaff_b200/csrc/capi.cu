@@ -1095,4 +1095,241 @@ int dg_host_constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t st
     });
 }
 
+// ---- test hooks: the coefficient-domain stage kernels of the prover, one call each, on host buffers ---------------------------------------
+// Each hook checks every argument before it touches the device and then calls the host function prover.cu calls, with the parameters
+// prover.cu gives it.  Output buffers are zero-filled on the device first, so that a test also sees what a kernel writes outside its range.
+static bool is_pow2(uint64_t v) { return v && !(v & (v - 1)); }
+static std::vector<fe> host_fes(const uint8_t *p, uint64_t n) {
+    std::vector<fe> v(n);
+    memcpy(v.data(), p, n * 16);
+    return v;
+}
+static void upload(Context &c, DevBuf &d, const uint8_t *p, size_t n) {
+    d.alloc(n * 16);
+    DG_CUDA(cudaMemcpyAsync(d.p, p, n * 16, cudaMemcpyHostToDevice, c.stream));
+}
+static void zeroed(Context &c, DevBuf &d, size_t n) {
+    d.alloc(n * 16);
+    DG_CUDA(cudaMemsetAsync(d.p, 0, n * 16, c.stream));
+}
+static void download(Context &c, uint8_t *p, const DevBuf &d, size_t bytes) {
+    DG_CUDA(cudaMemcpyAsync(p, d.p, bytes, cudaMemcpyDeviceToHost, c.stream));
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+}
+static void require_batch(uint32_t batch) { DG_REQUIRE(batch >= 1 && batch <= 65535, "batch must be in 1..65535"); }
+// a vector of len elements per batch entry, `stride` elements apart: the elements the buffer spans
+static uint64_t strided_span(uint32_t batch, uint64_t stride, uint64_t len, const char *what) {
+    DG_REQUIRE(stride >= len && stride <= (1ULL << 32), std::string(what) + " must be at least the vector length and at most 2^32");
+    return (uint64_t)(batch - 1) * stride + len;
+}
+
+int dg_test_syn_div(const uint8_t *in16, uint8_t *out16, uint32_t batch, uint64_t len, uint64_t in_stride, uint64_t out_stride, int in_place,
+                    const uint8_t *b16, int shared, const uint8_t *sub0_16) {
+    return guarded([&] {
+        DG_REQUIRE(in16 && out16 && b16 && sub0_16, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(is_pow2(len) && len >= 2 && len <= (1ULL << 28), "len must be a power of 2 in 2..2^28");
+        DG_REQUIRE((len + 1023) / 1024 * batch < (1ULL << 31), "division batch too large for one launch");
+        const uint64_t in_n = strided_span(batch, in_stride, len, "in_stride"), out_n = strided_span(batch, out_stride, len, "out_stride");
+        DG_REQUIRE(!in_place || in_stride == out_stride, "an in-place division has one stride");
+        const uint32_t tables = shared ? 1 : batch;
+        require_canonical(in16, in_n, 1, "input element");
+        require_canonical(b16, tables, 1, "point");
+        require_canonical(sub0_16, batch, 1, "sub0");
+        // the (base, step) pairs of the tables of b, then of 1 / b, as prover.cu packs them
+        const std::vector<fe> b = host_fes(b16, tables);
+        std::vector<fe> pack(4 * (size_t)tables);
+        for (uint32_t q = 0; q < tables; q++) {
+            DG_REQUIRE(b[q].lo || b[q].hi, "point " + std::to_string(q) + " is zero");
+            const fe bi = host_inv(b[q]);
+            pack[2 * q] = b[q]; pack[2 * q + 1] = PowTables::step(b[q], len + 1);
+            pack[2 * (tables + q)] = bi; pack[2 * (tables + q) + 1] = PowTables::step(bi, len + 1);
+        }
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_in, d_out, d_pack, d_sub0;
+        upload(c, d_in, in16, in_n);
+        upload(c, d_pack, (const uint8_t *)pack.data(), pack.size());
+        upload(c, d_sub0, sub0_16, batch);
+        if (!in_place) zeroed(c, d_out, out_n);
+        fe *out = in_place ? d_in.as<fe>() : d_out.as<fe>();
+        if (shared) {                       // one table for all vectors (stage 4: 1 and x_last)
+            PowTables pows(c, d_pack.as<fe>(), 2, len + 1);
+            syn_div(c, (int)batch, d_in.as<fe>(), in_stride, out, out_stride, len, pows.ref(0), 0, 0, pows.ref(1), 0, 0, d_sub0.as<fe>());
+        } else {                            // a table per vector (stage 6: z and z g of every proof)
+            PowTables t(c, d_pack.as<fe>(), (int)batch, len + 1), ti(c, d_pack.as<fe>() + 2 * batch, (int)batch, len + 1);
+            syn_div(c, (int)batch, d_in.as<fe>(), in_stride, out, out_stride, len, t.ref(0), t.lo_n, t.hi_n, ti.ref(0), ti.lo_n, ti.hi_n,
+                    d_sub0.as<fe>());
+        }
+        download(c, out16, in_place ? d_in : d_out, out_n * 16);
+    });
+}
+
+int dg_test_syn_div_expanded_sum(const uint8_t *a16, const uint8_t *add0_16, const uint8_t *add1_16, uint8_t *out16, uint32_t batch, uint64_t n,
+                                 uint64_t in_stride, uint64_t out_stride, const uint8_t *e16) {
+    return guarded([&] {
+        DG_REQUIRE(a16 && out16 && e16, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(is_pow2(n) && n <= (1ULL << 26), "n must be a power of 2 up to 2^26");
+        const uint64_t len = 8 * n;
+        const uint64_t in_n = strided_span(batch, in_stride, len, "in_stride"), out_n = strided_span(batch, out_stride, len, "out_stride");
+        require_canonical(a16, in_n, 1, "a element");
+        if (add0_16) require_canonical(add0_16, in_n, 1, "add0 element");
+        if (add1_16) require_canonical(add1_16, in_n, 1, "add1 element");
+        require_canonical(e16, 1, 1, "point");
+        const fe e = host_fes(e16, 1)[0];
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_a, d_add0, d_add1, d_scratch((size_t)batch * len * 16), d_out;
+        upload(c, d_a, a16, in_n);
+        if (add0_16) upload(c, d_add0, add0_16, in_n);
+        if (add1_16) upload(c, d_add1, add1_16, in_n);
+        zeroed(c, d_out, out_n);
+        syn_div_expanded_sum(c, d_a.as<fe>(), d_scratch.as<fe>(), add0_16 ? d_add0.as<fe>() : nullptr, add1_16 ? d_add1.as<fe>() : nullptr,
+                             d_out.as<fe>(), n, len, e, (int)batch, in_stride, out_stride);
+        download(c, out16, d_out, out_n * 16);
+    });
+}
+
+int dg_test_eval_polys_at(const uint8_t *polys16, uint32_t cols, uint32_t log_n, const uint8_t *z16, uint32_t n_z, const uint32_t *col_proof,
+                          uint8_t *out16) {
+    return guarded([&] {
+        DG_REQUIRE(polys16 && z16 && out16, "null buffer");
+        DG_REQUIRE(cols >= 1 && cols <= 65535 && n_z >= 1 && n_z <= 65535, "cols and n_z must be in 1..65535");
+        DG_REQUIRE(log_n >= 1 && log_n <= 26, "log_n must be in 1..26");
+        const uint64_t n = 1ULL << log_n, E = 8 * n, len = col_proof ? n : E;
+        if (col_proof) {
+            for (uint32_t j = 0; j < cols; j++) DG_REQUIRE(col_proof[j] < n_z, "column " + std::to_string(j) + " names no point");
+        } else {
+            DG_REQUIRE(cols == n_z, "the one-point form evaluates column q at point q");
+        }
+        require_canonical(polys16, cols * len, 1, "coefficient");
+        require_canonical(z16, n_z, 1, "point");
+        const std::vector<fe> z = host_fes(z16, n_z);
+        std::vector<fe> pack(2 * (size_t)n_z);
+        for (uint32_t q = 0; q < n_z; q++) { pack[2 * q] = z[q]; pack[2 * q + 1] = PowTables::step(z[q], E + 1); }
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_polys, d_pack, d_cp, d_out;
+        upload(c, d_polys, polys16, cols * len);
+        upload(c, d_pack, (const uint8_t *)pack.data(), pack.size());
+        zeroed(c, d_out, 2 * (size_t)cols);
+        PowTables z_t(c, d_pack.as<fe>(), (int)n_z, E + 1);
+        if (col_proof) {                    // stage 6: trace polynomials at z and z w_n, proofs of several widths
+            d_cp.alloc((size_t)cols * 4);
+            DG_CUDA(cudaMemcpyAsync(d_cp.p, col_proof, (size_t)cols * 4, cudaMemcpyHostToDevice, c.stream));
+            eval_polys_at(c, d_polys.as<fe>(), n, (int)cols, z_t.ref(0), c.twiddle((int)log_n, false), true, d_out.as<fe>(), 1 << 30, z_t.lo_n,
+                          z_t.hi_n, d_cp.as<unsigned>());
+        } else {                            // stage 6: the constraint polynomial of every proof at its z
+            eval_polys_at(c, d_polys.as<fe>(), E, (int)cols, z_t.ref(0), c.twiddle((int)log_n, false), false, d_out.as<fe>(), 1, z_t.lo_n,
+                          z_t.hi_n);
+        }
+        download(c, out16, d_out, 2 * (size_t)cols * 16);
+    });
+}
+
+int dg_test_eval_trace_rows(const uint8_t *polys16, uint32_t cols, uint32_t log_n, uint32_t log_N, const uint64_t *pos, const uint32_t *col,
+                            const uint32_t *width, uint32_t count, uint8_t *out16) {
+    return guarded([&] {
+        DG_REQUIRE(polys16 && pos && col && width && out16, "null buffer");
+        DG_REQUIRE(cols >= 1 && count >= 1, "cols and count must be at least 1");
+        DG_REQUIRE(log_n >= 1 && log_N >= log_n && log_N <= log_n + 8 && log_N <= 30, "log_n and log_N out of range");
+        const uint64_t n = 1ULL << log_n;
+        std::vector<TraceRow> points(count);
+        for (uint32_t m = 0; m < count; m++) {
+            DG_REQUIRE(pos[m] < (1ULL << log_N), "position " + std::to_string(m) + " is outside the domain");
+            DG_REQUIRE(width[m] >= 1 && width[m] <= 128 && col[m] <= cols && width[m] <= cols - col[m],
+                       "row " + std::to_string(m) + ": columns out of range (width 1..128)");
+            points[m] = TraceRow{pos[m], 0, col[m], width[m]};
+        }
+        require_canonical(polys16, cols * n, 1, "coefficient");
+        uint64_t values = 0;
+        for (uint32_t m = 0; m < count; m++) values += width[m];
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_polys, d_out;
+        upload(c, d_polys, polys16, cols * n);
+        zeroed(c, d_out, values);
+        eval_trace_rows(c, d_polys.as<fe>(), n, points, (int)log_N, d_out.as<fe>());
+        download(c, out16, d_out, values * 16);
+    });
+}
+
+int dg_test_lde_fold8(const uint8_t *coeffs16, uint8_t *out16, uint32_t log_n, uint32_t log_b, uint32_t coset0, uint32_t ncosets, uint32_t batch,
+                      uint64_t dst_stride) {
+    return guarded([&] {
+        DG_REQUIRE(coeffs16 && out16, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(log_n >= 1 && log_n <= 22 && log_b >= 3 && log_b <= 8, "log_n must be in 1..22 and log_b in 3..8");
+        const uint64_t n = 1ULL << log_n, E = 8 * n, b = 1ULL << log_b;
+        DG_REQUIRE(ncosets >= 1 && coset0 < b && ncosets <= b - coset0, "coset range out of bounds");
+        const uint64_t out_n = strided_span(batch, dst_stride, ncosets * n, "dst_stride");
+        require_canonical(coeffs16, batch * E, 1, "coefficient");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_in, d_out;
+        upload(c, d_in, coeffs16, batch * E);
+        zeroed(c, d_out, out_n);
+        // stages 5 and 6: the constraint / composition polynomials of the batch, E apart
+        lde_batch(c, d_in.as<fe>(), d_out.as<fe>(), (int)log_n, (int)log_b, 8, (int)batch, E, dst_stride, coset0, ncosets);
+        download(c, out16, d_out, out_n * 16);
+    });
+}
+
+int dg_test_coset_interp(const uint8_t *evals16, uint8_t *out16, uint32_t log_n, uint32_t batch, uint64_t out_stride) {
+    return guarded([&] {
+        DG_REQUIRE(evals16 && out16, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(log_n >= 1 && log_n <= 24, "log_n must be in 1..24");
+        const uint64_t n = 1ULL << log_n, E = 8 * n;
+        const uint64_t out_n = strided_span(batch, out_stride, E, "out_stride");
+        require_canonical(evals16, batch * E, 1, "evaluation");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_evals, d_out;
+        upload(c, d_evals, evals16, batch * E);
+        zeroed(c, d_out, out_n);
+        // stage 3: size-n inverse transforms of the 8 cosets of every vector, then the 8-point inverse DFT across them
+        ntt_batch(c, d_evals.as<fe>(), d_evals.as<fe>(), (int)log_n, (int)batch * 8, n, n, true);
+        coset_interp_finish(c, d_evals.as<fe>(), d_out.as<fe>(), (int)log_n, (int)batch, E, out_stride);
+        download(c, out16, d_out, out_n * 16);
+    });
+}
+
+int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_stride, uint32_t log_d, int32_t log_b, uint32_t log_N,
+                      const uint8_t *roots32, uint64_t root_stride, uint8_t *leaves32, uint8_t *alphas16, uint8_t *root_copies32, uint8_t *next16) {
+    return guarded([&] {
+        DG_REQUIRE(values16 && roots32 && leaves32 && alphas16 && root_copies32 && next16, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(log_N <= 30 && log_d >= 4 && log_d <= log_N && (log_N - log_d) % 2 == 0,
+                   "log_d must be in 4..log_N <= 30, an even number of folds below log_N");
+        DG_REQUIRE(log_b >= -1 && log_b <= (int32_t)log_d, "log_b must be -1 (natural layout) or in 0..log_d");
+        DG_REQUIRE(root_stride >= 32 && root_stride % 4 == 0 && root_stride <= (1ULL << 32), "root_stride must be a multiple of 4 in 32..2^32");
+        const uint64_t D = 1ULL << log_d, R = D / 4;
+        const uint64_t in_n = strided_span(batch, values_stride, D, "values_stride");
+        require_canonical(values16, in_n, 1, "value");
+        const Layout in{(int)log_d, log_b};
+        const int log_r = (int)log_d - 2;
+        const Layout rows{log_r, (in.log_b >= 0 && log_r >= in.log_b) ? in.log_b : -1};     // prover.cu: the next layer's layout
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_vals, d_roots((batch - 1) * root_stride + 32), d_leaves, d_alpha, d_copies, d_next;
+        upload(c, d_vals, values16, in_n);
+        DG_CUDA(cudaMemsetAsync(d_roots.p, 0, d_roots.bytes, c.stream));
+        DG_CUDA(cudaMemcpy2DAsync(d_roots.p, root_stride, roots32, 32, 32, batch, cudaMemcpyHostToDevice, c.stream));
+        zeroed(c, d_leaves, batch * R * 2);
+        zeroed(c, d_alpha, batch);
+        zeroed(c, d_copies, batch * 2);
+        zeroed(c, d_next, batch * R);
+        fri_hash_rows(c, d_vals.as<fe>(), in, rows, d_leaves.p, (int)batch, values_stride);
+        fri_alpha(c, d_roots.p, d_alpha.as<fe>(), d_copies.p, (int)batch, root_stride);
+        fri_fold(c, d_vals.as<fe>(), in, d_next.as<fe>(), rows, d_alpha.as<fe>(), c.twiddle((int)log_N, true), (int)log_N,
+                 host_inv(host_root_of_unity(2)), host_inv(fe_make(4, 0)), (int)batch, values_stride);
+        DG_CUDA(cudaMemcpyAsync(leaves32, d_leaves.p, batch * R * 32, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaMemcpyAsync(alphas16, d_alpha.p, (size_t)batch * 16, cudaMemcpyDeviceToHost, c.stream));
+        DG_CUDA(cudaMemcpyAsync(root_copies32, d_copies.p, (size_t)batch * 32, cudaMemcpyDeviceToHost, c.stream));
+        download(c, next16, d_next, batch * R * 16);
+    });
+}
+
 }  // extern "C"

@@ -556,6 +556,46 @@ int dg_host_periodic_tables(uint8_t *out16 /* 128*23 elements */);
  * "stack aux 1", "stack slot 5", ... (NUL-terminated, truncated to cap); DG_ERR_INVALID for a shape dg_prove rejects or index >= T */
 int dg_host_constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t stack_depth, uint32_t index, char *name, size_t cap);
 
+/* ---- test hooks: not user API --------------------------------------------------------------------------------------------------------
+ * The prover's coefficient-domain stage kernels one call at a time, on host buffers, for differential tests.  Each hook calls the host
+ * function the prover calls, with the power tables, strides and layouts the prover gives it.  Every argument is checked before the
+ * device is touched (DG_ERR_INVALID with a message, also without a GPU); every vector element must be < M.  Output buffers are
+ * zero-filled on the device before the kernels run, so gaps between strided vectors come back as zeros (or, in place, as the input).
+ *
+ * dg_test_syn_div: synthetic division by (x - b_q) of `batch` vectors of len (a power of 2) elements, vector q at q in_stride of in16,
+ * its quotient out[i] = sum_{j>i} (a[j] - [j == 0] sub0[q]) b_q^(j-i-1) at q out_stride of out16; out16 receives (batch - 1) out_stride
+ * + len elements.  in_place: one buffer (in_stride == out_stride).  shared = 0: one point per vector in b16 and a power table per vector
+ * (stage 6); shared = 1: one point b16[0] and one table for all vectors (stage 4). */
+int dg_test_syn_div(const uint8_t *in16, uint8_t *out16, uint32_t batch, uint64_t len, uint64_t in_stride, uint64_t out_stride, int in_place,
+                    const uint8_t *b16, int shared, const uint8_t *sub0_16);
+/* division of 8n coefficients by (x^n - 1) / (x - e), plus add0 and add1 (either may be NULL): vector q of a16 / add0_16 / add1_16 at
+ * q in_stride, of out16 at q out_stride ((batch - 1) out_stride + 8n elements) */
+int dg_test_syn_div_expanded_sum(const uint8_t *a16, const uint8_t *add0_16, const uint8_t *add1_16, uint8_t *out16, uint32_t batch, uint64_t n,
+                                 uint64_t in_stride, uint64_t out_stride, const uint8_t *e16);
+/* col_proof != NULL: cols columns of n = 2^log_n coefficients, column j at point z[col_proof[j]]: out16[2j] = P_j(z), out16[2j + 1] =
+ * P_j(z w_n).  col_proof == NULL: cols == n_z columns of 8n coefficients, out16[2q] = P_q(z_q), out16[2q + 1] = 0.  The powers of every
+ * z come from one table of 8n + 1 entries per point. */
+int dg_test_eval_polys_at(const uint8_t *polys16, uint32_t cols, uint32_t log_n, const uint8_t *z16, uint32_t n_z, const uint32_t *col_proof,
+                          uint8_t *out16);
+/* opened trace rows: for each m < count, P_j(w_N^pos[m]) for the width[m] (1..128) columns j from col[m] on, of cols columns of 2^log_n
+ * coefficients, N = 2^log_N; out16 receives the values of the rows one after another */
+int dg_test_eval_trace_rows(const uint8_t *polys16, uint32_t cols, uint32_t log_n, uint32_t log_N, const uint64_t *pos, const uint32_t *col,
+                            const uint32_t *width, uint32_t count, uint8_t *out16);
+/* the fold-8 extension of `batch` polynomials of 8n coefficients (8n apart in coeffs16) over the cosets [coset0, coset0 + ncosets) of the
+ * domain of 2^(log_n + log_b) points: vector q's coset c at q dst_stride + (c - coset0) n of out16, element k = P(w_N^(k b + c)) */
+int dg_test_lde_fold8(const uint8_t *coeffs16, uint8_t *out16, uint32_t log_n, uint32_t log_b, uint32_t coset0, uint32_t ncosets, uint32_t batch,
+                      uint64_t dst_stride);
+/* interpolation of 8n evaluations given by coset: evals16 holds `batch` vectors of [8][n] (8n apart), e_c[k] = P(w_8n^(8k + c)); out16
+ * receives the 8n coefficients of vector q at q out_stride */
+int dg_test_coset_interp(const uint8_t *evals16, uint8_t *out16, uint32_t log_n, uint32_t batch, uint64_t out_stride);
+/* one FRI layer of `batch` vectors of D = 2^log_d values (values_stride apart), stored natural (log_b = -1) or coset-major with 2^log_b
+ * cosets, on the domain of the powers w_N^(4^depth i), N = 2^log_N.  The rows layout is the one the prover chooses.  leaves32: batch x R
+ * digests (R = D/4) in logical row order; the folding point of vector q is derived from roots32[32 q] (placed root_stride bytes apart on
+ * the device) into alphas16[q], that root copied to root_copies32[32 q]; next16: batch x R folded values in the rows layout's storage
+ * order. */
+int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_stride, uint32_t log_d, int32_t log_b, uint32_t log_N,
+                      const uint8_t *roots32, uint64_t root_stride, uint8_t *leaves32, uint8_t *alphas16, uint8_t *root_copies32, uint8_t *next16);
+
 #ifdef __cplusplus
 }
 #endif

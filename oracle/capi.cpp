@@ -105,6 +105,17 @@ void or_quartic_transpose(const uint8_t *v, uint64_t len, uint64_t stride, uint8
     std::vector<quartic::Q> r = quartic::transpose(in.data(), len, stride);
     memcpy(out, r.data(), r.size() * 64);
 }
+// n cubics (rows of 4 coefficients) evaluated at x
+void or_quartic_evaluate_batch(const uint8_t *polys, uint64_t n, const uint8_t *x, uint8_t *out) {
+    std::vector<quartic::Q> p(n); memcpy(p.data(), polys, n * 64);
+    std::vector<u128> r = quartic::evaluate_batch(p, ld(x));
+    memcpy(out, r.data(), n * 16);
+}
+// field::get_power_series: b^0 .. b^(length - 1)
+void or_power_series(const uint8_t *b, uint64_t length, uint8_t *out) {
+    std::vector<u128> r = field::get_power_series(ld(b), length);
+    memcpy(out, r.data(), length * 16);
+}
 
 // ---- hashing / merkle -------------------------------------------------------------------------------------------
 int or_hash(int id, const uint8_t *in, uint64_t len, uint8_t *out32) {

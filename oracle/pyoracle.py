@@ -51,6 +51,8 @@ def lib():
         L.or_lagrange.argtypes = [u8p, u8p, ctypes.c_uint64, u8p]
         L.or_quartic_interpolate_batch.argtypes = [u8p, u8p, ctypes.c_uint64, u8p]
         L.or_quartic_transpose.argtypes = [u8p, ctypes.c_uint64, ctypes.c_uint64, u8p]
+        L.or_quartic_evaluate_batch.argtypes = [u8p, ctypes.c_uint64, u8p, u8p]
+        L.or_power_series.argtypes = [u8p, ctypes.c_uint64, u8p]
         L.or_hash.restype = ctypes.c_int
         L.or_hash.argtypes = [ctypes.c_int, u8p, ctypes.c_uint64, u8p]
         L.or_merkle_nodes.restype = ctypes.c_int
