@@ -197,6 +197,10 @@ EXPORTS = {
     "dg_test_lde_fold8": [vp, vp, u32, u32, u32, u32, u32, u64],
     "dg_test_coset_interp": [vp, vp, u32, u32, u64],
     "dg_test_fri_layer": [vp, u32, u64, u32, ctypes.c_int32, u32, vp, u64, vp, vp, vp, vp],
+    "dg_test_trace_lde": [vp, u32, u32, u32, u32, u32, u64, ctypes.c_int, vp, vp],
+    "dg_test_hash_trace_rows": [vp, u32, u32, u32, u32, u32, u32, vp, u64, vp],
+    "dg_test_merkle_batch": [vp, u64, u32, vp],
+    "dg_test_constraint_items": [vp, u32, u32, u32, vp],
 }
 VOID_EXPORTS = {"dg_proof_free": [vp], "dg_tree_free": [vp]}
 

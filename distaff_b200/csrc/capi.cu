@@ -1332,4 +1332,103 @@ int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_s
     });
 }
 
+// ---- test hooks: the evaluation-domain stage kernels (stage 1 trace extension, stage 2 trace commitment, stage 5 constraint items) -------
+int dg_test_trace_lde(const uint8_t *regs16, uint32_t cols, uint32_t log_n, uint32_t log_b, uint32_t coset0, uint32_t ncosets, uint64_t col_stride,
+                      int copy_coset0, uint8_t *polys16, uint8_t *ext16) {
+    return guarded([&] {
+        DG_REQUIRE(regs16 && polys16 && ext16, "null buffer");
+        DG_REQUIRE(cols >= 1 && cols <= 65535, "cols must be in 1..65535");
+        DG_REQUIRE(log_b >= 1 && log_b <= 16 && log_n >= 1 && log_n + log_b <= 30, "log_b must be in 1..16 and log_n in 1..30 - log_b");
+        const uint64_t n = 1ULL << log_n, b = 1ULL << log_b;
+        DG_REQUIRE(ncosets >= 1 && coset0 < b && ncosets <= b - coset0, "coset range out of bounds");
+        const uint64_t out_n = strided_span(cols, col_stride, ncosets * n, "col_stride");
+        require_canonical(regs16, cols * n, 1, "register element");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_regs, d_polys, d_ext;
+        upload(c, d_regs, regs16, cols * n);
+        zeroed(c, d_polys, cols * n);
+        zeroed(c, d_ext, out_n);
+        // stage 1: interpolate the register columns, then extend them onto the coset range (coset 0 copied from the registers when given)
+        ntt_batch(c, d_regs.as<fe>(), d_polys.as<fe>(), (int)log_n, (int)cols, n, n, true);
+        extend_trace_columns(c, d_polys.as<fe>(), copy_coset0 ? d_regs.as<fe>() : nullptr, d_ext.as<fe>(), (int)cols, (int)log_n, (int)log_b,
+                             col_stride, coset0, ncosets);
+        DG_CUDA(cudaMemcpyAsync(polys16, d_polys.p, cols * n * 16, cudaMemcpyDeviceToHost, c.stream));
+        download(c, ext16, d_ext, out_n * 16);
+    });
+}
+
+int dg_test_hash_trace_rows(const uint8_t *ext16, uint32_t total_cols, uint32_t log_n, uint32_t log_blowup, uint32_t c0, uint32_t nc, uint32_t batch,
+                            const uint32_t *col_table, uint64_t leaf_stride, uint8_t *leaves32) {
+    return guarded([&] {
+        DG_REQUIRE(ext16 && leaves32, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(log_blowup <= 16 && log_n >= 1 && log_n + log_blowup <= 30, "log_blowup must be in 0..16 and log_n in 1..30 - log_blowup");
+        const uint64_t n = 1ULL << log_n, all = n << log_blowup, rows = (uint64_t)nc * n;
+        DG_REQUIRE(nc >= 1 && c0 < (1ULL << log_blowup) && nc <= (1ULL << log_blowup) - c0, "coset range out of bounds");
+        DG_REQUIRE(total_cols >= 1 && total_cols <= 65535, "total_cols must be in 1..65535");
+        uint32_t w = 0;
+        if (col_table) {
+            for (uint32_t q = 0; q < batch; q++)
+                DG_REQUIRE(col_table[2 * q + 1] >= 1 && col_table[2 * q + 1] <= 127 && col_table[2 * q] < total_cols &&
+                               col_table[2 * q + 1] <= total_cols - col_table[2 * q],
+                           "matrix " + std::to_string(q) + ": columns out of range (width 1..127)");
+        } else {
+            DG_REQUIRE(total_cols % batch == 0, "without a column table the batch's matrices share total_cols evenly");
+            w = total_cols / batch;
+            DG_REQUIRE(w >= 1 && w <= 127, "width must be in 1..127");
+        }
+        DG_REQUIRE(leaf_stride == 0 || (leaf_stride >= all && leaf_stride <= (1ULL << 32)), "leaf_stride must be 0 or in 2^(log_n + log_blowup)..2^32");
+        const uint64_t stride = leaf_stride ? leaf_stride : all, leaves = (batch - 1) * stride + all;
+        require_canonical(ext16, total_cols * rows, 1, "extension element");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_ext, d_table, d_leaves;
+        upload(c, d_ext, ext16, total_cols * rows);
+        if (col_table) {
+            d_table.alloc((size_t)batch * 8);
+            DG_CUDA(cudaMemcpyAsync(d_table.p, col_table, (size_t)batch * 8, cudaMemcpyHostToDevice, c.stream));
+        }
+        zeroed(c, d_leaves, 2 * leaves);
+        // stage 2 (prove_core's hash_chunk): the rows of the cosets [c0, c0 + nc) of every matrix, column stride nc n
+        hash_trace_rows(c, d_ext.as<fe>(), d_leaves.p, (int)w, (int)log_n, (int)log_blowup, (int)batch, (unsigned long long)w * rows, c0, nc,
+                        leaf_stride, col_table ? d_table.as<uint2>() : nullptr);
+        download(c, leaves32, d_leaves, leaves * 32);
+    });
+}
+
+int dg_test_merkle_batch(const uint8_t *leaves32, uint64_t L, uint32_t batch, uint8_t *nodes32) {
+    return guarded([&] {
+        DG_REQUIRE(leaves32 && nodes32, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(is_pow2(L) && L >= 2 && L <= (1ULL << 30), "L must be a power of 2 in 2..2^30");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_leaves, d_nodes;
+        upload(c, d_leaves, leaves32, 2 * batch * L);
+        zeroed(c, d_nodes, 2 * batch * L);
+        // stages 2 and 5: the K trees of a batch, one launch per level for all of them
+        merkle_build(c, d_leaves.p, d_nodes.p, L, (int)batch);
+        download(c, nodes32, d_nodes, batch * L * 32);
+    });
+}
+
+int dg_test_constraint_items(const uint8_t *evals16, uint32_t log_n, uint32_t log_nc, uint32_t batch, uint8_t *items32) {
+    return guarded([&] {
+        DG_REQUIRE(evals16 && items32, "null buffer");
+        require_batch(batch);
+        DG_REQUIRE(log_nc >= 2 && log_nc <= 16 && log_n >= 1 && log_n + log_nc <= 30, "log_nc must be in 2..16 and log_n in 1..30 - log_nc");
+        const uint64_t slab = 1ULL << (log_n + log_nc), items = slab / 4;
+        require_canonical(evals16, batch * slab, 1, "evaluation");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        DevBuf d_evals, d_items;
+        upload(c, d_evals, evals16, batch * slab);
+        zeroed(c, d_items, 2 * batch * items);
+        // stage 5: the first level of the constraint tree of every slab
+        constraint_items_local(c, d_evals.as<fe>(), (int)log_n, (int)log_nc, d_items.p, (int)batch);
+        download(c, items32, d_items, batch * items * 32);
+    });
+}
+
 }  // extern "C"

@@ -87,20 +87,6 @@ void debug_dump_host(const char *name, const void *host, size_t bytes) {
     fclose(f);
 }
 
-// Trace LDE of `cols` columns (polynomials `polys`, stride n) onto the cosets [c0, c0 + nc), written to ext (column stride N_loc).
-// Coset 0 is P(w_n^k), which is register row k itself (polys = iNTT(regs) exactly): when the range starts at coset 0 and the registers
-// are on the device (`regs`, stride n; null if not), slab 0 is copied from them and only the other cosets are transformed.
-void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
-                          unsigned nc) {
-    const size_t n = (size_t)1 << log_n;
-    if (c0 != 0 || !regs) {
-        lde_batch(c, polys, ext, log_n, log_b, 1, cols, n, N_loc, c0, nc);
-        return;
-    }
-    if (nc > 1) lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
-    DG_CUDA(cudaMemcpy2DAsync(ext, N_loc * sizeof(fe), regs, n * sizeof(fe), n * sizeof(fe), cols, cudaMemcpyDeviceToDevice, c.stream));
-}
-
 void require_extension_factor(uint64_t b) {
     DG_REQUIRE(b >= 16 && b <= 256 && (b & (b - 1)) == 0, "extension_factor must be a power of 2 between 16 and 256");
 }
@@ -115,6 +101,18 @@ struct FriLayerDev {
 };
 
 }  // namespace
+
+// prover.h; dg_test_trace_lde calls it as stage 1 does
+void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
+                          unsigned nc) {
+    const size_t n = (size_t)1 << log_n;
+    if (c0 != 0 || !regs) {
+        lde_batch(c, polys, ext, log_n, log_b, 1, cols, n, N_loc, c0, nc);
+        return;
+    }
+    if (nc > 1) lde_batch(c, polys, ext + n, log_n, log_b, 1, cols, n, N_loc, 1, nc - 1);
+    DG_CUDA(cudaMemcpy2DAsync(ext, N_loc * sizeof(fe), regs, n * sizeof(fe), n * sizeof(fe), cols, cudaMemcpyDeviceToDevice, c.stream));
+}
 
 // Upload of a host trace, overlapped with stage 1: column chunk i is extended as soon as its copy has landed.
 //   * pinned (page-locked / registered) columns: cudaMemcpyAsync straight from the caller's memory on the copy stream;

@@ -102,6 +102,11 @@ size_t proof_footprint(uint32_t w, uint64_t n, uint32_t b, uint32_t chunk);
 // copies `cols` host register columns of n elements each to d_regs (column stride n) by the prover's upload path (pinned columns DMA'd
 // directly, pageable ones staged through the library's pinned slots) and orders c.stream after the copies
 void upload_trace_columns(Context &c, fe *d_regs, const uint8_t *const *host_cols, int cols, uint64_t n);
+// Stage 1's trace LDE of `cols` columns (polynomials `polys`, stride n) onto the cosets [c0, c0 + nc), written to ext (column stride N_loc).
+// Coset 0 is P(w_n^k), which is register row k itself (polys = iNTT(regs) exactly): when the range starts at coset 0 and the registers
+// are on the device (`regs`, stride n; null if not), slab 0 is copied from them and only the other cosets are transformed.
+void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
+                          unsigned nc);
 
 // the trace check (check.cu): per trace, which transition constraints fail at which steps and which boundary registers are wrong.
 // d_regs: [count][width][length] on the device, or null with host_cols (count * width column pointers) to upload; program_hashes32

@@ -595,6 +595,27 @@ int dg_test_coset_interp(const uint8_t *evals16, uint8_t *out16, uint32_t log_n,
  * order. */
 int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_stride, uint32_t log_d, int32_t log_b, uint32_t log_N,
                       const uint8_t *roots32, uint64_t root_stride, uint8_t *leaves32, uint8_t *alphas16, uint8_t *root_copies32, uint8_t *next16);
+/* The evaluation-domain stages the same way.
+ * dg_test_trace_lde: stage 1.  `cols` register columns of n = 2^log_n elements (n apart in regs16) are interpolated into polys16 (cols x n
+ * coefficients), then extended onto the cosets [coset0, coset0 + ncosets) of the domain of N = n 2^log_b points (log_b 1..16, log_n +
+ * log_b <= 30): column j's coset c at j col_stride + (c - coset0) n of ext16, element k = P_j(w_N^(k 2^log_b + c)); ext16 receives (cols -
+ * 1) col_stride + ncosets n elements.  copy_coset0 = 1: coset 0 (when in the range) is copied from the registers, as the prover does for a
+ * trace on the device; 0: every coset is transformed. */
+int dg_test_trace_lde(const uint8_t *regs16, uint32_t cols, uint32_t log_n, uint32_t log_b, uint32_t coset0, uint32_t ncosets, uint64_t col_stride,
+                      int copy_coset0, uint8_t *polys16, uint8_t *ext16);
+/* stage 2: the rows of the cosets [c0, c0 + nc) of a 2^log_blowup-coset extension, given as total_cols columns of nc n elements
+ * ([column][c - c0][k], n = 2^log_n).  col_table (may be NULL): `batch` (first column, width) pairs, one matrix per pair (widths 1..127);
+ * NULL: `batch` matrices of total_cols / batch columns one after another.  Matrix q's row of coset c at step k is leaf (k << log_blowup) + c
+ * of the q-th run of leaves, leaf_stride digests apart (0: 2^(log_n + log_blowup)); leaves32 receives (batch - 1) stride + 2^(log_n +
+ * log_blowup) digests, those of cosets outside the range zero. */
+int dg_test_hash_trace_rows(const uint8_t *ext16, uint32_t total_cols, uint32_t log_n, uint32_t log_blowup, uint32_t c0, uint32_t nc, uint32_t batch,
+                            const uint32_t *col_table, uint64_t leaf_stride, uint8_t *leaves32);
+/* stages 2 and 5: `batch` Merkle trees of L leaves (L a power of 2 in 2..2^30), tree q's leaves and heap (L digests, nodes[0] = 0, root =
+ * nodes[1]) at q L digests */
+int dg_test_merkle_batch(const uint8_t *leaves32, uint64_t L, uint32_t batch, uint8_t *nodes32);
+/* stage 5: the first level of the constraint tree of `batch` slabs of 2^log_nc cosets (log_nc >= 2) of n = 2^log_n evaluations ([c][k],
+ * n 2^log_nc elements apart): item (k << (log_nc - 2)) + c4 = blake3(ev[4 c4][k], ..., ev[4 c4 + 3][k]), n 2^(log_nc - 2) digests per slab */
+int dg_test_constraint_items(const uint8_t *evals16, uint32_t log_n, uint32_t log_nc, uint32_t batch, uint8_t *items32);
 
 #ifdef __cplusplus
 }

@@ -121,6 +121,19 @@ void or_power_series(const uint8_t *b, uint64_t length, uint8_t *out) {
 int or_hash(int id, const uint8_t *in, uint64_t len, uint8_t *out32) {
     try { hash_by_id(id)(in, len, out32); return 0; } catch (...) { return -1; }
 }
+// blake3 of every row of a column-major [w][rows] matrix, as the prover's trace commitment hashes the rows of the extension
+void or_hash_rows(const uint8_t *cols, uint64_t w, uint64_t rows, uint8_t *out32) {
+    const int T = fft::host_threads();
+    #pragma omp parallel num_threads(T) if (T > 1)
+    {
+        std::vector<u128> row(w);
+        #pragma omp for
+        for (uint64_t i = 0; i < rows; i++) {
+            for (uint64_t j = 0; j < w; j++) memcpy(&row[j], cols + 16 * (j * rows + i), 16);
+            blake3((const uint8_t *)row.data(), w * 16, out32 + 32 * i);
+        }
+    }
+}
 // nodes_out: n_leaves * 32 bytes (heap layout, nodes[0] = 0, root = nodes[1])
 int or_merkle_nodes(int id, const uint8_t *leaves, uint64_t n, uint8_t *nodes_out) {
     try {

@@ -55,6 +55,7 @@ def lib():
         L.or_power_series.argtypes = [u8p, ctypes.c_uint64, u8p]
         L.or_hash.restype = ctypes.c_int
         L.or_hash.argtypes = [ctypes.c_int, u8p, ctypes.c_uint64, u8p]
+        L.or_hash_rows.argtypes = [u8p, ctypes.c_uint64, ctypes.c_uint64, u8p]
         L.or_merkle_nodes.restype = ctypes.c_int
         L.or_merkle_nodes.argtypes = [ctypes.c_int, u8p, ctypes.c_uint64, u8p]
         L.or_merkle_prove_batch.restype = ctypes.c_int64
