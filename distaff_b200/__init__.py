@@ -17,10 +17,13 @@ Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.HasherTree(leaves)               <->  a Merkle tree of utils::hasher::digest, built on the GPU, with its smpath / pmpath inputs
     distaff_b200.prove_membership(tree, indexes)  <->  execute_batch of the smpath or pmpath program for leaves of a HasherTree
     distaff_b200.MerkleTree(leaves, hash)         <->  crypto::MerkleTree kept in device memory: paths of many leaves per call, leaf updates
+    tree.prove_batch(indexes)                     <->  MerkleTree::prove_batch: a BatchMerkleProof gathered on the GPU
+    distaff_b200.merkle_verify_paths / _batch     <->  MerkleTree::verify / verify_batch of many paths or batch proofs in one call
 The compute path is hand-written CUDA behind the C-ABI of include/distaff_gpu.h; there is no CPU fallback.
 """
 from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, prove_batch_device, prove_traces, prove_traces_device, verify, verify_batch, execute, ntt, intt, lde,  # noqa: F401
                   merkle_build, hash_rows, hash64, find_pow_nonce, field_op, field_dot, eval_transitions, TraceReport, check_trace, check_traces,
                   check_traces_device, constraint_name, set_memory_limit, memory_usage, plan_prove, ProgramInputs, trace_batch, trace_shapes,
                   execute_batch, trace_programs, execute_programs, group_traces, trace_one, execute_one,
-                  trace_many, execute_many, HasherTree, smpath_program, pmpath_program, prove_membership, MerkleTree)
+                  trace_many, execute_many, HasherTree, smpath_program, pmpath_program, prove_membership, MerkleTree,
+                  BatchMerkleProof, merkle_verify_paths, merkle_verify_batch)

@@ -985,6 +985,35 @@ class MerkleTree:
         backend.check(backend.lib().dg_tree_update(self._handle(), idx.ctypes.data if len(idx) else None, raw, len(idx), root))
         return root.raw
 
+    def prove_batch(self, indexes):
+        """MerkleTree::prove_batch (merkle.rs:64-124): the compressed opening of many leaves as one BatchMerkleProof, values in request
+        order.  An index >= len(tree) or a repeated index raises DgError with the crate's message."""
+        idx = self._indexes(indexes)
+        ptr = idx.ctypes.data if len(idx) else None
+        n = ctypes.c_size_t(0)
+        backend.check(backend.lib().dg_tree_prove_batch(self._handle(), ptr, len(idx), None, 0, ctypes.byref(n)))
+        out = ctypes.create_string_buffer(n.value)
+        backend.check(backend.lib().dg_tree_prove_batch(self._handle(), ptr, len(idx), out, n.value, ctypes.byref(n)))
+        return BatchMerkleProof.from_bytes(out.raw)
+
+    @staticmethod
+    def verify(root, index, path, hash="blake3"):
+        """MerkleTree::verify (merkle.rs:127-151): whether `path` (2 to 64 entries of 32 bytes) leads leaf `index` to `root`.  Only the low
+        len(path) - 1 bits of the index are read, as in the reference."""
+        (r,) = merkle_verify_paths(root, [index], [path], hash)
+        if isinstance(r, backend.DgError):
+            raise r
+        return r
+
+    @staticmethod
+    def verify_batch(root, indexes, proof, hash="blake3"):
+        """MerkleTree::verify_batch (merkle.rs:154-263) of a BatchMerkleProof (or its bytes); where the crate panics this raises DgError
+        with the crate's message."""
+        (r,) = merkle_verify_batch([(root, indexes, proof)], hash)
+        if isinstance(r, backend.DgError):
+            raise r
+        return r
+
     def leaves(self):
         out = ctypes.create_string_buffer(32 * self._n)
         backend.check(backend.lib().dg_tree_read(self._handle(), out, None))
@@ -1037,6 +1066,115 @@ class MerkleTree:
             self.close()
         except Exception:
             pass
+
+
+class BatchMerkleProof:
+    """crypto::BatchMerkleProof (merkle.rs:14-18): values (32-byte bytes, one per requested index in request order), nodes (one list of
+    32-byte bytes per normalised index) and depth.  to_bytes() / from_bytes() are its bincode: u64 count + 32 B per value; u64 count,
+    then per slot u64 count + 32 B per node; u8 depth."""
+
+    def __init__(self, values, nodes, depth):
+        self.values = [bytes(v) for v in values]
+        self.nodes = [[bytes(v) for v in slot] for slot in nodes]
+        self.depth = int(depth)
+
+    def to_bytes(self):
+        u64 = lambda n: int(n).to_bytes(8, "little")
+        return (u64(len(self.values)) + b"".join(self.values) + u64(len(self.nodes)) +
+                b"".join(u64(len(slot)) + b"".join(slot) for slot in self.nodes) + bytes([self.depth]))
+
+    @classmethod
+    def from_bytes(cls, data):
+        data, at = bytes(data), 0
+
+        def take(n):
+            nonlocal at
+            if len(data) - at < n:
+                raise ValueError("not a BatchMerkleProof: the bytes end early")
+            at += n
+            return data[at - n:at]
+
+        def digests():
+            n = int.from_bytes(take(8), "little")
+            if n > (len(data) - at) // 32:
+                raise ValueError("not a BatchMerkleProof: a length the bytes cannot hold")
+            return [take(32) for _ in range(n)]
+        values = digests()
+        n = int.from_bytes(take(8), "little")
+        if n > (len(data) - at) // 8:
+            raise ValueError("not a BatchMerkleProof: a length the bytes cannot hold")
+        nodes = [digests() for _ in range(n)]
+        depth = take(1)[0]
+        if at != len(data):
+            raise ValueError("not a BatchMerkleProof: trailing bytes")
+        return cls(values, nodes, depth)
+
+    def __eq__(self, other):
+        return isinstance(other, BatchMerkleProof) and (self.values, self.nodes, self.depth) == (other.values, other.nodes, other.depth)
+
+    def __repr__(self):
+        return f"BatchMerkleProof({len(self.values)} values, {sum(map(len, self.nodes))} nodes in {len(self.nodes)} slots, depth {self.depth})"
+
+
+def _hash_id(hash):
+    if hash not in HASH_IDS:
+        raise ValueError(f"hash is one of {', '.join(HASH_IDS)}, not {hash!r}")
+    return HASH_IDS[hash]
+
+
+def _verdicts(status):
+    """True (accepted), False (rejected) or the DgError of a malformed entry / a panic of the reference, per entry of the last call"""
+    return [True if e is None else False if e.code == -6 else e for e in _messages(status)]
+
+
+def merkle_verify_paths(roots, indexes, paths, hash="blake3"):
+    """MerkleTree::verify (merkle.rs:127-151) of many paths in one dg_merkle_verify_paths call.  `roots` is one 32-byte root or one per path;
+    `paths` is what MerkleTree.paths returns (lists of 32-byte entries, all of one length) or a uint8 array of shape (K, entries, 32).
+    Returns a list per path: True, False, or a DgError for a path with an element >= M (hashes other than blake3)."""
+    if isinstance(paths, np.ndarray):
+        if paths.dtype != np.uint8 or paths.ndim != 3 or paths.shape[2] != 32:
+            raise ValueError("a path array is uint8 of shape (K, entries, 32)")
+        raw = np.ascontiguousarray(paths)
+        k, entries = paths.shape[0], paths.shape[1]
+    else:
+        paths = [[bytes(e) for e in p] for p in paths]
+        k, entries = len(paths), len(paths[0]) if paths else 2
+        if any(len(p) != entries for p in paths) or any(len(e) != 32 for p in paths for e in p):
+            raise ValueError("paths have one number of entries, each of 32 bytes")
+        raw = np.frombuffer(b"".join(e for p in paths for e in p), dtype=np.uint8)
+    idx = MerkleTree._indexes(indexes)
+    if len(idx) != k:
+        raise ValueError(f"{len(idx)} indexes and {k} paths")
+    roots = bytes(roots) if isinstance(roots, (bytes, bytearray, memoryview)) else b"".join(bytes(r) for r in roots)
+    if len(roots) % 32:
+        raise ValueError("roots are 32 bytes each")
+    if k == 0:
+        return []
+    status = (ctypes.c_int * k)()
+    backend.check(backend.lib().dg_merkle_verify_paths(_hash_id(hash), roots, len(roots) // 32, idx.ctypes.data, raw.ctypes.data, entries, k,
+                                                       status))
+    return _verdicts(status)
+
+
+def merkle_verify_batch(items, hash="blake3"):
+    """MerkleTree::verify_batch (merkle.rs:154-263) of many batch proofs in one dg_merkle_verify_batch call.  items: (root, indexes, proof),
+    proof a BatchMerkleProof or its bytes.  Returns a list per item: True, False, or a DgError where the reference panics or the input is
+    malformed (bytes that are not one BatchMerkleProof, an element >= M for hashes other than blake3)."""
+    items = list(items)
+    k = len(items)
+    if k == 0:
+        return []
+    roots = b"".join(bytes(r) for r, _, _ in items)
+    if len(roots) != 32 * k:
+        raise ValueError("roots are 32 bytes each")
+    idx = [MerkleTree._indexes(i) for _, i, _ in items]
+    data = [p.to_bytes() if isinstance(p, BatchMerkleProof) else bytes(p) for _, _, p in items]
+    status = (ctypes.c_int * k)()
+    backend.check(backend.lib().dg_merkle_verify_batch(_hash_id(hash), k, roots, (backend.vp * k)(*[a.ctypes.data if len(a) else None for a in idx]),
+                                                       (backend.u32 * k)(*[len(a) for a in idx]),
+                                                       (backend.vp * k)(*[ctypes.cast(ctypes.c_char_p(d), backend.vp) for d in data]),
+                                                       (ctypes.c_size_t * k)(*[len(d) for d in data]), status))
+    return _verdicts(status)
 
 
 def hash_rows(columns):

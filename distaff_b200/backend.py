@@ -157,6 +157,10 @@ EXPORTS = {
     "dg_tree_paths": [vp, vp, u32, vp],
     "dg_tree_update": [vp, vp, vp, u32, vp],
     "dg_tree_read": [vp, vp, vp],
+    "dg_tree_prove_batch": [vp, vp, u32, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
+    "dg_merkle_verify_paths": [ctypes.c_int, vp, u32, vp, vp, u32, u32, ctypes.POINTER(ctypes.c_int)],
+    "dg_merkle_verify_batch": [ctypes.c_int, u32, vp, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_size_t),
+                               ctypes.POINTER(ctypes.c_int)],
     "dg_find_pow_nonce": [vp, u32, ctypes.POINTER(u64), vp],
     "dg_field_op": [ctypes.c_int, ctypes.c_int, vp, vp, vp, u64],
     "dg_field_dot": [vp, vp, vp, u64, u32],

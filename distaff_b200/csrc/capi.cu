@@ -421,6 +421,141 @@ void dg_tree_free(dg_tree_t *tree) {
     });
 }
 
+// ---- batch proofs of a tree, and verification of paths and batch proofs (tree.cu) ------------------------------------------------------
+// prove_batch's panics in the crate's order: map_indexes asserts index <= L, then that no index repeats; an index of L then fails the
+// slice index, named here as map_indexes names the others
+static void require_batch_indexes(const uint64_t *indexes, uint32_t count, uint64_t L) {
+    for (uint32_t k = 0; k < count; k++)
+        if (indexes[k] > L) throw Error(DG_ERR_INVALID, "invalid index " + std::to_string(indexes[k]));
+    std::vector<uint64_t> sorted(indexes, indexes + count);
+    std::sort(sorted.begin(), sorted.end());
+    if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end()) throw Error(DG_ERR_INVALID, "repeating indexes detected");
+    if (count && sorted.back() == L) throw Error(DG_ERR_INVALID, "invalid index " + std::to_string(L));
+}
+int dg_tree_prove_batch(const dg_tree_t *tree, const uint64_t *indexes, uint32_t count, uint8_t *proof_out, size_t cap, size_t *len) {
+    return guarded([&] {
+        DG_REQUIRE(tree && len, "null argument");
+        DG_REQUIRE(count == 0 || indexes, "null buffer");
+        const Tree &t = *(const Tree *)tree;
+        require_batch_indexes(indexes, count, t.L);
+        const fs::BatchPlan plan = fs::plan_batch_proof(std::vector<uint64_t>(indexes, indexes + count), t.L);
+        *len = batch_proof_len(plan);
+        if (!proof_out) return;
+        if (cap < *len) throw Error(DG_ERR_INVALID, "proof buffer too small: the proof has " + std::to_string(*len) + " bytes");
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        tree_prove_batch(c, t, plan, proof_out);
+    });
+}
+
+// the first of n little-endian u128 elements that is >= M, or -1
+static int64_t first_noncanonical(const uint8_t *elements, size_t n) {
+    for (size_t k = 0; k < n; k++) {
+        uint64_t lo, hi;
+        memcpy(&lo, elements + 16 * k, 8);
+        memcpy(&hi, elements + 16 * k + 8, 8);
+        if (hi == DG_M_HI && lo >= DG_M_LO) return (int64_t)k;
+    }
+    return -1;
+}
+static std::string noncanonical_message(const std::string &what, int64_t k) {
+    return what + " element " + std::to_string(k) + " is not a field element (>= M)";
+}
+static void require_hash_id(int hash) {
+    DG_REQUIRE(hash >= 0 && hash <= 3, "hash id must be 0 (blake3), 1 (rescue), 2 (poseidon) or 3 (hasher)");
+}
+int dg_merkle_verify_paths(int hash, const uint8_t *roots32, uint32_t n_roots, const uint64_t *indexes, const uint8_t *paths32,
+                           uint32_t entries, uint32_t count, int *status) {
+    return guarded([&] {
+        require_hash_id(hash);
+        DG_REQUIRE(entries >= 2 && entries <= 64, "a path has 2 to 64 entries");
+        DG_REQUIRE(n_roots == 1 || n_roots == count, "n_roots must be 1 or count");
+        DG_REQUIRE(roots32 && indexes && paths32 && status, "null array");
+        t_batch_messages.assign(count, std::string());
+        if (count == 0) return;
+        // the algebraic hashes take field elements only: a path with an entry element >= M is malformed input.  Its digests are computed with
+        // the others (the kernels' addresses do not depend on the values) and its verdict is replaced.
+        std::vector<uint8_t> valid(count, 1);
+        if (hash != DG_HASH_BLAKE3)
+            for (uint32_t k = 0; k < count; k++) {
+                const int64_t e = first_noncanonical(paths32 + (size_t)32 * entries * k, 2 * (size_t)entries);
+                if (e < 0) continue;
+                valid[k] = 0;
+                t_batch_messages[k] = noncanonical_message("entry " + std::to_string(e / 2), e % 2);
+            }
+        std::vector<uint8_t> accepted(count);
+        {
+            Context &c = ctx();
+            std::lock_guard<std::mutex> lk(c.mu);
+            merkle_verify_paths(c, hash, roots32, n_roots != 1, indexes, paths32, entries, count, accepted.data());
+        }
+        for (uint32_t k = 0; k < count; k++) {
+            status[k] = !valid[k] ? DG_ERR_INVALID : accepted[k] ? DG_OK : DG_ERR_REJECTED;
+            if (valid[k] && !accepted[k]) t_batch_messages[k] = "the path does not lead to the root";
+        }
+    });
+}
+int dg_merkle_verify_batch(int hash, uint32_t count, const uint8_t *roots32, const uint64_t *const *indexes, const uint32_t *n_indexes,
+                           const uint8_t *const *proofs, const size_t *proof_lens, int *status) {
+    return guarded([&] {
+        require_hash_id(hash);
+        DG_REQUIRE(roots32 && indexes && n_indexes && proofs && proof_lens && status, "null array");
+        t_batch_messages.assign(count, std::string());
+        // host: parse, check the elements, plan; the entries decided here never reach the device
+        std::vector<BatchMerkleProof> parsed(count);
+        std::vector<BatchCheck> checks;
+        std::vector<uint32_t> of;
+        std::vector<const uint8_t *> roots;
+        for (uint32_t i = 0; i < count; i++) {
+            std::string &msg = t_batch_messages[i];
+            BatchMerkleProof &p = parsed[i];
+            status[i] = DG_ERR_INVALID;
+            if ((n_indexes[i] && !indexes[i]) || (proof_lens[i] && !proofs[i])) { msg = "null indexes or proof bytes"; continue; }
+            if (!read_batch_proof(proofs[i], proof_lens[i], p)) {
+                msg = "malformed proof bytes (bincode layout of BatchMerkleProof, merkle.rs:14-18)";
+                continue;
+            }
+            if (p.depth > 63) { msg = "attempt to multiply with overflow"; continue; }           // usize::pow(2, depth)
+            if (hash != DG_HASH_BLAKE3) {
+                for (size_t v = 0; v < p.values.size() && msg.empty(); v++) {
+                    const int64_t e = first_noncanonical(p.values[v].data(), 2);
+                    if (e >= 0) msg = noncanonical_message("value " + std::to_string(v), e);
+                }
+                for (size_t s = 0; s < p.nodes.size() && msg.empty(); s++)
+                    for (size_t j = 0; j < p.nodes[s].size() && msg.empty(); j++) {
+                        const int64_t e = first_noncanonical(p.nodes[s][j].data(), 2);
+                        if (e >= 0) msg = noncanonical_message("node " + std::to_string(j) + " of slot " + std::to_string(s), e);
+                    }
+                if (!msg.empty()) continue;
+            }
+            std::vector<uint32_t> bases;
+            uint32_t next = (uint32_t)p.values.size();
+            for (auto &slot : p.nodes) { bases.push_back(next); next += (uint32_t)slot.size(); }
+            MerklePlan plan = plan_verify_batch(std::vector<uint64_t>(indexes[i], indexes[i] + n_indexes[i]), p.depth, p.values.size(), 0, p.nodes,
+                                                bases, next, 0, 63);
+            if (!plan.ok) {
+                status[i] = plan.panic ? DG_ERR_INVALID : DG_ERR_REJECTED;
+                msg = plan.why;
+                continue;
+            }
+            checks.push_back(BatchCheck{&p, std::move(plan)});
+            of.push_back(i);
+            roots.push_back(roots32 + (size_t)32 * i);
+        }
+        if (checks.empty()) return;
+        std::vector<uint8_t> accepted(checks.size());
+        {
+            Context &c = ctx();
+            std::lock_guard<std::mutex> lk(c.mu);
+            merkle_verify_batch(c, hash, checks, roots.data(), accepted.data());
+        }
+        for (size_t j = 0; j < checks.size(); j++) {
+            status[of[j]] = accepted[j] ? DG_OK : DG_ERR_REJECTED;
+            if (!accepted[j]) t_batch_messages[of[j]] = "the proof does not lead to the root";
+        }
+    });
+}
+
 int dg_hash_rows(const uint8_t *columns, uint32_t width, uint64_t rows, uint8_t *digests) {
     return guarded([&] {
         Context &c = ctx();

@@ -100,4 +100,10 @@ bool read_proof(const uint8_t *bytes, size_t len, StarkProof &P) {
     return r.ok && r.p == r.end;
 }
 
+bool read_batch_proof(const uint8_t *bytes, size_t len, BatchMerkleProof &P) {
+    Reader r(bytes, len);
+    P.values = r.dvec(); P.nodes = r.dvv(); P.depth = r.u8();
+    return r.ok && r.p == r.end;
+}
+
 }  // namespace dg

@@ -51,6 +51,8 @@ struct StarkProof {
 std::vector<uint8_t> write_proof(const StarkProof &P);
 // false when the bytes are not exactly one StarkProof: short input, trailing bytes, or a Vec length the remaining bytes cannot hold
 bool read_proof(const uint8_t *bytes, size_t len, StarkProof &P);
+// one BatchMerkleProof {values, nodes, depth} alone (MerkleTree::prove_batch / verify_batch), with read_proof's rule
+bool read_batch_proof(const uint8_t *bytes, size_t len, BatchMerkleProof &P);
 
 // A proof the library returns (dg_proof_t): its bytes and the commitments the C-ABI exposes
 struct Proof {

@@ -9,7 +9,7 @@
 //   prepare (host, proof by proof in input order): parse, option and PoW checks, query positions, every Fiat-Shamir draw (z, constraint
 //      and composition coefficients, FRI folding points), and every batch-Merkle verification as a plan of (left, right, out) hashing
 //      steps per tree level -- pure index logic, following verify_batch statement by statement, including its use of the current
-//      level's position as the slot of `proof.nodes`.  A proof decided here (malformed bytes, failed PoW, ...) skips the device.
+//      level's position as the slot of `proof.nodes` (plan_verify_batch, tree.cu).  A proof decided here (malformed bytes, failed PoW, ...) skips the device.
 //   device (per group of proofs: one upload, one synchronise), each step one launch for the whole group:
 //      1. BLAKE3 of the opened trace rows (one launch per row width) and of the opened FRI rows (the Merkle leaves),
 //      2. all Merkle plans of all proofs (one block per tree, one barrier per level),
@@ -32,110 +32,11 @@
 #include "proof.h"
 #include "prover.h"
 #include "shard.h"
+#include "tree.h"
 
 namespace dg {
 
 namespace {
-
-// ---- batch Merkle verification as a hashing plan (merkle.rs:154-263) -------------------------------------------------------------
-// pool slots: the caller lays out the proof's values and nodes in a pool of 32-byte digests; computed parents get fresh slots
-struct MerklePlan {
-    std::vector<uint32_t> ops;            // (left, right, out) pool indices
-    std::vector<uint32_t> level_start;    // op index where each level starts (+ final end)
-    uint32_t root_slot = 0;
-    bool ok = false;
-};
-MerklePlan plan_verify_batch(const std::vector<uint64_t> &indexes_in, int depth, size_t n_values, uint32_t values_base,
-                             const std::vector<std::vector<Digest>> &nodes, const std::vector<uint32_t> &nodes_base, uint32_t &next_slot) {
-    MerklePlan plan;
-    if (depth < 1 || depth > 40) return plan;
-    const uint64_t offset = 1ULL << depth;
-    std::map<uint64_t, uint64_t> index_map;
-    for (size_t i = 0; i < indexes_in.size(); i++) {
-        if (indexes_in[i] > offset - 1) return plan;             // the reference asserts here (map_indexes)
-        index_map[indexes_in[i]] = i;
-    }
-    if (index_map.size() != indexes_in.size()) return plan;
-    std::set<uint64_t> norm;
-    for (uint64_t idx : indexes_in) norm.insert(idx - (idx & 1));
-    std::vector<uint64_t> indexes(norm.begin(), norm.end());
-    if (indexes.size() != nodes.size()) return plan;
-
-    std::map<uint64_t, uint32_t> v;                              // node index -> pool slot of its computed hash
-    std::vector<uint64_t> next;
-    std::vector<size_t> ptrs;
-    plan.level_start.push_back(0);
-    for (size_t i = 0; i < indexes.size(); i++) {
-        const uint64_t index = indexes[i];
-        auto i1 = index_map.find(index), i2 = index_map.find(index + 1);
-        uint32_t left, right;
-        if (i1 != index_map.end()) {
-            if (n_values <= i1->second) return plan;
-            left = values_base + (uint32_t)i1->second;
-            if (i2 != index_map.end()) {
-                if (n_values <= i2->second) return plan;
-                right = values_base + (uint32_t)i2->second;
-                ptrs.push_back(0);
-            } else {
-                if (nodes[i].size() < 1) return plan;
-                right = nodes_base[i];
-                ptrs.push_back(1);
-            }
-        } else {
-            if (nodes[i].size() < 1) return plan;
-            left = nodes_base[i];
-            if (i2 == index_map.end()) return plan;
-            if (n_values <= i2->second) return plan;
-            right = values_base + (uint32_t)i2->second;
-            ptrs.push_back(1);
-        }
-        const uint32_t out = next_slot++;
-        plan.ops.insert(plan.ops.end(), {left, right, out});
-        const uint64_t parent = (offset + index) >> 1;
-        v[parent] = out;
-        next.push_back(parent);
-    }
-    for (int d = 1; d < depth; d++) {
-        plan.level_start.push_back((uint32_t)(plan.ops.size() / 3));
-        std::vector<uint64_t> cur = next;
-        next.clear();
-        std::map<uint64_t, uint32_t> vnext;
-        size_t i = 0;
-        while (i < cur.size()) {
-            const uint64_t node_index = cur[i], sibling_index = node_index ^ 1;
-            uint32_t sibling;
-            if (i + 1 < cur.size() && cur[i + 1] == sibling_index) {
-                auto s = v.find(sibling_index);
-                if (s == v.end()) return plan;
-                sibling = s->second;
-                i += 1;
-            } else {
-                // the reference indexes proof.nodes and the pointers with the position inside the CURRENT level's list
-                if (i >= ptrs.size() || i >= nodes.size()) return plan;
-                const size_t pointer = ptrs[i];
-                if (nodes[i].size() <= pointer) return plan;
-                sibling = nodes_base[i] + (uint32_t)pointer;
-                ptrs[i] += 1;
-            }
-            auto nd = v.find(node_index);
-            if (nd == v.end()) return plan;
-            const uint32_t out = next_slot++;
-            if (node_index & 1) plan.ops.insert(plan.ops.end(), {sibling, nd->second, out});
-            else plan.ops.insert(plan.ops.end(), {nd->second, sibling, out});
-            const uint64_t parent = node_index >> 1;
-            vnext[parent] = out;
-            next.push_back(parent);
-            i += 1;
-        }
-        for (auto &kv : vnext) v[kv.first] = kv.second;         // parents join the map (HashMap::insert in the reference)
-    }
-    plan.level_start.push_back((uint32_t)(plan.ops.size() / 3));
-    auto rt = v.find(1);
-    if (rt == v.end()) return plan;
-    plan.root_slot = rt->second;
-    plan.ok = true;
-    return plan;
-}
 
 struct TreeDesc { uint32_t ops_base, n_levels, levels_base, pad; };
 

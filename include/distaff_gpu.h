@@ -82,9 +82,9 @@ int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, ui
  * batch into groups that fit in device memory and in one launch ($DG_BATCH_GROUP caps the group size further); stats (may be NULL)
  * covers the whole batch.  dg_batch_message(i, ...) copies (NUL-terminated, truncated to message_cap) the message of entry i of the
  * calling thread's last batched call, dg_prove_batch, dg_prove_batch_device, dg_verify_batch, dg_trace_batch, dg_execute_batch,
- * dg_trace_programs, dg_execute_programs, dg_trace_many or dg_execute_many: why
- * trace i failed (the message dg_prove gives for that trace), why proof i was not accepted (what dg_verify reports for that proof) or
- * why execution i failed, and "" if it was proven / accepted / executed. */
+ * dg_trace_programs, dg_execute_programs, dg_trace_many, dg_execute_many, dg_merkle_verify_paths or dg_merkle_verify_batch: why
+ * trace i failed (the message dg_prove gives for that trace), why proof i was not accepted (what dg_verify reports for that proof),
+ * why execution i failed, or why path / batch proof i was not accepted, and "" if it was proven / accepted / executed. */
 int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                    const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                    int *status, dg_prove_stats_t *stats);
@@ -475,6 +475,37 @@ int dg_tree_update(dg_tree_t *tree, const uint64_t *indexes, const uint8_t *leav
 /* copies the L leaves and / or the L heap nodes to the host; either may be NULL */
 int dg_tree_read(const dg_tree_t *tree, uint8_t *leaves32, uint8_t *nodes32);
 void dg_tree_free(dg_tree_t *tree);
+
+/* ---- batch proofs and their verification (MerkleTree::prove_batch / verify / verify_batch, merkle.rs:64-263) --------------------------
+ * The encoding of a BatchMerkleProof {values, nodes, depth} is its bincode: u64 count + 32 B per value; u64 count, then per slot u64 count
+ * + 32 B per node; u8 depth.  Hash ids and the hasher's message layout are those of dg_merkle_build_with. */
+/* MerkleTree::prove_batch (merkle.rs:64-124) of a device tree: values in request order, node slots per normalised (even) index, and from
+ * level 2 up the slot of a sibling is its position in the current level's list (merkle.rs:107-114).  The crate's panics fail the call with
+ * DG_ERR_INVALID on the host, in its order, and leave the tree as it was: "invalid index i" for an index > L, "repeating indexes detected",
+ * then "invalid index L" for an index of L.  count == 0 gives the empty proof of depth d.  *len receives the proof's length; with
+ * proof_out == NULL that is all, from the host plan, and the device is not touched; a cap below *len fails with DG_ERR_INVALID.  Otherwise
+ * one gather launch and one copy. */
+int dg_tree_prove_batch(const dg_tree_t *tree, const uint64_t *indexes, uint32_t count, uint8_t *proof_out, size_t cap, size_t *len);
+/* MerkleTree::verify (merkle.rs:127-151) for `count` paths of `entries` (2..64) 32-byte entries each, path k at paths32 + 32 entries k;
+ * n_roots is 1 (every path against roots32) or count (path k against root k).  As in the reference only the low entries - 1 bits of an
+ * index are read, so an index >= L = 2^(entries - 1) is checked as index mod L. */
+int dg_merkle_verify_paths(int hash, const uint8_t *roots32, uint32_t n_roots, const uint64_t *indexes, const uint8_t *paths32,
+                           uint32_t entries, uint32_t count, int *status);
+/* MerkleTree::verify_batch (merkle.rs:154-263) for `count` batch proofs: proof i is proofs[i] (proof_lens[i] bytes, the encoding above)
+ * against root roots32 + 32 i and the n_indexes[i] indexes at indexes[i] (may be NULL when n_indexes[i] is 0).  Depths 0-63 are planned
+ * (a depth above 63 overflows usize::pow in the reference and is treated as its panic).
+ *
+ * Both verify calls: status[k] is DG_OK where the reference returns true, DG_ERR_REJECTED where it returns false, and DG_ERR_INVALID where
+ * it panics ("invalid index i", "repeating indexes detected", "called `Option::unwrap()` on a `None` value") or where the entry's input is
+ * malformed: bytes that are not exactly one BatchMerkleProof (read as dg_verify reads a StarkProof), and for hashes 1-3 an entry, value or
+ * node element >= M, named in the message (the algebraic kernels take canonical operands; roots are only compared).  Entry k's message is
+ * dg_batch_message(k), "" when accepted; one bad entry changes no other verdict.  The whole call fails with DG_ERR_INVALID before the
+ * device is touched for a hash id other than 0-3, entries outside 2..64, n_roots other than 1 or count, or a NULL array.  Hashing runs
+ * one level at a time over every path or proof of a group (a message launch and one digest launch per level, the hasher's narrow / wide
+ * choice by level size); groups fit the device-memory budget of dg_verify_batch (dg_set_memory_limit), and every buffer is the pool's and
+ * freed before the call returns. */
+int dg_merkle_verify_batch(int hash, uint32_t count, const uint8_t *roots32, const uint64_t *const *indexes, const uint32_t *n_indexes,
+                           const uint8_t *const *proofs, const size_t *proof_lens, int *status);
 
 /* element-wise field ops on vectors (op: 0 add, 1 sub, 2 mul, 3 inv, 4 exp(a, b), 6 mul with b as a fixed twiddle: the NTT pass
  * kernels' product with a precomputed companion b * 2^64), for differential tests of the arithmetic;
