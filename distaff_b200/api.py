@@ -8,6 +8,9 @@ import numpy as np
 from . import backend, felt, hostvm
 
 
+MAX_CONSTRAINT_DEGREE = 8       # stark/mod.rs: the constraint evaluation domain is 8 times the trace domain
+
+
 class ProofOptions:
     """stark::ProofOptions (options.rs:29-50): same argument checks, same defaults (options.rs:82-91)."""
 
@@ -25,6 +28,26 @@ class ProofOptions:
     def _c(self):
         return backend.DgOptions(self.extension_factor, self.num_queries, self.grinding_factor, 0)
 
+    def security_level(self, optimistic=True):
+        """ProofOptions::security_level (options.rs:68-79): log2(extension_factor / MAX_CONSTRAINT_DEGREE) bits per query, over all
+        queries (optimistic) or half of them; the grinding factor is added once that reaches 80 bits."""
+        security_factor = (self.extension_factor // MAX_CONSTRAINT_DEGREE).bit_length() - 1
+        queries = self.num_queries if optimistic else self.num_queries // 2
+        level = security_factor * queries
+        return level + self.grinding_factor if level >= 80 else level
+
+    def _key(self):
+        return (self.extension_factor, self.num_queries, self.grinding_factor)
+
+    def __eq__(self, other):
+        return isinstance(other, ProofOptions) and self._key() == other._key()
+
+    def __hash__(self):
+        return hash(self._key())
+
+    def __repr__(self):
+        return "ProofOptions(extension_factor=%d, num_queries=%d, grinding_factor=%d)" % self._key()
+
 
 class StarkProof:
     """Result of prove(): the bincode bytes of the reference's StarkProof plus a few commitments for differential tests."""
@@ -39,6 +62,17 @@ class StarkProof:
 
     def __len__(self):
         return len(self.bytes)
+
+    @property
+    def options(self):
+        """The ProofOptions the proof was made with: the last four bytes of its bincode (proof.rs:21, options.rs:15-23), log2 of the
+        extension factor, num_queries, grinding_factor and the hash id (0, blake3)."""
+        if len(self.bytes) < 4:
+            raise ValueError("proof bytes too short to hold proof options")
+        log_b, queries, grinding, hash_id = self.bytes[-4:]
+        if hash_id != 0:
+            raise ValueError("proof options name hash function %d; only blake3 (0) is serialisable" % hash_id)
+        return ProofOptions(1 << log_b, queries, grinding)
 
 
 def _collect(handle, stats):
@@ -198,15 +232,30 @@ def prove_batch_device(d_registers, count, width, length, ctx_depth, loop_depth,
     return _collect_batch(list(handles)[:count], list(status)[:count], stats)
 
 
+def _options_arg(options, k, what):
+    """(the C options argument, whether it holds one entry per trace / job): one ProofOptions (None: the defaults) for all k, or a
+    list of k ProofOptions"""
+    if options is None or isinstance(options, ProofOptions):
+        return ctypes.byref((options or ProofOptions())._c()), False
+    options = list(options)
+    if len(options) != k:
+        raise ValueError("options: one ProofOptions per %s, %d for %d %ss" % (what, len(options), k, what))
+    for o in options:
+        if not isinstance(o, ProofOptions):
+            raise TypeError("options: each entry must be a ProofOptions, not %s" % type(o).__name__)
+    return (backend.DgOptions * max(k, 1))(*[o._c() for o in options]), True
+
+
 def prove_traces(traces, options=None):
     """Proves many hostvm.ExecutionTraces of any register shapes and lengths in one dg_prove_traces call: every stage is launched once
     per group of traces of one length, whatever their shapes (the constraint evaluation once per shape).  Returns what prove_batch
     returns, in input order: a StarkProof byte-identical to prove() of the same trace (its stats: the whole call's), or the
-    backend.DgError of a trace that failed."""
-    options = options or ProofOptions()
-    opt = options._c()
+    backend.DgError of a trace that failed.  options: one ProofOptions for every trace, or a list with one per trace
+    (dg_prove_traces_with_options): each proof is then prove() of its trace with its options, and the call runs in groups of one length
+    and extension factor."""
     traces = list(traces)
     k = len(traces)
+    opt, per_trace = _options_arg(options, k, "trace")
     regs = [np.ascontiguousarray(tr.registers, dtype=np.uint64) for tr in traces]
     cols = [(backend.vp * r.shape[0])(*[r[j].ctypes.data for j in range(r.shape[0])]) for r in regs]
     ts = (backend.DgTrace * max(k, 1))(*[backend.DgTrace(cols[i], r.shape[0], r.shape[1], tr.ctx_depth, tr.loop_depth)
@@ -215,41 +264,48 @@ def prove_traces(traces, options=None):
     handles = (backend.vp * max(k, 1))()
     status = (ctypes.c_int * max(k, 1))()
     st = backend.DgStats()
-    backend.check(backend.lib().dg_prove_traces(ts, k, pin, nin, pout, nout, ctypes.byref(opt), handles, status, ctypes.byref(st)))
+    fn = backend.lib().dg_prove_traces_with_options if per_trace else backend.lib().dg_prove_traces
+    backend.check(fn(ts, k, pin, nin, pout, nout, opt, handles, status, ctypes.byref(st)))
     del keep, regs, cols
     return _collect_batch(list(handles)[:k], list(status)[:k], st)
 
 
 def prove_traces_device(d_registers, widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list, options=None):
     """prove_traces for traces already in device memory: trace i's widths[i] x lengths[i] registers (column-major) at d_registers[i]
-    (backend.DeviceBuffer or raw pointer); the other arguments hold one entry per trace."""
-    options = options or ProofOptions()
+    (backend.DeviceBuffer or raw pointer); the other arguments hold one entry per trace.  options as in prove_traces."""
     k = len(d_registers)
     assert all(len(a) == k for a in (widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list)), "one entry per trace"
+    opt, per_trace = _options_arg(options, k, "trace")
     ptrs = (backend.vp * max(k, 1))(*[d.ptr if isinstance(d, backend.DeviceBuffer) else int(d) for d in d_registers])
     arr = lambda t, xs: (t * max(k, 1))(*[int(x) for x in xs])
-    opt = options._c()
     keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
     handles = (backend.vp * max(k, 1))()
     status = (ctypes.c_int * max(k, 1))()
     st = backend.DgStats()
-    backend.check(backend.lib().dg_prove_traces_device(ptrs, arr(backend.u32, widths), arr(backend.u64, lengths), arr(backend.u32, ctx_depths),
-                                                      arr(backend.u32, loop_depths), k, pin, nin, pout, nout, ctypes.byref(opt), handles, status,
-                                                      ctypes.byref(st)))
+    fn = backend.lib().dg_prove_traces_device_with_options if per_trace else backend.lib().dg_prove_traces_device
+    backend.check(fn(ptrs, arr(backend.u32, widths), arr(backend.u64, lengths), arr(backend.u32, ctx_depths), arr(backend.u32, loop_depths), k, pin,
+                     nin, pout, nout, opt, handles, status, ctypes.byref(st)))
     del keep
     return _collect_batch(list(handles)[:k], list(status)[:k], st)
 
 
-def group_traces(lengths, widths, ctx_depths, loop_depths, footprints, budget, cap):
-    """dg_host_group_traces (no device): the groups prove_traces runs, as lists of trace indices in device order."""
+def group_traces(lengths, widths, ctx_depths, loop_depths, footprints, budget, cap, extension_factors=None):
+    """dg_host_group_traces (no device): the groups prove_traces runs, as lists of trace indices in device order.  With
+    extension_factors (one per trace; dg_host_group_traces_with_options) the partitions are those of per-trace options: one per
+    (length, extension factor)."""
     k = len(lengths)
     arr = lambda t, xs: (t * max(k, 1))(*[int(x) for x in xs])
     order = (backend.u32 * max(k, 1))()
     sizes = (backend.u32 * max(k, 1))()
     n = backend.u32(0)
-    backend.check(backend.lib().dg_host_group_traces(k, arr(backend.u64, lengths), arr(backend.u32, widths), arr(backend.u32, ctx_depths),
-                                                    arr(backend.u32, loop_depths), arr(backend.u64, footprints), int(budget), int(cap), order,
-                                                    sizes, ctypes.byref(n)))
+    rest = (arr(backend.u32, widths), arr(backend.u32, ctx_depths), arr(backend.u32, loop_depths), arr(backend.u64, footprints), int(budget),
+            int(cap), order, sizes, ctypes.byref(n))
+    if extension_factors is None:
+        backend.check(backend.lib().dg_host_group_traces(k, arr(backend.u64, lengths), *rest))
+    else:
+        if len(extension_factors) != k:
+            raise ValueError("extension_factors: one per trace, %d for %d traces" % (len(extension_factors), k))
+        backend.check(backend.lib().dg_host_group_traces_with_options(k, arr(backend.u64, lengths), arr(backend.u32, extension_factors), *rest))
     out, at = [], 0
     for s in list(sizes)[:n.value]:
         out.append(list(order)[at:at + s])
@@ -661,15 +717,16 @@ def _trace_jobs(entry, jobs, st, stats, *args):
 
 def _execute_jobs(entry, jobs, options, st, stats, *args):
     """execute_programs / execute_many: the C entry named `entry` (programs, n_programs, count, program_of, inputs, num_outputs, *args,
-    options, proofs_out, outputs16, status, prove_stats, st) through _proofs, its stats structure st into the dict `stats`"""
-    opt = (options or ProofOptions())._c()
+    options, proofs_out, outputs16, status, prove_stats, st) through _proofs, its stats structure st into the dict `stats`.  options: one
+    ProofOptions, or a list with one per job (the entry's _with_options form)"""
     jobs = list(jobs)
+    opt, per_job = _options_arg(options, len(jobs), "job")
     if not jobs:
         return []
     programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
-    k, fn = len(jobs), getattr(backend.lib(), entry)
+    k, fn = len(jobs), getattr(backend.lib(), entry + "_with_options" if per_job else entry)
     result = _proofs(lambda handles, outputs16, status, pst: fn(cprogs, len(programs), k, program_of, arr, (backend.u32 * k)(*num_outputs), *args,
-                                                                ctypes.byref(opt), handles, outputs16, status, pst, ctypes.byref(st)), num_outputs)
+                                                                opt, handles, outputs16, status, pst, ctypes.byref(st)), num_outputs)
     _fields(st, stats)
     return result
 
@@ -687,7 +744,8 @@ def execute_programs(jobs, options=None, max_steps=MAX_STEPS, stats=None):
     """execute_batch for executions of different programs in one call (dg_execute_programs): the VM runs every job on the GPU, and each
     trace shape's traces are proven together, whichever programs they came from, in the device memory they were written to.  Returns a
     list in job order: (outputs, StarkProof) -- what execute_batch of that program alone returns, byte for byte -- or the DgError of an
-    execution that failed.  `stats` as in trace_programs, prove_groups included."""
+    execution that failed.  `stats` as in trace_programs, prove_groups included.  options: one ProofOptions for every job, or a list with
+    one per job (dg_execute_programs_with_options)."""
     return _execute_jobs("dg_execute_programs", jobs, options, backend.DgExecutionStats(), stats, int(max_steps))
 
 
@@ -712,7 +770,7 @@ def trace_many(jobs, max_steps=MAX_STEPS, segment_steps=0, stats=None):
 def execute_many(jobs, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
     """execute_programs with every execution run as execute_one runs one (dg_execute_many): every trace is proven where it was written.
     Returns a list in job order: (outputs, StarkProof) -- what execute_programs returns, byte for byte -- or the DgError of an execution
-    that failed.  segment_steps and `stats` as in trace_many."""
+    that failed.  segment_steps and `stats` as in trace_many; options as in execute_programs."""
     return _execute_jobs("dg_execute_many", jobs, options, backend.DgManyStats(), stats, int(max_steps), _segment_steps(segment_steps))
 
 

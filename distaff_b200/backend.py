@@ -115,6 +115,11 @@ EXPORTS = {
     "dg_prove_traces_device": [ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32), u32,
                                ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(DgOptions),
                                ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_prove_traces_with_options": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                                     ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
+    "dg_prove_traces_device_with_options": [ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32),
+                                            u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
+                                            ctypes.POINTER(DgOptions), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats)],
     "dg_batch_message": [u32, ctypes.c_char_p, ctypes.c_size_t],
     "dg_trace_batch": [ctypes.POINTER(DgProgram), u32, ctypes.POINTER(DgProgramInputs), u64, ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp),
                        ctypes.POINTER(ctypes.c_int)],
@@ -125,6 +130,9 @@ EXPORTS = {
     "dg_execute_programs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32), u64,
                             ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
                             ctypes.POINTER(DgExecutionStats)],
+    "dg_execute_programs_with_options": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs),
+                                         ctypes.POINTER(u32), u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int),
+                                         ctypes.POINTER(DgStats), ctypes.POINTER(DgExecutionStats)],
     "dg_trace_one": [ctypes.POINTER(DgProgram), ctypes.POINTER(DgProgramInputs), u64, u64, ctypes.POINTER(DgExecutionInfo), vp,
                      ctypes.POINTER(DgTraceOneStats)],
     "dg_execute_one": [ctypes.POINTER(DgProgram), ctypes.POINTER(DgProgramInputs), u32, u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp,
@@ -134,6 +142,9 @@ EXPORTS = {
     "dg_execute_many": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32), u64, u64,
                         ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
                         ctypes.POINTER(DgManyStats)],
+    "dg_execute_many_with_options": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32),
+                                     u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
+                                     ctypes.POINTER(DgManyStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
@@ -182,6 +193,9 @@ EXPORTS = {
     "dg_host_shard_locate": [u64, ctypes.c_int, ctypes.c_int, ctypes.c_int, u64, ctypes.POINTER(ctypes.c_int64)],
     "dg_host_group_traces": [u32, ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u64), u64, u32,
                              ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32)],
+    "dg_host_group_traces_with_options": [u32, ctypes.POINTER(u64), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32),
+                                          ctypes.POINTER(u32), ctypes.POINTER(u64), u64, u32, ctypes.POINTER(u32), ctypes.POINTER(u32),
+                                          ctypes.POINTER(u32)],
     "dg_host_prng_vector": [vp, u64, vp],
     "dg_host_query_positions": [vp, u64, u32, u32, vp],
     "dg_host_blake3": [vp, ctypes.c_size_t, vp],

@@ -578,7 +578,7 @@ int dg_find_pow_nonce(const uint8_t seed[32], uint32_t grinding_factor, uint64_t
         DG_REQUIRE(grinding_factor <= 32, "grinding factor cannot be greater than 32");
         std::array<uint8_t, 32> s;
         memcpy(s.data(), seed, 32);
-        const unsigned long long n = pow_search_batch(c, {s}, grinding_factor)[0];
+        const unsigned long long n = pow_search_batch(c, {s}, {grinding_factor})[0];
         *nonce = n;
         if (new_seed) pow_hash(seed, n, new_seed);
     });
@@ -764,45 +764,84 @@ static void check_trace_entry(uint32_t i, uint32_t width, uint64_t length, uint3
         throw Error(e.code, "trace " + std::to_string(i) + ": " + e.what());
     }
 }
+// the options of a call: one set for every entry (per_entry false), or options[i] for entry i, each checked on the host with `what i: `
+// before the message (dg_*_with_options)
+static std::vector<dg_options_t> call_options(const dg_options_t *options, uint32_t count, bool per_entry, const char *what) {
+    if (!per_entry) return std::vector<dg_options_t>(count, *options);
+    for (uint32_t i = 0; i < count; i++) {
+        try {
+            check_options(options[i]);
+        } catch (const Error &e) {
+            throw Error(e.code, std::string(what) + " " + std::to_string(i) + ": " + e.what());
+        }
+    }
+    return std::vector<dg_options_t>(options, options + count);
+}
+static void prove_host_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                              const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, bool per_trace,
+                              dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+    std::vector<TraceRef> refs(count);
+    for (uint32_t i = 0; i < count; i++) {
+        const dg_trace_t &t = traces[i];
+        check_trace_entry(i, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs);
+        DG_REQUIRE(t.columns, "trace " + std::to_string(i) + ": null register columns");
+        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "trace " + std::to_string(i) + ": null register column");
+        refs[i].width = t.width; refs[i].length = t.length; refs[i].ctx_depth = t.ctx_depth; refs[i].loop_depth = t.loop_depth;
+        refs[i].host_cols = t.columns;
+    }
+    const std::vector<dg_options_t> opts = call_options(options, count, per_trace, "trace");
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, opts, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+}
+static void prove_device_traces(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                                const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                                const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, bool per_trace,
+                                dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
+    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
+    std::vector<TraceRef> refs(count);
+    for (uint32_t i = 0; i < count; i++) {
+        check_trace_entry(i, width[i], length[i], ctx_depth[i], loop_depth[i], inputs16, n_inputs, outputs16, n_outputs);
+        DG_REQUIRE(d_registers[i], "trace " + std::to_string(i) + ": null registers");
+        refs[i].width = width[i]; refs[i].length = length[i]; refs[i].ctx_depth = ctx_depth[i]; refs[i].loop_depth = loop_depth[i];
+        refs[i].d_regs = (const fe *)d_registers[i];
+    }
+    const std::vector<dg_options_t> opts = call_options(options, count, per_trace, "trace");
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, opts, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+}
 int dg_prove_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                     const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                     int *status, dg_prove_stats_t *stats) {
-    return guarded([&] {
-        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
-        std::vector<TraceRef> refs(count);
-        for (uint32_t i = 0; i < count; i++) {
-            const dg_trace_t &t = traces[i];
-            check_trace_entry(i, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs);
-            DG_REQUIRE(t.columns, "trace " + std::to_string(i) + ": null register columns");
-            for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "trace " + std::to_string(i) + ": null register column");
-            refs[i].width = t.width; refs[i].length = t.length; refs[i].ctx_depth = t.ctx_depth; refs[i].loop_depth = t.loop_depth;
-            refs[i].host_cols = t.columns;
-        }
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
-    });
+    return guarded([&] { prove_host_traces(traces, count, inputs16, n_inputs, outputs16, n_outputs, options, false, proofs_out, status, stats); });
+}
+int dg_prove_traces_with_options(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                                 const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                                 int *status, dg_prove_stats_t *stats) {
+    return guarded([&] { prove_host_traces(traces, count, inputs16, n_inputs, outputs16, n_outputs, options, true, proofs_out, status, stats); });
 }
 int dg_prove_traces_device(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
                            const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                            const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                            int *status, dg_prove_stats_t *stats) {
     return guarded([&] {
-        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-        DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
-        std::vector<TraceRef> refs(count);
-        for (uint32_t i = 0; i < count; i++) {
-            check_trace_entry(i, width[i], length[i], ctx_depth[i], loop_depth[i], inputs16, n_inputs, outputs16, n_outputs);
-            DG_REQUIRE(d_registers[i], "trace " + std::to_string(i) + ": null registers");
-            refs[i].width = width[i]; refs[i].length = length[i]; refs[i].ctx_depth = ctx_depth[i]; refs[i].loop_depth = loop_depth[i];
-            refs[i].d_regs = (const fe *)d_registers[i];
-        }
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+        prove_device_traces(d_registers, width, length, ctx_depth, loop_depth, count, inputs16, n_inputs, outputs16, n_outputs, options, false,
+                            proofs_out, status, stats);
+    });
+}
+int dg_prove_traces_device_with_options(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                                        const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                                        const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options,
+                                        dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        prove_device_traces(d_registers, width, length, ctx_depth, loop_depth, count, inputs16, n_inputs, outputs16, n_outputs, options, true,
+                            proofs_out, status, stats);
     });
 }
 int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -845,18 +884,35 @@ int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_
         trace_programs(c, x, info, registers_out, status, t_batch_messages, vm_stats);
     });
 }
+static void run_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                 const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                                 bool per_execution, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
+                                 dg_execution_stats_t *vm_stats) {
+    DG_REQUIRE(count >= 1, "at least one execution is needed");
+    DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
+    const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+    check_execution_call(x, OutputCounts{num_outputs, outputs16});
+    const std::vector<dg_options_t> opts = call_options(options, count, per_execution, "execution");
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    execute_programs(c, x, num_outputs, opts.data(), (Proof **)proofs_out, outputs16, status, t_batch_messages, stats, vm_stats);
+}
 int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
                         const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
                         dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
     return guarded([&] {
-        DG_REQUIRE(count >= 1, "at least one execution is needed");
-        DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
-        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x, OutputCounts{num_outputs, outputs16});
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        execute_programs(c, x, num_outputs, *options, (Proof **)proofs_out, outputs16, status, t_batch_messages, stats, vm_stats);
+        run_execute_programs(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, options, false, proofs_out, outputs16, status,
+                             stats, vm_stats);
+    });
+}
+int dg_execute_programs_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                     const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                                     dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
+                                     dg_execution_stats_t *vm_stats) {
+    return guarded([&] {
+        run_execute_programs(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, options, true, proofs_out, outputs16, status,
+                             stats, vm_stats);
     });
 }
 // the one-program case: program_of all 0
@@ -886,7 +942,8 @@ int dg_execute_batch(const dg_program_t *program, uint32_t count, const dg_progr
         std::lock_guard<std::mutex> lk(c.mu);
         t_batch_messages.clear();
         std::vector<uint8_t> outs((size_t)count * 8 * 16);
-        execute_programs(c, x, n_out.data(), *options, (Proof **)proofs_out, outs.data(), status, t_batch_messages, stats, nullptr);
+        const std::vector<dg_options_t> opts(count, *options);
+        execute_programs(c, x, n_out.data(), opts.data(), (Proof **)proofs_out, outs.data(), status, t_batch_messages, stats, nullptr);
         if (num_outputs)     // num_outputs elements per execution
             for (uint32_t i = 0; i < count; i++) memcpy(outputs16 + (size_t)16 * num_outputs * i, outs.data() + (size_t)128 * i, (size_t)16 * num_outputs);
     });
@@ -957,7 +1014,7 @@ int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *input
         uint8_t outs[8 * 16];             // execute_many writes 8 elements; the caller's buffer holds num_outputs
         dg_execution_info_t one;
         run_one(stats, [&](int *status, std::vector<std::string> &messages, dg_many_stats_t *m) {
-            execute_many(c, x, &num_outputs, segment_steps, *options, (Proof **)proof_out, outs, &one, status, messages, prove_stats, m);
+            execute_many(c, x, &num_outputs, segment_steps, options, (Proof **)proof_out, outs, &one, status, messages, prove_stats, m);
         });
         if (num_outputs) memcpy(outputs16, outs, (size_t)16 * num_outputs);
         if (info) *info = one;
@@ -977,20 +1034,37 @@ int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t co
         trace_many(c, x, segment_steps, info, registers_out, status, t_batch_messages, stats);
     });
 }
+static void run_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                             const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                             const dg_options_t *options, bool per_execution, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
+                             dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
+    DG_REQUIRE(count >= 1, "at least one execution is needed");
+    DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
+    const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+    check_execution_call(x, OutputCounts{num_outputs, outputs16}, segment_steps);
+    const std::vector<dg_options_t> opts = call_options(options, count, per_execution, "execution");
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    execute_many(c, x, num_outputs, segment_steps, opts.data(), (Proof **)proofs_out, outputs16, nullptr, status, t_batch_messages, prove_stats,
+                 stats);
+}
 int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
                     const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
                     const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
                     dg_many_stats_t *stats) {
     return guarded([&] {
-        DG_REQUIRE(count >= 1, "at least one execution is needed");
-        DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
-        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x, OutputCounts{num_outputs, outputs16}, segment_steps);
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        execute_many(c, x, num_outputs, segment_steps, *options, (Proof **)proofs_out, outputs16, nullptr, status, t_batch_messages, prove_stats,
-                     stats);
+        run_execute_many(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, segment_steps, options, false, proofs_out,
+                         outputs16, status, prove_stats, stats);
+    });
+}
+int dg_execute_many_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                 const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                                 const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
+                                 dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
+    return guarded([&] {
+        run_execute_many(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, segment_steps, options, true, proofs_out,
+                         outputs16, status, prove_stats, stats);
     });
 }
 int dg_batch_message(uint32_t index, char *message, size_t cap) {
@@ -1124,27 +1198,43 @@ int dg_host_shard_locate(uint64_t n, int log_blk, int log_g, int is_node, uint64
     });
 }
 
+static void host_group_traces(uint32_t count, const uint64_t *lengths, const uint32_t *extension_factors, const uint32_t *widths,
+                              const uint32_t *ctx_depths, const uint32_t *loop_depths, const uint64_t *footprints, uint64_t budget, uint32_t cap,
+                              uint32_t *order_out, uint32_t *group_sizes_out, uint32_t *n_groups) {
+    DG_REQUIRE(lengths && widths && ctx_depths && loop_depths && footprints && order_out && group_sizes_out && n_groups, "null argument");
+    DG_REQUIRE(cap >= 1, "a group holds at least one trace");
+    const std::vector<uint32_t> factors = extension_factors ? std::vector<uint32_t>(extension_factors, extension_factors + count)
+                                                            : std::vector<uint32_t>(count, 0);
+    uint32_t at = 0, groups = 0;
+    for (const std::vector<uint32_t> &idx : partition_traces(std::vector<uint64_t>(lengths, lengths + count), factors)) {
+        std::vector<uint32_t> w;
+        std::vector<size_t> foot;
+        for (uint32_t i : idx) { w.push_back(widths[i]); foot.push_back(footprints[i]); }
+        size_t first = 0;
+        for (uint32_t k : cut_groups(w, foot, budget, cap)) {
+            std::vector<RegisterShape> keys;
+            for (size_t m = first; m < first + k; m++) keys.push_back(RegisterShape{widths[idx[m]], ctx_depths[idx[m]], loop_depths[idx[m]]});
+            for (uint32_t m : shape_order(keys)) order_out[at++] = idx[first + m];
+            group_sizes_out[groups++] = k;
+            first += k;
+        }
+    }
+    *n_groups = groups;
+}
 int dg_host_group_traces(uint32_t count, const uint64_t *lengths, const uint32_t *widths, const uint32_t *ctx_depths, const uint32_t *loop_depths,
                          const uint64_t *footprints, uint64_t budget, uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out,
                          uint32_t *n_groups) {
     return guarded([&] {
-        DG_REQUIRE(lengths && widths && ctx_depths && loop_depths && footprints && order_out && group_sizes_out && n_groups, "null argument");
-        DG_REQUIRE(cap >= 1, "a group holds at least one trace");
-        uint32_t at = 0, groups = 0;
-        for (const std::vector<uint32_t> &idx : partition_by_length(std::vector<uint64_t>(lengths, lengths + count))) {
-            std::vector<uint32_t> w;
-            std::vector<size_t> foot;
-            for (uint32_t i : idx) { w.push_back(widths[i]); foot.push_back(footprints[i]); }
-            size_t first = 0;
-            for (uint32_t k : cut_groups(w, foot, budget, cap)) {
-                std::vector<RegisterShape> keys;
-                for (size_t m = first; m < first + k; m++) keys.push_back(RegisterShape{widths[idx[m]], ctx_depths[idx[m]], loop_depths[idx[m]]});
-                for (uint32_t m : shape_order(keys)) order_out[at++] = idx[first + m];
-                group_sizes_out[groups++] = k;
-                first += k;
-            }
-        }
-        *n_groups = groups;
+        host_group_traces(count, lengths, nullptr, widths, ctx_depths, loop_depths, footprints, budget, cap, order_out, group_sizes_out, n_groups);
+    });
+}
+int dg_host_group_traces_with_options(uint32_t count, const uint64_t *lengths, const uint32_t *extension_factors, const uint32_t *widths,
+                                      const uint32_t *ctx_depths, const uint32_t *loop_depths, const uint64_t *footprints, uint64_t budget,
+                                      uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out, uint32_t *n_groups) {
+    return guarded([&] {
+        DG_REQUIRE(extension_factors, "null argument");
+        host_group_traces(count, lengths, extension_factors, widths, ctx_depths, loop_depths, footprints, budget, cap, order_out, group_sizes_out,
+                     n_groups);
     });
 }
 

@@ -148,6 +148,8 @@ struct Context {
     int rank = 0, world = 1;                // multi-GPU sharding (comm.cu); world == 1: no communication
     size_t mem_limit = 0;                   // most device bytes the library may hold (arena + pool), 0 = no limit (dg_set_memory_limit)
     size_t mem_peak = 0;                    // most held since the limit was set, up to the last change of the arena (memory_usage)
+    size_t pool_floor = 0;                  // under a limit: pool memory the trim at dg_set_memory_limit could not hand back beside what
+                                            // was in use (chunks that persistent buffers keep partly used); Budget::FREE counts it as held
 
     TwiddleRef twiddle(int log_order, bool inverse);
     std::map<int, DevBuf> single_tables;    // full power tables w^e, e < 2^log_order (small orders only)

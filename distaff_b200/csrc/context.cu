@@ -112,7 +112,9 @@ size_t memory_budget(Context &c, Budget kind, size_t need, size_t scratch) {
         avail = (free_b + (kind == Budget::ARENA ? c.arena.cap : 0)) / 10 * 8;
     }
     if (c.mem_limit) {
-        const size_t held = memory_held_outside_arena(c) + scratch;
+        // free-memory budgets (execution buffers, trace checks) come on top of the pool's floor as well: memory the pool could not hand
+        // back when the limit was set, because persistent buffers of earlier calls keep its chunks partly used
+        const size_t held = memory_held_outside_arena(c) + scratch + (kind == Budget::FREE ? c.pool_floor : 0);
         avail = std::min(avail, c.mem_limit > held ? c.mem_limit - held : 0);
     }
     return avail;
@@ -121,10 +123,14 @@ size_t memory_budget(Context &c, Budget kind, size_t need, size_t scratch) {
 void memory_set_limit(Context &c, size_t bytes) {
     DG_CUDA(cudaStreamSynchronize(c.stream));
     c.mem_limit = bytes;
+    c.pool_floor = 0;
     apply_release_threshold(c);
     if (bytes) {
         if (c.arena.cap + memory_held_outside_arena(c) > bytes) arena_release(c);
-        DG_CUDA(cudaMemPoolTrimTo(device_pool(c), bytes > c.arena.cap ? bytes - c.arena.cap : 0));
+        // hand back everything the pool holds unused; what stays reserved beyond the memory in use is the floor
+        DG_CUDA(cudaMemPoolTrimTo(device_pool(c), 0));
+        const size_t reserved = pool_attr(c, cudaMemPoolAttrReservedMemCurrent), used = pool_attr(c, cudaMemPoolAttrUsedMemCurrent);
+        c.pool_floor = reserved > used ? reserved - used : 0;
     }
     fold_peak(c);
     c.mem_peak = c.arena.cap + pool_attr(c, cudaMemPoolAttrReservedMemCurrent);

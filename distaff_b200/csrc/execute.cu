@@ -300,11 +300,11 @@ struct Executions {
     // The executions `order` (in shape order) in waves: a wave is a run of them, given one slab per shape in a fresh register buffer and
     // handed to write(wave, slabs, last) while its traces are on the device; waves follow each other, so the executions reach write in
     // shape order, input order inside a shape.  A wave's traces take at most half of the device memory the library may use, and with
-    // `opt` they leave room beside them for one proof of the wave's largest shape.  $DG_BATCH_GROUP caps its executions.  L.out / L.outs
-    // and d_pad_ids (the wave, in slab order) are set for the wave.
-    template <typename F> void cut_waves(const std::vector<unsigned> &order, const dg_options_t *opt, uint8_t *const *registers_out, F &&write) {
+    // `opts` (the options of every execution) they leave room beside them for one proof of the wave's largest shape and extension factor.
+    // $DG_BATCH_GROUP caps its executions.  L.out / L.outs and d_pad_ids (the wave, in slab order) are set for the wave.
+    template <typename F> void cut_waves(const std::vector<unsigned> &order, const dg_options_t *opts, uint8_t *const *registers_out, F &&write) {
         const size_t most = (size_t)batch_group_cap(65535);         // one padding launch holds 65535 executions
-        std::map<ShapeKey, size_t> room;                           // bytes one proof of a shape needs beside the traces
+        std::map<std::pair<ShapeKey, uint32_t>, size_t> room;      // bytes one proof of a shape and extension factor needs beside the traces
         std::vector<VmOut> outs(x.count);
         for (size_t first = 0; first < order.size();) {
             size_t avail = memory_budget(c, Budget::FREE, 0);
@@ -314,17 +314,18 @@ struct Executions {
                 const dg_execution_info_t s = info(order[end]);
                 const size_t per = (size_t)s.width * s.length * 16;
                 size_t r = 0;
-                if (opt) {
-                    auto it = room.find(key(s));
+                if (opts) {
+                    const uint32_t b = opts[order[end]].extension_factor;
+                    auto it = room.find({key(s), b});
                     if (it == room.end()) {
-                        const ProvePlan P = plan_prove(c, s.width, s.length, opt->extension_factor, 1);
-                        it = room.emplace(key(s), P.per_proof + P.fixed - memory_held_outside_arena(c)).first;
+                        const ProvePlan P = plan_prove(c, s.width, s.length, b, 1);
+                        it = room.emplace(std::make_pair(key(s), b), P.per_proof + P.fixed - memory_held_outside_arena(c)).first;
                     }
                     r = it->second;
                 }
                 if (end > first && (bytes + per > avail / 2 || bytes + per + std::max(need, r) > avail)) break;
                 if (registers_out) DG_REQUIRE(registers_out[order[end]], "null register buffer of execution " + std::to_string(order[end]));
-                if (!opt && c.mem_limit && per > avail)
+                if (!opts && c.mem_limit && per > avail)
                     throw Error(DG_ERR_INVALID, "a trace of " + std::to_string(s.width) + " x " + std::to_string(s.length) + " needs " +
                                                     std::to_string(per) + " bytes of device memory beyond what the memory limit leaves");
                 bytes += per;
@@ -361,8 +362,8 @@ struct Executions {
 
     // The write pass of the successful executions of `ids`, in waves (cut_waves): one launch per wave for every shape in it, then
     // done(slabs).
-    template <typename F> void write_waves(const std::vector<unsigned> &ids, const dg_options_t *opt, uint8_t *const *registers_out, F &&done) {
-        cut_waves(shape_order(ids), opt, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool) {
+    template <typename F> void write_waves(const std::vector<unsigned> &ids, const dg_options_t *opts, uint8_t *const *registers_out, F &&done) {
+        cut_waves(shape_order(ids), opts, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool) {
             stats.lanes += launch_ids(wave);
             stats.write_ms += timed([&] {
                 vm_write_pass(c, L);
@@ -395,10 +396,11 @@ void copy_slabs(Context &c, const Executions &X, const std::vector<Slab> &slabs,
     DG_CUDA(cudaStreamSynchronize(c.stream));
 }
 
-// Each shape's successful traces of a wave proven together where they were written (prove_traces), RNG callbacks shape by shape and
-// in input order inside a shape.  Executions the rows failed are left out: the traces after them move down over them, and their outputs
-// (8 per execution in outs) are zeroed, as those of executions the VM failed earlier.  Adds the prove groups to `groups`.
-void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, const uint32_t *num_outputs, const dg_options_t &opt,
+// Each shape's successful traces of a wave proven together where they were written (prove_traces), each with its execution's options
+// (opts[i]): RNG callbacks shape by shape, inside a shape extension factor by extension factor (in order of first appearance) and in
+// input order inside those.  Executions the rows failed are left out: the traces after them move down over them, and their outputs (8 per
+// execution in outs) are zeroed, as those of executions the VM failed earlier.  Adds the prove groups to `groups`.
+void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, const uint32_t *num_outputs, const dg_options_t *opts,
                  std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats, uint32_t &groups) {
     const ExecutionCall &x = X.x;
     for (const Slab &s : slabs) {
@@ -417,9 +419,11 @@ void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, cons
         const uint32_t k = (uint32_t)ok.size();
         std::vector<const uint8_t *> in16(k), out16(k);
         std::vector<uint32_t> n_in(k), n_out(k);
+        std::vector<dg_options_t> opt(k);
         for (uint32_t q = 0; q < k; q++) {
             in16[q] = x.inputs[ok[q]].public16; n_in[q] = x.inputs[ok[q]].n_public;
             out16[q] = (const uint8_t *)&outs[(size_t)ok[q] * 8]; n_out[q] = num_outputs[ok[q]];
+            opt[q] = opts[ok[q]];
         }
         std::vector<Proof *> proofs(k, nullptr);
         std::vector<int> st(k, DG_OK);
@@ -427,8 +431,8 @@ void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, cons
         dg_prove_stats_t gs;
         memset(&gs, 0, sizeof gs);
         uint32_t g = 0;
-        prove_traces(c, s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth, in16.data(), n_in.data(),
-                     out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &g);
+        prove_traces(c, one_shape_traces(s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth), in16.data(),
+                     n_in.data(), out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &g);
         for (uint32_t q = 0; q < k; q++) {
             proofs_out[ok[q]] = proofs[q];
             if (st[q] != DG_OK) X.fail(ok[q], st[q], msg[q]);
@@ -455,13 +459,13 @@ void batch_trace(Context &c, Executions &X, const std::vector<unsigned> &ids, ui
 
 // The batch path for the executions `ids`, proven: the shape pass, outputs from the final stacks, the write pass in waves and each wave
 // proven in place
-void batch_execute(Context &c, Executions &X, const std::vector<unsigned> &ids, const uint32_t *num_outputs, const dg_options_t &opt,
+void batch_execute(Context &c, Executions &X, const std::vector<unsigned> &ids, const uint32_t *num_outputs, const dg_options_t *opts,
                    std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats) {
     X.shapes(ids);
     for (unsigned i : ids)
         if (X.status[i] == DG_OK) for (uint32_t j = 0; j < num_outputs[i]; j++) outs[(size_t)i * 8 + j] = X.res[i].top[j];
-    X.write_waves(ids, &opt, nullptr, [&](const std::vector<Slab> &slabs) {
-        prove_slabs(c, X, slabs, num_outputs, opt, outs, proofs_out, stats, X.stats.prove_groups);
+    X.write_waves(ids, opts, nullptr, [&](const std::vector<Slab> &slabs) {
+        prove_slabs(c, X, slabs, num_outputs, opts, outs, proofs_out, stats, X.stats.prove_groups);
     });
 }
 
@@ -738,8 +742,8 @@ struct TabledExecutions {
     // The rows of the successful executions of `run`, in waves as the batch path cuts them: per wave one segment launch for every
     // checkpoint of its executions and one padding launch per shape, then done(slabs).  A segment that fails is an internal error of its
     // execution.  The tables, logs and checkpoints are freed before the last wave's done.
-    template <typename F> void waves(const dg_options_t *opt, uint8_t *const *registers_out, F &&done) {
-        X.cut_waves(X.shape_order(run), opt, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool last) {
+    template <typename F> void waves(const dg_options_t *opts, uint8_t *const *registers_out, F &&done) {
+        X.cut_waves(X.shape_order(run), opts, registers_out, [&](const std::vector<unsigned> &wave, const std::vector<Slab> &slabs, bool last) {
             std::vector<unsigned long long> first{0};
             for (unsigned e : wave) first.push_back(first.back() + seq[e].checkpoints);
             const unsigned long long segments = first.back();
@@ -784,14 +788,14 @@ struct TabledExecutions {
         st.fallback = X.stats;
     }
     // dg_execute_many: the same, every trace proven where it was written; outs holds 8 elements per execution
-    void execute(const uint32_t *num_outputs, const dg_options_t &opt, std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats) {
+    void execute(const uint32_t *num_outputs, const dg_options_t *opts, std::vector<fe> &outs, Proof **proofs_out, dg_prove_stats_t *stats) {
         tables();
         if (run.empty()) release();
-        batch_execute(c, X, fallback, num_outputs, opt, outs, proofs_out, stats);
+        batch_execute(c, X, fallback, num_outputs, opts, outs, proofs_out, stats);
         sequential();
         for (unsigned e : run)
             if (X.status[e] == DG_OK) for (uint32_t j = 0; j < num_outputs[e]; j++) outs[(size_t)e * 8 + j] = X.res[e].top[j];
-        waves(&opt, nullptr, [&](const std::vector<Slab> &slabs) { prove_slabs(c, X, slabs, num_outputs, opt, outs, proofs_out, stats, st.prove_groups); });
+        waves(opts, nullptr, [&](const std::vector<Slab> &slabs) { prove_slabs(c, X, slabs, num_outputs, opts, outs, proofs_out, stats, st.prove_groups); });
         st.fallback = X.stats;
     }
 };
@@ -850,7 +854,7 @@ void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *inf
     finish(X, info, status, messages, vm_stats);
 }
 
-void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
+void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t *opts, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
     check_one_gpu(c);
     proven(x.count, proofs_out, outputs16, stats, [&](std::vector<fe> &outs) {
@@ -858,7 +862,7 @@ void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_ou
         X.setup();
         std::vector<unsigned> all(x.count);
         std::iota(all.begin(), all.end(), 0u);
-        batch_execute(c, X, all, num_outputs, opt, outs, proofs_out, stats);
+        batch_execute(c, X, all, num_outputs, opts, outs, proofs_out, stats);
         finish(X, nullptr, status, messages, vm_stats);
     });
 }
@@ -871,13 +875,13 @@ void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_e
     finish(E.X, info, status, messages, nullptr);
 }
 
-void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
+void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t *opts,
                   Proof **proofs_out, uint8_t *outputs16, dg_execution_info_t *info, int *status, std::vector<std::string> &messages,
                   dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
     check_one_gpu(c);
     proven(x.count, proofs_out, outputs16, prove_stats, [&](std::vector<fe> &outs) {
         TabledExecutions E(c, x, segment_steps, stats);
-        E.execute(num_outputs, opt, outs, proofs_out, prove_stats);
+        E.execute(num_outputs, opts, outs, proofs_out, prove_stats);
         finish(E.X, info, status, messages, nullptr);
     });
 }

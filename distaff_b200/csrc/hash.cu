@@ -10,6 +10,7 @@
 // on the CPU therefore costs no extra memory pass.
 #include "common.cuh"
 #include "blake3.cuh"
+#include <algorithm>
 
 namespace dg {
 
@@ -215,38 +216,46 @@ __device__ __forceinline__ bool pow_hit(const uint32_t *__restrict__ seed, unsig
     return tz >= grinding;
 }
 
-// one window [start, start + count) of nonces for each unfinished proof active[blockIdx.y]: seeds [proof][8 words], best [proof]
-__global__ void __launch_bounds__(256) pow_batch_kernel(const uint32_t *__restrict__ seeds, const unsigned *__restrict__ active,
-                                                        unsigned long long start, unsigned long long count, unsigned grinding,
-                                                        unsigned long long *best) {
+// one window [start, start + count) of nonces for each unfinished proof active[blockIdx.y]: seeds [proof][8 words], grinding [proof],
+// best [proof]
+__global__ void __launch_bounds__(256) pow_batch_kernel(const uint32_t *__restrict__ seeds, const unsigned *__restrict__ grinding,
+                                                        const unsigned *__restrict__ active, unsigned long long start,
+                                                        unsigned long long count, unsigned long long *best) {
     const unsigned long long g = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= count) return;
     const unsigned p = active[blockIdx.y];
     const unsigned long long nonce = start + g;
-    if (pow_hit(seeds + 8 * p, nonce, grinding)) atomicMin(best + p, nonce);
+    if (pow_hit(seeds + 8 * p, nonce, grinding[p])) atomicMin(best + p, nonce);
 }
 
-// For each of K seeds, the smallest nonce >= 1 whose hash has >= grinding trailing zero bits in its first 8 bytes.  Each round scans the
-// same window of nonces for every proof that has no hit yet (one launch, one copy of the K results back).  A proof finishes in the first
-// window where it has a hit, and the window's smallest hit is its smallest nonce.
+// For each of K seeds, the smallest nonce >= 1 whose hash has >= grinding[p] trailing zero bits in its first 8 bytes.  Each round scans
+// the same window of nonces for every proof that has no hit yet (one launch, one copy of the K results back).  A proof finishes in the
+// first window where it has a hit, and the window's smallest hit is its smallest nonce; proofs of low grinding factors drop out early.
 // One proof scans a 2^22 window per round.  A batch scans 2^22 / K nonces per proof and round (one 2^22-nonce round in all), but at least
-// 2^(grinding - 2), a quarter of the expected search (clamped to 2^10 .. 2^22): large batches run more rounds but hash little past each
-// proof's first hit, small ones keep few rounds.  Measured on an H100 at 400 W, grinding 20, PoW
+// 2^(g - 2) for the largest grinding factor g, a quarter of its expected search (clamped to 2^10 .. 2^22): large batches run more rounds
+// but hash little past each proof's first hit, small ones keep few rounds.  Measured on an H100 at 400 W, grinding 20, PoW
 // stage of a batch of 16 / 64 / 256 proofs: 2^16: 1.17 / 3.02 / 11.7 ms; 2^18: 0.76 / 2.57 / 10.9; 2^19: 0.74 / 2.75 / 12.2; 2^20: 0.86 /
 // 3.30 / 14.8; 2^21: 1.34 / 4.84 / 21.2; 2^22: 2.24 / 8.87 / 36.3 ms.
-std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<std::array<uint8_t, 32>> &seeds, unsigned grinding) {
+std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<std::array<uint8_t, 32>> &seeds,
+                                                 const std::vector<unsigned> &grinding) {
     const unsigned K = (unsigned)seeds.size();
     std::vector<unsigned long long> best(K, ~0ULL);
     if (K == 0) return best;
     DG_REQUIRE(K <= 65535, "too many proof-of-work seeds for one launch");
-    DevBuf d_seeds((size_t)32 * K), d_best((size_t)8 * K), d_active((size_t)4 * K);
-    DG_CUDA(cudaMemcpyAsync(d_seeds.p, seeds.data(), (size_t)32 * K, cudaMemcpyHostToDevice, c.stream));
+    DG_REQUIRE(grinding.size() == K, "one grinding factor per proof-of-work seed");
+    // one upload: the seeds [K][8 words], then the grinding factors [K]
+    std::vector<uint32_t> in((size_t)9 * K);
+    memcpy(in.data(), seeds.data(), (size_t)32 * K);
+    std::copy(grinding.begin(), grinding.end(), in.begin() + (size_t)8 * K);
+    DevBuf d_seeds(in.size() * 4), d_best((size_t)8 * K), d_active((size_t)4 * K);
+    DG_CUDA(cudaMemcpyAsync(d_seeds.p, in.data(), in.size() * 4, cudaMemcpyHostToDevice, c.stream));
     DG_CUDA(cudaMemcpyAsync(d_best.p, best.data(), (size_t)8 * K, cudaMemcpyHostToDevice, c.stream));
     unsigned long long window = 1ULL << 22;
     if (K > 1) {
         int log_k = 0;
         while ((1u << log_k) < K) log_k++;
-        window = 1ULL << std::max(10, std::min(22, std::max((int)grinding - 2, 22 - log_k)));
+        const unsigned gmax = *std::max_element(grinding.begin(), grinding.end());
+        window = 1ULL << std::max(10, std::min(22, std::max((int)gmax - 2, 22 - log_k)));
     }
     std::vector<unsigned> active(K);
     for (unsigned p = 0; p < K; p++) active[p] = p;
@@ -254,7 +263,8 @@ std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<s
     for (unsigned long long start = 1; start < (1ULL << 42); start += window) {
         if (upload) DG_CUDA(cudaMemcpyAsync(d_active.p, active.data(), (size_t)4 * active.size(), cudaMemcpyHostToDevice, c.stream));
         pow_batch_kernel<<<dim3((unsigned)(window / 256), (unsigned)active.size()), 256, 0, c.stream>>>(
-            d_seeds.as<uint32_t>(), d_active.as<unsigned>(), start, window, grinding, d_best.as<unsigned long long>()); c.launches++;
+            d_seeds.as<uint32_t>(), d_seeds.as<unsigned>() + (size_t)8 * K, d_active.as<unsigned>(), start, window, d_best.as<unsigned long long>());
+        c.launches++;
         DG_CUDA(cudaGetLastError());
         DG_CUDA(cudaMemcpyAsync(best.data(), d_best.p, (size_t)8 * K, cudaMemcpyDeviceToHost, c.stream));
         DG_CUDA(cudaStreamSynchronize(c.stream));

@@ -72,8 +72,9 @@ void alg_hash64(Context &c, int hash_id, const void *in, void *out, unsigned lon
 constexpr unsigned long long HASHER_WIDE_MIN = 1ULL << 16;     // measured crossover on an H100 (DESIGN.md section 7j)
 void hasher_digest(Context &c, const void *in, void *out, unsigned long long n);
 void alg_merkle_build(Context &c, int hash_id, const void *leaves, void *nodes, unsigned long long L);
-// the smallest proof-of-work nonce >= 1 of every seed, one kernel per round for all of them; result i belongs to seeds[i]
-std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<std::array<uint8_t, 32>> &seeds, unsigned grinding);
+// the smallest proof-of-work nonce >= 1 of every seed for its own grinding factor (grinding[i] of seeds[i]), one kernel per round for
+// all of them; result i belongs to seeds[i]
+std::vector<unsigned long long> pow_search_batch(Context &c, const std::vector<std::array<uint8_t, 32>> &seeds, const std::vector<unsigned> &grinding);
 void pow_hash(const uint8_t seed[32], unsigned long long nonce, uint8_t out[32]);
 
 // ---- FRI (fri.cu) ----

@@ -102,6 +102,13 @@ struct FriLayerDev {
 
 }  // namespace
 
+void check_options(const dg_options_t &o) {
+    DG_REQUIRE(o.hash_id == 0, "unsupported hash function (only blake3 is serialisable, options.rs:107)");
+    require_extension_factor(o.extension_factor);
+    DG_REQUIRE(o.num_queries > 0 && o.num_queries <= 128, "num_queries must be in 1..128");
+    DG_REQUIRE(o.grinding_factor <= 32, "grinding factor cannot be greater than 32");
+}
+
 // prover.h; dg_test_trace_lde calls it as stage 1 does
 void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
                           unsigned nc) {
@@ -259,7 +266,8 @@ struct OpenPlan {
 
 }  // namespace
 
-// Proves K traces of one length (K == 1: dg_prove / dg_prove_device).  Every device buffer is proof-major: the registers, polynomials and
+// Proves K traces of one length and extension factor (K == 1: dg_prove / dg_prove_device); opts[p] are proof p's options, which may
+// differ in num_queries and grinding_factor.  Every device buffer is proof-major: the registers, polynomials and
 // trace extension are sum(w_p) columns, proof p's w_p columns from column col0[p] on, and every per-proof vector ([K][...]) has the
 // single-proof layout inside.  So the transforms run once over all the proofs' columns, and each host round trip (violation flags, roots,
 // DEEP values, FRI roots, PoW, openings) moves the values of all K proofs at once.  shapes[p] is proof p's register shape; proofs of one
@@ -270,19 +278,19 @@ struct OpenPlan {
 // LDE).  chunk (one GPU): cosets of the trace extension held at a time (ProvePlan).  The full layout (chunk = b) keeps the whole extension;
 // the evaluation-coset layout (chunk < b) extends and hashes chunk cosets at a time and keeps only the 8 cosets stage 3 reads.
 static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, const std::vector<RegisterShape> &regs_shape, uint64_t length,
-                       const std::vector<int> &order, std::vector<ProofState> &ps, const dg_options_t &opt, dg_prove_stats_t *stats,
-                       unsigned chunk) {
+                       const std::vector<int> &order, std::vector<ProofState> &ps, const std::vector<dg_options_t> &opts,
+                       dg_prove_stats_t *stats, unsigned chunk) {
     // ---- argument checks (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) -----------------------------------------------
-    const uint64_t n = length, b = opt.extension_factor;
     const int K = (int)ps.size();
-    DG_REQUIRE(K >= 1 && regs_shape.size() == ps.size() && order.size() == ps.size(), "batch must hold at least one trace");
+    DG_REQUIRE(K >= 1 && regs_shape.size() == ps.size() && order.size() == ps.size() && opts.size() == ps.size(), "batch must hold at least one trace");
+    const uint64_t n = length, b = opts[0].extension_factor;
     size_t W = 0;                                              // columns of the whole batch
     for (const RegisterShape &r : regs_shape) W += r.width;
     DG_REQUIRE(W <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
-    DG_REQUIRE(opt.hash_id == 0, "unsupported hash function (only blake3 is serialisable, options.rs:107)");
-    require_extension_factor(b);
-    DG_REQUIRE(opt.num_queries > 0 && opt.num_queries <= 128, "num_queries must be in 1..128");
-    DG_REQUIRE(opt.grinding_factor <= 32, "grinding factor cannot be greater than 32");
+    for (const dg_options_t &o : opts) {
+        check_options(o);
+        DG_REQUIRE(o.extension_factor == b, "the proofs of a group share one extension factor");
+    }
     DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
     std::vector<TraceShape> shapes;
     for (const RegisterShape &r : regs_shape) shapes.push_back(TraceShape::of_trace(r.width, r.ctx_depth, r.loop_depth));
@@ -297,10 +305,10 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     const int log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
     DG_REQUIRE(log_N <= 30, "LDE domain too large");
     const uint64_t N = n * b, E = n * 8;
-    for (int p = 0; p < K; p++) {             // what the call fixes in every proof: the register shape and the options (blake3)
+    for (int p = 0; p < K; p++) {             // what the call fixes in every proof: the register shape and its options (blake3)
         TraceInfo &t = ps[p].stark.trace_info;
         t.ctx_depth = (uint8_t)shapes[p].ctx_depth; t.loop_depth = (uint8_t)shapes[p].loop_depth; t.stack_depth = (uint8_t)shapes[p].stack_depth;
-        ps[p].stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opt.num_queries, (uint8_t)opt.grinding_factor, 0};
+        ps[p].stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opts[p].num_queries, (uint8_t)opts[p].grinding_factor, 0};
     }
     // runs of proofs of one shape: [shape_first[s], shape_first[s + 1])
     std::vector<int> shape_first = {0};
@@ -817,6 +825,7 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
     sub.mark("7.fri");
     {
         std::vector<std::array<uint8_t, 32>> seeds;
+        std::vector<unsigned> grinding;
         std::vector<int> who;
         for (int p : order) {
             if (!ps[p].live) continue;
@@ -827,15 +836,16 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
             if (K == 1) debug_dump_host("fri_roots", roots.data(), roots.size());
             seeds.emplace_back();
             fs::blake3_short(roots.data(), roots.size(), seeds.back().data());
+            grinding.push_back(ps[p].stark.options.grinding_factor);
             who.push_back(p);
         }
-        std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, opt.grinding_factor);
+        std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, grinding);
         for (size_t i = 0; i < who.size(); i++) {
             ProofState &s = ps[who[i]];
             s.stark.pow_nonce = nonces[i];
             pow_hash(seeds[i].data(), s.stark.pow_nonce, s.proof->pow_seed);
             try {
-                s.positions = fs::query_positions(s.proof->pow_seed, N, b, opt.num_queries);
+                s.positions = fs::query_positions(s.proof->pow_seed, N, b, s.stark.options.num_queries);
             } catch (const std::exception &e) { s.fail(DG_ERR_EXHAUSTED, e.what()); continue; }
             if (K == 1) debug_dump_host("positions", s.positions.data(), s.positions.size() * 8);
         }
@@ -1144,12 +1154,13 @@ std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t co
     return cols;
 }
 
-std::vector<std::vector<uint32_t>> partition_by_length(const std::vector<uint64_t> &length) {
+std::vector<std::vector<uint32_t>> partition_traces(const std::vector<uint64_t> &length, const std::vector<uint32_t> &extension_factor) {
     std::vector<std::vector<uint32_t>> parts;
-    std::vector<uint64_t> seen;
+    std::vector<std::pair<uint64_t, uint32_t>> seen;
     for (uint32_t i = 0; i < length.size(); i++) {
-        const size_t at = std::find(seen.begin(), seen.end(), length[i]) - seen.begin();
-        if (at == seen.size()) { seen.push_back(length[i]); parts.emplace_back(); }
+        const std::pair<uint64_t, uint32_t> key{length[i], extension_factor[i]};
+        const size_t at = std::find(seen.begin(), seen.end(), key) - seen.begin();
+        if (at == seen.size()) { seen.push_back(key); parts.emplace_back(); }
         parts[at].push_back(i);
     }
     return parts;
@@ -1182,10 +1193,11 @@ std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape) {
 }
 
 void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const std::vector<dg_options_t> &opts, bool batch,
+                  Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
     const uint32_t count = (uint32_t)traces.size();
     DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+    DG_REQUIRE(opts.size() == count, "one set of options per trace");
     const bool host = traces[0].host_cols != nullptr;
     if (host)
         for (const TraceRef &t : traces)
@@ -1193,26 +1205,28 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
     if (batch)
         DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
-    // every length's plan and groups before any proof runs: a length that fits in no way fails the call before the device computes
+    // every partition's plan and groups before any proof runs: a partition that fits in no way fails the call before the device computes
     std::vector<uint64_t> lengths;
-    for (const TraceRef &t : traces) lengths.push_back(t.length);
-    struct LengthRun { std::vector<uint32_t> idx; ProvePlan plan; std::vector<uint32_t> sizes; };
-    std::vector<LengthRun> runs;
-    for (std::vector<uint32_t> &idx : partition_by_length(lengths)) {
-        LengthRun r;
+    std::vector<uint32_t> factors;
+    for (uint32_t i = 0; i < count; i++) { lengths.push_back(traces[i].length); factors.push_back(opts[i].extension_factor); }
+    struct PartitionRun { std::vector<uint32_t> idx; ProvePlan plan; std::vector<uint32_t> sizes; };
+    std::vector<PartitionRun> runs;
+    for (std::vector<uint32_t> &idx : partition_traces(lengths, factors)) {
+        PartitionRun r;
         r.idx = std::move(idx);
         r.sizes.assign(r.idx.size(), 1);           // several GPUs (one trace): one group, and prove_core shards the full layout
         if (c.world == 1) {
-            // planned for the widest shape of the length: its group's bytes are the budget the groups of mixed widths are cut to
+            // planned for the widest shape of the partition: its group's bytes are the budget the groups of mixed widths are cut to
             uint32_t wmax = 0;
             for (uint32_t i : r.idx) wmax = std::max(wmax, traces[i].width);
             const uint64_t n = traces[r.idx[0]].length;
-            r.plan = plan_prove(c, wmax, n, opt.extension_factor, (uint32_t)r.idx.size());
+            const uint32_t b = opts[r.idx[0]].extension_factor;
+            r.plan = plan_prove(c, wmax, n, b, (uint32_t)r.idx.size());
             std::vector<uint32_t> width;
             std::vector<size_t> foot;
             for (uint32_t i : r.idx) {
                 width.push_back(traces[i].width);
-                foot.push_back(proof_footprint(traces[i].width, n, opt.extension_factor, r.plan.chunk));
+                foot.push_back(proof_footprint(traces[i].width, n, b, r.plan.chunk));
             }
             r.sizes = cut_groups(width, foot, (size_t)r.plan.group * r.plan.per_proof, (uint32_t)r.plan.group);
         }
@@ -1227,7 +1241,7 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
         Proof **out; uint32_t count; bool done = false;
         ~ReleaseOnError() { if (!done) for (uint32_t i = 0; i < count; i++) { delete out[i]; out[i] = nullptr; } }
     } release{proofs_out, count};
-    for (const LengthRun &r : runs) {
+    for (const PartitionRun &r : runs) {
         const uint64_t n = traces[r.idx[0]].length;
         size_t first = 0;
         for (uint32_t k : r.sizes) {
@@ -1242,12 +1256,14 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
             for (uint32_t p = 0; p < k; p++) order[std::find(members.begin(), members.end(), dev[p]) - members.begin()] = (int)p;
             std::vector<ProofState> ps;
             std::vector<RegisterShape> shapes;
+            std::vector<dg_options_t> group_opts;
             std::vector<const uint8_t *> cols;
             size_t W = 0;
             for (uint32_t i : dev) {
                 const TraceRef &t = traces[i];
                 ps.push_back(std::move(all[i]));
                 shapes.push_back(t.shape());
+                group_opts.push_back(opts[i]);
                 if (host) cols.insert(cols.end(), t.host_cols, t.host_cols + t.width);
                 W += t.width;
             }
@@ -1255,11 +1271,13 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
             memset(&st, 0, sizeof st);
             prepare_arena(c, r.plan);
             // the group's registers as W columns: host traces are uploaded into the upload buffer by prove_core; device traces are read in
-            // place when they are adjacent in device memory (a one-shape batch), else copied there
+            // place when they are adjacent in one allocation (a one-shape batch), else copied there.  Separate allocations that happen to
+            // be adjacent are copied: a copy may not span two allocations.
             fe *regs = const_cast<fe *>(traces[dev[0]].d_regs);
             bool adjacent = !host;
             for (uint32_t p = 1; p < k && adjacent; p++)
-                adjacent = traces[dev[p]].d_regs == traces[dev[p - 1]].d_regs + (size_t)traces[dev[p - 1]].width * n;
+                adjacent = traces[dev[p]].slab && traces[dev[p]].slab == traces[dev[p - 1]].slab &&
+                           traces[dev[p]].d_regs == traces[dev[p - 1]].d_regs + (size_t)traces[dev[p - 1]].width * n;
             if (!adjacent) {
                 c.upload_buf.ensure((size_t)n * 16 * W, true);
                 regs = c.upload_buf.as<fe>();
@@ -1271,7 +1289,7 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
                     }
                 }
             }
-            prove_core(c, regs, host ? cols.data() : nullptr, shapes, n, order, ps, opt, &st, r.plan.chunk);
+            prove_core(c, regs, host ? cols.data() : nullptr, shapes, n, order, ps, group_opts, &st, r.plan.chunk);
             if (stats) add_stats(stats, st);
             if (groups) ++*groups;
             for (uint32_t p = 0; p < k; p++) {
@@ -1285,18 +1303,31 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
     release.done = true;
 }
 
-void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
                   int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
+    prove_traces(c, traces, inputs16, n_inputs, outputs16, n_outputs, std::vector<dg_options_t>(traces.size(), opt), batch, proofs_out, status,
+                 messages, stats, groups);
+}
+
+std::vector<TraceRef> one_shape_traces(const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                                       uint32_t ctx_depth, uint32_t loop_depth) {
     std::vector<TraceRef> traces(count);
     for (uint32_t i = 0; i < count; i++) {
         TraceRef &t = traces[i];
         t.width = width; t.length = length; t.ctx_depth = ctx_depth; t.loop_depth = loop_depth;
         if (host_cols) t.host_cols = host_cols + (size_t)i * width;
-        else t.d_regs = d_regs + (size_t)i * width * length;
+        else { t.d_regs = d_regs + (size_t)i * width * length; t.slab = d_regs; }
     }
-    prove_traces(c, traces, inputs16, n_inputs, outputs16, n_outputs, opt, batch, proofs_out, status, messages, stats, groups);
+    return traces;
+}
+
+void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
+                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
+    prove_traces(c, one_shape_traces(d_regs, host_cols, count, width, length, ctx_depth, loop_depth), inputs16, n_inputs, outputs16, n_outputs,
+                 opt, batch, proofs_out, status, messages, stats, groups);
 }
 
 }  // namespace dg

@@ -30,17 +30,28 @@ struct TraceRef {
     uint32_t ctx_depth = 0, loop_depth = 0;
     const uint8_t *const *host_cols = nullptr;
     const fe *d_regs = nullptr;
+    const void *slab = nullptr;        // device traces given as one allocation (a one-shape call): its base; null when not known
     RegisterShape shape() const { return RegisterShape{width, ctx_depth, loop_depth}; }
 };
-// The same for traces of any shapes and lengths (every trace host, or every trace on the device).  The call is partitioned by length
-// (partition_by_length); each length is planned for its widest shape (plan_prove) and cut into groups (cut_groups) of at most that plan's
-// bytes; inside a group the traces are laid out on the device by shape (shape_order).  The Fiat-Shamir draws run length by length, group
-// by group, stage by stage, and within a stage in input order.  Per trace, the result is the one-shape call's.
+// The same for traces of any shapes and lengths (every trace host, or every trace on the device), trace i proven with opts[i].  The call
+// is partitioned by (length, extension factor) (partition_traces); each partition is planned for its widest shape (plan_prove) and cut
+// into groups (cut_groups) of at most that plan's bytes; inside a group the traces are laid out on the device by shape (shape_order), and
+// their num_queries and grinding factors may differ.  The Fiat-Shamir draws run partition by partition, group by group, stage by stage,
+// and within a stage in input order.  Per trace, the result is the one-shape call's with that trace's options.
+void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const std::vector<dg_options_t> &opts, bool batch,
+                  Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
+// the same with one set of options for every trace
 void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
                   int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
-// the traces of each length, lengths in order of first appearance, traces in input order
-std::vector<std::vector<uint32_t>> partition_by_length(const std::vector<uint64_t> &length);
+// `count` traces of one shape: registers [count][width][length] on the device at d_regs, or host columns (count * width pointers)
+std::vector<TraceRef> one_shape_traces(const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
+                                       uint32_t ctx_depth, uint32_t loop_depth);
+// ProofOptions::new's checks (options.rs:29-50) and the hash (only blake3 is serialisable): DG_ERR_INVALID with the reason
+void check_options(const dg_options_t &o);
+// the traces of each (length, extension factor), partitions in order of first appearance, traces in input order
+std::vector<std::vector<uint32_t>> partition_traces(const std::vector<uint64_t> &length, const std::vector<uint32_t> &extension_factor);
 // sizes of the consecutive groups the traces (in this order) are cut into: a group holds at most `cap` traces, footprints summing to at
 // most `budget` bytes and widths summing to at most 65535 (one launch); a trace that exceeds the budget alone is a group of its own
 std::vector<uint32_t> cut_groups(const std::vector<uint32_t> &width, const std::vector<size_t> &footprint, size_t budget, uint32_t cap);
@@ -72,14 +83,15 @@ void check_execution_call(const ExecutionCall &x, const std::optional<OutputCoun
 // execute_programs writes 8 output elements per execution (zero past its num_outputs).
 void trace_programs(Context &c, const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
                     std::vector<std::string> &messages, dg_execution_stats_t *vm_stats);
-void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t &opt, Proof **proofs_out,
+// opts: the options of every execution (x.count entries)
+void execute_programs(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t *opts, Proof **proofs_out,
                       uint8_t *outputs16, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
 // dg_trace_many / dg_execute_many (dg_trace_one / dg_execute_one with one execution): trace_programs / execute_programs with the
 // executions run from the sponge tables.  info may be null.  stats (may be null) are written also when the tabled passes throw (dg_trace_one
 // reports a failed call's).
 void trace_many(Context &c, const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
                 std::vector<std::string> &messages, dg_many_stats_t *stats);
-void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t &opt,
+void execute_many(Context &c, const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t *opts,
                   Proof **proofs_out, uint8_t *outputs16, dg_execution_info_t *info, int *status, std::vector<std::string> &messages,
                   dg_prove_stats_t *prove_stats, dg_many_stats_t *stats);
 // the largest group of a batched call, after $DG_BATCH_GROUP

@@ -112,6 +112,20 @@ int dg_prove_traces_device(const void *const *d_registers, const uint32_t *width
                            const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                            const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                            int *status, dg_prove_stats_t *stats);
+/* Per-trace options: dg_prove_traces / dg_prove_traces_device with `options` an array of `count` entries, trace i proven with options[i];
+ * each proof is byte-identical to dg_prove of that trace with its options.  Every options[i] is checked on the host with the trace
+ * (DG_ERR_INVALID, "trace i: " before dg_prove's message).  The call is partitioned by (trace length, extension factor), partitions in
+ * order of first appearance; inside a partition the groups are cut as dg_prove_traces cuts a length, and the traces of one group may
+ * differ in num_queries and grinding_factor (every stage is still one launch per group; the proof-of-work rounds run until the largest
+ * grinding factor of the group is met, a proof leaving the rounds once it has its nonce).  RNG callbacks: partition by partition, inside a
+ * partition as dg_prove_traces inside a length; with all options equal this is dg_prove_traces' order and result. */
+int dg_prove_traces_with_options(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                                 const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                                 int *status, dg_prove_stats_t *stats);
+int dg_prove_traces_device_with_options(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                                        const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                                        const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options,
+                                        dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats);
 
 /* ---- checking a trace before proving it ------------------------------------------------------------------------------------------
  * dg_prove reports an unsatisfied trace late (after the trace LDE and commitment) and only with its lowest failing step; it does not check
@@ -263,6 +277,15 @@ int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_
 int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
                         const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
                         dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats);
+/* dg_execute_programs with `options` an array of `count` entries: execution i is proven with options[i], exactly as dg_execute_programs of
+ * it with those options alone.  Every options[i] is checked on the host before the device is touched (DG_ERR_INVALID, "execution i: "
+ * before dg_prove's message).  A wave leaves room for one proof of its largest shape and extension factor.  Each shape's traces of a wave
+ * are proven by one dg_prove_traces_with_options call: RNG callbacks shape by shape, inside a shape extension factor by extension factor
+ * (in order of first appearance), in input order inside those. */
+int dg_execute_programs_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                     const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                                     dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
+                                     dg_execution_stats_t *vm_stats);
 
 /* ---- executing one long program -------------------------------------------------------------------------------------------------
  * dg_trace_one / dg_execute_one: one execution of one program, split across GPU threads.  The batch calls above run an execution on one
@@ -332,6 +355,11 @@ int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t 
                     const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
                     const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
                     dg_many_stats_t *stats);
+/* dg_execute_many with `options` an array of `count` entries, as dg_execute_programs_with_options is to dg_execute_programs */
+int dg_execute_many_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                 const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                                 const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
+                                 dg_prove_stats_t *prove_stats, dg_many_stats_t *stats);
 
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
@@ -558,6 +586,11 @@ int dg_host_shard_locate(uint64_t n, int log_blk, int log_g, int is_node, uint64
 int dg_host_group_traces(uint32_t count, const uint64_t *lengths, const uint32_t *widths, const uint32_t *ctx_depths, const uint32_t *loop_depths,
                          const uint64_t *footprints, uint64_t budget, uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out,
                          uint32_t *n_groups);
+/* the same for dg_prove_traces_with_options: the traces partitioned by (length, extension_factors[i]), partitions in order of first
+ * appearance, each cut and ordered as above */
+int dg_host_group_traces_with_options(uint32_t count, const uint64_t *lengths, const uint32_t *extension_factors, const uint32_t *widths,
+                                      const uint32_t *ctx_depths, const uint32_t *loop_depths, const uint64_t *footprints, uint64_t budget,
+                                      uint32_t cap, uint32_t *order_out, uint32_t *group_sizes_out, uint32_t *n_groups);
 
 /* ---- host-side Fiat-Shamir glue, exported so that it can be unit-tested without a GPU (none of these touch the device) ---- */
 /* field::prng_vector (field.rs:271-275): count draws of StdRng::from_seed(seed) through Uniform(0..M) */
