@@ -96,33 +96,48 @@ def _collect(handle, stats):
     return StarkProof(buf.raw, digs[0], digs[1], digs[2], nonce.value, st)
 
 
-def prove(trace, options=None):
-    """stark::prove(&mut trace, inputs, outputs, options) for a hostvm.ExecutionTrace (host memory in, proof bytes out)."""
-    options = options or ProofOptions()
-    regs = np.ascontiguousarray(trace.registers, dtype=np.uint64)
-    w, n = regs.shape[0], regs.shape[1]
-    cols = (backend.vp * w)(*[regs[j].ctypes.data for j in range(w)])
-    t = backend.DgTrace(cols, w, n, trace.ctx_depth, trace.loop_depth)
-    fi, fo = felt.from_ints(trace.public_inputs), felt.from_ints(trace.outputs)
-    opt = options._c()
+def _dev_ptr(x):
+    """the address of device memory given as a backend.DeviceBuffer or a raw pointer"""
+    return x.ptr if isinstance(x, backend.DeviceBuffer) else int(x)
+
+
+def _c_traces(traces):
+    """the dg_trace_t array of hostvm.ExecutionTraces, and what keeps their columns alive"""
+    regs = [np.ascontiguousarray(tr.registers, dtype=np.uint64) for tr in traces]
+    cols = [(backend.vp * r.shape[0])(*[r[j].ctypes.data for j in range(r.shape[0])]) for r in regs]
+    ts = (backend.DgTrace * max(len(traces), 1))(*[backend.DgTrace(c, r.shape[0], r.shape[1], tr.ctx_depth, tr.loop_depth)
+                                                   for c, r, tr in zip(cols, regs, traces)])
+    return ts, (regs, cols)
+
+
+def _by_shape(traces):
+    """{(width, length, ctx_depth, loop_depth): indices of the traces of that shape}, shapes in order of first appearance"""
+    groups = {}
+    for i, tr in enumerate(traces):
+        groups.setdefault((tr.registers.shape[0], tr.registers.shape[1], tr.ctx_depth, tr.loop_depth), []).append(i)
+    return groups
+
+
+def _prove_one(entry, head, public_inputs, outputs, options):
+    """entry(*head, inputs, outputs, options, proof, stats) for one trace (dg_prove, dg_prove_device): its StarkProof"""
+    fi, fo = felt.from_ints(public_inputs), felt.from_ints(outputs)
+    opt = (options or ProofOptions())._c()
     handle = backend.vp()
     stats = backend.DgStats()
-    backend.check(backend.lib().dg_prove(ctypes.byref(t), fi.ctypes.data, len(fi), fo.ctypes.data, len(fo), ctypes.byref(opt),
-                                        ctypes.byref(handle), ctypes.byref(stats)))
+    backend.check(entry(*head, fi.ctypes.data, len(fi), fo.ctypes.data, len(fo), ctypes.byref(opt), ctypes.byref(handle), ctypes.byref(stats)))
     return _collect(handle, stats)
+
+
+def prove(trace, options=None):
+    """stark::prove(&mut trace, inputs, outputs, options) for a hostvm.ExecutionTrace (host memory in, proof bytes out)."""
+    ts, keep = _c_traces([trace])
+    return _prove_one(backend.lib().dg_prove, (ts,), trace.public_inputs, trace.outputs, options)
 
 
 def prove_device(d_registers, width, length, ctx_depth, loop_depth, public_inputs, outputs, options=None):
     """Same, for register traces already resident in device memory (backend.DeviceBuffer or raw pointer)."""
-    options = options or ProofOptions()
-    ptr = d_registers.ptr if isinstance(d_registers, backend.DeviceBuffer) else int(d_registers)
-    fi, fo = felt.from_ints(public_inputs), felt.from_ints(outputs)
-    opt = options._c()
-    handle = backend.vp()
-    stats = backend.DgStats()
-    backend.check(backend.lib().dg_prove_device(ptr, width, length, ctx_depth, loop_depth, fi.ctypes.data, len(fi), fo.ctypes.data, len(fo),
-                                               ctypes.byref(opt), ctypes.byref(handle), ctypes.byref(stats)))
-    return _collect(handle, stats)
+    return _prove_one(backend.lib().dg_prove_device, (_dev_ptr(d_registers), width, length, ctx_depth, loop_depth), public_inputs, outputs,
+                      options)
 
 
 def set_memory_limit(nbytes):
@@ -187,6 +202,18 @@ def _collect_batch(handles, status, stats):
     return [_collect(h, stats) if e is None else e for h, e in zip(handles, _messages(status))]
 
 
+def _prove_batched(entry, head, public_inputs_list, outputs_list, opt):
+    """entry(*head, public inputs / outputs, opt, proofs, status, stats) for a batched prove call, one trace per list of public inputs:
+    _collect_batch of its results"""
+    k = len(public_inputs_list)
+    keep, io = _batch_io(public_inputs_list, outputs_list)
+    handles = (backend.vp * max(k, 1))()
+    status = (ctypes.c_int * max(k, 1))()
+    stats = backend.DgStats()
+    backend.check(entry(*head, *io, opt, handles, status, ctypes.byref(stats)))
+    return _collect_batch(list(handles)[:k], list(status)[:k], stats)
+
+
 def prove_batch(traces, options=None):
     """Proves many hostvm.ExecutionTraces.  Traces of one shape (width, length, ctx_depth, loop_depth) are proven together by one
     dg_prove_batch call, each stage launched once for all of them.  Returns a list in input order: a StarkProof (byte-identical to
@@ -195,23 +222,13 @@ def prove_batch(traces, options=None):
     options = options or ProofOptions()
     opt = options._c()
     traces = list(traces)
-    groups = {}
-    for i, tr in enumerate(traces):
-        groups.setdefault((tr.registers.shape[0], tr.registers.shape[1], tr.ctx_depth, tr.loop_depth), []).append(i)
     result = [None] * len(traces)
-    for (w, n, ctx_depth, loop_depth), idx in groups.items():
-        k = len(idx)
-        regs = [np.ascontiguousarray(traces[i].registers, dtype=np.uint64) for i in idx]
-        cols = [(backend.vp * w)(*[r[j].ctypes.data for j in range(w)]) for r in regs]
-        ts = (backend.DgTrace * k)(*[backend.DgTrace(cols[m], w, n, ctx_depth, loop_depth) for m in range(k)])
-        keep, (pin, nin, pout, nout) = _batch_io([traces[i].public_inputs for i in idx], [traces[i].outputs for i in idx])
-        handles = (backend.vp * k)()
-        status = (ctypes.c_int * k)()
-        stats = backend.DgStats()
-        backend.check(backend.lib().dg_prove_batch(ts, k, pin, nin, pout, nout, ctypes.byref(opt), handles, status, ctypes.byref(stats)))
-        for i, entry in zip(idx, _collect_batch(list(handles), list(status), stats)):
+    for idx in _by_shape(traces).values():
+        ts, keep = _c_traces([traces[i] for i in idx])
+        proofs = _prove_batched(backend.lib().dg_prove_batch, (ts, len(idx)), [traces[i].public_inputs for i in idx],
+                                [traces[i].outputs for i in idx], ctypes.byref(opt))
+        for i, entry in zip(idx, proofs):
             result[i] = entry
-        del keep, regs, cols
     return result
 
 
@@ -220,16 +237,9 @@ def prove_batch_device(d_registers, count, width, length, ctx_depth, loop_depth,
     elements (backend.DeviceBuffer or raw pointer).  public_inputs_list / outputs_list hold one list per trace."""
     options = options or ProofOptions()
     assert len(public_inputs_list) == count and len(outputs_list) == count, "one list of public inputs and outputs per trace"
-    ptr = d_registers.ptr if isinstance(d_registers, backend.DeviceBuffer) else int(d_registers)
     opt = options._c()
-    keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
-    handles = (backend.vp * max(count, 1))()
-    status = (ctypes.c_int * max(count, 1))()
-    stats = backend.DgStats()
-    backend.check(backend.lib().dg_prove_batch_device(ptr, count, width, length, ctx_depth, loop_depth, pin, nin, pout, nout, ctypes.byref(opt),
-                                                     handles, status, ctypes.byref(stats)))
-    del keep
-    return _collect_batch(list(handles)[:count], list(status)[:count], stats)
+    return _prove_batched(backend.lib().dg_prove_batch_device, (_dev_ptr(d_registers), count, width, length, ctx_depth, loop_depth),
+                          public_inputs_list, outputs_list, ctypes.byref(opt))
 
 
 def _options_arg(options, k, what):
@@ -256,18 +266,9 @@ def prove_traces(traces, options=None):
     traces = list(traces)
     k = len(traces)
     opt, per_trace = _options_arg(options, k, "trace")
-    regs = [np.ascontiguousarray(tr.registers, dtype=np.uint64) for tr in traces]
-    cols = [(backend.vp * r.shape[0])(*[r[j].ctypes.data for j in range(r.shape[0])]) for r in regs]
-    ts = (backend.DgTrace * max(k, 1))(*[backend.DgTrace(cols[i], r.shape[0], r.shape[1], tr.ctx_depth, tr.loop_depth)
-                                        for i, (r, tr) in enumerate(zip(regs, traces))])
-    keep, (pin, nin, pout, nout) = _batch_io([tr.public_inputs for tr in traces], [tr.outputs for tr in traces])
-    handles = (backend.vp * max(k, 1))()
-    status = (ctypes.c_int * max(k, 1))()
-    st = backend.DgStats()
+    ts, keep = _c_traces(traces)
     fn = backend.lib().dg_prove_traces_with_options if per_trace else backend.lib().dg_prove_traces
-    backend.check(fn(ts, k, pin, nin, pout, nout, opt, handles, status, ctypes.byref(st)))
-    del keep, regs, cols
-    return _collect_batch(list(handles)[:k], list(status)[:k], st)
+    return _prove_batched(fn, (ts, k), [tr.public_inputs for tr in traces], [tr.outputs for tr in traces], opt)
 
 
 def prove_traces_device(d_registers, widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list, options=None):
@@ -276,17 +277,11 @@ def prove_traces_device(d_registers, widths, lengths, ctx_depths, loop_depths, p
     k = len(d_registers)
     assert all(len(a) == k for a in (widths, lengths, ctx_depths, loop_depths, public_inputs_list, outputs_list)), "one entry per trace"
     opt, per_trace = _options_arg(options, k, "trace")
-    ptrs = (backend.vp * max(k, 1))(*[d.ptr if isinstance(d, backend.DeviceBuffer) else int(d) for d in d_registers])
+    ptrs = (backend.vp * max(k, 1))(*[_dev_ptr(d) for d in d_registers])
     arr = lambda t, xs: (t * max(k, 1))(*[int(x) for x in xs])
-    keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
-    handles = (backend.vp * max(k, 1))()
-    status = (ctypes.c_int * max(k, 1))()
-    st = backend.DgStats()
     fn = backend.lib().dg_prove_traces_device_with_options if per_trace else backend.lib().dg_prove_traces_device
-    backend.check(fn(ptrs, arr(backend.u32, widths), arr(backend.u64, lengths), arr(backend.u32, ctx_depths), arr(backend.u32, loop_depths), k, pin,
-                     nin, pout, nout, opt, handles, status, ctypes.byref(st)))
-    del keep
-    return _collect_batch(list(handles)[:k], list(status)[:k], st)
+    head = (ptrs, arr(backend.u32, widths), arr(backend.u64, lengths), arr(backend.u32, ctx_depths), arr(backend.u32, loop_depths), k)
+    return _prove_batched(fn, head, public_inputs_list, outputs_list, opt)
 
 
 def group_traces(lengths, widths, ctx_depths, loop_depths, footprints, budget, cap, extension_factors=None):
@@ -454,15 +449,10 @@ def check_traces(traces, program_hashes=None, masks=False):
     traces = list(traces)
     if program_hashes is not None:
         program_hashes = list(program_hashes)
-    groups = {}
-    for i, tr in enumerate(traces):
-        groups.setdefault((tr.registers.shape[0], tr.registers.shape[1], tr.ctx_depth, tr.loop_depth), []).append(i)
     result = [None] * len(traces)
-    for (w, n, ctx_depth, loop_depth), idx in groups.items():
+    for (w, n, ctx_depth, loop_depth), idx in _by_shape(traces).items():
         k = len(idx)
-        regs = [np.ascontiguousarray(traces[i].registers, dtype=np.uint64) for i in idx]
-        cols = [(backend.vp * w)(*[r[j].ctypes.data for j in range(w)]) for r in regs]
-        ts = (backend.DgTrace * k)(*[backend.DgTrace(cols[m], w, n, ctx_depth, loop_depth) for m in range(k)])
+        ts, (regs, cols) = _c_traces([traces[i] for i in idx])
         keep, (pin, nin, pout, nout) = _batch_io([traces[i].public_inputs for i in idx], [traces[i].outputs for i in idx])
         hashes = _hashes([program_hashes[i] for i in idx], k) if program_hashes is not None else None
         reports = (backend.DgTraceReport * k)()
@@ -491,8 +481,8 @@ def check_traces_device(d_registers, count, width, length, ctx_depth, loop_depth
     (backend.DeviceBuffer or raw pointer), used in place.  d_masks: None, or device memory of count * length * 3 uint32 that receives
     the per-step masks.  Returns a TraceReport per trace."""
     assert len(public_inputs_list) == count and len(outputs_list) == count, "one list of public inputs and outputs per trace"
-    ptr = d_registers.ptr if isinstance(d_registers, backend.DeviceBuffer) else int(d_registers)
-    mptr = None if d_masks is None else (d_masks.ptr if isinstance(d_masks, backend.DeviceBuffer) else int(d_masks))
+    ptr = _dev_ptr(d_registers)
+    mptr = None if d_masks is None else _dev_ptr(d_masks)
     keep, (pin, nin, pout, nout) = _batch_io(public_inputs_list, outputs_list)
     reports = (backend.DgTraceReport * max(count, 1))()
     backend.check(backend.lib().dg_check_traces_device(ptr, count, width, length, ctx_depth, loop_depth, pin, nin, pout, nout,

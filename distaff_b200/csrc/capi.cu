@@ -677,93 +677,6 @@ int dg_eval_transitions(const uint8_t *ext16, uint32_t count, uint32_t ctx_depth
 }
 
 // ---- prover ------------------------------------------------------------------------------------------------------------------------
-// dg_prove / dg_prove_device: a batch of one whose failure is the call's error
-static Proof *prove_single(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t width, uint64_t length, uint32_t ctx_depth,
-                           uint32_t loop_depth, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
-                           const dg_options_t &opt, dg_prove_stats_t *stats) {
-    Proof *proof = nullptr;
-    int status = DG_OK;
-    std::vector<std::string> messages;
-    prove_traces(c, d_regs, host_cols, 1, width, length, ctx_depth, loop_depth, &inputs16, &n_inputs, &outputs16, &n_outputs, opt, false, &proof,
-                 &status, messages, stats);
-    if (status != DG_OK) throw Error(status, messages[0]);
-    return proof;
-}
-
-int dg_prove(const dg_trace_t *trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
-             const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats) {
-    return guarded([&] {
-        DG_REQUIRE(trace && options && proof_out, "null argument");
-        DG_REQUIRE((n_inputs == 0 || inputs16) && (n_outputs == 0 || outputs16), "null public inputs / outputs");
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        auto prove = [&](Context &cg, dg_prove_stats_t *st) {
-            const std::vector<const uint8_t *> cols = trace_columns(trace, 1, "call", true);
-            return prove_single(cg, nullptr, cols.data(), trace->width, trace->length, trace->ctx_depth, trace->loop_depth, inputs16, n_inputs,
-                                outputs16, n_outputs, *options, st);
-        };
-        *proof_out = (dg_proof_t *)(ctx_device_count() > 1 ? prove_on_all_devices(prove, stats) : prove(c, stats));
-    });
-}
-int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                    const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
-                    const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats) {
-    return guarded([&] {
-        DG_REQUIRE(d_registers && options && proof_out, "null argument");
-        DG_REQUIRE((n_inputs == 0 || inputs16) && (n_outputs == 0 || outputs16), "null public inputs / outputs");
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        // several devices: the trace lives on device 0; the other devices read their columns over NVLink (peer access)
-        auto prove = [&](Context &cg, dg_prove_stats_t *st) {
-            return prove_single(cg, (const fe *)d_registers, nullptr, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16,
-                                n_outputs, *options, st);
-        };
-        *proof_out = (dg_proof_t *)(ctx_device_count() > 1 ? prove_on_all_devices(prove, stats) : prove(c, stats));
-    });
-}
-int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
-                   int *status, dg_prove_stats_t *stats) {
-    return guarded([&] {
-        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        const std::vector<const uint8_t *> cols = trace_columns(traces, count, "batch", false);
-        const dg_trace_t &t = traces[0];
-        prove_traces(c, nullptr, cols.data(), count, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
-                     *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
-    });
-}
-int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
-                          const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
-                          const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
-    return guarded([&] {
-        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-        DG_REQUIRE(d_registers && options && proofs_out && status, "null argument");
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        prove_traces(c, (const fe *)d_registers, nullptr, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
-                     *options, true, (Proof **)proofs_out, status, t_batch_messages, stats);
-    });
-}
-// the checks dg_prove makes of a trace's shape, length and public inputs / outputs, on the host alone; a failure names the entry
-static void check_trace_entry(uint32_t i, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16,
-                              const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs) {
-    try {
-        DG_REQUIRE(width >= 16 && width < 128, "invalid trace");
-        DG_REQUIRE(length >= 16 && (length & (length - 1)) == 0 && length <= (1ULL << 30),
-                   "execution trace length must be a power of 2 and at least 16");
-        TraceShape::of_trace(width, ctx_depth, loop_depth);
-        const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
-        DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
-        DG_REQUIRE((ni == 0 || (inputs16 && inputs16[i])) && (no == 0 || (outputs16 && outputs16[i])), "null public inputs / outputs");
-    } catch (const Error &e) {
-        throw Error(e.code, "trace " + std::to_string(i) + ": " + e.what());
-    }
-}
 // the options of a call: one set for every entry (per_entry false), or options[i] for entry i, each checked on the host with `what i: `
 // before the message (dg_*_with_options)
 static std::vector<dg_options_t> call_options(const dg_options_t *options, uint32_t count, bool per_entry, const char *what) {
@@ -777,62 +690,169 @@ static std::vector<dg_options_t> call_options(const dg_options_t *options, uint3
     }
     return std::vector<dg_options_t>(options, options + count);
 }
-static void prove_host_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                              const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, bool per_trace,
-                              dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
-    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+
+// A prove or trace-check call as its entry received it: every trace host (dg_trace_t columns) or every trace on the device, and trace
+// i's n_inputs[i] public inputs at inputs16[i] and n_outputs[i] outputs at outputs16[i] (16 bytes each; a null count array: none).
+// one_shape: how the messages of a call of one shape name it ("batch" or "call": dg_prove, dg_prove_device, dg_prove_batch*,
+// dg_check_traces*); null for the per-trace calls (dg_prove_traces*), whose traces may differ in shape and whose messages name the trace.
+struct ProveCall {
+    std::vector<TraceRef> traces;
+    bool host;
+    const char *one_shape;
+    const uint8_t *const *inputs16;
+    const uint32_t *n_inputs;
+    const uint8_t *const *outputs16;
+    const uint32_t *n_outputs;
+};
+
+// Every prove and trace-check entry runs this once, before it touches the device.  Each trace in input order: the form of a host trace
+// (the shape of trace 0 in a call of one shape, columns, 16..127 registers), its length, its register shape (TraceShape::of_trace), its
+// registers and its public inputs / outputs; then the options of a prove call, one set or one per trace (per_trace).  A failure is
+// DG_ERR_INVALID, with `trace i: ` before the message of a per-trace call's trace and of per-trace options.  Returns every trace's options.
+static std::vector<dg_options_t> check_prove_call(const ProveCall &x, const dg_options_t *options = nullptr, bool per_trace = false) {
+    const TraceRef &t0 = x.traces[0];
+    for (uint32_t i = 0; i < x.traces.size(); i++) {
+        const TraceRef &t = x.traces[i];
+        try {
+            if (x.host) {
+                if (x.one_shape)
+                    DG_REQUIRE(t.shape() == t0.shape() && t.length == t0.length,
+                               std::string("all traces of a ") + x.one_shape + " must have the same width, length, context depth and loop depth");
+                DG_REQUIRE(t.host_cols && t.width >= 16 && t.width < 128, "invalid trace");
+            }
+            DG_REQUIRE(t.length >= 16 && (t.length & (t.length - 1)) == 0 && t.length <= (1ULL << 30),
+                       "execution trace length must be a power of 2 and at least 16");
+            TraceShape::of_trace(t.width, t.ctx_depth, t.loop_depth);
+            if (x.host)
+                for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.host_cols[j] != nullptr, "null register column");
+            else
+                DG_REQUIRE(t.d_regs, "null registers");
+            const uint32_t ni = x.n_inputs ? x.n_inputs[i] : 0, no = x.n_outputs ? x.n_outputs[i] : 0;
+            DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
+            DG_REQUIRE((ni == 0 || (x.inputs16 && x.inputs16[i])) && (no == 0 || (x.outputs16 && x.outputs16[i])), "null public inputs / outputs");
+        } catch (const Error &e) {
+            if (x.one_shape) throw;
+            throw Error(e.code, "trace " + std::to_string(i) + ": " + e.what());
+        }
+    }
+    if (!options) return {};
+    if (!per_trace) check_options(*options);
+    return call_options(options, (uint32_t)x.traces.size(), per_trace, "trace");
+}
+
+// the traces of a host call
+static std::vector<TraceRef> host_traces(const dg_trace_t *traces, uint32_t count) {
     std::vector<TraceRef> refs(count);
     for (uint32_t i = 0; i < count; i++) {
         const dg_trace_t &t = traces[i];
-        check_trace_entry(i, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs);
-        DG_REQUIRE(t.columns, "trace " + std::to_string(i) + ": null register columns");
-        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "trace " + std::to_string(i) + ": null register column");
         refs[i].width = t.width; refs[i].length = t.length; refs[i].ctx_depth = t.ctx_depth; refs[i].loop_depth = t.loop_depth;
         refs[i].host_cols = t.columns;
     }
-    const std::vector<dg_options_t> opts = call_options(options, count, per_trace, "trace");
-    Context &c = ctx();
-    std::lock_guard<std::mutex> lk(c.mu);
-    t_batch_messages.clear();
-    prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, opts, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+    return refs;
 }
-static void prove_device_traces(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
-                                const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                                const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, bool per_trace,
-                                dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
-    DG_REQUIRE(count >= 1, "batch must hold at least one trace");
-    DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
+// the traces of a per-trace device call: trace i's registers at d_registers[i]
+static std::vector<TraceRef> device_traces(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
+                                           const uint32_t *loop_depth, uint32_t count) {
     std::vector<TraceRef> refs(count);
     for (uint32_t i = 0; i < count; i++) {
-        check_trace_entry(i, width[i], length[i], ctx_depth[i], loop_depth[i], inputs16, n_inputs, outputs16, n_outputs);
-        DG_REQUIRE(d_registers[i], "trace " + std::to_string(i) + ": null registers");
         refs[i].width = width[i]; refs[i].length = length[i]; refs[i].ctx_depth = ctx_depth[i]; refs[i].loop_depth = loop_depth[i];
         refs[i].d_regs = (const fe *)d_registers[i];
     }
-    const std::vector<dg_options_t> opts = call_options(options, count, per_trace, "trace");
+    return refs;
+}
+
+// Checks a prove call (check_prove_call) and proves it.  A batched call (batch) writes every trace's proof and status, and its message to
+// the thread's dg_batch_message list.  dg_prove / dg_prove_device put the one proof in proofs_out[0] or throw its failure; when the
+// library spans several devices every device proves it, sharded.
+static void prove_call(const ProveCall &x, const dg_options_t *options, bool per_trace, bool batch, dg_proof_t **proofs_out, int *status,
+                       dg_prove_stats_t *stats) {
+    const std::vector<dg_options_t> opts = check_prove_call(x, options, per_trace);
     Context &c = ctx();
     std::lock_guard<std::mutex> lk(c.mu);
-    t_batch_messages.clear();
-    prove_traces(c, refs, inputs16, n_inputs, outputs16, n_outputs, opts, true, (Proof **)proofs_out, status, t_batch_messages, stats);
+    if (batch) {
+        t_batch_messages.clear();
+        prove_traces(c, x.traces, x.inputs16, x.n_inputs, x.outputs16, x.n_outputs, opts, true, (Proof **)proofs_out, status, t_batch_messages,
+                     stats);
+        return;
+    }
+    auto prove = [&](Context &cg, dg_prove_stats_t *st) {
+        Proof *proof = nullptr;
+        int one = DG_OK;
+        std::vector<std::string> messages;
+        prove_traces(cg, x.traces, x.inputs16, x.n_inputs, x.outputs16, x.n_outputs, opts, false, &proof, &one, messages, st);
+        if (one != DG_OK) throw Error(one, messages[0]);
+        return proof;
+    };
+    *proofs_out = (dg_proof_t *)(ctx_device_count() > 1 ? prove_on_all_devices(prove, stats) : prove(c, stats));
+}
+
+int dg_prove(const dg_trace_t *trace, const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
+             const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(trace && options && proof_out, "null argument");
+        prove_call({host_traces(trace, 1), true, "call", &inputs16, &n_inputs, &outputs16, &n_outputs},
+                   options, false, false, proof_out, nullptr, stats);
+    });
+}
+int dg_prove_device(const void *d_registers, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                    const uint8_t *inputs16, uint32_t n_inputs, const uint8_t *outputs16, uint32_t n_outputs,
+                    const dg_options_t *options, dg_proof_t **proof_out, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(d_registers && options && proof_out, "null argument");
+        // several devices: the trace lives on device 0; the other devices read their columns over NVLink (peer access)
+        prove_call({one_shape_traces((const fe *)d_registers, 1, width, length, ctx_depth, loop_depth), false, "call", &inputs16, &n_inputs,
+                    &outputs16, &n_outputs}, options, false, false, proof_out, nullptr, stats);
+    });
+}
+int dg_prove_batch(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
+                   int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+        prove_call({host_traces(traces, count), true, "batch", inputs16, n_inputs, outputs16, n_outputs},
+                   options, false, true, proofs_out, status, stats);
+    });
+}
+int dg_prove_batch_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
+                          const uint8_t *const *inputs16, const uint32_t *n_inputs, const uint8_t *const *outputs16, const uint32_t *n_outputs,
+                          const dg_options_t *options, dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(d_registers && options && proofs_out && status, "null argument");
+        prove_call({one_shape_traces((const fe *)d_registers, count, width, length, ctx_depth, loop_depth), false, "batch", inputs16, n_inputs,
+                    outputs16, n_outputs}, options, false, true, proofs_out, status, stats);
+    });
 }
 int dg_prove_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                     const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                     int *status, dg_prove_stats_t *stats) {
-    return guarded([&] { prove_host_traces(traces, count, inputs16, n_inputs, outputs16, n_outputs, options, false, proofs_out, status, stats); });
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+        prove_call({host_traces(traces, count), true, nullptr, inputs16, n_inputs, outputs16, n_outputs},
+                   options, false, true, proofs_out, status, stats);
+    });
 }
 int dg_prove_traces_with_options(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                                  int *status, dg_prove_stats_t *stats) {
-    return guarded([&] { prove_host_traces(traces, count, inputs16, n_inputs, outputs16, n_outputs, options, true, proofs_out, status, stats); });
+    return guarded([&] {
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(traces && options && proofs_out && status, "null argument");
+        prove_call({host_traces(traces, count), true, nullptr, inputs16, n_inputs, outputs16, n_outputs},
+                   options, true, true, proofs_out, status, stats);
+    });
 }
 int dg_prove_traces_device(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
                            const uint32_t *loop_depth, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                            const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options, dg_proof_t **proofs_out,
                            int *status, dg_prove_stats_t *stats) {
     return guarded([&] {
-        prove_device_traces(d_registers, width, length, ctx_depth, loop_depth, count, inputs16, n_inputs, outputs16, n_outputs, options, false,
-                            proofs_out, status, stats);
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
+        prove_call({device_traces(d_registers, width, length, ctx_depth, loop_depth, count), false, nullptr, inputs16, n_inputs, outputs16,
+                    n_outputs}, options, false, true, proofs_out, status, stats);
     });
 }
 int dg_prove_traces_device_with_options(const void *const *d_registers, const uint32_t *width, const uint64_t *length, const uint32_t *ctx_depth,
@@ -840,8 +860,10 @@ int dg_prove_traces_device_with_options(const void *const *d_registers, const ui
                                         const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t *options,
                                         dg_proof_t **proofs_out, int *status, dg_prove_stats_t *stats) {
     return guarded([&] {
-        prove_device_traces(d_registers, width, length, ctx_depth, loop_depth, count, inputs16, n_inputs, outputs16, n_outputs, options, true,
-                            proofs_out, status, stats);
+        DG_REQUIRE(count >= 1, "batch must hold at least one trace");
+        DG_REQUIRE(d_registers && width && length && ctx_depth && loop_depth && options && proofs_out && status, "null argument");
+        prove_call({device_traces(d_registers, width, length, ctx_depth, loop_depth, count), false, nullptr, inputs16, n_inputs, outputs16,
+                    n_outputs}, options, true, true, proofs_out, status, stats);
     });
 }
 int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *const *inputs16, const uint32_t *n_inputs,
@@ -850,12 +872,11 @@ int dg_check_traces(const dg_trace_t *traces, uint32_t count, const uint8_t *con
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one trace must be checked");
         DG_REQUIRE(traces && reports, "null argument");
-        const std::vector<const uint8_t *> cols = trace_columns(traces, count, "call", false);
-        const dg_trace_t &t = traces[0];
+        const ProveCall x{host_traces(traces, count), true, "call", inputs16, n_inputs, outputs16, n_outputs};
+        check_prove_call(x);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        check_traces(c, nullptr, cols.data(), count, t.width, t.length, t.ctx_depth, t.loop_depth, inputs16, n_inputs, outputs16, n_outputs,
-                     program_hashes32, reports, step_masks, nullptr);
+        check_traces(c, x.traces, inputs16, n_inputs, outputs16, n_outputs, program_hashes32, reports, step_masks, nullptr);
     });
 }
 int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth,
@@ -864,10 +885,12 @@ int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t wid
     return guarded([&] {
         DG_REQUIRE(count >= 1, "at least one trace must be checked");
         DG_REQUIRE(d_registers && reports, "null argument");
+        const ProveCall x{one_shape_traces((const fe *)d_registers, count, width, length, ctx_depth, loop_depth), false, "call", inputs16, n_inputs,
+                          outputs16, n_outputs};
+        check_prove_call(x);
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
-        check_traces(c, (const fe *)d_registers, nullptr, count, width, length, ctx_depth, loop_depth, inputs16, n_inputs, outputs16, n_outputs,
-                     program_hashes32, reports, nullptr, d_step_masks);
+        check_traces(c, x.traces, inputs16, n_inputs, outputs16, n_outputs, program_hashes32, reports, nullptr, d_step_masks);
     });
 }
 int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,

@@ -49,36 +49,29 @@ std::string constraint_name(uint32_t ctx_depth, uint32_t loop_depth, uint32_t st
     return "stack slot " + std::to_string(index - 2);
 }
 
-void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+void check_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
                   uint32_t *step_masks, uint32_t *d_step_masks) {
-    // ---- the argument checks of dg_prove (trace_table.rs:23-58) ---------------------------------------------------------------------
-    const uint64_t n = length;
-    DG_REQUIRE(count >= 1, "at least one trace must be checked");
-    DG_REQUIRE(reports && (d_regs || host_cols), "null argument");
-    DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    const TraceShape shape = TraceShape::of_trace(width, ctx_depth, loop_depth);
+    const uint32_t count = (uint32_t)traces.size();
+    const uint64_t n = traces[0].length;
+    const bool host = traces[0].host_cols != nullptr;
+    const TraceShape shape = TraceShape::of_trace(traces[0].width, traces[0].ctx_depth, traces[0].loop_depth);
     const int w = shape.w, stack_depth = shape.stack_depth, T = shape.T, stk = shape.stack_reg;
-    DG_REQUIRE(ceil_log2(n) <= 32, "execution trace too long");
-    for (uint32_t i = 0; i < count; i++) {
-        const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
-        DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
-        DG_REQUIRE((ni == 0 || (inputs16 && inputs16[i])) && (no == 0 || (outputs16 && outputs16[i])), "null public inputs / outputs");
-    }
     DG_REQUIRE(c.world == 1 && ctx_device_count() == 1,
                "the trace check runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
     const fe *periodic = periodic_table(c);
-    const int group = check_group_size(width, n, host_cols != nullptr, d_step_masks == nullptr, count);
+    const int group = check_group_size(w, n, host, d_step_masks == nullptr, count);
     DevBuf d_masks, d_stats;
     std::vector<unsigned long long> stats;
     std::vector<fe> rows_first, rows_last;
     for (uint32_t first = 0; first < count; first += group) {
         const int k = (int)std::min<uint32_t>(group, count - first);
-        const fe *regs = d_regs ? d_regs + (size_t)first * w * n : nullptr;
-        if (!regs) {
+        const fe *regs = traces[first].d_regs;
+        if (host) {
+            std::vector<const uint8_t *> cols;
+            for (int q = 0; q < k; q++) cols.insert(cols.end(), traces[first + q].host_cols, traces[first + q].host_cols + w);
             c.upload_buf.ensure((size_t)k * w * n * 16, true);
-            upload_trace_columns(c, c.upload_buf.as<fe>(), host_cols + (size_t)first * w, k * w, n);
+            upload_trace_columns(c, c.upload_buf.as<fe>(), cols.data(), k * w, n);
             regs = c.upload_buf.as<fe>();
         }
         unsigned *masks = d_step_masks;

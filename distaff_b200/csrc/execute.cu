@@ -431,17 +431,14 @@ void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, cons
         dg_prove_stats_t gs;
         memset(&gs, 0, sizeof gs);
         uint32_t g = 0;
-        prove_traces(c, one_shape_traces(s.regs, nullptr, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth), in16.data(),
+        prove_traces(c, one_shape_traces(s.regs, k, s.shape.width, s.shape.length, s.shape.ctx_depth, s.shape.loop_depth), in16.data(),
                      n_in.data(), out16.data(), n_out.data(), opt, true, proofs.data(), st.data(), msg, &gs, &g);
         for (uint32_t q = 0; q < k; q++) {
             proofs_out[ok[q]] = proofs[q];
             if (st[q] != DG_OK) X.fail(ok[q], st[q], msg[q]);
         }
         groups += g;
-        if (stats) {
-            for (int i = 0; i < 9; i++) stats->stage_ms[i] += gs.stage_ms[i];
-            stats->h2d_ms += gs.h2d_ms; stats->total_ms += gs.total_ms; stats->kernel_launches += gs.kernel_launches;
-        }
+        if (stats) add_stats(stats, gs);
     }
 }
 

@@ -1024,8 +1024,6 @@ std::vector<ProofState> make_states(uint32_t count, const uint8_t *const *inputs
     std::vector<ProofState> ps(count);
     for (uint32_t i = 0; i < count; i++) {
         const uint32_t ni = n_inputs ? n_inputs[i] : 0, no = n_outputs ? n_outputs[i] : 0;
-        DG_REQUIRE(ni <= 8 && no <= 8, "cannot have more than 8 public inputs / outputs");
-        DG_REQUIRE((ni == 0 || (inputs16 && inputs16[i])) && (no == 0 || (outputs16 && outputs16[i])), "null public inputs / outputs");
         ps[i].inputs.resize(ni);
         ps[i].outputs.resize(no);
         if (ni) memcpy(ps[i].inputs.data(), inputs16[i], ni * 16);
@@ -1130,28 +1128,13 @@ void prepare_arena(Context &c, const ProvePlan &P) {
     if (c.mem_limit && c.arena.base && (size_t)P.group * P.per_proof > c.arena.cap) arena_release(c);
 }
 
+}  // namespace
+
 void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s) {
     for (int i = 0; i < 9; i++) sum->stage_ms[i] += s.stage_ms[i];
     sum->h2d_ms += s.h2d_ms;
     sum->total_ms += s.total_ms;
     sum->kernel_launches += s.kernel_launches;
-}
-
-}  // namespace
-
-std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first) {
-    const dg_trace_t &t0 = traces[0];
-    std::vector<const uint8_t *> cols;
-    for (uint32_t i = 0; i < count; i++) {
-        const dg_trace_t &t = traces[i];
-        DG_REQUIRE(t.width == t0.width && t.length == t0.length && t.ctx_depth == t0.ctx_depth && t.loop_depth == t0.loop_depth,
-                   std::string("all traces of a ") + call + " must have the same width, length, context depth and loop depth");
-        DG_REQUIRE(t.columns && t.width >= 16 && t.width < 128, "invalid trace");
-        if (length_first) DG_REQUIRE(t.length >= 16 && (t.length & (t.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-        for (uint32_t j = 0; j < t.width; j++) DG_REQUIRE(t.columns[j] != nullptr, "null register column");
-        cols.insert(cols.end(), t.columns, t.columns + t.width);
-    }
-    return cols;
 }
 
 std::vector<std::vector<uint32_t>> partition_traces(const std::vector<uint64_t> &length, const std::vector<uint32_t> &extension_factor) {
@@ -1199,9 +1182,6 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
     DG_REQUIRE(count >= 1, "batch must hold at least one trace");
     DG_REQUIRE(opts.size() == count, "one set of options per trace");
     const bool host = traces[0].host_cols != nullptr;
-    if (host)
-        for (const TraceRef &t : traces)
-            DG_REQUIRE(t.length >= 16 && (t.length & (t.length - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
     std::vector<ProofState> all = make_states(count, inputs16, n_inputs, outputs16, n_outputs);
     if (batch)
         DG_REQUIRE(c.world == 1 && ctx_device_count() == 1, "batched proving runs on one GPU: the library was initialised for several (dg_init_devices / dg_comm_init)");
@@ -1303,31 +1283,15 @@ void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t
     release.done = true;
 }
 
-void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
-    prove_traces(c, traces, inputs16, n_inputs, outputs16, n_outputs, std::vector<dg_options_t>(traces.size(), opt), batch, proofs_out, status,
-                 messages, stats, groups);
-}
-
-std::vector<TraceRef> one_shape_traces(const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                                       uint32_t ctx_depth, uint32_t loop_depth) {
+std::vector<TraceRef> one_shape_traces(const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth) {
     std::vector<TraceRef> traces(count);
     for (uint32_t i = 0; i < count; i++) {
         TraceRef &t = traces[i];
         t.width = width; t.length = length; t.ctx_depth = ctx_depth; t.loop_depth = loop_depth;
-        if (host_cols) t.host_cols = host_cols + (size_t)i * width;
-        else { t.d_regs = d_regs + (size_t)i * width * length; t.slab = d_regs; }
+        t.d_regs = d_regs + (size_t)i * width * length;
+        t.slab = d_regs;
     }
     return traces;
-}
-
-void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups) {
-    prove_traces(c, one_shape_traces(d_regs, host_cols, count, width, length, ctx_depth, loop_depth), inputs16, n_inputs, outputs16, n_outputs,
-                 opt, batch, proofs_out, status, messages, stats, groups);
 }
 
 }  // namespace dg

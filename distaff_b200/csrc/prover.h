@@ -8,16 +8,6 @@
 
 namespace dg {
 
-// Proves `count` traces of one shape: registers on the device ([count][width][length] at d_regs), or host columns (host_cols: count * width
-// pointers) uploaded group by group into c.upload_buf.  On one GPU the call is planned (plan_prove) and runs in groups; on several
-// (dg_prove on every rank) it proves one trace, sharded.  batch: a batched call, which runs on one GPU only.  proofs_out[i] / status[i] /
-// messages[i] (why trace i failed, else empty) per trace; when the call throws, no proof is left in proofs_out.  groups (may be null)
-// receives the number of groups the traces ran in.
-void prove_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
-
 // what the caller gives of a trace's register shape (TraceShape::of_trace checks it and derives the rest)
 struct RegisterShape {
     uint32_t width, ctx_depth, loop_depth;
@@ -33,21 +23,23 @@ struct TraceRef {
     const void *slab = nullptr;        // device traces given as one allocation (a one-shape call): its base; null when not known
     RegisterShape shape() const { return RegisterShape{width, ctx_depth, loop_depth}; }
 };
-// The same for traces of any shapes and lengths (every trace host, or every trace on the device), trace i proven with opts[i].  The call
-// is partitioned by (length, extension factor) (partition_traces); each partition is planned for its widest shape (plan_prove) and cut
-// into groups (cut_groups) of at most that plan's bytes; inside a group the traces are laid out on the device by shape (shape_order), and
-// their num_queries and grinding factors may differ.  The Fiat-Shamir draws run partition by partition, group by group, stage by stage,
-// and within a stage in input order.  Per trace, the result is the one-shape call's with that trace's options.
+// Proves traces of any shapes and lengths (every trace host, or every trace on the device), trace i with opts[i] and the public inputs /
+// outputs inputs16[i] (n_inputs[i] elements) and outputs16[i].  The call is partitioned by (length, extension factor)
+// (partition_traces); each partition is planned for its widest shape (plan_prove) and cut into groups (cut_groups) of at most that
+// plan's bytes; inside a group the traces are laid out on the device by shape (shape_order), and their num_queries and grinding factors
+// may differ.  The Fiat-Shamir draws run partition by partition, group by group, stage by stage, and within a stage in input order.
+// batch: a batched call, which runs on one GPU only; otherwise, on several GPUs (dg_prove on every rank), one trace is proven sharded.
+// proofs_out[i] / status[i] / messages[i] (why trace i failed, else empty) per trace; when the call throws, no proof is left in
+// proofs_out.  groups (may be null) receives the number of groups the traces ran in.
+// prove_traces and check_traces take calls that passed check_prove_call (capi.cu) or check_execution_call: they do not check the
+// lengths, shapes, registers, public input / output counts or options again.
 void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const std::vector<dg_options_t> &opts, bool batch,
                   Proof **proofs_out, int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
-// the same with one set of options for every trace
-void prove_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
-                  const uint8_t *const *outputs16, const uint32_t *n_outputs, const dg_options_t &opt, bool batch, Proof **proofs_out,
-                  int *status, std::vector<std::string> &messages, dg_prove_stats_t *stats, uint32_t *groups = nullptr);
-// `count` traces of one shape: registers [count][width][length] on the device at d_regs, or host columns (count * width pointers)
-std::vector<TraceRef> one_shape_traces(const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                                       uint32_t ctx_depth, uint32_t loop_depth);
+// `count` traces of one shape in one device allocation, [count][width][length] at d_regs
+std::vector<TraceRef> one_shape_traces(const fe *d_regs, uint32_t count, uint32_t width, uint64_t length, uint32_t ctx_depth, uint32_t loop_depth);
+// adds a group's stats to a call's
+void add_stats(dg_prove_stats_t *sum, const dg_prove_stats_t &s);
 // ProofOptions::new's checks (options.rs:29-50) and the hash (only blake3 is serialisable): DG_ERR_INVALID with the reason
 void check_options(const dg_options_t &o);
 // the traces of each (length, extension factor), partitions in order of first appearance, traces in input order
@@ -57,9 +49,6 @@ std::vector<std::vector<uint32_t>> partition_traces(const std::vector<uint64_t> 
 std::vector<uint32_t> cut_groups(const std::vector<uint32_t> &width, const std::vector<size_t> &footprint, size_t budget, uint32_t cap);
 // the device order of a group: positions of the traces grouped by shape, shapes in order of first appearance, input order inside a shape
 std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape);
-// The register columns of `count` host traces, trace after trace.  Every trace must have the shape of the first ("all traces of a
-// <call> must ..."), 16..127 registers and no null column; length_first also checks each length before its columns (dg_prove).
-std::vector<const uint8_t *> trace_columns(const dg_trace_t *traces, uint32_t count, const char *call, bool length_first);
 
 // The execution calls (execute.cu).  Execution i runs programs[program_of[i]] on inputs[i]; status / messages per execution.
 struct ExecutionCall {
@@ -120,11 +109,10 @@ void upload_trace_columns(Context &c, fe *d_regs, const uint8_t *const *host_col
 void extend_trace_columns(Context &c, const fe *polys, const fe *regs, fe *ext, int cols, int log_n, int log_b, uint64_t N_loc, unsigned c0,
                           unsigned nc);
 
-// the trace check (check.cu): per trace, which transition constraints fail at which steps and which boundary registers are wrong.
-// d_regs: [count][width][length] on the device, or null with host_cols (count * width column pointers) to upload; program_hashes32
-// (count * 32 bytes) and step_masks (host, count * length * 3 words) / d_step_masks (device, same size) may be null
-void check_traces(Context &c, const fe *d_regs, const uint8_t *const *host_cols, uint32_t count, uint32_t width, uint64_t length,
-                  uint32_t ctx_depth, uint32_t loop_depth, const uint8_t *const *inputs16, const uint32_t *n_inputs,
+// the trace check (check.cu): per trace, which transition constraints fail at which steps and which boundary registers are wrong.  The
+// traces have one shape, host or in one device allocation (one_shape_traces); program_hashes32 (count * 32 bytes) and step_masks (host,
+// count * length * 3 words) / d_step_masks (device, same size) may be null
+void check_traces(Context &c, const std::vector<TraceRef> &traces, const uint8_t *const *inputs16, const uint32_t *n_inputs,
                   const uint8_t *const *outputs16, const uint32_t *n_outputs, const uint8_t *program_hashes32, dg_trace_report_t *reports,
                   uint32_t *step_masks, uint32_t *d_step_masks);
 // name of transition constraint `index` (evaluation order) of a register shape, as the trace check reports it
