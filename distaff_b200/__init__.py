@@ -14,8 +14,10 @@ Python host-side mirror of the reference interface for the prove hot path:
     distaff_b200.execute_programs(jobs)           <->  execute_batch for jobs of many programs in one call (trace_programs: the traces)
     distaff_b200.execute_one(program, inputs)     <->  distaff::execute of one long execution, split across GPU threads (trace_one)
     distaff_b200.execute_many(jobs)               <->  execute_programs with every execution split as execute_one splits one (trace_many)
+    distaff_b200.execute_programs_device(...)     <->  execute_programs / trace_programs / execute_many / trace_many with DeviceInputs:
+                                                      program inputs already in device memory (*_device forms of the four calls)
     distaff_b200.HasherTree(leaves)               <->  a Merkle tree of utils::hasher::digest, built on the GPU, with its smpath / pmpath inputs
-    distaff_b200.prove_membership(tree, indexes)  <->  execute_batch of the smpath or pmpath program for leaves of a HasherTree
+    distaff_b200.prove_membership(tree, indexes)  <->  the smpath or pmpath program with proofs for leaves of a HasherTree or MerkleTree
     distaff_b200.MerkleTree(leaves, hash)         <->  crypto::MerkleTree kept in device memory: paths of many leaves per call, leaf updates
     tree.prove_batch(indexes)                     <->  MerkleTree::prove_batch: a BatchMerkleProof gathered on the GPU
     distaff_b200.merkle_verify_paths / _batch     <->  MerkleTree::verify / verify_batch of many paths or batch proofs in one call
@@ -26,4 +28,5 @@ from .api import (ProofOptions, StarkProof, prove, prove_device, prove_batch, pr
                   check_traces_device, constraint_name, set_memory_limit, memory_usage, plan_prove, ProgramInputs, trace_batch, trace_shapes,
                   execute_batch, trace_programs, execute_programs, group_traces, trace_one, execute_one,
                   trace_many, execute_many, HasherTree, smpath_program, pmpath_program, prove_membership, MerkleTree,
-                  BatchMerkleProof, merkle_verify_paths, merkle_verify_batch)
+                  BatchMerkleProof, merkle_verify_paths, merkle_verify_batch, DeviceInputs, trace_programs_device, execute_programs_device,
+                  trace_many_device, execute_many_device)

@@ -551,24 +551,28 @@ def _fields(st, into=None):
     return d
 
 
-def _traces(call, jobs, programs, program_of, num_outputs):
+def _traces(call, public_of, programs, program_of, num_outputs):
     """The trace calls: call(info, registers_out, status) once without registers to size the buffers, then with one buffer per execution
-    that call let through.  Returns a list in job order: a hostvm.ExecutionTrace with num_outputs[i] outputs, or the DgError of an
-    execution that failed."""
-    k = len(jobs)
+    that call let through.  public_of(ids) gives the public inputs of the executions ids.  Returns a list in execution order: a
+    hostvm.ExecutionTrace with num_outputs[i] outputs, or the DgError of an execution that failed."""
+    k = len(program_of)
     info = (backend.DgExecutionInfo * k)()
     status = (ctypes.c_int * k)()
     backend.check(call(info, None, status))
     regs = [np.empty((info[i].width, info[i].length, 2), dtype=np.uint64) if status[i] == 0 else None for i in range(k)]
     backend.check(call(info, (backend.vp * k)(*[r.ctypes.data if r is not None else None for r in regs]), status))
     result = _messages(status)
-    for i, job in enumerate(jobs):
-        if result[i] is None:
-            sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
-            last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
-            result[i] = hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
-                                              list(job[1].public), last[:num_outputs[i]])
+    ok = [i for i in range(k) if result[i] is None]
+    for i, public in zip(ok, public_of(ok)):
+        sd, start, n = info[i].stack_depth, 15 + info[i].ctx_depth + info[i].loop_depth, info[i].length
+        last = [felt.to_ints(regs[i][start + j, n - 1])[0] if j < sd else 0 for j in range(8)]
+        result[i] = hostvm.ExecutionTrace(regs[i], info[i].ctx_depth, info[i].loop_depth, sd, programs[program_of[i]].hash,
+                                          list(public), last[:num_outputs[i]])
     return result
+
+
+def _job_publics(jobs):
+    return lambda ids: [jobs[i][1].public for i in ids]
 
 
 def _proofs(call, num_outputs, per=8):
@@ -609,7 +613,7 @@ def trace_batch(program, inputs, max_steps=MAX_STEPS, num_outputs=1):
     prog, cprog, arr, keep = _execution_args(program, [x for _, x in jobs])
     k = len(jobs)
     return _traces(lambda info, outs, status: backend.lib().dg_trace_batch(ctypes.byref(cprog), k, arr, int(max_steps), info, outs, status),
-                   jobs, [prog], [0] * k, [num_outputs] * k)
+                   _job_publics(jobs), [prog], [0] * k, [num_outputs] * k)
 
 
 def execute_batch(program, inputs, num_outputs=1, options=None, max_steps=MAX_STEPS):
@@ -645,7 +649,7 @@ def trace_one(program, inputs=None, max_steps=MAX_STEPS, num_outputs=1, segment_
                                         ctypes.byref(st))
         _fields(st, stats)
         return rc
-    return _traces(call, jobs, [prog], [0], [num_outputs])[0]
+    return _traces(call, _job_publics(jobs), [prog], [0], [num_outputs])[0]
 
 
 def execute_one(program, inputs=None, num_outputs=1, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
@@ -700,7 +704,7 @@ def _trace_jobs(entry, jobs, st, stats, *args):
     programs, cprogs, program_of, arr, num_outputs, keep = _programs_args(jobs)
     fn = getattr(backend.lib(), entry)
     result = _traces(lambda info, outs, status: fn(cprogs, len(programs), len(jobs), program_of, arr, *args, info, outs, status, ctypes.byref(st)),
-                     jobs, programs, program_of, num_outputs)
+                     _job_publics(jobs), programs, program_of, num_outputs)
     _fields(st, stats)
     return result
 
@@ -762,6 +766,173 @@ def execute_many(jobs, options=None, max_steps=MAX_STEPS, segment_steps=0, stats
     Returns a list in job order: (outputs, StarkProof) -- what execute_programs returns, byte for byte -- or the DgError of an execution
     that failed.  segment_steps and `stats` as in trace_many; options as in execute_programs."""
     return _execute_jobs("dg_execute_many", jobs, options, backend.DgManyStats(), stats, int(max_steps), _segment_steps(segment_steps))
+
+
+# ---- program inputs already in device memory ------------------------------------------------------------------------------------
+class DeviceInputs:
+    """The inputs of many executions whose values are all in one device buffer (dg_device_inputs_t): execution i reads its public inputs
+    from the range public[i] = (first, count) of the values, tape A from tape_a[i] and tape B from tape_b[i], each range in reading order
+    (its first value is read first).  values: a contiguous CUDA uint64 tensor of shape (n, 2) on the library's device (value k is
+    values[k, 0] + 2^64 values[k, 1]), or a (device pointer, n) pair -- a backend.DeviceBuffer or a dg_dev_alloc address holding n values.
+    Ranges may overlap or be shared; each of public, tape_a and tape_b is a sequence of (first, count) pairs, one per execution, or an
+    (executions, 2) integer array.  A range past the n values fails the call that reads it, before the device is touched.  The object
+    keeps the buffer alive."""
+
+    def __init__(self, values, public, tape_a, tape_b):
+        if getattr(values, "is_cuda", False):
+            import torch
+            if values.dtype != torch.uint64 or values.dim() != 2 or values.shape[1] != 2 or not values.is_contiguous():
+                raise ValueError("device values are a contiguous uint64 tensor of shape (n, 2)")
+            self.values, self.ptr, self.n_values = values, values.data_ptr(), int(values.shape[0])
+        elif isinstance(values, tuple) and len(values) == 2:
+            n = values[1]
+            if not isinstance(n, (int, np.integer)) or not 0 <= int(n) < 2**64:
+                raise ValueError("the number of device values is an integer in [0, 2^64)")
+            self.values, self.ptr, self.n_values = values[0], _dev_ptr(values[0]) if values[0] is not None else 0, int(n)
+        else:
+            raise TypeError("values: a CUDA uint64 tensor of shape (n, 2), or a (device pointer, n) pair")
+        ranges = [self._ranges(r, what) for r, what in ((public, "public"), (tape_a, "tape_a"), (tape_b, "tape_b"))]
+        if len({len(r) for r in ranges}) != 1:
+            raise ValueError("public, tape_a and tape_b hold one range per execution: %d, %d and %d" % tuple(len(r) for r in ranges))
+        if (ranges[0][:, 1] >= 2**32).any():
+            raise ValueError("a public-input count is below 2^32")
+        self.count = len(ranges[0])
+        self.ranges = ranges
+        self._arrays = [np.ascontiguousarray(a[:, c], dtype=t) for a in ranges for c, t in ((0, np.uint64), (1, np.uint64))]
+        self._arrays[1] = self._arrays[1].astype(np.uint32)
+        p = [a.ctypes.data_as(ctypes.POINTER(backend.u32 if a.dtype == np.uint32 else backend.u64)) for a in self._arrays]
+        self._c = backend.DgDeviceInputs(self.ptr or None, self.n_values, *p)
+
+    @staticmethod
+    def _ranges(pairs, what):
+        if isinstance(pairs, np.ndarray) and pairs.dtype.kind in "iu":
+            a = pairs.reshape(-1, 2) if pairs.size == 0 else pairs
+            if a.ndim != 2 or a.shape[1] != 2 or (a < 0).any():
+                raise ValueError(f"{what}: an (executions, 2) array of non-negative (first, count) pairs")
+            return a.astype(np.uint64)
+        out = []
+        for p in pairs:
+            p = tuple(p)
+            if len(p) != 2 or not all(isinstance(v, (int, np.integer)) and 0 <= int(v) < 2**64 for v in p):
+                raise ValueError(f"{what}: each range is a (first, count) pair of integers in [0, 2^64), not {p!r}")
+            out.append((int(p[0]), int(p[1])))
+        return np.array(out, dtype=np.uint64).reshape(-1, 2)
+
+    def public_inputs(self, ids):
+        """the public inputs of the executions ids (lists of ints), read from the device"""
+        ranges = [(int(self.ranges[0][i, 0]), int(self.ranges[0][i, 1])) for i in ids]
+        if getattr(self.values, "is_cuda", False):
+            import torch
+            pos = [f + j for f, n in ranges for j in range(n)]
+            at = torch.tensor(pos, dtype=torch.int64, device=self.values.device)
+            flat = felt.to_ints(self.values.view(torch.int64)[at].cpu().numpy().view(np.uint64)) if pos else []
+        else:
+            flat = []
+            for f, n in ranges:
+                if n:
+                    v = np.empty((n, 2), dtype=np.uint64)
+                    backend.check(backend.lib().dg_dev_download(v.ctypes.data, self.ptr + 16 * f, 16 * n))
+                    flat += felt.to_ints(v)
+        out, at = [], 0
+        for _, n in ranges:
+            out.append(flat[at:at + n])
+            at += n
+        return out
+
+    def _sync(self):
+        """orders the library's stream after work the caller queued on torch's stream to write the values"""
+        if getattr(self.values, "is_cuda", False):
+            import torch
+            torch.cuda.synchronize(self.values.device)
+
+
+def _device_args(programs, program_of, inputs, num_outputs):
+    """the programs (each distinct source compiled once), their dg_program_t table, program_of and num_outputs of a device-inputs call"""
+    if not isinstance(inputs, DeviceInputs):
+        raise TypeError("inputs: a DeviceInputs")
+    cache, progs = {}, []
+    for p in programs:
+        if isinstance(p, str):
+            if p not in cache:
+                cache[p] = hostvm.compile_program(p)
+            p = cache[p]
+        progs.append(p)
+    program_of = [int(j) for j in program_of]
+    k = inputs.count
+    if len(program_of) != k:
+        raise ValueError(f"program_of: one program per execution, {len(program_of)} for {k} executions")
+    num_outputs = [int(num_outputs)] * k if isinstance(num_outputs, (int, np.integer)) else [int(n) for n in num_outputs]
+    if len(num_outputs) != k:
+        raise ValueError(f"num_outputs: one count per execution, {len(num_outputs)} for {k} executions")
+    if any(not 0 <= n <= 8 for n in num_outputs):
+        raise ValueError("cannot have more than 8 outputs")
+    if any(not 0 <= j < 2**32 for j in program_of):
+        raise ValueError("program_of: indexes into programs")
+    cprogs = (backend.DgProgram * max(len(progs), 1))(*[p.c_struct() for p in progs])
+    return progs, cprogs, (backend.u32 * max(k, 1))(*program_of), num_outputs
+
+
+def _device_options(options, k):
+    """one dg_options_t per execution: one ProofOptions (None: the defaults) replicated, or a list of k"""
+    opt, per = _options_arg(options, k, "execution")
+    return opt if per else (backend.DgOptions * max(k, 1))(*[(options or ProofOptions())._c()] * k)
+
+
+def _trace_device(entry, programs, program_of, inputs, num_outputs, st, stats, *args):
+    progs, cprogs, of, num_outputs = _device_args(programs, program_of, inputs, num_outputs)
+    if inputs.count == 0:
+        return []
+    inputs._sync()
+    fn = getattr(backend.lib(), entry)
+    result = _traces(lambda info, outs, status: fn(cprogs, len(progs), inputs.count, of, ctypes.byref(inputs._c), *args, info, outs, status,
+                                                   ctypes.byref(st)), inputs.public_inputs, progs, program_of, num_outputs)
+    _fields(st, stats)
+    return result
+
+
+def _execute_device(entry, programs, program_of, inputs, num_outputs, options, st, stats, *args):
+    progs, cprogs, of, num_outputs = _device_args(programs, program_of, inputs, num_outputs)
+    k = inputs.count
+    opt = _device_options(options, k)
+    if k == 0:
+        return []
+    inputs._sync()
+    fn = getattr(backend.lib(), entry)
+    result = _proofs(lambda handles, outputs16, status, pst: fn(cprogs, len(progs), k, of, ctypes.byref(inputs._c), (backend.u32 * k)(*num_outputs),
+                                                                *args, opt, handles, outputs16, status, pst, ctypes.byref(st)), num_outputs)
+    _fields(st, stats)
+    return result
+
+
+def trace_programs_device(programs, program_of, inputs, num_outputs=1, max_steps=MAX_STEPS, stats=None):
+    """trace_programs with the inputs in device memory (dg_trace_programs_device_inputs): execution i runs programs[program_of[i]] (an
+    assembly source or a hostvm.Program; each distinct source is compiled once) on the inputs the DeviceInputs gives it.  num_outputs:
+    one count for every execution or one per execution.  Returns what trace_programs returns for the same inputs, in execution order,
+    each trace's public inputs read back from the device."""
+    return _trace_device("dg_trace_programs_device_inputs", programs, program_of, inputs, num_outputs, backend.DgExecutionStats(), stats,
+                         int(max_steps))
+
+
+def execute_programs_device(programs, program_of, inputs, num_outputs=1, options=None, max_steps=MAX_STEPS, stats=None):
+    """execute_programs with the inputs in device memory (dg_execute_programs_device_inputs); programs, program_of and num_outputs as in
+    trace_programs_device, options one ProofOptions for every execution or a list with one per execution.  Returns what execute_programs
+    returns for the same inputs, in execution order."""
+    return _execute_device("dg_execute_programs_device_inputs", programs, program_of, inputs, num_outputs, options, backend.DgExecutionStats(),
+                           stats, int(max_steps))
+
+
+def trace_many_device(programs, program_of, inputs, num_outputs=1, max_steps=MAX_STEPS, segment_steps=0, stats=None):
+    """trace_many with the inputs in device memory (dg_trace_many_device_inputs); arguments as in trace_programs_device, segment_steps and
+    stats as in trace_many."""
+    return _trace_device("dg_trace_many_device_inputs", programs, program_of, inputs, num_outputs, backend.DgManyStats(), stats, int(max_steps),
+                         _segment_steps(segment_steps))
+
+
+def execute_many_device(programs, program_of, inputs, num_outputs=1, options=None, max_steps=MAX_STEPS, segment_steps=0, stats=None):
+    """execute_many with the inputs in device memory (dg_execute_many_device_inputs); arguments as in execute_programs_device,
+    segment_steps and stats as in execute_many."""
+    return _execute_device("dg_execute_many_device_inputs", programs, program_of, inputs, num_outputs, options, backend.DgManyStats(), stats,
+                           int(max_steps), _segment_steps(segment_steps))
 
 
 # ---- building blocks ------------------------------------------------------------------------------------------------------
@@ -918,29 +1089,37 @@ class HasherTree:
 
 
 def prove_membership(tree, indexes, program="smpath", options=None):
-    """Proves that leaves of a HasherTree, or of a MerkleTree of hash "hasher" (its paths from one dg_tree_paths call, laid out as
-    HasherTree.smpath_inputs / pmpath_inputs lay them out), belong to it: one execute_batch call runs smpath_program(tree.depth) (index private) or
-    pmpath_program(tree.depth) (index public) for every index.  Returns a list in index order: (program_hash, public_inputs, outputs,
-    proof), an item of verify_batch whose outputs are the root in stack order, or a DgError for an entry whose execution failed or did not
-    output the root."""
+    """Proves that leaves of a HasherTree, or of a MerkleTree of hash "hasher", belong to it: smpath_program(tree.depth) (index private)
+    or pmpath_program(tree.depth) (index public) runs for every index in one call with proofs.  A HasherTree's inputs are built on the host
+    (HasherTree.smpath_inputs / pmpath_inputs, one execute_batch call); a MerkleTree's are gathered on the GPU from its heap
+    (MerkleTree.membership_inputs, one execute_programs_device call), so no path reaches the host.  Returns a list in index order:
+    (program_hash, public_inputs, outputs, proof), an item of verify_batch whose outputs are the root in stack order, or a DgError for an
+    entry whose execution failed or did not output the root."""
     if program not in ("smpath", "pmpath"):
         raise ValueError(f"program is smpath or pmpath, not {program!r}")
+    prog = hostvm.compile_program(smpath_program(tree.depth) if program == "smpath" else pmpath_program(tree.depth))
     if isinstance(tree, MerkleTree):
-        indexes, inputs, root = tree._membership_inputs(indexes, program)
+        idx = tree._indexes(indexes)
+        inputs = tree.membership_inputs(idx, program)
+        indexes = [int(i) for i in idx]
+        publics = [[i] if program == "pmpath" else [] for i in indexes]
+        root = list(_int_pairs(tree.root)[0])
+        results = execute_programs_device([prog], [0] * len(indexes), inputs, num_outputs=2, options=options)
     else:
         indexes = [tree._index(i) for i in indexes]
         inputs = [tree.smpath_inputs(i) if program == "smpath" else tree.pmpath_inputs(i) for i in indexes]
+        publics = [x.public for x in inputs]
         root = tree.root
-    prog = hostvm.compile_program(smpath_program(tree.depth) if program == "smpath" else pmpath_program(tree.depth))
+        results = execute_batch(prog, inputs, num_outputs=2, options=options)
     want = root[::-1]
     out = []
-    for i, x, r in zip(indexes, inputs, execute_batch(prog, inputs, num_outputs=2, options=options)):
+    for i, public, r in zip(indexes, publics, results):
         if isinstance(r, backend.DgError):
             out.append(r)
         elif r[0] != want:
             out.append(backend.DgError(-7, f"leaf {i}: the {program} program output {r[0]}, not the root"))
         else:
-            out.append((prog.hash, x.public, r[0], r[1]))
+            out.append((prog.hash, public, r[0], r[1]))
     return out
 
 
@@ -1079,24 +1258,29 @@ class MerkleTree:
             raise IndexError(f"leaf {i} of a tree of {self._n} leaves")
         return i
 
-    def _membership_inputs(self, indexes, program):
-        """prove_membership's indexes, ProgramInputs and root (field elements) from one paths() call"""
+    def membership_inputs(self, indexes, program="smpath"):
+        """The DeviceInputs of smpath_program(depth) ("smpath") or pmpath_program(depth) ("pmpath") for the leaves at indexes, written
+        from the heap into a new device buffer by one dg_tree_membership_inputs call, in the layout of HasherTree.smpath_inputs /
+        pmpath_inputs: per index one run of values, no path copied to the host.  Only a tree of hash "hasher" has them (ValueError
+        otherwise); an index >= len(tree) raises DgError naming it, as paths() does."""
+        if program not in ("smpath", "pmpath"):
+            raise ValueError(f"program is smpath or pmpath, not {program!r}")
         if self.hash != "hasher":
             raise ValueError(f"membership proofs verify paths of the VM's hash: a MerkleTree of hash 'hasher', not {self.hash!r}")
-        indexes = [self._index(i) for i in indexes]
-        inputs = []
-        for i, entries in zip(indexes, self.paths(indexes)):
-            path = _int_pairs(b"".join(entries))
-            if program == "smpath":                  # HasherTree.smpath_inputs: the leaf, then per entry (0, index bit) and the entry
-                a, b, bits = [path[0][0]], [path[0][1]], i
-                for node in path[1:]:
-                    a += [0, node[0]]
-                    b += [bits & 1, node[1]]
-                    bits >>= 1
-                inputs.append(ProgramInputs([], a, b))
-            else:                                    # HasherTree.pmpath_inputs: the index public, the path on the tapes
-                inputs.append(ProgramInputs([i], [e[0] for e in path], [e[1] for e in path]))
-        return indexes, inputs, list(_int_pairs(self.root)[0])
+        idx, pid = self._indexes(indexes), 0 if program == "smpath" else 1
+        k, ptr = len(idx), idx.ctypes.data if len(idx) else None
+        out = backend.DgDeviceInputs()
+        backend.check(backend.lib().dg_tree_membership_inputs(self._handle(), pid, ptr, k, None, 0, ctypes.byref(out)))
+        n = out.n_values
+        buf = backend.DeviceBuffer(max(n, 1) * 16)
+        first = [np.zeros(k, dtype=np.uint64) for _ in range(3)]
+        count = [np.zeros(k, dtype=np.uint32), np.zeros(k, dtype=np.uint64), np.zeros(k, dtype=np.uint64)]
+        p64, p32 = ctypes.POINTER(backend.u64), ctypes.POINTER(backend.u32)
+        out.public_first, out.n_public = first[0].ctypes.data_as(p64), count[0].ctypes.data_as(p32)
+        out.secret_a_first, out.n_secret_a = first[1].ctypes.data_as(p64), count[1].ctypes.data_as(p64)
+        out.secret_b_first, out.n_secret_b = first[2].ctypes.data_as(p64), count[2].ctypes.data_as(p64)
+        backend.check(backend.lib().dg_tree_membership_inputs(self._handle(), pid, ptr, k, buf.ptr, n, ctypes.byref(out)))
+        return DeviceInputs((buf, n), *[np.stack([f, c.astype(np.uint64)], axis=1) for f, c in zip(first, count)])
 
     def close(self):
         if self._h:

@@ -69,6 +69,12 @@ class DgProgramInputs(ctypes.Structure):
     _fields_ = [("public16", vp), ("n_public", u32), ("secret_a16", vp), ("n_secret_a", u64), ("secret_b16", vp), ("n_secret_b", u64)]
 
 
+class DgDeviceInputs(ctypes.Structure):
+    _fields_ = [("d_values", vp), ("n_values", u64), ("public_first", ctypes.POINTER(u64)), ("n_public", ctypes.POINTER(u32)),
+                ("secret_a_first", ctypes.POINTER(u64)), ("n_secret_a", ctypes.POINTER(u64)), ("secret_b_first", ctypes.POINTER(u64)),
+                ("n_secret_b", ctypes.POINTER(u64))]
+
+
 class DgExecutionInfo(ctypes.Structure):
     _fields_ = [("width", u32), ("length", u64), ("steps", u64), ("ctx_depth", u32), ("loop_depth", u32), ("stack_depth", u32)]
 
@@ -145,6 +151,17 @@ EXPORTS = {
     "dg_execute_many_with_options": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgProgramInputs), ctypes.POINTER(u32),
                                      u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgStats),
                                      ctypes.POINTER(DgManyStats)],
+    "dg_trace_programs_device_inputs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgDeviceInputs), u64,
+                                        ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int),
+                                        ctypes.POINTER(DgExecutionStats)],
+    "dg_execute_programs_device_inputs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgDeviceInputs),
+                                          ctypes.POINTER(u32), u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int),
+                                          ctypes.POINTER(DgStats), ctypes.POINTER(DgExecutionStats)],
+    "dg_trace_many_device_inputs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgDeviceInputs), u64, u64,
+                                    ctypes.POINTER(DgExecutionInfo), ctypes.POINTER(vp), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(DgManyStats)],
+    "dg_execute_many_device_inputs": [ctypes.POINTER(DgProgram), u32, u32, ctypes.POINTER(u32), ctypes.POINTER(DgDeviceInputs), ctypes.POINTER(u32),
+                                      u64, u64, ctypes.POINTER(DgOptions), ctypes.POINTER(vp), vp, ctypes.POINTER(ctypes.c_int),
+                                      ctypes.POINTER(DgStats), ctypes.POINTER(DgManyStats)],
     "dg_check_traces": [ctypes.POINTER(DgTrace), u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32), vp,
                         ctypes.POINTER(DgTraceReport), vp],
     "dg_check_traces_device": [vp, u32, u32, u64, u32, u32, ctypes.POINTER(vp), ctypes.POINTER(u32), ctypes.POINTER(vp), ctypes.POINTER(u32),
@@ -167,6 +184,7 @@ EXPORTS = {
     "dg_tree_info": [vp, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(u64), vp],
     "dg_tree_paths": [vp, vp, u32, vp],
     "dg_tree_update": [vp, vp, vp, u32, vp],
+    "dg_tree_membership_inputs": [vp, ctypes.c_int, vp, u32, vp, u64, ctypes.POINTER(DgDeviceInputs)],
     "dg_tree_read": [vp, vp, vp],
     "dg_tree_prove_batch": [vp, vp, u32, vp, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
     "dg_merkle_verify_paths": [ctypes.c_int, vp, u32, vp, vp, u32, u32, ctypes.POINTER(ctypes.c_int)],

@@ -384,6 +384,40 @@ int dg_tree_paths(const dg_tree_t *tree, const uint64_t *indexes, uint32_t count
         tree_paths(c, t, indexes, count, paths32);
     });
 }
+int dg_tree_membership_inputs(const dg_tree_t *tree, int program, const uint64_t *indexes, uint32_t count, void *d_values, uint64_t cap,
+                              dg_device_inputs_t *out) {
+    return guarded([&] {
+        DG_REQUIRE(tree && out, "null argument");
+        DG_REQUIRE(program == DG_PATH_SMPATH || program == DG_PATH_PMPATH, "program must be DG_PATH_SMPATH (0) or DG_PATH_PMPATH (1)");
+        DG_REQUIRE(count == 0 || indexes, "null buffer");
+        const Tree &t = *(const Tree *)tree;
+        DG_REQUIRE(t.hash == DG_HASH_HASHER, "membership inputs are paths of the VM's hash: a tree of hash 3 (hasher), not " + std::to_string(t.hash));
+        require_tree_indexes(t, indexes, count);
+        const bool pm = program == DG_PATH_PMPATH;
+        const uint64_t d = (uint64_t)ceil_log2(t.L), per = pm ? 2 * d + 3 : 4 * d + 2;
+        out->n_values = per * count;
+        if (!d_values) return;
+        DG_REQUIRE(cap >= out->n_values, "d_values holds " + std::to_string(cap) + " values, the inputs need " + std::to_string(out->n_values));
+        DG_REQUIRE(((uintptr_t)d_values & 15) == 0, "d_values is not 16-byte aligned");
+        DG_REQUIRE(out->public_first && out->n_public && out->secret_a_first && out->n_secret_a && out->secret_b_first && out->n_secret_b,
+                   "null offset or count array in out");
+        uint64_t *pf = (uint64_t *)out->public_first, *af = (uint64_t *)out->secret_a_first, *bf = (uint64_t *)out->secret_b_first;
+        uint32_t *np = (uint32_t *)out->n_public;
+        uint64_t *na = (uint64_t *)out->n_secret_a, *nb = (uint64_t *)out->n_secret_b;
+        const uint64_t tape = pm ? d + 1 : 2 * d + 1, pub = pm ? 1 : 0;
+        for (uint32_t k = 0; k < count; k++) {
+            pf[k] = k * per; np[k] = (uint32_t)pub;
+            af[k] = k * per + pub; na[k] = tape;
+            bf[k] = k * per + pub + tape; nb[k] = tape;
+        }
+        out->d_values = d_values;
+        if (count == 0) return;
+        Context &c = ctx();
+        std::lock_guard<std::mutex> lk(c.mu);
+        require_device_memory(c, d_values, "d_values");
+        tree_membership_inputs(c, t, pm, indexes, count, (fe *)d_values);
+    });
+}
 int dg_tree_update(dg_tree_t *tree, const uint64_t *indexes, const uint8_t *leaves32, uint32_t count, uint8_t root32[32]) {
     return guarded([&] {
         DG_REQUIRE(tree, "null tree");
@@ -893,29 +927,29 @@ int dg_check_traces_device(const void *d_registers, uint32_t count, uint32_t wid
         check_traces(c, x.traces, inputs16, n_inputs, outputs16, n_outputs, program_hashes32, reports, nullptr, d_step_masks);
     });
 }
+static void run_trace_programs(const ExecutionCall &x, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                               dg_execution_stats_t *vm_stats) {
+    DG_REQUIRE(x.count >= 1, "at least one execution is needed");
+    DG_REQUIRE(x.programs && x.program_of && (x.inputs || x.device_inputs) && status, "null argument");
+    check_execution_call(x);
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    trace_programs(c, x, info, registers_out, status, t_batch_messages, vm_stats);
+}
 int dg_trace_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
                       const dg_program_inputs_t *inputs, uint64_t max_steps, dg_execution_info_t *info, uint8_t *const *registers_out,
                       int *status, dg_execution_stats_t *vm_stats) {
     return guarded([&] {
-        DG_REQUIRE(count >= 1, "at least one execution is needed");
-        DG_REQUIRE(programs && program_of && inputs && status, "null argument");
-        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x);
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        trace_programs(c, x, info, registers_out, status, t_batch_messages, vm_stats);
+        run_trace_programs(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, info, registers_out, status, vm_stats);
     });
 }
-static void run_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
-                                 const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
-                                 bool per_execution, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
-                                 dg_execution_stats_t *vm_stats) {
-    DG_REQUIRE(count >= 1, "at least one execution is needed");
-    DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
-    const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+static void run_execute_programs(const ExecutionCall &x, const uint32_t *num_outputs, const dg_options_t *options, bool per_execution,
+                                 dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
+    DG_REQUIRE(x.count >= 1, "at least one execution is needed");
+    DG_REQUIRE(x.programs && x.program_of && (x.inputs || x.device_inputs) && options && proofs_out && status, "null argument");
     check_execution_call(x, OutputCounts{num_outputs, outputs16});
-    const std::vector<dg_options_t> opts = call_options(options, count, per_execution, "execution");
+    const std::vector<dg_options_t> opts = call_options(options, x.count, per_execution, "execution");
     Context &c = ctx();
     std::lock_guard<std::mutex> lk(c.mu);
     t_batch_messages.clear();
@@ -925,8 +959,8 @@ int dg_execute_programs(const dg_program_t *programs, uint32_t n_programs, uint3
                         const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
                         dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats, dg_execution_stats_t *vm_stats) {
     return guarded([&] {
-        run_execute_programs(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, options, false, proofs_out, outputs16, status,
-                             stats, vm_stats);
+        run_execute_programs(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, num_outputs, options, false, proofs_out,
+                             outputs16, status, stats, vm_stats);
     });
 }
 int dg_execute_programs_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
@@ -934,8 +968,8 @@ int dg_execute_programs_with_options(const dg_program_t *programs, uint32_t n_pr
                                      dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
                                      dg_execution_stats_t *vm_stats) {
     return guarded([&] {
-        run_execute_programs(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, options, true, proofs_out, outputs16, status,
-                             stats, vm_stats);
+        run_execute_programs(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, num_outputs, options, true, proofs_out,
+                             outputs16, status, stats, vm_stats);
     });
 }
 // the one-program case: program_of all 0
@@ -1043,29 +1077,30 @@ int dg_execute_one(const dg_program_t *program, const dg_program_inputs_t *input
         if (info) *info = one;
     });
 }
+static void run_trace_many(const ExecutionCall &x, uint64_t segment_steps, dg_execution_info_t *info, uint8_t *const *registers_out, int *status,
+                           dg_many_stats_t *stats) {
+    DG_REQUIRE(x.count >= 1, "at least one execution is needed");
+    DG_REQUIRE(x.programs && x.program_of && (x.inputs || x.device_inputs) && status, "null argument");
+    check_execution_call(x, std::nullopt, segment_steps);
+    Context &c = ctx();
+    std::lock_guard<std::mutex> lk(c.mu);
+    t_batch_messages.clear();
+    trace_many(c, x, segment_steps, info, registers_out, status, t_batch_messages, stats);
+}
 int dg_trace_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
                   const dg_program_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps, dg_execution_info_t *info,
                   uint8_t *const *registers_out, int *status, dg_many_stats_t *stats) {
     return guarded([&] {
-        DG_REQUIRE(count >= 1, "at least one execution is needed");
-        DG_REQUIRE(programs && program_of && inputs && status, "null argument");
-        const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
-        check_execution_call(x, std::nullopt, segment_steps);
-        Context &c = ctx();
-        std::lock_guard<std::mutex> lk(c.mu);
-        t_batch_messages.clear();
-        trace_many(c, x, segment_steps, info, registers_out, status, t_batch_messages, stats);
+        run_trace_many(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, segment_steps, info, registers_out, status, stats);
     });
 }
-static void run_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
-                             const dg_program_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
-                             const dg_options_t *options, bool per_execution, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
-                             dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
-    DG_REQUIRE(count >= 1, "at least one execution is needed");
-    DG_REQUIRE(programs && program_of && inputs && options && proofs_out && status, "null argument");
-    const ExecutionCall x{programs, n_programs, count, program_of, inputs, max_steps};
+static void run_execute_many(const ExecutionCall &x, const uint32_t *num_outputs, uint64_t segment_steps, const dg_options_t *options,
+                             bool per_execution, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
+                             dg_many_stats_t *stats) {
+    DG_REQUIRE(x.count >= 1, "at least one execution is needed");
+    DG_REQUIRE(x.programs && x.program_of && (x.inputs || x.device_inputs) && options && proofs_out && status, "null argument");
     check_execution_call(x, OutputCounts{num_outputs, outputs16}, segment_steps);
-    const std::vector<dg_options_t> opts = call_options(options, count, per_execution, "execution");
+    const std::vector<dg_options_t> opts = call_options(options, x.count, per_execution, "execution");
     Context &c = ctx();
     std::lock_guard<std::mutex> lk(c.mu);
     t_batch_messages.clear();
@@ -1077,8 +1112,8 @@ int dg_execute_many(const dg_program_t *programs, uint32_t n_programs, uint32_t 
                     const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *prove_stats,
                     dg_many_stats_t *stats) {
     return guarded([&] {
-        run_execute_many(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, segment_steps, options, false, proofs_out,
-                         outputs16, status, prove_stats, stats);
+        run_execute_many(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, num_outputs, segment_steps, options, false,
+                         proofs_out, outputs16, status, prove_stats, stats);
     });
 }
 int dg_execute_many_with_options(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
@@ -1086,8 +1121,47 @@ int dg_execute_many_with_options(const dg_program_t *programs, uint32_t n_progra
                                  const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
                                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
     return guarded([&] {
-        run_execute_many(programs, n_programs, count, program_of, inputs, num_outputs, max_steps, segment_steps, options, true, proofs_out,
-                         outputs16, status, prove_stats, stats);
+        run_execute_many(ExecutionCall{programs, n_programs, count, program_of, inputs, max_steps}, num_outputs, segment_steps, options, true,
+                         proofs_out, outputs16, status, prove_stats, stats);
+    });
+}
+
+// ---- program inputs in device memory: the calls above with ExecutionCall::device_inputs ----------------------------------------------
+static ExecutionCall device_call(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                 const dg_device_inputs_t *inputs, uint64_t max_steps) {
+    DG_REQUIRE(inputs, "null device inputs");
+    return ExecutionCall{programs, n_programs, count, program_of, nullptr, max_steps, inputs};
+}
+int dg_trace_programs_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                    const dg_device_inputs_t *inputs, uint64_t max_steps, dg_execution_info_t *info, uint8_t *const *registers_out,
+                                    int *status, dg_execution_stats_t *vm_stats) {
+    return guarded([&] {
+        run_trace_programs(device_call(programs, n_programs, count, program_of, inputs, max_steps), info, registers_out, status, vm_stats);
+    });
+}
+int dg_execute_programs_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                      const dg_device_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                                      dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
+                                      dg_execution_stats_t *vm_stats) {
+    return guarded([&] {
+        run_execute_programs(device_call(programs, n_programs, count, program_of, inputs, max_steps), num_outputs, options, true, proofs_out,
+                             outputs16, status, stats, vm_stats);
+    });
+}
+int dg_trace_many_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                const dg_device_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps, dg_execution_info_t *info,
+                                uint8_t *const *registers_out, int *status, dg_many_stats_t *stats) {
+    return guarded([&] {
+        run_trace_many(device_call(programs, n_programs, count, program_of, inputs, max_steps), segment_steps, info, registers_out, status, stats);
+    });
+}
+int dg_execute_many_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                  const dg_device_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                                  const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
+                                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats) {
+    return guarded([&] {
+        run_execute_many(device_call(programs, n_programs, count, program_of, inputs, max_steps), num_outputs, segment_steps, options, true,
+                         proofs_out, outputs16, status, prove_stats, stats);
     });
 }
 int dg_batch_message(uint32_t index, char *message, size_t cap) {

@@ -166,6 +166,8 @@ void ctx_init(int device);
 void ctx_init_devices(int n);               // contexts for devices 0 .. n-1 + one NCCL communicator per device (single-process multi-GPU)
 int ctx_device_count();                     // number of contexts (1 unless ctx_init_devices was called)
 Context &ctx_of(int index);
+// throws DG_ERR_INVALID ("<what> is not device memory of the library's device") unless p is device or managed memory of c's device
+void require_device_memory(const Context &c, const void *p, const std::string &what);
 void ctx_bind(Context *c);                  // makes c the calling thread's current context (and its device current)
 // raises the dynamic shared-memory limit of a kernel on c's device once
 void set_func_smem(Context &c, const void *func, size_t bytes);

@@ -303,4 +303,11 @@ TwiddleRef Context::twiddle(int log_order, bool inverse) {
     return r;
 }
 
+void require_device_memory(const Context &c, const void *p, const std::string &what) {
+    cudaPointerAttributes a;
+    DG_CUDA(cudaPointerGetAttributes(&a, p));
+    DG_REQUIRE((a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) && a.device == c.device,
+               what + " is not device memory of the library's device");
+}
+
 }  // namespace dg

@@ -17,6 +17,36 @@
 #include <tuple>
 
 namespace dg {
+
+// One execution's inputs for pack_inputs_kernel: its values go to data[dst ..), the public inputs (n[0]) from src[src[0] ..) in order, tape
+// A (n[1]) and tape B (n[2]) from src[src[1] ..) and src[src[2] ..) reversed.  The items of a launch have values and follow each other in
+// data, so dst grows with the item.
+struct PackItem { unsigned long long dst, src[3], n[3]; };
+
+// Thread t writes data[t]: it finds its item (the last whose dst <= t) and the region r and reading position j of the value there, copies
+// it, and for the public inputs also to pubs[8 q + j].  A value at or above M lowers bad[3 q + r] to j, so that each region keeps the first
+// bad position.
+__global__ void __launch_bounds__(256) pack_inputs_kernel(const PackItem *__restrict__ items, unsigned n_items, unsigned long long total,
+                                                          const fe *__restrict__ src, fe *__restrict__ data, fe *__restrict__ pubs,
+                                                          unsigned long long *__restrict__ bad) {
+    const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    unsigned q = 0, hi = n_items;
+    while (hi - q > 1) {
+        const unsigned mid = (q + hi) / 2;
+        if (items[mid].dst <= t) q = mid; else hi = mid;
+    }
+    const PackItem &it = items[q];
+    unsigned long long k = t - it.dst;
+    int r = 0;
+    while (r < 2 && k >= it.n[r]) k -= it.n[r++];
+    const unsigned long long j = r == 0 ? k : it.n[r] - 1 - k;
+    const fe v = src[it.src[r] + j];
+    if (v.hi == DG_M_HI && v.lo >= DG_M_LO) atomicMin(bad + 3ULL * q + r, j);
+    data[t] = v;
+    if (r == 0) pubs[8ULL * q + j] = v;
+}
+
 namespace {
 
 // ---- validation of the encoding (Span::new, validate_block_list, the ctx / loop limits) ---------------------------------------------
@@ -110,6 +140,8 @@ struct Executions {
     const ExecutionCall &x;
     DevBuf d_ops, d_hints, d_blocks, d_children, d_programs, d_in, d_data, d_res, d_tapes, d_off, d_cap, d_ids, d_outs, d_pad_ids;
     VmLaunch L;
+    std::vector<VmInput> in;                      // what setup() packed; zero but the program for an execution the inputs failed
+    std::vector<fe> pub;                          // 8 per execution: its public inputs (in[i].n_pub of them), for the prover
     std::vector<VmResult> res;
     std::vector<int> status;
     std::vector<std::string> messages;
@@ -118,7 +150,8 @@ struct Executions {
     cudaEvent_t ev[2] = {nullptr, nullptr};
 
     Executions(Context &ctx_, const ExecutionCall &call)
-        : c(ctx_), x(call), res(call.count), status(call.count, DG_OK), messages(call.count), off(call.count, 0), cap(2 * (size_t)call.count, 0) {
+        : c(ctx_), x(call), in(call.count), pub(8 * (size_t)call.count), res(call.count), status(call.count, DG_OK), messages(call.count),
+          off(call.count, 0), cap(2 * (size_t)call.count, 0) {
         memset(&stats, 0, sizeof stats);
         DG_CUDA(cudaEventCreate(&ev[0]));
         DG_CUDA(cudaEventCreate(&ev[1]));
@@ -126,15 +159,6 @@ struct Executions {
     ~Executions() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
 
     void fail(uint32_t i, int code, const std::string &m) { status[i] = code; messages[i] = m; }
-    // "<what> <j> is not a field element" for the first of n values at or above M, else ""
-    static std::string first_non_element(const uint8_t *p, uint64_t n, const char *what) {
-        for (uint64_t j = 0; j < n; j++) {
-            fe e;
-            memcpy(&e, p + 16 * j, 16);
-            if (e.hi == DG_M_HI && e.lo >= DG_M_LO) return std::string(what) + " " + std::to_string(j) + " is not a field element";
-        }
-        return "";
-    }
 
     template <typename T> void upload(DevBuf &d, const std::vector<T> &v) {
         d.alloc(std::max<size_t>(v.size(), 1) * sizeof(T));
@@ -189,30 +213,7 @@ struct Executions {
             memcpy(&programs[p].hash[0], g.hash32, 16); memcpy(&programs[p].hash[1], g.hash32 + 16, 16);
         }
         upload(d_ops, ops); upload(d_hints, hints); upload(d_blocks, blocks); upload(d_children, children); upload(d_programs, programs);
-        // inputs, packed: public inputs, then both tapes reversed (the next value to read is the last one, as in the host VM)
-        std::vector<VmInput> in(x.count);
-        std::vector<fe> data;
-        for (uint32_t i = 0; i < x.count; i++) {
-            const dg_program_inputs_t &v = x.inputs[i];
-            memset(&in[i], 0, sizeof(VmInput));
-            in[i].program = x.program_of[i];
-            if (v.n_public > 8) { fail(i, DG_ERR_EXECUTION, "expected no more than 8 public inputs"); continue; }      // lib.rs:32
-            if (v.n_secret_a < v.n_secret_b) { fail(i, DG_ERR_EXECUTION, "tape A cannot be shorter than tape B"); continue; }   // inputs.rs:17
-            // the VM's arithmetic assumes canonical operands: a value in [M, 2^128) fails its execution (the reference does not check)
-            std::string bad = first_non_element(v.public16, v.n_public, "public input");
-            if (bad.empty()) bad = first_non_element(v.secret_a16, v.n_secret_a, "tape A value");
-            if (bad.empty()) bad = first_non_element(v.secret_b16, v.n_secret_b, "tape B value");
-            if (!bad.empty()) { fail(i, DG_ERR_EXECUTION, bad); continue; }
-            auto put = [&](const uint8_t *p, uint64_t n, bool reverse) {
-                const size_t at = data.size();
-                for (uint64_t j = 0; j < n; j++) { fe e; memcpy(&e, p + 16 * (reverse ? n - 1 - j : j), 16); data.push_back(e); }
-                return (unsigned long long)at;
-            };
-            in[i].n_pub = v.n_public; in[i].pub = put(v.public16, v.n_public, false);
-            in[i].n_a = v.n_secret_a; in[i].a = put(v.secret_a16, v.n_secret_a, true);
-            in[i].n_b = v.n_secret_b; in[i].b = put(v.secret_b16, v.n_secret_b, true);
-        }
-        upload(d_in, in); upload(d_data, data);
+        pack_inputs();
         d_res.alloc((size_t)x.count * sizeof(VmResult));
         DG_CUDA(cudaMemsetAsync(d_res.p, 0, (size_t)x.count * sizeof(VmResult), c.stream));
         L.ops = d_ops.as<uint8_t>(); L.hints = d_hints.as<VmHint>(); L.blocks = d_blocks.as<VmBlock>(); L.children = d_children.as<unsigned>();
@@ -221,6 +222,82 @@ struct Executions {
         L.res = d_res.as<VmResult>();
         L.max_steps = x.max_steps;
         for (uint32_t i = 0; i < x.count; i++) { cap[2 * i] = in[i].n_a; cap[2 * i + 1] = in[i].n_b; }
+    }
+
+    // The inputs, packed for the VM into d_data: per execution its public inputs, then both tapes reversed (the next value to read is the
+    // last one, as in the host VM), executions one after the other; d_in describes them.  The counts are checked here; the values by one
+    // pack_inputs_kernel launch over every value of the call, from one source buffer: the caller's device buffer (device inputs), or the
+    // host inputs gathered into one upload.  Only the first bad index of each region and the public inputs come back.
+    void pack_inputs() {
+        const dg_device_inputs_t *dv = x.device_inputs;
+        std::vector<PackItem> items;
+        std::vector<unsigned> item_of;            // the execution of each item
+        std::vector<fe> staged;                   // host inputs: the values of every item, in reading order
+        unsigned long long total = 0;
+        for (uint32_t i = 0; i < x.count; i++) {
+            memset(&in[i], 0, sizeof(VmInput));
+            in[i].program = x.program_of[i];
+            const uint64_t n[3] = {dv ? dv->n_public[i] : x.inputs[i].n_public, dv ? dv->n_secret_a[i] : x.inputs[i].n_secret_a,
+                                   dv ? dv->n_secret_b[i] : x.inputs[i].n_secret_b};
+            if (n[0] > 8) { fail(i, DG_ERR_EXECUTION, "expected no more than 8 public inputs"); continue; }      // lib.rs:32
+            if (n[1] < n[2]) { fail(i, DG_ERR_EXECUTION, "tape A cannot be shorter than tape B"); continue; }   // inputs.rs:17
+            in[i].n_pub = (unsigned)n[0]; in[i].pub = total;
+            in[i].n_a = n[1]; in[i].a = total + n[0];
+            in[i].n_b = n[2]; in[i].b = total + n[0] + n[1];
+            if (n[0] + n[1] + n[2] == 0) continue;
+            PackItem it{total, {0, 0, 0}, {n[0], n[1], n[2]}};
+            if (dv) {
+                it.src[0] = dv->public_first[i]; it.src[1] = dv->secret_a_first[i]; it.src[2] = dv->secret_b_first[i];
+            } else {
+                const uint8_t *p[3] = {x.inputs[i].public16, x.inputs[i].secret_a16, x.inputs[i].secret_b16};
+                for (int r = 0; r < 3; r++) {
+                    it.src[r] = staged.size();
+                    staged.resize(staged.size() + n[r]);
+                    if (n[r]) memcpy(&staged[it.src[r]], p[r], 16 * n[r]);
+                }
+            }
+            items.push_back(it);
+            item_of.push_back(i);
+            total += n[0] + n[1] + n[2];
+        }
+        d_data.alloc(std::max<unsigned long long>(total, 1) * sizeof(fe));
+        if (!items.empty()) {
+            const fe *src = (const fe *)(dv ? dv->d_values : nullptr);
+            DevBuf d_staged, d_items, d_checks(items.size() * (8 * sizeof(fe) + 3 * sizeof(unsigned long long)));
+            if (dv) {
+                require_device_memory(c, src, "device inputs: d_values");
+            } else {
+                upload(d_staged, staged);
+                src = d_staged.as<fe>();
+            }
+            upload(d_items, items);
+            fe *pubs = d_checks.as<fe>();         // 8 per item, then 3 first bad indexes per item (all ones: none)
+            unsigned long long *bad = (unsigned long long *)(pubs + 8 * items.size());
+            DG_CUDA(cudaMemsetAsync(bad, 0xff, items.size() * 3 * sizeof(unsigned long long), c.stream));
+            pack_inputs_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.stream>>>(d_items.as<PackItem>(), (unsigned)items.size(), total, src,
+                                                                                         d_data.as<fe>(), pubs, bad);
+            c.launches++;
+            DG_CUDA(cudaGetLastError());
+            std::vector<uint8_t> checks(d_checks.bytes);
+            DG_CUDA(cudaMemcpyAsync(checks.data(), d_checks.p, checks.size(), cudaMemcpyDeviceToHost, c.stream));
+            DG_CUDA(cudaStreamSynchronize(c.stream));
+            const fe *got_pub = (const fe *)checks.data();
+            const unsigned long long *got_bad = (const unsigned long long *)(got_pub + 8 * items.size());
+            // the VM's arithmetic assumes canonical operands: a value in [M, 2^128) fails its execution (the reference does not check)
+            static const char *what[3] = {"public input", "tape A value", "tape B value"};
+            for (size_t q = 0; q < items.size(); q++) {
+                const unsigned i = item_of[q];
+                for (int r = 0; r < 3; r++)
+                    if (got_bad[3 * q + r] != ~0ULL) {
+                        fail(i, DG_ERR_EXECUTION, std::string(what[r]) + " " + std::to_string(got_bad[3 * q + r]) + " is not a field element");
+                        memset(&in[i], 0, sizeof(VmInput));
+                        in[i].program = x.program_of[i];
+                        break;
+                    }
+                if (status[i] == DG_OK) std::copy(got_pub + 8 * q, got_pub + 8 * q + in[i].n_pub, pub.begin() + 8 * (size_t)i);
+            }
+        }
+        upload(d_in, in);
     }
 
     // tape scratch for `ids`: capacity cap[2e], cap[2e + 1] each
@@ -257,7 +334,7 @@ struct Executions {
         std::vector<unsigned> pending;
         for (unsigned i : ids) if (status[i] == DG_OK) pending.push_back(i);
         for (unsigned long long extra = 256; !pending.empty(); extra *= 16) {
-            for (unsigned e : pending) { cap[2 * e] = x.inputs[e].n_secret_a + extra; cap[2 * e + 1] = x.inputs[e].n_secret_b + extra; }
+            for (unsigned e : pending) { cap[2 * e] = in[e].n_a + extra; cap[2 * e + 1] = in[e].n_b + extra; }
             place_tapes(pending);
             launch_ids(pending);
             stats.shape_ms += timed([&] { vm_shape_pass(c, L); });
@@ -421,7 +498,7 @@ void prove_slabs(Context &c, Executions &X, const std::vector<Slab> &slabs, cons
         std::vector<uint32_t> n_in(k), n_out(k);
         std::vector<dg_options_t> opt(k);
         for (uint32_t q = 0; q < k; q++) {
-            in16[q] = x.inputs[ok[q]].public16; n_in[q] = x.inputs[ok[q]].n_public;
+            in16[q] = (const uint8_t *)&X.pub[(size_t)ok[q] * 8]; n_in[q] = X.in[ok[q]].n_pub;
             out16[q] = (const uint8_t *)&outs[(size_t)ok[q] * 8]; n_out[q] = num_outputs[ok[q]];
             opt[q] = opts[ok[q]];
         }
@@ -696,7 +773,7 @@ struct TabledExecutions {
         X.upload(d_seq, seq);
         std::vector<unsigned> pending = run;
         while (!pending.empty()) {
-            for (unsigned e : pending) { X.cap[2 * e] = x.inputs[e].n_secret_a + extra[e]; X.cap[2 * e + 1] = x.inputs[e].n_secret_b + extra[e]; }
+            for (unsigned e : pending) { X.cap[2 * e] = X.in[e].n_a + extra[e]; X.cap[2 * e + 1] = X.in[e].n_b + extra[e]; }
             X.place_tapes(pending);
             // one warp per execution: the executions of a warp would take different paths through the interpreter (DESIGN.md section 7i)
             std::vector<unsigned> lanes;
@@ -799,11 +876,35 @@ struct TabledExecutions {
 
 }  // namespace
 
+// the whole-call checks of device inputs: every array there, and every non-empty range inside d_values, which is there and aligned when
+// some range is not empty
+static void check_device_inputs(const dg_device_inputs_t &d, uint32_t count) {
+    DG_REQUIRE(d.public_first && d.n_public && d.secret_a_first && d.n_secret_a && d.secret_b_first && d.n_secret_b,
+               "device inputs: null offset or count array");
+    bool any = false;
+    static const char *what[3] = {"public inputs", "tape A", "tape B"};
+    for (uint32_t i = 0; i < count; i++) {
+        const uint64_t first[3] = {d.public_first[i], d.secret_a_first[i], d.secret_b_first[i]};
+        const uint64_t n[3] = {d.n_public[i], d.n_secret_a[i], d.n_secret_b[i]};
+        for (int r = 0; r < 3; r++) {
+            if (n[r] == 0) continue;
+            any = true;
+            const std::string at = "device inputs of execution " + std::to_string(i) + ": " + what[r] + " [" + std::to_string(first[r]) + ", + " +
+                                   std::to_string(n[r]) + ")";
+            DG_REQUIRE(first[r] + n[r] >= first[r], at + " overflows");
+            DG_REQUIRE(first[r] + n[r] <= d.n_values, at + " ends past n_values = " + std::to_string(d.n_values));
+        }
+    }
+    if (!any) return;
+    DG_REQUIRE(d.d_values, "device inputs: d_values is null");
+    DG_REQUIRE(((uintptr_t)d.d_values & 15) == 0, "device inputs: d_values is not 16-byte aligned");
+}
+
 void check_execution_call(const ExecutionCall &x, const std::optional<OutputCounts> &outputs, std::optional<uint64_t> segment_steps) {
     DG_REQUIRE(x.count >= 1, "at least one execution is needed");
     DG_REQUIRE(x.n_programs >= 1, "at least one program is needed");
     DG_REQUIRE(x.programs && x.program_of, "null program table");
-    DG_REQUIRE(x.inputs, "null inputs");
+    DG_REQUIRE(x.inputs || x.device_inputs, "null inputs");
     DG_REQUIRE(x.max_steps >= 16, "max_steps must be at least 16");
     uint64_t ops = 0, blocks = 0, children = 0;
     for (uint32_t p = 0; p < x.n_programs; p++) {
@@ -821,10 +922,12 @@ void check_execution_call(const ExecutionCall &x, const std::optional<OutputCoun
     for (uint32_t i = 0; i < x.count; i++) {
         DG_REQUIRE(x.program_of[i] < x.n_programs, "program_of[" + std::to_string(i) + "] = " + std::to_string(x.program_of[i]) +
                                                        " is out of range: the call has " + std::to_string(x.n_programs) + " programs");
+        if (x.device_inputs) continue;
         const dg_program_inputs_t &v = x.inputs[i];
         DG_REQUIRE((v.n_public == 0 || v.public16) && (v.n_secret_a == 0 || v.secret_a16) && (v.n_secret_b == 0 || v.secret_b16),
                    "null inputs of execution " + std::to_string(i));
     }
+    if (x.device_inputs) check_device_inputs(*x.device_inputs, x.count);
     if (outputs) {
         DG_REQUIRE(outputs->num_outputs, "null num_outputs");
         bool any = false;

@@ -50,13 +50,15 @@ std::vector<uint32_t> cut_groups(const std::vector<uint32_t> &width, const std::
 // the device order of a group: positions of the traces grouped by shape, shapes in order of first appearance, input order inside a shape
 std::vector<uint32_t> shape_order(const std::vector<RegisterShape> &shape);
 
-// The execution calls (execute.cu).  Execution i runs programs[program_of[i]] on inputs[i]; status / messages per execution.
+// The execution calls (execute.cu).  Execution i runs programs[program_of[i]] on inputs[i], or, when inputs is null, on the inputs the
+// device descriptor gives it; status / messages per execution.
 struct ExecutionCall {
     const dg_program_t *programs;
     uint32_t n_programs, count;
     const uint32_t *program_of;
     const dg_program_inputs_t *inputs;
     uint64_t max_steps;
+    const dg_device_inputs_t *device_inputs = nullptr;
 };
 // the output counts of an execute call: num_outputs[i] <= 8 per execution; outputs16 may be null when every count is 0
 struct OutputCounts {

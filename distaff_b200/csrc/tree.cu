@@ -95,6 +95,45 @@ void tree_paths(Context &c, const Tree &t, const uint64_t *indexes, uint32_t cou
     DG_CUDA(cudaStreamSynchronize(c.stream));
 }
 
+// Thread t of a launch writes value t % per of leaf indexes[t / per] (dg_tree_membership_inputs), each from the heap or the index itself.
+// Path entry e of leaf i is leaf i (e = 0), leaf i ^ 1 (e = 1) or nodes[((L + i) >> 1 >> (e - 2)) ^ 1]; a tape takes element 0 (A) or 1 (B)
+// of an entry.  smpath (per = 4 d + 2): per tape 2 d + 1 values, entry 0, then for e = 1 .. d the pair (0 on A / bit e - 1 of i on B,
+// entry e).  pmpath (per = 2 d + 3): i, then tape A = element 0 of entries 0 .. d, then tape B = element 1 of them.
+__global__ void __launch_bounds__(256) membership_inputs_kernel(const uint4 *__restrict__ leaves, const uint4 *__restrict__ nodes,
+                                                                const unsigned long long *__restrict__ indexes, unsigned long long total,
+                                                                unsigned d, bool pmpath, unsigned long long L, uint4 *__restrict__ out) {
+    const unsigned long long t = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= total) return;
+    const unsigned per = pmpath ? 2 * d + 3 : 4 * d + 2;
+    const unsigned long long i = indexes[t / per];
+    const unsigned s = (unsigned)(t % per);
+    unsigned e, elem;
+    if (pmpath) {
+        if (s == 0) { out[t] = make_uint4((unsigned)i, (unsigned)(i >> 32), 0, 0); return; }
+        elem = (s - 1) / (d + 1);
+        e = (s - 1) % (d + 1);
+    } else {
+        elem = s / (2 * d + 1);
+        const unsigned j = s % (2 * d + 1);
+        if (j % 2 == 1) { out[t] = make_uint4(elem ? (unsigned)(i >> (j / 2)) & 1u : 0u, 0, 0, 0); return; }
+        e = j / 2;
+    }
+    out[t] = e == 0 ? leaves[2 * i + elem] : e == 1 ? leaves[2 * (i ^ 1) + elem] : nodes[2 * ((((L + i) >> 1) >> (e - 2)) ^ 1) + elem];
+}
+
+void tree_membership_inputs(Context &c, const Tree &t, bool pmpath, const uint64_t *indexes, uint32_t count, fe *values) {
+    if (count == 0) return;
+    const unsigned d = (unsigned)ceil_log2(t.L);
+    const unsigned long long total = (unsigned long long)count * (pmpath ? 2 * d + 3 : 4 * d + 2);
+    DevBuf d_idx((size_t)count * 8);
+    DG_CUDA(cudaMemcpyAsync(d_idx.p, indexes, (size_t)count * 8, cudaMemcpyHostToDevice, c.stream));
+    membership_inputs_kernel<<<(unsigned)((total + 255) / 256), 256, 0, c.stream>>>(t.leaves.as<uint4>(), t.nodes.as<uint4>(),
+                                                                                   d_idx.as<unsigned long long>(), total, d, pmpath, t.L, (uint4 *)values);
+    c.launches++;
+    DG_CUDA(cudaGetLastError());
+    DG_CUDA(cudaStreamSynchronize(c.stream));
+}
+
 static void launch_level(Context &c, const void *src, const unsigned long long *below_ids, size_t n_below, void *below,
                          const unsigned long long *ids, const unsigned *first, size_t n, unsigned long long base, void *msgs) {
     tree_level_kernel<<<(unsigned)((n_below + 255) / 256), 256, 0, c.stream>>>((const uint4 *)src, below_ids, (unsigned)n_below, (uint4 *)below,

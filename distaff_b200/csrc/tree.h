@@ -32,6 +32,9 @@ TreePlan plan_tree_update(const uint64_t *indexes, uint32_t count, unsigned long
 void tree_build(Context &c, Tree &t);
 // paths32[k (d + 1) + e], entry e of the authentication path of leaf indexes[k] (MerkleTree::prove order); indexes are < L
 void tree_paths(Context &c, const Tree &t, const uint64_t *indexes, uint32_t count, uint8_t *paths32);
+// dg_tree_membership_inputs: the smpath (pmpath false) or pmpath values of leaf indexes[k] at values + k per, per = 4 d + 2 or 2 d + 3 for
+// L = 2^d, in one gather launch from the heap; indexes are < L
+void tree_membership_inputs(Context &c, const Tree &t, bool pmpath, const uint64_t *indexes, uint32_t count, fe *values);
 // the leaf at the plan's leaves[k] becomes leaves32[source[k]]; rehashes the plan's nodes (or the whole tree, tree_update_rebuilds) and
 // reads the root
 void tree_update(Context &c, Tree &t, const TreePlan &plan, const uint8_t *leaves32);

@@ -361,6 +361,45 @@ int dg_execute_many_with_options(const dg_program_t *programs, uint32_t n_progra
                                  const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
                                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats);
 
+/* ---- program inputs in device memory -------------------------------------------------------------------------------------------------
+ * ProgramInputs::new (programs/inputs.rs:12-26) of `count` executions whose values are all in one device buffer: execution i reads its
+ * public inputs from d_values[public_first[i] .. + n_public[i]), tape A from d_values[secret_a_first[i] .. + n_secret_a[i]) and tape B
+ * from d_values[secret_b_first[i] .. + n_secret_b[i]), each range in reading order (its first value is read first).  Ranges may overlap
+ * or be shared between executions (one tape read by many of them): the values are only read.  d_values is device memory on the library's
+ * device, 16-byte aligned, n_values field elements of 16 little-endian bytes; it may be NULL when every count is 0.  The six arrays are
+ * host arrays of `count` entries each.  Writes to d_values must be complete (or ordered before the call on the library's stream). */
+typedef struct {
+    const void *d_values;
+    uint64_t n_values;
+    const uint64_t *public_first; const uint32_t *n_public;          /* at most 8 public inputs (lib.rs:32), else the execution fails */
+    const uint64_t *secret_a_first; const uint64_t *n_secret_a;      /* tape A */
+    const uint64_t *secret_b_first; const uint64_t *n_secret_b;      /* tape B, not longer than tape A, else the execution fails */
+} dg_device_inputs_t;
+/* dg_trace_programs, dg_execute_programs_with_options, dg_trace_many and dg_execute_many_with_options with `inputs` in device memory:
+ * the same arguments, results, statuses, messages and stats, with the inputs of execution i given by the descriptor.  The execute forms
+ * take one options entry per execution (a caller with one set of options replicates it).  Per execution the failures are exactly those of
+ * the host form: more than 8 public inputs, tape A shorter than tape B, and the first value >= M in the order public inputs, tape A, tape B
+ * ("tape A value 3 is not a field element", the index counted from the start of its range); each fails only its own execution.  Checked
+ * on the host before the device is touched (DG_ERR_INVALID, also without a GPU): everything the host forms check, a NULL descriptor or
+ * array ("null device inputs"), a NULL or unaligned d_values while any count is non-zero, and a range that overflows or ends past
+ * n_values (named by execution and region).  d_values must be device memory (DG_ERR_INVALID otherwise).  One GPU only, as every
+ * execution call.  The values are checked and packed for the VM by one kernel; only the public inputs (at most 8 per execution) and the
+ * first bad index per region come back to the host. */
+int dg_trace_programs_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                    const dg_device_inputs_t *inputs, uint64_t max_steps, dg_execution_info_t *info, uint8_t *const *registers_out,
+                                    int *status, dg_execution_stats_t *vm_stats);
+int dg_execute_programs_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                      const dg_device_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, const dg_options_t *options,
+                                      dg_proof_t **proofs_out, uint8_t *outputs16, int *status, dg_prove_stats_t *stats,
+                                      dg_execution_stats_t *vm_stats);
+int dg_trace_many_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                const dg_device_inputs_t *inputs, uint64_t max_steps, uint64_t segment_steps, dg_execution_info_t *info,
+                                uint8_t *const *registers_out, int *status, dg_many_stats_t *stats);
+int dg_execute_many_device_inputs(const dg_program_t *programs, uint32_t n_programs, uint32_t count, const uint32_t *program_of,
+                                  const dg_device_inputs_t *inputs, const uint32_t *num_outputs, uint64_t max_steps, uint64_t segment_steps,
+                                  const dg_options_t *options, dg_proof_t **proofs_out, uint8_t *outputs16, int *status,
+                                  dg_prove_stats_t *prove_stats, dg_many_stats_t *stats);
+
 /* ---- device memory ----------------------------------------------------------------------------------------------------------------
  * dg_set_memory_limit caps the device memory the library may hold on the current device: the per-proof arena, the stream-ordered pool it
  * allocates from otherwise, and its persistent tables.  0 (the default) means no limit.  The arena is never sized above the limit and the
@@ -503,6 +542,23 @@ int dg_tree_update(dg_tree_t *tree, const uint64_t *indexes, const uint8_t *leav
 /* copies the L leaves and / or the L heap nodes to the host; either may be NULL */
 int dg_tree_read(const dg_tree_t *tree, uint8_t *leaves32, uint8_t *nodes32);
 void dg_tree_free(dg_tree_t *tree);
+
+/* ---- membership inputs of a device tree ----------------------------------------------------------------------------------------------
+ * dg_tree_membership_inputs: the inputs of smpath.n (DG_PATH_SMPATH, index private) or pmpath.n (DG_PATH_PMPATH, index public), n = d + 1,
+ * for the leaves indexes[0 .. count) of a tree of hash 3 (DG_HASH_HASHER), written from the tree's heap straight into d_values in one
+ * gather launch; no path reaches the host.  Per index k the values are one run of the layout of the examples' merkle.rs:63-85:
+ *   smpath: tape A = leaf[0], then per later path entry e (0, e[0]); tape B = leaf[1], then (index bit, e[1]); no public input.
+ *           4 d + 2 values: A at k (4 d + 2), B after it.
+ *   pmpath: the index as the one public input, then tape A = e[0] and tape B = e[1] of every path entry.  2 d + 3 values: the index at
+ *           k (2 d + 3), A after it, B after A.
+ * out->n_values receives count times the values per index.  With d_values NULL that is all (the device is not touched).  Otherwise
+ * d_values (device, 16-byte aligned) holds cap values, at least out->n_values; out->d_values becomes d_values and the six arrays of `out`,
+ * which the caller points at host arrays of `count` entries, receive the ranges.  Indexes may repeat; one >= L fails the call with
+ * DG_ERR_INVALID naming it, as dg_tree_paths does, and so does a tree of another hash. */
+#define DG_PATH_SMPATH 0
+#define DG_PATH_PMPATH 1
+int dg_tree_membership_inputs(const dg_tree_t *tree, int program, const uint64_t *indexes, uint32_t count, void *d_values, uint64_t cap,
+                              dg_device_inputs_t *out);
 
 /* ---- batch proofs and their verification (MerkleTree::prove_batch / verify / verify_batch, merkle.rs:64-263) --------------------------
  * The encoding of a BatchMerkleProof {values, nodes, depth} is its bincode: u64 count + 32 B per value; u64 count, then per slot u64 count

@@ -9,7 +9,8 @@ the card's name and power limit, read in the same run.
               leaves, device ms (CUDA events) and wall ms of the call.
   paths       dg_tree_paths of 256 random leaves: wall ms of the call (one launch, the paths copied back).
   membership  --members leaves of a 2^20-leaf hasher tree, end to end, MerkleTree next to HasherTree: wall seconds to build the tree,
-              to get the paths and lay out the smpath inputs, and to run prove_membership (one execute_batch call with proofs).
+              to build the smpath inputs (gathered on the device from a MerkleTree, laid out on the host from a HasherTree), and to run
+              prove_membership (one execution call with proofs).
 
     python tools/tree_bench.py [--logs 14,20] [--ks 1,16,256,4096,65536] [--reps 3] [--members 256]
 """
@@ -119,7 +120,7 @@ def main():
             tree = dg.MerkleTree(pairs, "hasher") if arm == "MerkleTree" else dg.HasherTree(pairs)
             t1 = time.perf_counter()
             if arm == "MerkleTree":
-                tree._membership_inputs(idx, "smpath")
+                tree.membership_inputs(idx, "smpath")
             else:
                 [tree.smpath_inputs(i) for i in idx]
             t2 = time.perf_counter()
