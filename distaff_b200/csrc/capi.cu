@@ -1458,14 +1458,12 @@ int dg_test_syn_div(const uint8_t *in16, uint8_t *out16, uint32_t batch, uint64_
         require_canonical(in16, in_n, 1, "input element");
         require_canonical(b16, tables, 1, "point");
         require_canonical(sub0_16, batch, 1, "sub0");
-        // the (base, step) pairs of the tables of b, then of 1 / b, as prover.cu packs them
+        // the (base, step) pairs of the tables of b, then of 1 / b
         const std::vector<fe> b = host_fes(b16, tables);
         std::vector<fe> pack(4 * (size_t)tables);
         for (uint32_t q = 0; q < tables; q++) {
             DG_REQUIRE(b[q].lo || b[q].hi, "point " + std::to_string(q) + " is zero");
-            const fe bi = host_inv(b[q]);
-            pack[2 * q] = b[q]; pack[2 * q + 1] = PowTables::step(b[q], len + 1);
-            pack[2 * (tables + q)] = bi; pack[2 * (tables + q) + 1] = PowTables::step(bi, len + 1);
+            PowTables::pack_point(&pack[2 * q], 2 * (size_t)tables, b[q], len + 1);
         }
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
@@ -1630,9 +1628,8 @@ int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_s
         const uint64_t D = 1ULL << log_d, R = D / 4;
         const uint64_t in_n = strided_span(batch, values_stride, D, "values_stride");
         require_canonical(values16, in_n, 1, "value");
-        const Layout in{(int)log_d, log_b};
-        const int log_r = (int)log_d - 2;
-        const Layout rows{log_r, (in.log_b >= 0 && log_r >= in.log_b) ? in.log_b : -1};     // prover.cu: the next layer's layout
+        const Layout in{(int)log_d, log_b}, rows = fri_next_layout(in);
+        const FoldConstants fold = fri_fold_constants();
         Context &c = ctx();
         std::lock_guard<std::mutex> lk(c.mu);
         DevBuf d_vals, d_roots((batch - 1) * root_stride + 32), d_leaves, d_alpha, d_copies, d_next;
@@ -1645,8 +1642,8 @@ int dg_test_fri_layer(const uint8_t *values16, uint32_t batch, uint64_t values_s
         zeroed(c, d_next, batch * R);
         fri_hash_rows(c, d_vals.as<fe>(), in, rows, d_leaves.p, (int)batch, values_stride);
         fri_alpha(c, d_roots.p, d_alpha.as<fe>(), d_copies.p, (int)batch, root_stride);
-        fri_fold(c, d_vals.as<fe>(), in, d_next.as<fe>(), rows, d_alpha.as<fe>(), c.twiddle((int)log_N, true), (int)log_N,
-                 host_inv(host_root_of_unity(2)), host_inv(fe_make(4, 0)), (int)batch, values_stride);
+        fri_fold(c, d_vals.as<fe>(), in, d_next.as<fe>(), rows, d_alpha.as<fe>(), c.twiddle((int)log_N, true), (int)log_N, fold.tau_inv, fold.inv4,
+                 (int)batch, values_stride);
         DG_CUDA(cudaMemcpyAsync(leaves32, d_leaves.p, batch * R * 32, cudaMemcpyDeviceToHost, c.stream));
         DG_CUDA(cudaMemcpyAsync(alphas16, d_alpha.p, (size_t)batch * 16, cudaMemcpyDeviceToHost, c.stream));
         DG_CUDA(cudaMemcpyAsync(root_copies32, d_copies.p, (size_t)batch * 32, cudaMemcpyDeviceToHost, c.stream));
@@ -1712,7 +1709,7 @@ int dg_test_hash_trace_rows(const uint8_t *ext16, uint32_t total_cols, uint32_t 
             DG_CUDA(cudaMemcpyAsync(d_table.p, col_table, (size_t)batch * 8, cudaMemcpyHostToDevice, c.stream));
         }
         zeroed(c, d_leaves, 2 * leaves);
-        // stage 2 (prove_core's hash_chunk): the rows of the cosets [c0, c0 + nc) of every matrix, column stride nc n
+        // stage 2 (the prover's Group::hash_chunk): the rows of the cosets [c0, c0 + nc) of every matrix, column stride nc n
         hash_trace_rows(c, d_ext.as<fe>(), d_leaves.p, (int)w, (int)log_n, (int)log_blowup, (int)batch, (unsigned long long)w * rows, c0, nc,
                         leaf_stride, col_table ? d_table.as<uint2>() : nullptr);
         download(c, leaves32, d_leaves, leaves * 32);

@@ -126,6 +126,11 @@ void fri_fold(Context &c, const fe *values, Layout in, fe *next, Layout out, con
     c.launches++;
     DG_CUDA(cudaGetLastError());
 }
+Layout fri_next_layout(Layout in) {
+    const int log_r = in.log_d - 2;
+    return Layout{log_r, (in.log_b >= 0 && log_r >= in.log_b) ? in.log_b : -1};
+}
+FoldConstants fri_fold_constants() { return FoldConstants{host_inv(host_root_of_unity(2)), host_inv(fe_make(4, 0))}; }
 
 // ---- coset-sharded layers (multi-GPU): a rank holds the cosets [c0, c0 + 2^log_nc) of a layer of 2^log_d values as the slab
 //      [c - c0][k], k < 2^(log_d - log_b).  Row r = b k' + c and its three companions r + jR (R = D/4) have k = k' + j R/b inside the

@@ -38,6 +38,13 @@ static unsigned long long pow_hi_n(unsigned long long len) {
 }
 
 fe PowTables::step(fe base, unsigned long long len) { return fe_pow_u64(base, 1ULL << pow_lo_bits(len)); }
+void PowTables::pack_point(fe *pairs, size_t inv_at, fe x, unsigned long long len) {
+    const fe xi = host_inv(x);
+    pairs[0] = x;
+    pairs[1] = step(x, len);
+    pairs[inv_at] = xi;
+    pairs[inv_at + 1] = step(xi, len);
+}
 unsigned long long PowTables::entries(unsigned long long len) { return (1ULL << pow_lo_bits(len)) + pow_hi_n(len); }
 
 PowTables::PowTables(Context &c, const fe *base_step, int batch, unsigned long long len) {

@@ -14,6 +14,8 @@ struct PowTables {
     unsigned long long lo_n = 0, hi_n = 0;
     PowTables(Context &c, const fe *base_step, int batch, unsigned long long len);
     static fe step(fe base, unsigned long long len);          // the second entry of a table's pair
+    // the pairs of the tables of x and of 1 / x, both of length len, at pairs[0..2) and pairs[inv_at .. inv_at + 2)
+    static void pack_point(fe *pairs, size_t inv_at, fe x, unsigned long long len);
     static unsigned long long entries(unsigned long long len);   // lo_n + hi_n of one table
     PowRef ref(int q) const { PowRef r; r.lo = lo.as<fe>() + q * lo_n; r.hi = hi.as<fe>() + q * hi_n; r.lo_bits = lo_bits; return r; }
 };
@@ -100,6 +102,12 @@ void fri_hash_rows(Context &c, const fe *values, Layout in, Layout rows, void *l
 // batch > 1: `batch` layers values_stride elements apart, next R elements apart, folding point alpha[q] for layer q
 void fri_fold(Context &c, const fe *values, Layout in, fe *next, Layout out, const fe *alpha, const TwiddleRef &inv_root_table, int log_n_total,
               fe tau_inv, fe inv4, int batch = 1, unsigned long long values_stride = 0);
+// the layout of the layer that folding a layer of layout `in` produces (the layout of its row hashes): D / 4 values, coset-major while
+// at least 2^log_b of them remain, natural below
+Layout fri_next_layout(Layout in);
+// what fri_fold and fri_fold_local take besides the layer: 1 / tau (tau the 4th root of unity) and 1 / 4
+struct FoldConstants { fe tau_inv, inv4; };
+FoldConstants fri_fold_constants();
 // alpha_dev[0] = field::prng(root) (fri/prover.rs:29); root_copy_dev receives the 32 root bytes (collected for one host copy at the end)
 // batch > 1: the roots root_stride_bytes apart -> alpha_dev[q], root_copy_dev + 32 q
 void fri_alpha(Context &c, const void *root_dev, fe *alpha_dev, void *root_copy_dev, int batch = 1, unsigned long long root_stride_bytes = 0);

@@ -239,6 +239,11 @@ struct ProofState {
     void fail(int code, const std::string &m) { live = false; status = code; message = m; }
 };
 
+bool any_live(const std::vector<ProofState> &ps) {
+    for (auto &s : ps) if (s.live) return true;
+    return false;
+}
+
 // the 32-byte roots at `roots_dev` on the host: one copy for one tree, one FetchBatch for many
 std::vector<Digest> fetch_roots(Context &c, const std::vector<const void *> &roots_dev) {
     std::vector<Digest> out(roots_dev.size());
@@ -254,6 +259,11 @@ std::vector<Digest> fetch_roots(Context &c, const std::vector<const void *> &roo
     return out;
 }
 
+// the fine-grained device timeline (DG_SUBSTAGE): prove_core routes c.mark to its SubClock while the marks are on
+void substage(Context &c, const char *name) {
+    if (c.mark) c.mark(name);
+}
+
 // everything a proof opens, as offsets into the batch's FetchBatch (stage 9)
 struct LayerOpen { std::vector<size_t> val_off; Offsets node_off; uint8_t depth; };
 struct OpenPlan {
@@ -263,6 +273,800 @@ struct OpenPlan {
     std::vector<size_t> cval_off, rem_off;
     std::vector<LayerOpen> fri_open;
 };
+
+// The group of K proofs prove_core proves: what the call fixes (the constructor checks it and derives the geometry) and the device
+// buffers that one stage writes and a later stage reads.  Each buffer is allocated by the stage that first writes it and lives until the
+// group ends; a buffer only one stage uses is a local of that stage's function.
+struct Group {
+    // ---- the batch (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) ----
+    fe *d_regs;                                // [W][n] on the device; with host_cols not there yet (stage 1 uploads them)
+    const uint8_t *const *host_cols;
+    const std::vector<int> &order;             // Fiat-Shamir order of the proofs
+    int K = 0;
+    size_t W = 0;                              // columns of the whole batch
+    std::vector<TraceShape> shapes;
+    std::vector<uint32_t> col0;                // the column table: proof p's registers are the columns [col0[p], col0[p] + w_p) of the batch
+    std::vector<int> shape_first = {0};        // runs of proofs of one shape: [shape_first[s], shape_first[s + 1])
+    int wmax = 0, Tmax = 0;
+    uint64_t n = 0, b = 0, N = 0, E = 0;
+    int log_n = 0, log_b = 0, log_N = 0;
+    fe root_n;                                 // w_n, generator of the trace domain
+    // ---- sharding: rank g owns the LDE cosets [c0, c0 + nc) of every column (world == 1: all of them) ----
+    int G = 1, g = 0, log_g = 0, log_nc = 0;
+    uint64_t nc = 0, N_loc = 0;
+    unsigned c0 = 0;
+    // G > 1: the interpolation is sharded by columns -- rank r interpolates the columns [col_start(r), col_start(r) + col_count(r)), an even
+    // split (the first w mod G ranks own one more), and the polynomials are all-gathered in equal slots of cpr columns per rank
+    int w = 0, cpr = 0;                        // the width of the one proof; slot size of the gather = largest share
+    // ---- layout of the extension.  ext holds `chunk` cosets of every column at a time ([W][chunk][n]).  The retained slab holds the
+    // cosets stage 3 reads: in the full layout the whole extension (slab = ext), in the evaluation-coset layout the 8 cosets
+    // c = 0 (mod b / 8), [W][8][n].  An opened row outside the retained cosets is computed from the trace polynomials in stage 9. ----
+    unsigned chunk = 0;
+    bool full = true;
+    int log_ret = 0;                           // retained cosets: all of this rank's, or the 8 evaluation cosets
+    uint64_t slab_col = 0, rstep = 0;          // slab column stride; retained cosets are c = 0 (mod rstep)
+    uint64_t ext_col = 0;                      // column stride of ext (N_loc in the full layout)
+    // the column table on the device: [K] (first column, width) of every proof, then [W] the proof of every column
+    DevBuf d_table;
+    const uint2 *d_cols = nullptr;
+    const unsigned *d_col_proof = nullptr;
+    // ---- buffers that cross stages (and those a stage keeps to the end of the group) ----
+    DevBuf polys, ext, slab_own, t_leaves, t_nodes;      // 1-2: trace polynomials, extension, retained slab, trace trees
+    DevBuf d_violation, d_coef, evals;                   // 3: violation flags, coefficients, [K][3][E] boundary / transition coefficients
+    DevBuf combined, scratch, scratch2;                  // 4: the constraint polynomial, division scratch (scratch2: stage 6)
+    DevBuf c_ext, c_items, c_nodes;                      // 5: constraint extension and trees
+    DevBuf comp, comp_ext;                               // 6: composition polynomial and its extension
+    DevBuf fri_gathered;                                 // 7, multi-GPU: the first replicated layer, gathered from the ranks' slabs
+    std::vector<DevBuf> layer_bufs;                      // 7: replicated layers: row hashes, trees and folded values of all K proofs
+    DevBuf d_rows;                                       // 9: opened trace rows computed from the polynomials
+
+    Group(Context &c, fe *d_regs, const uint8_t *const *host_cols, const std::vector<RegisterShape> &regs_shape, uint64_t length,
+          const std::vector<int> &order, std::vector<ProofState> &ps, const std::vector<dg_options_t> &opts, unsigned chunk);
+    int col_count(int r) const { return w / G + (r < w % G ? 1 : 0); }
+    int col_start(int r) const { return r * (w / G) + std::min(r, w % G); }
+    const fe *slab_of(int p) const { return (full ? ext.as<fe>() : slab_own.as<fe>()) + (size_t)col0[p] * slab_col; }
+    const fe *c_ext_of(int p) const { return c_ext.as<fe>() + (size_t)p * N_loc; }
+    bool retained(uint64_t pos) const { return ((pos & (b - 1)) & (rstep - 1)) == 0; }
+    void alloc_extension();
+    void hash_chunk(Context &c, unsigned cc);
+};
+
+Group::Group(Context &c, fe *d_regs_, const uint8_t *const *host_cols_, const std::vector<RegisterShape> &regs_shape, uint64_t length,
+             const std::vector<int> &order_, std::vector<ProofState> &ps, const std::vector<dg_options_t> &opts, unsigned chunk_)
+    : d_regs(d_regs_), host_cols(host_cols_), order(order_) {
+    K = (int)ps.size();
+    DG_REQUIRE(K >= 1 && regs_shape.size() == ps.size() && order.size() == ps.size() && opts.size() == ps.size(), "batch must hold at least one trace");
+    n = length;
+    b = opts[0].extension_factor;
+    for (const RegisterShape &r : regs_shape) W += r.width;
+    DG_REQUIRE(W <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
+    for (const dg_options_t &o : opts) {
+        check_options(o);
+        DG_REQUIRE(o.extension_factor == b, "the proofs of a group share one extension factor");
+    }
+    DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
+    for (const RegisterShape &r : regs_shape) shapes.push_back(TraceShape::of_trace(r.width, r.ctx_depth, r.loop_depth));
+    col0.assign(K + 1, 0);
+    for (int p = 0; p < K; p++) {
+        col0[p + 1] = col0[p] + shapes[p].w;
+        wmax = std::max(wmax, shapes[p].w);
+        Tmax = std::max(Tmax, shapes[p].T);
+    }
+    log_n = ceil_log2(n);
+    log_b = ceil_log2(b);
+    log_N = log_n + log_b;
+    DG_REQUIRE(log_N <= 30, "LDE domain too large");
+    N = n * b;
+    E = n * 8;
+    for (int p = 0; p < K; p++) {             // what the call fixes in every proof: the register shape and its options (blake3)
+        TraceInfo &t = ps[p].stark.trace_info;
+        t.ctx_depth = (uint8_t)shapes[p].ctx_depth; t.loop_depth = (uint8_t)shapes[p].loop_depth; t.stack_depth = (uint8_t)shapes[p].stack_depth;
+        ps[p].stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opts[p].num_queries, (uint8_t)opts[p].grinding_factor, 0};
+    }
+    for (int p = 1; p < K; p++)
+        if (!(regs_shape[p] == regs_shape[p - 1])) shape_first.push_back(p);
+    shape_first.push_back(K);
+    root_n = host_root_of_unity(log_n);
+
+    G = c.world;
+    g = c.rank;
+    DG_REQUIRE(G == 1 || K == 1, "a batch of proofs runs on one GPU (the context spans several)");
+    log_g = ceil_log2(G);
+    DG_REQUIRE((b >> log_g) >= 4 && G <= 8, "extension factor too small for this many GPUs (need >= 4 cosets per rank)");
+    log_nc = log_b - log_g;
+    nc = 1ULL << log_nc;
+    N_loc = n * nc;
+    c0 = (unsigned)(g * nc);
+    w = shapes[0].w;
+    cpr = (w + G - 1) / G;
+
+    chunk = chunk_;
+    if (G > 1 || chunk == 0 || chunk > nc) chunk = (unsigned)nc;
+    DG_REQUIRE((chunk & (chunk - 1)) == 0, "coset chunk must be a power of 2");
+    full = chunk == nc;
+    log_ret = full ? log_nc : 3;
+    slab_col = n << log_ret;
+    rstep = nc >> log_ret;
+    ext_col = n * chunk;
+
+    d_table.alloc((2 * K + W) * 4);
+    std::vector<uint32_t> table(2 * K + W);
+    for (int p = 0; p < K; p++) {
+        table[2 * p] = col0[p];
+        table[2 * p + 1] = (uint32_t)shapes[p].w;
+        for (uint32_t j = col0[p]; j < col0[p + 1]; j++) table[2 * K + j] = (uint32_t)p;
+    }
+    h2d(c, d_table.p, table.data(), table.size() * 4);
+    d_cols = d_table.as<uint2>();
+    d_col_proof = d_table.as<unsigned>() + 2 * K;
+}
+
+// ---- 1: extend execution trace ------------------------------------------------------------------------------------------------------------
+void Group::alloc_extension() {
+    polys.alloc(W * n * 16);
+    ext.alloc(W * ext_col * 16);
+    if (!full) slab_own.alloc(W * slab_col * 16);
+    t_leaves.alloc((size_t)K * N_loc * 32);
+}
+
+// rows of the chunk at cc: leaves (k << log_b) + c of every proof; then its retained cosets into the slab
+void Group::hash_chunk(Context &c, unsigned cc) {
+    hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, 0, cc, chunk, N_loc, d_cols);   // local rows, [k][c - c0], per proof
+    if (full) return;
+    for (unsigned cs = cc; cs < cc + chunk; cs++)
+        if (cs % rstep == 0)
+            DG_CUDA(cudaMemcpy2DAsync(slab_own.as<fe>() + (cs / rstep) * n, slab_col * 16, ext.as<fe>() + (size_t)(cs - cc) * n, ext_col * 16, n * 16, W,
+                                      cudaMemcpyDeviceToDevice, c.stream));
+}
+
+// One GPU: the K proofs' registers are the W columns of one batch, interpolated in column chunks: a host trace is uploaded in chunks of
+// ~64 MB, but a short ramp first (1, 2 columns), so that the first transform starts after one column's worth of copying; every column
+// chunk is extended on the first coset chunk as soon as it has been interpolated.  Every coset chunk but the last is hashed here.
+void extend_trace(Context &c, Group &grp) {
+    grp.alloc_extension();
+    const uint64_t n = grp.n;
+    const int W = (int)grp.W;
+    fe *regs = grp.d_regs, *polys = grp.polys.as<fe>(), *ext = grp.ext.as<fe>();
+    std::vector<int> bounds = {0};
+    std::unique_ptr<TraceUploader> up;
+    if (grp.host_cols) {
+        const int step_max = (int)std::max<uint64_t>(1, std::min<uint64_t>(W, ((uint64_t)1 << 26) / (n * 16)));
+        for (int step = 1; bounds.back() < W; step = std::min(step_max, step * 2)) bounds.push_back(std::min(W, bounds.back() + step));
+        up.reset(new TraceUploader(c, regs, grp.host_cols, W, n, bounds));
+    } else {
+        bounds.push_back(W);
+    }
+    for (unsigned cc = 0; cc < grp.nc; cc += grp.chunk) {
+        if (cc > 0) grp.hash_chunk(c, cc - grp.chunk);          // the last chunk is hashed in stage 2
+        for (size_t i = 0; i + 1 < bounds.size(); i++) {
+            const int j0 = bounds[i], cols = bounds[i + 1] - j0;
+            if (cc == 0) {
+                if (up) up->wait_chunk((int)i);
+                ntt_batch(c, regs + (size_t)j0 * n, polys + (size_t)j0 * n, grp.log_n, cols, n, n, true);
+            }
+            extend_trace_columns(c, polys + (size_t)j0 * n, regs + (size_t)j0 * n, ext + (size_t)j0 * grp.ext_col, cols, grp.log_n, grp.log_b,
+                                 grp.ext_col, cc, grp.chunk);
+        }
+    }
+}
+
+// Several GPUs (one proof): rank g interpolates its share of the columns and only needs (from a host trace: only uploads) those
+// registers; the polynomials are all-gathered (and compacted into natural column order) while the rank extends its own columns, then
+// every rank extends all columns on its cosets.
+void extend_trace_sharded(Context &c, Group &grp) {
+    grp.alloc_extension();
+    const uint64_t n = grp.n, N_loc = grp.N_loc;
+    const int G = grp.G, cpr = grp.cpr, w = grp.w, log_n = grp.log_n, log_b = grp.log_b;
+    const unsigned c0 = grp.c0, nc = (unsigned)grp.nc;
+    fe *regs = grp.d_regs, *polys = grp.polys.as<fe>(), *ext = grp.ext.as<fe>();
+    const uint8_t *const *host_cols = grp.host_cols;
+    const int j0 = grp.col_start(grp.g), mine = grp.col_count(grp.g);
+    DevBuf own((size_t)cpr * n * 16), slots((size_t)cpr * G * n * 16);
+    if (mine > 0) {
+        if (host_cols) {
+            std::vector<int> bounds(mine + 1);
+            for (int i = 0; i <= mine; i++) bounds[i] = i;
+            TraceUploader up(c, regs + (size_t)j0 * n, host_cols + j0, mine, n, bounds);      // one column per chunk: all staging workers busy
+            for (int i = 0; i < up.chunks(); i++) {              // interpolate every column as soon as it has landed
+                up.wait_chunk(i);
+                ntt_batch(c, regs + (size_t)(j0 + i) * n, own.as<fe>() + (size_t)i * n, log_n, 1, n, n, true);
+            }
+        } else {
+            ntt_batch(c, regs + (size_t)j0 * n, own.as<fe>(), log_n, mine, n, n, true);
+        }
+    }
+    substage(c, "1.intt");
+    // the all-gather of the polynomials (and their compaction into column order) runs on the communication stream while this rank
+    // already extends its own columns
+    cudaEvent_t ev_own, ev_all;
+    DG_CUDA(cudaEventCreateWithFlags(&ev_own, cudaEventDisableTiming));
+    DG_CUDA(cudaEventCreateWithFlags(&ev_all, cudaEventDisableTiming));
+    DG_CUDA(cudaEventRecord(ev_own, c.stream));
+    DG_CUDA(cudaStreamWaitEvent(c.comm_stream, ev_own, 0));
+    comm_all_gather(c, own.p, slots.p, (size_t)cpr * n * 16, c.comm_stream);
+    for (int r = 0; r < G; r++)
+        if (grp.col_count(r) > 0)
+            DG_CUDA(cudaMemcpyAsync(polys + (size_t)grp.col_start(r) * n, slots.as<fe>() + (size_t)r * cpr * n, (size_t)grp.col_count(r) * n * 16,
+                                    cudaMemcpyDeviceToDevice, c.comm_stream));
+    DG_CUDA(cudaEventRecord(ev_all, c.comm_stream));
+    if (mine > 0) extend_trace_columns(c, own.as<fe>(), regs + (size_t)j0 * n, ext + (size_t)j0 * N_loc, mine, log_n, log_b, N_loc, c0, nc);
+    substage(c, "1.lde_own");
+    DG_CUDA(cudaStreamWaitEvent(c.stream, ev_all, 0));
+    // the other ranks' registers are on this device only when the trace was given in device memory (a host trace uploads own columns only)
+    if (j0 > 0) extend_trace_columns(c, polys, host_cols ? nullptr : regs, ext, j0, log_n, log_b, N_loc, c0, nc);
+    if (j0 + mine < w)
+        extend_trace_columns(c, polys + (size_t)(j0 + mine) * n, host_cols ? nullptr : regs + (size_t)(j0 + mine) * n, ext + (size_t)(j0 + mine) * N_loc,
+                             w - j0 - mine, log_n, log_b, N_loc, c0, nc);
+    cudaEventDestroy(ev_own);
+    cudaEventDestroy(ev_all);
+}
+
+// ---- 2: trace Merkle tree -------------------------------------------------------------------------------------------------------------------
+// one GPU: the K trees level by level in one launch per level; several GPUs (K == 1): the sharded tree
+void commit_trace(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K;
+    const uint64_t N_loc = grp.N_loc;
+    grp.hash_chunk(c, (unsigned)(grp.nc - grp.chunk));
+    substage(c, "2.hash_rows");
+    if (grp.G == 1) {
+        grp.t_nodes.alloc((size_t)K * N_loc * 32);
+        merkle_build(c, grp.t_leaves.p, grp.t_nodes.p, N_loc, K);
+    }
+    std::vector<const void *> roots;
+    for (int p = 0; p < K; p++) {
+        const uint8_t *leaves = (const uint8_t *)grp.t_leaves.p + (size_t)p * N_loc * 32;
+        if (grp.G == 1) ps[p].t_tree.attach(c, leaves, (const uint8_t *)grp.t_nodes.p + (size_t)p * N_loc * 32, grp.n, grp.log_nc);
+        else ps[p].t_tree.build(c, leaves, grp.n, grp.log_nc, false);
+        roots.push_back(ps[p].t_tree.root_dev());
+    }
+    std::vector<Digest> r = fetch_roots(c, roots);
+    for (int p = 0; p < K; p++) ps[p].stark.trace_root = r[p];
+}
+
+// ---- 3: evaluate constraints --------------------------------------------------------------------------------------------------------------
+// false when every proof failed its transition constraints: the group ends there
+bool evaluate_constraints(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K, G = grp.G, log_n = grp.log_n;
+    const uint64_t n = grp.n, E = grp.E;
+    const std::vector<TraceShape> &shapes = grp.shapes;
+    std::vector<fe> last_rows((size_t)3 * K);      // op_counter and program hash of the last trace step of every proof (evaluator.rs:73-74)
+    if (grp.host_cols) {
+        for (int p = 0; p < K; p++)
+            for (int j = 0; j < 3; j++) memcpy(&last_rows[3 * p + j], grp.host_cols[grp.col0[p] + j] + (n - 1) * 16, 16);
+    } else {
+        DevBuf d_last((size_t)48 * K);
+        for (size_t s = 0; s + 1 < grp.shape_first.size(); s++) {          // the proofs of one shape are w n elements apart
+            const int p0 = grp.shape_first[s], k = grp.shape_first[s + 1] - p0;
+            for (int j = 0; j < 3; j++)
+                DG_CUDA(cudaMemcpy2DAsync((uint8_t *)d_last.p + 48 * p0 + 16 * j, 48, grp.d_regs + (size_t)(grp.col0[p0] + j) * n + (n - 1),
+                                          (size_t)shapes[p0].w * n * 16, 16, k, cudaMemcpyDeviceToDevice, c.stream));
+        }
+        d2h(c, last_rows.data(), d_last.p, (size_t)48 * K);
+    }
+    grp.d_violation.alloc((size_t)4 * K);
+    // per proof [coefA | coefB | bAi | bBi | bAf | bBf], coef_stride elements apart, then the boundary constants [K][KiA, KiB, KfA, KfB].
+    // The transition coefficients of a proof are T of its shape: coefA and coefB are padded to the batch's largest count Tmax.  The
+    // boundary vectors have one entry per register that carries a boundary constraint, which depends on the shape and on the number of
+    // public inputs / outputs: they are padded with zero coefficients to the largest count nbm (a zero coefficient adds nothing to the
+    // boundary numerators).
+    const size_t T = grp.Tmax;
+    size_t nbm = 0;
+    for (int p : grp.order) {
+        ProofState &s = ps[p];
+        s.stark.trace_info.op_count = (uint32_t)last_rows[3 * p].lo;       // op_count as u32 (proof.rs:62)
+        const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
+        s.cc = fs::draw_constraint_coefficients(s.stark.trace_root.data(), shapes[p], s.inputs, s.outputs, last_rows[3 * p], program_hash);
+        DG_REQUIRE(s.cc.bAi.size() <= (size_t)shapes[p].w, "more boundary registers than registers");
+        nbm = std::max(nbm, s.cc.bAi.size());
+    }
+    const size_t coef_stride = 2 * T + 4 * nbm;
+    {
+        std::vector<fe> pack(coef_stride * K + 4 * K, fe_make(0, 0));
+        for (int p = 0; p < K; p++) {
+            ProofState &s = ps[p];
+            auto at = pack.begin() + (size_t)p * coef_stride;
+            std::copy(s.cc.coefA.begin(), s.cc.coefA.end(), at);
+            std::copy(s.cc.coefB.begin(), s.cc.coefB.end(), at + T);
+            int slot = 0;
+            for (const auto *v : {&s.cc.bAi, &s.cc.bBi, &s.cc.bAf, &s.cc.bBf}) std::copy(v->begin(), v->end(), at + 2 * T + (slot++) * nbm);
+            const fe consts[4] = {s.cc.KiA, s.cc.KiB, s.cc.KfA, s.cc.KfB};
+            std::copy(consts, consts + 4, pack.begin() + coef_stride * K + 4 * p);
+        }
+        grp.d_coef.alloc(pack.size() * 16);
+        h2d(c, grp.d_coef.p, pack.data(), pack.size() * 16);
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    const fe *coef = grp.d_coef.as<fe>();
+    DG_CUDA(cudaMemsetAsync(grp.d_violation.p, 0, (size_t)4 * K, c.stream));
+    // per proof: [boundary numerator, first step | boundary numerator, last step | transition combination]
+    grp.evals.alloc((size_t)K * 3 * E * 16);
+    fe *evals = grp.evals.as<fe>();
+    const int num_c8 = 8 >> grp.log_g;
+    const uint64_t E_loc = n * num_c8;
+    DevBuf evals_loc((size_t)K * E_loc * 16), gathered;
+    if (G > 1) gathered.alloc(E * 16);
+    // one launch per register shape, over that shape's proofs (adjacent, so at uniform strides)
+    for (size_t s = 0; s + 1 < grp.shape_first.size(); s++) {
+        const int p0 = grp.shape_first[s], k = grp.shape_first[s + 1] - p0;
+        AirParams P = shapes[p0].air_params(n);
+        // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
+        // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
+        P.log_blowup = grp.full ? grp.log_b : 3;
+        P.ext = grp.slab_of(p0); P.col_stride = grp.slab_col;
+        P.c8_base = grp.g * num_c8; P.num_c8 = num_c8;
+        P.t_ev = evals_loc.as<fe>() + (size_t)p0 * E_loc;
+        P.periodic = periodic_table(c);
+        const fe *base = coef + (size_t)p0 * coef_stride;
+        P.coefA = base; P.coefB = base + T;
+        P.twN = c.twiddle(grp.full ? grp.log_N : log_n + 3, false);
+        P.violation = grp.d_violation.as<unsigned>() + p0;
+        P.ext_stride = (size_t)shapes[p0].w * grp.slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
+        if (s == 0) substage(c, "3.setup");
+        launch_constraint_eval(c, P, k);
+    }
+    substage(c, "3.eval");
+    comm_all_reduce_max_u32(c, grp.d_violation.as<unsigned>(), 1);
+    std::vector<unsigned> violation(K);
+    d2h(c, violation.data(), grp.d_violation.p, (size_t)4 * K);
+    for (int p = 0; p < K; p++)
+        if (violation[p])
+            ps[p].fail(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation_step(violation[p])) + " were not satisfied");
+    if (!any_live(ps)) return false;
+    // interpolation of the transition combination (constraint_table.rs:54-63), coset by coset: size-n inverse transforms of the own
+    // cosets (sharded), all-gather, then the 8-point inverse DFT across cosets (poly.cu: coset_interp_finish) -> the 8n coefficients
+    // in natural order; no transposition and no replicated 8n-point transform
+    substage(c, "3.violation_sync");
+    ntt_batch(c, evals_loc.as<fe>(), evals_loc.as<fe>(), log_n, K * num_c8, n, n, true);
+    if (G > 1) comm_all_gather(c, evals_loc.as<fe>(), gathered.as<fe>(), E_loc * 16);
+    substage(c, "3.intt+gather");
+    coset_interp_finish(c, G > 1 ? gathered.as<fe>() : evals_loc.as<fe>(), evals + 2 * E, log_n, K, E_loc, 3 * E);
+    // boundary constraints (evaluator.rs:181-326), directly as the 8n coefficients the reference obtains by interpolation
+    boundary_coeffs(c, K, grp.polys.as<fe>(), 0, n, (int)nbm, coef + 2 * T, coef_stride, coef + coef_stride * K, evals, evals + E, 3 * E, grp.d_cols);
+    if (K == 1) debug_dump(c, "t_coeffs", evals + 2 * E, E * 16);
+    return true;
+}
+
+// ---- 4: convert constraint evaluations into a polynomial -----------------------------------------------------------------------------------
+void constraint_polynomial(Context &c, Group &grp) {
+    const int K = grp.K;
+    const uint64_t E = grp.E;
+    grp.combined.alloc((size_t)K * E * 16);
+    grp.scratch.alloc((size_t)K * E * 16);
+    grp.scratch2.alloc((size_t)K * E * 16);
+    const fe x_last = host_inv(grp.root_n);                    // w_n^(n-1)   (evaluator.rs:128-131)
+    fe *ic = grp.evals.as<fe>(), *fc = ic + E, *tc = ic + 2 * E;          // of proof 0; proof p at + 3 E p
+    if (K == 1) {
+        debug_dump(c, "i_coeffs", ic, E * 16);
+        debug_dump(c, "f_coeffs", fc, E * 16);
+    }
+    // one upload: the (base, step) pairs of the power tables of 1, x_last and 1 / x_last (shared by the K proofs), then K zeros (sub0)
+    std::vector<fe> pack(6 + K, fe_make(0, 0));
+    pack[0] = fe_make(1, 0);
+    pack[1] = PowTables::step(pack[0], E + 1);
+    PowTables::pack_point(pack.data() + 2, 2, x_last, E + 1);
+    DevBuf d_pack(pack.size() * 16);
+    h2d(c, d_pack.p, pack.data(), pack.size() * 16);
+    PowTables pows(c, d_pack.as<fe>(), 3, E + 1);
+    const fe *zeros = d_pack.as<fe>() + 6;
+    syn_div(c, K, ic, 3 * E, ic, 3 * E, E, pows.ref(0), 0, 0, pows.ref(0), 0, 0, zeros);   // / (x - 1)
+    syn_div(c, K, fc, 3 * E, fc, 3 * E, E, pows.ref(1), 0, 0, pows.ref(2), 0, 0, zeros);   // / (x - x_last)
+    syn_div_expanded_sum(c, tc, grp.scratch.as<fe>(), ic, fc, grp.combined.as<fe>(), grp.n, E, x_last, K, 3 * E, E);   // / ((x^n - 1)/(x - x_last)), summed
+    if (K == 1) debug_dump(c, "constraint_poly", grp.combined.p, E * 16);
+}
+
+// ---- 5: constraint evaluations over the LDE domain + their Merkle tree ---------------------------------------------------------------------
+void commit_constraints(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K, log_nc = grp.log_nc;
+    const uint64_t N_loc = grp.N_loc;
+    grp.c_ext.alloc((size_t)K * N_loc * 16);
+    grp.c_items.alloc((size_t)K * (N_loc / 4) * 32);
+    lde_batch(c, grp.combined.as<fe>(), grp.c_ext.as<fe>(), grp.log_n, grp.log_b, 8, K, grp.E, N_loc, grp.c0, (unsigned)grp.nc);
+    substage(c, "5.lde");
+    constraint_items_local(c, grp.c_ext.as<fe>(), grp.log_n, log_nc, grp.c_items.p, K);      // first tree level: H(4 evaluations), [k][c4 local], per proof
+    substage(c, "5.items");
+    if (grp.G == 1) {
+        grp.c_nodes.alloc((size_t)K * (N_loc / 4) * 32);
+        merkle_build(c, grp.c_items.p, grp.c_nodes.p, N_loc / 4, K);
+    }
+    std::vector<const void *> roots;
+    std::vector<int> who;
+    for (int p = 0; p < K; p++) {
+        if (!ps[p].live) continue;
+        const uint8_t *items = (const uint8_t *)grp.c_items.p + (size_t)p * (N_loc / 4) * 32;
+        if (grp.G == 1) ps[p].c_tree.attach(c, items, (const uint8_t *)grp.c_nodes.p + (size_t)p * (N_loc / 4) * 32, grp.n, log_nc - 2);
+        else ps[p].c_tree.build(c, items, grp.n, log_nc - 2, false);
+        roots.push_back(ps[p].c_tree.root_dev());
+        who.push_back(p);
+    }
+    std::vector<Digest> r = fetch_roots(c, roots);
+    for (size_t i = 0; i < who.size(); i++) ps[who[i]].stark.constraint_root = r[i];
+}
+
+// ---- 6: DEEP composition polynomial --------------------------------------------------------------------------------------------------------
+void deep_composition(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K, G = grp.G, cpr = grp.cpr, wmax = grp.wmax;
+    const uint64_t n = grp.n, E = grp.E;
+    fe *polys = grp.polys.as<fe>(), *combined = grp.combined.as<fe>();
+    grp.comp.alloc((size_t)K * E * 16);
+    grp.comp_ext.alloc((size_t)K * grp.N_loc * 16);
+    TwiddleRef g_t = c.twiddle(grp.log_n, false);
+    // trace polynomials at z and z*g: every rank evaluates its own columns (the split of stage 1); slots of 2 cpr values are gathered.
+    // d_deep = 2 trace values per column (one GPU: proof p's from column col0[p] on; several: G slots of cpr columns), then [K][2]
+    // values of the constraint polynomial at z
+    const size_t deep_cols = G == 1 ? grp.W : (size_t)cpr * G;
+    DevBuf d_deep((2 * deep_cols + 2 * K) * 16);
+    fe *deep_c = d_deep.as<fe>() + 2 * deep_cols;
+    DG_CUDA(cudaMemsetAsync(d_deep.p, 0, d_deep.bytes, c.stream));
+    // powers of z, 1/z, z g, 1/(z g) of every proof: four batched tables from one upload of the (base, step) pairs, [table][proof][2]
+    std::vector<fe> base_step((size_t)8 * K, fe_make(0, 0));
+    for (int p : grp.order) {
+        ProofState &s = ps[p];
+        if (!s.live) continue;
+        s.dc = fs::draw_composition_coefficients(s.stark.constraint_root.data(), grp.shapes[p].w);
+        PowTables::pack_point(&base_step[(size_t)2 * p], (size_t)2 * K, s.dc.z, E + 1);
+        PowTables::pack_point(&base_step[(size_t)2 * (2 * K + p)], (size_t)2 * K, fe_mul(s.dc.z, grp.root_n), n + 1);
+    }
+    DevBuf d_base_step(base_step.size() * 16);
+    h2d(c, d_base_step.p, base_step.data(), base_step.size() * 16);
+    const fe *bs = d_base_step.as<fe>();
+    PowTables z_t(c, bs, K, E + 1), zi_t(c, bs + 2 * K, K, E + 1), zg_t(c, bs + 4 * K, K, n + 1), zgi_t(c, bs + 6 * K, K, n + 1);
+    if (G == 1) {
+        eval_polys_at(c, polys, n, (int)grp.W, z_t.ref(0), g_t, true, d_deep.as<fe>(), 1 << 30, z_t.lo_n, z_t.hi_n, grp.d_col_proof);
+    } else {
+        const int j0 = grp.col_start(grp.g), mine = grp.col_count(grp.g);
+        if (mine > 0) eval_polys_at(c, polys + (size_t)j0 * n, n, mine, z_t.ref(0), g_t, true, d_deep.as<fe>() + (size_t)2 * grp.g * cpr);
+        comm_all_gather(c, d_deep.as<fe>() + (size_t)2 * grp.g * cpr, d_deep.p, (size_t)2 * cpr * 16);
+    }
+    eval_polys_at(c, combined, E, K, z_t.ref(0), g_t, false, deep_c, 1, z_t.lo_n, z_t.hi_n);
+    std::vector<fe> deep_slots(2 * deep_cols + 2 * K);
+    d2h(c, deep_slots.data(), d_deep.p, deep_slots.size() * 16);
+    substage(c, "6.deep_values");
+    // one upload: [K][2 wmax] coefficients of the trace combinations (proof p's trace1 | trace2 at p 2 wmax, p 2 wmax + wmax) | sub0
+    // of the three divisions [3][K] | compose's k1, k2, kc [K][3]
+    std::vector<fe> pack((size_t)K * (2 * wmax + 6), fe_make(0, 0));
+    fe *ccs = pack.data(), *subs = ccs + (size_t)K * 2 * wmax, *ks = subs + (size_t)3 * K;
+    for (int p = 0; p < K; p++) {
+        ProofState &s = ps[p];
+        if (!s.live) continue;
+        const int wq = grp.shapes[p].w;
+        const fe *slots = deep_slots.data() + 2 * (size_t)grp.col0[p];           // several GPUs: K == 1, col0[0] == 0
+        std::vector<fe> deep(2 * wq);
+        for (int r = 0; r < G; r++)
+            for (int o = 0; o < (G == 1 ? wq : grp.col_count(r)); o++) {
+                const int from = G == 1 ? o : r * cpr + o, to = G == 1 ? o : grp.col_start(r) + o;
+                deep[2 * to] = slots[2 * from];
+                deep[2 * to + 1] = slots[2 * from + 1];
+            }
+        std::vector<fe> &z1 = s.stark.trace_at_z1, &z2 = s.stark.trace_at_z2;
+        z1.resize(wq); z2.resize(wq);
+        fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
+        for (int i = 0; i < wq; i++) {
+            z1[i] = deep[2 * i]; z2[i] = deep[2 * i + 1];
+            sub1 = fe_add(sub1, fe_mul(z1[i], s.dc.trace1[i]));
+            sub2 = fe_add(sub2, fe_mul(z2[i], s.dc.trace2[i]));
+        }
+        subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[2 * deep_cols + 2 * p];
+        std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + wq, ccs + (size_t)p * 2 * wmax);
+        std::copy(s.dc.trace2.begin(), s.dc.trace2.begin() + wq, ccs + (size_t)p * 2 * wmax + wmax);
+        ks[3 * p] = s.dc.t1_degree; ks[3 * p + 1] = s.dc.t2_degree; ks[3 * p + 2] = s.dc.constraints;
+    }
+    DevBuf d_pack(pack.size() * 16), t12((size_t)K * 2 * n * 16);
+    h2d(c, d_pack.p, pack.data(), pack.size() * 16);
+    const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * wmax, *d_ks = d_subs + (size_t)3 * K;
+    fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
+    fe *scratch2 = grp.scratch2.as<fe>();
+    lincomb2(c, polys, n, wmax, d_cc, d_cc + wmax, t1, t2, K, 2 * wmax, 2 * n, grp.d_cols);
+    syn_div(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs);
+    //                                                                                                   (T1(x) - T1(z)) / (x - z)
+    syn_div(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K);
+    //                                                                                                   (T2(x) - T2(zg)) / (x - zg)
+    syn_div(c, K, combined, E, scratch2, E, E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs + 2 * K);
+    //                                                                                                   (C(x) - C(z)) / (x - z)
+    substage(c, "6.lincomb+syndiv");
+    compose(c, K, t1, t2, 2 * n, scratch2, grp.comp.as<fe>(), n, E, 6 * n + 1, d_ks);
+    if (K == 1) debug_dump(c, "composition_poly", grp.comp.p, E * 16);
+    // every rank extends its own cosets; the first FRI layers work on these slabs directly (no all-gather of the N evaluations)
+    lde_batch(c, grp.comp.as<fe>(), grp.comp_ext.as<fe>(), grp.log_n, grp.log_b, 8, K, E, grp.N_loc, grp.c0, (unsigned)grp.nc);
+}
+
+// ---- 7: FRI layers -------------------------------------------------------------------------------------------------------------------------
+// The layer roots and folding points of a group stay on the device, [layer][proof] (special_x = prng(root) is derived by fri_alpha): the
+// host sees the roots in one copy after the last layer.  With host RNG callbacks registered each layer asks the host instead: one copy
+// of the layer's K roots, the callbacks of the live proofs in proof order, one upload of the K folding points.
+struct FriRun {
+    static const int MAX_LAYERS = 20;
+    Context &c;
+    const std::vector<ProofState> &ps;
+    const std::vector<int> &order;
+    const int K;
+    DevBuf d_alpha, d_roots;
+    const bool host_rng = fs::rng_hooks_active();
+    FriRun(Context &c_, const Group &grp, const std::vector<ProofState> &ps_)
+        : c(c_), ps(ps_), order(grp.order), K(grp.K), d_alpha((size_t)MAX_LAYERS * K * 16), d_roots((size_t)MAX_LAYERS * K * 32) {}
+    fe *alpha(size_t layer) { return d_alpha.as<fe>() + layer * K; }
+    uint8_t *root_slots(size_t layer) { return (uint8_t *)d_roots.p + 32 * layer * K; }
+    // the K roots of layer `li`, root_stride bytes apart from root0, into their slots
+    void copy_roots(const void *root0, size_t root_stride, size_t li) {
+        DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
+        DG_CUDA(cudaMemcpy2DAsync(root_slots(li), 32, root0, std::max<size_t>(root_stride, 32), 32, K, cudaMemcpyDeviceToDevice, c.stream));
+    }
+    void folding_points(const void *root0, size_t root_stride, size_t li) {
+        DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
+        if (!host_rng) { fri_alpha(c, root0, alpha(li), root_slots(li), K, root_stride); return; }
+        copy_roots(root0, root_stride, li);
+        std::vector<uint8_t> r((size_t)32 * K);
+        d2h(c, r.data(), root_slots(li), r.size());
+        std::vector<fe> alphas(K, fe_make(0, 0));
+        for (int p : order)
+            if (ps[p].live) alphas[p] = fs::prng_vector(r.data() + 32 * p, 1)[0];   // field::prng(seed) = first draw of the generator (field.rs:264-269)
+        DG_CUDA(cudaMemcpyAsync(alpha(li), alphas.data(), (size_t)16 * K, cudaMemcpyHostToDevice, c.stream));
+        DG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+};
+
+void fri_layers(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K, log_b = grp.log_b, log_N = grp.log_N;
+    TwiddleRef inv_root = c.twiddle(log_N, true);
+    const FoldConstants fold = fri_fold_constants();
+    // the K proofs' layers are one buffer each: layer d of proof p = cur + p * cur_stride
+    const fe *cur = grp.comp_ext.as<fe>();
+    uint64_t cur_stride = grp.N_loc;
+    Layout lay{log_N, log_b};
+    bool local = grp.G > 1;                                // `cur` is this rank's coset slab of the layer (K == 1)
+    FriRun run(c, grp, ps);
+    size_t n_layers = 0;
+    for (;;) {
+        const int log_r = lay.log_d - 2;
+        const uint64_t R = 1ULL << log_r;
+        // layers below 2^22 values are latency-bound (two collectives per sharded tree cost more than hashing them whole): gather the
+        // first such layer once (<= 32 MB) and finish redundantly on every rank
+        if (local && (lay.log_d < 22 || log_r - log_b < 6)) {
+            grp.fri_gathered.alloc((size_t)16 << lay.log_d);
+            comm_all_gather(c, cur, grp.fri_gathered.p, ((size_t)16 << lay.log_d) >> grp.log_g);     // rank-major == coset-major
+            cur = grp.fri_gathered.as<fe>();
+            local = false;
+        }
+        const size_t li = n_layers++;
+        if (local) {
+            FriLayerDev &L = ps[0].layers.emplace_back();
+            L.vals = cur; L.layout = lay; L.sharded = true;
+            // rows r = b k' + c of the own cosets: hashes in ShardedTree order, n' = R / b subtrees of nc leaves per rank
+            L.leaves.alloc((R >> grp.log_g) * 32);
+            fri_hash_rows_local(c, cur, lay.log_d, log_b, grp.log_nc, L.leaves.p);
+            L.tree.build(c, L.leaves.p, R >> log_b, grp.log_nc, false);
+            run.folding_points(L.tree.root_dev(), 0, li);
+            L.folded.alloc((R >> grp.log_g) * 16);
+            fri_fold_local(c, cur, lay.log_d, log_b, grp.log_nc, grp.c0, L.folded.as<fe>(), run.alpha(li), inv_root, log_N, fold.tau_inv, fold.inv4);
+            cur = L.folded.as<fe>();
+            lay = Layout{log_r, log_b};
+            continue;
+        }
+        const Layout rows = fri_next_layout(lay);
+        grp.layer_bufs.emplace_back((size_t)K * R * 32);
+        const uint8_t *leaves = grp.layer_bufs.back().as<uint8_t>();
+        grp.layer_bufs.emplace_back((size_t)K * R * 32);
+        const uint8_t *nodes = grp.layer_bufs.back().as<uint8_t>();
+        fri_hash_rows(c, cur, lay, rows, (void *)leaves, K, cur_stride);
+        merkle_build(c, leaves, (void *)nodes, R, K);
+        for (int p = 0; p < K; p++) {
+            if (!ps[p].live) continue;
+            FriLayerDev &L = ps[p].layers.emplace_back();
+            L.vals = cur + (size_t)p * cur_stride; L.layout = lay; L.sharded = false;
+            L.leaves_p = leaves + (size_t)p * R * 32; L.nodes_p = nodes + (size_t)p * R * 32;
+        }
+        if (R * 4 <= 256) {                                    // MAX_REMAINDER_LENGTH (fri/mod.rs:13): the remainder's root only
+            run.copy_roots(nodes + 32, R * 32, li);
+            break;
+        }
+        run.folding_points(nodes + 32, R * 32, li);            // special_x = prng(root)  (fri/prover.rs:29)
+        grp.layer_bufs.emplace_back((size_t)K * R * 16);       // values of the next layer
+        fe *folded = grp.layer_bufs.back().as<fe>();
+        fri_fold(c, cur, lay, folded, rows, run.alpha(li), inv_root, log_N, fold.tau_inv, fold.inv4, K, cur_stride);
+        cur = folded;
+        cur_stride = R;
+        lay = rows;
+    }
+    std::vector<uint8_t> roots(32 * n_layers * K);
+    d2h(c, roots.data(), run.d_roots.p, roots.size());
+    // the last layer is the remainder: its root is the FRI proof's rem_root
+    for (int p = 0; p < K; p++) {
+        if (!ps[p].live) continue;
+        FriProof &f = ps[p].stark.degree_proof;
+        auto root = [&](size_t i) { return roots.data() + 32 * (i * K + p); };
+        f.layers.resize(n_layers - 1);
+        for (size_t i = 0; i + 1 < n_layers; i++) memcpy(f.layers[i].root.data(), root(i), 32);
+        memcpy(f.rem_root.data(), root(n_layers - 1), 32);
+    }
+}
+
+// ---- 8: query positions --------------------------------------------------------------------------------------------------------------------
+void query_positions(Context &c, const Group &grp, std::vector<ProofState> &ps) {
+    std::vector<std::array<uint8_t, 32>> seeds;
+    std::vector<unsigned> grinding;
+    std::vector<int> who;
+    for (int p : grp.order) {
+        if (!ps[p].live) continue;
+        const FriProof &f = ps[p].stark.degree_proof;
+        std::vector<uint8_t> roots;
+        for (auto &l : f.layers) roots.insert(roots.end(), l.root.begin(), l.root.end());
+        roots.insert(roots.end(), f.rem_root.begin(), f.rem_root.end());
+        if (grp.K == 1) debug_dump_host("fri_roots", roots.data(), roots.size());
+        seeds.emplace_back();
+        fs::blake3_short(roots.data(), roots.size(), seeds.back().data());
+        grinding.push_back(ps[p].stark.options.grinding_factor);
+        who.push_back(p);
+    }
+    std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, grinding);
+    for (size_t i = 0; i < who.size(); i++) {
+        ProofState &s = ps[who[i]];
+        s.stark.pow_nonce = nonces[i];
+        pow_hash(seeds[i].data(), s.stark.pow_nonce, s.proof->pow_seed);
+        try {
+            s.positions = fs::query_positions(s.proof->pow_seed, grp.N, grp.b, s.stark.options.num_queries);
+        } catch (const std::exception &e) { s.fail(DG_ERR_EXHAUSTED, e.what()); continue; }
+        if (grp.K == 1) debug_dump_host("positions", s.positions.data(), s.positions.size() * 8);
+    }
+}
+
+// ---- 9: build proof objects ----------------------------------------------------------------------------------------------------------------
+// Every opening of every proof is planned on the host, all opened values / digests are fetched in one batched pass (FetchBatch), then
+// each proof is written.
+
+// registers the nodes of a batch-proof plan; leaf_ref / node_ref map leaf indices / heap indices to fetch references
+template <class LeafRef, class NodeRef>
+Offsets plan_offsets(FetchBatch &fb, const fs::BatchPlan &plan, LeafRef leaf_ref, NodeRef node_ref) {
+    Offsets o(plan.nodes.size());
+    for (size_t sidx = 0; sidx < plan.nodes.size(); sidx++)
+        for (auto &r : plan.nodes[sidx]) o[sidx].push_back(fb.add32(r.leaf ? leaf_ref(r.index) : node_ref(r.index)));
+    return o;
+}
+
+std::vector<std::vector<Digest>> digests_at(const FetchBatch &fb, const Offsets &o) {
+    std::vector<std::vector<Digest>> v(o.size());
+    for (size_t i = 0; i < o.size(); i++)
+        for (size_t off : o[i]) v[i].push_back(fb.digest(off));
+    return v;
+}
+
+// what proof p opens; its trace rows outside the retained cosets are in grp.d_rows from value row0 on
+OpenPlan plan_openings(const Group &grp, FetchBatch &fb, ProofState &s, int p, size_t row0) {
+    const uint64_t n = grp.n, b = grp.b, N = grp.N, nc = grp.nc;
+    const int log_n = grp.log_n, log_b = grp.log_b, log_nc = grp.log_nc, w = grp.shapes[p].w;
+    const fe *slab_p = grp.slab_of(p), *c_ext_p = grp.c_ext_of(p);
+    OpenPlan O;
+    const std::vector<uint64_t> &positions = s.positions;
+    const int nq = (int)positions.size();
+    // trace rows at the queried positions (trace_table.rs:127-134): the rank owning the position's coset reads the row from the retained
+    // slab, or it was computed into d_rows
+    O.row_off.resize(nq);
+    for (int q = 0; q < nq; q++) {
+        const uint64_t cpos = positions[q] & (b - 1), k = positions[q] >> log_b;
+        if (!grp.retained(positions[q])) {
+            O.row_off[q] = fb.add16(FetchRef{grp.d_rows.p, row0, -1});
+            for (int j = 1; j < w; j++) fb.add16(FetchRef{grp.d_rows.p, row0 + j, -1});
+            row0 += w;
+            continue;
+        }
+        const int owner = (int)(cpos >> log_nc);
+        const uint64_t phys = (((cpos - (uint64_t)owner * nc) / grp.rstep) << log_n) + k;
+        for (int j = 0; j < w; j++) {
+            const size_t off = fb.add16(FetchRef{slab_p + (size_t)j * grp.slab_col, phys, owner});
+            if (j == 0) O.row_off[q] = off;
+        }
+    }
+    // trace tree openings: leaves are the row hashes
+    O.tplan = fs::plan_batch_proof(positions, N);
+    O.t_off = plan_offsets(fb, O.tplan, [&](uint64_t i) { return s.t_tree.item_ref(i); }, [&](uint64_t h) { return s.t_tree.node_ref(h); });
+
+    // constraint tree openings: leaf j = evaluations (2j, 2j+1), unhashed (prover.rs:180-187); evaluation 2j+1 lives in the next
+    // coset at the same k, i.e. n elements further in the owner's slab: two 16-byte units registered back to back = one 32-byte item
+    auto constraint_leaf = [&](uint64_t j) {
+        const uint64_t i = 2 * j, cpos = i & (b - 1), k = i >> log_b;
+        const int owner = (int)(cpos >> log_nc);
+        const uint64_t p0 = ((cpos - (uint64_t)owner * nc) << log_n) + k;
+        const size_t off = fb.add16(FetchRef{c_ext_p, p0, owner});
+        fb.add16(FetchRef{c_ext_p, p0 + n, owner});
+        return off;
+    };
+    std::vector<uint64_t> c_positions = fs::constraint_positions(positions);
+    O.cplan = fs::plan_batch_proof(c_positions, N / 2);
+    for (uint64_t j : O.cplan.value_leaves) O.cval_off.push_back(constraint_leaf(j));
+    O.c_off.resize(O.cplan.nodes.size());
+    for (size_t sidx = 0; sidx < O.cplan.nodes.size(); sidx++)
+        for (auto &r : O.cplan.nodes[sidx]) {
+            // heap indices of the tree over N/2 leaves: [N/4, N/2) is the first hashed level (= level-0 items of c_tree)
+            if (r.leaf) O.c_off[sidx].push_back(constraint_leaf(r.index));
+            else if (r.index >= N / 4) O.c_off[sidx].push_back(fb.add32(s.c_tree.item_ref(r.index - N / 4)));
+            else O.c_off[sidx].push_back(fb.add32(s.c_tree.node_ref(r.index)));
+        }
+
+    // FRI layers (fri/prover.rs:55-95)
+    O.fri_open.resize(s.layers.size() - 1);
+    std::vector<uint64_t> fpos = positions;
+    for (size_t d = 0; d + 1 < s.layers.size(); d++) {
+        FriLayerDev &L = s.layers[d];
+        LayerOpen &lo = O.fri_open[d];
+        const uint64_t D = 1ULL << L.layout.log_d, R = D / 4;
+        fpos = fs::augmented_positions(fpos, D);
+        fs::BatchPlan plan = fs::plan_batch_proof(fpos, R);
+        lo.depth = plan.depth;
+        for (uint64_t p : fpos)
+            for (int j = 0; j < 4; j++) {
+                size_t off;
+                if (L.sharded) {
+                    const uint64_t cpos = p & (b - 1), k = (p >> log_b) + (uint64_t)j * (R >> log_b);
+                    const int owner = (int)(cpos >> log_nc);
+                    off = fb.add16(FetchRef{L.vals, ((cpos - (uint64_t)owner * nc) << (L.layout.log_d - log_b)) + k, owner});
+                } else {
+                    off = fb.add16(FetchRef{L.vals, L.layout.phys(p + j * R), -1});
+                }
+                if (j == 0) lo.val_off.push_back(off);
+            }
+        if (L.sharded) lo.node_off = plan_offsets(fb, plan, [&](uint64_t i) { return L.tree.item_ref(i); }, [&](uint64_t h) { return L.tree.node_ref(h); });
+        else lo.node_off = plan_offsets(fb, plan, [&](uint64_t i) { return FetchRef{L.leaves_p, i, -1}; }, [&](uint64_t h) { return FetchRef{L.nodes_p, h, -1}; });
+    }
+    {
+        FriLayerDev &L = s.layers.back();
+        const uint64_t D = 1ULL << L.layout.log_d;
+        for (uint64_t i = 0; i < D; i++) O.rem_off.push_back(fb.add16(FetchRef{L.vals, L.layout.phys(i), -1}));   // remainder, natural order
+    }
+    return O;
+}
+
+// the opened values and digests into the proof, which is then written out
+void fill_openings(const FetchBatch &fb, ProofState &s, const OpenPlan &O, int w) {
+    StarkProof &P = s.stark;
+    P.trace_info.domain_depth = O.tplan.depth;
+    P.trace_nodes = digests_at(fb, O.t_off);
+    P.trace_evaluations.assign(O.row_off.size(), std::vector<fe>(w));
+    for (size_t q = 0; q < O.row_off.size(); q++)
+        for (int j = 0; j < w; j++) P.trace_evaluations[q][j] = fb.value(O.row_off[q] + j);
+    for (size_t off : O.cval_off) P.constraint_proof.values.push_back(fb.digest(off));
+    P.constraint_proof.nodes = digests_at(fb, O.c_off);
+    P.constraint_proof.depth = O.cplan.depth;
+    for (size_t d = 0; d < O.fri_open.size(); d++) {
+        const LayerOpen &lo = O.fri_open[d];
+        FriLayer &l = P.degree_proof.layers[d];
+        for (size_t off : lo.val_off) l.values.push_back({fb.value(off), fb.value(off + 1), fb.value(off + 2), fb.value(off + 3)});
+        l.nodes = digests_at(fb, lo.node_off);
+        l.depth = lo.depth;
+    }
+    for (size_t off : O.rem_off) P.degree_proof.rem_values.push_back(fb.value(off));
+    Proof &h = *s.proof;
+    h.bytes = write_proof(P);
+    memcpy(h.trace_root, P.trace_root.data(), 32);
+    memcpy(h.constraint_root, P.constraint_root.data(), 32);
+    h.pow_nonce = P.pow_nonce;
+}
+
+void build_proofs(Context &c, Group &grp, std::vector<ProofState> &ps) {
+    const int K = grp.K;
+    FetchBatch fb(c);
+    // opened trace rows outside the retained cosets (evaluation-coset layout): the trace polynomials at w_N^pos, all proofs in one launch,
+    // into d_rows (the w_p values of each computed row of the batch, rows in proof and query order)
+    std::vector<size_t> first_row(K, 0);                       // proof p's first value in d_rows
+    std::vector<TraceRow> points;
+    size_t values = 0;
+    for (int p = 0; p < K; p++) {
+        first_row[p] = values;
+        if (ps[p].live)
+            for (uint64_t pos : ps[p].positions)
+                if (!grp.retained(pos)) {
+                    points.push_back(TraceRow{pos, 0, grp.col0[p], (unsigned)grp.shapes[p].w});
+                    values += grp.shapes[p].w;
+                }
+    }
+    if (!points.empty()) {
+        grp.d_rows.alloc(values * 16);
+        eval_trace_rows(c, grp.polys.as<fe>(), grp.n, points, grp.log_N, grp.d_rows.as<fe>());
+    }
+    std::vector<OpenPlan> plans(K);
+    for (int p = 0; p < K; p++)
+        if (ps[p].live) plans[p] = plan_openings(grp, fb, ps[p], p, first_row[p]);
+    fb.run();
+    for (int p = 0; p < K; p++)
+        if (ps[p].live) fill_openings(fb, ps[p], plans[p], grp.shapes[p].w);
+}
 
 }  // namespace
 
@@ -277,46 +1081,10 @@ struct OpenPlan {
 // column chunks are uploaded on the copy stream while the previous chunk is being interpolated and extended (the upload hides behind the
 // LDE).  chunk (one GPU): cosets of the trace extension held at a time (ProvePlan).  The full layout (chunk = b) keeps the whole extension;
 // the evaluation-coset layout (chunk < b) extends and hashes chunk cosets at a time and keeps only the 8 cosets stage 3 reads.
+// The stages are the reference's nine debug!() sections, one function each, in order.
 static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, const std::vector<RegisterShape> &regs_shape, uint64_t length,
                        const std::vector<int> &order, std::vector<ProofState> &ps, const std::vector<dg_options_t> &opts,
                        dg_prove_stats_t *stats, unsigned chunk) {
-    // ---- argument checks (trace_table.rs:23-58, options.rs:29-50, lib.rs:33-34) -----------------------------------------------
-    const int K = (int)ps.size();
-    DG_REQUIRE(K >= 1 && regs_shape.size() == ps.size() && order.size() == ps.size() && opts.size() == ps.size(), "batch must hold at least one trace");
-    const uint64_t n = length, b = opts[0].extension_factor;
-    size_t W = 0;                                              // columns of the whole batch
-    for (const RegisterShape &r : regs_shape) W += r.width;
-    DG_REQUIRE(W <= 65535, "batch too large for one launch (batched calls split larger batches into groups)");
-    for (const dg_options_t &o : opts) {
-        check_options(o);
-        DG_REQUIRE(o.extension_factor == b, "the proofs of a group share one extension factor");
-    }
-    DG_REQUIRE(n >= 16 && (n & (n - 1)) == 0, "execution trace length must be a power of 2 and at least 16");
-    std::vector<TraceShape> shapes;
-    for (const RegisterShape &r : regs_shape) shapes.push_back(TraceShape::of_trace(r.width, r.ctx_depth, r.loop_depth));
-    // the column table: proof p's registers are the columns [col0[p], col0[p] + w_p) of the batch
-    std::vector<uint32_t> col0(K + 1, 0);
-    int wmax = 0, Tmax = 0;
-    for (int p = 0; p < K; p++) {
-        col0[p + 1] = col0[p] + shapes[p].w;
-        wmax = std::max(wmax, shapes[p].w);
-        Tmax = std::max(Tmax, shapes[p].T);
-    }
-    const int log_n = ceil_log2(n), log_b = ceil_log2(b), log_N = log_n + log_b;
-    DG_REQUIRE(log_N <= 30, "LDE domain too large");
-    const uint64_t N = n * b, E = n * 8;
-    for (int p = 0; p < K; p++) {             // what the call fixes in every proof: the register shape and its options (blake3)
-        TraceInfo &t = ps[p].stark.trace_info;
-        t.ctx_depth = (uint8_t)shapes[p].ctx_depth; t.loop_depth = (uint8_t)shapes[p].loop_depth; t.stack_depth = (uint8_t)shapes[p].stack_depth;
-        ps[p].stark.options = ProofOptions{(uint8_t)log_b, (uint8_t)opts[p].num_queries, (uint8_t)opts[p].grinding_factor, 0};
-    }
-    // runs of proofs of one shape: [shape_first[s], shape_first[s + 1])
-    std::vector<int> shape_first = {0};
-    for (int p = 1; p < K; p++)
-        if (!(regs_shape[p] == regs_shape[p - 1])) shape_first.push_back(p);
-    shape_first.push_back(K);
-    auto any_live = [&] { for (auto &s : ps) if (s.live) return true; return false; };
-
     ArenaScope arena_scope;                   // all DevBufs below come from the per-proof arena (no driver allocation inside a proof)
     StageClock clk(c.stream);
     SubClock sub(c.stream);
@@ -328,683 +1096,37 @@ static void prove_core(Context &c, fe *d_regs, const uint8_t *const *host_cols, 
         ~DeviceStateReset() { for (auto &s : ps) { s.t_tree = ShardedTree(); s.c_tree = ShardedTree(); s.layers.clear(); } }
     } state_reset{ps};
     const unsigned long long launches0 = c.launches;
-    // the column table on the device: [K] (first column, width) of every proof, then [W] the proof of every column
-    DevBuf d_table((2 * K + W) * 4);
-    {
-        std::vector<uint32_t> table(2 * K + W);
-        for (int p = 0; p < K; p++) {
-            table[2 * p] = col0[p];
-            table[2 * p + 1] = (uint32_t)shapes[p].w;
-            for (uint32_t j = col0[p]; j < col0[p + 1]; j++) table[2 * K + j] = (uint32_t)p;
-        }
-        h2d(c, d_table.p, table.data(), table.size() * 4);
-    }
-    const uint2 *d_cols = d_table.as<uint2>();
-    const unsigned *d_col_proof = d_table.as<unsigned>() + 2 * K;
+    Group grp(c, d_regs, host_cols, regs_shape, length, order, ps, opts, chunk);
 
-    // ---- sharding: rank g owns the LDE cosets [c0, c0 + nc) of every column (world == 1: all of them) ------------------------------
-    const int G = c.world, g = c.rank;
-    DG_REQUIRE(G == 1 || K == 1, "a batch of proofs runs on one GPU (the context spans several)");
-    const int log_g = ceil_log2(G);
-    DG_REQUIRE((b >> log_g) >= 4 && G <= 8, "extension factor too small for this many GPUs (need >= 4 cosets per rank)");
-    const int log_nc = log_b - log_g;
-    const uint64_t nc = 1ULL << log_nc, N_loc = n * nc;
-    const unsigned c0 = (unsigned)(g * nc);
-    const int w = shapes[0].w;                                 // several GPUs: the width of the one proof
-
-    // ---- 1: extend execution trace ---------------------------------------------------------------------------------------------------
     clk.mark(0);
     sub.mark("start");
-    // G > 1: the interpolation is sharded by columns -- rank r interpolates the columns [col_start(r), col_start(r) + col_count(r)), an
-    // even split (the first w mod G ranks own one more), and only needs (from a host trace: only uploads) those registers -- the
-    // polynomials are all-gathered (equal slots of cpr columns per rank, then compacted into natural column order) and every rank
-    // extends all columns on its cosets
-    const int cpr = (w + G - 1) / G;                           // slot size of the gather = largest share
-    auto col_count = [&](int r) { return w / G + (r < w % G ? 1 : 0); };
-    auto col_start = [&](int r) { return r * (w / G) + std::min(r, w % G); };
-    // Layout of the extension.  ext holds `chunk` cosets of every column at a time ([W][chunk][n]).  The retained slab holds the cosets
-    // stage 3 reads: in the full layout the whole extension (slab = ext), in the evaluation-coset layout the 8 cosets c = 0 (mod b / 8),
-    // [W][8][n].  An opened row outside the retained cosets is computed from the trace polynomials in stage 9.
-    if (G > 1 || chunk == 0 || chunk > nc) chunk = (unsigned)nc;
-    DG_REQUIRE((chunk & (chunk - 1)) == 0, "coset chunk must be a power of 2");
-    const bool full = chunk == nc;
-    const int log_ret = full ? log_nc : 3;                     // retained cosets: all of this rank's, or the 8 evaluation cosets
-    const uint64_t slab_col = n << log_ret, rstep = nc >> log_ret;      // slab column stride; retained cosets are c = 0 (mod rstep)
-    const uint64_t ext_col = n * chunk;                        // column stride of ext (N_loc in the full layout)
-    DevBuf polys(W * n * 16), ext(W * ext_col * 16), slab_own;
-    if (!full) slab_own.alloc(W * slab_col * 16);
-    const fe *slab = full ? ext.as<fe>() : slab_own.as<fe>();
-    DevBuf t_leaves((size_t)K * N_loc * 32), t_nodes;
-    // rows of the chunk at cc: leaves (k << log_b) + c of every proof; then its retained cosets into the slab
-    auto hash_chunk = [&](unsigned cc) {
-        hash_trace_rows(c, ext.as<fe>(), t_leaves.p, w, log_n, log_nc, K, 0, cc, chunk, N_loc, d_cols);   // local rows, [k][c - c0], per proof
-        if (full) return;
-        for (unsigned cs = cc; cs < cc + chunk; cs++)
-            if (cs % rstep == 0)
-                DG_CUDA(cudaMemcpy2DAsync(slab_own.as<fe>() + (cs / rstep) * n, slab_col * 16, ext.as<fe>() + (size_t)(cs - cc) * n, ext_col * 16, n * 16, W,
-                                          cudaMemcpyDeviceToDevice, c.stream));
-    };
-    if (G == 1) {
-        // the K proofs' registers are the W columns of one batch, interpolated in column chunks: a host trace is uploaded in chunks of
-        // ~64 MB, but a short ramp first (1, 2 columns), so that the first transform starts after one column's worth of copying; every
-        // column chunk is extended on the first coset chunk as soon as it has been interpolated
-        std::vector<int> bounds = {0};
-        std::unique_ptr<TraceUploader> up;
-        if (host_cols) {
-            const int step_max = (int)std::max<uint64_t>(1, std::min<uint64_t>(W, ((uint64_t)1 << 26) / (n * 16)));
-            for (int step = 1; bounds.back() < (int)W; step = std::min(step_max, step * 2)) bounds.push_back(std::min((int)W, bounds.back() + step));
-            up.reset(new TraceUploader(c, d_regs, host_cols, (int)W, n, bounds));
-        } else {
-            bounds.push_back((int)W);
-        }
-        for (unsigned cc = 0; cc < nc; cc += chunk) {
-            if (cc > 0) hash_chunk(cc - chunk);                // the last chunk is hashed in stage 2
-            for (size_t i = 0; i + 1 < bounds.size(); i++) {
-                const int j0 = bounds[i], cols = bounds[i + 1] - j0;
-                if (cc == 0) {
-                    if (up) up->wait_chunk((int)i);
-                    ntt_batch(c, d_regs + (size_t)j0 * n, polys.as<fe>() + (size_t)j0 * n, log_n, cols, n, n, true);
-                }
-                extend_trace_columns(c, polys.as<fe>() + (size_t)j0 * n, d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * ext_col, cols, log_n, log_b,
-                                     ext_col, cc, chunk);
-            }
-        }
-    } else {
-        const int j0 = col_start(g), mine = col_count(g);
-        DevBuf own((size_t)cpr * n * 16), slots((size_t)cpr * G * n * 16);
-        if (mine > 0) {
-            if (host_cols) {
-                std::vector<int> bounds(mine + 1);
-                for (int i = 0; i <= mine; i++) bounds[i] = i;
-                TraceUploader up(c, d_regs + (size_t)j0 * n, host_cols + j0, mine, n, bounds);      // one column per chunk: all staging workers busy
-                for (int i = 0; i < up.chunks(); i++) {              // interpolate every column as soon as it has landed
-                    up.wait_chunk(i);
-                    ntt_batch(c, d_regs + (size_t)(j0 + i) * n, own.as<fe>() + (size_t)i * n, log_n, 1, n, n, true);
-                }
-            } else {
-                ntt_batch(c, d_regs + (size_t)j0 * n, own.as<fe>(), log_n, mine, n, n, true);
-            }
-        }
-    sub.mark("1.intt");
-        // the all-gather of the polynomials (and their compaction into column order) runs on the communication stream while this rank
-        // already extends its own columns
-        cudaEvent_t ev_own, ev_all;
-        DG_CUDA(cudaEventCreateWithFlags(&ev_own, cudaEventDisableTiming));
-        DG_CUDA(cudaEventCreateWithFlags(&ev_all, cudaEventDisableTiming));
-        DG_CUDA(cudaEventRecord(ev_own, c.stream));
-        DG_CUDA(cudaStreamWaitEvent(c.comm_stream, ev_own, 0));
-        comm_all_gather(c, own.p, slots.p, (size_t)cpr * n * 16, c.comm_stream);
-        for (int r = 0; r < G; r++)
-            if (col_count(r) > 0)
-                DG_CUDA(cudaMemcpyAsync(polys.as<fe>() + (size_t)col_start(r) * n, slots.as<fe>() + (size_t)r * cpr * n, (size_t)col_count(r) * n * 16,
-                                        cudaMemcpyDeviceToDevice, c.comm_stream));
-        DG_CUDA(cudaEventRecord(ev_all, c.comm_stream));
-        if (mine > 0)
-            extend_trace_columns(c, own.as<fe>(), d_regs + (size_t)j0 * n, ext.as<fe>() + (size_t)j0 * N_loc, mine, log_n, log_b, N_loc, c0, (unsigned)nc);
-    sub.mark("1.lde_own");
-        DG_CUDA(cudaStreamWaitEvent(c.stream, ev_all, 0));
-        // the other ranks' registers are on this device only when the trace was given in device memory (a host trace uploads own columns only)
-        if (j0 > 0) extend_trace_columns(c, polys.as<fe>(), host_cols ? nullptr : d_regs, ext.as<fe>(), j0, log_n, log_b, N_loc, c0, (unsigned)nc);
-        if (j0 + mine < w)
-            extend_trace_columns(c, polys.as<fe>() + (size_t)(j0 + mine) * n, host_cols ? nullptr : d_regs + (size_t)(j0 + mine) * n,
-                                 ext.as<fe>() + (size_t)(j0 + mine) * N_loc, w - j0 - mine, log_n, log_b, N_loc, c0, (unsigned)nc);
-        cudaEventDestroy(ev_own);
-        cudaEventDestroy(ev_all);
-    }
-    auto slab_of = [&](int p) { return slab + (size_t)col0[p] * slab_col; };
-
-    // ---- 2: trace Merkle tree ----------------------------------------------------------------------------------------------------------
+    if (grp.G == 1) extend_trace(c, grp);
+    else extend_trace_sharded(c, grp);
     clk.mark(1);
     sub.mark("1.lde");
-    hash_chunk((unsigned)(nc - chunk));
-    sub.mark("2.hash_rows");
-    {
-        // one GPU: the K trees level by level in one launch per level; several GPUs (K == 1): the sharded tree
-        if (G == 1) {
-            t_nodes.alloc((size_t)K * N_loc * 32);
-            merkle_build(c, t_leaves.p, t_nodes.p, N_loc, K);
-        }
-        std::vector<const void *> roots;
-        for (int p = 0; p < K; p++) {
-            const uint8_t *leaves = (const uint8_t *)t_leaves.p + (size_t)p * N_loc * 32;
-            if (G == 1) ps[p].t_tree.attach(c, leaves, (const uint8_t *)t_nodes.p + (size_t)p * N_loc * 32, n, log_nc);
-            else ps[p].t_tree.build(c, leaves, n, log_nc, false);
-            roots.push_back(ps[p].t_tree.root_dev());
-        }
-        std::vector<Digest> r = fetch_roots(c, roots);
-        for (int p = 0; p < K; p++) ps[p].stark.trace_root = r[p];
-    }
-
-    // ---- 3: evaluate constraints --------------------------------------------------------------------------------------------------------
+    commit_trace(c, grp, ps);
     clk.mark(2);
     sub.mark("2.tree");
-    std::vector<fe> last_rows((size_t)3 * K);      // op_counter and program hash of the last trace step of every proof (evaluator.rs:73-74)
-    if (host_cols) {
-        for (int p = 0; p < K; p++)
-            for (int j = 0; j < 3; j++) memcpy(&last_rows[3 * p + j], host_cols[col0[p] + j] + (n - 1) * 16, 16);
-    } else {
-        DevBuf d_last((size_t)48 * K);
-        for (size_t s = 0; s + 1 < shape_first.size(); s++) {          // the proofs of one shape are w n elements apart
-            const int p0 = shape_first[s], k = shape_first[s + 1] - p0;
-            for (int j = 0; j < 3; j++)
-                DG_CUDA(cudaMemcpy2DAsync((uint8_t *)d_last.p + 48 * p0 + 16 * j, 48, d_regs + (size_t)(col0[p0] + j) * n + (n - 1),
-                                          (size_t)shapes[p0].w * n * 16, 16, k, cudaMemcpyDeviceToDevice, c.stream));
-        }
-        d2h(c, last_rows.data(), d_last.p, (size_t)48 * K);
-    }
-    DevBuf d_coef, d_violation((size_t)4 * K);
-    // per proof [coefA | coefB | bAi | bBi | bAf | bBf], coef_stride elements apart, then the boundary constants [K][KiA, KiB, KfA, KfB].
-    // The transition coefficients of a proof are T of its shape: coefA and coefB are padded to the batch's largest count Tmax.  The
-    // boundary vectors have one entry per register that carries a boundary constraint, which depends on the shape and on the number of
-    // public inputs / outputs: they are padded with zero coefficients to the largest count nbm (a zero coefficient adds nothing to the
-    // boundary numerators).
-    const size_t T = Tmax;
-    size_t coef_stride = 0, nbm = 0;
-    {
-        for (int p : order) {
-            ProofState &s = ps[p];
-            s.stark.trace_info.op_count = (uint32_t)last_rows[3 * p].lo;       // op_count as u32 (proof.rs:62)
-            const fe program_hash[2] = {last_rows[3 * p + 1], last_rows[3 * p + 2]};
-            s.cc = fs::draw_constraint_coefficients(s.stark.trace_root.data(), shapes[p], s.inputs, s.outputs, last_rows[3 * p], program_hash);
-            DG_REQUIRE(s.cc.bAi.size() <= (size_t)shapes[p].w, "more boundary registers than registers");
-            nbm = std::max(nbm, s.cc.bAi.size());
-        }
-        coef_stride = 2 * T + 4 * nbm;
-        std::vector<fe> pack(coef_stride * K + 4 * K, fe_make(0, 0));
-        for (int p = 0; p < K; p++) {
-            ProofState &s = ps[p];
-            auto at = pack.begin() + (size_t)p * coef_stride;
-            std::copy(s.cc.coefA.begin(), s.cc.coefA.end(), at);
-            std::copy(s.cc.coefB.begin(), s.cc.coefB.end(), at + T);
-            int slot = 0;
-            for (const auto *v : {&s.cc.bAi, &s.cc.bBi, &s.cc.bAf, &s.cc.bBf}) std::copy(v->begin(), v->end(), at + 2 * T + (slot++) * nbm);
-            const fe consts[4] = {s.cc.KiA, s.cc.KiB, s.cc.KfA, s.cc.KfB};
-            std::copy(consts, consts + 4, pack.begin() + coef_stride * K + 4 * p);
-        }
-        d_coef.alloc(pack.size() * 16);
-        h2d(c, d_coef.p, pack.data(), pack.size() * 16);
-        DG_CUDA(cudaStreamSynchronize(c.stream));
-    }
-    DG_CUDA(cudaMemsetAsync(d_violation.p, 0, (size_t)4 * K, c.stream));
-    // per proof: [boundary numerator, first step | boundary numerator, last step | transition combination]
-    DevBuf evals((size_t)K * 3 * E * 16);
-    {
-        const int num_c8 = 8 >> log_g;
-        const uint64_t E_loc = n * num_c8;
-        DevBuf evals_loc((size_t)K * E_loc * 16), gathered;
-        if (G > 1) gathered.alloc(E * 16);
-        // one launch per register shape, over that shape's proofs (adjacent, so at uniform strides)
-        for (size_t s = 0; s + 1 < shape_first.size(); s++) {
-            const int p0 = shape_first[s], k = shape_first[s + 1] - p0;
-            AirParams P = shapes[p0].air_params(n);
-            // the retained slab: all cosets (log_blowup = log_b, powers of w_N), or the 8 evaluation cosets as an extension by 8 (powers of
-            // w_8n = w_N^(b/8): lde_index * inc selects the same power of the root)
-            P.log_blowup = full ? log_b : 3;
-            P.ext = slab_of(p0); P.col_stride = slab_col;
-            P.c8_base = g * num_c8; P.num_c8 = num_c8;
-            P.t_ev = evals_loc.as<fe>() + (size_t)p0 * E_loc;
-            P.periodic = periodic_table(c);
-            const fe *base = d_coef.as<fe>() + (size_t)p0 * coef_stride;
-            P.coefA = base; P.coefB = base + T;
-            P.twN = c.twiddle(full ? log_N : log_n + 3, false);
-            P.violation = d_violation.as<unsigned>() + p0;
-            P.ext_stride = (size_t)shapes[p0].w * slab_col; P.t_ev_stride = E_loc; P.coef_stride = coef_stride;
-            if (s == 0) sub.mark("3.setup");
-            launch_constraint_eval(c, P, k);
-        }
-    sub.mark("3.eval");
-        comm_all_reduce_max_u32(c, d_violation.as<unsigned>(), 1);
-        std::vector<unsigned> violation(K);
-        d2h(c, violation.data(), d_violation.p, (size_t)4 * K);
-        for (int p = 0; p < K; p++)
-            if (violation[p])
-                ps[p].fail(DG_ERR_UNSATISFIED, "transition constraints at step " + std::to_string(violation_step(violation[p])) + " were not satisfied");
-        if (!any_live()) return;
-        // interpolation of the transition combination (constraint_table.rs:54-63), coset by coset: size-n inverse transforms of the own
-        // cosets (sharded), all-gather, then the 8-point inverse DFT across cosets (poly.cu: coset_interp_finish) -> the 8n coefficients
-        // in natural order; no transposition and no replicated 8n-point transform
-    sub.mark("3.violation_sync");
-        ntt_batch(c, evals_loc.as<fe>(), evals_loc.as<fe>(), log_n, K * num_c8, n, n, true);
-        if (G > 1) comm_all_gather(c, evals_loc.as<fe>(), gathered.as<fe>(), E_loc * 16);
-    sub.mark("3.intt+gather");
-        coset_interp_finish(c, G > 1 ? gathered.as<fe>() : evals_loc.as<fe>(), evals.as<fe>() + 2 * E, log_n, K, E_loc, 3 * E);
-        // boundary constraints (evaluator.rs:181-326), directly as the 8n coefficients the reference obtains by interpolation
-        boundary_coeffs(c, K, polys.as<fe>(), 0, n, (int)nbm, d_coef.as<fe>() + 2 * T, coef_stride, d_coef.as<fe>() + coef_stride * K,
-                        evals.as<fe>(), evals.as<fe>() + E, 3 * E, d_cols);
-    }
-    if (K == 1) debug_dump(c, "t_coeffs", evals.as<fe>() + 2 * E, E * 16);
-
-    // ---- 4: convert constraint evaluations into a polynomial -----------------------------------------------------------------------------
+    if (!evaluate_constraints(c, grp, ps)) return;
     clk.mark(3);
     sub.mark("3.finish+boundary");
-    DevBuf combined((size_t)K * E * 16), scratch((size_t)K * E * 16), scratch2((size_t)K * E * 16);
-    const fe root_n = host_root_of_unity(log_n);
-    const fe x_last = host_inv(root_n);                        // w_n^(n-1)   (evaluator.rs:128-131)
-    {
-        if (K == 1) {
-            debug_dump(c, "i_coeffs", evals.as<fe>(), E * 16);
-            debug_dump(c, "f_coeffs", evals.as<fe>() + E, E * 16);
-        }
-        // one upload: the (base, step) pairs of the power tables of 1, x_last and 1 / x_last (shared by the K proofs), then K zeros (sub0)
-        std::vector<fe> pack(6 + K, fe_make(0, 0));
-        const fe bases[3] = {fe_make(1, 0), x_last, root_n};
-        for (int t = 0; t < 3; t++) { pack[2 * t] = bases[t]; pack[2 * t + 1] = PowTables::step(bases[t], E + 1); }
-        DevBuf d_pack(pack.size() * 16);
-        h2d(c, d_pack.p, pack.data(), pack.size() * 16);
-        PowTables pows(c, d_pack.as<fe>(), 3, E + 1);
-        const fe *zeros = d_pack.as<fe>() + 6;
-        fe *ic = evals.as<fe>(), *fc = evals.as<fe>() + E, *tc = evals.as<fe>() + 2 * E;          // of proof 0; proof p at + 3 E p
-        syn_div(c, K, ic, 3 * E, ic, 3 * E, E, pows.ref(0), 0, 0, pows.ref(0), 0, 0, zeros);   // / (x - 1)
-        syn_div(c, K, fc, 3 * E, fc, 3 * E, E, pows.ref(1), 0, 0, pows.ref(2), 0, 0, zeros);   // / (x - x_last)
-        syn_div_expanded_sum(c, tc, scratch.as<fe>(), ic, fc, combined.as<fe>(), n, E, x_last, K, 3 * E, E);   // / ((x^n - 1)/(x - x_last)), summed
-    }
-    if (K == 1) debug_dump(c, "constraint_poly", combined.p, E * 16);
-
-    // ---- 5: constraint evaluations over the LDE domain + their Merkle tree -----------------------------------------------------------------
+    constraint_polynomial(c, grp);
     clk.mark(4);
     sub.mark("4.combine");
-    DevBuf c_ext((size_t)K * N_loc * 16), c_items((size_t)K * (N_loc / 4) * 32), c_nodes;
-    auto c_ext_of = [&](int p) { return c_ext.as<fe>() + (size_t)p * N_loc; };
-    lde_batch(c, combined.as<fe>(), c_ext.as<fe>(), log_n, log_b, 8, K, E, N_loc, c0, (unsigned)nc);
-    sub.mark("5.lde");
-    constraint_items_local(c, c_ext.as<fe>(), log_n, log_nc, c_items.p, K);      // first tree level: H(4 evaluations), [k][c4 local], per proof
-    sub.mark("5.items");
-    {
-        if (G == 1) {
-            c_nodes.alloc((size_t)K * (N_loc / 4) * 32);
-            merkle_build(c, c_items.p, c_nodes.p, N_loc / 4, K);
-        }
-        std::vector<const void *> roots;
-        std::vector<int> who;
-        for (int p = 0; p < K; p++) {
-            if (!ps[p].live) continue;
-            const uint8_t *items = (const uint8_t *)c_items.p + (size_t)p * (N_loc / 4) * 32;
-            if (G == 1) ps[p].c_tree.attach(c, items, (const uint8_t *)c_nodes.p + (size_t)p * (N_loc / 4) * 32, n, log_nc - 2);
-            else ps[p].c_tree.build(c, items, n, log_nc - 2, false);
-            roots.push_back(ps[p].c_tree.root_dev());
-            who.push_back(p);
-        }
-        std::vector<Digest> r = fetch_roots(c, roots);
-        for (size_t i = 0; i < who.size(); i++) ps[who[i]].stark.constraint_root = r[i];
-    }
-
-    // ---- 6: DEEP composition polynomial ---------------------------------------------------------------------------------------------------------
+    commit_constraints(c, grp, ps);
     clk.mark(5);
     sub.mark("5.tree");
-    DevBuf comp((size_t)K * E * 16), comp_ext((size_t)K * N_loc * 16);
-    {
-        TwiddleRef g_t = c.twiddle(log_n, false);
-        // trace polynomials at z and z*g: every rank evaluates its own columns (the split of stage 1); slots of 2 cpr values are gathered.
-        // d_deep = 2 trace values per column (one GPU: proof p's from column col0[p] on; several: G slots of cpr columns), then [K][2]
-        // values of the constraint polynomial at z
-        const size_t deep_cols = G == 1 ? W : (size_t)cpr * G;
-        DevBuf d_deep((2 * deep_cols + 2 * K) * 16);
-        fe *deep_c = d_deep.as<fe>() + 2 * deep_cols;
-        DG_CUDA(cudaMemsetAsync(d_deep.p, 0, d_deep.bytes, c.stream));
-        // powers of z, 1/z, z g, 1/(z g) of every proof: four batched tables from one upload of the (base, step) pairs, [table][proof][2]
-        std::vector<fe> base_step((size_t)8 * K, fe_make(0, 0));
-        for (int p : order) {
-            ProofState &s = ps[p];
-            if (!s.live) continue;
-            s.dc = fs::draw_composition_coefficients(s.stark.constraint_root.data(), shapes[p].w);
-            const fe z = s.dc.z, zg = fe_mul(z, root_n);
-            const fe bases[4] = {z, host_inv(z), zg, host_inv(zg)};
-            for (int t = 0; t < 4; t++) {
-                base_step[(size_t)2 * (t * K + p)] = bases[t];
-                base_step[(size_t)2 * (t * K + p) + 1] = PowTables::step(bases[t], t < 2 ? E + 1 : n + 1);
-            }
-        }
-        DevBuf d_base_step(base_step.size() * 16);
-        h2d(c, d_base_step.p, base_step.data(), base_step.size() * 16);
-        const fe *bs = d_base_step.as<fe>();
-        PowTables z_t(c, bs, K, E + 1), zi_t(c, bs + 2 * K, K, E + 1), zg_t(c, bs + 4 * K, K, n + 1), zgi_t(c, bs + 6 * K, K, n + 1);
-        if (G == 1) {
-            eval_polys_at(c, polys.as<fe>(), n, (int)W, z_t.ref(0), g_t, true, d_deep.as<fe>(), 1 << 30, z_t.lo_n, z_t.hi_n, d_col_proof);
-        } else {
-            const int j0 = col_start(g), mine = col_count(g);
-            if (mine > 0) eval_polys_at(c, polys.as<fe>() + (size_t)j0 * n, n, mine, z_t.ref(0), g_t, true, d_deep.as<fe>() + (size_t)2 * g * cpr);
-            comm_all_gather(c, d_deep.as<fe>() + (size_t)2 * g * cpr, d_deep.p, (size_t)2 * cpr * 16);
-        }
-        eval_polys_at(c, combined.as<fe>(), E, K, z_t.ref(0), g_t, false, deep_c, 1, z_t.lo_n, z_t.hi_n);
-        std::vector<fe> deep_slots(2 * deep_cols + 2 * K);
-        d2h(c, deep_slots.data(), d_deep.p, deep_slots.size() * 16);
-    sub.mark("6.deep_values");
-        // one upload: [K][2 wmax] coefficients of the trace combinations (proof p's trace1 | trace2 at p 2 wmax, p 2 wmax + wmax) | sub0
-        // of the three divisions [3][K] | compose's k1, k2, kc [K][3]
-        std::vector<fe> pack((size_t)K * (2 * wmax + 6), fe_make(0, 0));
-        fe *ccs = pack.data(), *subs = ccs + (size_t)K * 2 * wmax, *ks = subs + (size_t)3 * K;
-        for (int p = 0; p < K; p++) {
-            ProofState &s = ps[p];
-            if (!s.live) continue;
-            const int wq = shapes[p].w;
-            const fe *slots = deep_slots.data() + 2 * (size_t)col0[p];           // several GPUs: K == 1, col0[0] == 0
-            std::vector<fe> deep(2 * wq);
-            for (int r = 0; r < G; r++)
-                for (int o = 0; o < (G == 1 ? wq : col_count(r)); o++) {
-                    const int from = G == 1 ? o : r * cpr + o, to = G == 1 ? o : col_start(r) + o;
-                    deep[2 * to] = slots[2 * from];
-                    deep[2 * to + 1] = slots[2 * from + 1];
-                }
-            std::vector<fe> &z1 = s.stark.trace_at_z1, &z2 = s.stark.trace_at_z2;
-            z1.resize(wq); z2.resize(wq);
-            fe sub1 = fe_make(0, 0), sub2 = fe_make(0, 0);
-            for (int i = 0; i < wq; i++) {
-                z1[i] = deep[2 * i]; z2[i] = deep[2 * i + 1];
-                sub1 = fe_add(sub1, fe_mul(z1[i], s.dc.trace1[i]));
-                sub2 = fe_add(sub2, fe_mul(z2[i], s.dc.trace2[i]));
-            }
-            subs[p] = sub1; subs[K + p] = sub2; subs[2 * K + p] = deep_slots[2 * deep_cols + 2 * p];
-            std::copy(s.dc.trace1.begin(), s.dc.trace1.begin() + wq, ccs + (size_t)p * 2 * wmax);
-            std::copy(s.dc.trace2.begin(), s.dc.trace2.begin() + wq, ccs + (size_t)p * 2 * wmax + wmax);
-            ks[3 * p] = s.dc.t1_degree; ks[3 * p + 1] = s.dc.t2_degree; ks[3 * p + 2] = s.dc.constraints;
-        }
-        DevBuf d_pack(pack.size() * 16), t12((size_t)K * 2 * n * 16);
-        h2d(c, d_pack.p, pack.data(), pack.size() * 16);
-        const fe *d_cc = d_pack.as<fe>(), *d_subs = d_cc + (size_t)K * 2 * wmax, *d_ks = d_subs + (size_t)3 * K;
-        fe *t1 = t12.as<fe>(), *t2 = t12.as<fe>() + n;                      // of proof 0; proof p at + 2 n p
-        lincomb2(c, polys.as<fe>(), n, wmax, d_cc, d_cc + wmax, t1, t2, K, 2 * wmax, 2 * n, d_cols);
-        syn_div(c, K, t1, 2 * n, t1, 2 * n, n, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n, d_subs);
-        //                                                                                                   (T1(x) - T1(z)) / (x - z)
-        syn_div(c, K, t2, 2 * n, t2, 2 * n, n, zg_t.ref(0), zg_t.lo_n, zg_t.hi_n, zgi_t.ref(0), zgi_t.lo_n, zgi_t.hi_n, d_subs + K);
-        //                                                                                                   (T2(x) - T2(zg)) / (x - zg)
-        syn_div(c, K, combined.as<fe>(), E, scratch2.as<fe>(), E, E, z_t.ref(0), z_t.lo_n, z_t.hi_n, zi_t.ref(0), zi_t.lo_n, zi_t.hi_n,
-                d_subs + 2 * K);                                                                           // (C(x) - C(z)) / (x - z)
-    sub.mark("6.lincomb+syndiv");
-        compose(c, K, t1, t2, 2 * n, scratch2.as<fe>(), comp.as<fe>(), n, E, 6 * n + 1, d_ks);
-        if (K == 1) debug_dump(c, "composition_poly", comp.p, E * 16);
-        // every rank extends its own cosets; the first FRI layers work on these slabs directly (no all-gather of the N evaluations)
-        lde_batch(c, comp.as<fe>(), comp_ext.as<fe>(), log_n, log_b, 8, K, E, N_loc, c0, (unsigned)nc);
-    }
-
-    // ---- 7: FRI layers ---------------------------------------------------------------------------------------------------------------------------
+    deep_composition(c, grp, ps);
     clk.mark(6);
     sub.mark("6.compose+lde");
-    DevBuf fri_gathered;                                       // multi-GPU: the first replicated layer, gathered from the ranks' slabs
-    std::vector<DevBuf> layer_bufs;                            // replicated layers: row hashes, trees and folded values of all K proofs
-    size_t n_layers = 0;
-    {
-        TwiddleRef inv_root = c.twiddle(log_N, true);
-        const fe tau_inv = host_inv(host_root_of_unity(2));
-        const fe inv4 = host_inv(fe_make(4, 0));
-        // the K proofs' layers are one buffer each: layer d of proof p = cur + p * cur_stride
-        const fe *cur = comp_ext.as<fe>();
-        uint64_t cur_stride = N_loc;
-        Layout lay{log_N, log_b};
-        bool local = G > 1;                                    // `cur` is this rank's coset slab of the layer (K == 1)
-        // layer roots and folding points stay on the device, [layer][proof] (special_x = prng(root) is derived by fri_alpha): the host
-        // sees the roots in one copy after the last layer.  With host RNG callbacks registered each layer asks the host instead: one
-        // copy of the layer's K roots, the callbacks of the live proofs in proof order, one upload of the K folding points.
-        const int MAX_LAYERS = 20;
-        DevBuf d_alpha((size_t)MAX_LAYERS * K * 16), d_roots((size_t)MAX_LAYERS * K * 32);
-        const bool host_rng = fs::rng_hooks_active();
-        auto alpha_dev = [&](size_t layer) { return d_alpha.as<fe>() + layer * K; };
-        auto root_slots = [&](size_t layer) { return (uint8_t *)d_roots.p + 32 * layer * K; };
-        // the K roots of layer `li`, root_stride bytes apart from root0, into their slots
-        auto copy_roots = [&](const void *root0, size_t root_stride, size_t li) {
-            DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
-            DG_CUDA(cudaMemcpy2DAsync(root_slots(li), 32, root0, std::max<size_t>(root_stride, 32), 32, K, cudaMemcpyDeviceToDevice, c.stream));
-        };
-        auto folding_points = [&](const void *root0, size_t root_stride, size_t li) {
-            DG_REQUIRE(li < (size_t)MAX_LAYERS, "too many FRI layers");
-            if (!host_rng) { fri_alpha(c, root0, alpha_dev(li), root_slots(li), K, root_stride); return; }
-            copy_roots(root0, root_stride, li);
-            std::vector<uint8_t> r((size_t)32 * K);
-            d2h(c, r.data(), root_slots(li), r.size());
-            std::vector<fe> alphas(K, fe_make(0, 0));
-            for (int p : order)
-                if (ps[p].live) alphas[p] = fs::prng_vector(r.data() + 32 * p, 1)[0];   // field::prng(seed) = first draw of the generator (field.rs:264-269)
-            DG_CUDA(cudaMemcpyAsync(alpha_dev(li), alphas.data(), (size_t)16 * K, cudaMemcpyHostToDevice, c.stream));
-            DG_CUDA(cudaStreamSynchronize(c.stream));
-        };
-        for (;;) {
-            const int log_r = lay.log_d - 2;
-            const uint64_t R = 1ULL << log_r;
-            // layers below 2^22 values are latency-bound (two collectives per sharded tree cost more than hashing them whole): gather the
-            // first such layer once (<= 32 MB) and finish redundantly on every rank
-            if (local && (lay.log_d < 22 || log_r - log_b < 6)) {
-                fri_gathered.alloc((size_t)16 << lay.log_d);
-                comm_all_gather(c, cur, fri_gathered.p, ((size_t)16 << lay.log_d) >> log_g);     // rank-major == coset-major
-                cur = fri_gathered.as<fe>();
-                local = false;
-            }
-            const size_t li = n_layers++;
-            if (local) {
-                FriLayerDev &L = ps[0].layers.emplace_back();
-                L.vals = cur; L.layout = lay; L.sharded = true;
-                // rows r = b k' + c of the own cosets: hashes in ShardedTree order, n' = R / b subtrees of nc leaves per rank
-                L.leaves.alloc((R >> log_g) * 32);
-                fri_hash_rows_local(c, cur, lay.log_d, log_b, log_nc, L.leaves.p);
-                L.tree.build(c, L.leaves.p, R >> log_b, log_nc, false);
-                folding_points(L.tree.root_dev(), 0, li);
-                L.folded.alloc((R >> log_g) * 16);
-                fri_fold_local(c, cur, lay.log_d, log_b, log_nc, c0, L.folded.as<fe>(), alpha_dev(li), inv_root, log_N, tau_inv, inv4);
-                cur = L.folded.as<fe>();
-                lay = Layout{log_r, log_b};
-                continue;
-            }
-            const Layout rows{log_r, (lay.log_b >= 0 && log_r >= lay.log_b) ? lay.log_b : -1};
-            layer_bufs.emplace_back((size_t)K * R * 32);
-            const uint8_t *leaves = layer_bufs.back().as<uint8_t>();
-            layer_bufs.emplace_back((size_t)K * R * 32);
-            const uint8_t *nodes = layer_bufs.back().as<uint8_t>();
-            fri_hash_rows(c, cur, lay, rows, (void *)leaves, K, cur_stride);
-            merkle_build(c, leaves, (void *)nodes, R, K);
-            for (int p = 0; p < K; p++) {
-                if (!ps[p].live) continue;
-                FriLayerDev &L = ps[p].layers.emplace_back();
-                L.vals = cur + (size_t)p * cur_stride; L.layout = lay; L.sharded = false;
-                L.leaves_p = leaves + (size_t)p * R * 32; L.nodes_p = nodes + (size_t)p * R * 32;
-            }
-            if (R * 4 <= 256) {                                    // MAX_REMAINDER_LENGTH (fri/mod.rs:13): the remainder's root only
-                copy_roots(nodes + 32, R * 32, li);
-                break;
-            }
-            folding_points(nodes + 32, R * 32, li);                // special_x = prng(root)  (fri/prover.rs:29)
-            layer_bufs.emplace_back((size_t)K * R * 16);           // values of the next layer
-            fe *folded = layer_bufs.back().as<fe>();
-            fri_fold(c, cur, lay, folded, rows, alpha_dev(li), inv_root, log_N, tau_inv, inv4, K, cur_stride);
-            cur = folded;
-            cur_stride = R;
-            lay = rows;
-        }
-        std::vector<uint8_t> roots(32 * n_layers * K);
-        d2h(c, roots.data(), d_roots.p, roots.size());
-        // the last layer is the remainder: its root is the FRI proof's rem_root
-        for (int p = 0; p < K; p++) {
-            if (!ps[p].live) continue;
-            FriProof &f = ps[p].stark.degree_proof;
-            auto root = [&](size_t i) { return roots.data() + 32 * (i * K + p); };
-            f.layers.resize(n_layers - 1);
-            for (size_t i = 0; i + 1 < n_layers; i++) memcpy(f.layers[i].root.data(), root(i), 32);
-            memcpy(f.rem_root.data(), root(n_layers - 1), 32);
-        }
-    }
-
-    // ---- 8: query positions ------------------------------------------------------------------------------------------------------------------------
+    fri_layers(c, grp, ps);
     clk.mark(7);
     sub.mark("7.fri");
-    {
-        std::vector<std::array<uint8_t, 32>> seeds;
-        std::vector<unsigned> grinding;
-        std::vector<int> who;
-        for (int p : order) {
-            if (!ps[p].live) continue;
-            const FriProof &f = ps[p].stark.degree_proof;
-            std::vector<uint8_t> roots;
-            for (auto &l : f.layers) roots.insert(roots.end(), l.root.begin(), l.root.end());
-            roots.insert(roots.end(), f.rem_root.begin(), f.rem_root.end());
-            if (K == 1) debug_dump_host("fri_roots", roots.data(), roots.size());
-            seeds.emplace_back();
-            fs::blake3_short(roots.data(), roots.size(), seeds.back().data());
-            grinding.push_back(ps[p].stark.options.grinding_factor);
-            who.push_back(p);
-        }
-        std::vector<unsigned long long> nonces = pow_search_batch(c, seeds, grinding);
-        for (size_t i = 0; i < who.size(); i++) {
-            ProofState &s = ps[who[i]];
-            s.stark.pow_nonce = nonces[i];
-            pow_hash(seeds[i].data(), s.stark.pow_nonce, s.proof->pow_seed);
-            try {
-                s.positions = fs::query_positions(s.proof->pow_seed, N, b, s.stark.options.num_queries);
-            } catch (const std::exception &e) { s.fail(DG_ERR_EXHAUSTED, e.what()); continue; }
-            if (K == 1) debug_dump_host("positions", s.positions.data(), s.positions.size() * 8);
-        }
-        if (!any_live()) return;
-    }
-
-    // ---- 9: build proof objects --------------------------------------------------------------------------------------------------------------------------
+    query_positions(c, grp, ps);
+    if (!any_live(ps)) return;
     clk.mark(8);
     sub.mark("8.pow");
-    // Plan every opening of every proof on the host, fetch all opened values / digests in one batched pass (FetchBatch), then write each proof.
-    FetchBatch fb(c);
-    // registers the nodes of a batch-proof plan; leaf_ref / node_ref map leaf indices / heap indices to fetch references
-    auto plan_offsets = [&](const fs::BatchPlan &plan, auto leaf_ref, auto node_ref) {
-        Offsets o(plan.nodes.size());
-        for (size_t sidx = 0; sidx < plan.nodes.size(); sidx++)
-            for (auto &r : plan.nodes[sidx]) o[sidx].push_back(fb.add32(r.leaf ? leaf_ref(r.index) : node_ref(r.index)));
-        return o;
-    };
-    auto digests_at = [&](const Offsets &o) {
-        std::vector<std::vector<Digest>> v(o.size());
-        for (size_t i = 0; i < o.size(); i++)
-            for (size_t off : o[i]) v[i].push_back(fb.digest(off));
-        return v;
-    };
-    // opened trace rows outside the retained cosets (evaluation-coset layout): the trace polynomials at w_N^pos, all proofs in one launch,
-    // into d_rows (the w_p values of each computed row of the batch, rows in proof and query order)
-    auto retained = [&](uint64_t pos) { return ((pos & (b - 1)) & (rstep - 1)) == 0; };
-    DevBuf d_rows;
-    std::vector<size_t> first_row(K, 0);                       // proof p's first value in d_rows
-    {
-        std::vector<TraceRow> points;
-        size_t values = 0;
-        for (int p = 0; p < K; p++) {
-            first_row[p] = values;
-            if (ps[p].live)
-                for (uint64_t pos : ps[p].positions)
-                    if (!retained(pos)) {
-                        points.push_back(TraceRow{pos, 0, col0[p], (unsigned)shapes[p].w});
-                        values += shapes[p].w;
-                    }
-        }
-        if (!points.empty()) {
-            d_rows.alloc(values * 16);
-            eval_trace_rows(c, polys.as<fe>(), n, points, log_N, d_rows.as<fe>());
-        }
-    }
-    auto plan_openings = [&](ProofState &s, const fe *slab_p, const fe *c_ext_p, size_t row0, int w) {
-        OpenPlan O;
-        const std::vector<uint64_t> &positions = s.positions;
-        const int nq = (int)positions.size();
-        // trace rows at the queried positions (trace_table.rs:127-134): the rank owning the position's coset reads the row from the retained
-        // slab, or it was computed into d_rows
-        O.row_off.resize(nq);
-        for (int q = 0; q < nq; q++) {
-            const uint64_t cpos = positions[q] & (b - 1), k = positions[q] >> log_b;
-            if (!retained(positions[q])) {
-                O.row_off[q] = fb.add16(FetchRef{d_rows.p, row0, -1});
-                for (int j = 1; j < w; j++) fb.add16(FetchRef{d_rows.p, row0 + j, -1});
-                row0 += w;
-                continue;
-            }
-            const int owner = (int)(cpos >> log_nc);
-            const uint64_t phys = (((cpos - (uint64_t)owner * nc) / rstep) << log_n) + k;
-            for (int j = 0; j < w; j++) {
-                const size_t off = fb.add16(FetchRef{slab_p + (size_t)j * slab_col, phys, owner});
-                if (j == 0) O.row_off[q] = off;
-            }
-        }
-        // trace tree openings: leaves are the row hashes
-        O.tplan = fs::plan_batch_proof(positions, N);
-        O.t_off = plan_offsets(O.tplan, [&](uint64_t i) { return s.t_tree.item_ref(i); }, [&](uint64_t h) { return s.t_tree.node_ref(h); });
-
-        // constraint tree openings: leaf j = evaluations (2j, 2j+1), unhashed (prover.rs:180-187); evaluation 2j+1 lives in the next
-        // coset at the same k, i.e. n elements further in the owner's slab: two 16-byte units registered back to back = one 32-byte item
-        auto constraint_leaf = [&](uint64_t j) {
-            const uint64_t i = 2 * j, cpos = i & (b - 1), k = i >> log_b;
-            const int owner = (int)(cpos >> log_nc);
-            const uint64_t p0 = ((cpos - (uint64_t)owner * nc) << log_n) + k;
-            const size_t off = fb.add16(FetchRef{c_ext_p, p0, owner});
-            fb.add16(FetchRef{c_ext_p, p0 + n, owner});
-            return off;
-        };
-        std::vector<uint64_t> c_positions = fs::constraint_positions(positions);
-        O.cplan = fs::plan_batch_proof(c_positions, N / 2);
-        for (uint64_t j : O.cplan.value_leaves) O.cval_off.push_back(constraint_leaf(j));
-        O.c_off.resize(O.cplan.nodes.size());
-        for (size_t sidx = 0; sidx < O.cplan.nodes.size(); sidx++)
-            for (auto &r : O.cplan.nodes[sidx]) {
-                // heap indices of the tree over N/2 leaves: [N/4, N/2) is the first hashed level (= level-0 items of c_tree)
-                if (r.leaf) O.c_off[sidx].push_back(constraint_leaf(r.index));
-                else if (r.index >= N / 4) O.c_off[sidx].push_back(fb.add32(s.c_tree.item_ref(r.index - N / 4)));
-                else O.c_off[sidx].push_back(fb.add32(s.c_tree.node_ref(r.index)));
-            }
-
-        // FRI layers (fri/prover.rs:55-95)
-        O.fri_open.resize(s.layers.size() - 1);
-        std::vector<uint64_t> fpos = positions;
-        for (size_t d = 0; d + 1 < s.layers.size(); d++) {
-            FriLayerDev &L = s.layers[d];
-            LayerOpen &lo = O.fri_open[d];
-            const uint64_t D = 1ULL << L.layout.log_d, R = D / 4;
-            fpos = fs::augmented_positions(fpos, D);
-            fs::BatchPlan plan = fs::plan_batch_proof(fpos, R);
-            lo.depth = plan.depth;
-            for (uint64_t p : fpos)
-                for (int j = 0; j < 4; j++) {
-                    size_t off;
-                    if (L.sharded) {
-                        const uint64_t cpos = p & (b - 1), k = (p >> log_b) + (uint64_t)j * (R >> log_b);
-                        const int owner = (int)(cpos >> log_nc);
-                        off = fb.add16(FetchRef{L.vals, ((cpos - (uint64_t)owner * nc) << (L.layout.log_d - log_b)) + k, owner});
-                    } else {
-                        off = fb.add16(FetchRef{L.vals, L.layout.phys(p + j * R), -1});
-                    }
-                    if (j == 0) lo.val_off.push_back(off);
-                }
-            if (L.sharded) lo.node_off = plan_offsets(plan, [&](uint64_t i) { return L.tree.item_ref(i); }, [&](uint64_t h) { return L.tree.node_ref(h); });
-            else lo.node_off = plan_offsets(plan, [&](uint64_t i) { return FetchRef{L.leaves_p, i, -1}; }, [&](uint64_t h) { return FetchRef{L.nodes_p, h, -1}; });
-        }
-        {
-            FriLayerDev &L = s.layers.back();
-            const uint64_t D = 1ULL << L.layout.log_d;
-            for (uint64_t i = 0; i < D; i++) O.rem_off.push_back(fb.add16(FetchRef{L.vals, L.layout.phys(i), -1}));   // remainder, natural order
-        }
-        return O;
-    };
-    // the opened values and digests into the proof, which is then written out
-    auto fill_openings = [&](ProofState &s, const OpenPlan &O, int w) {
-        StarkProof &P = s.stark;
-        P.trace_info.domain_depth = O.tplan.depth;
-        P.trace_nodes = digests_at(O.t_off);
-        P.trace_evaluations.assign(O.row_off.size(), std::vector<fe>(w));
-        for (size_t q = 0; q < O.row_off.size(); q++)
-            for (int j = 0; j < w; j++) P.trace_evaluations[q][j] = fb.value(O.row_off[q] + j);
-        for (size_t off : O.cval_off) P.constraint_proof.values.push_back(fb.digest(off));
-        P.constraint_proof.nodes = digests_at(O.c_off);
-        P.constraint_proof.depth = O.cplan.depth;
-        for (size_t d = 0; d < O.fri_open.size(); d++) {
-            const LayerOpen &lo = O.fri_open[d];
-            FriLayer &l = P.degree_proof.layers[d];
-            for (size_t off : lo.val_off) l.values.push_back({fb.value(off), fb.value(off + 1), fb.value(off + 2), fb.value(off + 3)});
-            l.nodes = digests_at(lo.node_off);
-            l.depth = lo.depth;
-        }
-        for (size_t off : O.rem_off) P.degree_proof.rem_values.push_back(fb.value(off));
-        Proof &h = *s.proof;
-        h.bytes = write_proof(P);
-        memcpy(h.trace_root, P.trace_root.data(), 32);
-        memcpy(h.constraint_root, P.constraint_root.data(), 32);
-        h.pow_nonce = P.pow_nonce;
-    };
-    {
-        std::vector<OpenPlan> plans(K);
-        for (int p = 0; p < K; p++)
-            if (ps[p].live) plans[p] = plan_openings(ps[p], slab_of(p), c_ext_of(p), first_row[p], shapes[p].w);
-        fb.run();
-        for (int p = 0; p < K; p++)
-            if (ps[p].live) fill_openings(ps[p], plans[p], shapes[p].w);
-    }
+    build_proofs(c, grp, ps);
     clk.mark(9);
     sub.mark("9.openings");
     sub.report(c.rank);
